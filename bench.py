@@ -40,7 +40,6 @@ sys.path.insert(0, ROOT)
 METRIC = "image-pairs/s (line-descriptor forward x2 + mutual-NN match)"
 UNIT = "pairs/s"
 DTYPE = "f32 io / split-bf16 x3 tensor-core products, fp32 accumulate"
-NCU_SUMMARY = os.path.join(ROOT, "profiles", "r2_ncu_summary.json")
 
 WORKLOADS = {
     "cfg1": dict(pairs=64, lines=128, tokens=21, desc="cfg1: {P} pairs/GPU x 128 lines x 21 tokens x d256, 1 descriptive + 7 signature layers"),
@@ -62,19 +61,10 @@ def load_peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
-def load_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch and kernel class, parsed from the committed
-    `ncu --set full` summary of the FINAL kernels (tools/ncu_summary.py writes it); {} until one exists."""
-    if os.path.exists(NCU_SUMMARY):
-        with open(NCU_SUMMARY) as f:
-            return json.load(f).get("traffic_bytes_per_launch", {})
-    return {}
-
-
-# ---------------------------------------------------------------- algorithmic work (SURVEY §8d)
 def flops_per_image(L, T, n_sig=7):
     """Useful FLOPs (2*MAC) of one image under reference semantics (CLS row of the last layer)."""
     N = T + 1
@@ -151,6 +141,24 @@ class ClockSampler(threading.Thread):
             return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "reasons": ["nvml_unavailable"]}
         return {"sm_mhz": float(np.median(self.samples)), "sm_max_mhz": self.max_mhz, "reasons": sorted(self.reasons),
                 "samples": len(self.samples)}
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Outputs of the timed path as float64 .npy files, so that two builds can be compared output for output (the
+    inputs are seeded, hence identical between runs with the same arguments).  An array larger than its share of
+    DUMP_MAX_BYTES is replaced by a fixed, seeded sample of its elements (`<name>_sample_index.npy` says which)."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_MAX_BYTES // (2 * len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().reshape(-1).cpu().numpy().astype(np.float64)
+        if a.nbytes > share:
+            idx = np.sort(np.random.Generator(np.random.PCG64(0)).choice(a.size, share // 8, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_sample_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 # ---------------------------------------------------------------- synthetic workloads
@@ -293,6 +301,8 @@ def main():
     ap.add_argument("--e2e-chunks", type=int, default=4, help="pair groups whose H2D copy overlaps compute in the e2e leg")
     ap.add_argument("--profile-only", action="store_true", help="resident steps only (for runs under ncu)")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (matches0, counts, scores0) as DIR/<name>.npy")
     ap.add_argument("--cpu-worker", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--threads", type=int, default=1, help=argparse.SUPPRESS)
     ap.add_argument("--n", type=int, default=10, help=argparse.SUPPRESS)
@@ -358,7 +368,7 @@ def main():
         Ls0 = [int(a["desc_sublines"].shape[1]) for a, _ in pairs]
         Ls1 = [int(b["desc_sublines"].shape[1]) for _, b in pairs]
         n_out = sum(Ls0)
-    config["l2_policy"] = f"inputs {in_bytes / 1e6:.0f} MB per step > 126 MB L2"
+    config["l2_policy"] = f"inputs {in_bytes / 1e6:.0f} MB per step vs 50 MB L2"
     torch.cuda.synchronize()
 
     def barrier():
@@ -393,28 +403,28 @@ def main():
         if wl == "cfg4":
             out = _ops.match_descriptors(res0, res1, _native.LAYOUT_ROWS, P, 0.8, True, n0=1024, n1=1024, want_dist=False,
                                          gather=gather)
-            return out["matches0"], out["counts"]
+            return out["matches0"], out["counts"], out["scores0"]
         res = eng.match_packed(resident, P, 0.8, gather=gather)
-        return res.matches0, res.counts
+        return res.matches0, res.counts, res.scores0
 
     def step_resident():
         if peer is not None:
-            m0, cnt = run_resident(peer.publish())
+            m0, cnt, sc = run_resident(peer.publish())
             # counts of step i-2: one exchange stays in flight across the step boundary.  A host that waits for the
             # previous step's counts (and the peers' flags) before it enqueues the next step lets the launch queue run dry
             # whenever the ranks drift into ping-pong - the same box measured 0.99 and 1.41 ms per step that way.  With
             # LTR_GATHER_SLOTS = 8 a peer can only overwrite a slot 8 steps later, when this rank has long read it.
             drain(max(KEEP, 1))
             pending.append((None, peer.collect_async())) # copy-engine D2H of this step's slot behind this step's kernels
-            return m0, cnt
-        m0, cnt = run_resident()
+            return m0, cnt, sc
+        m0, cnt, sc = run_resident()
         if world > 1 and gather_mode != "off":
             # NCCL path: one all-gather stays in flight across the step boundary - its kernel has to find an SM between
             # persistent CTAs that follow each other without a gap (PDL), and a host that waits for it every step lets
             # the launch queue run dry (measured 1.41 ms per step against 1.05 ms)
             drain(max(KEEP, 1))
             pending.append(gather_counts(cnt, P * world, async_op=True))
-        return m0, cnt
+        return m0, cnt, sc
 
     out_host = {"m": torch.empty(n_out, dtype=torch.int32).pin_memory(), "c": torch.empty(P, dtype=torch.int32).pin_memory()}
 
@@ -441,11 +451,14 @@ def main():
     _native.reset_launch_count()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
+    timed_out = None
     for _ in range(args.steps):
-        step_resident()
+        timed_out = step_resident()
     drain()            # the last step's all-gather is inside the timed region
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0 and timed_out is not None:
+        dump_outputs(args.dump_outputs, dict(zip(("matches0", "counts", "scores0"), timed_out)))
     launches = _native.launch_count()
     ms_total = e0.elapsed_time(e1)
     clocks = sampler.result()
@@ -454,7 +467,7 @@ def main():
     #      kernels serialises them and would switch off the programmatic dependent launch overlap. ----
     _native.profile_begin()
     for _ in range(args.steps):
-        m_last, c_last = step_resident()
+        m_last, c_last, _ = step_resident()
     drain()
     barrier()
     prof = _native.profile_end()
@@ -494,7 +507,6 @@ def main():
         assert mism == 0 and int(c_last[0]) == int((got0 >= 0).sum()), f"bench output check failed: {check}"
 
         peaks = load_peaks()
-        traffic = load_traffic()
         ms_step = ms_total / args.steps
         value = P * world / (ms_step / 1e3)
         dom = max(prof.items(), key=lambda kv: kv[1][0]) if prof else ("none", (0.0, 0))
@@ -513,10 +525,10 @@ def main():
                            "match_tc": match_flops}
             useful_flops_step = sum(flops_per_image(l, T) for l in Ls0 + Ls1) + match_flops
             alg_bytes_step = sum(bytes_per_image(l, T) for l in Ls0 + Ls1) + 8 * n_out
-        class_kernel = {"linear": "gemm_img_kernel (tcgen05, split-bf16 x3, TMA-fed tile images)",
-                        "token_fused": "token_fused_kernel (tcgen05 + CUDA-core pooling)",
-                        "sig_attention": "sig_attention_tc_kernel (tcgen05)",
-                        "match_tc": "match_tc_kernel (tcgen05 desc x desc^T both directions, row argmin in the epilogue)"}
+        class_kernel = {"linear": "gemm_img_kernel (wgmma, split-bf16 x3, TMA-fed tile images)",
+                        "token_fused": "token_fused_kernel (register-A wgmma + CUDA-core pooling)",
+                        "sig_attention": "sig_attention_tc_kernel (wgmma)",
+                        "match_tc": "match_tc_kernel (wgmma desc x desc^T both directions, row argmin in the epilogue)"}
         roof = None
         if dom_name in class_flops and dom_launches:
             per_launch_flops = class_flops[dom_name] * args.steps / dom_launches
@@ -525,9 +537,8 @@ def main():
             roof = {"bound": "tensor", "kernel": class_kernel[dom_name], "achieved": ach,
                     "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / peaks["bf16_tflops"],
                     "frac_of_sustained_peak": ach / peaks["bf16_tflops_sustained"],
-                    "traffic": traffic.get(dom_name),
-                    "peak_source": f"{peaks['source']} bf16 burst (MEASURED_PEAKS.json; the timed region is tens of ms at full clocks); "
-                                   "useful FLOPs only",
+                    "peak_source": (f"{peaks['source']} bf16 burst (MEASURED_PEAKS.json; the timed region is tens of ms at full clocks); "
+                                    if peaks["source"] == "measured" else f"{peaks['source']} dense bf16; ") + "useful FLOPs only",
                     "issued_over_useful_flops": 6.0 if dom_name == "match_tc" else 3.0,
                     "launches_per_step": dom_launches / args.steps, "avg_launch_ms": avg_ms,
                     "algorithmic_flops_per_launch": per_launch_flops}
@@ -539,7 +550,7 @@ def main():
                 tf = class_flops[name] * args.steps / (ms_c * 1e-3) / 1e12
                 by_class[name] = {"kernel": class_kernel[name], "launches_per_step": n_c / args.steps,
                                   "avg_launch_ms": ms_c / n_c, "useful_tflops": tf,
-                                  "frac_tensor_peak": tf / peaks["bf16_tflops"], "traffic": traffic.get(name)}
+                                  "frac_tensor_peak": tf / peaks["bf16_tflops"]}
         if "token_fused" in by_class:
             tok_bytes = alg_bytes_step - 8 * n_out - 4 * 256 * sumL + 4 * 1024 * sumL   # inputs + z image (hi/lo bf16)
             gbs = tok_bytes * args.steps / (prof["token_fused"][0] * 1e-3) / 1e9

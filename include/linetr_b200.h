@@ -1,5 +1,5 @@
 /*
- * linetr_b200 - C ABI of the B200-native LineTR line-descriptor + NN-matcher hot path.
+ * linetr_b200 - C ABI of the H100-native LineTR line-descriptor + NN-matcher hot path.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch types, no exceptions.
  * Every entry point replaces a piece of the reference's Python call surface (paths are
@@ -267,7 +267,7 @@ int ltr_linear(const float* x, int32_t ldx, const float* w, const float* bias, c
                int32_t device, void* stream);
 
 /* The same on the tensor-core engine (gemm_img.cuh: persistent, TMA-fed split-bf16 tile images,
- * tcgen05): x is converted to a
+ * wgmma): x is converted to a
  * split-bf16 tile image, the GEMM writes fp32 rows into `y` (may be NULL) and - when
  * `y_from_image` is given - also the split-bf16 image of the result, which is converted back
  * to fp32 rows [m, n] there so that both outputs can be checked.  n % 64 == 0, k % 64 == 0;

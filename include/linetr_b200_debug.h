@@ -18,7 +18,7 @@ float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t o
 
 /* clock64 stamps of CTA 0 recorded by the last ltr_gemm_bench call (64 slots, 16 per tile:
  * 0 MMA acc_empty ok, 1 first operands landed, 2 MMAs issued, 3 epilogue acc_full ok, 4 first
- * TMEM chunk read, 5 epilogue done, 6 producer slot free). */
+ * accumulator complete, 5 epilogue done, 6 producer slot free). */
 const unsigned long long* ltr_gemm_trace(void);
 
 /* Kernels instrumented with LTR_DBG_STAMP store clock64 stamps of their first CTA into a

@@ -1,4 +1,4 @@
-"""linetr_b200 - B200-native LineTR line-descriptor forward + mutual-NN matcher.
+"""linetr_b200 - H100-native LineTR line-descriptor forward + mutual-NN matcher.
 
 Drop-in names (same call surface as yosungho/LineTR `models/`):
     LineTransformer, get_dist_matrix, nn_matcher, nn_matcher_distmat

@@ -20,7 +20,7 @@ def _stream_ptr(device) -> C.c_void_p:
 
 def _req_cuda(t: torch.Tensor, name: str):
     if not t.is_cuda:
-        raise N.LtrError(f"linetr_b200: '{name}' is on {t.device}; the B200 path needs CUDA tensors "
+        raise N.LtrError(f"linetr_b200: '{name}' is on {t.device}; the CUDA path needs CUDA tensors "
                          "(there is no CPU fallback)")
 
 

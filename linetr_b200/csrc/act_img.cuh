@@ -1,7 +1,7 @@
 // Split-bf16 activation image: the operand format of the tensor-core GEMM engine.
 // See gemm_img.cuh for the layout description.
 #pragma once
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltr {
 

@@ -1,4 +1,4 @@
-// Shared host/device utilities of the linetr_b200 CUDA library (sm_100a only).
+// Shared host/device utilities of the linetr_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -81,7 +81,7 @@ struct LaunchScope {
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
 // Every kernel of the path is launched with programmaticStreamSerialization: its CTAs may become
 // resident as soon as SMs free up at the tail of the previous kernel and run their prologue
-// (barrier init, TMEM allocation, constant staging) there; pdl_wait() then blocks until the
+// (barrier init, constant staging) there; pdl_wait() then blocks until the
 // previous grid has completed and flushed, BEFORE anything it produced is read or anything it
 // still reads is overwritten.  pdl_launch_dependents() at kernel entry lets the next kernel do
 // the same behind this one.
@@ -110,9 +110,6 @@ __device__ int g_dbg_on = 0;
   do {                                                                 \
     if (g_dbg_on && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) g_dbg_trace[slot] = clock64(); \
   } while (0)
-// host side: trace only the n-th chained GEMM launch after arming (ltr_debug_trace_arm(100 + n)); -1 = no selection
-inline int& dbg_chain_sel() { static int v = -1; return v; }
-inline int& dbg_chain_cnt() { static int v = 0; return v; }
 
 // ---------------------------------------------------------------- device helpers
 __device__ __forceinline__ float warp_sum(float v) {

@@ -15,7 +15,6 @@
 #include "gemm_img.cuh"
 #include "token_fused.cuh"
 #include "sig_attention_tc.cuh"
-#include "sig_attention_img.cuh"
 #include "tokenizer_kernels.cuh"
 #include "match_kernels.cuh"
 #include "match_tc.cuh"
@@ -273,34 +272,6 @@ static int gemm(const Lin& L, const ActImg& A, int a_kb0, int M, int act, cudaSt
   return launch_gemm_img(gemm_args(L, A, a_kb0, M, act, C, ldc, O, o_kb0, R, ldr, Rimg, r_kb0, a_kb_nb), s, bn_hint);
 }
 
-// Batches with at least this many 128-row tiles run the row-local GEMMs of a signature layer as ONE chained
-// launch (gemm_chain_kernel); smaller ones keep one launch per layer, which spreads the n-blocks of the few
-// m-tiles over more SMs.  LTR_CHAIN_MIN_TILES overrides (0 = never chain).
-static int chain_min_tiles() {
-  static const int v = [] {
-    const char* e = std::getenv("LTR_CHAIN_MIN_TILES");
-    return e ? std::atoi(e) : 96;
-  }();
-  return v;
-}
-// LTR_ATTN_IMG=1 runs uniform 128-line batches on the per-image pipelined attention kernel (sig_attention_img.cuh).
-// Off by default: measured 33.4 us per launch against 25.4 us for the general kernel (profiles/r2_attention_img.md).
-static bool attn_img() {
-  static const bool v = [] {
-    const char* e = std::getenv("LTR_ATTN_IMG");
-    return e ? std::atoi(e) != 0 : false;
-  }();
-  return v;
-}
-// LTR_GEMM_PAIR=0 runs the chains on the single-CTA engine instead of the CTA-pair (cta_group::2) one.
-static bool gemm_pair() {
-  static const bool v = [] {
-    const char* e = std::getenv("LTR_GEMM_PAIR");
-    return e ? std::atoi(e) != 0 : true;
-  }();
-  return v;
-}
-
 template <bool TOKEN>
 static int launch_small_mlp(const SmallMlpWeights& w, const float* in0, const float* in1, const float* in2, ActImg out,
                             int rows, float width, float height, cudaStream_t s) {
@@ -310,7 +281,7 @@ static int launch_small_mlp(const SmallMlpWeights& w, const float* in0, const fl
   LTR_CUDA_TRY(ensure_dynamic_smem(small_mlp_kernel<TOKEN>, smem));
   const int groups = cdiv(rows, SM_ROWS);
   int grid = cdiv(groups, SM_WARPS);
-  if (grid > 148 * 3) grid = 148 * 3;
+  if (grid > 132 * 3) grid = 132 * 3;
   const float scale = fmaxf(width, height) * 0.7f;
   LaunchScope ls(KC_SMALL_MLP, s);
   LTR_CUDA_TRY(launch_pdl(small_mlp_kernel<TOKEN>, dim3(grid), dim3(SM_WARPS * 32), (size_t)smem, s, w, in0, in1, in2, out, rows,
@@ -352,8 +323,6 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
   }
   // ---- line stage: V projection (block diagonal over heads), fc + CLS residual, LN, FFN, LN, + line pos ----
   LTR_TRY(gemm(m->wv, w.z, 0, R, ACT_NONE, s, nullptr, 0, &w.ctx, 0, nullptr, 0, nullptr, 0, 64, 4));
-  const bool chain = chain_min_tiles() > 0 && cdiv(R, 128) >= chain_min_tiles() && !out_cf && !m->sig.empty();
-  const bool chain_line = chain && m->cfg.d_inner % 256 == 0;
   // line positional encoder first (its output is added in the w_2 epilogue)
   LTR_TRY(launch_small_mlp<false>(m->lpe.head, in.sublines, in.resp, in.angle, w.l128, R, in.image_width,
                                   in.image_height, s));
@@ -369,14 +338,9 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
     // sentence = klines_pos + LN(y1 + ffn)  -> image xm[:, :256] (the running descriptor), all in the w_2 epilogue
     GemmImgArgs w2 = gemm_args(m->w2, w.g, 0, R, ACT_NONE, nullptr, 0, &w.xm, 0, nullptr, 0, &w.y1i, 0);
     w2.norm = NORM_LAYER; w2.eps = 1e-6f; w2.ng = m->ln2g; w2.nbeta = m->ln2b; w2.NaddImg = w.lpos; w2.nadd_kb0 = 0;
-    if (chain_line) {   // row-local: fc -> w_1 -> w_2 -> qkv of signature layer 0 in one launch
-      GemmImgArgs ops[4] = {fc, w1, w2, gemm_args(m->sig[0].qkv, w.xm, 0, R, ACT_NONE, nullptr, 0, &w.qkv, 0)};
-      LTR_TRY(launch_gemm_chain(ops, 4, s, gemm_pair()));
-    } else {
-      LTR_TRY(launch_gemm_img(fc, s, 256));
-      LTR_TRY(launch_gemm_img(w1, s));
-      LTR_TRY(launch_gemm_img(w2, s, 256));
-    }
+    LTR_TRY(launch_gemm_img(fc, s, 256));
+    LTR_TRY(launch_gemm_img(w1, s));
+    LTR_TRY(launch_gemm_img(w2, s, 256));
   }
   // ---- line signature layers ----
   int max_l = in.lines_per_image;
@@ -390,25 +354,14 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
   fin.norm = NORM_L2; fin.eps = 1e-6f;   // final_proj + F.normalize in one epilogue (rows-only output)
   for (size_t li = 0; li < m->sig.size(); ++li) {
     const SigLayer& L = m->sig[li];
-    if (!chain || (li == 0 && !chain_line)) LTR_TRY(gemm(L.qkv, w.xm, 0, R, ACT_NONE, s, nullptr, 0, &w.qkv, 0));
-    // o -> xm[:, 256:]; images of exactly 128 lines are the 128-row tiles of the qkv image: per-image pipelined kernel
-    if (!cu && in.lines_per_image == 128 && attn_img()) LTR_TRY(launch_sig_attention_img(w.qkv, w.xm, 256, in.n_images, s));
-    else LTR_TRY(launch_sig_attention_tc(w.qkv, w.xm, 256, cu, in.lines_per_image, max_l, in.n_images, s));
+    LTR_TRY(gemm(L.qkv, w.xm, 0, R, ACT_NONE, s, nullptr, 0, &w.qkv, 0));
+    // o -> xm[:, 256:]
+    LTR_TRY(launch_sig_attention_tc(w.qkv, w.xm, 256, cu, in.lines_per_image, max_l, in.n_images, s));
     // x += delta: the running descriptor lives ONLY as the split-bf16 image xm[:, :256] (hi + lo carries
     // ~2^-17 relative precision; an fp32 copy would double the store traffic of this epilogue)
-    if (chain) {
-      // mlp1 -> mlp2 (+ residual, in place) -> qkv of the next layer / final projection: row-local, one launch
-      const bool last = li + 1 == m->sig.size();
-      GemmImgArgs ops[3] = {gemm_args(L.mlp1, w.xm, 0, R, ACT_RELU, nullptr, 0, &w.hm, 0),
-                            gemm_args(L.mlp2, w.hm, 0, R, ACT_NONE, nullptr, 0, &w.xm, 0, nullptr, 0, &w.xm, 0),
-                            last ? fin : gemm_args(m->sig[li + 1].qkv, w.xm, 0, R, ACT_NONE, nullptr, 0, &w.qkv, 0)};
-      LTR_TRY(launch_gemm_chain(ops, 3, s, gemm_pair()));
-    } else {
-      LTR_TRY(gemm(L.mlp1, w.xm, 0, R, ACT_RELU, s, nullptr, 0, &w.hm, 0));
-      LTR_TRY(gemm(L.mlp2, w.hm, 0, R, ACT_NONE, s, nullptr, 0, &w.xm, 0, nullptr, 0, &w.xm, 0));
-    }
+    LTR_TRY(gemm(L.mlp1, w.xm, 0, R, ACT_RELU, s, nullptr, 0, &w.hm, 0));
+    LTR_TRY(gemm(L.mlp2, w.hm, 0, R, ACT_NONE, s, nullptr, 0, &w.xm, 0, nullptr, 0, &w.xm, 0));
   }
-  if (chain) return 0;
   if (!out_cf) {   // rows (+ matcher tile image): projection + L2 normalisation in one launch
     LTR_TRY(launch_gemm_img(fin, s, 256));
     return 0;
@@ -1022,12 +975,6 @@ int ltr_linear_img_norm(const float* x, int32_t ldx, const float* w_host, const 
 // debug: arm / read the clock64 stamps kernels of CTA 0 leave in g_dbg_trace (see LTR_DBG_STAMP)
 void ltr_debug_trace_arm(int32_t on) {
   int v = on;
-  dbg_chain_sel() = -1;
-  if (on >= 100) {   // trace only chained-GEMM launch number (on - 100) from now on
-    dbg_chain_sel() = on - 100;
-    dbg_chain_cnt() = 0;
-    v = 0;
-  }
   cudaMemcpyToSymbol(g_dbg_on, &v, sizeof(int));
   if (on) {
     static unsigned long long zeros[128] = {0};

@@ -1,4 +1,4 @@
-// Tensor-core descriptor matcher (K3): all-pairs distance D = 2 - 2 <a_i, b_j> on tcgen05 with the
+// Tensor-core descriptor matcher (K3): all-pairs distance D = 2 - 2 <a_i, b_j> on wgmma with the
 // row-argmin fused into the epilogue, for BOTH directions (side 0 rows vs side 1 and side 1 rows vs
 // side 0 - the second one is the column argmin the mutual check needs), a tail kernel that applies
 // threshold + mutual check + per-pair counts, and an exact fp32 re-check for decisions the
@@ -10,7 +10,7 @@
 // evaluations/matcher.py:51-102 (||a||^2 + ||b||^2 - 2 ab).
 //
 // Precision contract.  The contraction is a 3-term split-bf16 product (hi*hi + lo*hi + hi*lo, fp32
-// accumulate in TMEM): ~1e-5 absolute on a distance.  Match indices must be bit-exact, so every row
+// accumulate in registers): ~1e-5 absolute on a distance.  Match indices must be bit-exact, so every row
 // whose best and second-best distance are closer than MATCH_EPS, or whose best distance lies within
 // MATCH_EPS of the threshold, is recomputed by the tail kernel with fp32 FMAs in ascending k order
 // (the arithmetic of the round-1 FFMA matcher the golden vectors were pinned with) before any decision
@@ -24,7 +24,8 @@
 #pragma once
 #include "act_img.cuh"
 #include "common.cuh"
-#include "ptx_sm100.cuh"
+#include "gemm_img.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltr {
 
@@ -34,12 +35,13 @@ constexpr int MT_KB = MT_D / 64;                  // k-blocks per tile row
 constexpr int MT_TILE = 16384;                    // one plane of a 128 x 64 bf16 tile
 constexpr int MT_A_BYTES = MT_KB * 2 * MT_TILE;   // resident A: 4 k-blocks x (hi + lo) = 128 KB
 constexpr int MT_STAGE = 2 * MT_TILE;             // B ring stage: one k-block, hi + lo
-constexpr int MT_STAGES = 3;
+constexpr int MT_STAGES = 2;
 constexpr int MT_OFF_B = MT_A_BYTES;
-constexpr int MT_OFF_BAR = MT_OFF_B + MT_STAGES * MT_STAGE;
+constexpr int MT_OFF_STG = MT_OFF_B + MT_STAGES * MT_STAGE;   // accumulator staging: 8 blocks of 32 x 32 fp32
+constexpr int MT_OFF_BAR = MT_OFF_STG + 8 * 4096;
 constexpr int MT_OFF_XCH = MT_OFF_BAR + 256;      // half-merge exchange: 3 x 128 x 4 B
 constexpr int MT_SMEM = MT_OFF_XCH + 1536 + 1024; // + alignment slack (<= 227 KB)
-constexpr int MT_THREADS = 320;                   // TMA warp, MMA warp, 8 epilogue warps
+constexpr int MT_THREADS = 288;                   // 2 consumer warpgroups (MMA + epilogue), TMA warp
 static_assert(MT_SMEM <= 232448, "match_tc: shared memory budget");
 
 // One side of a batch of pairs.
@@ -82,10 +84,8 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
   uint64_t* full = bars;                   // [STAGES] B stage landed
   uint64_t* empty = bars + MT_STAGES;      // [STAGES] B stage consumed
   uint64_t* a_full = bars + 2 * MT_STAGES; // [1] resident A landed
-  uint64_t* acc_full = a_full + 1;         // [2]
-  uint64_t* acc_empty = acc_full + 2;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float* xch = reinterpret_cast<float*>(smem + MT_OFF_XCH);
+  float* stg_all = reinterpret_cast<float*>(smem + MT_OFF_STG);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int pair = blockIdx.y;
@@ -95,26 +95,15 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
   const MatchSide& SB = p.s[side ^ 1];
   pdl_launch_dependents();
 
-  if (warp == 0 && lane == 0) {
+  if (tid == 0) {
     for (int s = 0; s < MT_STAGES; ++s) {
       ptx::mbar_init(&full[s], 1);
-      ptx::mbar_init(&empty[s], 1);
+      ptx::mbar_init(&empty[s], 8);
     }
     ptx::mbar_init(a_full, 1);
-    for (int b = 0; b < 2; ++b) {
-      ptx::mbar_init(&acc_full[b], 1);
-      ptx::mbar_init(&acc_empty[b], 8);
-    }
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();   // descriptors / tile images of the producing kernel are complete from here on
 
   int ba, ea, bb, eb;
@@ -126,7 +115,7 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
   const bool active = rb * 128 < na && nb > 0;   // uniform per CTA
   const int n_ct = active ? (nb + 127) >> 7 : 0;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ---------------------------------------------------------------- TMA producer
     if (lane == 0 && active) {
       const size_t ta = (size_t)(side_tile0(SA, pair, ba) + rb) * MT_KB;
@@ -150,46 +139,14 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
           ptx::bulk_g2s(st + MT_TILE, SB.img.lo + toff, MT_TILE, &full[s]);
         }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    if (lane == 0 && active) {
-      constexpr uint32_t idesc = ptx::make_idesc_bf16_f32(128, 128);
-      ptx::mbar_wait(a_full, 0);
-      ptx::tc_fence_after();
-      uint32_t it = 0;
-      for (int ct = 0; ct < n_ct; ++ct) {
-        const uint32_t buf = ct & 1, aph = (ct >> 1) & 1;
-        ptx::mbar_wait(&acc_empty[buf], aph ^ 1);
-        ptx::tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * 128;
-        for (int kb = 0; kb < MT_KB; ++kb, ++it) {
-          const int s = it % MT_STAGES;
-          const uint32_t ph = (it / MT_STAGES) & 1;
-          ptx::mbar_wait(&full[s], ph);
-          ptx::tc_fence_after();
-          const uint32_t a_hi = ptx::smem_u32(smem + kb * 2 * MT_TILE), a_lo = a_hi + MT_TILE;
-          const uint32_t b_hi = ptx::smem_u32(smem + MT_OFF_B + s * MT_STAGE), b_lo = b_hi + MT_TILE;
-#pragma unroll
-          for (int k16 = 0; k16 < 4; ++k16) {
-            const uint32_t ko = k16 * 32;
-            const uint64_t dah = ptx::make_sw128_kmajor_desc(a_hi + ko, 1024);
-            const uint64_t dal = ptx::make_sw128_kmajor_desc(a_lo + ko, 1024);
-            const uint64_t dbh = ptx::make_sw128_kmajor_desc(b_hi + ko, 1024);
-            const uint64_t dbl = ptx::make_sw128_kmajor_desc(b_lo + ko, 1024);
-            ptx::umma_bf16(d_tmem, dal, dbh, idesc, (kb | k16) != 0);
-            ptx::umma_bf16(d_tmem, dah, dbl, idesc, 1);
-            ptx::umma_bf16(d_tmem, dah, dbh, idesc, 1);
-          }
-          ptx::umma_commit(&empty[s]);
-        }
-        ptx::umma_commit(&acc_full[buf]);
-      }
-    }
   } else {
-    // ---------------------------------------------------------------- epilogue (8 warps)
-    // thread = accumulator row (TMEM lane) x one half of the tile's 128 columns; running best /
+    // ---------------------------------------------------------------- consumers (2 warpgroups x 64 rows)
+    // wgmma per 128-column tile of side B (accumulator in registers), then the tile goes through the staging
+    // blocks in 64-column chunks: thread = row (lane) x one 32-column half of each chunk; running best /
     // second-best over all column tiles stay in registers.
-    const int q = warp & 3, half = (warp - 2) >> 2;
+    const int wg = warp >> 2, q = warp & 3, half = warp >> 2;
+    const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    float* stg = stg_all + warp * 1024;
     const int r_in = q * 32 + lane;
     const int row = rb * 128 + r_in;             // line of side A inside the pair
     const bool valid_row = row < na;
@@ -198,15 +155,46 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
     const float sqa = (p.dist_mode == 1 && valid_row) ? SA.sq[ba + row] : 0.f;
     float* drow = (p.dist && side == 0 && valid_row) ? p.dist + (long long)pair * p.dist_stride + (long long)row * nb : nullptr;
     const bool dvec = drow && (nb % 8 == 0) && (p.dist_stride % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.dist) & 31) == 0);
+    if (active) ptx::mbar_wait(a_full, 0);
+    uint32_t it = 0;
     for (int ct = 0; ct < n_ct; ++ct) {
-      const uint32_t buf = ct & 1, aph = (ct >> 1) & 1;
-      ptx::mbar_wait(&acc_full[buf], aph);
-      ptx::tc_fence_after();
+      float d[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < MT_KB; ++kb, ++it) {
+        const int s = it % MT_STAGES;
+        ptx::mbar_wait(&full[s], (it / MT_STAGES) & 1);
+        const uint32_t a_hi = ptx::smem_u32(smem + kb * 2 * MT_TILE) + wg * 8192, a_lo = a_hi + MT_TILE;
+        const uint32_t b_hi = ptx::smem_u32(smem + MT_OFF_B + s * MT_STAGE), b_lo = b_hi + MT_TILE;
+        ptx::wg_fence_regs(d);
+        ptx::wg_fence();
+#pragma unroll
+        for (int k16 = 0; k16 < 4; ++k16) {
+          const uint32_t ko = k16 * 32;
+          const uint64_t dah = ptx::make_sw128_kmajor_desc(a_hi + ko, 1024);
+          const uint64_t dal = ptx::make_sw128_kmajor_desc(a_lo + ko, 1024);
+          const uint64_t dbh = ptx::make_sw128_kmajor_desc(b_hi + ko, 1024);
+          const uint64_t dbl = ptx::make_sw128_kmajor_desc(b_lo + ko, 1024);
+          ptx::wgmma_ss_n128(d, dal, dbh, (kb | k16) != 0);
+          ptx::wgmma_ss_n128(d, dah, dbl, 1);
+          ptx::wgmma_ss_n128(d, dah, dbh, 1);
+        }
+        ptx::wg_commit();
+        ptx::wg_wait<1>();
+        ptx::wg_fence_regs(d);
+        if (kb > 0 && lane == 0) ptx::mbar_arrive(&empty[(it - 1) % MT_STAGES]);
+      }
+      ptx::wg_wait<0>();
+      ptx::wg_fence_regs(d);
+      if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % MT_STAGES]);
 #pragma unroll 1
-      for (int c0 = half * 64; c0 < half * 64 + 64; c0 += 32) {
+      for (int ch = 0; ch < 2; ++ch) {
         float acc[32];
-        ptx::tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * 128 + (uint32_t)c0, acc);
-        const int j0 = ct * 128 + c0;            // first column (line of side B) of this chunk
+        mt_epi_bar();
+        stage_acc64(d, ch, stg_all, row_a, lane);
+        mt_epi_bar();
+        load_stage(stg, lane, acc);
+        const int j0 = ct * 128 + ch * 64 + half * 32;   // first column (line of side B) of this chunk
         if (j0 >= nb) continue;                  // whole chunk is padding
         if (p.dist_mode == 1) {
 #pragma unroll
@@ -258,9 +246,6 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
           }
         }
       }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&acc_empty[buf]);
     }
     // merge the two column halves of every row (lexicographic (value, index): first minimum wins)
     if (half == 1) {
@@ -278,9 +263,6 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
       SA.slot[ba + row] = make_uint2(__float_as_uint(best), (uint32_t)bidx | (amb ? 0x80000000u : 0u));
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem_base, 256);
 }
 
 // ---------------------------------------------------------------- fp32 descriptors -> pair-aligned tile images

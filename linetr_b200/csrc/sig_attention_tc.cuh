@@ -1,37 +1,53 @@
-// Line-signature attention on tensor cores (sm_100a): softmax(q k^T) v over the L_i lines of ONE
+// Line-signature attention on tensor cores (sm_90a): softmax(q k^T) v over the L_i lines of ONE
 // image, per head, no mask (attention(), models/line_transformer.py:132-136; 1/8 is folded into
 // W_q and the heads are head-major, see ltr_create).
 //
-// CTA = (128-query tile, head, image), 256 threads: thread pair <-> query row (TMEM lane), the two
-// threads of a pair own the two halves of the columns.  Per key tile of 128 lines:
+// CTA = (128-query tile, head, image), 256 threads = two warpgroups of 64 query rows each; the
+// accumulators live in registers (wgmma fragment: a thread holds two rows, a quad of threads a row).
+// Per key tile of 128 lines:
 //   * q, k, v arrive as the split-bf16 tile image the qkv GEMM epilogue wrote (k-block h = q of head h,
 //     4 + h = k, 8 + h = v).  Images of the batch are not 128-row aligned in the row space, so the
 //     operand tiles are assembled from 16-byte chunks with cp.async (re-swizzled for the new row
 //     phase, rows past the image zero-filled) - no conversion, no registers, all copies in flight;
 //     v lands behind the S MMA.  V is staged exactly like K ([keys x 64 dims]) and consumed as an
 //     MN-major B operand - no transpose anywhere.
-//   * S = Q K^T      tcgen05 (M128 N128 K64, 3 split products), accumulator in TMEM
+//   * S = Q K^T      wgmma (M64 N128 K64 per warpgroup, 3 split products)
 //   * p = exp(s - m), row sums in registers; P written as the A operand of the second MMA
 //     (re-using the Q/K shared memory, which is dead once S is complete)
-//   * O += P V       tcgen05 (M128 N64 K128), accumulated in TMEM across key tiles
+//   * O += P V       wgmma (M64 N64 K128 per warpgroup), accumulated in registers across key tiles
 // Images with more than 128 lines run a first pass that only computes the row maxima (S is
 // recomputed in the second pass - QK^T is 1/3 of the work and far from the bottleneck), so no
-// rescaling of the TMEM accumulator is ever needed.  Output: columns [out_k0, out_k0+256) of a split-bf16
+// rescaling of the accumulator is ever needed.  Output: columns [out_k0, out_k0+256) of a split-bf16
 // activation image (the second half of the signature MLP input; the `merge` projection is folded into W1).
 #pragma once
 #include "act_img.cuh"
 #include "common.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltr {
 
 struct SigAttnSmem {
   static constexpr int QK = 64 * 1024;   // Q hi/lo + K hi/lo (4 x 16 KB); later P hi/lo (2 x 32 KB)
   static constexpr int V = 32 * 1024;    // V hi/lo: [128 keys x 64 d] each
-  static constexpr int OFF_RED = QK + V;             // float [2][128] pair reduction scratch
-  static constexpr int OFF_BAR = OFF_RED + 2 * 128 * 4;
+  static constexpr int OFF_BAR = QK + V;
   static constexpr int TOTAL = OFF_BAR + 64 + 1024;
 };
+
+// the S accumulator of one warpgroup (64 rows x 128 keys) from the staged Q and K tiles
+__device__ __forceinline__ void attn_qk(float (&d)[64], uint32_t qh, uint32_t ql, uint32_t kh, uint32_t kl) {
+  ptx::wg_fence_regs(d);
+  ptx::wg_fence();
+#pragma unroll
+  for (int k16 = 0; k16 < 4; ++k16) {
+    const uint32_t ko = k16 * 32;
+    ptx::wgmma_ss_n128(d, ptx::make_sw128_kmajor_desc(ql + ko, 1024), ptx::make_sw128_kmajor_desc(kh + ko, 1024), k16 != 0);
+    ptx::wgmma_ss_n128(d, ptx::make_sw128_kmajor_desc(qh + ko, 1024), ptx::make_sw128_kmajor_desc(kl + ko, 1024), 1);
+    ptx::wgmma_ss_n128(d, ptx::make_sw128_kmajor_desc(qh + ko, 1024), ptx::make_sw128_kmajor_desc(kh + ko, 1024), 1);
+  }
+  ptx::wg_commit();
+  ptx::wg_wait<0>();
+  ptx::wg_fence_regs(d);
+}
 
 __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActImg out, int out_k0,
                                                                 const int* __restrict__ cu, int lpi) {
@@ -44,8 +60,9 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
   const int q0 = blockIdx.x * 128;
   if (!cu && q0 >= L) return;
   const int h = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int qd = warp & 3, half = warp >> 2;
-  const int row = qd * 32 + lane;   // query row of this thread (shared with its pair thread)
+  const int wg = warp >> 2;
+  const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // query rows row_a and row_a + 8 of this thread
+  const int cq = 2 * (lane & 3);                                 // first of the thread's two columns per 8-column group
   if (tid == 0) LTR_DBG_STAMP(30);
   pdl_launch_dependents();
 
@@ -60,41 +77,21 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
   uint8_t* p_lo = smem + 32768;
   uint8_t* v_hi = smem + S::QK;         // [128 keys x 64 d]
   uint8_t* v_lo = v_hi + 16384;
-  float* red = reinterpret_cast<float*>(smem + S::OFF_RED);
-  uint64_t* mma_done = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
-  uint64_t* ld_qk = mma_done + 1;      // TMA path: q and k tiles landed
-  uint64_t* ld_v = mma_done + 2;       // TMA path: v tile landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(mma_done + 3);
+  uint64_t* ld_qk = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);   // TMA path: q and k tiles landed
+  uint64_t* ld_v = ld_qk + 1;                                         // TMA path: v tile landed
 
   if (tid == 0) {
-    ptx::mbar_init(mma_done, 1);
     ptx::mbar_init(ld_qk, 1);
     ptx::mbar_init(ld_v, 1);
     ptx::fence_mbar_init();
   }
-  if (warp == 0) {
-    ptx::tmem_alloc(tmem_slot, 256);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t t_s = tmem_base;          // S: 128 columns
-  const uint32_t t_o = tmem_base + 128;    // O: 64 columns
-  const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-  uint32_t phase = 0;
   pdl_wait();   // qkv of this layer is complete; the previous reader of the output image is done
   if (tid == 0) LTR_DBG_STAMP(31);
   if (cu) {
     lb = cu[blockIdx.z]; le = cu[blockIdx.z + 1];
     L = le - lb;
-    if (q0 >= L) {   // uniform per CTA: give the TMEM columns back and leave
-      ptx::tc_fence_before();
-      __syncthreads();
-      if (warp == 0) ptx::tmem_dealloc(tmem_base, 256);
-      return;
-    }
+    if (q0 >= L) return;   // uniform per CTA
   }
 
   // [128 rows x 64] operand tile (hi and lo plane) <- rows row0.. of this image, k-block kb of the qkv image:
@@ -111,39 +108,23 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
       ptx::cp_async16(lo + dst, reinterpret_cast<const uint8_t*>(qkv.lo) + src, ok ? 16u : 0u);
     }
   };
-  auto issue_s = [&]() {   // S = Q K^T
-    constexpr uint32_t idesc = ptx::make_idesc_bf16_f32(128, 128);
-    const uint32_t qh = ptx::smem_u32(q_hi), ql = ptx::smem_u32(q_lo), kh = ptx::smem_u32(k_hi), kl = ptx::smem_u32(k_lo);
+  const uint32_t qh = ptx::smem_u32(q_hi) + wg * 8192, ql = ptx::smem_u32(q_lo) + wg * 8192;
+  const uint32_t kh = ptx::smem_u32(k_hi), kl = ptx::smem_u32(k_lo);
+  // row maxima of this thread's two rows over the valid key columns of S (a quad shares a row)
+  auto row_max = [&](const float (&sd)[64], int kn, float& m0, float& m1) {
 #pragma unroll
-    for (int k16 = 0; k16 < 4; ++k16) {
-      const uint32_t ko = k16 * 32;
-      ptx::umma_bf16(t_s, ptx::make_sw128_kmajor_desc(ql + ko, 1024), ptx::make_sw128_kmajor_desc(kh + ko, 1024), idesc, k16 != 0);
-      ptx::umma_bf16(t_s, ptx::make_sw128_kmajor_desc(qh + ko, 1024), ptx::make_sw128_kmajor_desc(kl + ko, 1024), idesc, 1);
-      ptx::umma_bf16(t_s, ptx::make_sw128_kmajor_desc(qh + ko, 1024), ptx::make_sw128_kmajor_desc(kh + ko, 1024), idesc, 1);
-    }
-    ptx::umma_commit(mma_done);
-  };
-  auto wait_mma = [&]() {
-    ptx::mbar_wait(mma_done, phase & 1);
-    ++phase;
-    ptx::tc_fence_after();
-  };
-  // row maximum over this thread's 64 columns of S, combined with the pair thread through smem
-  auto row_max = [&](int kn, float m_in) {
-    float m = m_in;
-#pragma unroll 1
-    for (int c0 = half * 64; c0 < half * 64 + 64; c0 += 32) {
-      float s[32];
-      ptx::tmem_ld32(t_s + lane_addr + c0, s);
+    for (int j = 0; j < 16; ++j)
 #pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (c0 + j < kn) m = fmaxf(m, s[j]);
+      for (int e = 0; e < 2; ++e)
+        if (8 * j + cq + e < kn) {
+          m0 = fmaxf(m0, sd[4 * j + e]);
+          m1 = fmaxf(m1, sd[4 * j + 2 + e]);
+        }
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+      m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
     }
-    red[half * 128 + row] = m;
-    __syncthreads();
-    m = fmaxf(red[row], red[128 + row]);
-    __syncthreads();
-    return m;
   };
 
   const int n_kt = (L + 127) / 128;
@@ -151,7 +132,8 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
   // q, k, v operand tiles ARE tiles of that image - six 16 KB bulk copies (TMA) by one thread instead of 24 cp.async
   // per thread; v still lands behind the S MMA.  Single key tile: the shared memory is written exactly once.
   const bool tma = L == 128 && ((lb & 127) == 0);
-  float m = -INFINITY;
+  float m0 = -INFINITY, m1 = -INFINITY;
+  float sd[64];
   if (n_kt > 1) {
     // ---- pass 1: row maxima over all key tiles
     for (int kt = 0; kt < n_kt; ++kt) {
@@ -161,14 +143,15 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
       ptx::cp_async_wait_all();
       ptx::fence_proxy_async_smem();
       __syncthreads();
-      if (tid == 0) { ptx::tc_fence_after(); issue_s(); }
-      wait_mma();
-      m = row_max(kn, m);
-      ptx::tc_fence_before();
+      attn_qk(sd, qh, ql, kh, kl);
+      row_max(sd, kn, m0, m1);
       __syncthreads();
     }
   }
-  float l = 0.f;
+  float l0 = 0.f, l1 = 0.f;
+  float od[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) od[i] = 0.f;
   constexpr float LOG2E = 1.4426950408889634f;
   for (int kt = 0; kt < n_kt; ++kt) {
     const int k0 = kt * 128, kn = min(128, L - k0);
@@ -186,94 +169,91 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
         ptx::bulk_g2s(v_hi, qkv.hi + tv, 16384, ld_v);
         ptx::bulk_g2s(v_lo, qkv.lo + tv, 16384, ld_v);
       }
-      if (tid == 0) LTR_DBG_STAMP(33);
       ptx::mbar_wait(ld_qk, 0);
-      if (tid == 0) LTR_DBG_STAMP(34);
     } else {
       stage_tile(q0, h, q_hi, q_lo);
       stage_tile(k0, 4 + h, k_hi, k_lo);
       ptx::cp_async_commit();
       stage_tile(k0, 8 + h, v_hi, v_lo);
       ptx::cp_async_commit();
-      if (tid == 0) LTR_DBG_STAMP(33);
       ptx::cp_async_wait_group<1>();   // q and k have landed; v is still in flight behind the S MMA
-      if (tid == 0) LTR_DBG_STAMP(34);
       ptx::fence_proxy_async_smem();
     }
     __syncthreads();
-    if (tid == 0) { ptx::tc_fence_after(); issue_s(); }
-    wait_mma();
+    attn_qk(sd, qh, ql, kh, kl);
     if (tid == 0) LTR_DBG_STAMP(35);
-    if (n_kt == 1) m = row_max(kn, m);
-    // p = exp(s - m) -> P operand (q/k shared memory is dead: the S MMAs have completed);
-    // this thread's 64 key columns are exactly k-block `half` of the P tile
-    const float mb = m * LOG2E;
-#pragma unroll 1
-    for (int c0 = half * 64; c0 < half * 64 + 64; c0 += 32) {
-      float s[32];
-      ptx::tmem_ld32(t_s + lane_addr + c0, s);
+    if (n_kt == 1) row_max(sd, kn, m0, m1);
+    __syncthreads();   // both warpgroups are done reading Q / K: P may overwrite them
+    // p = exp(s - m) -> P operand: key column c of row r at k-block c / 64 of the P tile
+    const float mb0 = m0 * LOG2E, mb1 = m1 * LOG2E;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        s[j] = (c0 + j < kn) ? ptx::ex2_approx(fmaf(s[j], LOG2E, -mb)) : 0.f;
-        l += s[j];
-      }
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        uint4 hh, ll;
-        ptx::split8_bf16(&s[j], hh, ll);
-        const uint32_t off = half * 16384 + ptx::sw128_offset(row, (c0 & 63) + j);
-        *reinterpret_cast<uint4*>(p_hi + off) = hh;
-        *reinterpret_cast<uint4*>(p_lo + off) = ll;
-      }
+    for (int j = 0; j < 16; ++j) {
+      const int c = 8 * j + cq;
+      const bool v0 = c < kn, v1 = c + 1 < kn;
+      const float p00 = v0 ? ptx::ex2_approx(fmaf(sd[4 * j], LOG2E, -mb0)) : 0.f;
+      const float p01 = v1 ? ptx::ex2_approx(fmaf(sd[4 * j + 1], LOG2E, -mb0)) : 0.f;
+      const float p10 = v0 ? ptx::ex2_approx(fmaf(sd[4 * j + 2], LOG2E, -mb1)) : 0.f;
+      const float p11 = v1 ? ptx::ex2_approx(fmaf(sd[4 * j + 3], LOG2E, -mb1)) : 0.f;
+      l0 += p00 + p01;
+      l1 += p10 + p11;
+      uint32_t hh, ll;
+      const uint32_t off0 = (c >> 6) * 16384 + ptx::sw128_offset(row_a, c & 63);
+      const uint32_t off1 = (c >> 6) * 16384 + ptx::sw128_offset(row_a + 8, c & 63);
+      ptx::split2_bf16(p00, p01, hh, ll);
+      *reinterpret_cast<uint32_t*>(p_hi + off0) = hh;
+      *reinterpret_cast<uint32_t*>(p_lo + off0) = ll;
+      ptx::split2_bf16(p10, p11, hh, ll);
+      *reinterpret_cast<uint32_t*>(p_hi + off1) = hh;
+      *reinterpret_cast<uint32_t*>(p_lo + off1) = ll;
     }
     if (tma) ptx::mbar_wait(ld_v, 0);
     else ptx::cp_async_wait_group<0>();   // v
-    ptx::tc_fence_before();
     ptx::fence_proxy_async_smem();
-    if (tid == 0) LTR_DBG_STAMP(36);
     __syncthreads();
-    if (tid == 0) {   // O += P V    (B = V as an MN-major operand: [K = keys][N = 64 dims])
-      ptx::tc_fence_after();
-      constexpr uint32_t idesc = ptx::make_idesc_bf16_f32(128, 64) | (1u << 16);
-      const uint32_t ph = ptx::smem_u32(p_hi), pl = ptx::smem_u32(p_lo), vh = ptx::smem_u32(v_hi), vl = ptx::smem_u32(v_lo);
+    {   // O += P V    (B = V as an MN-major operand: [K = keys][N = 64 dims])
+      const uint32_t ph = ptx::smem_u32(p_hi) + wg * 8192, pl = ptx::smem_u32(p_lo) + wg * 8192;
+      const uint32_t vh = ptx::smem_u32(v_hi), vl = ptx::smem_u32(v_lo);
+      ptx::wg_fence_regs(od);
+      ptx::wg_fence();
 #pragma unroll
       for (int kb = 0; kb < 2; ++kb) {
 #pragma unroll
         for (int k16 = 0; k16 < 4; ++k16) {
           const uint32_t pa = kb * 16384 + k16 * 32;          // A: 16 keys = 32 bytes along K
           const uint32_t va = (kb * 4 + k16) * 2048;          // B: 16 key rows of 128 bytes
-          const uint32_t first = (kt | kb | k16) == 0 ? 0u : 1u;
-          ptx::umma_bf16(t_o, ptx::make_sw128_kmajor_desc(pl + pa, 1024), ptx::make_sw128_mnmajor_desc(vh + va, 1024, 1024), idesc, first);
-          ptx::umma_bf16(t_o, ptx::make_sw128_kmajor_desc(ph + pa, 1024), ptx::make_sw128_mnmajor_desc(vl + va, 1024, 1024), idesc, 1);
-          ptx::umma_bf16(t_o, ptx::make_sw128_kmajor_desc(ph + pa, 1024), ptx::make_sw128_mnmajor_desc(vh + va, 1024, 1024), idesc, 1);
+          ptx::wgmma_ss_n64_tb(od, ptx::make_sw128_kmajor_desc(pl + pa, 1024), ptx::make_sw128_mnmajor_desc(vh + va, 1024, 1024), 1);
+          ptx::wgmma_ss_n64_tb(od, ptx::make_sw128_kmajor_desc(ph + pa, 1024), ptx::make_sw128_mnmajor_desc(vl + va, 1024, 1024), 1);
+          ptx::wgmma_ss_n64_tb(od, ptx::make_sw128_kmajor_desc(ph + pa, 1024), ptx::make_sw128_mnmajor_desc(vh + va, 1024, 1024), 1);
         }
       }
-      ptx::umma_commit(mma_done);
+      ptx::wg_commit();
+      ptx::wg_wait<0>();
+      ptx::wg_fence_regs(od);
     }
-    wait_mma();   // P, V shared memory may be overwritten by the next key tile
+    __syncthreads();   // P, V shared memory may be overwritten by the next key tile
     if (tid == 0) LTR_DBG_STAMP(37);
   }
-  // ---- epilogue: o / l -> image (this thread: 32 of the 64 head dims)
+  // ---- epilogue: o / l -> image (this thread: rows row_a, row_a + 8, dims 8 j + cq, + 1)
   {
-    red[half * 128 + row] = l;
-    __syncthreads();
-    const float inv = 1.f / (red[row] + red[128 + row]);
-    const bool live = q0 + row < L;
-    float o[32];
-    ptx::tmem_ld32(t_o + lane_addr + half * 32, o);
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+      l0 += __shfl_xor_sync(0xffffffffu, l0, o);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, o);
+    }
+    const float inv0 = 1.f / l0, inv1 = 1.f / l1;
     if (tma) {
       // aligned 128-line image: this CTA's output (128 rows x 64 head dims) is ONE k-block tile of the output image -
       // stage hi / lo planes in tile layout (the P operand's memory is dead: the PV MMAs have completed) and store each
-      // with one 16 KB bulk copy instead of eight scattered 16-byte stores per thread
+      // with one 16 KB bulk copy
 #pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        const float v[8] = {o[j] * inv, o[j + 1] * inv, o[j + 2] * inv, o[j + 3] * inv,
-                            o[j + 4] * inv, o[j + 5] * inv, o[j + 6] * inv, o[j + 7] * inv};
-        uint4 hh, ll;
-        ptx::split8_bf16(v, hh, ll);
-        const uint32_t off = ptx::sw128_offset(row, half * 32 + j);
-        *reinterpret_cast<uint4*>(smem + off) = hh;
-        *reinterpret_cast<uint4*>(smem + 16384 + off) = ll;
+      for (int j = 0; j < 8; ++j) {
+        uint32_t hh, ll;
+        ptx::split2_bf16(od[4 * j] * inv0, od[4 * j + 1] * inv0, hh, ll);
+        *reinterpret_cast<uint32_t*>(smem + ptx::sw128_offset(row_a, 8 * j + cq)) = hh;
+        *reinterpret_cast<uint32_t*>(smem + 16384 + ptx::sw128_offset(row_a, 8 * j + cq)) = ll;
+        ptx::split2_bf16(od[4 * j + 2] * inv1, od[4 * j + 3] * inv1, hh, ll);
+        *reinterpret_cast<uint32_t*>(smem + ptx::sw128_offset(row_a + 8, 8 * j + cq)) = hh;
+        *reinterpret_cast<uint32_t*>(smem + 16384 + ptx::sw128_offset(row_a + 8, 8 * j + cq)) = ll;
       }
       ptx::fence_proxy_async_smem();
       __syncthreads();
@@ -286,19 +266,24 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
         // complete (and visible to the next kernel behind griddepcontrol.wait) when the grid is
         ptx::bulk_wait_read_all();
       }
-    } else if (live) {
+    } else {
 #pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        const float v[8] = {o[j] * inv, o[j + 1] * inv, o[j + 2] * inv, o[j + 3] * inv,
-                            o[j + 4] * inv, o[j + 5] * inv, o[j + 6] * inv, o[j + 7] * inv};
-        img_store8(out, lb + q0 + row, out_k0 + h * 64 + half * 32 + j, v);
+      for (int e = 0; e < 2; ++e) {
+        const int r = row_a + 8 * e;
+        if (q0 + r >= L) continue;
+        const float inv = e ? inv1 : inv0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          uint32_t hh, ll;
+          ptx::split2_bf16(od[4 * j + 2 * e] * inv, od[4 * j + 2 * e + 1] * inv, hh, ll);
+          const size_t i = img_index(out, lb + q0 + r, out_k0 + h * 64 + 8 * j + cq);
+          *reinterpret_cast<uint32_t*>(out.hi + i) = hh;
+          *reinterpret_cast<uint32_t*>(out.lo + i) = ll;
+        }
       }
     }
   }
   if (tid == 0) LTR_DBG_STAMP(38);
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) ptx::tmem_dealloc(tmem_base, 256);
 }
 
 inline int launch_sig_attention_tc(ActImg qkv, ActImg out, int out_k0, const int* cu, int lpi, int max_l,

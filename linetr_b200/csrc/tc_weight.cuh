@@ -7,7 +7,7 @@
 #include <cstring>
 #include "common.cuh"
 #include "linear_f32.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltr {
 

@@ -1,12 +1,12 @@
-// Fused token stage of the line-descriptor forward (sm_100a, tcgen05 + TMA).
+// Fused token stage of the line-descriptor forward (sm_90a, wgmma + TMA).
 //
 // One persistent CTA per SM walks tiles of LPT = floor(128 / T) whole lines (LPT*T <= 128 token
 // rows).  Per tile, entirely on chip:
-//   P0  3 -> 32 (+ReLU) on CUDA cores                                        -> h32  (TMEM, split-bf16)
-//   L2  32 -> 64 (+ReLU)    tcgen05 (N = 64, two K steps)                    -> h64
-//   L3  64 -> 128 (+ReLU)   tcgen05, accumulator in TMEM, epilogue -> TMEM   -> h128
-//   L4  128 -> 256 (+ReLU)  tcgen05                                          -> h256
-//   L5  256 -> 256          tcgen05, epilogue adds the sampled descriptors   -> x = desc + wpe (fp32, smem)
+//   P0  3 -> 32 (+ReLU) on CUDA cores                                        -> h32  (registers, split-bf16)
+//   L2  32 -> 64 (+ReLU)    wgmma (N = 64, two K steps)                      -> h64
+//   L3  64 -> 128 (+ReLU)   wgmma                                            -> h128
+//   L4  128 -> 256 (+ReLU)  wgmma, two n-blocks of 128                       -> h256
+//   L5  256 -> 256          wgmma, epilogue adds the sampled descriptors     -> x = desc + wpe (fp32, smem)
 //   CLS pooling: folded CLS-query scores x.u_h, softmax over the T tokens + CLS per head,
 //       z_h = sum_n p_h[n] x[n]                                               -> z image (global)
 // Replaces WordPositionalEncoder (models/line_transformer.py:61-73), `desc + pos` and the CLS
@@ -16,29 +16,20 @@
 // SWIZZLE_128B tensor-map TMA per 32-column block of the tile), the weights (L2 resident, streamed
 // by 1-D TMA through a 2-slot ring) and the pooled z leave/enter the SM.
 //
-// The activations never touch shared memory: the A operand of every layer lives in TENSOR MEMORY
-// (tcgen05.mma with A from TMEM) as split-bf16 - packed hi pairs and packed lo pairs, written by the
-// previous layer's epilogue with tcgen05.st.  With A in shared memory a 128 x 128 x 16 MMA read
-// 8 KB of operands per 64 cycles - the whole 128 B/clk of the SM's shared memory - while the weight
-// ring and the descriptor stream were writing into the same memory (L5: 9.9 k cycles for 6.1 k of
-// MMAs); and the 128 KB activation image shared its memory with the tile's descriptors, so the last
-// descriptor group could only be fetched after L5 (it landed 6.1 k cycles into the L5 epilogue).
-// Now the 128 KB are the descriptor / x tile alone: the next tile's descriptors are requested the
-// moment the pooling of this tile has read x, and land under the next tile's P0 .. L5.
-// TMEM columns (512): accumulators [0, 256); h128 hi [256, 320) lo [320, 384);
-// h32 hi [256, 272) lo [272, 288); h64 hi [384, 416) lo [416, 448); h256: k < 128 hi [384, 448) lo [448, 512), k >= 128 hi [256, 320)
-// lo [320, 384) - the first half of h256 is written while L4's second n-block still reads h128.
+// The activations never touch shared memory: every layer is a register-A wgmma, and the accumulator
+// fragment of a layer (after bias, ReLU and the split into packed bf16 hi / lo pairs) is exactly the A
+// fragment of the next layer.  The 128 KB of shared memory beside the weight ring are the descriptor /
+// x tile alone: the next tile's descriptors are requested the moment the pooling of this tile has read x.
 //
-// Warp roles: warp 0 = TMA weight producer, warp 1 = MMA issuer (+TMEM alloc, descriptor TMA),
-// warps 2-9 = 256 worker threads (thread pair per token row: lane = row within the warp's TMEM lane
-// quarter; the pair splits every 128-column n-block of a layer in halves, so the first n-block's
-// epilogue runs under the second n-block's MMAs).
+// Warp roles: warps 0-7 = two warpgroups of 64 token rows (MMA, epilogues, softmax and pooling),
+// warps 8-11 = producer warpgroup (its first lane streams the weights by TMA; it hands its registers to the
+// workers with setmaxnreg: 128 x 40 + 256 x 232 <= 64 K).
 #pragma once
 #include <cuda.h>   // CUtensorMap (types only; the encoder is fetched through cudaGetDriverEntryPoint)
 #include "act_img.cuh"
 #include "common.cuh"
 #include "tc_weight.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 
 namespace ltr {
 
@@ -59,7 +50,7 @@ struct TokenFusedArgs {
 };
 
 struct TokenFusedSmem {
-  static constexpr int ACT = 128 * 1024;   // the descriptor / x tile (fp32); the activations live in tensor memory
+  static constexpr int ACT = 128 * 1024;   // the descriptor / x tile (fp32); the activations live in registers
   static constexpr int SLOT = 32 * 1024;   // one W tile [128 n x 64 k] hi + lo
   static constexpr int NSLOT = 2;
   static constexpr int OFF_RING = ACT;
@@ -79,12 +70,51 @@ struct TokenFusedSmem {
 
 // x tile: 8 column blocks of [128 rows x 32 fp32 (128 B)], each row's eight
 // 16-byte chunks XOR-swizzled by row & 7 - the layout a SWIZZLE_128B tensor-map box load produces.
-// Conflict-free both for a thread per row (L5 epilogue) and for a thread per channel quad (pooling).
+// Conflict-free for a thread per channel quad (pooling).
 __device__ __forceinline__ int xs_index(int row, int col) {
   return (col >> 5) * 4096 + row * 32 + (((((col >> 2) & 7) ^ (row & 7)) << 2) | (col & 3));
 }
 
-__global__ void __launch_bounds__(320, 1) token_fused_kernel(TokenFusedArgs p, const __grid_constant__ CUtensorMap desc_map) {
+// relu(acc + bias) of a warpgroup accumulator fragment (N = 2 NR columns) -> split-bf16 A fragments of the next layer,
+// K = 16 steps KK0 .. KK0 + NR / 8 (a K = 16 step of A takes the columns of two 8-column accumulator groups)
+template <int KK0, int NR, int NK>
+__device__ __forceinline__ void acc_to_afrag(const float (&d)[NR], const float* bias, int cq, uint32_t (&ah)[NK][4], uint32_t (&al)[NK][4]) {
+#pragma unroll
+  for (int kk = 0; kk < NR / 8; ++kk)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int jj = 2 * kk + (e >> 1), hr = (e & 1) * 2, c = 8 * jj + cq;
+      const float v0 = fmaxf(d[4 * jj + hr] + bias[c], 0.f), v1 = fmaxf(d[4 * jj + hr + 1] + bias[c + 1], 0.f);
+      ptx::split2_bf16(v0, v1, ah[KK0 + kk][e], al[KK0 + kk][e]);
+    }
+}
+
+// One W slot (64 k) of a layer: A fragments KA0 .. KA0 + NK16 - 1, three split products per K = 16 step
+template <int KA0, int NK16, int NR, int NK>
+__device__ __forceinline__ void slot_mma(float (&d)[NR], const uint32_t (&ah)[NK][4], const uint32_t (&al)[NK][4], uint32_t w_hi,
+                                         bool first) {
+  ptx::wg_fence_regs(d);
+  ptx::wg_fence();
+#pragma unroll
+  for (int k16 = 0; k16 < NK16; ++k16) {
+    const uint64_t dwh = ptx::make_sw128_kmajor_desc(w_hi + k16 * 32, 1024);
+    const uint64_t dwl = ptx::make_sw128_kmajor_desc(w_hi + 16384 + k16 * 32, 1024);
+    if constexpr (NR == 32) {
+      ptx::wgmma_rs_n64(d, al[KA0 + k16], dwh, (first && k16 == 0) ? 0u : 1u);
+      ptx::wgmma_rs_n64(d, ah[KA0 + k16], dwl, 1);
+      ptx::wgmma_rs_n64(d, ah[KA0 + k16], dwh, 1);
+    } else {
+      ptx::wgmma_rs_n128(d, al[KA0 + k16], dwh, (first && k16 == 0) ? 0u : 1u);
+      ptx::wgmma_rs_n128(d, ah[KA0 + k16], dwl, 1);
+      ptx::wgmma_rs_n128(d, ah[KA0 + k16], dwh, 1);
+    }
+  }
+  ptx::wg_commit();
+  ptx::wg_wait<0>();
+  ptx::wg_fence_regs(d);
+}
+
+__global__ void __launch_bounds__(384, 1) token_fused_kernel(TokenFusedArgs p, const __grid_constant__ CUtensorMap desc_map) {
   using S = TokenFusedSmem;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
@@ -102,12 +132,9 @@ __global__ void __launch_bounds__(320, 1) token_fused_kernel(TokenFusedArgs p, c
   float* sP = reinterpret_cast<float*>(smem + S::OFF_P);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
   uint64_t* full = bars;            // [2] W slot filled (TMA tx)
-  uint64_t* empty = bars + 2;       // [2] W slot consumed (tcgen05.commit)
-  uint64_t* a_ready = bars + 4;     // workers -> MMA: A operand complete in tensor memory (256 arrivals)
-  uint64_t* acc_bar = bars + 5;     // [2] MMA -> workers: first / second 128-column n-block of the layer complete (tcgen05.commit)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 7);
-  uint64_t* dbar = bars + 8;        // [4] descriptor columns {32 s .. 32 s + 32} u {128 + 32 s ..} of the tile have landed
-  uint64_t* x_free = bars + 12;     // workers -> MMA thread: the pooling has read the x tile (256 arrivals)
+  uint64_t* empty = bars + 2;       // [2] W slot consumed (8 consumer warps)
+  uint64_t* dbar = bars + 4;        // [4] descriptor columns {32 s .. 32 s + 32} u {128 + 32 s ..} of the tile have landed
+  uint64_t* x_free = bars + 8;      // workers -> descriptor request: the pooling has read the x tile (256 arrivals)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   pdl_launch_dependents();
@@ -118,164 +145,64 @@ __global__ void __launch_bounds__(320, 1) token_fused_kernel(TokenFusedArgs p, c
   for (int i = tid; i < 128; i += blockDim.x) sB3[i] = p.b3[i];
   for (int i = tid; i < 256; i += blockDim.x) { sB4[i] = p.b4[i]; sB5[i] = p.b5[i]; sCls[i] = p.cls[i]; }
   for (int i = tid; i < 1024; i += blockDim.x) sU[i] = p.U[i];
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 1); }
-    ptx::mbar_init(a_ready, 256);
-    ptx::mbar_init(&acc_bar[0], 1);
-    ptx::mbar_init(&acc_bar[1], 1);
+  if (tid == 0) {
+    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&full[s], 1); ptx::mbar_init(&empty[s], 8); }
     for (int i = 0; i < 4; ++i) ptx::mbar_init(&dbar[i], 1);
     ptx::mbar_init(x_free, 256);
     ptx::prefetch_tensormap(&desc_map);
     ptx::fence_mbar_init();
   }
-  if (warp == 1) {
-    ptx::tmem_alloc(tmem_slot, 512);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // tensor-memory columns (see the header)
-  constexpr uint32_t T_H128_HI = 256, T_H128_LO = 320, T_H64_HI = 384, T_H64_LO = 416, T_H32_HI = 256, T_H32_LO = 272;
-  constexpr uint32_t T_H256A_HI = 384, T_H256A_LO = 448, T_H256B_HI = 256, T_H256B_LO = 320;   // A: k < 128, B: k >= 128
   pdl_wait();   // z (output image) may still be read by the previous launch sequence
 
-  if (warp == 0) {
+  if (warp >= 8) {
     // ---------------------------------------------------------------- W producer: 14 slots per tile
-    {
-      uint32_t it = 0;
-      auto push = [&](const TcWeight& W, int nb, int kb) {
-        const int s = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
-        ptx::mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* dst = smem + S::OFF_RING + s * S::SLOT;
-        const size_t off = ((size_t)kb * (W.N / 8) + (size_t)nb * 16) * 1024;
-        const uint32_t bytes = (uint32_t)min(128, W.N - nb * 128) * 128u;   // rows of this n-block x 128 B, per plane
-        ptx::mbar_arrive_expect_tx(&full[s], 2 * bytes);
-        ptx::bulk_g2s(dst, reinterpret_cast<const uint8_t*>(W.hi) + off, bytes, &full[s]);
-        ptx::bulk_g2s(dst + 16384, reinterpret_cast<const uint8_t*>(W.lo) + off, bytes, &full[s]);
-        ++it;
-      };
-      if (lane == 0) {
-        for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-          push(p.W2, 0, 0);
-          push(p.W3, 0, 0);
-          for (int nb = 0; nb < 2; ++nb)
-            for (int kb = 0; kb < 2; ++kb) push(p.W4, nb, kb);
-          for (int nb = 0; nb < 2; ++nb)
-            for (int kb = 0; kb < 4; ++kb) push(p.W5, nb, kb);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc128 = ptx::make_idesc_bf16_f32(128, 128), idesc64 = ptx::make_idesc_bf16_f32(128, 64);
-      uint32_t it = 0, na = 0;
-      // one [128 x 128 x 64] block: K steps k0 .. k0 + 3 (16 wide) of an A operand whose packed hi / lo pairs start at
-      // tensor-memory columns a_hi / a_lo (8 columns per step), W from the ring, accumulator columns nb * 128 ..
-      auto block = [&](uint32_t a_hi, uint32_t a_lo, int nb, bool first, uint32_t idesc, int nk16) {
-        const int s = it & 1;
-        const uint32_t ph = (it >> 1) & 1;
-        ptx::mbar_wait(&full[s], ph);
-        ptx::tc_fence_after();
-        const uint32_t w_hi = ptx::smem_u32(smem + S::OFF_RING + s * S::SLOT), w_lo = w_hi + 16384;
-        const uint32_t d = tmem_base + nb * 128;
-#pragma unroll
-        for (int k16 = 0; k16 < 4; ++k16) {
-          if (k16 >= nk16) break;
-          const uint32_t ko = k16 * 32;
-          const uint64_t dwh = ptx::make_sw128_kmajor_desc(w_hi + ko, 1024);
-          const uint64_t dwl = ptx::make_sw128_kmajor_desc(w_lo + ko, 1024);
-          ptx::umma_bf16_ts(d, tmem_base + a_lo + k16 * 8, dwh, idesc, !(first && k16 == 0));
-          ptx::umma_bf16_ts(d, tmem_base + a_hi + k16 * 8, dwl, idesc, 1);
-          ptx::umma_bf16_ts(d, tmem_base + a_hi + k16 * 8, dwh, idesc, 1);
-        }
-        ptx::umma_commit(&empty[s]);
-        ++it;
-      };
+    ptx::setmaxnreg_dec<40>();
+    uint32_t it = 0;
+    auto push = [&](const TcWeight& W, int nb, int kb) {
+      const int s = it & 1;
+      const uint32_t ph = (it >> 1) & 1;
+      ptx::mbar_wait(&empty[s], ph ^ 1);
+      uint8_t* dst = smem + S::OFF_RING + s * S::SLOT;
+      const size_t off = ((size_t)kb * (W.N / 8) + (size_t)nb * 16) * 1024;
+      const uint32_t bytes = (uint32_t)min(128, W.N - nb * 128) * 128u;   // rows of this n-block x 128 B, per plane
+      ptx::mbar_arrive_expect_tx(&full[s], 2 * bytes);
+      ptx::bulk_g2s(dst, reinterpret_cast<const uint8_t*>(W.hi) + off, bytes, &full[s]);
+      ptx::bulk_g2s(dst + 16384, reinterpret_cast<const uint8_t*>(W.lo) + off, bytes, &full[s]);
+      ++it;
+    };
+    if (warp == 8 && lane == 0) {
       for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
-        ptx::mbar_wait(a_ready, na++ & 1);   // h32
-        ptx::tc_fence_after();
-        block(T_H32_HI, T_H32_LO, 0, true, idesc64, 2);   // K = 32: the k-block's upper half is zero padding
-        ptx::umma_commit(&acc_bar[0]);
-        ptx::mbar_wait(a_ready, na++ & 1);   // h64
-        ptx::tc_fence_after();
-        block(T_H64_HI, T_H64_LO, 0, true, idesc128, 4);
-        ptx::umma_commit(&acc_bar[0]);
-        ptx::mbar_wait(a_ready, na++ & 1);   // h128
-        ptx::tc_fence_after();
-        for (int nb = 0; nb < 2; ++nb) {
-          for (int kb = 0; kb < 2; ++kb) block(T_H128_HI + kb * 32, T_H128_LO + kb * 32, nb, kb == 0, idesc128, 4);
-          ptx::umma_commit(&acc_bar[nb]);
-        }
-        ptx::mbar_wait(a_ready, na++ & 1);   // h256
-        ptx::tc_fence_after();
-        for (int nb = 0; nb < 2; ++nb) {
-          for (int kb = 0; kb < 4; ++kb)
-            block((kb < 2 ? T_H256A_HI : T_H256B_HI) + (kb & 1) * 32, (kb < 2 ? T_H256A_LO : T_H256B_LO) + (kb & 1) * 32, nb, kb == 0, idesc128, 4);
-          ptx::umma_commit(&acc_bar[nb]);
-        }
+        push(p.W2, 0, 0);
+        push(p.W3, 0, 0);
+        for (int nb = 0; nb < 2; ++nb)
+          for (int kb = 0; kb < 2; ++kb) push(p.W4, nb, kb);
+        for (int nb = 0; nb < 2; ++nb)
+          for (int kb = 0; kb < 4; ++kb) push(p.W5, nb, kb);
       }
     }
   } else {
-    // ---------------------------------------------------------------- workers (256 threads)
-    const int q = warp & 3;            // TMEM lane quarter
-    const int half = (warp - 2) >> 2;  // column half
-    const int r_in = q * 32 + lane;    // token row inside the tile
-    const int wt = tid - 64;           // 0..255
+    // ---------------------------------------------------------------- workers (2 warpgroups x 64 token rows)
+    // Every layer is a register-A wgmma: the accumulator fragment of one layer, after bias + ReLU and the split into
+    // bf16 hi / lo, is exactly the A fragment of the next, so the activations never leave the registers.
+    ptx::setmaxnreg_inc<232>();
+    const int wg = warp >> 2;
+    const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // token rows row_a and row_a + 8 of the tile
+    const int cq = 2 * (lane & 3);
+    const int wt = tid;                // 0..255
     const int rows_used = p.lpt * p.T;
-    uint32_t nacc0 = 0, nacc1 = 0, dph = 0;   // phase parities: the two accumulator barriers, descriptor-group barriers
+    uint32_t dph = 0, it = 0;
     auto worker_sync = [&]() { asm volatile("bar.sync 1, 256;" ::: "memory"); };
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(q * 32) << 16);
-    // relu(acc + bias) of 32 consecutive columns -> split-bf16 pairs -> 16 + 16 tensor-memory columns of the next
-    // layer's A operand (hi pairs at t_hi, lo pairs at t_lo; the caller passes the column of the first pair)
-    auto act_store32 = [&](const float (&acc)[32], const float* bias, uint32_t t_hi, uint32_t t_lo) {
-      uint32_t hi[16], lo[16];
-#pragma unroll
-      for (int j = 0; j < 32; j += 2) {   // packed fp32 pairs (add.f32x2 / fma.f32x2): half the issue slots of the scalar form
-        const float2 v = __fadd2_rn(make_float2(acc[j], acc[j + 1]), *reinterpret_cast<const float2*>(bias + j));
-        ptx::split2_bf16_x2(make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f)), hi[j >> 1], lo[j >> 1]);
-      }
-      ptx::tmem_st16(lane_addr + t_hi, hi);
-      ptx::tmem_st16(lane_addr + t_lo, lo);
+    auto slot_wait = [&]() -> uint32_t {
+      ptx::mbar_wait(&full[it & 1], (it >> 1) & 1);
+      return ptx::smem_u32(smem + S::OFF_RING + (it & 1) * S::SLOT);
+    };
+    auto slot_release = [&]() {
+      __syncwarp();
+      if (lane == 0) ptx::mbar_arrive(&empty[it & 1]);
+      ++it;
     };
     const float scls0 = p.s_cls[0], scls1 = p.s_cls[1], scls2 = p.s_cls[2], scls3 = p.s_cls[3];
-    // token coordinates + score of this thread's row of tile `t` (raw; requested one tile ahead of their use)
-    float in0 = 0.f, in1 = 0.f, in2 = 0.f;
-    auto p0_fetch = [&](int t) {
-      const long long tk0 = (long long)t * p.lpt * p.T;
-      in0 = in1 = in2 = 0.f;
-      if (t < p.n_tiles && r_in < rows_used && tk0 + r_in < (long long)p.R * p.T) {
-        const long long tk = tk0 + r_in;
-        in0 = p.pnt[2 * tk]; in1 = p.pnt[2 * tk + 1]; in2 = p.score[tk];
-      }
-    };
-    p0_fetch(blockIdx.x);
-    // P0: first layer 3 -> 32 (+ReLU) of this thread's token row; the pair of threads of a row splits the 32 outputs.
-    // Result: 8 + 8 packed split-bf16 pairs -> tensor-memory columns of the h32 operand.
-    auto p0 = [&](int t) {
-      const long long tk0 = (long long)t * p.lpt * p.T;
-      float x0 = 0.f, x1 = 0.f, x2 = 0.f;
-      if (r_in < rows_used && tk0 + r_in < (long long)p.R * p.T) {
-        x0 = (in0 - p.cx) / p.scale;
-        x1 = (in1 - p.cy) / p.scale;
-        x2 = in2;
-      }
-      p0_fetch(t + (int)gridDim.x);
-      uint32_t hi[8], lo[8];
-#pragma unroll
-      for (int j = 0; j < 16; j += 2) {
-        const int n = half * 16 + j;
-        const float a = fmaxf(fmaf(sW1[n * 3 + 2], x2, fmaf(sW1[n * 3 + 1], x1, fmaf(sW1[n * 3], x0, sB1[n]))), 0.f);
-        const float b = fmaxf(fmaf(sW1[n * 3 + 5], x2, fmaf(sW1[n * 3 + 4], x1, fmaf(sW1[n * 3 + 3], x0, sB1[n + 1]))), 0.f);
-        ptx::split2_bf16(a, b, hi[j >> 1], lo[j >> 1]);
-      }
-      ptx::tmem_st8(lane_addr + T_H32_HI + half * 8, hi);
-      ptx::tmem_st8(lane_addr + T_H32_LO + half * 8, lo);
-      ptx::tmem_wait_st();
-    };
     // ---- Softmax and pooling of a tile are DEFERRED into the next tile's MMA phases: they need only shared memory
     //      (the tile's partial scores and its x tile), while the workers would otherwise idle behind L2, L3, the first
     //      n-blocks of L4 and L5 (8.8 k of a 26.6 k-cycle tile in the clock64 trace).  The x tile is handed back for the
@@ -361,9 +288,8 @@ __global__ void __launch_bounds__(320, 1) token_fused_kernel(TokenFusedArgs p, c
 #pragma unroll
           for (int h = 0; h < 4; ++h) {
             const float2 pp = make_float2(prv[h], prv[h]);
-            const float2 za = __ffma2_rn(pp, make_float2(xv.x, xv.y), make_float2(z[h][0], z[h][1]));
-            const float2 zb = __ffma2_rn(pp, make_float2(xv.z, xv.w), make_float2(z[h][2], z[h][3]));
-            z[h][0] = za.x; z[h][1] = za.y; z[h][2] = zb.x; z[h][3] = zb.y;
+            z[h][0] = fmaf(pp.x, xv.x, z[h][0]); z[h][1] = fmaf(pp.y, xv.y, z[h][1]);
+            z[h][2] = fmaf(pp.x, xv.z, z[h][2]); z[h][3] = fmaf(pp.y, xv.w, z[h][3]);
           }
         }
         const float4 iv = *reinterpret_cast<const float4*>(&sInv[ln * 4]);
@@ -375,63 +301,68 @@ __global__ void __launch_bounds__(320, 1) token_fused_kernel(TokenFusedArgs p, c
     };
     for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x) {
       const int line0 = tile * p.lpt;
-      const bool tr = (tile == blockIdx.x + gridDim.x) && warp == 2 && lane == 0;   // trace the CTA's 2nd tile
-      if (tr) LTR_DBG_STAMP(0);
-      // ---- P0 -> h32 operand
-      p0(tile);
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(a_ready);
-      if (have_prev) softmax_prev();   // under the L2 MMAs
-      // ---- epilogue L2: 64 columns (32 per thread of the pair) -> h64
-      ptx::mbar_wait(&acc_bar[0], nacc0++ & 1);
-      ptx::tc_fence_after();
+      // ---- P0: first layer 3 -> 32 (+ReLU) on CUDA cores, straight into the A fragments of L2 (K = 32)
+      uint32_t a32h[2][4], a32l[2][4];
       {
-        float acc[32];
-        ptx::tmem_ld32(lane_addr + (uint32_t)(half * 32), acc);
-        act_store32(acc, sB2 + half * 32, T_H64_HI + half * 16, T_H64_LO + half * 16);
-      }
-      ptx::tmem_wait_st();
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(a_ready);
-      if (tr) LTR_DBG_STAMP(1);
-      if (have_prev) pool_prev(0, 1);   // under the L3 MMAs
-      // ---- epilogue L3: 128 columns (64 per half) -> h128
-      ptx::mbar_wait(&acc_bar[0], nacc0++ & 1);
-      ptx::tc_fence_after();
-      if (tr) LTR_DBG_STAMP(2);
-#pragma unroll 1
-      for (int c0 = half * 64; c0 < half * 64 + 64; c0 += 32) {
-        float acc[32];
-        ptx::tmem_ld32(lane_addr + (uint32_t)c0, acc);
-        act_store32(acc, sB3 + c0, T_H128_HI + (c0 >> 1), T_H128_LO + (c0 >> 1));
-      }
-      ptx::tmem_wait_st();
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(a_ready);
-      if (tr) LTR_DBG_STAMP(3);
-      if (have_prev) pool_prev(1, 1);   // under L4's first n-block
-      // ---- epilogue L4: 256 columns -> h256.  The pair of threads of a row halves EACH 128-column n-block (this
-      //      thread: columns nb * 128 + half * 64 .. + 64), so the first n-block is converted while the second
-      //      is still being multiplied; its pairs go to the h256 columns that do not alias h128 (see the header).
-#pragma unroll 1
-      for (int nb = 0; nb < 2; ++nb) {
-        if (nb == 0) ptx::mbar_wait(&acc_bar[0], nacc0++ & 1);
-        else ptx::mbar_wait(&acc_bar[1], nacc1++ & 1);
-        ptx::tc_fence_after();
-        if (tr && nb == 0) LTR_DBG_STAMP(4);
-#pragma unroll 1
-        for (int c0 = nb * 128 + half * 64; c0 < nb * 128 + half * 64 + 64; c0 += 32) {
-          float acc[32];
-          ptx::tmem_ld32(lane_addr + (uint32_t)c0, acc);
-          const uint32_t pc = (uint32_t)(c0 & 127) >> 1;   // pair column inside the 64-column half of h256
-          act_store32(acc, sB4 + c0, (nb == 0 ? T_H256A_HI : T_H256B_HI) + pc, (nb == 0 ? T_H256A_LO : T_H256B_LO) + pc);
+        const long long tk0 = (long long)tile * p.lpt * p.T;
+        float x0[2], x1[2], x2[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = row_a + 8 * e;
+          x0[e] = x1[e] = x2[e] = 0.f;
+          if (r < rows_used && tk0 + r < (long long)p.R * p.T) {
+            const long long tk = tk0 + r;
+            x0[e] = (p.pnt[2 * tk] - p.cx) / p.scale;
+            x1[e] = (p.pnt[2 * tk + 1] - p.cy) / p.scale;
+            x2[e] = p.score[tk];
+          }
         }
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int r = e & 1, n = 16 * kk + 8 * (e >> 1) + cq;
+            const float a = fmaxf(fmaf(sW1[n * 3 + 2], x2[r], fmaf(sW1[n * 3 + 1], x1[r], fmaf(sW1[n * 3], x0[r], sB1[n]))), 0.f);
+            const float b = fmaxf(fmaf(sW1[n * 3 + 5], x2[r], fmaf(sW1[n * 3 + 4], x1[r], fmaf(sW1[n * 3 + 3], x0[r], sB1[n + 1]))), 0.f);
+            ptx::split2_bf16(a, b, a32h[kk][e], a32l[kk][e]);
+          }
       }
-      ptx::tmem_wait_st();
-      ptx::tc_fence_before();
-      ptx::mbar_arrive(a_ready);
-      if (tr) LTR_DBG_STAMP(5);
-      if (have_prev) {                  // under L5's first n-block: the rest, then the x tile is free for this tile's descriptors
+      if (have_prev) softmax_prev();
+      // ---- L2: 32 -> 64 (the k-block's upper half is zero padding)
+      uint32_t a64h[4][4], a64l[4][4];
+      {
+        float d[32];
+        const uint32_t w = slot_wait();
+        slot_mma<0, 2>(d, a32h, a32l, w, true);
+        slot_release();
+        acc_to_afrag<0>(d, sB2, cq, a64h, a64l);
+      }
+      if (have_prev) pool_prev(0, 1);
+      // ---- L3: 64 -> 128
+      uint32_t a128h[8][4], a128l[8][4];
+      {
+        float d[64];
+        const uint32_t w = slot_wait();
+        slot_mma<0, 4>(d, a64h, a64l, w, true);
+        slot_release();
+        acc_to_afrag<0>(d, sB3, cq, a128h, a128l);
+      }
+      if (have_prev) pool_prev(1, 1);
+      // ---- L4: 128 -> 256, two n-blocks of 128
+      uint32_t a256h[16][4], a256l[16][4];
+#pragma unroll
+      for (int nb = 0; nb < 2; ++nb) {
+        float d[64];
+        uint32_t w = slot_wait();
+        slot_mma<0, 4>(d, a128h, a128l, w, true);
+        slot_release();
+        w = slot_wait();
+        slot_mma<4, 4>(d, a128h, a128l, w, false);
+        slot_release();
+        if (nb == 0) acc_to_afrag<0>(d, sB4, cq, a256h, a256l);
+        else acc_to_afrag<8>(d, sB4 + 128, cq, a256h, a256l);
+      }
+      if (have_prev) {                  // the rest of the pooling, then the x tile is free for this tile's descriptors
         pool_prev(2, 1 << 30);
         ptx::fence_proxy_async_smem();  // this thread's generic accesses to the x tile before the TMA writes that follow
         ptx::mbar_arrive(x_free);
@@ -440,61 +371,67 @@ __global__ void __launch_bounds__(320, 1) token_fused_kernel(TokenFusedArgs p, c
           request_desc(tile);
         }
       }
-      // ---- epilogue L5: x = acc + b5 + desc -> fp32, in place in the x tile (where the TMA put desc);
-      //      partial CLS scores over this thread's 128 columns (64 of each n-block, first n-block first)
-      float2 s0 = make_float2(0.f, 0.f), s1 = s0, s2 = s0, s3 = s0;
-#pragma unroll 1
-      for (int nb = 0; nb < 2; ++nb) {
-        if (nb == 0) ptx::mbar_wait(&acc_bar[0], nacc0++ & 1);
-        else ptx::mbar_wait(&acc_bar[1], nacc1++ & 1);
-        ptx::tc_fence_after();
-        if (tr && nb == 0) LTR_DBG_STAMP(6);
-        if (tr && nb == 1) LTR_DBG_STAMP(12);
-#pragma unroll 1
-        for (int c0 = nb * 128 + half * 64; c0 < nb * 128 + half * 64 + 64; c0 += 32) {
-          float acc[32];
-          ptx::tmem_ld32(lane_addr + (uint32_t)c0, acc);
-          ptx::mbar_wait(&dbar[(c0 >> 5) & 3], dph);   // this column group of every row has landed (long ago, normally)
+      // ---- L5: 256 -> 256; x = acc + b5 + desc -> fp32, in place in the x tile (where the TMA put desc);
+      //      partial CLS scores x . u_h of this thread's two rows
+      float sc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const int n = c0 + j;
-            float4* xp = reinterpret_cast<float4*>(&xs[xs_index(r_in, n)]);
-            const float4 d = *xp;
-            const float4 b = *reinterpret_cast<const float4*>(&sB5[n]);
-            // packed fp32 pairs: per head an (even, odd) column pair of partial scores, summed after the loop
-            const float2 xa = __fadd2_rn(__fadd2_rn(make_float2(acc[j], acc[j + 1]), make_float2(b.x, b.y)), make_float2(d.x, d.y));
-            const float2 xb = __fadd2_rn(__fadd2_rn(make_float2(acc[j + 2], acc[j + 3]), make_float2(b.z, b.w)), make_float2(d.z, d.w));
-            *xp = make_float4(xa.x, xa.y, xb.x, xb.y);
-            const float4 u0 = *reinterpret_cast<const float4*>(&sU[n]);
-            const float4 u1 = *reinterpret_cast<const float4*>(&sU[256 + n]);
-            const float4 u2 = *reinterpret_cast<const float4*>(&sU[512 + n]);
-            const float4 u3 = *reinterpret_cast<const float4*>(&sU[768 + n]);
-            s0 = __ffma2_rn(xa, make_float2(u0.x, u0.y), __ffma2_rn(xb, make_float2(u0.z, u0.w), s0));
-            s1 = __ffma2_rn(xa, make_float2(u1.x, u1.y), __ffma2_rn(xb, make_float2(u1.z, u1.w), s1));
-            s2 = __ffma2_rn(xa, make_float2(u2.x, u2.y), __ffma2_rn(xb, make_float2(u2.z, u2.w), s2));
-            s3 = __ffma2_rn(xa, make_float2(u3.x, u3.y), __ffma2_rn(xb, make_float2(u3.z, u3.w), s3));
+      for (int nb = 0; nb < 2; ++nb) {
+        float d[64];
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb) {
+          const uint32_t w = slot_wait();
+          if (kb == 0) slot_mma<0, 4>(d, a256h, a256l, w, true);
+          if (kb == 1) slot_mma<4, 4>(d, a256h, a256l, w, false);
+          if (kb == 2) slot_mma<8, 4>(d, a256h, a256l, w, false);
+          if (kb == 3) slot_mma<12, 4>(d, a256h, a256l, w, false);
+          slot_release();
+        }
+        if (nb == 0)
+          for (int g = 0; g < 4; ++g) ptx::mbar_wait(&dbar[g], dph);   // the tile's descriptors have landed
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const int n = nb * 128 + 8 * j + cq;
+          const float2 b = *reinterpret_cast<const float2*>(&sB5[n]);
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float2* xp = reinterpret_cast<float2*>(&xs[xs_index(row_a + 8 * e, n)]);
+            const float2 dv = *xp;
+            const float2 x = make_float2(d[4 * j + 2 * e] + b.x + dv.x, d[4 * j + 2 * e + 1] + b.y + dv.y);
+            *xp = x;
+#pragma unroll
+            for (int hh = 0; hh < 4; ++hh) {
+              const float2 u = *reinterpret_cast<const float2*>(&sU[hh * 256 + n]);
+              sc[e][hh] = fmaf(x.x, u.x, fmaf(x.y, u.y, sc[e][hh]));
+            }
           }
         }
       }
       dph ^= 1;
-      ptx::tc_fence_before();
-      *reinterpret_cast<float4*>(&sSc[(half * 128 + r_in) * 4]) = make_float4(s0.x + s0.y, s1.x + s1.y, s2.x + s2.y, s3.x + s3.y);
-      if (tr) LTR_DBG_STAMP(7);
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+#pragma unroll
+        for (int hh = 0; hh < 4; ++hh) {
+          sc[e][hh] += __shfl_xor_sync(0xffffffffu, sc[e][hh], 1);
+          sc[e][hh] += __shfl_xor_sync(0xffffffffu, sc[e][hh], 2);
+        }
+      if ((lane & 3) == 0) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int r = row_a + 8 * e;
+          *reinterpret_cast<float4*>(&sSc[r * 4]) = make_float4(sc[e][0], sc[e][1], sc[e][2], sc[e][3]);
+          *reinterpret_cast<float4*>(&sSc[(128 + r) * 4]) = make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+      }
       worker_sync();
-      if (tr) LTR_DBG_STAMP(8);
-      // softmax + pooling of THIS tile run inside the next tile's MMA phases (or after the loop for the last one)
+      // softmax + pooling of THIS tile run inside the next tile (or after the loop for the last one)
       prev_line0 = line0;
       have_prev = true;
-      if (tr) LTR_DBG_STAMP(11);
     }
     if (have_prev) {   // drain: the CTA's last tile
       softmax_prev();
       pool_prev(0, 1 << 30);
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) ptx::tmem_dealloc(tmem_base, 512);
 }
 
 // cuTensorMapEncodeTiled through the runtime (no link against libcuda)
@@ -533,13 +470,13 @@ inline int launch_token_fused(TokenFusedArgs a, cudaStream_t s) {
                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) return set_error(-1, "token_fused: cuTensorMapEncodeTiled failed (" + std::to_string((int)cr) + ")");
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   const int grid = a.n_tiles < sms ? a.n_tiles : sms;
   LaunchScope ls(KC_TOKEN_FUSED, s);
-  LTR_CUDA_TRY(launch_pdl(token_fused_kernel, dim3(grid), dim3(320), TokenFusedSmem::TOTAL, s, a, map));
+  LTR_CUDA_TRY(launch_pdl(token_fused_kernel, dim3(grid), dim3(384), TokenFusedSmem::TOTAL, s, a, map));
   return 0;
 }
 

@@ -1,4 +1,4 @@
-"""Training-side matchers of the reference (`evaluations/matcher.py`) on the B200 library.
+"""Training-side matchers of the reference (`evaluations/matcher.py`) on the CUDA library.
 
 Same names, arguments and return values as the reference functions:
 

@@ -1,4 +1,4 @@
-"""Drop-in `LineTransformer` with the reference's call surface, computing on the B200 library.
+"""Drop-in `LineTransformer` with the reference's call surface, computing on the CUDA library.
 
 Mirrors yosungho/LineTR `models/line_transformer.py:185-291` (class LineTransformer):
 same constructor/config dict, same state-dict keys (so the shipped `LineTR_weight.pth` loads
@@ -88,7 +88,7 @@ def _find_weights(config):
 
 
 class LineTransformer(nn.Module):
-    """Line-Transformer networks (line descriptive + line signature), B200-native."""
+    """Line-Transformer networks (line descriptive + line signature), H100-native."""
 
     default_config = {
         "mode": "test",

@@ -1,5 +1,5 @@
 """Drop-in `nn_matcher` / `nn_matcher_distmat` (reference models/nn_matcher.py:3-43) and the
-`subline2keyline` merge (reference models/line_transformer.py:277-282) on the B200 library.
+`subline2keyline` merge (reference models/line_transformer.py:277-282) on the CUDA library.
 
 Same signatures, host numpy in / host numpy out, dense float64 0/1 match matrix [1,n0,n1] as
 the reference returns it.  The arithmetic (distance GEMM, clip, argmin, threshold, mutual

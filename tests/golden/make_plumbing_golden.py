@@ -11,11 +11,18 @@ dict - but the tokeniser, LineTransformer.forward, get_dist_matrix, subline2keyl
 nn_matcher_distmat calls are the reference's own, with real SuperPoint descriptors, real line
 geometry, real key-line -> subline splits (mat_klines2sublines is not the identity).
 
-Stored per image (fixture `plumbing_pairs.npz`): the tokeniser dict (descriptors of padded token
-slots are all the descriptor sampled at (0, 0), so only real-token descriptors + that one pad
-descriptor are stored and `tests/helpers.plumbing_image` rebuilds the tensor bit-exactly) and the
-reference outputs `line_desc`, `matches_l`, `matching_scores_l`; for one pair also the SuperPoint point
-descriptors + `matches_p` (the nn_matcher call of matching.py:69-71).
+Stored per image: the tokeniser dict (descriptors of padded token slots are all the descriptor sampled
+at (0, 0), so only real-token descriptors + that one pad descriptor are stored and
+`tests/helpers.plumbing_image` rebuilds the tensor) and the outputs `line_desc`, `matches_l`,
+`matching_scores_l`; for one pair also the SuperPoint point descriptors + `matches_p` (the nn_matcher
+call of matching.py:69-71).  To keep every fixture file under 1 MB the SuperPoint descriptors are stored
+as float16, and the LineTR outputs are then recomputed by the reference's own LineTransformer and
+line-matching calls, with the shipped checkpoint, from exactly those (float16-valued) inputs (`finalize`).
+The shipped checkpoint stays necessary here: with seeded random weights the descriptors of real images
+collapse (key-line distances within ~0.2 of each other, top-2 gaps ~1e-7), so the match decisions these
+fixtures pin would be ties.  Files:
+`plumbing_pairs.npz` (tokeniser fields, matches, scores), `plumbing_img_<pair>_<side>.npz` (descriptors
+and line_desc of one image), `plumbing_pnt.npz` (point branch).
 Also writes tokenizer fixtures (`tokenizer_outputs.npz`): outputs of the reference tokeniser
 (`LineTransformer.preprocess`, models/line_transformer.py:251-275 -> models/line_process.py:100-196) for the seeded
 fake detections / fake SuperPoint maps of tests/test_tokenizer.py, so that the GPU tokenizer is
@@ -131,7 +138,7 @@ def main():
                                            pred["matches_p"][0].numpy().argmax(1), -1).astype(np.int32)
         meta["pairs"].append(info)
         print(info)
-    np.savez_compressed(os.path.join(HERE, "plumbing_pairs.npz"), **out)
+    finalize(out, meta)
     meta["torch"] = torch.__version__
     meta["note"] = "reference Matching (CPU) with a cv2.createLineSegmentDetector shim for the LSD wrapper"
 
@@ -173,11 +180,73 @@ def main():
     for mutual in (False, True):
         ev[f"eval_score_m{int(mutual)}"] = ref_eval.nn_matcher_score(dm, 0.5, mutual)
     np.savez_compressed(os.path.join(HERE, "eval_matcher_outputs.npz"), **ev)
-    np.savez_compressed(os.path.join(HERE, "tokenizer_outputs.npz"), **tok)
+    np.savez_compressed(os.path.join(HERE, "tokenizer_outputs.npz"), **sample_tokenizer_desc(tok))
     with open(os.path.join(HERE, "plumbing_pairs.json"), "w") as f:
         json.dump(meta, f, indent=1, sort_keys=True)
-    for fn in ("plumbing_pairs.npz", "tokenizer_outputs.npz", "eval_matcher_outputs.npz"):
-        print(fn, os.path.getsize(os.path.join(HERE, fn)) / 1e6, "MB")
+    for fn in sorted(os.listdir(HERE)):
+        if fn.endswith(".npz"):
+            print(fn, os.path.getsize(os.path.join(HERE, fn)) / 1e6, "MB")
+
+
+TOK_DESC_STRIDE = 3   # tokenizer fixture: every third real-token descriptor row is stored (file size)
+
+
+def sample_tokenizer_desc(tok):
+    out = dict(tok)
+    for k in [k for k in tok if k.endswith("_desc_real")]:
+        idx = np.arange(0, len(tok[k]), TOK_DESC_STRIDE)
+        out[k] = tok[k][idx]
+        out[k[:-len("real")] + "real_rows"] = idx.astype(np.int32)
+    return out
+
+
+def finalize(out, meta):
+    """float16 SuperPoint descriptors; LineTR outputs of the reference recomputed from them with the shipped checkpoint;
+    written in files of < 1 MB each."""
+    sys.path.insert(0, HERE)
+    from make_golden import ref_model
+    from models.line_process import get_dist_matrix
+    from models.nn_matcher import nn_matcher, nn_matcher_distmat
+    from tests.helpers import plumbing_image
+    for k in list(out):
+        if k.endswith(("_desc_real", "_desc_pad")) or "_desc_pnt" in k:
+            out[k] = out[k].astype(np.float16)
+    ckpt = torch.load(os.path.join(REF, "models", "weights", "LineTR_weight.pth"), map_location="cpu")
+    mr = ref_model({k: v.numpy() for k, v in ckpt.items()}, 1)
+    meta["weights"] = "shipped"
+    for i, info in enumerate(meta["pairs"]):
+        a, _ = plumbing_image(out, f"p{i}_0")
+        b, _ = plumbing_image(out, f"p{i}_1")
+        # float64 forward of the reference model: the fixture holds the exact result for these inputs
+        d0, d1 = (mr.double()({k: torch.from_numpy(v.astype(np.float64)) for k, v in x.items()})["line_desc"].numpy()
+                  .astype(np.float32) for x in (a, b))
+        out[f"p{i}_0_line_desc"], out[f"p{i}_1_line_desc"] = d0, d1
+        # models/matching.py:77-81, the reference's own calls
+        dist = get_dist_matrix(d0, d1)[0]
+        dk = mr.subline2keyline(dist, torch.from_numpy(a["mat_klines2sublines"][0]), torch.from_numpy(b["mat_klines2sublines"][0]))
+        dk = np.asarray(dk)
+        dk = dk[0] if dk.ndim == 3 else dk
+        mat = nn_matcher_distmat(dk[None], 0.8, True)[0]
+        out[f"p{i}_matches_l"] = np.where(mat.sum(1) > 0, mat.argmax(1), -1).astype(np.int32)
+        out[f"p{i}_scores_l"] = dk.astype(np.float32)
+        info["n_matches_l"] = int(mat.sum())
+        srt = np.sort(dk.astype(np.float64), axis=1)
+        info["min_top2_gap_rows"] = float((srt[:, 1] - srt[:, 0]).min())
+    mat, _ = nn_matcher(out["p0_desc_pnt0"].astype(np.float32), out["p0_desc_pnt1"].astype(np.float32), 0.7, True)
+    mat = mat[0] if mat.ndim == 3 else mat
+    out["p0_matches_p"] = np.where(mat.sum(1) > 0, mat.argmax(1), -1).astype(np.int32)
+    meta["pairs"][0]["n_matches_p"] = int(mat.sum())
+    files = {"plumbing_pairs.npz": {}, "plumbing_pnt.npz": {}}
+    for k, v in out.items():
+        if "_desc_pnt" in k:
+            files["plumbing_pnt.npz"][k] = v
+        elif k.endswith(("_desc_real", "_desc_pad", "_line_desc")):
+            pre = k[:len("p0_0")]
+            files.setdefault(f"plumbing_img_{pre[1:]}.npz", {})[k] = v
+        else:
+            files["plumbing_pairs.npz"][k] = v
+    for fn, arrays in files.items():
+        np.savez_compressed(os.path.join(HERE, fn), **arrays)
 
 
 if __name__ == "__main__":

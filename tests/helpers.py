@@ -7,6 +7,8 @@ import numpy as np
 from linetr_b200 import synthetic as syn
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+# the original project's models package, checkpoints and image pairs, staged by build() (oracle/stage_reference.py)
+REF_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "_ref", "reference")
 _cache = {}
 
 
@@ -19,8 +21,8 @@ def golden():
 
 
 def golden_full():
-    """Full-size images (256 x 32, ragged 512 x 64) through the reference with the shipped checkpoint
-    (tests/golden/make_golden.py::main_full)."""
+    """Full-size images (256 x 32, ragged 512 x 64) through the reference with the seeded weight set named in
+    the fixture's metadata (tests/golden/make_golden.py::main_full)."""
     if "npz_full" not in _cache:
         _cache["npz_full"] = dict(np.load(os.path.join(GOLDEN_DIR, "reference_outputs_full.npz")))
         with open(os.path.join(GOLDEN_DIR, "reference_outputs_full.json")) as f:
@@ -50,12 +52,8 @@ def weights_for(tag):
 
 
 def shipped_weights_path():
-    """The reference checkpoint, if a copy travelled with the repo (git-ignored) or the
-    reference checkout is mounted (build container only)."""
-    root = os.path.dirname(GOLDEN_DIR[:-len("/golden")])
-    for p in (os.environ.get("LINETR_WEIGHTS", ""),
-              os.path.join(root, "linetr_b200", "weights", "LineTR_weight.pth"),
-              "/root/reference/models/weights/LineTR_weight.pth"):
+    """The reference checkpoint: $LINETR_WEIGHTS, or the copy build() staged under oracle/_ref/ (git-ignored)."""
+    for p in (os.environ.get("LINETR_WEIGHTS", ""), os.path.join(REF_DIR, "models", "weights", "LineTR_weight.pth")):
         if p and os.path.exists(p):
             return p
     return None
@@ -91,7 +89,12 @@ TOK_KEYS = ("klines", "length_klines", "angles", "sublines", "pnt_sublines", "ma
 def plumbing():
     """Fixtures of tests/golden/make_plumbing_golden.py: the reference `Matching` run on the four bundled pairs."""
     if "plumb" not in _cache:
-        _cache["plumb"] = dict(np.load(os.path.join(GOLDEN_DIR, "plumbing_pairs.npz")))
+        npz = {}
+        for fn in sorted(os.listdir(GOLDEN_DIR)):   # plumbing_pairs / plumbing_img_<pair>_<side> / plumbing_pnt
+            if fn.startswith("plumbing_") and fn.endswith(".npz"):
+                npz.update(np.load(os.path.join(GOLDEN_DIR, fn)))
+        # SuperPoint descriptors are stored as float16 values; the models consume them as float32
+        _cache["plumb"] = {k: v.astype(np.float32) if v.dtype == np.float16 else v for k, v in npz.items()}
         with open(os.path.join(GOLDEN_DIR, "plumbing_pairs.json")) as f:
             _cache["plumb_meta"] = json.load(f)
     return _cache["plumb"], _cache["plumb_meta"]
@@ -114,12 +117,13 @@ def plumbing_image(npz, prefix):
 
 
 def tokenizer_fixture(ci):
+    """-> (tokeniser fields except desc_sublines, (rows, real-token descriptors at those rows, pad descriptor)): the
+    fixture keeps a fixed sample (every third row) of the real-token descriptors."""
     if "tok" not in _cache:
         _cache["tok"] = dict(np.load(os.path.join(GOLDEN_DIR, "tokenizer_outputs.npz")))
     npz = _cache["tok"]
     d = {k[len(f"c{ci}_"):]: v for k, v in npz.items() if k.startswith(f"c{ci}_") and not k.startswith(f"c{ci}_desc_")}
-    d["desc_sublines"] = _rebuild_desc(d["mask_sublines"], npz[f"c{ci}_desc_real"], npz[f"c{ci}_desc_pad"])
-    return d
+    return d, (npz[f"c{ci}_desc_real_rows"], npz[f"c{ci}_desc_real"], npz[f"c{ci}_desc_pad"])
 
 
 def matching_line_branch(get_dist_matrix, subline2keyline, nn_matcher_distmat, line_desc0, line_desc1, A0, A1, thr):

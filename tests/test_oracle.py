@@ -22,12 +22,10 @@ def test_forward_matches_reference(name):
 
 @pytest.mark.parametrize("name", H.FULL_CASES)
 def test_forward_matches_reference_full_size(name):
-    """cfg[2] / cfg[3]-sized images with the shipped checkpoint: the oracle against the committed reference output."""
-    sd = H.load_shipped_weights()
-    if sd is None:
-        pytest.skip("shipped checkpoint not available")
+    """cfg[2] / cfg[3]-sized images: the oracle against the committed reference output (seeded weights)."""
     npz, meta = H.golden_full()
     case = meta["cases"][name]
+    sd = H.weights_for(case["weights"])
     data = H.case_inputs(case)
     H.assert_checksum(data, case["checksum"])
     got = orc.line_transformer_forward(sd, data)
@@ -102,12 +100,11 @@ def test_subline2keyline():
     assert np.array_equal(orc.nn_matcher_distmat(dk, 0.8, True), npz["s2k_mat"])
 
 
-def test_shipped_checkpoint():
-    sd = H.load_shipped_weights()
-    if sd is None:
-        pytest.skip("shipped LineTR_weight.pth not available on this machine")
+def test_second_weight_set_encoder_and_pair():
+    """A second seeded weight set (make_golden.GOLDEN_WEIGHTS): a ragged 16-line image and a 128-line pair."""
     npz, meta = H.golden()
     case = meta["cases"]["real_enc_L16_T21"]
+    sd = H.weights_for(case["weights"])
     data = H.case_inputs(case)
     got = orc.line_transformer_forward(sd, data)
     assert np.abs(got - npz["real_enc_L16_T21"]).max() < TOL
