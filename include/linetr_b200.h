@@ -260,6 +260,43 @@ typedef struct {
 int ltr_tokenize(const LtrTokenizeInput* in, float* sublines, float* pnt, float* mask, float* resp,
                  float* angle, float* desc, float* score, int32_t device, void* stream);
 
+/* ltr_tokenize over many images in one call (the same kernels; a batch equals per-image calls bit
+ * for bit).  Key lines of all images are concatenated, image by image: sub0 [K+1] and sub2line [S]
+ * use global subline numbering and line_image [K] (device) names the image of every key line.
+ * images [n_images] and cu_sublines [n_images+1] are HOST arrays read during the call only: image i
+ * owns output rows [cu_sublines[i], cu_sublines[i+1]) of the packed outputs (the LineBatch layout)
+ * and is tokenised with its own token_distance and sampled from its own maps, whose sizes may
+ * differ between images.  An image without key lines is an empty range; its maps may be NULL (and
+ * so may the outputs of a batch without any key line).
+ * n_tokens must be 1..128 (the encoder's limit) and desc_channels 256.  Nothing synchronises. */
+typedef struct {
+  const float* dense_desc;     /* device [256, desc_h, desc_w] */
+  const float* dense_score;    /* device [score_h, score_w] */
+  double token_distance;
+  int32_t desc_h, desc_w;
+  int32_t score_h, score_w;
+} LtrTokenizeImage;
+
+typedef struct {
+  const double* sp;
+  const double* ep;
+  const double* ep_clipped;
+  const double* length;
+  const float* angle;
+  const int32_t* n_tok;
+  const int32_t* sub0;
+  const int32_t* sub2line;
+  const int32_t* line_image;
+  int32_t n_images, n_keylines, n_sublines, n_tokens;
+  int32_t desc_channels;
+  int32_t align_corners;
+  const LtrTokenizeImage* images;   /* host [n_images] */
+  const int32_t* cu_sublines;       /* host [n_images+1] */
+} LtrTokenizeBatchInput;
+
+int ltr_tokenize_batch(const LtrTokenizeBatchInput* in, float* sublines, float* pnt, float* mask, float* resp,
+                       float* angle, float* desc, float* score, int32_t device, void* stream);
+
 /* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
  * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */
 int ltr_linear(const float* x, int32_t ldx, const float* w, const float* bias, const float* res,

@@ -3,7 +3,7 @@
 Drop-in names (same call surface as yosungho/LineTR `models/`):
     LineTransformer, get_dist_matrix, nn_matcher, nn_matcher_distmat
 Batched front-end:
-    PairEngine, LineBatch
+    PairEngine, LineBatch, ImagePairMatches
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -22,6 +22,7 @@ _LAZY = {
     "nn_matcher_distmat": ("nn_matcher", "nn_matcher_distmat"),
     "PairEngine": ("engine", "PairEngine"),
     "LineBatch": ("engine", "LineBatch"),
+    "ImagePairMatches": ("engine", "ImagePairMatches"),
 }
 
 

@@ -22,7 +22,7 @@ LAYOUT_CHANNEL_FIRST = 1
 EXPORTED_SYMBOLS = (
     "ltr_abi_version", "ltr_last_error", "ltr_create", "ltr_destroy", "ltr_encode_workspace_bytes",
     "ltr_desc_tiles_bytes", "ltr_encode", "ltr_match_workspace_bytes", "ltr_match", "ltr_gather_wait", "ltr_match_distmat",
-    "ltr_merge_sublines", "ltr_tokenize", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
+    "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
@@ -90,6 +90,19 @@ class LtrTokenizeInput(C.Structure):
                 ("score_w", C.c_int32), ("align_corners", C.c_int32)]
 
 
+class LtrTokenizeImage(C.Structure):
+    _fields_ = [("dense_desc", C.c_void_p), ("dense_score", C.c_void_p), ("token_distance", C.c_double),
+                ("desc_h", C.c_int32), ("desc_w", C.c_int32), ("score_h", C.c_int32), ("score_w", C.c_int32)]
+
+
+class LtrTokenizeBatchInput(C.Structure):
+    _fields_ = [("sp", C.c_void_p), ("ep", C.c_void_p), ("ep_clipped", C.c_void_p), ("length", C.c_void_p),
+                ("angle", C.c_void_p), ("n_tok", C.c_void_p), ("sub0", C.c_void_p), ("sub2line", C.c_void_p),
+                ("line_image", C.c_void_p), ("n_images", C.c_int32), ("n_keylines", C.c_int32),
+                ("n_sublines", C.c_int32), ("n_tokens", C.c_int32), ("desc_channels", C.c_int32),
+                ("align_corners", C.c_int32), ("images", C.POINTER(LtrTokenizeImage)), ("cu_sublines", c_int32_p)]
+
+
 def lib_path() -> str:
     return _LIB_PATH
 
@@ -134,6 +147,8 @@ def load():
     lib.ltr_merge_sublines.restype = C.c_int
     lib.ltr_tokenize.argtypes = [C.POINTER(LtrTokenizeInput)] + [C.c_void_p] * 7 + [C.c_int32, C.c_void_p]
     lib.ltr_tokenize.restype = C.c_int
+    lib.ltr_tokenize_batch.argtypes = [C.POINTER(LtrTokenizeBatchInput)] + [C.c_void_p] * 7 + [C.c_int32, C.c_void_p]
+    lib.ltr_tokenize_batch.restype = C.c_int
     lib.ltr_linear.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
     lib.ltr_linear.restype = C.c_int

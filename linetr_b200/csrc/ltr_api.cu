@@ -395,6 +395,30 @@ static int run_nn(const NNArgs& a, int n_pairs, int max_k0, int max_k1, cudaStre
   return 0;
 }
 
+// Images per launch of the tokenizer kernels: their table travels as a kernel parameter (40 bytes each, 5 KB in
+// all: above the classic 4 KB, within the 32 KB parameter limit CUDA 12.1 brought to sm_70 and newer).
+constexpr int kTokImagesPerLaunch = 128;
+
+// The two tokenizer launches for the sublines [s_begin, s_end) of images I.first ...
+template <int NI>
+static int launch_tokenize(const TokLines& L, const TokImages<NI>& I, int s_begin, int s_end, int align_corners,
+                           float* sublines, float* pnt, float* mask, float* resp, float* angle, float* desc, float* score,
+                           cudaStream_t s) {
+  const long long n_tok = (long long)(s_end - s_begin) * L.T;
+  if (n_tok <= 0) return LTR_OK;
+  {
+    LaunchScope ls(KC_TOKENIZE, s);
+    tok_points_kernel<NI><<<cdiv(n_tok, 256), 256, 0, s>>>(L, I, s_begin, s_end, pnt, mask, sublines, resp, angle);
+    LTR_CUDA_TRY(cudaGetLastError());
+  }
+  {
+    LaunchScope ls(KC_TOKENIZE, s);
+    tok_sample_kernel<NI><<<cdiv(n_tok, 8), 256, 0, s>>>(L, I, s_begin, s_end, align_corners, pnt, desc, score);
+    LTR_CUDA_TRY(cudaGetLastError());
+  }
+  return LTR_OK;
+}
+
 }  // namespace ltr
 
 using namespace ltr;
@@ -881,20 +905,49 @@ int ltr_tokenize(const LtrTokenizeInput* in, float* sublines, float* pnt, float*
       !in->dense_desc || !in->dense_score)
     return set_error(LTR_E_INVALID, "ltr_tokenize: null input array");
   LTR_CUDA_TRY(cudaSetDevice(device));
-  cudaStream_t s = as_stream(stream);
-  TokLines L{in->sp, in->ep, in->ep_clipped, in->length, in->angle, in->n_tok, in->sub0, in->sub2line,
-             in->n_keylines, in->n_sublines, in->n_tokens, in->token_distance};
-  const long long n_tok = (long long)in->n_sublines * in->n_tokens;
-  {
-    LaunchScope ls(KC_TOKENIZE, s);
-    tok_points_kernel<<<cdiv(n_tok, 256), 256, 0, s>>>(L, pnt, mask, sublines, resp, angle);
-    LTR_CUDA_TRY(cudaGetLastError());
+  TokLines L{in->sp, in->ep, in->ep_clipped, in->length, in->angle, in->n_tok, in->sub0, in->sub2line, nullptr,
+             in->n_keylines, in->n_sublines, in->n_tokens};
+  TokImages<1> I{};
+  I.im[0] = TokImage{in->dense_desc, in->dense_score, in->token_distance, in->desc_h, in->desc_w, in->score_h, in->score_w};
+  return launch_tokenize(L, I, 0, in->n_sublines, in->align_corners, sublines, pnt, mask, resp, angle, desc, score,
+                         as_stream(stream));
+}
+
+int ltr_tokenize_batch(const LtrTokenizeBatchInput* in, float* sublines, float* pnt, float* mask, float* resp,
+                       float* angle, float* desc, float* score, int32_t device, void* stream) {
+  if (!in) return set_error(LTR_E_INVALID, "ltr_tokenize_batch: null argument");
+  if (in->n_images < 0 || in->n_keylines < 0 || in->n_sublines < 0)
+    return set_error(LTR_E_INVALID, "ltr_tokenize_batch: negative count");
+  // a batch without key lines has empty outputs, whose pointers may be NULL
+  if (in->n_images == 0 || in->n_sublines == 0 || in->n_keylines == 0) return LTR_OK;
+  if (!sublines || !pnt || !mask || !resp || !angle || !desc || !score)
+    return set_error(LTR_E_INVALID, "ltr_tokenize_batch: null output");
+  if (in->n_tokens < 1 || in->n_tokens > 128 || in->desc_channels != 256)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_tokenize_batch: n_tokens in 1..128 and 256 descriptor channels required");
+  if (!in->sp || !in->ep || !in->ep_clipped || !in->length || !in->angle || !in->n_tok || !in->sub0 || !in->sub2line ||
+      !in->line_image || !in->images || !in->cu_sublines)
+    return set_error(LTR_E_INVALID, "ltr_tokenize_batch: null input array");
+  const int32_t* cu = in->cu_sublines;
+  if (cu[0] != 0 || cu[in->n_images] != in->n_sublines)
+    return set_error(LTR_E_INVALID, "ltr_tokenize_batch: cu_sublines must start at 0 and end at n_sublines");
+  for (int i = 0; i < in->n_images; ++i) {
+    if (cu[i + 1] < cu[i]) return set_error(LTR_E_INVALID, "ltr_tokenize_batch: cu_sublines must not decrease");
+    if (cu[i + 1] > cu[i] && (!in->images[i].dense_desc || !in->images[i].dense_score))
+      return set_error(LTR_E_INVALID, "ltr_tokenize_batch: null map of an image with key lines");
   }
-  {
-    LaunchScope ls(KC_TOKENIZE, s);
-    tok_sample_kernel<<<cdiv(n_tok, 8), 256, 0, s>>>(pnt, (int)n_tok, in->dense_desc, in->desc_h, in->desc_w, in->dense_score,
-                                                      in->score_h, in->score_w, in->align_corners, desc, score);
-    LTR_CUDA_TRY(cudaGetLastError());
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  TokLines L{in->sp, in->ep, in->ep_clipped, in->length, in->angle, in->n_tok, in->sub0, in->sub2line, in->line_image,
+             in->n_keylines, in->n_sublines, in->n_tokens};
+  for (int i0 = 0; i0 < in->n_images; i0 += kTokImagesPerLaunch) {
+    const int i1 = std::min(in->n_images, i0 + kTokImagesPerLaunch);
+    TokImages<kTokImagesPerLaunch> I{};
+    I.first = i0;
+    for (int i = i0; i < i1; ++i) {
+      const LtrTokenizeImage& g = in->images[i];
+      I.im[i - i0] = TokImage{g.dense_desc, g.dense_score, g.token_distance, g.desc_h, g.desc_w, g.score_h, g.score_w};
+    }
+    LTR_TRY(launch_tokenize(L, I, cu[i0], cu[i1], in->align_corners, sublines, pnt, mask, resp, angle, desc, score, s));
   }
   return LTR_OK;
 }

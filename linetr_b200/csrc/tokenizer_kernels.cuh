@@ -5,7 +5,9 @@
 // L2 normalisation of the dense 256-d descriptor map, score lookup.
 //
 // The host prepares per key line (vectorised numpy, no loops): end points in float64, the
-// clipped end point, n_tokens = ceil(length / token_distance), first subline index.  Token
+// clipped end point, n_tokens = ceil(length / token_distance), first subline index, image index.
+// One launch pair covers many images (ltr_tokenize_batch); each image has its own maps, sizes and
+// token_distance, and its sublines land at its rows of the concatenated output.  Token
 // positions are computed in float64 exactly as the reference's numpy code does (IEEE sqrt/div),
 // then rounded to fp32, so positions, sublines, masks and responses are bit-identical; sampled
 // descriptors agree to fp32 rounding.
@@ -14,6 +16,22 @@
 
 namespace ltr {
 
+// Per image: the token spacing and the SuperPoint maps the image's tokens are sampled from.
+struct TokImage {
+  const float* dense;     // [256, Hc, Wc]
+  const float* score;     // [H, W]
+  double token_distance;
+  int Hc, Wc, H, W;
+};
+
+// The images of one launch, passed by value (__grid_constant__: indexed in place, never copied to local
+// memory).  Key line k belongs to im[line_image[k] - first]; line_image == nullptr means one image.
+template <int NI>
+struct TokImages {
+  TokImage im[NI];
+  int first;
+};
+
 struct TokLines {
   const double* sp;       // [K,2] start point (x, y)
   const double* ep;       // [K,2] end point BEFORE the in-place clip (direction of the line)
@@ -21,11 +39,16 @@ struct TokLines {
   const double* length;   // [K] length_klines (detector length, NOT the geometric one)
   const float* angle;     // [K,2]
   const int* n_tok;       // [K]
-  const int* sub0;        // [K+1] first subline of each key line (prefix sum of n_sub)
+  const int* sub0;        // [K+1] first subline of each key line (prefix sum of n_sub, over all images)
   const int* sub2line;    // [S]
+  const int* line_image;  // [K] image of each key line, or nullptr (one image)
   int K, S, T;
-  double token_distance;
 };
+
+template <int NI>
+__device__ __forceinline__ const TokImage& image_of_line(const TokLines& L, const TokImages<NI>& I, int k) {
+  return I.im[L.line_image ? L.line_image[k] - I.first : 0];
+}
 
 // point at distance d from sp along the line (reference point_on_line, line_process.py:43-59)
 __device__ __forceinline__ void point_on_line_f64(double spx, double spy, double epx, double epy, double d, double& x, double& y) {
@@ -44,55 +67,61 @@ __device__ __forceinline__ void point_on_line_f64(double spx, double spy, double
 }
 
 // token i of key line k (i < n_tok): i < n_tok-1 -> point at i*token_distance, last -> clipped end point
-__device__ __forceinline__ void token_of_line(const TokLines& L, int k, int i, double& x, double& y) {
+__device__ __forceinline__ void token_of_line(const TokLines& L, double token_distance, int k, int i, double& x, double& y) {
   if (i < L.n_tok[k] - 1) {
-    point_on_line_f64(L.sp[2 * k], L.sp[2 * k + 1], L.ep[2 * k], L.ep[2 * k + 1], (double)i * L.token_distance, x, y);
+    point_on_line_f64(L.sp[2 * k], L.sp[2 * k + 1], L.ep[2 * k], L.ep[2 * k + 1], (double)i * token_distance, x, y);
   } else {
     x = L.epc[2 * k];
     y = L.epc[2 * k + 1];
   }
 }
 
-// one thread per (subline, token slot): pnt [S,T,2], mask [S,T+1,1]; slot 0 threads also write the
-// subline end points [S,2,2], resp [S,1], angle [S,2]
+// one thread per (subline, token slot) of sublines [s_begin, s_end): pnt [S,T,2], mask [S,T+1,1]; slot 0
+// threads also write the subline end points [S,2,2], resp [S,1], angle [S,2]
+template <int NI>
 __global__ void __launch_bounds__(256)
-tok_points_kernel(TokLines L, float* __restrict__ pnt, float* __restrict__ mask, float* __restrict__ sublines,
-                  float* __restrict__ resp, float* __restrict__ angle) {
-  const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
-  if (idx >= (long long)L.S * L.T) return;
+tok_points_kernel(TokLines L, const __grid_constant__ TokImages<NI> I, int s_begin, int s_end, float* __restrict__ pnt,
+                  float* __restrict__ mask, float* __restrict__ sublines, float* __restrict__ resp, float* __restrict__ angle) {
+  const long long idx = (long long)s_begin * L.T + (long long)blockIdx.x * 256 + threadIdx.x;
+  if (idx >= (long long)s_end * L.T) return;
   const int s = (int)(idx / L.T), j = (int)(idx % L.T);
   const int k = L.sub2line[s];
+  const double td = image_of_line(L, I, k).token_distance;
   const int sl = s - L.sub0[k];          // subline index within the key line
   const int n_sub = L.sub0[k + 1] - L.sub0[k];
   const int i = sl * L.T + j;
   const bool live = i < L.n_tok[k];
   double x = 0.0, y = 0.0;
-  if (live) token_of_line(L, k, i, x, y);
+  if (live) token_of_line(L, td, k, i, x, y);
   pnt[2 * idx] = (float)x;
   pnt[2 * idx + 1] = (float)y;
   mask[(long long)s * (L.T + 1) + 1 + j] = live ? 1.f : 0.f;
   if (j == 0) {
     mask[(long long)s * (L.T + 1)] = 1.f;
     double ax, ay, bx, by;
-    if (sl == 0) { ax = L.sp[2 * k]; ay = L.sp[2 * k + 1]; } else token_of_line(L, k, sl * L.T - 1, ax, ay);
-    if (sl == n_sub - 1) { bx = L.epc[2 * k]; by = L.epc[2 * k + 1]; } else token_of_line(L, k, (sl + 1) * L.T - 1, bx, by);
+    if (sl == 0) { ax = L.sp[2 * k]; ay = L.sp[2 * k + 1]; } else token_of_line(L, td, k, sl * L.T - 1, ax, ay);
+    if (sl == n_sub - 1) { bx = L.epc[2 * k]; by = L.epc[2 * k + 1]; } else token_of_line(L, td, k, (sl + 1) * L.T - 1, bx, by);
     sublines[4 * s + 0] = (float)ax; sublines[4 * s + 1] = (float)ay;
     sublines[4 * s + 2] = (float)bx; sublines[4 * s + 3] = (float)by;
     const double dxx = bx - ax, dyy = by - ay;
-    resp[s] = (float)(sqrt(dxx * dxx + dyy * dyy) / (L.token_distance * (double)L.T));
+    resp[s] = (float)(sqrt(dxx * dxx + dyy * dyy) / (td * (double)L.T));
     angle[2 * s] = L.angle[2 * k];
     angle[2 * s + 1] = L.angle[2 * k + 1];
   }
 }
 
-// one warp per token: bilinear sample of dense [C=256, Hc, Wc] at the token (torch grid_sample,
-// mode bilinear, zeros padding), L2 normalise over channels, nearest score lookup.
+// one warp per token of sublines [s_begin, s_end): bilinear sample of its image's dense [C=256, Hc, Wc] at the
+// token (torch grid_sample, mode bilinear, zeros padding), L2 normalise over channels, nearest score lookup.
+template <int NI>
 __global__ void __launch_bounds__(256)
-tok_sample_kernel(const float* __restrict__ pnt, int n_tokens, const float* __restrict__ dense, int Hc, int Wc,
-                  const float* __restrict__ score_map, int H, int W, int align_corners, float* __restrict__ desc,
-                  float* __restrict__ score) {
-  const int t = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (t >= n_tokens) return;
+tok_sample_kernel(TokLines L, const __grid_constant__ TokImages<NI> I, int s_begin, int s_end, int align_corners,
+                  const float* __restrict__ pnt, float* __restrict__ desc, float* __restrict__ score) {
+  const long long t = (long long)s_begin * L.T + (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (t >= (long long)s_end * L.T) return;
+  const TokImage& im = image_of_line(L, I, L.sub2line[t / L.T]);
+  const float* __restrict__ dense = im.dense;
+  const int Hc = im.Hc, Wc = im.Wc;
   const float px = pnt[2 * t], py = pnt[2 * t + 1];
   // reference sample_descriptors: (kp - s/2 + 0.5) / (w*s - s/2 - 0.5) * 2 - 1 with s = 8, fp32 arithmetic
   const float gx = ((px - 4.0f) + 0.5f) / ((float)Wc * 8.0f - 4.0f - 0.5f) * 2.0f - 1.0f;
@@ -127,12 +156,12 @@ tok_sample_kernel(const float* __restrict__ pnt, int n_tokens, const float* __re
   ss = warp_sum(ss);
   const float inv = 1.f / fmaxf(sqrtf(ss), 1e-12f);
 #pragma unroll
-  for (int i = 0; i < 8; ++i) desc[(long long)t * 256 + lane + 32 * i] = v[i] * inv;
+  for (int i = 0; i < 8; ++i) desc[t * 256 + lane + 32 * i] = v[i] * inv;
   if (lane == 0) {
     int rx = (int)rintf(px), ry = (int)rintf(py);   // torch.round: half to even
-    rx = min(rx, W - 1);
-    ry = min(ry, H - 1);
-    score[t] = score_map[(long long)ry * W + rx];
+    rx = min(rx, im.W - 1);
+    ry = min(ry, im.H - 1);
+    score[t] = im.score[(long long)ry * im.W + rx];
   }
 }
 

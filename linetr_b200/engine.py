@@ -21,6 +21,7 @@ import torch
 
 from . import _native as N
 from . import _ops
+from . import line_process as LP
 
 _KEYS = ("sublines", "resp_sublines", "angle_sublines", "pnt_sublines", "desc_sublines", "score_sublines")
 
@@ -151,6 +152,69 @@ class PairMatches:
         return self.matches0[int(self.offsets0[p]):int(self.offsets0[p + 1])]
 
 
+def _first(x):
+    """SuperPoint returns per-image lists (or a batch of one): the first entry."""
+    return x[0] if isinstance(x, (list, tuple)) or (isinstance(x, torch.Tensor) and x.dim() == 3 and x.shape[0] == 1) else x
+
+
+def _dense_scores(dist: Optional[torch.Tensor], stride: int, p: int, n0: int, n1: int) -> np.ndarray:
+    if dist is None or n0 == 0 or n1 == 0:
+        return np.zeros((1, n0, n1), dtype=np.float32)
+    return dist[p * stride:p * stride + n0 * n1].view(1, n0, n1).cpu().numpy()
+
+
+@dataclass
+class ImagePairMatches:
+    """Line and point matches of a batch of image pairs (`PairEngine.match_images`).
+
+    matches_l int32 [total side-0 key lines] (index local to the pair or -1), scores_l float32 (distance to the
+    nearest neighbour), counts_l int32 [P], offsets_l np.int32 [P+1] (side-0 key lines of pair p); the same
+    four fields for the SuperPoint keypoints (matches_p, scores_p, counts_p, offsets_p).  With want_scores the
+    distance matrices: pair p at p * stride, row-major [K0_p, K1_p] / [N0_p, N1_p].  klines0/1: each image's
+    tokenised key lines (after the reference's in-place clip), keypoints0/1: each image's keypoints."""
+    matches_l: torch.Tensor
+    scores_l: torch.Tensor
+    counts_l: torch.Tensor
+    offsets_l: np.ndarray
+    matches_p: torch.Tensor
+    scores_p: torch.Tensor
+    counts_p: torch.Tensor
+    offsets_p: np.ndarray
+    klines0: List[np.ndarray]
+    klines1: List[np.ndarray]
+    keypoints0: list
+    keypoints1: list
+    dist_l: Optional[torch.Tensor] = None
+    stride_l: int = 0
+    dist_p: Optional[torch.Tensor] = None
+    stride_p: int = 0
+
+    @property
+    def n_pairs(self) -> int:
+        return len(self.offsets_l) - 1
+
+    def pair_lines(self, p: int) -> torch.Tensor:
+        return self.matches_l[int(self.offsets_l[p]):int(self.offsets_l[p + 1])]
+
+    def pair_points(self, p: int) -> torch.Tensor:
+        return self.matches_p[int(self.offsets_p[p]):int(self.offsets_p[p + 1])]
+
+    def reference_dict(self, p: int) -> dict:
+        """The match keys `Matching.forward` returns for pair p (models/matching.py:69-84): matches_l float64
+        [1,K0,K1], matching_scores_l float32 [1,K0,K1], matches_p float64 [1,N0,N1], matching_scores_p float32
+        [1,N0,N1].  Needs want_scores=True; copies to the host."""
+        if self.dist_l is None or self.dist_p is None:
+            raise N.LtrError("reference_dict needs match_images(..., want_scores=True)")
+        from .match_io import indices_to_dense
+        K0, K1 = len(self.klines0[p]), len(self.klines1[p])
+        N0, N1 = len(self.keypoints0[p]), len(self.keypoints1[p])
+        ml, mp = self.pair_lines(p).cpu().numpy(), self.pair_points(p).cpu().numpy()
+        return {"matches_l": torch.from_numpy(indices_to_dense(ml, K1)[None]),
+                "matching_scores_l": torch.from_numpy(_dense_scores(self.dist_l, self.stride_l, p, K0, K1)),
+                "matches_p": torch.from_numpy(indices_to_dense(mp, N1)[None]),
+                "matching_scores_p": torch.from_numpy(_dense_scores(self.dist_p, self.stride_p, p, N0, N1))}
+
+
 class PairEngine:
     """Batched line-descriptor forward + mutual-NN matching on one GPU."""
 
@@ -278,6 +342,151 @@ class PairEngine:
                                      gather=gather, **kw)
         return PairMatches(out["matches0"], out["scores0"], out["counts"], np.asarray(off0, dtype=np.int32),
                            out["dist_key"], out["stride"], d0 if keep_desc else None, d1 if keep_desc else None)
+
+    # ------------------------------------------------------------------ image-level front-end
+    def _stage(self, arrays: dict) -> dict:
+        """One pinned staging buffer, one non-blocking H2D copy: -> device views of the host arrays.  The buffer
+        is held (with an event behind the copy) until the copy has finished, so it is never reused early."""
+        self._staging = [(b, e) for b, e in getattr(self, "_staging", []) if not e.query()]
+        layout, total = {}, 0
+        for k, a in arrays.items():
+            a = np.ascontiguousarray(a)
+            total = (total + 15) // 16 * 16
+            layout[k] = (total, a)
+            total += a.nbytes
+        host = torch.empty(max(total, 16), dtype=torch.uint8, pin_memory=True)
+        hv = host.numpy()
+        for o, a in layout.values():
+            hv[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
+        dev = host.to(self.device, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record(torch.cuda.current_stream(self.device))
+        self._staging.append((host, ev))
+        tdt = {np.dtype(np.float64): torch.float64, np.dtype(np.float32): torch.float32, np.dtype(np.int32): torch.int32}
+        return {k: dev[o:o + a.nbytes].view(tdt[a.dtype]).view(a.shape) for k, (o, a) in layout.items()}
+
+    def _image_specs(self, images, auto_min_length):
+        specs = [(im["klines"], tuple(im["image_shape"]), im.get("valid_mask")) for im in images]
+        return specs, [LP.tokenizer_config(self.model.config, sh, auto_min_length) for _, sh, _ in specs]
+
+    def _tokenize(self, host: "LP.TokenizerBatch", images: Sequence[dict], dv: dict) -> LineBatch:
+        """ltr_tokenize_batch of `host` (its per-key-line arrays already staged in `dv`) -> the packed LineBatch."""
+        S, T, K, n = host.n_sublines, host.max_tokens, host.n_keylines, host.n_images
+        f32 = dict(dtype=torch.float32, device=self.device)
+        out = [torch.empty(shape, **f32) for shape in ((S, 2, 2), (S, T, 2), (S, T + 1, 1), (S, 1), (S, 2), (S, T, 256), (S, T, 1))]
+        slines, pnt, mask, resp, ang, desc, score = out
+        keep, tab = [], (N.LtrTokenizeImage * max(n, 1))()
+        for i, im in enumerate(images):
+            if host.cu_lines[i + 1] == host.cu_lines[i]:
+                continue
+            dense = im["dense_descriptor"]
+            if not dense.is_cuda or dense.device != self.device:
+                raise N.LtrError(f"match_images: SuperPoint maps must be on {self.device} (there is no CPU fallback)")
+            dense = dense.float().contiguous()
+            smap = im["dense_score"].float().contiguous()
+            keep += [dense, smap]
+            tab[i] = N.LtrTokenizeImage(dense.data_ptr(), smap.data_ptr(), float(host.token_distance[i]),
+                                        dense.shape[-2], dense.shape[-1], smap.shape[-2], smap.shape[-1])
+        cu = np.ascontiguousarray(host.cu_lines, dtype=np.int32)
+        ptr = lambda k: dv[k].data_ptr()
+        inp = N.LtrTokenizeBatchInput(ptr("sp"), ptr("ep"), ptr("epc"), ptr("length"), ptr("angle"), ptr("n_tok"),
+                                      ptr("sub0"), ptr("sub2line"), ptr("line_image"), n, K, S, T, 256,
+                                      1 if int(torch.__version__[2]) > 2 else 0, tab,
+                                      cu.ctypes.data_as(N.c_int32_p))
+        p = lambda t: C.c_void_p(t.data_ptr())
+        with torch.cuda.device(self.device):
+            rc = N.load().ltr_tokenize_batch(C.byref(inp), *[p(t) for t in out], self.device.index,
+                                             C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
+        N.check(rc, "ltr_tokenize_batch")
+        batch = LineBatch(slines, resp, ang, pnt, desc, score, cu, host.sub0 if host.split else None,
+                          host.cuk if host.split else None)
+        batch._dev_cache[("cu_lines", str(self.device))] = dv["cu_lines"]
+        return batch
+
+    @staticmethod
+    def _tok_arrays(host: "LP.TokenizerBatch") -> dict:
+        return {"sp": host.sp, "ep": host.ep, "epc": host.epc, "length": host.length, "angle": host.angle,
+                "n_tok": host.n_tok, "sub0": host.sub0, "sub2line": host.sub2line, "line_image": host.line_image,
+                "cu_lines": host.cu_lines}
+
+    def tokenize_images(self, images: Sequence[dict], auto_min_length: bool = True) -> LineBatch:
+        """Tokenise many images in one `ltr_tokenize_batch` call -> device LineBatch (rows of all images
+        concatenated; sub_off / cuk set whenever some key line is split into sublines).
+
+        Per image a dict: 'klines' (cv2 KeyLine list or `change_cv2_T_np` dict), 'image_shape' (1,1,H,W),
+        the SuperPoint outputs on this engine's device ('dense_descriptor' [1,256,H/8,W/8], 'dense_score'
+        [1,H,W], ...) and optionally 'valid_mask'.  Filters and settings follow `Matching.forward`
+        (auto_min_length: min_length and token_distance from each image's size)."""
+        specs, cfgs = self._image_specs(images, auto_min_length)
+        return self.tokenize_prepared(LP.prepare_tokenizer_batch(specs, cfgs), images)
+
+    def tokenize_prepared(self, host: "LP.TokenizerBatch", images: Sequence[dict]) -> LineBatch:
+        """`tokenize_images` for a batch already prepared on the host (`line_process.prepare_tokenizer_batch`,
+        whose per-image settings may differ except for max_tokens); `images` supply the SuperPoint maps."""
+        return self._tokenize(host, images, self._stage(self._tok_arrays(host)))
+
+    def match_images(self, images0: Sequence[dict], images1: Sequence[dict], line_thresh: Optional[float] = None,
+                     point_thresh: float = 0.7, want_scores: bool = False, auto_min_length: bool = True) -> ImagePairMatches:
+        """`Matching.forward` (models/matching.py:18-86) for P image pairs at once, from detector + SuperPoint
+        outputs (image dicts as for `tokenize_images`, plus 'keypoints' [N,2] and 'descriptors' [256,N]):
+        one `ltr_tokenize_batch` over the 2P images, one encode and one line `ltr_match` with key-line merging
+        (`match_packed`), one point `ltr_match` over all pairs (mutual NN, threshold point_thresh).
+        line_thresh defaults to the model's nn_threshold.  Host sizes come from the inputs' shapes: the call
+        never waits for the device."""
+        if len(images0) != len(images1):
+            raise N.LtrError(f"match_images: {len(images0)} side-0 images but {len(images1)} side-1 images")
+        if line_thresh is None:
+            line_thresh = self.model.config.get("nn_threshold", 0.8)
+        P = len(images0)
+        images = list(images0) + list(images1)
+        specs, cfgs = self._image_specs(images, auto_min_length)
+        host = LP.prepare_tokenizer_batch(specs, cfgs)
+        kp = [_first(im["keypoints"]) for im in images]
+        dp = [_first(im["descriptors"]) for im in images]
+        npts = np.array([int(d.shape[1]) for d in dp], dtype=np.int64)
+        cup = np.zeros(2 * P + 1, dtype=np.int64)
+        cup[1:] = np.cumsum(npts)
+        i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
+        cu, cuk, so = host.cu_lines, host.cuk, host.sub0
+        R0, K0 = int(cu[P]), int(cuk[P])
+        arrays = self._tok_arrays(host)
+        # everything match_packed and the point match upload, in the same staging buffer
+        arrays.update(cu0=i32(cu[:P + 1]), cu1=i32(cu[P:] - R0), p_cu0=i32(cup[:P + 1]), p_cu1=i32(cup[P:] - cup[P]))
+        if host.split:
+            arrays.update(cuk0=i32(cuk[:P + 1]), cuk1=i32(cuk[P:] - K0), sub_off0=i32(so[:K0 + 1]), sub_off1=i32(so[K0:] - R0))
+        dv = self._stage(arrays)
+        batch = self._tokenize(host, images, dv)
+        mx = lambda a: int(np.diff(a).max(initial=0))
+        split = dict(cu0=dv["cu0"], cu1=dv["cu1"], max_n0=mx(cu[:P + 1]), max_n1=mx(cu[P:]), total_k0=K0,
+                     total_k1=int(cuk[-1]) - K0)
+        if host.split:
+            split.update(cuk0=dv["cuk0"], cuk1=dv["cuk1"], sub_off0=dv["sub_off0"], sub_off1=dv["sub_off1"],
+                         max_k0=mx(cuk[:P + 1]), max_k1=mx(cuk[P:]))
+        batch._dev_cache[("packed_split", str(self.device))] = split
+        i32d = dict(dtype=torch.int32, device=self.device)
+        f32d = dict(dtype=torch.float32, device=self.device)
+
+        def unmatched(n_rows):   # a side without any line / point in the whole batch: nothing to match
+            return (torch.full((n_rows,), -1, **i32d), torch.full((n_rows,), float("inf"), **f32d),
+                    torch.zeros(P, **i32d), torch.empty(0, **f32d) if want_scores else None, 0)
+
+        if K0 > 0 and int(cuk[-1]) > K0:
+            lm = self.match_packed(batch, P, line_thresh, want_dist=want_scores)
+            lines = (lm.matches0, lm.scores0, lm.counts, lm.dist, lm.stride)
+        else:
+            lines = unmatched(K0)
+        N0 = int(cup[P])
+        if N0 > 0 and int(cup[-1]) > N0:
+            cat = lambda ds: torch.cat([d.float().contiguous().reshape(-1) for d in ds])   # [256, N_i] blocks back to back
+            pm = _ops.match_descriptors(cat(dp[:P]), cat(dp[P:]), N.LAYOUT_CHANNEL_FIRST, P, float(point_thresh), True,
+                                        cu0=dv["p_cu0"], cu1=dv["p_cu1"], max_n0=mx(cup[:P + 1]), max_n1=mx(cup[P:]),
+                                        d=256, want_dist=want_scores)
+            points = (pm["matches0"], pm["scores0"], pm["counts"], pm["dist_key"], pm["stride"])
+        else:
+            points = unmatched(N0)
+        return ImagePairMatches(*lines[:3], i32(cuk[:P + 1]), *points[:3], i32(cup[:P + 1]),
+                                host.klines[:P], host.klines[P:], kp[:P], kp[P:],
+                                lines[3], lines[4], points[3], points[4])
 
     def match_packed_host(self, host: LineBatch, n_pairs: int, nn_thresh: Optional[float] = None, mutual=True,
                           n_chunks: int = 4):

@@ -13,6 +13,8 @@ tokeniser is tested against.  The cheap per-image filters (`remove_borders`,
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass
+from typing import List, Tuple
 
 import numpy as np
 import torch
@@ -36,6 +38,140 @@ def get_dist_matrix(desc0, desc1):
 
 
 # --------------------------------------------------------------------------- tokeniser glue
+def keyline_geometry(kl, length, token_distance, max_tokens, width, height):
+    """Per-key-line geometry of the tokeniser (reference line_tokenizer, models/line_process.py:100-196),
+    vectorised over the key lines of one image or of many images concatenated.  `kl` [K,2,2] float64
+    has its end points clipped IN PLACE to (width-0.6, height-0.6), as the reference does; token_distance,
+    width and height are scalars or per-key-line arrays.  -> dict of n_tok, n_sub [K] int64, sub0 [K+1]
+    (first subline of every key line, the key-line CSR), sub2line [S], and the float64 start point sp,
+    end point ep (before the clip) and epc (after it), each [K,2]."""
+    T = int(max_tokens)
+    K = len(kl)
+    length = np.asarray(length, dtype=np.float64)
+    n_tok = np.ceil(length / token_distance).astype(np.int64)
+    n_sub = -(-n_tok // T)
+    geo = np.sqrt(((kl[:, 1] - kl[:, 0]) ** 2).sum(axis=1))
+    assert bool((geo >= np.maximum(n_tok - 2, 0) * token_distance).all()), "distance should be smaller than line length!"
+    sp = np.ascontiguousarray(kl[:, 0], dtype=np.float64)
+    ep = np.ascontiguousarray(kl[:, 1], dtype=np.float64).copy()
+    kl[:, 1, 0] = np.minimum(kl[:, 1, 0], np.asarray(width) - 0.6)      # in place, like the reference
+    kl[:, 1, 1] = np.minimum(kl[:, 1, 1], np.asarray(height) - 0.6)
+    epc = np.ascontiguousarray(kl[:, 1], dtype=np.float64)
+    sub0 = np.zeros(K + 1, dtype=np.int64)
+    sub0[1:] = np.cumsum(n_sub)
+    sub2line = np.repeat(np.arange(K), n_sub)
+    return {"n_tok": n_tok, "n_sub": n_sub, "sub0": sub0, "sub2line": sub2line, "sp": sp, "ep": ep, "epc": epc}
+
+
+def tokenizer_config(config, image_shape, auto_min_length=True):
+    """The tokeniser settings `Matching.forward` uses for an image of shape (1,1,H,W) (models/matching.py:29-32):
+    with auto_min_length, min_length and token_distance follow the image size."""
+    cfg = {k: config[k] for k in ("min_length", "token_distance", "max_tokens", "remove_borders", "max_keylines")}
+    if auto_min_length:
+        cfg["min_length"] = max(16, max(image_shape) / 40)
+        cfg["token_distance"] = max(8, max(image_shape) / 80)
+    return cfg
+
+
+def filter_keylines(klines, image_shape, cfg, valid_mask=None):
+    """`LineTransformer.preprocess` up to the tokeniser: cv2 KeyLine list (or a `change_cv2_T_np` dict, which is
+    copied, not modified) -> the kept key lines.  valid_mask None means all valid; it is honoured only as a
+    numpy array, like the reference."""
+    if isinstance(klines, dict):
+        klines = {k: np.array(v, copy=True) for k, v in klines.items()}
+    else:
+        klines = change_cv2_T_np(klines)
+    height, width = int(image_shape[-2]), int(image_shape[-1])
+    if valid_mask is None:
+        valid_mask = np.ones((height, width))
+    klines = remove_borders(klines, cfg["remove_borders"], height, width, valid_mask)
+    klines = filter_by_length(klines, cfg["min_length"], cfg["max_keylines"])
+    klines["klines"] = np.asarray(klines["klines"], dtype=np.float64).reshape(-1, 2, 2)
+    klines["length_klines"] = np.asarray(klines["length_klines"], dtype=np.float64).reshape(-1)
+    klines["angles"] = np.asarray(klines["angles"], dtype=np.float64).reshape(-1, 2)
+    return klines
+
+
+@dataclass
+class TokenizerBatch:
+    """Host side of one `ltr_tokenize_batch` call: the key lines of many images concatenated image by image.
+
+    Per key line: sp, ep, epc [K,2] float64, length [K] float64, angle [K,2] float32, n_tok, line_image [K]
+    int32; sub0 int32 [K+1] (global subline numbering: the key-line CSR of the packed LineBatch),
+    sub2line int32 [S]; per image: cu_lines int32 [n+1] (subline offsets), cuk int32 [n+1] (key-line
+    offsets), token_distance float64 [n], shapes (H, W), and its kept key lines after the in-place clip
+    (klines, views into one [K,2,2] array) with their length_klines and angles."""
+    sp: np.ndarray
+    ep: np.ndarray
+    epc: np.ndarray
+    length: np.ndarray
+    angle: np.ndarray
+    n_tok: np.ndarray
+    line_image: np.ndarray
+    sub0: np.ndarray
+    sub2line: np.ndarray
+    cu_lines: np.ndarray
+    cuk: np.ndarray
+    token_distance: np.ndarray
+    shapes: List[Tuple[int, int]]
+    max_tokens: int
+    klines: List[np.ndarray]
+    length_klines: List[np.ndarray]
+    angles: List[np.ndarray]
+
+    @property
+    def n_images(self) -> int:
+        return len(self.shapes)
+
+    @property
+    def n_keylines(self) -> int:
+        return int(self.cuk[-1])
+
+    @property
+    def n_sublines(self) -> int:
+        return int(self.cu_lines[-1])
+
+    @property
+    def split(self) -> bool:
+        """True when some key line is cut into several sublines (key-line merging is needed)."""
+        return self.n_sublines != self.n_keylines
+
+
+def prepare_tokenizer_batch(images, configs) -> TokenizerBatch:
+    """images: per image (klines, image_shape (1,1,H,W), valid_mask or None), klines a cv2 KeyLine list or a
+    `change_cv2_T_np` dict; configs: per-image tokeniser settings (`tokenizer_config`).  Every image must use
+    the same max_tokens (one token-slot count per batch)."""
+    from . import _native as N
+    if len(images) != len(configs):
+        raise N.LtrError("prepare_tokenizer_batch: one config per image required")
+    Ts = {int(c["max_tokens"]) for c in configs}
+    if len(Ts) > 1:
+        raise N.LtrError(f"prepare_tokenizer_batch: all images of a batch need the same max_tokens, got {sorted(Ts)}")
+    T = Ts.pop() if Ts else 21
+    kept = [filter_keylines(kl, shape, cfg, vm) for (kl, shape, vm), cfg in zip(images, configs)]
+    counts = np.array([len(k["klines"]) for k in kept], dtype=np.int64)
+    n = len(kept)
+    shapes = [(int(shape[-2]), int(shape[-1])) for _, shape, _ in images]
+    td = np.array([float(c["token_distance"]) for c in configs], dtype=np.float64)
+    cat = lambda key, shp, dt: (np.concatenate([k[key] for k in kept]).astype(dt, copy=False) if n
+                                else np.zeros(shp, dtype=dt))
+    kl = np.ascontiguousarray(cat("klines", (0, 2, 2), np.float64))
+    length = np.ascontiguousarray(cat("length_klines", (0,), np.float64))
+    angle = np.ascontiguousarray(cat("angles", (0, 2), np.float32))
+    line_image = np.repeat(np.arange(n), counts)
+    H = np.array([h for h, _ in shapes], dtype=np.int64)[line_image]
+    W = np.array([w for _, w in shapes], dtype=np.int64)[line_image]
+    g = keyline_geometry(kl, length, td[line_image], T, W, H)
+    cuk = np.zeros(n + 1, dtype=np.int64)
+    cuk[1:] = np.cumsum(counts)
+    bounds = list(zip(cuk[:-1], cuk[1:]))
+    i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
+    return TokenizerBatch(g["sp"], g["ep"], g["epc"], length, angle, i32(g["n_tok"]), i32(line_image), i32(g["sub0"]),
+                          i32(g["sub2line"]), i32(g["sub0"][cuk]), i32(cuk), td, shapes, T,
+                          [kl[a:b] for a, b in bounds], [length[a:b] for a, b in bounds],
+                          [angle[a:b] for a, b in bounds])
+
+
 def get_angles(lines):
     """Orientation code (cos 2a, sin 2a) with a = atan2(dx, dy) folded into [0, pi)."""
     if len(lines) == 0:
@@ -193,22 +329,11 @@ def line_tokenizer_gpu(klines, token_distance, max_tokens, pred_superpoint, imag
     dev = dense.device
     height, width = image_shape
     T = int(max_tokens)
-    kl = klines["klines"]
-    K = len(kl)
+    K = len(klines["klines"])
     length = np.ascontiguousarray(klines["length_klines"], dtype=np.float64)
-    n_tok = np.ceil(length / token_distance).astype(np.int64)
-    n_sub = -(-n_tok // T)
-    geo = np.sqrt(((kl[:, 1] - kl[:, 0]) ** 2).sum(axis=1))
-    assert bool((geo >= np.maximum(n_tok - 2, 0) * token_distance).all()), "distance should be smaller than line length!"
-    sp = np.ascontiguousarray(kl[:, 0], dtype=np.float64)
-    ep = np.ascontiguousarray(kl[:, 1], dtype=np.float64).copy()
-    kl[:, 1, 0] = np.minimum(kl[:, 1, 0], width - 0.6)      # in place, like the reference
-    kl[:, 1, 1] = np.minimum(kl[:, 1, 1], height - 0.6)
-    epc = np.ascontiguousarray(kl[:, 1], dtype=np.float64)
-    sub0 = np.zeros(K + 1, dtype=np.int64)
-    sub0[1:] = np.cumsum(n_sub)
+    g = keyline_geometry(klines["klines"], length, token_distance, T, width, height)
+    n_tok, n_sub, sub0, sub2line, sp, ep, epc = (g[k] for k in ("n_tok", "n_sub", "sub0", "sub2line", "sp", "ep", "epc"))
     S = int(sub0[-1])
-    sub2line = np.repeat(np.arange(K), n_sub)
     angles = np.ascontiguousarray(klines["angles"], dtype=np.float32)
     up = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
     d_sp, d_ep, d_epc, d_len = up(sp, np.float64), up(ep, np.float64), up(epc, np.float64), up(length, np.float64)

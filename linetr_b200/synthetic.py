@@ -182,3 +182,52 @@ def make_descriptor_pair(seed: int, n0: int, n1: int = None, d: int = D_MODEL, n
     perm = perm[perm < n0][:n1] if n1 <= n0 else np.concatenate([rng.permutation(n0), rng.integers(0, n0, n1 - n0)])
     d1 = _unit(d0[perm] + np.float32(noise) * rng.standard_normal((n1, d)).astype(np.float32))
     return np.ascontiguousarray(d0.T), np.ascontiguousarray(d1.T), perm
+
+
+# ------------------------------------------------------------------ image-level inputs (PairEngine.match_images)
+class SyntheticKeyLine:
+    """The fields of a cv2 line_descriptor KeyLine the tokeniser reads (reference models/line_process.py:6-20)."""
+
+    def __init__(self, x0, y0, x1, y1, octave=0):
+        self.startPointX, self.startPointY, self.endPointX, self.endPointY = float(x0), float(y0), float(x1), float(y1)
+        self.lineLength = float(np.hypot(x1 - x0, y1 - y0)) / (2 ** octave)
+        self.octave = int(octave)
+
+
+def make_image_pair(seed: int, n_lines: int, n_points: int, w: int = 640, h: int = 480, jitter_px: float = 0.5,
+                    map_noise: float = 0.05):
+    """A synthetic image pair as detector + SuperPoint outputs (CPU torch tensors): image 1 is a jittered copy of
+    image 0 (key lines, keypoints, dense maps and point descriptors), so lines and points have true matches.
+    Each image dict holds 'klines' (SyntheticKeyLine list), 'image_shape' (1,1,h,w), 'keypoints' [N,2],
+    'scores' [N], 'descriptors' [256,N], 'dense_descriptor' [1,256,h/8,w/8] and 'dense_score' [1,h,w]."""
+    import torch
+    rng = np.random.Generator(np.random.PCG64(seed))
+    x0, y0 = rng.uniform(8, w - 9, n_lines), rng.uniform(8, h - 9, n_lines)
+    ang, ln = rng.uniform(0, 2 * np.pi, n_lines), rng.uniform(20, 300, n_lines)
+    x1 = np.clip(x0 + ln * np.cos(ang), 8, w - 9)
+    y1 = np.clip(y0 + ln * np.sin(ang), 8, h - 9)
+    ends0 = np.stack([x0, y0, x1, y1], 1)
+    ends1 = np.clip(ends0 + rng.normal(0, jitter_px, ends0.shape), 8, [w - 9, h - 9, w - 9, h - 9])
+    octave = rng.integers(0, 2, n_lines)
+    kp0 = np.stack([rng.uniform(0, w - 1, n_points), rng.uniform(0, h - 1, n_points)], 1).astype(np.float32)
+    kp1 = np.clip(kp0 + rng.normal(0, jitter_px, kp0.shape), 0, [w - 1, h - 1]).astype(np.float32)
+    d0 = _unit(rng.standard_normal((n_points, D_MODEL)).astype(np.float32))
+    d1 = _unit(d0 + map_noise * rng.standard_normal(d0.shape).astype(np.float32))
+    dense0 = rng.standard_normal((1, D_MODEL, h // 8, w // 8)).astype(np.float32)
+    dense1 = dense0 + map_noise * rng.standard_normal(dense0.shape).astype(np.float32)
+    score0 = rng.uniform(0, 1, (1, h, w)).astype(np.float32)
+    score1 = np.clip(score0 + map_noise * rng.standard_normal(score0.shape), 0, 1).astype(np.float32)
+
+    def image(ends, kp, desc, dense, score):
+        dn = torch.from_numpy(dense)
+        return {"klines": [SyntheticKeyLine(*e, o) for e, o in zip(ends, octave)], "image_shape": (1, 1, h, w),
+                "keypoints": torch.from_numpy(kp), "scores": torch.from_numpy(score.reshape(-1)[:len(kp)].copy()),
+                "descriptors": torch.from_numpy(np.ascontiguousarray(desc.T)),
+                "dense_descriptor": torch.nn.functional.normalize(dn, dim=1), "dense_score": torch.from_numpy(score)}
+    return image(ends0, kp0, d0, dense0, score0), image(ends1, kp1, d1, dense1, score1)
+
+
+def image_to(im: dict, device) -> dict:
+    """Tensors of an image dict moved to `device` (klines and shapes untouched)."""
+    import torch
+    return {k: (v.to(device) if isinstance(v, torch.Tensor) else v) for k, v in im.items()}
