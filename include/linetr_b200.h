@@ -19,6 +19,8 @@
  *                                 + nn_matcher_distmat (models/nn_matcher.py:3-31); with
  *                                 descriptors as input it is nn_matcher (models/nn_matcher.py:33-43).
  *   ltr_match_distmat          <- nn_matcher_distmat on a caller-supplied distance matrix.
+ *   ltr_image_tiles +          <- Matching.forward with a side already in `data` (models/matching.py:20-60):
+ *   ltr_match_indexed             images encoded once, matched in any number of pairs.
  *
  * Conventions: return 0 on success, a negative LTR_E_* code on failure (message via
  * ltr_last_error(), thread-local).  All device pointers are caller-owned and must live on
@@ -213,6 +215,51 @@ typedef struct {
 int64_t ltr_match_workspace_bytes(const LtrMatchInput* in);
 
 int ltr_match(const LtrMatchInput* in, const LtrMatchOutput* out, int32_t device, void* stream);
+
+/* Image sets: encode each image once, then match any list of pairs between two image pools.
+ *
+ * An image-aligned tile image holds the descriptors of a pool of images in the split-bf16 format the
+ * tensor-core matcher contracts (the format of LtrEncodeOutput.desc_tiles): image i occupies the
+ * ceil(L_i / 128) 128-row tiles starting at tile tile_off[i], where tile_off is the prefix sum of
+ * ceil(L_i / 128) (tile_off[0] = 0, n_tiles = tile_off[n_images]); rows past L_i in an image's last tile are
+ * zero.  ltr_image_tiles_bytes(n_images, cu_host) = n_tiles * 128 KB (cu_host: HOST [n_images+1] line
+ * offsets).  ltr_image_tiles builds it in one launch: desc is the pool's fp32 descriptors, either rows
+ * [cu[n_images], 256] (LTR_LAYOUT_ROWS) or channel-first [256, L_i] per image, image i at 256 * cu[i]
+ * (LTR_LAYOUT_CHANNEL_FIRST, the layout of SuperPoint's point descriptors); cu_dev and tile_off_dev are device
+ * copies of the offsets, max_n = max L_i, out is 16-byte aligned. */
+int64_t ltr_image_tiles_bytes(int32_t n_images, const int32_t* cu_host);
+int ltr_image_tiles(const float* desc, int32_t layout, const int32_t* cu_dev, const int32_t* tile_off_dev, int32_t n_images,
+                    int32_t max_n, int32_t n_tiles, void* out, int32_t device, void* stream);
+
+/* Pair list over two image pools for ltr_match_indexed (device arrays unless noted).  Pair p matches image
+ * img0[p] of pool 0 against image img1[p] of pool 1.  img0 / img1 are NOT range-checked on the device: every
+ * entry must lie in [0, n_images) of its pool (validate on the host before the call).  out_off0 / out_off1
+ * [n_pairs+1] are the per-pair output offsets: prefix sums over the pairs of the side-0 / side-1 key-line counts
+ * (line counts without key-line merging; point counts for points); total_out0 / total_out1 = out_off0[n_pairs] /
+ * out_off1[n_pairs] (host values: scratch sizing). */
+typedef struct {
+  const int32_t* img0;
+  const int32_t* img1;
+  const void* tiles0;        /* image-aligned tile image of pool 0 (ltr_image_tiles) */
+  const void* tiles1;
+  const int32_t* tile_off0;  /* [n_images0 + 1] */
+  const int32_t* tile_off1;
+  int32_t n_tiles0, n_tiles1;
+  const int32_t* out_off0;
+  const int32_t* out_off1;
+  int32_t total_out0, total_out1;
+} LtrPairIndex;
+
+/* ltr_match over a pair list.  In this mode desc0/desc1, cu0/cu1 (required), cuk0/cuk1 and sub_off0/sub_off1
+ * describe the IMAGES of pool 0 and pool 1 (the two pools may be the same arrays), max_n* / max_k* bound the
+ * images' line / key-line counts and total_n0/total_n1 are the pools' line counts; n0, n1, tiles* of
+ * LtrMatchInput are ignored.  Outputs are per pair: matches0 / scores0 of pair p at out_off0[p] + k, nn1 at
+ * out_off1[p] + j, counts[p], dist_key at p * dist_pair_stride, dist_sub at p * max_n0 * max_n1.
+ * Supported: d == 256, dist_mode 0, with or without key-line merging; dist_mode 1 and `gather` return
+ * LTR_E_UNSUPPORTED. */
+int64_t ltr_match_indexed_workspace_bytes(const LtrMatchInput* in, const LtrPairIndex* idx);
+int ltr_match_indexed(const LtrMatchInput* in, const LtrPairIndex* idx, const LtrMatchOutput* out, int32_t device,
+                      void* stream);
 
 /* nn_matcher_distmat on caller-supplied distance matrices (device, row-major [n0, n1],
  * pair p at p*dist_pair_stride, 0 = n0*n1); negative entries are clipped to 0 as the

@@ -3,7 +3,7 @@
 Drop-in names (same call surface as yosungho/LineTR `models/`):
     LineTransformer, get_dist_matrix, nn_matcher, nn_matcher_distmat
 Batched front-end:
-    PairEngine, LineBatch, ImagePairMatches
+    PairEngine, LineBatch, ImagePairMatches, ImageSet, exhaustive_pairs
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -23,6 +23,8 @@ _LAZY = {
     "PairEngine": ("engine", "PairEngine"),
     "LineBatch": ("engine", "LineBatch"),
     "ImagePairMatches": ("engine", "ImagePairMatches"),
+    "ImageSet": ("engine", "ImageSet"),
+    "exhaustive_pairs": ("engine", "exhaustive_pairs"),
 }
 
 

@@ -24,6 +24,7 @@ EXPORTED_SYMBOLS = (
     "ltr_desc_tiles_bytes", "ltr_encode", "ltr_match_workspace_bytes", "ltr_match", "ltr_gather_wait", "ltr_match_distmat",
     "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
+    "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
@@ -65,6 +66,12 @@ class LtrMatchInput(C.Structure):
                 ("total_n0", C.c_int32), ("total_n1", C.c_int32), ("dist_mode", C.c_int32),
                 ("tiles0", C.c_void_p), ("tiles1", C.c_void_p), ("tiles_lines0", C.c_int32), ("tiles_lines1", C.c_int32),
                 ("tiles_row0_0", C.c_int32), ("tiles_row0_1", C.c_int32)]
+
+
+class LtrPairIndex(C.Structure):
+    _fields_ = [("img0", C.c_void_p), ("img1", C.c_void_p), ("tiles0", C.c_void_p), ("tiles1", C.c_void_p),
+                ("tile_off0", C.c_void_p), ("tile_off1", C.c_void_p), ("n_tiles0", C.c_int32), ("n_tiles1", C.c_int32),
+                ("out_off0", C.c_void_p), ("out_off1", C.c_void_p), ("total_out0", C.c_int32), ("total_out1", C.c_int32)]
 
 
 GATHER_SLOTS = 8
@@ -117,6 +124,9 @@ def load():
             f"linetr_b200: native CUDA library not built ({_LIB_PATH}); run tools/build_native.sh "
             "or __graft_entry__.build().  There is no CPU/PyTorch fallback.")
     lib = C.CDLL(_LIB_PATH)
+    missing = [s for s in EXPORTED_SYMBOLS if not hasattr(lib, s)]
+    if missing:
+        raise LtrError(f"linetr_b200: the native library predates this binding (missing {', '.join(missing)}); rebuild it")
     lib.ltr_abi_version.restype = C.c_int
     lib.ltr_last_error.restype = C.c_char_p
     lib.ltr_create.argtypes = [C.POINTER(LtrTensor), C.c_int32, C.POINTER(LtrConfig), C.c_int32,
@@ -135,6 +145,16 @@ def load():
     lib.ltr_match_workspace_bytes.restype = C.c_int64
     lib.ltr_match.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrMatchOutput), C.c_int32, C.c_void_p]
     lib.ltr_match.restype = C.c_int
+    lib.ltr_image_tiles_bytes.argtypes = [C.c_int32, c_int32_p]
+    lib.ltr_image_tiles_bytes.restype = C.c_int64
+    lib.ltr_image_tiles.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                    C.c_void_p, C.c_int32, C.c_void_p]
+    lib.ltr_image_tiles.restype = C.c_int
+    lib.ltr_match_indexed_workspace_bytes.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrPairIndex)]
+    lib.ltr_match_indexed_workspace_bytes.restype = C.c_int64
+    lib.ltr_match_indexed.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrPairIndex), C.POINTER(LtrMatchOutput),
+                                      C.c_int32, C.c_void_p]
+    lib.ltr_match_indexed.restype = C.c_int
     lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.ltr_gather_wait.restype = C.c_int
     lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,

@@ -223,6 +223,73 @@ def match_descriptors(desc0, desc1, layout, n_pairs, nn_thresh, mutual=True, *, 
     return out
 
 
+def tile_offsets(cu: np.ndarray) -> np.ndarray:
+    """First 128-row tile of every image in an image-aligned tile image: prefix sum of ceil(L_i / 128), int32 [n+1]."""
+    n = np.diff(np.asarray(cu, dtype=np.int64))
+    t = np.zeros(len(n) + 1, dtype=np.int64)
+    t[1:] = np.cumsum((n + 127) // 128)
+    return t.astype(np.int32)
+
+
+def image_tiles(desc: torch.Tensor, layout: int, cu_host: np.ndarray, cu_dev: torch.Tensor, tile_off_dev: torch.Tensor,
+                n_tiles: int) -> torch.Tensor:
+    """ltr_image_tiles: the image-aligned tile image (uint8 tensor, the matcher's operand format) of a pool of
+    images' descriptors, rows [R, 256] or channel-first [256, L_i] per image back to back."""
+    _req_cuda(desc, "desc")
+    dev = desc.device
+    desc = _f32c(desc)
+    cu_host = np.ascontiguousarray(cu_host, dtype=np.int32)
+    n = len(cu_host) - 1
+    lib = N.load()
+    nbytes = int(lib.ltr_image_tiles_bytes(n, cu_host.ctypes.data_as(N.c_int32_p)))
+    if nbytes < 0:
+        N.check(nbytes, "ltr_image_tiles_bytes")
+    out = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        rc = lib.ltr_image_tiles(_ptr(desc), int(layout), _ptr(cu_dev), _ptr(tile_off_dev), n,
+                                 int(np.diff(cu_host).max(initial=0)), int(n_tiles), _ptr(out), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_image_tiles")
+    return out
+
+
+def match_indexed(desc0, desc1, layout, n_pairs, nn_thresh, *, cu0, cu1, max_n0, max_n1, img0, img1, tiles0, tiles1,
+                  tile_off0, tile_off1, n_tiles0, n_tiles1, out_off0, out_off1, total_out0, total_out1,
+                  matches0, scores0, nn1, counts, sub_off0=None, sub_off1=None, cuk0=None, cuk1=None, max_k0=0, max_k1=0,
+                  dist_key=None, dist_stride=0, mutual=True):
+    """ltr_match_indexed: P pairs over two image pools (pair p = image img0[p] of pool 0 against image img1[p] of
+    pool 1) into caller-allocated outputs (matches0 / scores0 at out_off0[p] + k, nn1 at out_off1[p] + j,
+    counts[p], dist_key at p * dist_stride when given).  Key-line merging when sub_off0 is given; its distance
+    scratch (n_pairs * max_n0 * max_n1 floats) is allocated here."""
+    _req_cuda(desc0, "desc0")
+    _req_cuda(desc1, "desc1")
+    dev = desc0.device
+    desc0, desc1 = _f32c(desc0), _f32c(desc1)
+    seg = sub_off0 is not None
+    f32 = dict(dtype=torch.float32, device=dev)
+    if seg and dist_key is None:
+        dist_stride = max_k0 * max_k1
+        dist_key = torch.empty(max(n_pairs * dist_stride, 1), **f32)
+    dist_sub = torch.empty(max(n_pairs * max_n0 * max_n1, 1), **f32) if seg else None
+    inp = N.LtrMatchInput(desc0.data_ptr(), desc1.data_ptr(), int(layout), 256, int(n_pairs), 0, 0,
+                          *[t.data_ptr() if t is not None else None for t in (cu0, cu1, sub_off0, sub_off1, cuk0, cuk1)],
+                          int(max_n0), int(max_n1), int(max_k0), int(max_k1), int(dist_stride), float(nn_thresh),
+                          int(bool(mutual)), int(desc0.numel() // 256), int(desc1.numel() // 256), 0,
+                          None, None, 0, 0, 0, 0)
+    idx = N.LtrPairIndex(img0.data_ptr(), img1.data_ptr(), tiles0.data_ptr(), tiles1.data_ptr(), tile_off0.data_ptr(),
+                         tile_off1.data_ptr(), int(n_tiles0), int(n_tiles1), out_off0.data_ptr(), out_off1.data_ptr(),
+                         int(total_out0), int(total_out1))
+    lib = N.load()
+    need = int(lib.ltr_match_indexed_workspace_bytes(C.byref(inp), C.byref(idx)))
+    if need < 0:
+        N.check(need, "ltr_match_indexed_workspace_bytes")
+    ws = _match_workspace(dev, need)
+    o = N.LtrMatchOutput(_ptr(matches0).value, _ptr(scores0).value, _ptr(nn1).value, _ptr(counts).value,
+                         _ptr(dist_key).value, _ptr(dist_sub).value, ws.data_ptr(), ws.numel(), None)
+    with torch.cuda.device(dev):
+        rc = lib.ltr_match_indexed(C.byref(inp), C.byref(idx), C.byref(o), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_match_indexed")
+
+
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     """ltr_match_distmat on dist [P, n0, n1] (CUDA).  Returns dict(matches0 [P,n0], scores0, nn1, counts)."""
     _req_cuda(dist, "dist_mat")

@@ -704,6 +704,35 @@ static MatchPlan plan_match(const LtrMatchInput& in, char* base) {
   return pl;
 }
 
+// Pair lists over image pools: both operands are the caller's image-aligned tile images, so the scratch is the
+// per-(pair, line) argmin slots (not needed with key-line merging, whose decisions run on dist_key).
+static MatchPlan plan_match_indexed(const LtrMatchInput& in, const LtrPairIndex& ix, char* base) {
+  MatchPlan pl{};
+  const int mxn[2] = {in.max_n0, in.max_n1};
+  const int tot[2] = {ix.total_out0, ix.total_out1};
+  const int ntiles[2] = {ix.n_tiles0, ix.n_tiles1};
+  const void* tiles[2] = {ix.tiles0, ix.tiles1};
+  const bool seg = in.sub_off0 != nullptr;
+  int64_t off = 0;
+  auto take = [&](int64_t bytes) {
+    char* p = base + off;
+    off = align_up(off + bytes, 1024);
+    return p;
+  };
+  for (int s = 0; s < 2; ++s) {
+    pl.mx[s] = mxn[s];
+    pl.tmax[s] = cdiv(pl.mx[s], 128);
+    pl.total[s] = tot[s];
+    pl.direct[s] = true;
+    pl.img[s] = tiles_image(const_cast<void*>(tiles[s]), (int64_t)ntiles[s] * 128);
+    pl.slot[s] = seg ? nullptr : reinterpret_cast<uint2*>(take((int64_t)std::max(tot[s], 1) * 8));
+    pl.sq[s] = nullptr;
+  }
+  pl.done = reinterpret_cast<int*>(take(256));
+  pl.bytes = off;
+  return pl;
+}
+
 static const char* check_match_input(const LtrMatchInput* in) {
   if (in->d <= 0 || in->d % 16) return "ltr_match: descriptor dim must be a multiple of 16";
   const bool seg = in->sub_off0 != nullptr || in->sub_off1 != nullptr;
@@ -718,9 +747,10 @@ static const char* check_match_input(const LtrMatchInput* in) {
 
 }  // extern "C"
 
-// launch sequence of the tensor-core matcher; returns 0 or an error code
+// launch sequence of the tensor-core matcher; returns 0 or an error code.  ix != nullptr: pair list over image
+// pools (ltr_match_indexed), both sides read the caller's image-aligned tiles
 static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, const MatchPlan& pl, bool seg, long long stride_key,
-                        cudaStream_t s) {
+                        cudaStream_t s, const LtrPairIndex* ix = nullptr) {
   const int P = in.n_pairs;
   const bool want_nn = out.matches0 != nullptr && !seg;
   const bool both = want_nn && in.mutual;
@@ -749,6 +779,12 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
       ma.s[sd].img = pl.img[sd]; ma.s[sd].cu = cu[sd]; ma.s[sd].n = n[sd];
       ma.s[sd].tile_mode = pl.direct[sd] ? 1 : 0; ma.s[sd].tile_row0 = pl.direct[sd] ? tr0[sd] : 0;
       ma.s[sd].tmax = pl.tmax[sd]; ma.s[sd].sq = pl.sq[sd]; ma.s[sd].slot = pl.slot[sd];
+      if (ix) {
+        ma.s[sd].tile_mode = 2; ma.s[sd].tile_row0 = 0;
+        ma.s[sd].pimg = sd ? ix->img1 : ix->img0;
+        ma.s[sd].tile_off = sd ? ix->tile_off1 : ix->tile_off0;
+        ma.s[sd].out_off = sd ? ix->out_off1 : ix->out_off0;
+      }
     }
     ma.dist_mode = in.dist_mode;
     ma.dist = seg ? out.dist_sub : out.dist_key;
@@ -773,6 +809,10 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
     ta.matches0 = out.matches0; ta.scores0 = out.scores0; ta.nn1 = out.nn1; ta.counts = out.counts;
     ta.max0 = pl.mx[0];
     ta.done = pl.done; ta.n_pairs = P; ta.world = 1;
+    if (ix) {
+      ta.pimg[0] = ix->img0; ta.pimg[1] = ix->img1;
+      ta.out_off[0] = ix->out_off0; ta.out_off[1] = ix->out_off1;
+    }
     if (out.gather && out.gather->world > 1) {
       const LtrPeerGather& g = *out.gather;
       ta.mc_base = reinterpret_cast<int*>(g.mc_base);
@@ -849,6 +889,98 @@ int ltr_match(const LtrMatchInput* in, const LtrMatchOutput* out, int32_t device
   na.dist = out->dist_key; na.stride = stride_key;
   na.cuk0 = seg ? in->cuk0 : in->cu0; na.cuk1 = seg ? in->cuk1 : in->cu1;
   na.n0 = in->n0; na.n1 = in->n1; na.thr = in->nn_thresh; na.mutual = in->mutual;
+  na.matches0 = out->matches0; na.scores0 = out->scores0; na.nn1 = out->nn1; na.counts = out->counts;
+  return run_nn(na, in->n_pairs, mk0, mk1, s);
+}
+
+int64_t ltr_image_tiles_bytes(int32_t n_images, const int32_t* cu_host) {
+  if (n_images < 0 || (n_images > 0 && !cu_host)) return set_error(LTR_E_INVALID, "ltr_image_tiles_bytes: bad argument");
+  int64_t tiles = 0;
+  for (int i = 0; i < n_images; ++i) {
+    const int L = cu_host[i + 1] - cu_host[i];
+    if (L < 0) return set_error(LTR_E_INVALID, "ltr_image_tiles_bytes: cu must not decrease");
+    tiles += cdiv(L, 128);
+  }
+  return tiles * 128 * MT_D * 2 * 2;   // hi + lo plane, bf16
+}
+
+int ltr_image_tiles(const float* desc, int32_t layout, const int32_t* cu_dev, const int32_t* tile_off_dev, int32_t n_images,
+                    int32_t max_n, int32_t n_tiles, void* out, int32_t device, void* stream) {
+  if (n_images < 0 || max_n < 0 || n_tiles < 0) return set_error(LTR_E_INVALID, "ltr_image_tiles: negative count");
+  if (layout != LTR_LAYOUT_ROWS && layout != LTR_LAYOUT_CHANNEL_FIRST) return set_error(LTR_E_INVALID, "ltr_image_tiles: bad layout");
+  if (n_images == 0 || max_n == 0 || n_tiles == 0) return LTR_OK;
+  if (!desc || !cu_dev || !tile_off_dev || !out) return set_error(LTR_E_INVALID, "ltr_image_tiles: null argument");
+  if (reinterpret_cast<uintptr_t>(out) & 15) return set_error(LTR_E_INVALID, "ltr_image_tiles: out must be 16-byte aligned");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  DescTilesArgs da{};
+  da.layout = layout;
+  da.d[0] = desc; da.cu[0] = cu_dev; da.tile_off[0] = tile_off_dev;
+  da.img[0] = tiles_image(out, (int64_t)n_tiles * 128);
+  da.tmax[0] = cdiv(max_n, 128);
+  LaunchScope ls(KC_DESC_TILES, s);
+  LTR_CUDA_TRY(launch_pdl(desc_tiles_kernel, dim3(da.tmax[0] * 4, n_images, 1), dim3(256), 0, s, da));
+  return LTR_OK;
+}
+
+static const char* check_match_indexed(const LtrMatchInput* in, const LtrPairIndex* ix) {
+  if (in->cu0 == nullptr || in->cu1 == nullptr) return "ltr_match_indexed: cu0 and cu1 (image offsets of the pools) are required";
+  const bool seg = in->sub_off0 != nullptr || in->sub_off1 != nullptr;
+  if (seg && (!in->sub_off0 || !in->sub_off1 || !in->cuk0 || !in->cuk1))
+    return "ltr_match_indexed: keyline merging needs sub_off0/1 and cuk0/1";
+  if (!ix->img0 || !ix->img1 || !ix->out_off0 || !ix->out_off1) return "ltr_match_indexed: img0/1 and out_off0/1 are required";
+  if (in->max_n0 < 0 || in->max_n1 < 0 || ix->n_tiles0 < 0 || ix->n_tiles1 < 0 || ix->total_out0 < 0 || ix->total_out1 < 0)
+    return "ltr_match_indexed: negative count";
+  if (in->max_n0 > 0 && in->max_n1 > 0 && (!ix->tiles0 || !ix->tiles1 || !ix->tile_off0 || !ix->tile_off1))
+    return "ltr_match_indexed: tiles0/1 and tile_off0/1 (ltr_image_tiles) are required";
+  return nullptr;
+}
+
+int64_t ltr_match_indexed_workspace_bytes(const LtrMatchInput* in, const LtrPairIndex* idx) {
+  if (!in || !idx) return set_error(LTR_E_INVALID, "ltr_match_indexed_workspace_bytes: null argument");
+  if (const char* e = check_match_indexed(in, idx)) return set_error(LTR_E_INVALID, e);
+  if (in->n_pairs <= 0) return 0;
+  return plan_match_indexed(*in, *idx, nullptr).bytes + 1024;
+}
+
+int ltr_match_indexed(const LtrMatchInput* in, const LtrPairIndex* idx, const LtrMatchOutput* out, int32_t device, void* stream) {
+  if (!in || !idx || !out) return set_error(LTR_E_INVALID, "ltr_match_indexed: null argument");
+  if (in->d != MT_D || in->dist_mode != 0)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_match_indexed: needs d == 256 and dist_mode 0");
+  if (out->gather && out->gather->world > 1) return set_error(LTR_E_UNSUPPORTED, "ltr_match_indexed: gather is not supported");
+  if (in->n_pairs <= 0) return LTR_OK;
+  if (const char* e = check_match_indexed(in, idx)) return set_error(LTR_E_INVALID, e);
+  const bool seg = in->sub_off0 != nullptr;
+  const bool want_nn = out->matches0 != nullptr;
+  if (want_nn && (!out->scores0 || !out->nn1 || !out->counts))
+    return set_error(LTR_E_INVALID, "ltr_match_indexed: matches0 needs scores0, nn1 and counts");
+  if (!want_nn && !out->dist_key) return set_error(LTR_E_INVALID, "ltr_match_indexed: nothing to compute (matches0 and dist_key are NULL)");
+  if (seg && (!out->dist_sub || !out->dist_key)) return set_error(LTR_E_INVALID, "ltr_match_indexed: keyline merging needs dist_sub and dist_key");
+  const int mx0 = in->max_n0, mx1 = in->max_n1;
+  const int mk0 = seg ? in->max_k0 : mx0, mk1 = seg ? in->max_k1 : mx1;
+  const long long stride_key = in->dist_pair_stride > 0 ? in->dist_pair_stride : (long long)mk0 * mk1;
+  if (mx0 > 0 && mx1 > 0 && (!in->desc0 || !in->desc1)) return set_error(LTR_E_INVALID, "ltr_match_indexed: null descriptors");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(out->workspace), 1024));
+  MatchPlan pl = plan_match_indexed(*in, *idx, base);
+  if (!out->workspace || (base - (char*)out->workspace) + pl.bytes > out->workspace_bytes)
+    return set_error(LTR_E_WORKSPACE, "ltr_match_indexed: workspace too small, need " + std::to_string(pl.bytes + 1024));
+  LTR_TRY(run_match_tc(*in, *out, pl, seg, stride_key, s, idx));
+  if (!seg) return LTR_OK;
+  if (mx0 > 0 && mx1 > 0 && mk0 > 0 && mk1 > 0) {
+    SegMeanArgs sa{out->dist_sub, (long long)mx0 * mx1, out->dist_key, stride_key, in->cuk0, in->cuk1, in->sub_off0, in->sub_off1,
+                   idx->img0, idx->img1};
+    LaunchScope ls(KC_SEGMEAN, s);
+    segmean_kernel<<<dim3(cdiv(mk1, 32), cdiv(mk0, 8), in->n_pairs), 256, 0, s>>>(sa);
+    LTR_CUDA_TRY(cudaGetLastError());
+  }
+  if (!want_nn) return LTR_OK;
+  // the per-pair output offsets play the role cuk0/cuk1 play in ltr_match: the NN kernels need no indirection
+  NNArgs na{};
+  na.dist = out->dist_key; na.stride = stride_key;
+  na.cuk0 = idx->out_off0; na.cuk1 = idx->out_off1;
+  na.thr = in->nn_thresh; na.mutual = in->mutual;
   na.matches0 = out->matches0; na.scores0 = out->scores0; na.nn1 = out->nn1; na.counts = out->counts;
   return run_nn(na, in->n_pairs, mk0, mk1, s);
 }

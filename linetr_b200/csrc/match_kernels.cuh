@@ -96,12 +96,15 @@ struct SegMeanArgs {
   float* dist_key; long long stride_key;
   const int* cuk0; const int* cuk1;        // [n_pairs+1]
   const int* sub_off0; const int* sub_off1;  // [total keylines + 1]
+  const int* img0; const int* img1;        // image pools: image of every pair's side [n_pairs], cuk over images;
+                                           // nullptr: pair p is image p
 };
 
 __global__ void __launch_bounds__(256) segmean_kernel(SegMeanArgs p) {
   const int pair = blockIdx.z;
-  const int kb0 = p.cuk0[pair], K0 = p.cuk0[pair + 1] - kb0;
-  const int kb1 = p.cuk1[pair], K1 = p.cuk1[pair + 1] - kb1;
+  const int im0 = p.img0 ? p.img0[pair] : pair, im1 = p.img1 ? p.img1[pair] : pair;
+  const int kb0 = p.cuk0[im0], K0 = p.cuk0[im0 + 1] - kb0;
+  const int kb1 = p.cuk1[im1], K1 = p.cuk1[im1 + 1] - kb1;
   const int sb0 = p.sub_off0[kb0], sb1 = p.sub_off1[kb1];
   const int N1 = p.sub_off1[kb1 + K1] - sb1;
   const int b = blockIdx.x * 32 + (threadIdx.x & 31);

@@ -47,14 +47,18 @@ static_assert(MT_SMEM <= 232448, "match_tc: shared memory budget");
 // One side of a batch of pairs.
 struct MatchSide {
   ActImg img;            // descriptor tile image (kblocks = 4)
-  const int* cu;         // [n_pairs + 1] line offsets or nullptr (uniform n)
+  const int* cu;         // [n_pairs + 1] line offsets or nullptr (uniform n); indexed: [n_images + 1] of the pool
   int n;                 // lines per pair when cu == nullptr
   int tile_mode;         // 0: pair p starts at tile p * tmax (pair-aligned scratch tiles)
                          // 1: pair p starts at tile (tile_row0 + first line of p) / 128 (encoder image, aligned pairs)
+                         // 2: pair p starts at tile tile_off[pimg[p]] (image-aligned pool, ltr_image_tiles)
   int tile_row0;         // mode 1: row of this side's first line inside the image
   int tmax;              // row tiles per pair (grid sizing; tile stride in mode 0)
   const float* sq;       // mode-1 distance only: squared norms, indexed like the lines (cu / p * n)
-  uint2* slot;           // out: per line {bits(best distance), best index | ambiguous << 31}
+  uint2* slot;           // out: per line {bits(best distance), best index | ambiguous << 31}; nullptr = not needed
+  const int* pimg;       // indexed: image of every pair [n_pairs] (nullptr: pair p is image p)
+  const int* tile_off;   // mode 2: first tile of every image [n_images + 1]
+  const int* out_off;    // indexed: first slot of every pair [n_pairs + 1] (one image line takes part in many pairs)
 };
 
 struct MatchTcArgs {
@@ -67,9 +71,11 @@ struct MatchTcArgs {
   int n_pairs;
 };
 
-__device__ __forceinline__ void side_range(const MatchSide& s, int pair, int& b, int& e) { image_range(s.cu, s.n, pair, b, e); }
-__device__ __forceinline__ int side_tile0(const MatchSide& s, int pair, int b) {
-  return s.tile_mode ? (s.tile_row0 + b) >> 7 : pair * s.tmax;
+// image of a pair's side: itself unless the side indexes an image pool
+__device__ __forceinline__ int side_image(const MatchSide& s, int pair) { return s.pimg ? s.pimg[pair] : pair; }
+__device__ __forceinline__ void side_range(const MatchSide& s, int im, int& b, int& e) { image_range(s.cu, s.n, im, b, e); }
+__device__ __forceinline__ int side_tile0(const MatchSide& s, int pair, int im, int b) {
+  return s.tile_mode == 2 ? s.tile_off[im] : s.tile_mode ? (s.tile_row0 + b) >> 7 : pair * s.tmax;
 }
 
 __device__ __forceinline__ void mt_epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
@@ -106,9 +112,10 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
   __syncthreads();
   pdl_wait();   // descriptors / tile images of the producing kernel are complete from here on
 
+  const int ia = side_image(SA, pair), ib = side_image(SB, pair);
   int ba, ea, bb, eb;
-  side_range(SA, pair, ba, ea);
-  side_range(SB, pair, bb, eb);
+  side_range(SA, ia, ba, ea);
+  side_range(SB, ib, bb, eb);
   const int na = ea - ba, nb = eb - bb;
   if (p.counts && blockIdx.x == 0 && tid == 0) p.counts[pair] = 0;
   if (p.done && blockIdx.x == 0 && pair == 0 && tid == 0) *p.done = 0;
@@ -118,14 +125,14 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
   if (warp == 8) {
     // ---------------------------------------------------------------- TMA producer
     if (lane == 0 && active) {
-      const size_t ta = (size_t)(side_tile0(SA, pair, ba) + rb) * MT_KB;
+      const size_t ta = (size_t)(side_tile0(SA, pair, ia, ba) + rb) * MT_KB;
       ptx::mbar_arrive_expect_tx(a_full, MT_A_BYTES);
 #pragma unroll
       for (int kb = 0; kb < MT_KB; ++kb) {
         ptx::bulk_g2s(smem + kb * 2 * MT_TILE, SA.img.hi + (ta + kb) * IMG_TILE_ELEMS, MT_TILE, a_full);
         ptx::bulk_g2s(smem + kb * 2 * MT_TILE + MT_TILE, SA.img.lo + (ta + kb) * IMG_TILE_ELEMS, MT_TILE, a_full);
       }
-      const size_t tb0 = (size_t)side_tile0(SB, pair, bb) * MT_KB;
+      const size_t tb0 = (size_t)side_tile0(SB, pair, ib, bb) * MT_KB;
       uint32_t it = 0;
       for (int ct = 0; ct < n_ct; ++ct)
         for (int kb = 0; kb < MT_KB; ++kb, ++it) {
@@ -260,18 +267,23 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
       if (ob < best || (ob == best && oi < bidx)) { second = fminf(best, os); best = ob; bidx = oi; }
       else second = fminf(second, ob);
       const bool amb = !(second - best >= MATCH_EPS);   // also true for NaN
-      SA.slot[ba + row] = make_uint2(__float_as_uint(best), (uint32_t)bidx | (amb ? 0x80000000u : 0u));
+      if (SA.slot) {
+        const int sbase = SA.pimg ? SA.out_off[pair] : ba;   // slots are per (pair, line) when images are shared
+        SA.slot[sbase + row] = make_uint2(__float_as_uint(best), (uint32_t)bidx | (amb ? 0x80000000u : 0u));
+      }
     }
   }
 }
 
-// ---------------------------------------------------------------- fp32 descriptors -> pair-aligned tile images
+// ---------------------------------------------------------------- fp32 descriptors -> pair- or image-aligned tile images
 struct DescTilesArgs {
   const float* d[2];     // fp32 descriptors of side 0 / 1
   int layout;            // 0 rows [n, 256] per line; 1 channel-first [256, n_p] per pair (pair p at 256 * first line)
   const int* cu[2]; int n[2];
   ActImg img[2]; int tmax[2];
   float* sq[2];          // optional squared norms per line (distance mode 1) or nullptr
+  const int* tile_off[2];  // image-aligned pool (ltr_image_tiles): "pair" p is image p, its ceil(n_p / 128) tiles
+                           // start at tile_off[p]; nullptr: pair-aligned, pair p at tile p * tmax
 };
 
 // grid = (max(tmax0, tmax1) * 4, n_pairs, 2): block = 32 lines of one tile; 256 threads.
@@ -285,10 +297,11 @@ __global__ void __launch_bounds__(256) desc_tiles_kernel(DescTilesArgs p) {
   int b, e;
   image_range(p.cu[side], p.n[side], pair, b, e);
   const int n = e - b;
+  if (p.tile_off[side] && tile * 128 >= n) return;   // an image owns only the tiles its lines need
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float* __restrict__ src = p.d[side];
   const ActImg& img = p.img[side];
-  const size_t t0 = ((size_t)pair * p.tmax[side] + tile) * MT_KB;
+  const size_t t0 = ((p.tile_off[side] ? (size_t)p.tile_off[side][pair] : (size_t)pair * p.tmax[side]) + tile) * MT_KB;
   uint8_t* hi = reinterpret_cast<uint8_t*>(img.hi);
   uint8_t* lo = reinterpret_cast<uint8_t*>(img.lo);
   if (p.layout == 0) {
@@ -357,6 +370,9 @@ struct MatchTailArgs {
   float thr; int mutual;
   int* matches0; float* scores0; int* nn1; int* counts;
   int max0;                        // max lines of side 0 per pair (row part of the grid)
+  // indexed mode (image pools): cu[s] are image offsets, pimg[s][pair] the image of a pair's side, and slots /
+  // outputs of the pair start at out_off[s][pair]; nullptr: pair p is image p and its outputs start at cu[s][p]
+  const int* pimg[2]; const int* out_off[2];
   // multi-GPU publication of `counts` (LtrPeerGather): symmetric buffer = counts[SLOTS][world][n_pairs] | flags[SLOTS][world]
   int* done;                       // block counter for last-block detection
   int* mc_base; int* const* peer_bases;
@@ -421,16 +437,17 @@ __device__ __forceinline__ void exact_row(const MatchTailArgs& p, int sa, int pa
 }
 
 // One decision (warp-cooperative; used for the lines whose slots are flagged ambiguous): side-0 line i ->
-// matches0 / scores0 (returns keep), or side-1 line j -> nn1.
-__device__ __forceinline__ bool tail_decide_row(const MatchTailArgs& p, int i, int b0, int n0, int b1, int n1, float* xrow, int lane,
-                                                bool force_exact) {
-  const uint2 s = p.slot[0][b0 + i];
+// matches0 / scores0 (returns keep), or side-1 line j -> nn1.  b0 / b1: first descriptor row of each side,
+// o0 / o1: first slot / output of each side (equal unless images are shared between pairs).
+__device__ __forceinline__ bool tail_decide_row(const MatchTailArgs& p, int i, int b0, int o0, int n0, int b1, int o1, int n1,
+                                                float* xrow, int lane, bool force_exact) {
+  const uint2 s = p.slot[0][o0 + i];
   float v = __uint_as_float(s.x);
   int idx = (int)(s.y & 0x7fffffffu);
   if (force_exact || (s.y >> 31) || !(fabsf(v - p.thr) >= MATCH_EPS)) exact_row(p, 0, b0, n0, i, b1, n1, xrow, lane, v, idx);
   bool keep = v < p.thr;   // strict '<' (nn_matcher.py:18)
   if (keep && p.mutual) {
-    const uint2 t = p.slot[1][b1 + idx];
+    const uint2 t = p.slot[1][o1 + idx];
     int back = (int)(t.y & 0x7fffffffu);
     if (t.y >> 31) {
       float bv;
@@ -439,8 +456,8 @@ __device__ __forceinline__ bool tail_decide_row(const MatchTailArgs& p, int i, i
     keep = back == i;
   }
   if (lane == 0) {
-    p.matches0[b0 + i] = keep ? idx : -1;
-    p.scores0[b0 + i] = v;
+    p.matches0[o0 + i] = keep ? idx : -1;
+    p.scores0[o0 + i] = v;
   }
   return keep;
 }
@@ -458,9 +475,10 @@ __global__ void __launch_bounds__(256) match_tail_kernel(MatchTailArgs p) {
   pdl_wait();
   const int pair = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   int b0, e0, b1, e1;
-  image_range(p.cu[0], p.n[0], pair, b0, e0);
-  image_range(p.cu[1], p.n[1], pair, b1, e1);
+  image_range(p.cu[0], p.n[0], p.pimg[0] ? p.pimg[0][pair] : pair, b0, e0);
+  image_range(p.cu[1], p.n[1], p.pimg[1] ? p.pimg[1][pair] : pair, b1, e1);
   const int n0 = e0 - b0, n1 = e1 - b1;
+  const int o0 = p.out_off[0] ? p.out_off[0][pair] : b0, o1 = p.out_off[1] ? p.out_off[1][pair] : b1;
   if (tid == 0) { n_work = 0; n_keep = 0; }
   __syncthreads();
   const int w = blockIdx.x * 256 + tid;
@@ -469,33 +487,33 @@ __global__ void __launch_bounds__(256) match_tail_kernel(MatchTailArgs p) {
     const int i = w;
     if (i < n0) {
       if (n1 == 0) {
-        p.matches0[b0 + i] = -1;
-        p.scores0[b0 + i] = INFINITY;
+        p.matches0[o0 + i] = -1;
+        p.scores0[o0 + i] = INFINITY;
       } else {
-        const uint2 s = p.slot[0][b0 + i];
+        const uint2 s = p.slot[0][o0 + i];
         const float v = __uint_as_float(s.x);
         const int idx = (int)(s.y & 0x7fffffffu);
         bool hard = (s.y >> 31) || !(fabsf(v - p.thr) >= MATCH_EPS);
         if (!hard) {
           keep = v < p.thr;
           if (keep && p.mutual) {
-            const uint2 t = p.slot[1][b1 + idx];
+            const uint2 t = p.slot[1][o1 + idx];
             if (t.y >> 31) { hard = true; keep = false; }
             else keep = (int)(t.y & 0x7fffffffu) == i;
           }
         }
         if (hard) work[atomicAdd(&n_work, 1)] = w;
-        else { p.matches0[b0 + i] = keep ? idx : -1; p.scores0[b0 + i] = v; }
+        else { p.matches0[o0 + i] = keep ? idx : -1; p.scores0[o0 + i] = v; }
       }
     }
   } else if (p.mutual) {
     const int j = w - p.max0;
     if (j < n1) {
-      if (n0 == 0) p.nn1[b1 + j] = -1;
+      if (n0 == 0) p.nn1[o1 + j] = -1;
       else {
-        const uint2 t = p.slot[1][b1 + j];
+        const uint2 t = p.slot[1][o1 + j];
         if (t.y >> 31) work[atomicAdd(&n_work, 1)] = w;
-        else p.nn1[b1 + j] = (int)(t.y & 0x7fffffffu);
+        else p.nn1[o1 + j] = (int)(t.y & 0x7fffffffu);
       }
     }
   }
@@ -505,12 +523,12 @@ __global__ void __launch_bounds__(256) match_tail_kernel(MatchTailArgs p) {
   for (int e = warp; e < n_work; e += 8) {     // exact path, one work item per warp at a time
     const int ww = work[e];
     if (ww < p.max0) {
-      if (tail_decide_row(p, ww, b0, n0, b1, n1, xrows[warp], lane, false) && lane == 0) atomicAdd(&n_keep, 1);
+      if (tail_decide_row(p, ww, b0, o0, n0, b1, o1, n1, xrows[warp], lane, false) && lane == 0) atomicAdd(&n_keep, 1);
     } else {
       const int j = ww - p.max0;
       float bv; int back;
       exact_row(p, 1, b1, n1, j, b0, n0, xrows[warp], lane, bv, back);
-      if (lane == 0) p.nn1[b1 + j] = back;
+      if (lane == 0) p.nn1[o1 + j] = back;
     }
   }
   __syncthreads();

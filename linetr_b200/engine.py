@@ -215,6 +215,90 @@ class ImagePairMatches:
                 "matching_scores_p": torch.from_numpy(_dense_scores(self.dist_p, self.stride_p, p, N0, N1))}
 
 
+@dataclass
+class ImageSet:
+    """Images encoded once (`PairEngine.encode_images`) for any number of `PairEngine.match_sets` calls.
+
+    desc_l [R,256] unit line descriptors (rows; image i owns sublines [cu_lines[i], cu_lines[i+1])), tiles_l their
+    image-aligned tile image (image i from tile tile_off_l[i]); the key-line CSR cuk [n+1] / sub_off [K+1] (global
+    subline numbering, the identity for images without split lines); desc_p the SuperPoint point descriptors of all
+    images, channel-first [256, N_i] blocks back to back (image i at 256 * cu_points[i]), tiles_p their tile image.
+    Host int32 offset arrays, their device copies in `dev`.  klines / keypoints: each image's tokenised key lines
+    (after the reference's in-place clip) and keypoints.  The tokenised token descriptors are not kept."""
+    desc_l: torch.Tensor
+    tiles_l: torch.Tensor
+    desc_p: torch.Tensor
+    tiles_p: torch.Tensor
+    cu_lines: np.ndarray
+    cuk: np.ndarray
+    sub_off: np.ndarray
+    tile_off_l: np.ndarray
+    cu_points: np.ndarray
+    tile_off_p: np.ndarray
+    dev: dict
+    klines: List[np.ndarray]
+    keypoints: list
+    device: torch.device
+
+    def __len__(self) -> int:
+        return len(self.cu_lines) - 1
+
+
+# Cap on the subline distance scratch of one line match with key-line merging (n_pairs * max_n0 * max_n1 fp32):
+# match_sets cuts longer pair lists into consecutive chunks that stay under it.
+DIST_SUB_CAP = 512 << 20
+# Pairs per matcher launch: the pair index is the grid's y dimension.
+MAX_PAIRS_PER_CALL = 65535
+
+
+def exhaustive_pairs(n: int) -> np.ndarray:
+    """All pairs (i, j) with i < j of n images, row-major order: int32 [n(n-1)/2, 2]."""
+    i, j = np.triu_indices(int(n), k=1)
+    return np.ascontiguousarray(np.stack([i, j], 1), dtype=np.int32).reshape(-1, 2)
+
+
+def check_pairs(pairs, n0: int, n1: int) -> np.ndarray:
+    """A host pair list [P, 2] of image indices, column 0 into a set of n0 images and column 1 into one of n1 ->
+    int32 [P, 2]; raises LtrError on a wrong shape or dtype or an index out of range."""
+    if isinstance(pairs, torch.Tensor):
+        if pairs.is_cuda:
+            raise N.LtrError("match_sets: pairs must be a host array")
+        pairs = pairs.numpy()
+    a = np.asarray(pairs)
+    if a.ndim == 1 and a.size == 0:   # an empty list
+        a = a.reshape(0, 2)
+    if a.ndim != 2 or a.shape[1] != 2:
+        raise N.LtrError(f"match_sets: pairs must have shape [P, 2], got {list(a.shape)}")
+    if a.size == 0:
+        return np.zeros((0, 2), dtype=np.int32)
+    if not np.issubdtype(a.dtype, np.integer):
+        raise N.LtrError(f"match_sets: pairs must be integers, got {a.dtype}")
+    if (a < 0).any():
+        raise N.LtrError("match_sets: negative image index in pairs")
+    if (a[:, 0] >= n0).any():
+        raise N.LtrError(f"match_sets: pairs[:, 0] out of range for a set of {n0} images")
+    if (a[:, 1] >= n1).any():
+        raise N.LtrError(f"match_sets: pairs[:, 1] out of range for a set of {n1} images")
+    return np.ascontiguousarray(a, dtype=np.int32)
+
+
+def plan_chunks(n0, n1, cap_bytes: Optional[int] = None, max_pairs: int = MAX_PAIRS_PER_CALL):
+    """Consecutive chunks [(begin, end)] of a pair list with per-pair subline counts n0 / n1 such that each chunk's
+    distance scratch, len * max n0 * max n1 * 4 bytes, stays within cap_bytes (default DIST_SUB_CAP) and a chunk
+    holds at most max_pairs pairs.  A pair that alone exceeds the cap gets a chunk of its own."""
+    cap = DIST_SUB_CAP if cap_bytes is None else int(cap_bytes)
+    chunks, a, m0, m1 = [], 0, 0, 0
+    for p in range(len(n0)):
+        c0, c1 = max(m0, int(n0[p])), max(m1, int(n1[p]))
+        if p > a and ((p - a + 1) * c0 * c1 * 4 > cap or p - a >= max_pairs):
+            chunks.append((a, p))
+            a, c0, c1 = p, int(n0[p]), int(n1[p])
+        m0, m1 = c0, c1
+    if len(n0):
+        chunks.append((a, len(n0)))
+    return chunks
+
+
 class PairEngine:
     """Batched line-descriptor forward + mutual-NN matching on one GPU."""
 
@@ -487,6 +571,100 @@ class PairEngine:
         return ImagePairMatches(*lines[:3], i32(cuk[:P + 1]), *points[:3], i32(cup[:P + 1]),
                                 host.klines[:P], host.klines[P:], kp[:P], kp[P:],
                                 lines[3], lines[4], points[3], points[4])
+
+    # ------------------------------------------------------------------ image sets: encode once, match many pairs
+    def encode_images(self, images: Sequence[dict], auto_min_length: bool = True) -> ImageSet:
+        """Encode each image once for later `match_sets` calls (image dicts as for `match_images`): one
+        `ltr_tokenize_batch`, one `ltr_encode`, one `ltr_image_tiles` for the line descriptors and one for the
+        SuperPoint point descriptors (concatenated channel-first into one pool).  All index arrays go up in one
+        pinned copy; the call never waits for the device."""
+        specs, cfgs = self._image_specs(images, auto_min_length)
+        host = LP.prepare_tokenizer_batch(specs, cfgs)
+        kp = [_first(im["keypoints"]) for im in images]
+        dp = [_first(im["descriptors"]) for im in images]
+        cup = np.zeros(len(images) + 1, dtype=np.int64)
+        cup[1:] = np.cumsum([int(d.shape[1]) for d in dp])
+        i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
+        cu, cup = i32(host.cu_lines), i32(cup)
+        to_l, to_p = _ops.tile_offsets(cu), _ops.tile_offsets(cup)
+        arrays = self._tok_arrays(host)
+        arrays.update(cuk=i32(host.cuk), tile_off_l=to_l, cu_points=cup, tile_off_p=to_p)
+        dv = self._stage(arrays)
+        batch = self._tokenize(host, images, dv)
+        rows = self.encode(batch)
+        tiles_l = _ops.image_tiles(rows, N.LAYOUT_ROWS, cu, dv["cu_lines"], dv["tile_off_l"], int(to_l[-1]))
+        pool = (torch.cat([d.float().contiguous().reshape(-1) for d in dp]) if dp
+                else torch.empty(0, dtype=torch.float32, device=self.device))
+        tiles_p = _ops.image_tiles(pool, N.LAYOUT_CHANNEL_FIRST, cup, dv["cu_points"], dv["tile_off_p"], int(to_p[-1]))
+        dev = {k: dv[k] for k in ("cu_lines", "cuk", "tile_off_l", "cu_points", "tile_off_p")}
+        dev["sub_off"] = dv["sub0"]
+        return ImageSet(rows, tiles_l, pool, tiles_p, cu, i32(host.cuk), i32(host.sub0), to_l, cup, to_p, dev,
+                        list(host.klines), kp, self.device)
+
+    def match_set(self, images: ImageSet, pairs, **kw) -> ImagePairMatches:
+        """`match_sets(images, images, pairs, ...)`: pairs of images of one set."""
+        return self.match_sets(images, images, pairs, **kw)
+
+    def match_sets(self, set0: ImageSet, set1: ImageSet, pairs, line_thresh: Optional[float] = None,
+                   point_thresh: float = 0.7, want_scores: bool = False) -> ImagePairMatches:
+        """Line and point matches of a list of image pairs between two encoded sets: pair p = (i, j) is image i of
+        set0 against image j of set1 (pairs: host integer array [P, 2], validated before any device work).  The
+        result equals `match_images` over the same pairs, images passed again per pair.  One indexed line match
+        and one indexed point match per chunk of pairs (see `plan_chunks`; with key-line merging a chunk's subline
+        distance scratch stays under DIST_SUB_CAP); the call never waits for the device."""
+        pr = check_pairs(pairs, len(set0), len(set1))
+        for s in (set0, set1):
+            if s.device != self.device:
+                raise N.LtrError(f"match_sets: image set on {s.device}, engine on {self.device}")
+        if line_thresh is None:
+            line_thresh = self.model.config.get("nn_threshold", 0.8)
+        P = len(pr)
+        i0, i1 = pr[:, 0], pr[:, 1]
+        cnt = lambda a, i: np.diff(np.asarray(a, dtype=np.int64))[i]
+        n0, n1 = cnt(set0.cu_lines, i0), cnt(set1.cu_lines, i1)      # sublines
+        k0, k1 = cnt(set0.cuk, i0), cnt(set1.cuk, i1)                # key lines
+        q0, q1 = cnt(set0.cu_points, i0), cnt(set1.cu_points, i1)    # keypoints
+        # key-line merging exactly when match_images would merge these pairs: some image has a split key line
+        merge = bool((n0 != k0).any() or (n1 != k1).any())
+        pref = lambda c: np.concatenate([[0], np.cumsum(c)]).astype(np.int32)
+        ol0, ol1, op0, op1 = pref(k0), pref(k1), pref(q0), pref(q1)
+        dv = self._stage({"img0": pr[:, 0].copy(), "img1": pr[:, 1].copy(), "ol0": ol0, "ol1": ol1, "op0": op0, "op1": op1})
+        i32d = dict(dtype=torch.int32, device=self.device)
+        f32d = dict(dtype=torch.float32, device=self.device)
+        alloc = lambda n, kw: torch.empty(max(int(n), 1), **kw)[:int(n)]   # never a null pointer
+        mx = lambda a: int(a.max(initial=0))
+        ml, sl, nl, cl = alloc(ol0[-1], i32d), alloc(ol0[-1], f32d), alloc(ol1[-1], i32d), alloc(P, i32d)
+        mp, spp, npp, cp = alloc(op0[-1], i32d), alloc(op0[-1], f32d), alloc(op1[-1], i32d), alloc(P, i32d)
+        stride_l = mx(k0) * mx(k1) if want_scores else 0
+        stride_p = mx(q0) * mx(q1) if want_scores else 0
+        dist_l = alloc(P * stride_l, f32d) if want_scores else None
+        dist_p = alloc(P * stride_p, f32d) if want_scores else None
+        zero = np.zeros(P, dtype=np.int64)
+        for a, b in plan_chunks(n0 if merge else zero, n1 if merge else zero):
+            def pools(cu, tiles, tile_off):   # the two image pools (lines or points) and this chunk's pairs
+                return dict(cu0=set0.dev[cu], cu1=set1.dev[cu], tiles0=getattr(set0, tiles), tiles1=getattr(set1, tiles),
+                            tile_off0=set0.dev[tile_off], tile_off1=set1.dev[tile_off],
+                            n_tiles0=int(getattr(set0, tile_off)[-1]), n_tiles1=int(getattr(set1, tile_off)[-1]),
+                            img0=dv["img0"][a:b], img1=dv["img1"][a:b])
+            kw = pools("cu_lines", "tiles_l", "tile_off_l")
+            kw.update(max_n0=mx(n0[a:b]), max_n1=mx(n1[a:b]), out_off0=dv["ol0"][a:b + 1], out_off1=dv["ol1"][a:b + 1],
+                      total_out0=int(ol0[-1]), total_out1=int(ol1[-1]), matches0=ml, scores0=sl, nn1=nl, counts=cl[a:b])
+            if want_scores:
+                kw.update(dist_key=dist_l[a * stride_l:], dist_stride=stride_l)
+            if merge:
+                kw.update(sub_off0=set0.dev["sub_off"], sub_off1=set1.dev["sub_off"], cuk0=set0.dev["cuk"],
+                          cuk1=set1.dev["cuk"], max_k0=mx(k0[a:b]), max_k1=mx(k1[a:b]))
+            _ops.match_indexed(set0.desc_l, set1.desc_l, N.LAYOUT_ROWS, b - a, float(line_thresh), **kw)
+            kw = pools("cu_points", "tiles_p", "tile_off_p")
+            kw.update(max_n0=mx(q0[a:b]), max_n1=mx(q1[a:b]), out_off0=dv["op0"][a:b + 1], out_off1=dv["op1"][a:b + 1],
+                      total_out0=int(op0[-1]), total_out1=int(op1[-1]), matches0=mp, scores0=spp, nn1=npp, counts=cp[a:b])
+            if want_scores:
+                kw.update(dist_key=dist_p[a * stride_p:], dist_stride=stride_p)
+            _ops.match_indexed(set0.desc_p, set1.desc_p, N.LAYOUT_CHANNEL_FIRST, b - a, float(point_thresh), **kw)
+        return ImagePairMatches(ml, sl, cl, ol0, mp, spp, cp, op0,
+                                [set0.klines[i] for i in i0], [set1.klines[j] for j in i1],
+                                [set0.keypoints[i] for i in i0], [set1.keypoints[j] for j in i1],
+                                dist_l, stride_l, dist_p, stride_p)
 
     def match_packed_host(self, host: LineBatch, n_pairs: int, nn_thresh: Optional[float] = None, mutual=True,
                           n_chunks: int = 4):

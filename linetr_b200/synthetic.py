@@ -227,6 +227,37 @@ def make_image_pair(seed: int, n_lines: int, n_points: int, w: int = 640, h: int
     return image(ends0, kp0, d0, dense0, score0), image(ends1, kp1, d1, dense1, score1)
 
 
+def make_image_set(seed: int, n_views: int, n_lines: int, n_points: int, w: int = 640, h: int = 480,
+                   jitter_px: float = 0.5, map_noise: float = 0.05):
+    """n_views synthetic views of one scene (image dicts as `make_image_pair` returns): every view is a jittered copy of
+    the scene's key lines, keypoints, dense maps and point descriptors, made the way `make_image_pair` makes its
+    second image, so every pair of views has true line and point matches."""
+    import torch
+    rng = np.random.Generator(np.random.PCG64(seed))
+    x0, y0 = rng.uniform(8, w - 9, n_lines), rng.uniform(8, h - 9, n_lines)
+    ang, ln = rng.uniform(0, 2 * np.pi, n_lines), rng.uniform(20, 300, n_lines)
+    x1 = np.clip(x0 + ln * np.cos(ang), 8, w - 9)
+    y1 = np.clip(y0 + ln * np.sin(ang), 8, h - 9)
+    ends = np.stack([x0, y0, x1, y1], 1)
+    octave = rng.integers(0, 2, n_lines)
+    kp = np.stack([rng.uniform(0, w - 1, n_points), rng.uniform(0, h - 1, n_points)], 1).astype(np.float32)
+    desc = _unit(rng.standard_normal((n_points, D_MODEL)).astype(np.float32))
+    dense = rng.standard_normal((1, D_MODEL, h // 8, w // 8)).astype(np.float32)
+    score = rng.uniform(0, 1, (1, h, w)).astype(np.float32)
+    views = []
+    for _ in range(n_views):
+        e = np.clip(ends + rng.normal(0, jitter_px, ends.shape), 8, [w - 9, h - 9, w - 9, h - 9])
+        k = np.clip(kp + rng.normal(0, jitter_px, kp.shape), 0, [w - 1, h - 1]).astype(np.float32)
+        d = _unit(desc + map_noise * rng.standard_normal(desc.shape).astype(np.float32))
+        dn = torch.from_numpy(dense + map_noise * rng.standard_normal(dense.shape).astype(np.float32))
+        s = np.clip(score + map_noise * rng.standard_normal(score.shape), 0, 1).astype(np.float32)
+        views.append({"klines": [SyntheticKeyLine(*x, o) for x, o in zip(e, octave)], "image_shape": (1, 1, h, w),
+                      "keypoints": torch.from_numpy(k), "scores": torch.from_numpy(s.reshape(-1)[:len(k)].copy()),
+                      "descriptors": torch.from_numpy(np.ascontiguousarray(d.T)),
+                      "dense_descriptor": torch.nn.functional.normalize(dn, dim=1), "dense_score": torch.from_numpy(s)})
+    return views
+
+
 def image_to(im: dict, device) -> dict:
     """Tensors of an image dict moved to `device` (klines and shapes untouched)."""
     import torch
