@@ -16,6 +16,11 @@ extern "C" {
 float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t out_mode, int32_t iters,
                      int32_t device);
 
+/* One signature layer's row-local GEMMs (mlp1 ReLU -> mlp2 + x -> qkv) at m rows, zero-filled operands:
+ * average device milliseconds per layer as one chained launch (chained != 0) or three launches.
+ * -1 on failure. */
+float ltr_gemm_chain_bench(int32_t m, int32_t chained, int32_t iters, int32_t device);
+
 /* clock64 stamps of CTA 0 recorded by the last ltr_gemm_bench call (64 slots, 16 per tile:
  * 0 MMA acc_empty ok, 1 first operands landed, 2 MMAs issued, 3 epilogue acc_full ok, 4 first
  * accumulator complete, 5 epilogue done, 6 producer slot free). */

@@ -27,7 +27,7 @@ EXPORTED_SYMBOLS = (
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
-DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
+DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
 ABI_VERSION = 3
 
 
@@ -182,6 +182,8 @@ def load():
     lib.ltr_linear_img_norm.restype = C.c_int
     lib.ltr_gemm_bench.argtypes = [C.c_int32] * 7
     lib.ltr_gemm_bench.restype = C.c_float
+    lib.ltr_gemm_chain_bench.argtypes = [C.c_int32] * 4
+    lib.ltr_gemm_chain_bench.restype = C.c_float
     lib.ltr_gemm_trace.restype = C.POINTER(C.c_uint64)
     lib.ltr_debug_trace_arm.argtypes = [C.c_int32]
     lib.ltr_debug_trace_arm.restype = None

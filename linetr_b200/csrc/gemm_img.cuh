@@ -222,6 +222,20 @@ struct GemmImgCfg {
 // barrier over the 8 consumer warps only (the producer warpgroup never joins it)
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
+// Chained GEMMs (gemm_chain_kernel): this warp has stored its part of one 64-column output k-block; order the stores
+// before the TMA reads of the next op (generic -> async proxy fence in every lane, then the warp's arrival on the
+// k-block's barrier, a release that the producer thread of the same CTA acquires before it issues the copy) and count
+// the warp (8 arrivals = the whole 128 x 64 block is written).  CTA scope is enough: writer and TMA issuer share the CTA.
+// A device-scope __threadfence() here cost ~4 % of a chained signature layer on H100 and is not needed.
+// The epilogues publish a chunk after the NEXT chunk's arithmetic, when its stores have long been issued.
+// `ready` == nullptr: no consumer, nothing to do.
+__device__ __forceinline__ void publish_kblock(uint64_t* ready, int kb, int lane) {
+  if (!ready) return;
+  ptx::fence_proxy_async_global();
+  __syncwarp();
+  if (lane == 0) ptx::mbar_arrive(&ready[kb]);
+}
+
 // Columns [64 chunk, 64 chunk + 64) of a consumer warpgroup's accumulator fragment (64 rows x N, see ptx::wg_*) ->
 // the eight 32 x 32 fp32 staging blocks of the tile (block 4 * column half + q holds rows 32 q .. 32 q + 31, chunk
 // columns 32 * column half ..; a row's float4 groups XOR-swizzled by row & 7, the layout epi_add_rows_f32 reads).
@@ -252,10 +266,11 @@ __device__ __forceinline__ void load_stage(const float* stg, int lane, float (&a
 
 // Row-normalising epilogue of one 128 x 256 tile (see GemmImgArgs::norm).  A row's 256 columns sit in two
 // threads (column halves of every 64-column chunk, different warps); partial sums are exchanged through `xch`.
-// The accumulator stays in registers and is staged again for every pass.
+// The accumulator stays in registers and is staged again for every pass.  ready: see publish_kblock.
 template <int NR>
 __device__ __forceinline__ void epi_norm_tile(const GemmImgArgs& p, const float (&d)[NR], int mt, int q, int half, int lane,
-                                              int row_a, float* stg_all, float* stg, uint8_t* stgb, float* xch) {
+                                              int row_a, float* stg_all, float* stg, uint8_t* stgb, float* xch,
+                                              uint64_t* ready = nullptr) {
   const int row0 = mt * 128 + q * 32, r_in = q * 32 + lane;
   auto chunk = [&](int ch, float (&v)[32]) {
     epi_bar();
@@ -333,16 +348,20 @@ __device__ __forceinline__ void epi_norm_tile(const GemmImgArgs& p, const float 
     }
     if (p.nadd) epi_add_rows_f32(p.nadd, p.ldadd, row0, c0, p.M, lane, stg, v);
     if (p.NaddImg.hi) epi_add_rows_img(p.NaddImg, p.nadd_kb0, mt, c0, q, row0, p.M, lane, stgb, v);
+    if (ch > 0) publish_kblock(ready, ch - 1, lane);   // one chunk late: its stores have drained by now
     if (p.C) epi_store_rows_f32(p.C, p.ldc, row0, c0, p.M, lane, stg, v);
     if (p.O.hi) epi_store_image(p.O, p.o_kb0, mt, c0, q, row0, p.M, lane, stgb, v);
   }
+  publish_kblock(ready, 3, lane);
 }
 
 // Plain epilogue of one 128 x BN tile: this warp's 32 rows x one half of every 64-column chunk:
 // bias -> activation -> residual (fp32 rows or split-bf16 image) -> fp32 rows and/or image output.
+// An in-place residual (Rimg == O, same k-blocks: mlp2's x += delta) is race-free: an element is read
+// (epi_add_rows_img) and written back (epi_store_image) by the same warp within the same chunk.
 template <int BN, int NR>
 __device__ __forceinline__ void epi_plain_tile(const GemmImgArgs& p, const float (&d)[NR], int mt, int nb, int q, int half, int lane,
-                                               int row_a, float* stg_all, float* stg, uint8_t* stgb) {
+                                               int row_a, float* stg_all, float* stg, uint8_t* stgb, uint64_t* ready = nullptr) {
   const int row0 = mt * 128 + q * 32;   // first row of this warp
 #pragma unroll 1
   for (int ch = 0; ch < BN / 64; ++ch) {
@@ -373,9 +392,11 @@ __device__ __forceinline__ void epi_plain_tile(const GemmImgArgs& p, const float
     }
     if (p.R) epi_add_rows_f32(p.R, p.ldr, row0, nbase, p.M, lane, stg, acc);
     if (p.Rimg.hi) epi_add_rows_img(p.Rimg, p.r_kb0, mt, nbase, q, row0, p.M, lane, stgb, acc);
+    if (ch > 0) publish_kblock(ready, nb * (BN / 64) + ch - 1, lane);   // one chunk late: its stores have drained by now
     if (p.C) epi_store_rows_f32(p.C, p.ldc, row0, nbase, p.M, lane, stg, acc);
     if (p.O.hi) epi_store_image(p.O, p.o_kb0, mt, nbase, q, row0, p.M, lane, stgb, acc);
   }
+  publish_kblock(ready, nb * (BN / 64) + BN / 64 - 1, lane);
 }
 
 // One k-block (64 deep) of a warpgroup's 64 x BN accumulator: three split products per K = 16 step
@@ -554,6 +575,189 @@ inline int launch_gemm_img(const GemmImgArgs& a, cudaStream_t s, int bn_hint = 0
   }
   if (bn == 256 && a.W.N % 256 == 0) return launch_gemm_img_bn<256>(a, s);
   return launch_gemm_img_bn<128>(a, s);
+}
+
+// ---------------------------------------------------------------- chained GEMMs (one launch, several row-local layers)
+// Layers whose every output row depends only on the same row of the previous layer's output run back to back in ONE
+// persistent launch: CTA b owns m-tiles b, b + grid, ... and walks through all n-blocks of op 0, then of op 1, ... for
+// each of them, with the main loop, epilogues and TMA / mbarrier ring of gemm_img_kernel<256> (same tile arithmetic, so
+// the results are bit-identical to one launch per op).  What a chain saves over separate launches: the ring fill, the
+// idle SMs of the last wave and the grid-wide wait at every op boundary.
+// Dependency between consecutive ops, inside the CTA: op o+1 reads A k-block kb of its m-tile (TMA) only after all 8
+// epilogue warps have stored - and fenced to the async proxy - output columns [64 kb, 64 kb + 64) of op o for that
+// m-tile (`kb_ready[kb]`, 8 arrivals; publish_kblock).  One barrier per k-block rather than per op lets the producer
+// load op o+1's first k-blocks while the epilogue still writes the later ones.  Each arrival phase of kb_ready[kb] is
+// waited for exactly once, in order: op o+1 reads exactly the k-blocks op o writes (gemm_chain_check), the last op of
+// the chain publishes nothing, and op o+1 cannot reach its epilogue (its next publication) before the producer has
+// loaded - so waited for - all its A k-blocks.  W tiles depend on nothing; the first ones are requested before
+// pdl_wait.  BN = 256 only.
+constexpr int CHAIN_MAX_OPS = 4;
+constexpr int CHAIN_MAX_KB = 16;   // output k-blocks of an op that feeds the next one (N <= 1024)
+struct GemmChainArgs {
+  GemmImgArgs op[CHAIN_MAX_OPS];
+  int n_ops, m_tiles;
+};
+
+__global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constant__ GemmChainArgs c) {
+  constexpr int BN = 256;
+  using Cfg = GemmImgCfg<BN>;
+  static_assert((2 * Cfg::STAGES + CHAIN_MAX_KB) * 8 <= Cfg::OFF_XCH - Cfg::OFF_BAR, "gemm_chain: barrier area");
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const uint32_t raw = ptx::smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
+  uint64_t* full = bars;
+  uint64_t* empty = bars + Cfg::STAGES;
+  uint64_t* kb_ready = bars + 2 * Cfg::STAGES;
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  pdl_launch_dependents();
+
+  if (tid == 0) {
+    for (int s = 0; s < Cfg::STAGES; ++s) {
+      ptx::mbar_init(&full[s], 1);
+      ptx::mbar_init(&empty[s], 8);
+    }
+    for (int k = 0; k < CHAIN_MAX_KB; ++k) ptx::mbar_init(&kb_ready[k], 8);
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ---------------------------------------------------------------- TMA producer
+    ptx::setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
+      // the first STAGES k-blocks of op 0 go to fresh slots: their W tiles are requested before pdl_wait
+      const int npre = (int)blockIdx.x < c.m_tiles ? min(Cfg::STAGES, c.op[0].W.K / 64) : 0;
+      for (int kb = 0; kb < npre; ++kb) {
+        const size_t woff = (size_t)kb * (c.op[0].W.N / 8) * 1024;
+        uint8_t* st = smem + kb * Cfg::STAGE;
+        ptx::mbar_arrive_expect_tx(&full[kb], Cfg::STAGE);
+        ptx::bulk_g2s(st + 2 * Cfg::A_TILE, reinterpret_cast<const uint8_t*>(c.op[0].W.hi) + woff, Cfg::W_TILE, &full[kb]);
+        ptx::bulk_g2s(st + 2 * Cfg::A_TILE + Cfg::W_TILE, reinterpret_cast<const uint8_t*>(c.op[0].W.lo) + woff, Cfg::W_TILE, &full[kb]);
+      }
+      pdl_wait();   // the previous kernel's outputs (op 0's A image, residuals, addends) are complete from here on
+      uint32_t it = 0, ph = 0;   // ph bit kb: parity of the next kb_ready[kb] phase to wait for
+      for (int mt = blockIdx.x; mt < c.m_tiles; mt += gridDim.x)
+        for (int o = 0; o < c.n_ops; ++o) {
+          const GemmImgArgs& p = c.op[o];
+          const int nk = p.W.K / 64;
+          const uint8_t* whi = reinterpret_cast<const uint8_t*>(p.W.hi);
+          const uint8_t* wlo = reinterpret_cast<const uint8_t*>(p.W.lo);
+          for (int nb = 0; nb < p.n_blks; ++nb)
+            for (int kb = 0; kb < nk; ++kb, ++it) {
+              const int s = it % Cfg::STAGES;
+              uint8_t* st = smem + s * Cfg::STAGE;
+              if (it >= (uint32_t)npre) {
+                ptx::mbar_wait(&empty[s], ((it / Cfg::STAGES) & 1) ^ 1);
+                const size_t woff = ((size_t)kb * (p.W.N / 8) + (size_t)nb * (BN / 8)) * 1024;
+                ptx::mbar_arrive_expect_tx(&full[s], Cfg::STAGE);
+                ptx::bulk_g2s(st + 2 * Cfg::A_TILE, whi + woff, Cfg::W_TILE, &full[s]);
+                ptx::bulk_g2s(st + 2 * Cfg::A_TILE + Cfg::W_TILE, wlo + woff, Cfg::W_TILE, &full[s]);
+              }
+              if (o > 0 && nb == 0) {   // A k-block kb = output k-block kb of op o-1 for this m-tile
+                ptx::mbar_wait(&kb_ready[kb], (ph >> kb) & 1);
+                ph ^= 1u << kb;
+              }
+              const size_t aoff = ((size_t)mt * p.A.kblocks + p.a_kb0 + kb) * IMG_TILE_ELEMS;
+              ptx::bulk_g2s(st, p.A.hi + aoff, Cfg::A_TILE, &full[s]);
+              ptx::bulk_g2s(st + Cfg::A_TILE, p.A.lo + aoff, Cfg::A_TILE, &full[s]);
+            }
+        }
+    }
+  } else {
+    // ---------------------------------------------------------------- consumers (2 warpgroups x 64 rows), as gemm_img_kernel
+    ptx::setmaxnreg_inc<232>();
+    pdl_wait();   // residual / addend images of op 0 may come from the previous kernel
+    const int wg = warp >> 2, q = warp & 3, half = warp >> 2;
+    const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    float* stg_all = reinterpret_cast<float*>(smem + Cfg::OFF_STG);
+    float* stg = stg_all + warp * (Cfg::STG_WARP / 4);
+    uint8_t* stgb = reinterpret_cast<uint8_t*>(stg);
+    float* xch = reinterpret_cast<float*>(smem + Cfg::OFF_XCH);
+    uint32_t it = 0;
+    for (int mt = blockIdx.x; mt < c.m_tiles; mt += gridDim.x)
+      for (int o = 0; o < c.n_ops; ++o) {
+        const GemmImgArgs& p = c.op[o];
+        const int nk = p.W.K / 64;
+        uint64_t* ready = o + 1 < c.n_ops ? kb_ready : nullptr;
+        for (int nb = 0; nb < p.n_blks; ++nb) {
+          float d[BN / 2];
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+          for (int kb = 0; kb < nk; ++kb, ++it) {
+            const int s = it % Cfg::STAGES;
+            ptx::mbar_wait(&full[s], (it / Cfg::STAGES) & 1);
+            const uint32_t a_hi = ptx::smem_u32(smem + s * Cfg::STAGE) + wg * 8192;
+            const uint32_t w_hi = ptx::smem_u32(smem + s * Cfg::STAGE + 2 * Cfg::A_TILE);
+            ptx::wg_fence_regs(d);
+            ptx::wg_fence();
+            mma_kblock<BN>(d, a_hi, a_hi + Cfg::A_TILE, w_hi, w_hi + Cfg::W_TILE, kb == 0);
+            ptx::wg_commit();
+            ptx::wg_wait<1>();
+            ptx::wg_fence_regs(d);
+            if (kb > 0 && lane == 0) ptx::mbar_arrive(&empty[(it - 1) % Cfg::STAGES]);
+          }
+          ptx::wg_wait<0>();
+          ptx::wg_fence_regs(d);
+          if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % Cfg::STAGES]);
+          if (p.norm != NORM_NONE)
+            epi_norm_tile(p, d, mt, q, half, lane, row_a, stg_all, stg, stgb, xch, ready);
+          else
+            epi_plain_tile<BN>(p, d, mt, nb, q, half, lane, row_a, stg_all, stg, stgb, ready);
+        }
+      }
+  }
+}
+
+// nullptr if ops[0 .. n_ops) can run as one gemm_chain_kernel launch, else why not.  Every op: BN = 256 tiles (N % 256),
+// a plain A operand (no block-diagonal slices), k-block ranges inside their images; op i > 0 must read exactly the
+// image k-blocks op i-1 writes (the row-local hand-over the kernel's dependencies are built on).
+inline const char* gemm_chain_check(const GemmImgArgs* ops, int n_ops) {
+  if (n_ops < 1 || n_ops > CHAIN_MAX_OPS) return "gemm_chain: 1..4 ops";
+  for (int i = 0; i < n_ops; ++i) {
+    const GemmImgArgs& a = ops[i];
+    if (a.M != ops[0].M || a.W.K <= 0 || a.W.K % 64 || a.W.N <= 0 || a.W.N % 256 || a.a_kb_nb || !a.A.hi ||
+        (a.C && a.ldc % 8) || (a.R && a.ldr % 4))
+      return "gemm_chain: ops need equal M, K % 64, N % 256, a plain A image, ldc % 8, ldr % 4";
+    if (a.a_kb0 < 0 || a.a_kb0 + a.W.K / 64 > a.A.kblocks || (a.O.hi && (a.o_kb0 < 0 || a.o_kb0 + a.W.N / 64 > a.O.kblocks)) ||
+        (a.Rimg.hi && (a.r_kb0 < 0 || a.r_kb0 + a.W.N / 64 > a.Rimg.kblocks)))
+      return "gemm_chain: a k-block range exceeds its image";
+    if ((a.R && a.Rimg.hi) || (a.nadd && a.NaddImg.hi))
+      return "gemm_chain: residual or addend given twice";
+    if (a.norm != NORM_NONE &&
+        (a.W.N != 256 || a.act != ACT_NONE || (a.nadd && a.ldadd % 4) || (a.norm == NORM_LAYER && (!a.ng || !a.nbeta)) ||
+         (a.NaddImg.hi && (a.nadd_kb0 < 0 || a.nadd_kb0 + 4 > a.NaddImg.kblocks))))
+      return "gemm_chain: the row-norm epilogue needs N == 256, no activation, ldadd % 4, LayerNorm parameters";
+    if (i == 0) continue;
+    const GemmImgArgs& prev = ops[i - 1];
+    if (!prev.O.hi || a.A.hi != prev.O.hi || a.A.lo != prev.O.lo || a.A.kblocks != prev.O.kblocks)
+      return "gemm_chain: op i must read the image op i-1 writes (row-local chain)";
+    if (a.a_kb0 != prev.o_kb0 || a.W.K != prev.W.N)
+      return "gemm_chain: op i must read exactly the k-blocks op i-1 writes";
+    if (prev.W.N / 64 > CHAIN_MAX_KB) return "gemm_chain: an op that feeds the next one may write at most 16 k-blocks";
+  }
+  return nullptr;
+}
+
+inline int launch_gemm_chain(const GemmImgArgs* ops, int n_ops, cudaStream_t s) {
+  if (const char* why = gemm_chain_check(ops, n_ops)) return set_error(-1, why);
+  if (ops[0].M <= 0) return 0;
+  GemmChainArgs c{};
+  c.n_ops = n_ops;
+  c.m_tiles = cdiv(ops[0].M, 128);
+  for (int i = 0; i < n_ops; ++i) {
+    c.op[i] = ops[i];
+    c.op[i].m_tiles = c.m_tiles;
+    c.op[i].n_blks = ops[i].W.N / 256;
+    c.op[i].trace = nullptr;
+  }
+  using Cfg = GemmImgCfg<256>;
+  LTR_CUDA_TRY(ensure_dynamic_smem(gemm_chain_kernel, Cfg::SMEM));
+  const int grid = c.m_tiles < device_sm_count() ? c.m_tiles : device_sm_count();
+  LaunchScope ls(KC_LINEAR, s);
+  LTR_CUDA_TRY(launch_pdl(gemm_chain_kernel, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, c));
+  return 0;
 }
 
 // ---------------------------------------------------------------- image <-> fp32 helpers

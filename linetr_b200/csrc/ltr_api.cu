@@ -3,6 +3,7 @@
 #include "../../include/linetr_b200.h"
 #include "../../include/linetr_b200_debug.h"
 
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -304,6 +305,20 @@ static ActImg tiles_image(void* tiles, int64_t n_lines) {
   return a;
 }
 
+// Fewest 128-row tiles for which an encode chains its row-local GEMMs (gemm_chain_kernel: one CTA per m-tile, so it
+// needs about as many m-tiles as SMs to pay).  128 = bench.py cfg1, the smallest batch measured faster chained on
+// H100 (a layer chain at 64 and 96 tiles was slower than its three launches, tools/gemm_chain_bench.py).
+// LTR_CHAIN_MIN_TILES overrides it, 0 = never chain; read at every call so that one process can run both paths.
+static int chain_min_tiles() {
+  const char* e = std::getenv("LTR_CHAIN_MIN_TILES");
+  if (e && *e) {
+    char* end = nullptr;
+    const long v = std::strtol(e, &end, 10);
+    if (*end == '\0' && v >= 0) return v == 0 || v > INT_MAX ? INT_MAX : (int)v;
+  }
+  return 128;
+}
+
 static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, float* out_rows, void* out_tiles,
                        const EncodeWs& w, cudaStream_t s) {
   const int R = in.n_lines, T = in.n_tokens;
@@ -328,6 +343,23 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
                                   in.image_height, s));
   LTR_TRY(gemm(m->lpe.l4, w.l128, 0, R, ACT_RELU, s, nullptr, 0, &w.l256, 0));
   LTR_TRY(gemm(m->lpe.l5, w.l256, 0, R, ACT_NONE, s, nullptr, 0, &w.lpos, 0));
+  // The row-local GEMM runs fc -> w_1 -> w_2 -> qkv(0) and, per signature layer, mlp1 -> mlp2 -> qkv(l+1) (or
+  // final_proj) go out as one gemm_chain_kernel launch each when the batch fills the GPU with m-tiles; small batches
+  // keep one launch per layer, which spreads the n-blocks of a layer over more SMs.
+  const bool chain = !out_cf && cdiv(R, 128) >= chain_min_tiles();
+  GemmImgArgs pend[CHAIN_MAX_OPS];
+  int n_pend = 0;
+  auto flush = [&]() -> int {
+    const int n = n_pend;
+    n_pend = 0;
+    if (n == 0) return 0;
+    return n == 1 ? launch_gemm_img(pend[0], s) : launch_gemm_chain(pend, n, s);
+  };
+  auto row_local = [&](const GemmImgArgs& a) -> int {   // queued for the current chain, or launched now
+    if (!chain) return launch_gemm_img(a, s);
+    pend[n_pend++] = a;
+    return 0;
+  };
   {
     // fc (+ CLS residual folded into the bias) -> LayerNorm in the epilogue -> y1.  y1 and the line position code live
     // only as split-bf16 images (hi + lo: ~2^-17 relative): the FFN residual and the post-norm addend are read back
@@ -338,9 +370,15 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
     // sentence = klines_pos + LN(y1 + ffn)  -> image xm[:, :256] (the running descriptor), all in the w_2 epilogue
     GemmImgArgs w2 = gemm_args(m->w2, w.g, 0, R, ACT_NONE, nullptr, 0, &w.xm, 0, nullptr, 0, &w.y1i, 0);
     w2.norm = NORM_LAYER; w2.eps = 1e-6f; w2.ng = m->ln2g; w2.nbeta = m->ln2b; w2.NaddImg = w.lpos; w2.nadd_kb0 = 0;
-    LTR_TRY(launch_gemm_img(fc, s, 256));
-    LTR_TRY(launch_gemm_img(w1, s));
-    LTR_TRY(launch_gemm_img(w2, s, 256));
+    if (m->cfg.d_inner % 256 == 0 && m->cfg.d_inner <= 64 * CHAIN_MAX_KB) {   // w_1 output fits the chain's k-block barriers
+      LTR_TRY(row_local(fc));
+      LTR_TRY(row_local(w1));
+      LTR_TRY(row_local(w2));
+    } else {
+      LTR_TRY(launch_gemm_img(fc, s));
+      LTR_TRY(launch_gemm_img(w1, s));
+      LTR_TRY(launch_gemm_img(w2, s));
+    }
   }
   // ---- line signature layers ----
   int max_l = in.lines_per_image;
@@ -354,17 +392,18 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
   fin.norm = NORM_L2; fin.eps = 1e-6f;   // final_proj + F.normalize in one epilogue (rows-only output)
   for (size_t li = 0; li < m->sig.size(); ++li) {
     const SigLayer& L = m->sig[li];
-    LTR_TRY(gemm(L.qkv, w.xm, 0, R, ACT_NONE, s, nullptr, 0, &w.qkv, 0));
+    LTR_TRY(row_local(gemm_args(L.qkv, w.xm, 0, R, ACT_NONE, nullptr, 0, &w.qkv, 0)));
+    LTR_TRY(flush());
     // o -> xm[:, 256:]
     LTR_TRY(launch_sig_attention_tc(w.qkv, w.xm, 256, cu, in.lines_per_image, max_l, in.n_images, s));
     // x += delta: the running descriptor lives ONLY as the split-bf16 image xm[:, :256] (hi + lo carries
     // ~2^-17 relative precision; an fp32 copy would double the store traffic of this epilogue)
-    LTR_TRY(gemm(L.mlp1, w.xm, 0, R, ACT_RELU, s, nullptr, 0, &w.hm, 0));
-    LTR_TRY(gemm(L.mlp2, w.hm, 0, R, ACT_NONE, s, nullptr, 0, &w.xm, 0, nullptr, 0, &w.xm, 0));
+    LTR_TRY(row_local(gemm_args(L.mlp1, w.xm, 0, R, ACT_RELU, nullptr, 0, &w.hm, 0)));
+    LTR_TRY(row_local(gemm_args(L.mlp2, w.hm, 0, R, ACT_NONE, nullptr, 0, &w.xm, 0, nullptr, 0, &w.xm, 0)));
   }
   if (!out_cf) {   // rows (+ matcher tile image): projection + L2 normalisation in one launch
-    LTR_TRY(launch_gemm_img(fin, s, 256));
-    return 0;
+    LTR_TRY(row_local(fin));
+    return flush();
   }
   LTR_TRY(gemm(m->wf, w.xm, 0, R, ACT_NONE, s, w.yf, 256));
   if (max_l > 0) {
@@ -1212,6 +1251,61 @@ float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t o
   cudaEventDestroy(e0); cudaEventDestroy(e1);
   cudaFree(dw); cudaFree(da); cudaFree(dout); cudaFree(dc);
   return cudaGetLastError() == cudaSuccess ? ms / iters : -1.f;
+}
+
+// One signature layer's row-local GEMMs at m rows (zero-filled operands, timing only):
+// mlp1 [512 x 512] ReLU -> hm, mlp2 [256 x 512] + x -> xm[:, :256] in place, qkv [768 x 256] -> qkv image,
+// as one gemm_chain_kernel launch (chained != 0) or three gemm_img_kernel launches.  Average device ms per layer.
+float ltr_gemm_chain_bench(int32_t m, int32_t chained, int32_t iters, int32_t device) {
+  if (m <= 0 || iters <= 0 || cudaSetDevice(device) != cudaSuccess) return -1.f;
+  const size_t mpad = (size_t)cdiv(m, 256) * 256;
+  const int Ns[3] = {512, 256, 768}, Ks[3] = {512, 512, 256}, acts[3] = {ACT_RELU, ACT_NONE, ACT_NONE};
+  uint16_t* dw[3] = {nullptr, nullptr, nullptr};
+  uint16_t *dxm = nullptr, *dhm = nullptr, *dqkv = nullptr;
+  bool ok = true;
+  for (int i = 0; i < 3; ++i) ok = ok && cudaMalloc(&dw[i], 2 * (size_t)Ns[i] * Ks[i] * 2) == cudaSuccess;
+  ok = ok && cudaMalloc(&dxm, 2 * mpad * 512 * 2) == cudaSuccess && cudaMalloc(&dhm, 2 * mpad * 512 * 2) == cudaSuccess &&
+       cudaMalloc(&dqkv, 2 * mpad * 768 * 2) == cudaSuccess;
+  float ms = -1.f;
+  if (ok) {
+    for (int i = 0; i < 3; ++i) cudaMemset(dw[i], 0, 2 * (size_t)Ns[i] * Ks[i] * 2);
+    cudaMemset(dxm, 0, 2 * mpad * 512 * 2);
+    auto img = [&](uint16_t* p, int K) {
+      return ActImg{reinterpret_cast<__nv_bfloat16*>(p), reinterpret_cast<__nv_bfloat16*>(p + mpad * K), K / 64};
+    };
+    const ActImg xm = img(dxm, 512), hm = img(dhm, 512), qkv = img(dqkv, 768);
+    const ActImg A[3] = {xm, hm, xm}, O[3] = {hm, xm, qkv};
+    GemmImgArgs ops[3];
+    for (int i = 0; i < 3; ++i) {
+      GemmImgArgs a{};
+      a.A = A[i]; a.O = O[i]; a.M = m; a.act = acts[i];
+      a.W.hi = reinterpret_cast<const __nv_bfloat16*>(dw[i]);
+      a.W.lo = reinterpret_cast<const __nv_bfloat16*>(dw[i] + (size_t)Ns[i] * Ks[i]);
+      a.W.N = Ns[i]; a.W.K = Ks[i];
+      ops[i] = a;
+    }
+    ops[1].Rimg = xm;   // x += delta
+    auto layer = [&]() {
+      if (chained) return launch_gemm_chain(ops, 3, 0);
+      for (int i = 0; i < 3; ++i)
+        if (int rc = launch_gemm_img(ops[i], 0)) return rc;
+      return 0;
+    };
+    cudaEvent_t e0, e1;
+    cudaEventCreate(&e0); cudaEventCreate(&e1);
+    int rc = 0;
+    for (int i = 0; i < 3 && !rc; ++i) rc = layer();
+    cudaEventRecord(e0, 0);
+    for (int i = 0; i < iters && !rc; ++i) rc = layer();
+    cudaEventRecord(e1, 0);
+    cudaEventSynchronize(e1);
+    if (!rc && cudaGetLastError() == cudaSuccess && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess) ms /= iters;
+    else ms = -1.f;
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+  }
+  for (int i = 0; i < 3; ++i) cudaFree(dw[i]);
+  cudaFree(dxm); cudaFree(dhm); cudaFree(dqkv);
+  return ms;
 }
 
 }  // extern "C"

@@ -51,6 +51,11 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// generic-proxy global writes -> visible to the async proxy (later TMA reads of the same addresses)
+__device__ __forceinline__ void fence_proxy_async_global() {
+  asm volatile("fence.proxy.async.global;" ::: "memory");
+}
+
 // ------------------------------------------------------------------ bulk async copy (TMA 1-D)
 // global -> shared, completion signalled on an mbarrier with complete_tx::bytes.
 // bytes % 16 == 0, both addresses 16-byte aligned.
