@@ -21,6 +21,9 @@
  *   ltr_match_distmat          <- nn_matcher_distmat on a caller-supplied distance matrix.
  *   ltr_image_tiles +          <- Matching.forward with a side already in `data` (models/matching.py:20-60):
  *   ltr_match_indexed             images encoded once, matched in any number of pairs.
+ *   ltr_line_gt                <- mat_assign_sublines of the homography dataset builder
+ *                                 (dataloaders/build_homography_dataset.py:210-234) + Evaluate_PR.calc_TFPN
+ *                                 (evaluations/evaluate_pr.py:10-22) for a batch of pairs.
  *
  * Conventions: return 0 on success, a negative LTR_E_* code on failure (message via
  * ltr_last_error(), thread-local).  All device pointers are caller-owned and must live on
@@ -343,6 +346,68 @@ typedef struct {
 
 int ltr_tokenize_batch(const LtrTokenizeBatchInput* in, float* sublines, float* pnt, float* mask, float* resp,
                        float* angle, float* desc, float* score, int32_t device, void* stream);
+
+/* Homography ground truth for line matches, and precision/recall counts of predicted matches, for a batch of
+ * pairs.  Per pair this is the homography dataset builder's mat_assign_sublines
+ * (dataloaders/build_homography_dataset.py:210-234): find_line_matches (dataloaders/utils/util_lines.py:67-114) of
+ * side 0 against side 1 projected into image 0 and of side 1 against side 0 projected into image 1, the mutual AND,
+ * calculate_line_overlaps (:116-171) both ways on the mutual entries, then their element-wise max.  Counts follow
+ * Evaluate_PR.calc_TFPN (evaluations/evaluate_pr.py:10-22).
+ *
+ * Side s of pair p owns segments [cu_s[p], cu_s[p+1]) of segs_s ([S, 2, 2] fp32 pixels, start xy then end xy).
+ * homography[p] maps image 0 to image 1 and homography_inv[p] is its inverse (computed by the caller; the library
+ * never inverts a matrix).  proj0 = segs0 mapped by H and proj1 = segs1 mapped by H^-1 follow
+ * cv2.perspectiveTransform: in fp64, w = x*m6 + y*m7 + m8, the point is ((x*m0 + y*m1 + m2) * (1/w), ...) rounded
+ * to fp32 if |w| > FLT_EPSILON, else (0, 0).  A caller may pass proj0 / proj1 itself (e.g. the projections a dataset
+ * stored); the kernel then skips its own.
+ *
+ * Arithmetic reproduces the reference's numpy float32 scalars: every + - * / sqrt is an IEEE fp32 operation in the
+ * reference's order, so distances, lengths and overlap ratios are bit-identical for the same projections.  Literal
+ * behaviours kept on purpose:
+ *   - the angle is degrees(atan2(dx, dy)) (x and y swapped) and the difference is |a1 - a0| % 180, so anti-parallel
+ *     lines just past 180 degrees pass and lines at ~179 degrees fail;
+ *   - a zero-length segment gives a 0/0 = NaN point-line distance, which fails every comparison, so the "both
+ *     endpoints far" skip does not fire;
+ *   - all comparisons are the reference's strict < / > (overlap: both end points inside -> len1/len0, one inside ->
+ *     the distance ratio, neither -> 1 if max distance <= len0 + len1);
+ *   - TN counts rows whose number of columns with neither a prediction nor ground truth equals the number of ROWS
+ *     (shape[0]); this differs from "all columns" for non-square pairs only.
+ * The one deliberate difference: the angle is computed in fp64 (atan2, * 180/pi, fmod) where numpy's float32
+ * arctan2 / degrees are not correctly rounded, so the angle decision can differ from the reference's only where
+ * its |ang_diff - thres_angdiff| (or |a1 - a0| against 180 / 360) is within about 1e-3 degrees.
+ * Inputs must be finite. */
+typedef struct {
+  const float* segs0;            /* device [S0, 2, 2] */
+  const float* segs1;            /* device [S1, 2, 2] */
+  const int32_t* cu0;            /* device [n_pairs + 1] */
+  const int32_t* cu1;
+  const double* homography;      /* device [n_pairs, 3, 3], image 0 -> image 1 */
+  const double* homography_inv;  /* device [n_pairs, 3, 3] */
+  const float* proj0;            /* optional device [S0, 2, 2]: segs0 mapped by H (NULL: computed) */
+  const float* proj1;            /* optional device [S1, 2, 2]: segs1 mapped by H^-1 */
+  const int32_t* pred0;          /* optional device [S0]: predicted match of every side-0 segment, local index into
+                                    side 1, or -1 (values outside [0, n1_p) count as no prediction) */
+  int32_t n_pairs;
+  int32_t max_n0, max_n1;        /* bounds of every pair's segment counts (grid sizing) */
+  float thres_reprojected;       /* pixels (confs/homography.yaml: 3) */
+  double thres_angdiff;          /* degrees (2) */
+  double min_overlap_ratio;      /* n_gt counts entries > this (0.3) */
+} LtrLineGtInput;
+
+/* Outputs (device, caller-owned).  assign (optional): mat_assign_sublines of pair p as fp32 row-major [n0_p, n1_p]
+ * at p * assign_stride (values 0, 1 or fp32 ratios, so lossless), assign_stride >= max_n0 * max_n1.  n_gt [n_pairs]
+ * (required): entries > min_overlap_ratio, the length of the builder's lmatches.  tfpn [n_pairs, 4] (required iff
+ * pred0): TP, FP, FN, TN with score_gt = assign > 0.  With assign == NULL no dense matrix is written: the counts-only
+ * mode for large evaluations. */
+typedef struct {
+  float* assign;
+  int64_t assign_stride;
+  int32_t* n_gt;
+  int32_t* tfpn;
+} LtrLineGtOutput;
+
+/* Asynchronous on `stream`; never synchronises. */
+int ltr_line_gt(const LtrLineGtInput* in, const LtrLineGtOutput* out, int32_t device, void* stream);
 
 /* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
  * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */

@@ -4,6 +4,8 @@ Drop-in names (same call surface as yosungho/LineTR `models/`):
     LineTransformer, get_dist_matrix, nn_matcher, nn_matcher_distmat
 Batched front-end:
     PairEngine, LineBatch, ImagePairMatches, ImageSet, exhaustive_pairs
+Match quality against homography ground truth (eval_homography):
+    line_assignment, get_precision_recall, homography_ground_truth, score_line_matches
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -25,6 +27,10 @@ _LAZY = {
     "ImagePairMatches": ("engine", "ImagePairMatches"),
     "ImageSet": ("engine", "ImageSet"),
     "exhaustive_pairs": ("engine", "exhaustive_pairs"),
+    "line_assignment": ("eval_homography", "line_assignment"),
+    "get_precision_recall": ("eval_homography", "get_precision_recall"),
+    "homography_ground_truth": ("eval_homography", "homography_ground_truth"),
+    "score_line_matches": ("eval_homography", "score_line_matches"),
 }
 
 

@@ -25,6 +25,7 @@ EXPORTED_SYMBOLS = (
     "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
+    "ltr_line_gt",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
@@ -110,6 +111,17 @@ class LtrTokenizeBatchInput(C.Structure):
                 ("align_corners", C.c_int32), ("images", C.POINTER(LtrTokenizeImage)), ("cu_sublines", c_int32_p)]
 
 
+class LtrLineGtInput(C.Structure):
+    _fields_ = [("segs0", C.c_void_p), ("segs1", C.c_void_p), ("cu0", C.c_void_p), ("cu1", C.c_void_p),
+                ("homography", C.c_void_p), ("homography_inv", C.c_void_p), ("proj0", C.c_void_p), ("proj1", C.c_void_p),
+                ("pred0", C.c_void_p), ("n_pairs", C.c_int32), ("max_n0", C.c_int32), ("max_n1", C.c_int32),
+                ("thres_reprojected", C.c_float), ("thres_angdiff", C.c_double), ("min_overlap_ratio", C.c_double)]
+
+
+class LtrLineGtOutput(C.Structure):
+    _fields_ = [("assign", C.c_void_p), ("assign_stride", C.c_int64), ("n_gt", C.c_void_p), ("tfpn", C.c_void_p)]
+
+
 def lib_path() -> str:
     return _LIB_PATH
 
@@ -155,6 +167,8 @@ def load():
     lib.ltr_match_indexed.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrPairIndex), C.POINTER(LtrMatchOutput),
                                       C.c_int32, C.c_void_p]
     lib.ltr_match_indexed.restype = C.c_int
+    lib.ltr_line_gt.argtypes = [C.POINTER(LtrLineGtInput), C.POINTER(LtrLineGtOutput), C.c_int32, C.c_void_p]
+    lib.ltr_line_gt.restype = C.c_int
     lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.ltr_gather_wait.restype = C.c_int
     lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,

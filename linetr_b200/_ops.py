@@ -290,6 +290,36 @@ def match_indexed(desc0, desc1, layout, n_pairs, nn_thresh, *, cu0, cu1, max_n0,
     N.check(rc, "ltr_match_indexed")
 
 
+def line_gt(segs0, segs1, n_pairs, *, cu0, cu1, max_n0, max_n1, homography, homography_inv, n_gt, assign=None,
+            assign_stride=0, pred0=None, tfpn=None, proj0=None, proj1=None, thres_reprojected=3.0, thres_angdiff=2.0,
+            min_overlap_ratio=0.3):
+    """ltr_line_gt into caller-allocated outputs: homography ground truth of P line-segment pairs (segs [S,2,2] fp32,
+    side s of pair p = [cu_s[p], cu_s[p+1]), homography [P,3,3] fp64 image 0 -> 1 and its inverse), n_gt [P] int32,
+    optionally the dense assignment (pair p at p * assign_stride, row-major [n0_p, n1_p]) and, with pred0 (int32 [S0]
+    local side-1 index or -1), tfpn [P,4] int32 (TP, FP, FN, TN)."""
+    _req_cuda(segs0, "segs0")
+    _req_cuda(segs1, "segs1")
+    dev = segs0.device
+    for nm, t, dt in (("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32), ("cu0", cu0, torch.int32),
+                      ("cu1", cu1, torch.int32), ("homography", homography, torch.float64),
+                      ("homography_inv", homography_inv, torch.float64), ("n_gt", n_gt, torch.int32),
+                      ("assign", assign, torch.float32), ("pred0", pred0, torch.int32), ("tfpn", tfpn, torch.int32),
+                      ("proj0", proj0, torch.float32), ("proj1", proj1, torch.float32)):
+        if t is None:
+            continue
+        _req_cuda(t, nm)
+        if t.dtype != dt or not t.is_contiguous() or t.device != dev:
+            raise N.LtrError(f"line_gt: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    inp = N.LtrLineGtInput(_ptr(segs0).value, _ptr(segs1).value, _ptr(cu0).value, _ptr(cu1).value, _ptr(homography).value,
+                           _ptr(homography_inv).value, _ptr(proj0).value, _ptr(proj1).value, _ptr(pred0).value,
+                           int(n_pairs), int(max_n0), int(max_n1), float(thres_reprojected), float(thres_angdiff),
+                           float(min_overlap_ratio))
+    out = N.LtrLineGtOutput(_ptr(assign).value, int(assign_stride), _ptr(n_gt).value, _ptr(tfpn).value)
+    with torch.cuda.device(dev):
+        rc = N.load().ltr_line_gt(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_line_gt")
+
+
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     """ltr_match_distmat on dist [P, n0, n1] (CUDA).  Returns dict(matches0 [P,n0], scores0, nn1, counts)."""
     _req_cuda(dist, "dist_mat")

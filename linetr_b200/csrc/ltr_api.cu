@@ -19,6 +19,7 @@
 #include "tokenizer_kernels.cuh"
 #include "match_kernels.cuh"
 #include "match_tc.cuh"
+#include "line_gt.cuh"
 
 namespace ltr {
 
@@ -36,7 +37,7 @@ int set_error(int code, const std::string& msg) {
 const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
-                                         "tokenize", "desc_tiles", "match_tc", "match_tail"};
+                                         "tokenize", "desc_tiles", "match_tc", "match_tail", "line_gt"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1120,6 +1121,36 @@ int ltr_tokenize_batch(const LtrTokenizeBatchInput* in, float* sublines, float* 
     }
     LTR_TRY(launch_tokenize(L, I, cu[i0], cu[i1], in->align_corners, sublines, pnt, mask, resp, angle, desc, score, s));
   }
+  return LTR_OK;
+}
+
+int ltr_line_gt(const LtrLineGtInput* in, const LtrLineGtOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_line_gt: null argument");
+  if (in->n_pairs < 0 || in->max_n0 < 0 || in->max_n1 < 0) return set_error(LTR_E_INVALID, "ltr_line_gt: negative count");
+  if (out->assign && out->assign_stride < (int64_t)in->max_n0 * in->max_n1)
+    return set_error(LTR_E_INVALID, "ltr_line_gt: assign_stride < max_n0 * max_n1");
+  if (in->n_pairs == 0) return LTR_OK;
+  if (!out->n_gt) return set_error(LTR_E_INVALID, "ltr_line_gt: null n_gt");
+  if (in->pred0 && !out->tfpn) return set_error(LTR_E_INVALID, "ltr_line_gt: pred0 needs tfpn");
+  if (!in->cu0 || !in->cu1 || !in->homography || !in->homography_inv)
+    return set_error(LTR_E_INVALID, "ltr_line_gt: null input array");
+  if ((in->max_n0 > 0 && !in->segs0) || (in->max_n1 > 0 && !in->segs1))
+    return set_error(LTR_E_INVALID, "ltr_line_gt: null segments");
+  for (const void* p : {(const void*)in->segs0, (const void*)in->segs1, (const void*)in->proj0, (const void*)in->proj1})
+    if (reinterpret_cast<uintptr_t>(p) & 15) return set_error(LTR_E_INVALID, "ltr_line_gt: segments must be 16-byte aligned");
+  if (cdiv(in->max_n0, LG_ROWS) > 65535) return set_error(LTR_E_INVALID, "ltr_line_gt: too many side-0 segments per pair");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  LTR_CUDA_TRY(cudaMemsetAsync(out->n_gt, 0, sizeof(int32_t) * in->n_pairs, s));
+  if (in->pred0) LTR_CUDA_TRY(cudaMemsetAsync(out->tfpn, 0, sizeof(int32_t) * 4 * in->n_pairs, s));
+  if (in->max_n0 == 0) return LTR_OK;
+  LineGtArgs a{in->segs0, in->segs1, in->cu0, in->cu1, in->homography, in->homography_inv, in->proj0, in->proj1, in->pred0,
+               in->thres_reprojected, in->thres_angdiff, in->min_overlap_ratio, out->assign, (long long)out->assign_stride,
+               out->n_gt, out->tfpn};
+  const dim3 grid(in->n_pairs, cdiv(in->max_n0, LG_ROWS));
+  LaunchScope ls(KC_LINE_GT, s);
+  if (out->assign) LTR_CUDA_TRY(launch_pdl(line_gt_kernel<true>, grid, dim3(LG_ROWS), 0, s, a));
+  else LTR_CUDA_TRY(launch_pdl(line_gt_kernel<false>, grid, dim3(LG_ROWS), 0, s, a));
   return LTR_OK;
 }
 
