@@ -135,7 +135,8 @@ typedef struct {
   const float* desc0;
   const float* desc1;
   int32_t layout;          /* LTR_LAYOUT_* of desc0/desc1 */
-  int32_t d;               /* descriptor dim, multiple of 16 */
+  int32_t d;               /* descriptor dim, multiple of 16 (others: LTR_E_UNSUPPORTED, from
+                              ltr_match_workspace_bytes too) */
   int32_t n_pairs;
   int32_t n0, n1;          /* sublines per image when cu0/cu1 are NULL */
   const int32_t* cu0;      /* device [n_pairs+1] or NULL */

@@ -785,6 +785,9 @@ static const char* check_match_input(const LtrMatchInput* in) {
   return nullptr;
 }
 
+// a descriptor dimension that is not a multiple of 16 is a valid request the kernels do not serve
+static int match_input_code(const LtrMatchInput* in) { return in->d > 0 && in->d % 16 ? LTR_E_UNSUPPORTED : LTR_E_INVALID; }
+
 }  // extern "C"
 
 // launch sequence of the tensor-core matcher; returns 0 or an error code.  ix != nullptr: pair list over image
@@ -827,6 +830,7 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
       }
     }
     ma.dist_mode = in.dist_mode;
+    ma.thr = in.nn_thresh;
     ma.dist = seg ? out.dist_sub : out.dist_key;
     ma.dist_stride = seg ? (long long)pl.mx[0] * pl.mx[1] : stride_key;
     ma.counts = want_nn ? out.counts : nullptr;
@@ -869,7 +873,7 @@ extern "C" {
 
 int64_t ltr_match_workspace_bytes(const LtrMatchInput* in) {
   if (!in) return set_error(LTR_E_INVALID, "ltr_match_workspace_bytes: null argument");
-  if (const char* e = check_match_input(in)) return set_error(LTR_E_INVALID, e);
+  if (const char* e = check_match_input(in)) return set_error(match_input_code(in), e);
   if (in->n_pairs <= 0 || in->d != MT_D) return 0;
   return plan_match(*in, nullptr).bytes + 1024;
 }
@@ -877,7 +881,7 @@ int64_t ltr_match_workspace_bytes(const LtrMatchInput* in) {
 int ltr_match(const LtrMatchInput* in, const LtrMatchOutput* out, int32_t device, void* stream) {
   if (!in || !out) return set_error(LTR_E_INVALID, "ltr_match: null argument");
   if (in->n_pairs <= 0) return LTR_OK;
-  if (const char* e = check_match_input(in)) return set_error(in->d % 16 ? LTR_E_UNSUPPORTED : LTR_E_INVALID, e);
+  if (const char* e = check_match_input(in)) return set_error(match_input_code(in), e);
   const bool seg = in->sub_off0 != nullptr;
   const bool tc = in->d == MT_D;
   const bool want_nn = out->matches0 != nullptr;

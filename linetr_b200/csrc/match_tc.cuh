@@ -10,11 +10,16 @@
 // evaluations/matcher.py:51-102 (||a||^2 + ||b||^2 - 2 ab).
 //
 // Precision contract.  The contraction is a 3-term split-bf16 product (hi*hi + lo*hi + hi*lo, fp32
-// accumulate in registers): ~1e-5 absolute on a distance.  Match indices must be bit-exact, so every row
-// whose best and second-best distance are closer than MATCH_EPS, or whose best distance lies within
-// MATCH_EPS of the threshold, is recomputed by the tail kernel with fp32 FMAs in ascending k order
-// (the arithmetic of the round-1 FFMA matcher the golden vectors were pinned with) before any decision
-// is taken.  Exact ties therefore resolve to the lowest index exactly as np.argmin does.
+// accumulate in registers): ~1e-5 absolute on a distance of unit descriptors, growing with |a| |b|.  Match
+// indices must be bit-exact, so every row whose best and second-best distance are closer than a margin eps,
+// or whose best distance lies within eps of the threshold, is recomputed by the tail kernel with fp32 FMAs in
+// ascending k order (the arithmetic of the round-1 FFMA matcher the golden vectors were pinned with) before
+// any decision is taken.  Exact ties therefore resolve to the lowest index exactly as np.argmin does.
+// eps = MATCH_EPS in distance mode 0 (unit descriptors) and MATCH_EPS * max(1, |a_i| * max_j |b_j|) in mode 1
+// (j over the pair's other side).  The exact distance of lines a, b is
+//     acc = 0; for k = 0..255: acc = fmaf(a_k, b_k, acc)
+//     mode 0: max(0, 2 - 2 acc)      mode 1: max(0, (sq(a) + sq(b)) - 2 acc)
+// with sq(x) the same ascending-k fmaf chain of x_k * x_k (desc_tiles_kernel, both layouts).
 //
 // Operands are "descriptor tile images": the split-bf16 activation-image format of gemm_img.cuh
 // (planes hi / lo, 16 KB tiles [row/128][k/64] of 128 rows x 64 k, K-major SWIZZLE_128B), 4 k-blocks
@@ -64,6 +69,7 @@ struct MatchSide {
 struct MatchTcArgs {
   MatchSide s[2];
   int dist_mode;         // 0: 2 - 2 s (unit descriptors, nn_matcher.py:37-38)   1: |a|^2 + |b|^2 - 2 s (evaluations/matcher.py:66-70)
+  float thr;             // match threshold (distance mode 1: side-0 rows near it are flagged ambiguous here)
   float* dist;           // optional dense output of side 0 vs side 1, pair p at p * dist_stride, row-major [n0_p, n1_p]
   long long dist_stride;
   int* counts;           // zeroed here (the tail kernel accumulates into it)
@@ -162,6 +168,18 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
     const float sqa = (p.dist_mode == 1 && valid_row) ? SA.sq[ba + row] : 0.f;
     float* drow = (p.dist && side == 0 && valid_row) ? p.dist + (long long)pair * p.dist_stride + (long long)row * nb : nullptr;
     const bool dvec = drow && (nb % 8 == 0) && (p.dist_stride % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.dist) & 31) == 0);
+    // distance mode 1: the largest squared norm of side B, for the margin of this row (see eps below)
+    float sqb_max = 0.f;
+    if (p.dist_mode == 1 && active) {
+      for (int j = tid; j < nb; j += 256) sqb_max = fmaxf(sqb_max, SB.sq[bb + j]);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sqb_max = fmaxf(sqb_max, __shfl_xor_sync(0xffffffffu, sqb_max, o));
+      if (lane == 0) xch[warp] = sqb_max;
+      mt_epi_bar();
+#pragma unroll
+      for (int w = 0; w < 8; ++w) sqb_max = fmaxf(sqb_max, xch[w]);
+      mt_epi_bar();   // xch is reused by the half merge
+    }
     if (active) ptx::mbar_wait(a_full, 0);
     uint32_t it = 0;
     for (int ct = 0; ct < n_ct; ++ct) {
@@ -266,7 +284,14 @@ __global__ void __launch_bounds__(MT_THREADS, 1) match_tc_kernel(MatchTcArgs p) 
       const int oi = reinterpret_cast<int*>(xch)[256 + r_in];
       if (ob < best || (ob == best && oi < bidx)) { second = fminf(best, os); best = ob; bidx = oi; }
       else second = fminf(second, ob);
-      const bool amb = !(second - best >= MATCH_EPS);   // also true for NaN
+      // Margin below which the tensor-core value cannot decide: MATCH_EPS for unit descriptors (mode 0).  In mode 1
+      // the product error grows with |a| |b|, so the margin is MATCH_EPS * max(1, |a_i| * max_j |b_j|), and it also
+      // covers the distance to the threshold on side 0 (the tail's own MATCH_EPS check is then never the tighter one).
+      bool amb = !(second - best >= MATCH_EPS);   // also true for NaN
+      if (p.dist_mode == 1) {
+        const float eps = MATCH_EPS * fmaxf(1.f, sqrtf(sqa * sqb_max));
+        amb = !(second - best >= eps) || (side == 0 && !(fabsf(best - p.thr) >= eps));
+      }
       if (SA.slot) {
         const int sbase = SA.pimg ? SA.out_off[pair] : ba;   // slots are per (pair, line) when images are shared
         SA.slot[sbase + row] = make_uint2(__float_as_uint(best), (uint32_t)bidx | (amb ? 0x80000000u : 0u));
@@ -286,9 +311,18 @@ struct DescTilesArgs {
                            // start at tile_off[p]; nullptr: pair-aligned, pair p at tile p * tmax
 };
 
+// Squared norm of one line for distance mode 1: a single ascending-k fmaf chain, s = fmaf(x_k, x_k, s) for
+// k = 0..255 - the order of exact_row's dot products, and the same in both descriptor layouts, so the same
+// descriptors get the same bits wherever they come from.  x_k is at x[k * stride].
+__device__ __forceinline__ float sq_chain(const float* __restrict__ x, size_t stride) {
+  float s = 0.f;
+#pragma unroll 8
+  for (int k = 0; k < MT_D; ++k) s = fmaf(x[k * stride], x[k * stride], s);
+  return s;
+}
+
 // grid = (max(tmax0, tmax1) * 4, n_pairs, 2): block = 32 lines of one tile; 256 threads.
 __global__ void __launch_bounds__(256) desc_tiles_kernel(DescTilesArgs p) {
-  __shared__ float part[8][33];
   pdl_launch_dependents();
   pdl_wait();
   const int side = blockIdx.z, pair = blockIdx.y;
@@ -320,19 +354,15 @@ __global__ void __launch_bounds__(256) desc_tiles_kernel(DescTilesArgs p) {
       const size_t off = (t0 + (lane >> 3)) * (size_t)MT_TILE + ptx::sw128_offset(r_in, (lane & 7) * 8);
       *reinterpret_cast<uint4*>(hi + off) = h;
       *reinterpret_cast<uint4*>(lo + off) = l;
-      if (p.sq[side]) {
-        float s = 0.f;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) s = fmaf(v[j], v[j], s);
-        s = warp_sum(s);
-        if (lane == 0 && r < n) p.sq[side][b + r] = s;
-      }
+    }
+    if (p.sq[side] && lane < 4) {   // lanes 0-3: the 4 lines this warp just converted
+      const int r = tile * 128 + sub * 32 + warp * 4 + lane;
+      if (r < n) p.sq[side][b + r] = sq_chain(src + (size_t)(b + r) * MT_D, 1);
     }
   } else {
     // lane -> line, warp -> groups of 8 consecutive k (4 groups per warp): loads coalesced along lines
     const int r_in = sub * 32 + lane, r = tile * 128 + r_in;
     const float* __restrict__ base = src + (size_t)b * MT_D;   // [256, n] of this pair
-    float s = 0.f;
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
       const int k0 = (g * 8 + warp) * 8;
@@ -344,19 +374,8 @@ __global__ void __launch_bounds__(256) desc_tiles_kernel(DescTilesArgs p) {
       const size_t off = (t0 + (k0 >> 6)) * (size_t)MT_TILE + ptx::sw128_offset(r_in, k0 & 63);
       *reinterpret_cast<uint4*>(hi + off) = h;
       *reinterpret_cast<uint4*>(lo + off) = l;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s = fmaf(v[j], v[j], s);
     }
-    if (p.sq[side]) {
-      part[warp][lane] = s;
-      __syncthreads();
-      if (warp == 0 && r < n) {
-        float t = 0.f;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) t += part[w][lane];
-        p.sq[side][b + r] = t;
-      }
-    }
+    if (p.sq[side] && warp == 0 && r < n) p.sq[side][b + r] = sq_chain(base + r, n);   // coalesced along lines
   }
 }
 
