@@ -160,6 +160,31 @@ def _match_workspace(dev, need: int) -> torch.Tensor:
     return ws
 
 
+def _struct(cls, **fields):
+    """A ctypes struct by field name: tensors go in as device pointers, None and fields not given as NULL / 0.  The
+    caller keeps the tensors alive until the call."""
+    return cls(**{k: v.data_ptr() if isinstance(v, torch.Tensor) else v for k, v in fields.items() if v is not None})
+
+
+def _match(entry: str, dev, inp: dict, out: dict, idx=None, gather=None):
+    """One matcher call on the current stream of `dev`: `entry` is ltr_match, or ltr_match_indexed with the pair index
+    `idx`.  LtrMatchInput fields in `inp`, LtrPairIndex fields in `idx` and output tensors in `out`, all by field name;
+    the scratch is the per-stream workspace, grown to what `entry`_workspace_bytes asks for."""
+    lib = N.load()
+    args = [C.byref(_struct(N.LtrMatchInput, **inp))]
+    if idx is not None:
+        args.append(C.byref(_struct(N.LtrPairIndex, **idx)))
+    need = int(getattr(lib, entry + "_workspace_bytes")(*args))
+    if need < 0:
+        N.check(need, entry + "_workspace_bytes")
+    ws = _match_workspace(dev, need)
+    o = _struct(N.LtrMatchOutput, workspace=ws, workspace_bytes=ws.numel(),
+                gather=C.pointer(gather) if gather is not None else None, **out)
+    with torch.cuda.device(dev):
+        rc = getattr(lib, entry)(*args, C.byref(o), dev.index, _stream_ptr(dev))
+    N.check(rc, entry)
+
+
 def match_descriptors(desc0, desc1, layout, n_pairs, nn_thresh, mutual=True, *, n0=0, n1=0, cu0=None, cu1=None,
                       max_n0=0, max_n1=0, sub_off0=None, sub_off1=None, cuk0=None, cuk1=None, max_k0=0, max_k1=0,
                       total_k0=None, total_k1=None, d=256, want_dist=True, want_matches=True, dist_mode=0,
@@ -199,27 +224,17 @@ def match_descriptors(desc0, desc1, layout, n_pairs, nn_thresh, mutual=True, *, 
     if n_pairs == 0:
         return out
     dist_sub = torch.empty(max(n_pairs * mx0 * mx1, 1), **f32) if seg else None
-    tensors = [cu0, cu1, sub_off0, sub_off1, cuk0, cuk1]
-    tensors = [(_i32c(t) if t is not None else None) for t in tensors]
-    inp = N.LtrMatchInput(desc0.data_ptr(), desc1.data_ptr(), int(layout), int(d), int(n_pairs), int(n0), int(n1),
-                          *[t.data_ptr() if t is not None else None for t in tensors],
-                          int(max_n0), int(max_n1), int(max_k0), int(max_k1), 0, float(nn_thresh), int(bool(mutual)),
-                          int(total_n0), int(total_n1), int(dist_mode),
-                          tiles0.data_ptr() if tiles0 is not None else None,
-                          tiles1.data_ptr() if tiles1 is not None else None,
-                          int(tiles_lines[0]), int(tiles_lines[1]), int(tiles_row0[0]), int(tiles_row0[1]))
-    lib = N.load()
-    need = int(lib.ltr_match_workspace_bytes(C.byref(inp)))
-    if need < 0:
-        N.check(need, "ltr_match_workspace_bytes")
-    ws = _match_workspace(dev, need)
-    g = lambda k: out[k].data_ptr() if out.get(k) is not None else None
-    o = N.LtrMatchOutput(g("matches0"), g("scores0"), g("nn1"), g("counts"), g("dist_key"),
-                         dist_sub.data_ptr() if dist_sub is not None else None, ws.data_ptr(), ws.numel(),
-                         C.pointer(gather) if gather is not None else None)
-    with torch.cuda.device(dev):
-        rc = lib.ltr_match(C.byref(inp), C.byref(o), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_match")
+    cu0, cu1, sub_off0, sub_off1, cuk0, cuk1 = (_i32c(t) if t is not None else None
+                                                for t in (cu0, cu1, sub_off0, sub_off1, cuk0, cuk1))
+    _match("ltr_match", dev,
+           dict(desc0=desc0, desc1=desc1, layout=layout, d=d, n_pairs=n_pairs, n0=n0, n1=n1, cu0=cu0, cu1=cu1,
+                sub_off0=sub_off0, sub_off1=sub_off1, cuk0=cuk0, cuk1=cuk1, max_n0=max_n0, max_n1=max_n1, max_k0=max_k0,
+                max_k1=max_k1, nn_thresh=nn_thresh, mutual=bool(mutual), total_n0=total_n0, total_n1=total_n1,
+                dist_mode=dist_mode, tiles0=tiles0, tiles1=tiles1, tiles_lines0=tiles_lines[0],
+                tiles_lines1=tiles_lines[1], tiles_row0_0=tiles_row0[0], tiles_row0_1=tiles_row0[1]),
+           dict(matches0=out.get("matches0"), scores0=out.get("scores0"), nn1=out.get("nn1"), counts=out.get("counts"),
+                dist_key=out["dist_key"], dist_sub=dist_sub),
+           gather=gather)
     return out
 
 
@@ -270,24 +285,15 @@ def match_indexed(desc0, desc1, layout, n_pairs, nn_thresh, *, cu0, cu1, max_n0,
         dist_stride = max_k0 * max_k1
         dist_key = torch.empty(max(n_pairs * dist_stride, 1), **f32)
     dist_sub = torch.empty(max(n_pairs * max_n0 * max_n1, 1), **f32) if seg else None
-    inp = N.LtrMatchInput(desc0.data_ptr(), desc1.data_ptr(), int(layout), 256, int(n_pairs), 0, 0,
-                          *[t.data_ptr() if t is not None else None for t in (cu0, cu1, sub_off0, sub_off1, cuk0, cuk1)],
-                          int(max_n0), int(max_n1), int(max_k0), int(max_k1), int(dist_stride), float(nn_thresh),
-                          int(bool(mutual)), int(desc0.numel() // 256), int(desc1.numel() // 256), 0,
-                          None, None, 0, 0, 0, 0)
-    idx = N.LtrPairIndex(img0.data_ptr(), img1.data_ptr(), tiles0.data_ptr(), tiles1.data_ptr(), tile_off0.data_ptr(),
-                         tile_off1.data_ptr(), int(n_tiles0), int(n_tiles1), out_off0.data_ptr(), out_off1.data_ptr(),
-                         int(total_out0), int(total_out1))
-    lib = N.load()
-    need = int(lib.ltr_match_indexed_workspace_bytes(C.byref(inp), C.byref(idx)))
-    if need < 0:
-        N.check(need, "ltr_match_indexed_workspace_bytes")
-    ws = _match_workspace(dev, need)
-    o = N.LtrMatchOutput(_ptr(matches0).value, _ptr(scores0).value, _ptr(nn1).value, _ptr(counts).value,
-                         _ptr(dist_key).value, _ptr(dist_sub).value, ws.data_ptr(), ws.numel(), None)
-    with torch.cuda.device(dev):
-        rc = lib.ltr_match_indexed(C.byref(inp), C.byref(idx), C.byref(o), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_match_indexed")
+    _match("ltr_match_indexed", dev,
+           dict(desc0=desc0, desc1=desc1, layout=layout, d=256, n_pairs=n_pairs, cu0=cu0, cu1=cu1, sub_off0=sub_off0,
+                sub_off1=sub_off1, cuk0=cuk0, cuk1=cuk1, max_n0=max_n0, max_n1=max_n1, max_k0=max_k0, max_k1=max_k1,
+                dist_pair_stride=dist_stride, nn_thresh=nn_thresh, mutual=bool(mutual), total_n0=desc0.numel() // 256,
+                total_n1=desc1.numel() // 256),
+           dict(matches0=matches0, scores0=scores0, nn1=nn1, counts=counts, dist_key=dist_key, dist_sub=dist_sub),
+           idx=dict(img0=img0, img1=img1, tiles0=tiles0, tiles1=tiles1, tile_off0=tile_off0, tile_off1=tile_off1,
+                    n_tiles0=n_tiles0, n_tiles1=n_tiles1, out_off0=out_off0, out_off1=out_off1, total_out0=total_out0,
+                    total_out1=total_out1))
 
 
 def line_gt(segs0, segs1, n_pairs, *, cu0, cu1, max_n0, max_n1, homography, homography_inv, n_gt, assign=None,

@@ -706,16 +706,22 @@ struct MatchPlan {
   int64_t bytes;
 };
 
-static MatchPlan plan_match(const LtrMatchInput& in, char* base) {
+// Scratch carve-up of one match.  ix == nullptr: a batch of pairs; a side either reads the caller's tile image
+// (written by ltr_encode) or is converted into the scratch.  ix != nullptr: a pair list over image pools; both operands
+// are the caller's image-aligned tile images, so the scratch is the per-(pair, line) argmin slots (not needed with
+// key-line merging, whose decisions run on dist_key).
+static MatchPlan plan_match(const LtrMatchInput& in, const LtrPairIndex* ix, char* base) {
   MatchPlan pl{};
   const int P = in.n_pairs;
   const int n[2] = {in.n0, in.n1};
   const int mxn[2] = {in.max_n0, in.max_n1};
-  const int tot[2] = {in.total_n0, in.total_n1};
-  const void* tiles[2] = {in.tiles0, in.tiles1};
-  const int tl[2] = {in.tiles_lines0, in.tiles_lines1};
+  const int tot[2] = {ix ? ix->total_out0 : in.total_n0, ix ? ix->total_out1 : in.total_n1};
+  const void* tiles[2] = {ix ? ix->tiles0 : in.tiles0, ix ? ix->tiles1 : in.tiles1};
+  const int64_t tl[2] = {ix ? (int64_t)ix->n_tiles0 * 128 : in.tiles_lines0,
+                         ix ? (int64_t)ix->n_tiles1 * 128 : in.tiles_lines1};
   const int tr0[2] = {in.tiles_row0_0, in.tiles_row0_1};
   const bool varlen = in.cu0 != nullptr;
+  const bool slots = !ix || in.sub_off0 == nullptr;
   int64_t off = 0;
   auto take = [&](int64_t bytes) {
     char* p = base + off;
@@ -726,8 +732,8 @@ static MatchPlan plan_match(const LtrMatchInput& in, char* base) {
     pl.mx[s] = varlen ? mxn[s] : n[s];
     pl.tmax[s] = cdiv(pl.mx[s], 128);
     pl.total[s] = varlen ? tot[s] : P * n[s];
-    pl.direct[s] = tiles[s] && !varlen && in.dist_mode == 0 && n[s] % 128 == 0 && tr0[s] % 128 == 0 && tr0[s] >= 0 &&
-                   (int64_t)tr0[s] + (int64_t)P * n[s] <= align_up(tl[s], 128);
+    pl.direct[s] = ix || (tiles[s] && !varlen && in.dist_mode == 0 && n[s] % 128 == 0 && tr0[s] % 128 == 0 && tr0[s] >= 0 &&
+                          (int64_t)tr0[s] + (int64_t)P * n[s] <= align_up(tl[s], 128));
     if (pl.direct[s]) {
       pl.img[s] = tiles_image(const_cast<void*>(tiles[s]), tl[s]);
     } else {
@@ -736,37 +742,8 @@ static MatchPlan plan_match(const LtrMatchInput& in, char* base) {
       pl.img[s].lo = reinterpret_cast<__nv_bfloat16*>(take(plane * 2));
       pl.img[s].kblocks = MT_KB;
     }
-    pl.slot[s] = reinterpret_cast<uint2*>(take((int64_t)std::max(pl.total[s], 1) * 8));
-    pl.sq[s] = in.dist_mode == 1 ? reinterpret_cast<float*>(take((int64_t)std::max(pl.total[s], 1) * 4)) : nullptr;
-  }
-  pl.done = reinterpret_cast<int*>(take(256));
-  pl.bytes = off;
-  return pl;
-}
-
-// Pair lists over image pools: both operands are the caller's image-aligned tile images, so the scratch is the
-// per-(pair, line) argmin slots (not needed with key-line merging, whose decisions run on dist_key).
-static MatchPlan plan_match_indexed(const LtrMatchInput& in, const LtrPairIndex& ix, char* base) {
-  MatchPlan pl{};
-  const int mxn[2] = {in.max_n0, in.max_n1};
-  const int tot[2] = {ix.total_out0, ix.total_out1};
-  const int ntiles[2] = {ix.n_tiles0, ix.n_tiles1};
-  const void* tiles[2] = {ix.tiles0, ix.tiles1};
-  const bool seg = in.sub_off0 != nullptr;
-  int64_t off = 0;
-  auto take = [&](int64_t bytes) {
-    char* p = base + off;
-    off = align_up(off + bytes, 1024);
-    return p;
-  };
-  for (int s = 0; s < 2; ++s) {
-    pl.mx[s] = mxn[s];
-    pl.tmax[s] = cdiv(pl.mx[s], 128);
-    pl.total[s] = tot[s];
-    pl.direct[s] = true;
-    pl.img[s] = tiles_image(const_cast<void*>(tiles[s]), (int64_t)ntiles[s] * 128);
-    pl.slot[s] = seg ? nullptr : reinterpret_cast<uint2*>(take((int64_t)std::max(tot[s], 1) * 8));
-    pl.sq[s] = nullptr;
+    pl.slot[s] = slots ? reinterpret_cast<uint2*>(take((int64_t)std::max(pl.total[s], 1) * 8)) : nullptr;
+    pl.sq[s] = !ix && in.dist_mode == 1 ? reinterpret_cast<float*>(take((int64_t)std::max(pl.total[s], 1) * 4)) : nullptr;
   }
   pl.done = reinterpret_cast<int*>(take(256));
   pl.bytes = off;
@@ -869,26 +846,88 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
   return 0;
 }
 
+static int launch_segmean(const SegMeanArgs& a, int max_k0, int max_k1, int n_pairs, cudaStream_t s) {
+  LaunchScope ls(KC_SEGMEAN, s);
+  segmean_kernel<<<dim3(cdiv(max_k1, 32), cdiv(max_k0, 8), n_pairs), 256, 0, s>>>(a);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
+// the output checks both matcher entries share; `who` (the entry's name) prefixes the message
+static int check_match_output(const char* who, const LtrMatchInput& in, const LtrMatchOutput& out) {
+  const std::string w(who);
+  if (out.matches0 && (!out.scores0 || !out.nn1 || !out.counts))
+    return set_error(LTR_E_INVALID, w + ": matches0 needs scores0, nn1 and counts");
+  if (!out.matches0 && !out.dist_key) return set_error(LTR_E_INVALID, w + ": nothing to compute (matches0 and dist_key are NULL)");
+  if (in.sub_off0 && (!out.dist_sub || !out.dist_key)) return set_error(LTR_E_INVALID, w + ": keyline merging needs dist_sub and dist_key");
+  return LTR_OK;
+}
+
+// Everything after an entry's own checks: the match of a batch of pairs (ix == nullptr, ltr_match) or of a pair list
+// over two image pools (ltr_match_indexed).  d != 256 (ltr_match only) runs the fp32 FMA distance tiles instead of the
+// tensor-core matcher.  `who` prefixes every error message.
+static int run_match(const char* who, const LtrMatchInput& in, const LtrPairIndex* ix, const LtrMatchOutput& out,
+                     int32_t device, void* stream) {
+  const bool seg = in.sub_off0 != nullptr;
+  const int mx0 = in.cu0 ? in.max_n0 : in.n0, mx1 = in.cu1 ? in.max_n1 : in.n1;
+  const int mk0 = seg ? in.max_k0 : mx0, mk1 = seg ? in.max_k1 : mx1;
+  const long long stride_key = in.dist_pair_stride > 0 ? in.dist_pair_stride : (long long)mk0 * mk1;
+  const bool null_desc = mx0 > 0 && mx1 > 0 && (!in.desc0 || !in.desc1);
+  // a pair list is refused before any CUDA call; ltr_match selects its device first
+  if (ix && null_desc) return set_error(LTR_E_INVALID, std::string(who) + ": null descriptors");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  if (null_desc) return set_error(LTR_E_INVALID, std::string(who) + ": null descriptors");
+  cudaStream_t s = as_stream(stream);
+  if (in.d == MT_D) {
+    char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(out.workspace), 1024));
+    MatchPlan pl = plan_match(in, ix, base);
+    if (!out.workspace || (base - (char*)out.workspace) + pl.bytes > out.workspace_bytes)
+      return set_error(LTR_E_WORKSPACE, std::string(who) + ": workspace too small, need " + std::to_string(pl.bytes + 1024));
+    LTR_TRY(run_match_tc(in, out, pl, seg, stride_key, s, ix));
+    if (!seg) return LTR_OK;
+  } else if (mx0 > 0 && mx1 > 0) {
+    // generic descriptor dimension: fp32 FMA distance tiles
+    DistArgs da{};
+    da.d0 = in.desc0; da.d1 = in.desc1; da.layout = in.layout; da.d = in.d;
+    da.cu0 = in.cu0; da.cu1 = in.cu1; da.n0 = in.n0; da.n1 = in.n1;
+    da.out = seg ? out.dist_sub : out.dist_key;
+    da.stride = seg ? (long long)mx0 * mx1 : stride_key;
+    dim3 grid(cdiv(mx0, DK_BM), cdiv(mx1, DK_BN), in.n_pairs);
+    LaunchScope ls(KC_DIST, s);
+    if (in.layout == LTR_LAYOUT_CHANNEL_FIRST) LTR_CUDA_TRY(launch_pdl(dist_kernel<true>, grid, dim3(DK_THREADS), 0, s, da));
+    else LTR_CUDA_TRY(launch_pdl(dist_kernel<false>, grid, dim3(DK_THREADS), 0, s, da));
+  }
+  if (seg && mx0 > 0 && mx1 > 0 && mk0 > 0 && mk1 > 0)
+    LTR_TRY(launch_segmean({out.dist_sub, (long long)mx0 * mx1, out.dist_key, stride_key, in.cuk0, in.cuk1, in.sub_off0,
+                            in.sub_off1, ix ? ix->img0 : nullptr, ix ? ix->img1 : nullptr},
+                           mk0, mk1, in.n_pairs, s));
+  if (!out.matches0) return LTR_OK;
+  // a pair list's per-pair output offsets play the role cuk0/cuk1 play for a batch: the NN kernels need no indirection
+  NNArgs na{};
+  na.dist = out.dist_key; na.stride = stride_key;
+  na.cuk0 = ix ? ix->out_off0 : seg ? in.cuk0 : in.cu0; na.cuk1 = ix ? ix->out_off1 : seg ? in.cuk1 : in.cu1;
+  na.n0 = in.n0; na.n1 = in.n1; na.thr = in.nn_thresh; na.mutual = in.mutual;
+  na.matches0 = out.matches0; na.scores0 = out.scores0; na.nn1 = out.nn1; na.counts = out.counts;
+  return run_nn(na, in.n_pairs, mk0, mk1, s);
+}
+
 extern "C" {
 
 int64_t ltr_match_workspace_bytes(const LtrMatchInput* in) {
   if (!in) return set_error(LTR_E_INVALID, "ltr_match_workspace_bytes: null argument");
   if (const char* e = check_match_input(in)) return set_error(match_input_code(in), e);
   if (in->n_pairs <= 0 || in->d != MT_D) return 0;
-  return plan_match(*in, nullptr).bytes + 1024;
+  return plan_match(*in, nullptr, nullptr).bytes + 1024;
 }
 
 int ltr_match(const LtrMatchInput* in, const LtrMatchOutput* out, int32_t device, void* stream) {
   if (!in || !out) return set_error(LTR_E_INVALID, "ltr_match: null argument");
   if (in->n_pairs <= 0) return LTR_OK;
   if (const char* e = check_match_input(in)) return set_error(match_input_code(in), e);
+  LTR_TRY(check_match_output("ltr_match", *in, *out));
   const bool seg = in->sub_off0 != nullptr;
   const bool tc = in->d == MT_D;
   const bool want_nn = out->matches0 != nullptr;
-  if (want_nn && (!out->scores0 || !out->nn1 || !out->counts))
-    return set_error(LTR_E_INVALID, "ltr_match: matches0 needs scores0, nn1 and counts");
-  if (!want_nn && !out->dist_key) return set_error(LTR_E_INVALID, "ltr_match: nothing to compute (matches0 and dist_key are NULL)");
-  if (seg && (!out->dist_sub || !out->dist_key)) return set_error(LTR_E_INVALID, "ltr_match: keyline merging needs dist_sub and dist_key");
   if (out->gather && out->gather->world > 1) {
     const LtrPeerGather& g = *out->gather;
     if (seg || !tc || !want_nn) return set_error(LTR_E_UNSUPPORTED, "ltr_match: gather needs d == 256, no keyline merging, matches0");
@@ -897,44 +936,7 @@ int ltr_match(const LtrMatchInput* in, const LtrMatchOutput* out, int32_t device
     if ((in->cu0 ? in->max_n0 : in->n0) <= 0) return set_error(LTR_E_UNSUPPORTED, "ltr_match: gather needs a non-empty side 0");
   }
   if (!tc && !out->dist_key) return set_error(LTR_E_INVALID, "ltr_match: dist_key is required when d != 256");
-  LTR_CUDA_TRY(cudaSetDevice(device));
-  cudaStream_t s = as_stream(stream);
-  const int mx0 = in->cu0 ? in->max_n0 : in->n0, mx1 = in->cu1 ? in->max_n1 : in->n1;
-  const int mk0 = seg ? in->max_k0 : mx0, mk1 = seg ? in->max_k1 : mx1;
-  const long long stride_key = in->dist_pair_stride > 0 ? in->dist_pair_stride : (long long)mk0 * mk1;
-  if (mx0 > 0 && mx1 > 0 && (!in->desc0 || !in->desc1)) return set_error(LTR_E_INVALID, "ltr_match: null descriptors");
-  if (tc) {
-    char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(out->workspace), 1024));
-    MatchPlan pl = plan_match(*in, base);
-    if (pl.bytes > 0 && (!out->workspace || (base - (char*)out->workspace) + pl.bytes > out->workspace_bytes))
-      return set_error(LTR_E_WORKSPACE, "ltr_match: workspace too small, need " + std::to_string(pl.bytes + 1024));
-    LTR_TRY(run_match_tc(*in, *out, pl, seg, stride_key, s));
-    if (!seg) return LTR_OK;
-  } else if (mx0 > 0 && mx1 > 0) {
-    // generic descriptor dimension: fp32 FMA distance tiles
-    DistArgs da{};
-    da.d0 = in->desc0; da.d1 = in->desc1; da.layout = in->layout; da.d = in->d;
-    da.cu0 = in->cu0; da.cu1 = in->cu1; da.n0 = in->n0; da.n1 = in->n1;
-    da.out = seg ? out->dist_sub : out->dist_key;
-    da.stride = seg ? (long long)mx0 * mx1 : stride_key;
-    dim3 grid(cdiv(mx0, DK_BM), cdiv(mx1, DK_BN), in->n_pairs);
-    LaunchScope ls(KC_DIST, s);
-    if (in->layout == LTR_LAYOUT_CHANNEL_FIRST) LTR_CUDA_TRY(launch_pdl(dist_kernel<true>, grid, dim3(DK_THREADS), 0, s, da));
-    else LTR_CUDA_TRY(launch_pdl(dist_kernel<false>, grid, dim3(DK_THREADS), 0, s, da));
-  }
-  if (seg && mx0 > 0 && mx1 > 0 && mk0 > 0 && mk1 > 0) {
-    SegMeanArgs sa{out->dist_sub, (long long)mx0 * mx1, out->dist_key, stride_key, in->cuk0, in->cuk1, in->sub_off0, in->sub_off1};
-    LaunchScope ls(KC_SEGMEAN, s);
-    segmean_kernel<<<dim3(cdiv(mk1, 32), cdiv(mk0, 8), in->n_pairs), 256, 0, s>>>(sa);
-    LTR_CUDA_TRY(cudaGetLastError());
-  }
-  if (!want_nn) return LTR_OK;
-  NNArgs na{};
-  na.dist = out->dist_key; na.stride = stride_key;
-  na.cuk0 = seg ? in->cuk0 : in->cu0; na.cuk1 = seg ? in->cuk1 : in->cu1;
-  na.n0 = in->n0; na.n1 = in->n1; na.thr = in->nn_thresh; na.mutual = in->mutual;
-  na.matches0 = out->matches0; na.scores0 = out->scores0; na.nn1 = out->nn1; na.counts = out->counts;
-  return run_nn(na, in->n_pairs, mk0, mk1, s);
+  return run_match("ltr_match", *in, nullptr, *out, device, stream);
 }
 
 int64_t ltr_image_tiles_bytes(int32_t n_images, const int32_t* cu_host) {
@@ -984,7 +986,7 @@ int64_t ltr_match_indexed_workspace_bytes(const LtrMatchInput* in, const LtrPair
   if (!in || !idx) return set_error(LTR_E_INVALID, "ltr_match_indexed_workspace_bytes: null argument");
   if (const char* e = check_match_indexed(in, idx)) return set_error(LTR_E_INVALID, e);
   if (in->n_pairs <= 0) return 0;
-  return plan_match_indexed(*in, *idx, nullptr).bytes + 1024;
+  return plan_match(*in, idx, nullptr).bytes + 1024;
 }
 
 int ltr_match_indexed(const LtrMatchInput* in, const LtrPairIndex* idx, const LtrMatchOutput* out, int32_t device, void* stream) {
@@ -994,39 +996,8 @@ int ltr_match_indexed(const LtrMatchInput* in, const LtrPairIndex* idx, const Lt
   if (out->gather && out->gather->world > 1) return set_error(LTR_E_UNSUPPORTED, "ltr_match_indexed: gather is not supported");
   if (in->n_pairs <= 0) return LTR_OK;
   if (const char* e = check_match_indexed(in, idx)) return set_error(LTR_E_INVALID, e);
-  const bool seg = in->sub_off0 != nullptr;
-  const bool want_nn = out->matches0 != nullptr;
-  if (want_nn && (!out->scores0 || !out->nn1 || !out->counts))
-    return set_error(LTR_E_INVALID, "ltr_match_indexed: matches0 needs scores0, nn1 and counts");
-  if (!want_nn && !out->dist_key) return set_error(LTR_E_INVALID, "ltr_match_indexed: nothing to compute (matches0 and dist_key are NULL)");
-  if (seg && (!out->dist_sub || !out->dist_key)) return set_error(LTR_E_INVALID, "ltr_match_indexed: keyline merging needs dist_sub and dist_key");
-  const int mx0 = in->max_n0, mx1 = in->max_n1;
-  const int mk0 = seg ? in->max_k0 : mx0, mk1 = seg ? in->max_k1 : mx1;
-  const long long stride_key = in->dist_pair_stride > 0 ? in->dist_pair_stride : (long long)mk0 * mk1;
-  if (mx0 > 0 && mx1 > 0 && (!in->desc0 || !in->desc1)) return set_error(LTR_E_INVALID, "ltr_match_indexed: null descriptors");
-  LTR_CUDA_TRY(cudaSetDevice(device));
-  cudaStream_t s = as_stream(stream);
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(out->workspace), 1024));
-  MatchPlan pl = plan_match_indexed(*in, *idx, base);
-  if (!out->workspace || (base - (char*)out->workspace) + pl.bytes > out->workspace_bytes)
-    return set_error(LTR_E_WORKSPACE, "ltr_match_indexed: workspace too small, need " + std::to_string(pl.bytes + 1024));
-  LTR_TRY(run_match_tc(*in, *out, pl, seg, stride_key, s, idx));
-  if (!seg) return LTR_OK;
-  if (mx0 > 0 && mx1 > 0 && mk0 > 0 && mk1 > 0) {
-    SegMeanArgs sa{out->dist_sub, (long long)mx0 * mx1, out->dist_key, stride_key, in->cuk0, in->cuk1, in->sub_off0, in->sub_off1,
-                   idx->img0, idx->img1};
-    LaunchScope ls(KC_SEGMEAN, s);
-    segmean_kernel<<<dim3(cdiv(mk1, 32), cdiv(mk0, 8), in->n_pairs), 256, 0, s>>>(sa);
-    LTR_CUDA_TRY(cudaGetLastError());
-  }
-  if (!want_nn) return LTR_OK;
-  // the per-pair output offsets play the role cuk0/cuk1 play in ltr_match: the NN kernels need no indirection
-  NNArgs na{};
-  na.dist = out->dist_key; na.stride = stride_key;
-  na.cuk0 = idx->out_off0; na.cuk1 = idx->out_off1;
-  na.thr = in->nn_thresh; na.mutual = in->mutual;
-  na.matches0 = out->matches0; na.scores0 = out->scores0; na.nn1 = out->nn1; na.counts = out->counts;
-  return run_nn(na, in->n_pairs, mk0, mk1, s);
+  LTR_TRY(check_match_output("ltr_match_indexed", *in, *out));
+  return run_match("ltr_match_indexed", *in, idx, *out, device, stream);
 }
 
 int ltr_gather_wait(const void* local_base, int32_t world, int32_t n_pairs, int32_t slot, int32_t epoch, int32_t* out,
@@ -1062,12 +1033,8 @@ int ltr_merge_sublines(const float* dist_sub, int64_t stride_sub, int32_t n_pair
   if (!dist_sub || !cuk0 || !cuk1 || !sub_off0 || !sub_off1 || !dist_key)
     return set_error(LTR_E_INVALID, "ltr_merge_sublines: null argument");
   LTR_CUDA_TRY(cudaSetDevice(device));
-  cudaStream_t s = as_stream(stream);
-  SegMeanArgs sa{dist_sub, stride_sub, dist_key, stride_key, cuk0, cuk1, sub_off0, sub_off1};
-  LaunchScope ls(KC_SEGMEAN, s);
-  segmean_kernel<<<dim3(cdiv(max_k1, 32), cdiv(max_k0, 8), n_pairs), 256, 0, s>>>(sa);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch_segmean({dist_sub, stride_sub, dist_key, stride_key, cuk0, cuk1, sub_off0, sub_off1}, max_k0, max_k1, n_pairs,
+                        as_stream(stream));
 }
 
 int ltr_tokenize(const LtrTokenizeInput* in, float* sublines, float* pnt, float* mask, float* resp, float* angle,

@@ -26,6 +26,12 @@ from . import line_process as LP
 _KEYS = ("sublines", "resp_sublines", "angle_sublines", "pnt_sublines", "desc_sublines", "score_sublines")
 
 
+def _uniform(cu) -> Optional[int]:
+    """The line count of every image of line offsets `cu` when they all have the same, else None."""
+    d = np.diff(cu)
+    return int(d[0]) if len(d) and bool((d == d[0]).all()) else None
+
+
 @dataclass
 class LineBatch:
     """Tokenised lines of a batch of images, rows of all images concatenated.
@@ -60,8 +66,7 @@ class LineBatch:
 
     @property
     def uniform_lines(self) -> Optional[int]:
-        d = np.diff(self.cu_lines)
-        return int(d[0]) if len(d) and bool((d == d[0]).all()) else None
+        return _uniform(self.cu_lines)
 
     def nbytes(self) -> int:
         return sum(t.numel() * t.element_size() for t in self.tensors())
@@ -115,9 +120,13 @@ class LineBatch:
                          self.sub_off, self.cuk)
 
     def dev_i32(self, name: str, device) -> torch.Tensor:
-        key = (name, str(device))
+        return self._dev_i32((name,), getattr(self, name), device)
+
+    def _dev_i32(self, key: tuple, a: np.ndarray, device) -> torch.Tensor:
+        """Device int32 copy of a host array of this batch, made once per key and device."""
+        key = key + (str(device),)
         if key not in self._dev_cache:
-            self._dev_cache[key] = torch.from_numpy(np.ascontiguousarray(getattr(self, name), dtype=np.int32)).to(device)
+            self._dev_cache[key] = torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(device)
         return self._dev_cache[key]
 
 
@@ -299,6 +308,27 @@ def plan_chunks(n0, n1, cap_bytes: Optional[int] = None, max_pairs: int = MAX_PA
     return chunks
 
 
+def _side(batch: LineBatch, a: int, b: int, split: bool) -> dict:
+    """Images [a, b) of `batch` as one side of a batch of pairs, in the side's own line numbering (host arrays): line
+    offsets 'cu' and, when `split` (some key line of the match is cut into sublines), key-line offsets 'cuk' and the
+    key-line CSR 'sub_off', the identity for a batch without split key lines."""
+    cu = batch.cu_lines
+    side = dict(cu=cu[a:b + 1] - cu[a])
+    if split and batch.sub_off is None:
+        side.update(cuk=side["cu"], sub_off=np.arange(cu[b] - cu[a] + 1))
+    elif split:
+        ck = batch.cuk
+        side.update(cuk=ck[a:b + 1] - ck[a], sub_off=batch.sub_off[ck[a]:ck[b] + 1] - cu[a])
+    return side
+
+
+def _tiled(s0: dict, s1: dict) -> bool:
+    """Whether the encoder's final GEMM can write the matcher's operand tiles itself: no key-line merging and, on each
+    side, every image with the same positive multiple of 128 lines."""
+    uniform = (_uniform(s0["cu"]), _uniform(s1["cu"]))
+    return "sub_off" not in s0 and all(L is not None and L > 0 and L % 128 == 0 for L in uniform)
+
+
 class PairEngine:
     """Batched line-descriptor forward + mutual-NN matching on one GPU."""
 
@@ -331,98 +361,67 @@ class PairEngine:
         epilogue of the tensor-core contraction) unless key-line merging needs them."""
         if side0.n_images != side1.n_images:
             raise ValueError("match_pairs: both sides need the same number of images")
-        if nn_thresh is None:
-            nn_thresh = self.model.config.get("nn_threshold", 0.8)
         P = side0.n_images
-        seg = side0.sub_off is not None or side1.sub_off is not None
-        L0, L1 = side0.uniform_lines, side1.uniform_lines
-        tiled = not seg and L0 is not None and L1 is not None and L0 % 128 == 0 and L1 % 128 == 0 and L0 > 0 and L1 > 0
-        if tiled:
+        split = side0.sub_off is not None or side1.sub_off is not None
+        s0, s1 = _side(side0, 0, P, split), _side(side1, 0, P, split)
+        if _tiled(s0, s1):
             d0, t0 = self.encode(side0, want_tiles=True)
             d1, t1 = self.encode(side1, want_tiles=True)
+            tiles = dict(tiles0=t0, tiles1=t1, tiles_lines=(side0.n_lines, side1.n_lines), tiles_row0=(0, 0))
         else:
-            d0 = self.encode(side0)
-            d1 = self.encode(side1)
-        kw = {}
-        if seg:
-            def csr(b):
-                if b.sub_off is None:  # identity on this side
-                    b.sub_off = np.arange(b.n_lines + 1, dtype=np.int32)
-                    b.cuk = b.cu_lines.copy()
-                return b.dev_i32("sub_off", self.device), b.dev_i32("cuk", self.device)
-            so0, ck0 = csr(side0)
-            so1, ck1 = csr(side1)
-            kw = dict(cu0=side0.dev_i32("cu_lines", self.device), cu1=side1.dev_i32("cu_lines", self.device),
-                      max_n0=int(np.diff(side0.cu_lines).max(initial=0)), max_n1=int(np.diff(side1.cu_lines).max(initial=0)),
-                      sub_off0=so0, sub_off1=so1, cuk0=ck0, cuk1=ck1,
-                      max_k0=int(np.diff(side0.cuk).max(initial=0)), max_k1=int(np.diff(side1.cuk).max(initial=0)),
-                      total_k0=int(side0.cuk[-1]), total_k1=int(side1.cuk[-1]))
-            off0 = side0.cuk
-        elif L0 is not None and L1 is not None:
-            kw = dict(n0=L0, n1=L1)
-            if tiled:
-                kw.update(tiles0=t0, tiles1=t1, tiles_lines=(side0.n_lines, side1.n_lines), tiles_row0=(0, 0))
-            off0 = side0.cu_lines
-        else:
-            kw = dict(cu0=side0.dev_i32("cu_lines", self.device), cu1=side1.dev_i32("cu_lines", self.device),
-                      max_n0=int(np.diff(side0.cu_lines).max(initial=0)), max_n1=int(np.diff(side1.cu_lines).max(initial=0)),
-                      total_k0=side0.n_lines, total_k1=side1.n_lines)
-            off0 = side0.cu_lines
-        out = _ops.match_descriptors(d0, d1, N.LAYOUT_ROWS, P, float(nn_thresh), mutual, want_dist=want_dist,
-                                     gather=gather, **kw)
-        return PairMatches(out["matches0"], out["scores0"], out["counts"], np.asarray(off0, dtype=np.int32),
-                           out["dist_key"], out["stride"], d0 if keep_desc else None, d1 if keep_desc else None)
-
+            d0, d1, tiles = self.encode(side0), self.encode(side1), {}
+        dev = lambda s, k: (side0, side1)[s]._dev_i32(("match_side", 0, P, k), (s0, s1)[s][k], self.device)
+        return self._match_sides(d0, d1, s0, s1, dev, tiles, nn_thresh, mutual, keep_desc, want_dist, gather)
 
     def match_packed(self, batch: LineBatch, n_pairs: int, nn_thresh: Optional[float] = None, mutual=True,
                      keep_desc=False, want_dist=False, gather=None) -> PairMatches:
         """Same as match_pairs for a batch that holds BOTH sides: images [0, P) are the side-0
         images of the P pairs, images [P, 2P) their side-1 partners.  One `ltr_encode` over all
         2P images (twice the rows per GEMM launch) and one `ltr_match`."""
+        return self._match_packed(batch, n_pairs, nn_thresh, mutual, keep_desc, want_dist, gather)
+
+    def _match_packed(self, batch: LineBatch, n_pairs: int, nn_thresh, mutual=True, keep_desc=False, want_dist=False,
+                      gather=None, staged: Optional[dict] = None) -> PairMatches:
+        """match_packed.  staged: device copies the caller has already made of the sides' offsets, by matcher keyword
+        (cu0, cu1 and, with split key lines, cuk0, cuk1, sub_off0, sub_off1)."""
         P = int(n_pairs)
         if batch.n_images != 2 * P:
             raise ValueError("match_packed: batch must hold 2 * n_pairs images")
+        split = batch.sub_off is not None
+        s0, s1 = _side(batch, 0, P, split), _side(batch, P, 2 * P, split)
+        R0 = int(batch.cu_lines[P])
+        if _tiled(s0, s1):
+            rows, t = self.encode(batch, want_tiles=True)
+            tiles = dict(tiles0=t, tiles1=t, tiles_lines=(batch.n_lines, batch.n_lines), tiles_row0=(0, R0))
+        else:
+            rows, tiles = self.encode(batch), {}
+        if staged is not None:
+            dev = lambda s, k: staged[f"{k}{s}"]
+        else:
+            dev = lambda s, k: batch._dev_i32(("match_side", s * P, s * P + P, k), (s0, s1)[s][k], self.device)
+        return self._match_sides(rows[:R0], rows[R0:], s0, s1, dev, tiles, nn_thresh, mutual, keep_desc, want_dist,
+                                 gather)
+
+    def _match_sides(self, d0, d1, s0: dict, s1: dict, dev, tiles: dict, nn_thresh, mutual, keep_desc, want_dist,
+                     gather) -> PairMatches:
+        """One `ltr_match` of the pairs whose side 0 / side 1 are `s0` / `s1` (`_side`), descriptor rows d0 / d1.
+        dev(s, name): the device copy of array `name` of side s, asked for only when a side is ragged or key lines
+        are merged; tiles: the encoder's operand tiles (matcher keywords), used only when both sides are uniform."""
         if nn_thresh is None:
             nn_thresh = self.model.config.get("nn_threshold", 0.8)
-        cu = batch.cu_lines
-        R0 = int(cu[P])
-        L = batch.uniform_lines
-        # uniform 128-aligned images: the encoder's final GEMM writes the matcher's operand tiles itself
-        tiled = batch.sub_off is None and L is not None and L > 0 and L % 128 == 0
-        if tiled:
-            rows, tiles = self.encode(batch, want_tiles=True)
+        L0, L1 = _uniform(s0["cu"]), _uniform(s1["cu"])
+        if "sub_off" not in s0 and L0 is not None and L1 is not None:
+            kw = dict(n0=L0, n1=L1, **tiles)
         else:
-            rows = self.encode(batch)
-        d0, d1 = rows[:R0], rows[R0:]
-        if batch.sub_off is not None:
-            key = ("packed_split", str(self.device))
-            if key not in batch._dev_cache:
-                K0 = int(batch.cuk[P])
-                t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(self.device)
-                batch._dev_cache[key] = dict(
-                    cu0=t(cu[:P + 1]), cu1=t(cu[P:] - cu[P]), cuk0=t(batch.cuk[:P + 1]), cuk1=t(batch.cuk[P:] - K0),
-                    sub_off0=t(batch.sub_off[:K0 + 1]), sub_off1=t(batch.sub_off[K0:] - R0),
-                    max_n0=int(np.diff(cu[:P + 1]).max(initial=0)), max_n1=int(np.diff(cu[P:]).max(initial=0)),
-                    max_k0=int(np.diff(batch.cuk[:P + 1]).max(initial=0)), max_k1=int(np.diff(batch.cuk[P:]).max(initial=0)),
-                    total_k0=K0, total_k1=int(batch.cuk[-1]) - K0)
-            kw = batch._dev_cache[key]
-            off0 = batch.cuk[:P + 1]
-        elif L is not None:
-            kw = dict(n0=L, n1=L)
-            if tiled:
-                kw.update(tiles0=tiles, tiles1=tiles, tiles_lines=(batch.n_lines, batch.n_lines), tiles_row0=(0, R0))
-            off0 = cu[:P + 1]
-        else:
-            key = ("packed_split", str(self.device))
-            if key not in batch._dev_cache:
-                t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.int32)).to(self.device)
-                batch._dev_cache[key] = dict(cu0=t(cu[:P + 1]), cu1=t(cu[P:] - cu[P]),
-                                             max_n0=int(np.diff(cu[:P + 1]).max(initial=0)),
-                                             max_n1=int(np.diff(cu[P:]).max(initial=0)),
-                                             total_k0=R0, total_k1=int(cu[-1]) - R0)
-            kw = batch._dev_cache[key]
-            off0 = cu[:P + 1]
-        out = _ops.match_descriptors(d0, d1, N.LAYOUT_ROWS, P, float(nn_thresh), mutual, want_dist=want_dist,
+            mx = lambda a: int(np.diff(a).max(initial=0))
+            kw = {}
+            for s, side in enumerate((s0, s1)):
+                kw.update({f"{k}{s}": dev(s, k) for k in side})
+                kw.update({f"max_n{s}": mx(side["cu"]), f"total_k{s}": int(side.get("cuk", side["cu"])[-1])})
+                if "cuk" in side:
+                    kw[f"max_k{s}"] = mx(side["cuk"])
+        off0 = s0.get("cuk", s0["cu"])
+        out = _ops.match_descriptors(d0, d1, N.LAYOUT_ROWS, len(off0) - 1, float(nn_thresh), mutual, want_dist=want_dist,
                                      gather=gather, **kw)
         return PairMatches(out["matches0"], out["scores0"], out["counts"], np.asarray(off0, dtype=np.int32),
                            out["dist_key"], out["stride"], d0 if keep_desc else None, d1 if keep_desc else None)
@@ -541,12 +540,6 @@ class PairEngine:
         dv = self._stage(arrays)
         batch = self._tokenize(host, images, dv)
         mx = lambda a: int(np.diff(a).max(initial=0))
-        split = dict(cu0=dv["cu0"], cu1=dv["cu1"], max_n0=mx(cu[:P + 1]), max_n1=mx(cu[P:]), total_k0=K0,
-                     total_k1=int(cuk[-1]) - K0)
-        if host.split:
-            split.update(cuk0=dv["cuk0"], cuk1=dv["cuk1"], sub_off0=dv["sub_off0"], sub_off1=dv["sub_off1"],
-                         max_k0=mx(cuk[:P + 1]), max_k1=mx(cuk[P:]))
-        batch._dev_cache[("packed_split", str(self.device))] = split
         i32d = dict(dtype=torch.int32, device=self.device)
         f32d = dict(dtype=torch.float32, device=self.device)
 
@@ -555,7 +548,7 @@ class PairEngine:
                     torch.zeros(P, **i32d), torch.empty(0, **f32d) if want_scores else None, 0)
 
         if K0 > 0 and int(cuk[-1]) > K0:
-            lm = self.match_packed(batch, P, line_thresh, want_dist=want_scores)
+            lm = self._match_packed(batch, P, line_thresh, want_dist=want_scores, staged=dv)
             lines = (lm.matches0, lm.scores0, lm.counts, lm.dist, lm.stride)
         else:
             lines = unmatched(K0)

@@ -301,16 +301,24 @@ def test_pair_batch_with_keyline_merging_vs_oracle():
         K0, K1 = dk.shape[1:]
         got = res.dist[p * res.stride:p * res.stride + K0 * K1].view(K0, K1).cpu().numpy()
         assert np.abs(got - dk[0]).max() < 1e-3
+    # key lines split on side 0 only: side 1 keeps one subline per key line, and its batch is left as it was
+    plain = [dict(b, mat_klines2sublines=np.eye(b["desc_sublines"].shape[1], dtype=np.float32)[None]) for _, b in pairs]
+    side1 = engine.LineBatch.from_images(plain).to(DEV)
+    res = eng.match_pairs(engine.LineBatch.from_images([a for a, _ in pairs]).to(DEV), side1, 0.8)
+    assert side1.sub_off is None and side1.cuk is None
+    for p, (a, _) in enumerate(pairs):
+        mat, _, _, _ = orc.match_pair(sd, a, plain[p], 0.8)
+        assert np.array_equal(res.pair(p).cpu().numpy(), orc.match_indices(mat)), f"pair {p}, side 1 not split"
 
 
 def test_match_packed_equals_match_pairs():
     model, sd = model_for("synthetic:0:1")
     eng = engine.PairEngine(model, DEV)
-    for uniform in (True, False):
+    # uniform, ragged, each side uniform with its own line count, and the same with 128-aligned counts (operand tiles)
+    for sizes in ([(40, 40)] * 3, [(20 + 7 * p, 20 + 6 * p) for p in range(3)], [(40, 37)] * 3, [(256, 128)] * 3):
         pairs = []
-        for p in range(3):
-            L = 40 if uniform else 20 + 7 * p
-            a, b, _ = syn.make_pair_inputs(400 + p, L, 21, n_lines1=L if uniform else L - p)
+        for p, (L0, L1) in enumerate(sizes):
+            a, b, _ = syn.make_pair_inputs(400 + p, L0, 21, n_lines1=L1)
             pairs.append((a, b))
         r1 = eng.match_pairs(engine.LineBatch.from_images([a for a, _ in pairs]).to(DEV),
                              engine.LineBatch.from_images([b for _, b in pairs]).to(DEV), 0.8)
