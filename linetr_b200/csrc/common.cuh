@@ -37,6 +37,7 @@ enum KernelClass : int {
   KC_TOKENIZE,
   KC_DESC_TILES,
   KC_MATCH_TC,
+  KC_MATCH_EXACT,
   KC_MATCH_TAIL,
   KC_LINE_GT,
   KC_COUNT

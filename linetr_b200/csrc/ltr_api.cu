@@ -37,7 +37,7 @@ int set_error(int code, const std::string& msg) {
 const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
-                                         "tokenize", "desc_tiles", "match_tc", "match_tail", "line_gt"};
+                                         "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -820,11 +820,26 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
     LTR_CUDA_TRY(cudaMemsetAsync(out.counts, 0, sizeof(int) * P, s));
     LTR_CUDA_TRY(cudaMemsetAsync(pl.done, 0, sizeof(int), s));
   }
+  if (want_nn && pl.mx[0] > 0 && pl.mx[1] > 0) {
+    // exact fp32 re-check of the lines whose tensor-core result match_tc_kernel flagged, written back into their slots
+    MatchExactArgs xa{};
+    xa.d[0] = in.desc0; xa.d[1] = in.desc1; xa.layout = in.layout;
+    xa.cu[0] = in.cu0; xa.cu[1] = in.cu1; xa.n[0] = in.n0; xa.n[1] = in.n1;
+    xa.sq[0] = pl.sq[0]; xa.sq[1] = pl.sq[1]; xa.dist_mode = in.dist_mode;
+    xa.slot[0] = pl.slot[0]; xa.slot[1] = pl.slot[1];
+    xa.thr = in.nn_thresh; xa.mutual = in.mutual;
+    if (ix) {
+      xa.pimg[0] = ix->img0; xa.pimg[1] = ix->img1;
+      xa.out_off[0] = ix->out_off0; xa.out_off[1] = ix->out_off1;
+    }
+    const int windows = std::min(cdiv(std::max(pl.mx[0], in.mutual ? pl.mx[1] : 0), MX_WIN), 65535);
+    LTR_CUDA_TRY(ensure_dynamic_smem(match_exact_kernel, MX_SMEM));
+    LaunchScope ls(KC_MATCH_EXACT, s);
+    LTR_CUDA_TRY(launch_pdl(match_exact_kernel, dim3(P, 2, windows), dim3(256), (size_t)MX_SMEM, s, xa));
+  }
   if (want_nn && pl.mx[0] > 0) {
     MatchTailArgs ta{};
-    ta.d[0] = in.desc0; ta.d[1] = in.desc1; ta.layout = in.layout;
     ta.cu[0] = in.cu0; ta.cu[1] = in.cu1; ta.n[0] = in.n0; ta.n[1] = in.n1;
-    ta.sq[0] = pl.sq[0]; ta.sq[1] = pl.sq[1]; ta.dist_mode = in.dist_mode;
     ta.slot[0] = pl.slot[0]; ta.slot[1] = pl.slot[1];
     ta.thr = in.nn_thresh; ta.mutual = in.mutual;
     ta.matches0 = out.matches0; ta.scores0 = out.scores0; ta.nn1 = out.nn1; ta.counts = out.counts;
@@ -879,6 +894,9 @@ static int run_match(const char* who, const LtrMatchInput& in, const LtrPairInde
   if (null_desc) return set_error(LTR_E_INVALID, std::string(who) + ": null descriptors");
   cudaStream_t s = as_stream(stream);
   if (in.d == MT_D) {
+    // a slot keeps a line index in 30 bits (match_tc.cuh)
+    if (mx0 >= (1 << 30) || mx1 >= (1 << 30))
+      return set_error(LTR_E_INVALID, std::string(who) + ": a pair side has 2^30 lines or more");
     char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(out.workspace), 1024));
     MatchPlan pl = plan_match(in, ix, base);
     if (!out.workspace || (base - (char*)out.workspace) + pl.bytes > out.workspace_bytes)

@@ -1,8 +1,8 @@
 // Tensor-core descriptor matcher (K3): all-pairs distance D = 2 - 2 <a_i, b_j> on wgmma with the
 // row-argmin fused into the epilogue, for BOTH directions (side 0 rows vs side 1 and side 1 rows vs
-// side 0 - the second one is the column argmin the mutual check needs), a tail kernel that applies
-// threshold + mutual check + per-pair counts, and an exact fp32 re-check for decisions the
-// tensor-core arithmetic cannot make safely.
+// side 0 - the second one is the column argmin the mutual check needs), an exact fp32 re-check pass
+// (match_exact_kernel) for the decisions the tensor-core arithmetic cannot make safely, and a tail kernel
+// that applies threshold + mutual check + per-pair counts.
 //
 // Reference: get_dist_matrix (models/line_process.py:198-201: einsum('bdn,bdm->bnm'), (2 - 2 s).clip(0)),
 // nn_matcher / nn_matcher_distmat (models/nn_matcher.py:3-43: argmin axis 1, strict '<' threshold,
@@ -12,7 +12,7 @@
 // Precision contract.  The contraction is a 3-term split-bf16 product (hi*hi + lo*hi + hi*lo, fp32
 // accumulate in registers): ~1e-5 absolute on a distance of unit descriptors, growing with |a| |b|.  Match
 // indices must be bit-exact, so every row whose best and second-best distance are closer than a margin eps,
-// or whose best distance lies within eps of the threshold, is recomputed by the tail kernel with fp32 FMAs in
+// or whose best distance lies within eps of the threshold, is recomputed by match_exact_kernel with fp32 FMAs in
 // ascending k order (the arithmetic of the round-1 FFMA matcher the golden vectors were pinned with) before
 // any decision is taken.  Exact ties therefore resolve to the lowest index exactly as np.argmin does.
 // eps = MATCH_EPS in distance mode 0 (unit descriptors) and MATCH_EPS * max(1, |a_i| * max_j |b_j|) in mode 1
@@ -312,7 +312,7 @@ struct DescTilesArgs {
 };
 
 // Squared norm of one line for distance mode 1: a single ascending-k fmaf chain, s = fmaf(x_k, x_k, s) for
-// k = 0..255 - the order of exact_row's dot products, and the same in both descriptor layouts, so the same
+// k = 0..255 - the order of the exact pass's dot products, and the same in both descriptor layouts, so the same
 // descriptors get the same bits wherever they come from.  x_k is at x[k * stride].
 __device__ __forceinline__ float sq_chain(const float* __restrict__ x, size_t stride) {
   float s = 0.f;
@@ -379,12 +379,195 @@ __global__ void __launch_bounds__(256) desc_tiles_kernel(DescTilesArgs p) {
   }
 }
 
-// ---------------------------------------------------------------- tail: exact re-check, threshold, mutual, counts
-struct MatchTailArgs {
-  const float* d[2]; int layout;   // the fp32 descriptors the tiles were made from (exact re-check)
+// ---------------------------------------------------------------- exact re-check of the flagged lines
+// Slot word y after match_exact_kernel: bit 31 ambiguous (tensor-core result, not trusted), bit 30 decided exactly.
+// An exact slot holds the index in bits 0-29, all ones when no column had a distance below infinity (index
+// 0x7fffffff, as np.argmin never returns it); line counts per pair stay below 2^30 (run_match checks it).
+constexpr uint32_t SLOT_AMBIGUOUS = 0x80000000u, SLOT_EXACT = 0x40000000u;
+__device__ __forceinline__ int slot_index(uint32_t y) {
+  const uint32_t i = y & 0x3fffffffu;
+  return i == 0x3fffffffu ? 0x7fffffff : (int)i;
+}
+
+struct MatchExactArgs {
+  const float* d[2]; int layout;   // the fp32 descriptors the tiles were made from
   const int* cu[2]; int n[2];
   const float* sq[2];              // distance mode 1
   int dist_mode;
+  uint2* slot[2];                  // read (flags), and the flagged lines' slots rewritten
+  float thr; int mutual;
+  const int* pimg[2]; const int* out_off[2];   // indexed mode, as in MatchTailArgs
+};
+
+// The exact distance of two lines from their ascending-k fmaf chain acc (see the header), shared by every exact path.
+__device__ __forceinline__ float exact_dist(float acc, float sqa, float sqb, int dist_mode) {
+  return dist_mode == 1 ? fmaxf((sqa + sqb) - 2.f * acc, 0.f) : fmaxf(2.f - 2.f * acc, 0.f);
+}
+
+constexpr int MX_WIN = 256;                 // lines of one side a CTA scans for flags per window (one per thread)
+constexpr int MX_R = 32;                    // flagged rows per group: 4 row blocks of 8 rows
+constexpr int MX_C = 64;                    // columns of the other side per staged chunk
+constexpr int MX_BLD = MX_C + 1;            // padded k-row of the chunk: transposing stores hit 32 banks
+constexpr int MX_OFF_B = MT_D * MX_R * 4;   // As [256][32] k-major, then Bs [256][65]
+constexpr int MX_SMEM = MX_OFF_B + MT_D * MX_BLD * 4;
+
+// grid = (n_pairs, 2 sides, S), 256 threads.  CTA (pair, side, z) scans the windows w = z, z + S, ... of MX_WIN lines
+// of its side, compacts the lines whose slot cannot be trusted (side 0: ambiguous or within MATCH_EPS of the
+// threshold; side 1: ambiguous, only when mutual) and recomputes each with fp32 FMAs in ascending k against every
+// line of the other side.  Groups of 32 rows sit k-major in shared memory; the other side streams through in
+// 64-column chunks.  Thread = 8 rows (broadcast LDS.128) x 1 column, 8 independent fmaf chains; each thread keeps a
+// running first-minimum over its columns in ascending j, then the 64 column threads of a row merge lexicographically.
+__global__ void __launch_bounds__(256) match_exact_kernel(MatchExactArgs p) {
+  extern __shared__ __align__(16) float mx_smem[];
+  float* As = mx_smem;                      // [k][MX_R]
+  float* Bs = mx_smem + MT_D * MX_R;        // [k][MX_BLD]
+  __shared__ int list[MX_WIN];
+  __shared__ int wcount[8];
+  __shared__ float xb[MX_R];
+  __shared__ int xi[MX_R];
+  pdl_launch_dependents();
+  const int pair = blockIdx.x, sa = blockIdx.y;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  if (sa == 1 && !p.mutual) return;
+  pdl_wait();
+  // side a = the lines re-checked here, side b = the other side (selects, not indexing: the params stay in constant bank)
+  const int* pimg_a = sa ? p.pimg[1] : p.pimg[0];
+  const int* pimg_b = sa ? p.pimg[0] : p.pimg[1];
+  const int* oo_a = sa ? p.out_off[1] : p.out_off[0];
+  int ba, ea, bb, eb;
+  image_range(sa ? p.cu[1] : p.cu[0], sa ? p.n[1] : p.n[0], pimg_a ? pimg_a[pair] : pair, ba, ea);
+  image_range(sa ? p.cu[0] : p.cu[1], sa ? p.n[0] : p.n[1], pimg_b ? pimg_b[pair] : pair, bb, eb);
+  const int na = ea - ba, nb = eb - bb;
+  if (na == 0 || nb == 0) return;           // match_tc_kernel wrote no slots for this pair
+  uint2* slot = (sa ? p.slot[1] : p.slot[0]) + (oo_a ? oo_a[pair] : ba);
+  const float* __restrict__ A = sa ? p.d[1] : p.d[0];
+  const float* __restrict__ B = sa ? p.d[0] : p.d[1];
+  const float* __restrict__ sq_a = sa ? p.sq[1] : p.sq[0];
+  const float* __restrict__ sq_b = sa ? p.sq[0] : p.sq[1];
+  const int rb = tid >> 6, c = tid & 63;    // row block (rows rb * 8 .. + 7 of a group), column in the chunk
+  for (int w0 = blockIdx.z * MX_WIN; w0 < na; w0 += gridDim.z * MX_WIN) {
+    // ---- compact the flagged lines of the window (ballot + prefix over the warps)
+    bool flag = false;
+    if (w0 + tid < na) {
+      const uint2 s = slot[w0 + tid];
+      flag = (s.y & SLOT_AMBIGUOUS) != 0;
+      if (sa == 0) flag = flag || !(fabsf(__uint_as_float(s.x) - p.thr) >= MATCH_EPS);
+    }
+    const unsigned fb = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) wcount[warp] = __popc(fb);
+    __syncthreads();
+    int pre = 0, nf = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      pre += q < warp ? wcount[q] : 0;
+      nf += wcount[q];
+    }
+    if (flag) list[pre + __popc(fb & ((1u << lane) - 1u))] = w0 + tid;
+    __syncthreads();
+    for (int g0 = 0; g0 < nf; g0 += MX_R) {
+      const int nr = min(MX_R, nf - g0);
+      // ---- stage the group's rows k-major: lane -> row, warps split k into float4 steps (stores conflict-free)
+      if (lane < nr) {
+        const int r = list[g0 + lane];
+        if (p.layout == 0) {
+          const float4* __restrict__ x = reinterpret_cast<const float4*>(A + (size_t)(ba + r) * MT_D);
+          for (int k4 = warp; k4 < MT_D / 4; k4 += 8) {
+            const float4 v = x[k4];
+            As[(4 * k4) * MX_R + lane] = v.x; As[(4 * k4 + 1) * MX_R + lane] = v.y;
+            As[(4 * k4 + 2) * MX_R + lane] = v.z; As[(4 * k4 + 3) * MX_R + lane] = v.w;
+          }
+        } else {
+          const float* __restrict__ x = A + (size_t)ba * MT_D + r;
+          for (int k = warp; k < MT_D; k += 8) As[k * MX_R + lane] = x[(size_t)k * na];
+        }
+      }
+      float sqa[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int gi = rb * 8 + i;
+        sqa[i] = (p.dist_mode == 1 && gi < nr) ? sq_a[ba + list[g0 + gi]] : 0.f;
+      }
+      float best[8];
+      int bidx[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { best[i] = INFINITY; bidx[i] = 0x7fffffff; }
+      for (int j0 = 0; j0 < nb; j0 += MX_C) {
+        __syncthreads();   // As staged / the previous chunk consumed
+        // ---- stage columns j0 .. j0 + 63 of the other side k-major (zeros past nb)
+        if (p.layout == 0) {
+          // 8 lanes read one line's 128 B run of float4s (coalesced), 4 lines per warp; padded transpose into Bs
+          for (int e = tid; e < MX_C * (MT_D / 4); e += 256) {
+            const int cc = (e >> 3) & (MX_C - 1), k4 = ((e >> 9) << 3) | (e & 7);
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (j0 + cc < nb) v = reinterpret_cast<const float4*>(B + (size_t)(bb + j0 + cc) * MT_D)[k4];
+            Bs[(4 * k4) * MX_BLD + cc] = v.x; Bs[(4 * k4 + 1) * MX_BLD + cc] = v.y;
+            Bs[(4 * k4 + 2) * MX_BLD + cc] = v.z; Bs[(4 * k4 + 3) * MX_BLD + cc] = v.w;
+          }
+        } else {
+          const float* __restrict__ y = B + (size_t)bb * MT_D + j0 + c;
+          const bool col = j0 + c < nb;
+          for (int k = rb; k < MT_D; k += 4) Bs[k * MX_BLD + c] = col ? y[(size_t)k * nb] : 0.f;
+        }
+        __syncthreads();
+        if (rb * 8 < nr) {
+          float acc[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+          const float4* __restrict__ a4 = reinterpret_cast<const float4*>(As) + rb * 2;
+#pragma unroll 8
+          for (int k = 0; k < MT_D; ++k) {
+            const float4 x0 = a4[k * (MX_R / 4)], x1 = a4[k * (MX_R / 4) + 1];
+            const float y = Bs[k * MX_BLD + c];
+            acc[0] = fmaf(x0.x, y, acc[0]); acc[1] = fmaf(x0.y, y, acc[1]);
+            acc[2] = fmaf(x0.z, y, acc[2]); acc[3] = fmaf(x0.w, y, acc[3]);
+            acc[4] = fmaf(x1.x, y, acc[4]); acc[5] = fmaf(x1.y, y, acc[5]);
+            acc[6] = fmaf(x1.z, y, acc[6]); acc[7] = fmaf(x1.w, y, acc[7]);
+          }
+          const int j = j0 + c;
+          if (j < nb) {
+            const float sqb = p.dist_mode == 1 ? sq_b[bb + j] : 0.f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const float v = exact_dist(acc[i], sqa[i], sqb, p.dist_mode);
+              if (v < best[i]) { best[i] = v; bidx[i] = j; }
+            }
+          }
+        }
+      }
+      // ---- merge the 64 column threads of every row: 32 lanes by shuffles, then the two warps of a row block
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, best[i], o);
+          const int oi = __shfl_xor_sync(0xffffffffu, bidx[i], o);
+          if (ov < best[i] || (ov == best[i] && oi < bidx[i])) { best[i] = ov; bidx[i] = oi; }
+        }
+      }
+      if ((warp & 1) && lane == 0) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { xb[rb * 8 + i] = best[i]; xi[rb * 8 + i] = bidx[i]; }
+      }
+      __syncthreads();
+      if (!(warp & 1) && lane < 8 && rb * 8 + lane < nr) {
+        float v = best[0];
+        int idx = bidx[0];
+#pragma unroll
+        for (int i = 1; i < 8; ++i)
+          if (lane == i) { v = best[i]; idx = bidx[i]; }
+        const float ov = xb[rb * 8 + lane];
+        const int oi = xi[rb * 8 + lane];
+        if (ov < v || (ov == v && oi < idx)) { v = ov; idx = oi; }
+        slot[list[g0 + rb * 8 + lane]] = make_uint2(__float_as_uint(v), (uint32_t)idx | SLOT_EXACT);
+      }
+    }
+    __syncthreads();   // list / wcount / xb are rewritten by the next window
+  }
+}
+
+// ---------------------------------------------------------------- tail: threshold, mutual, counts
+struct MatchTailArgs {
+  const int* cu[2]; int n[2];
   const uint2* slot[2];
   float thr; int mutual;
   int* matches0; float* scores0; int* nn1; int* counts;
@@ -408,97 +591,20 @@ __device__ __forceinline__ int ld_acquire_sys(const int* p) {
   return v;
 }
 
-// Exact fp32 distances of line `r` of side `sa` to every line of the other side (ascending-k fmaf chain,
-// the arithmetic of the round-1 FFMA matcher), first-minimum argmin over them; whole warp.
-__device__ __forceinline__ void exact_row(const MatchTailArgs& p, int sa, int pair_b_a, int na, int r, int pair_b_b, int nb,
-                                          float* xrow, int lane, float& best, int& bidx) {
-  const int sb = sa ^ 1;
-  const float* __restrict__ A = p.d[sa];
-  const float* __restrict__ B = p.d[sb];
-  // stage the row in shared memory (per-warp 1 KB)
-  if (p.layout == 0) {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) xrow[i * 32 + lane] = A[(size_t)(pair_b_a + r) * MT_D + i * 32 + lane];
-  } else {
-#pragma unroll
-    for (int i = 0; i < 8; ++i) xrow[i * 32 + lane] = A[(size_t)pair_b_a * MT_D + (size_t)(i * 32 + lane) * na + r];
-  }
-  __syncwarp();
-  const float sqa = p.dist_mode == 1 ? p.sq[sa][pair_b_a + r] : 0.f;
-  best = INFINITY; bidx = 0x7fffffff;
-  for (int j = lane; j < nb; j += 32) {
-    float acc = 0.f;
-    if (p.layout == 0) {
-      const float4* __restrict__ y = reinterpret_cast<const float4*>(B + (size_t)(pair_b_b + j) * MT_D);
-#pragma unroll 8
-      for (int k = 0; k < MT_D / 4; ++k) {
-        const float4 b = y[k];
-        acc = fmaf(xrow[4 * k], b.x, acc);
-        acc = fmaf(xrow[4 * k + 1], b.y, acc);
-        acc = fmaf(xrow[4 * k + 2], b.z, acc);
-        acc = fmaf(xrow[4 * k + 3], b.w, acc);
-      }
-    } else {
-      const float* __restrict__ y = B + (size_t)pair_b_b * MT_D + j;
-#pragma unroll 8
-      for (int k = 0; k < MT_D; ++k) acc = fmaf(xrow[k], y[(size_t)k * nb], acc);
-    }
-    const float v = p.dist_mode == 1 ? fmaxf((sqa + p.sq[sb][pair_b_b + j]) - 2.f * acc, 0.f) : fmaxf(2.f - 2.f * acc, 0.f);
-    if (v < best) { best = v; bidx = j; }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bidx, o);
-    if (ov < best || (ov == best && oi < bidx)) { best = ov; bidx = oi; }
-  }
-  __syncwarp();
-}
-
-// One decision (warp-cooperative; used for the lines whose slots are flagged ambiguous): side-0 line i ->
-// matches0 / scores0 (returns keep), or side-1 line j -> nn1.  b0 / b1: first descriptor row of each side,
-// o0 / o1: first slot / output of each side (equal unless images are shared between pairs).
-__device__ __forceinline__ bool tail_decide_row(const MatchTailArgs& p, int i, int b0, int o0, int n0, int b1, int o1, int n1,
-                                                float* xrow, int lane, bool force_exact) {
-  const uint2 s = p.slot[0][o0 + i];
-  float v = __uint_as_float(s.x);
-  int idx = (int)(s.y & 0x7fffffffu);
-  if (force_exact || (s.y >> 31) || !(fabsf(v - p.thr) >= MATCH_EPS)) exact_row(p, 0, b0, n0, i, b1, n1, xrow, lane, v, idx);
-  bool keep = v < p.thr;   // strict '<' (nn_matcher.py:18)
-  if (keep && p.mutual) {
-    const uint2 t = p.slot[1][o1 + idx];
-    int back = (int)(t.y & 0x7fffffffu);
-    if (t.y >> 31) {
-      float bv;
-      exact_row(p, 1, b1, n1, idx, b0, n0, xrow, lane, bv, back);
-    }
-    keep = back == i;
-  }
-  if (lane == 0) {
-    p.matches0[o0 + i] = keep ? idx : -1;
-    p.scores0[o0 + i] = v;
-  }
-  return keep;
-}
-
-// grid = (ceil((max0 + max1) / 256), n_pairs), 256 threads, one line per THREAD on the fast path: items below
-// max0 decide side-0 lines (matches0 / scores0 / counts), the others publish nn1 (argmin over axis 0).
-// Lines whose tensor-core result cannot be trusted (ambiguous slot, score next to the threshold, or an
-// ambiguous partner column) go to a shared work list that the block's 8 warps then process
-// cooperatively with exact fp32 arithmetic.
+// grid = (ceil((max0 + max1) / 256), n_pairs), 256 threads, one line per thread: items below max0 decide side-0
+// lines (matches0 / scores0 / counts), the others publish nn1 (argmin over axis 0).  Every slot holds a result
+// that can be trusted as it stands: match_exact_kernel has already re-taken the ones match_tc_kernel flagged.
 __global__ void __launch_bounds__(256) match_tail_kernel(MatchTailArgs p) {
-  __shared__ float xrows[8][MT_D];
-  __shared__ int work[256];
-  __shared__ int n_work, n_keep;
+  __shared__ int n_keep;
   pdl_launch_dependents();
   pdl_wait();
-  const int pair = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int pair = blockIdx.y, tid = threadIdx.x, lane = tid & 31;
   int b0, e0, b1, e1;
   image_range(p.cu[0], p.n[0], p.pimg[0] ? p.pimg[0][pair] : pair, b0, e0);
   image_range(p.cu[1], p.n[1], p.pimg[1] ? p.pimg[1][pair] : pair, b1, e1);
   const int n0 = e0 - b0, n1 = e1 - b1;
   const int o0 = p.out_off[0] ? p.out_off[0][pair] : b0, o1 = p.out_off[1] ? p.out_off[1][pair] : b1;
-  if (tid == 0) { n_work = 0; n_keep = 0; }
+  if (tid == 0) n_keep = 0;
   __syncthreads();
   const int w = blockIdx.x * 256 + tid;
   bool keep = false;
@@ -511,45 +617,19 @@ __global__ void __launch_bounds__(256) match_tail_kernel(MatchTailArgs p) {
       } else {
         const uint2 s = p.slot[0][o0 + i];
         const float v = __uint_as_float(s.x);
-        const int idx = (int)(s.y & 0x7fffffffu);
-        bool hard = (s.y >> 31) || !(fabsf(v - p.thr) >= MATCH_EPS);
-        if (!hard) {
-          keep = v < p.thr;
-          if (keep && p.mutual) {
-            const uint2 t = p.slot[1][o1 + idx];
-            if (t.y >> 31) { hard = true; keep = false; }
-            else keep = (int)(t.y & 0x7fffffffu) == i;
-          }
-        }
-        if (hard) work[atomicAdd(&n_work, 1)] = w;
-        else { p.matches0[o0 + i] = keep ? idx : -1; p.scores0[o0 + i] = v; }
+        const int idx = slot_index(s.y);
+        keep = v < p.thr;   // strict '<' (nn_matcher.py:18)
+        if (keep && p.mutual) keep = slot_index(p.slot[1][o1 + idx].y) == i;
+        p.matches0[o0 + i] = keep ? idx : -1;
+        p.scores0[o0 + i] = v;
       }
     }
   } else if (p.mutual) {
     const int j = w - p.max0;
-    if (j < n1) {
-      if (n0 == 0) p.nn1[o1 + j] = -1;
-      else {
-        const uint2 t = p.slot[1][o1 + j];
-        if (t.y >> 31) work[atomicAdd(&n_work, 1)] = w;
-        else p.nn1[o1 + j] = (int)(t.y & 0x7fffffffu);
-      }
-    }
+    if (j < n1) p.nn1[o1 + j] = n0 == 0 ? -1 : slot_index(p.slot[1][o1 + j].y);
   }
   const unsigned kb = __ballot_sync(0xffffffffu, keep);
   if (lane == 0 && kb) atomicAdd(&n_keep, __popc(kb));
-  __syncthreads();
-  for (int e = warp; e < n_work; e += 8) {     // exact path, one work item per warp at a time
-    const int ww = work[e];
-    if (ww < p.max0) {
-      if (tail_decide_row(p, ww, b0, o0, n0, b1, o1, n1, xrows[warp], lane, false) && lane == 0) atomicAdd(&n_keep, 1);
-    } else {
-      const int j = ww - p.max0;
-      float bv; int back;
-      exact_row(p, 1, b1, n1, j, b0, n0, xrows[warp], lane, bv, back);
-      if (lane == 0) p.nn1[o1 + j] = back;
-    }
-  }
   __syncthreads();
   if (tid == 0 && n_keep) atomicAdd(&p.counts[pair], n_keep);
   if (p.world > 1) {
