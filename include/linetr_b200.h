@@ -24,6 +24,8 @@
  *   ltr_line_gt                <- mat_assign_sublines of the homography dataset builder
  *                                 (dataloaders/build_homography_dataset.py:210-234) + Evaluate_PR.calc_TFPN
  *                                 (evaluations/evaluate_pr.py:10-22) for a batch of pairs.
+ *   ltr_triplet_loss           <- descriptor_loss.forward (evaluations/criteria.py:35-192) of the validation step
+ *                                 (train.py:198-240) + Evaluate_PR.calc_TFPN, for groups of pairs.
  *
  * Conventions: return 0 on success, a negative LTR_E_* code on failure (message via
  * ltr_last_error(), thread-local).  All device pointers are caller-owned and must live on
@@ -409,6 +411,62 @@ typedef struct {
 
 /* Asynchronous on `stream`; never synchronises. */
 int ltr_line_gt(const LtrLineGtInput* in, const LtrLineGtOutput* out, int32_t device, void* stream);
+
+/* Semi-hard triplet loss of the validation step, forward value only: descriptor_loss.compute_distances + forward
+ * (evaluations/criteria.py:35-192) for a batch of pairs, and optionally Evaluate_PR.calc_TFPN
+ * (evaluations/evaluate_pr.py:10-22) of predicted matches against the same assignment.
+ *
+ * Per pair, d[i, j] = 2 - 2 <a_i, b_j> with <a_i, b_j> one ascending-k fmaf chain (the matcher's exact fp32 path), NOT
+ * clipped.  With v = the pair's assignment entry (i, j): match iff (double)v > match_thr, unmatch iff
+ * (double)v <= unmatch_thr.  Anchors: every side-0 line i (candidates d[i, :]), then every side-1 line j (candidates
+ * d[:, j]).  pos = max of d over the anchor's match candidates; the anchor has a positive iff pos > 0.  u = d on unmatch
+ * candidates and the literal 10000.f on the others; neg = min of u over pos < u < pos + 0.5f (strict, fp32 sum); the
+ * anchor is valid iff that window is not empty.  Per group: n_valid, loss = float(sum of relu((pos - neg) + 1.f) in fp64
+ * over the valid anchors, in a fixed order / n_valid), hardest_pos = max pos, hardest_neg = min neg; all three NaN
+ * when n_valid == 0.  The reference requires n0 == n1 per pair; this call does not.
+ *
+ * Thresholds: match_thr = (double)0.3f, unmatch_thr = 0 reproduce torch's float32 comparisons of
+ * `mat_assign_sublines` (an entry exactly 0.3f is not a match); match_thr = unmatch_thr = 0.3 on the builder's raw
+ * overlaps reproduce the 0/1 matrix train.py builds from `lmatches`. */
+typedef struct {
+  const float* desc0;            /* device, LTR_LAYOUT_ROWS [S0, 256] or channel-first [256, n0_p] per pair at 256*cu0[p] */
+  const float* desc1;
+  int32_t layout;
+  int32_t d;                     /* must be 256 (others: LTR_E_UNSUPPORTED) */
+  int32_t n_pairs;
+  int32_t n0, n1;                /* lines per pair when cu0/cu1 are NULL */
+  const int32_t* cu0;            /* device [n_pairs + 1] or NULL (uniform) */
+  const int32_t* cu1;
+  int32_t max_n0, max_n1;        /* bounds of every pair's line counts (var-len only) */
+  const float* assign;           /* device fp32, pair p at p * assign_stride, row i at i * assign_ld (0: n1 of the pair),
+                                    so [b, n0+1, n1+1] with its dustbin row / column is read in place */
+  int64_t assign_stride;
+  int32_t assign_ld;
+  double match_thr;
+  double unmatch_thr;
+  const int32_t* pred0;          /* optional device [S0]: predicted side-1 index (local) of every side-0 line, or -1
+                                    (values outside [0, n1_p) count as no prediction) */
+  int32_t n_groups;              /* groups are contiguous pair ranges [group_off[g], group_off[g+1]) */
+  const int32_t* group_off;      /* device [n_groups + 1] or NULL: one group of all pairs (n_groups must be 1) */
+} LtrTripletInput;
+
+/* Outputs (device, caller-owned).  Per anchor [S0 + S1]: side-0 line i of pair p at cu0[p] + cu1[p] + i, side-1 line j
+ * at cu0[p+1] + cu1[p] + j; pos (NaN without a positive), neg (NaN unless valid), state (0 no positive, 1 positive but
+ * empty window, 2 valid).  Per group: loss, hardest_pos, hardest_neg, n_valid.  tfpn [n_pairs, 4] (required iff
+ * pred0): TP, FP, FN, TN with ground truth = the match class. */
+typedef struct {
+  float* pos;
+  float* neg;
+  int32_t* state;
+  float* loss;
+  float* hardest_pos;
+  float* hardest_neg;
+  int32_t* n_valid;
+  int32_t* tfpn;
+} LtrTripletOutput;
+
+/* Asynchronous on `stream`; never synchronises.  n_pairs == 0 writes nothing. */
+int ltr_triplet_loss(const LtrTripletInput* in, const LtrTripletOutput* out, int32_t device, void* stream);
 
 /* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
  * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */

@@ -6,6 +6,8 @@ Batched front-end:
     PairEngine, LineBatch, ImagePairMatches, ImageSet, exhaustive_pairs
 Match quality against homography ground truth (eval_homography):
     line_assignment, get_precision_recall, homography_ground_truth, score_line_matches
+The validation step's descriptor loss and metrics (eval_criteria; drop-in eval_criteria.descriptor_loss):
+    triplet_loss, validation_metrics
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -31,6 +33,8 @@ _LAZY = {
     "get_precision_recall": ("eval_homography", "get_precision_recall"),
     "homography_ground_truth": ("eval_homography", "homography_ground_truth"),
     "score_line_matches": ("eval_homography", "score_line_matches"),
+    "triplet_loss": ("eval_criteria", "triplet_loss"),
+    "validation_metrics": ("eval_criteria", "validation_metrics"),
 }
 
 

@@ -25,7 +25,7 @@ EXPORTED_SYMBOLS = (
     "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
-    "ltr_line_gt",
+    "ltr_line_gt", "ltr_triplet_loss",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
@@ -122,6 +122,19 @@ class LtrLineGtOutput(C.Structure):
     _fields_ = [("assign", C.c_void_p), ("assign_stride", C.c_int64), ("n_gt", C.c_void_p), ("tfpn", C.c_void_p)]
 
 
+class LtrTripletInput(C.Structure):
+    _fields_ = [("desc0", C.c_void_p), ("desc1", C.c_void_p), ("layout", C.c_int32), ("d", C.c_int32),
+                ("n_pairs", C.c_int32), ("n0", C.c_int32), ("n1", C.c_int32), ("cu0", C.c_void_p), ("cu1", C.c_void_p),
+                ("max_n0", C.c_int32), ("max_n1", C.c_int32), ("assign", C.c_void_p), ("assign_stride", C.c_int64),
+                ("assign_ld", C.c_int32), ("match_thr", C.c_double), ("unmatch_thr", C.c_double), ("pred0", C.c_void_p),
+                ("n_groups", C.c_int32), ("group_off", C.c_void_p)]
+
+
+class LtrTripletOutput(C.Structure):
+    _fields_ = [("pos", C.c_void_p), ("neg", C.c_void_p), ("state", C.c_void_p), ("loss", C.c_void_p),
+                ("hardest_pos", C.c_void_p), ("hardest_neg", C.c_void_p), ("n_valid", C.c_void_p), ("tfpn", C.c_void_p)]
+
+
 def lib_path() -> str:
     return _LIB_PATH
 
@@ -169,6 +182,8 @@ def load():
     lib.ltr_match_indexed.restype = C.c_int
     lib.ltr_line_gt.argtypes = [C.POINTER(LtrLineGtInput), C.POINTER(LtrLineGtOutput), C.c_int32, C.c_void_p]
     lib.ltr_line_gt.restype = C.c_int
+    lib.ltr_triplet_loss.argtypes = [C.POINTER(LtrTripletInput), C.POINTER(LtrTripletOutput), C.c_int32, C.c_void_p]
+    lib.ltr_triplet_loss.restype = C.c_int
     lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.ltr_gather_wait.restype = C.c_int
     lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,

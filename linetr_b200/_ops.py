@@ -326,6 +326,34 @@ def line_gt(segs0, segs1, n_pairs, *, cu0, cu1, max_n0, max_n1, homography, homo
     N.check(rc, "ltr_line_gt")
 
 
+def triplet_loss(desc0, desc1, layout, n_pairs, *, assign, assign_stride, pos, neg, state, loss, hardest_pos,
+                 hardest_neg, n_valid, n0=0, n1=0, cu0=None, cu1=None, max_n0=0, max_n1=0, assign_ld=0, match_thr=0.3,
+                 unmatch_thr=0.0, pred0=None, tfpn=None, n_groups=1, group_off=None):
+    """ltr_triplet_loss into caller-allocated outputs: per anchor pos / neg (fp32) and state (int32) [S0 + S1], per
+    group loss / hardest_pos / hardest_neg (fp32) and n_valid (int32), tfpn [P, 4] int32 with pred0."""
+    _req_cuda(desc0, "desc0")
+    _req_cuda(desc1, "desc1")
+    dev = desc0.device
+    for nm, t, dt in (("desc0", desc0, torch.float32), ("desc1", desc1, torch.float32), ("assign", assign, torch.float32),
+                      ("cu0", cu0, torch.int32), ("cu1", cu1, torch.int32), ("pred0", pred0, torch.int32),
+                      ("group_off", group_off, torch.int32), ("pos", pos, torch.float32), ("neg", neg, torch.float32),
+                      ("state", state, torch.int32), ("loss", loss, torch.float32), ("hardest_pos", hardest_pos, torch.float32),
+                      ("hardest_neg", hardest_neg, torch.float32), ("n_valid", n_valid, torch.int32), ("tfpn", tfpn, torch.int32)):
+        if t is None:
+            continue
+        if t.dtype != dt or not t.is_contiguous() or t.device != dev:
+            raise N.LtrError(f"triplet_loss: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    inp = _struct(N.LtrTripletInput, desc0=desc0, desc1=desc1, layout=int(layout), d=256, n_pairs=int(n_pairs), n0=int(n0),
+                  n1=int(n1), cu0=cu0, cu1=cu1, max_n0=int(max_n0), max_n1=int(max_n1), assign=assign,
+                  assign_stride=int(assign_stride), assign_ld=int(assign_ld), match_thr=float(match_thr),
+                  unmatch_thr=float(unmatch_thr), pred0=pred0, n_groups=int(n_groups), group_off=group_off)
+    out = _struct(N.LtrTripletOutput, pos=pos, neg=neg, state=state, loss=loss, hardest_pos=hardest_pos,
+                  hardest_neg=hardest_neg, n_valid=n_valid, tfpn=tfpn)
+    with torch.cuda.device(dev):
+        rc = N.load().ltr_triplet_loss(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_triplet_loss")
+
+
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     """ltr_match_distmat on dist [P, n0, n1] (CUDA).  Returns dict(matches0 [P,n0], scores0, nn1, counts)."""
     _req_cuda(dist, "dist_mat")

@@ -40,6 +40,7 @@ enum KernelClass : int {
   KC_MATCH_EXACT,
   KC_MATCH_TAIL,
   KC_LINE_GT,
+  KC_TRIPLET,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

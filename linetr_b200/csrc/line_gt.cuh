@@ -114,6 +114,23 @@ __device__ __forceinline__ Seg project_seg(const double* __restrict__ m, const S
   return o;
 }
 
+// Evaluate_PR.calc_TFPN, one row of a pair: n_tp += TP (the predicted column is ground truth), n_pos += positive (the
+// row has ground truth), n_tn += TN.  TN is literal calc_TFPN: the row's count of columns with neither a prediction nor
+// ground truth equals the number of ROWS.
+__device__ __forceinline__ void tfpn_row(bool any_gt, bool tp, int neither, int n_rows, int& n_tp, int& n_pos, int& n_tn) {
+  n_tp += tp;
+  n_pos += any_gt ? 1 : 0;
+  n_tn += neither == n_rows;
+}
+
+// A block's row sums into the pair's TP, FP = negatives - TN, FN = positives - TP, TN.
+__device__ __forceinline__ void tfpn_add(int* o, int rows, int pos, int tp, int tn) {
+  atomicAdd(o + 0, tp);
+  atomicAdd(o + 1, rows - pos - tn);
+  atomicAdd(o + 2, pos - tp);
+  atomicAdd(o + 3, tn);
+}
+
 // Grid (pairs, ceil(max_n0 / 128)), 128 threads: thread t owns side-0 row blockIdx.y*128 + t of pair blockIdx.x and
 // keeps its whole ground-truth row, so the per-row TP / TN / positive tests need no atomics; one atomic per count
 // and block.  Side 1 goes through shared memory 32 lines at a time; in dense mode the 128 x 32 block of the
@@ -197,14 +214,11 @@ __global__ void __launch_bounds__(LG_ROWS) line_gt_kernel(LineGtArgs a) {
     }
   }
 
-  // per-pair counts: n_gt; with predictions TP, FP = negatives - TN, FN = positives - TP, TN.  TN is literal
-  // calc_TFPN: a row whose count of columns with neither a prediction nor ground truth equals the number of ROWS.
+  // per-pair counts: n_gt; with predictions the calc_TFPN row terms
   int c[4] = {0, 0, 0, 0};
   if (live) {
     c[0] = n_gt;
-    c[1] = tp;
-    c[2] = any_gt ? 1 : 0;
-    c[3] = neither == n0;
+    tfpn_row(any_gt, tp, neither, n0, c[1], c[2], c[3]);
   }
   const int lane = t & 31, w = t >> 5;
 #pragma unroll
@@ -224,15 +238,7 @@ __global__ void __launch_bounds__(LG_ROWS) line_gt_kernel(LineGtArgs a) {
       for (int q = 0; q < LG_ROWS / 32; ++q) s[k] += s_red[k][q];
     }
     atomicAdd(a.n_gt + pair, s[0]);
-    if (a.pred0) {
-      const int rows = min(LG_ROWS, n0 - row0);
-      const int pos = s[2], neg = rows - pos, tpc = s[1], tnc = s[3];
-      int* o = a.tfpn + 4 * pair;
-      atomicAdd(o + 0, tpc);
-      atomicAdd(o + 1, neg - tnc);
-      atomicAdd(o + 2, pos - tpc);
-      atomicAdd(o + 3, tnc);
-    }
+    if (a.pred0) tfpn_add(a.tfpn + 4 * pair, min(LG_ROWS, n0 - row0), s[2], s[1], s[3]);
   }
 }
 

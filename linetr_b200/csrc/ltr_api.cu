@@ -20,6 +20,7 @@
 #include "match_kernels.cuh"
 #include "match_tc.cuh"
 #include "line_gt.cuh"
+#include "triplet.cuh"
 
 namespace ltr {
 
@@ -37,7 +38,8 @@ int set_error(int code, const std::string& msg) {
 const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
-                                         "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt"};
+                                         "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
+                                         "triplet"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1140,6 +1142,54 @@ int ltr_line_gt(const LtrLineGtInput* in, const LtrLineGtOutput* out, int32_t de
   LaunchScope ls(KC_LINE_GT, s);
   if (out->assign) LTR_CUDA_TRY(launch_pdl(line_gt_kernel<true>, grid, dim3(LG_ROWS), 0, s, a));
   else LTR_CUDA_TRY(launch_pdl(line_gt_kernel<false>, grid, dim3(LG_ROWS), 0, s, a));
+  return LTR_OK;
+}
+
+int ltr_triplet_loss(const LtrTripletInput* in, const LtrTripletOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_triplet_loss: null argument");
+  if (in->d != MT_D) return set_error(LTR_E_UNSUPPORTED, "ltr_triplet_loss: descriptor dim must be 256");
+  if (in->layout != LTR_LAYOUT_ROWS && in->layout != LTR_LAYOUT_CHANNEL_FIRST) return set_error(LTR_E_INVALID, "ltr_triplet_loss: bad layout");
+  if (in->n_pairs < 0 || in->n0 < 0 || in->n1 < 0 || in->max_n0 < 0 || in->max_n1 < 0 || in->assign_ld < 0 || in->assign_stride < 0)
+    return set_error(LTR_E_INVALID, "ltr_triplet_loss: negative count");
+  if ((in->cu0 == nullptr) != (in->cu1 == nullptr)) return set_error(LTR_E_INVALID, "ltr_triplet_loss: cu0/cu1 must be given together");
+  if (in->n_groups < 1 || (!in->group_off && in->n_groups != 1))
+    return set_error(LTR_E_INVALID, "ltr_triplet_loss: n_groups must be >= 1 (1 without group_off)");
+  const int mx0 = in->cu0 ? in->max_n0 : in->n0, mx1 = in->cu1 ? in->max_n1 : in->n1;
+  if (mx0 >= (1 << 30) || mx1 >= (1 << 30)) return set_error(LTR_E_INVALID, "ltr_triplet_loss: a pair side has 2^30 lines or more");
+  if (in->assign_ld > 0 && in->assign_ld < mx1) return set_error(LTR_E_INVALID, "ltr_triplet_loss: assign_ld < max_n1");
+  if (in->assign_stride < (int64_t)mx0 * (in->assign_ld ? in->assign_ld : mx1))
+    return set_error(LTR_E_INVALID, "ltr_triplet_loss: assign_stride < max_n0 * row pitch");
+  if (in->n_pairs == 0) return LTR_OK;
+  if (!out->pos || !out->neg || !out->state || !out->loss || !out->hardest_pos || !out->hardest_neg || !out->n_valid)
+    return set_error(LTR_E_INVALID, "ltr_triplet_loss: null output");
+  if (in->pred0 && !out->tfpn) return set_error(LTR_E_INVALID, "ltr_triplet_loss: pred0 needs tfpn");
+  const bool lines = mx0 > 0 || mx1 > 0;
+  if (lines && (!in->desc0 || !in->desc1 || !in->assign)) return set_error(LTR_E_INVALID, "ltr_triplet_loss: null descriptors or assign");
+  if (in->layout == LTR_LAYOUT_ROWS && ((reinterpret_cast<uintptr_t>(in->desc0) | reinterpret_cast<uintptr_t>(in->desc1)) & 15))
+    return set_error(LTR_E_INVALID, "ltr_triplet_loss: row descriptors must be 16-byte aligned");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  if (in->pred0) LTR_CUDA_TRY(cudaMemsetAsync(out->tfpn, 0, sizeof(int32_t) * 4 * in->n_pairs, s));
+  if (lines) {
+    TripletArgs a{};
+    a.d[0] = in->desc0; a.d[1] = in->desc1; a.layout = in->layout;
+    a.cu[0] = in->cu0; a.cu[1] = in->cu1; a.n[0] = in->n0; a.n[1] = in->n1;
+    a.assign = in->assign; a.assign_stride = in->assign_stride; a.assign_ld = in->assign_ld;
+    a.match_thr = in->match_thr; a.unmatch_thr = in->unmatch_thr;
+    a.pred0 = in->pred0;
+    a.pos = out->pos; a.neg = out->neg; a.state = out->state; a.tfpn = out->tfpn;
+    const int windows = std::min(cdiv(std::max(mx0, mx1), MX_R), 65535);
+    LTR_CUDA_TRY(ensure_dynamic_smem(triplet_mine_kernel, MX_SMEM));
+    LaunchScope ls(KC_TRIPLET, s);
+    LTR_CUDA_TRY(launch_pdl(triplet_mine_kernel, dim3(in->n_pairs, 2, windows), dim3(256), (size_t)MX_SMEM, s, a));
+  }
+  TripletReduceArgs r{};
+  r.cu[0] = in->cu0; r.cu[1] = in->cu1; r.n[0] = in->n0; r.n[1] = in->n1;
+  r.group_off = in->group_off; r.n_pairs = in->n_pairs;
+  r.pos = out->pos; r.neg = out->neg; r.state = out->state;
+  r.loss = out->loss; r.hardest_pos = out->hardest_pos; r.hardest_neg = out->hardest_neg; r.n_valid = out->n_valid;
+  LaunchScope ls(KC_TRIPLET, s);
+  LTR_CUDA_TRY(launch_pdl(triplet_reduce_kernel, dim3(in->n_groups), dim3(256), 0, s, r));
   return LTR_OK;
 }
 

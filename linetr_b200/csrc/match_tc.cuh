@@ -399,9 +399,13 @@ struct MatchExactArgs {
   const int* pimg[2]; const int* out_off[2];   // indexed mode, as in MatchTailArgs
 };
 
-// The exact distance of two lines from their ascending-k fmaf chain acc (see the header), shared by every exact path.
+// The exact distance of two lines from their ascending-k fmaf chain acc (see the header), before the clip at 0.
+__device__ __forceinline__ float exact_dist_raw(float acc, float sqa, float sqb, int dist_mode) {
+  return dist_mode == 1 ? (sqa + sqb) - 2.f * acc : 2.f - 2.f * acc;
+}
+// ... and clipped, shared by every exact matcher path.
 __device__ __forceinline__ float exact_dist(float acc, float sqa, float sqb, int dist_mode) {
-  return dist_mode == 1 ? fmaxf((sqa + sqb) - 2.f * acc, 0.f) : fmaxf(2.f - 2.f * acc, 0.f);
+  return fmaxf(exact_dist_raw(acc, sqa, sqb, dist_mode), 0.f);
 }
 
 constexpr int MX_WIN = 256;                 // lines of one side a CTA scans for flags per window (one per thread)
@@ -410,6 +414,61 @@ constexpr int MX_C = 64;                    // columns of the other side per sta
 constexpr int MX_BLD = MX_C + 1;            // padded k-row of the chunk: transposing stores hit 32 banks
 constexpr int MX_OFF_B = MT_D * MX_R * 4;   // As [256][32] k-major, then Bs [256][65]
 constexpr int MX_SMEM = MX_OFF_B + MT_D * MX_BLD * 4;
+
+// The exact FMA tiling (match_exact_kernel, triplet_mine_kernel), 256 threads.  A group of up to 32 rows of side a sits
+// k-major in As [k][MX_R]; chunks of 64 lines of side b go k-major into Bs [k][MX_BLD]; thread (rb = tid / 64,
+// c = tid % 64) runs the 8 fmaf chains of rows rb * 8 .. + 7 against column c.
+//
+// Row r of side a (lines [ba, ba + na)) into column `lane` of As: lane -> row, warps split k in float4 steps.
+__device__ __forceinline__ void mx_stage_row(float* As, const float* __restrict__ A, int layout, int ba, int na, int r,
+                                             int lane, int warp) {
+  if (layout == 0) {
+    const float4* __restrict__ x = reinterpret_cast<const float4*>(A + (size_t)(ba + r) * MT_D);
+    for (int k4 = warp; k4 < MT_D / 4; k4 += 8) {
+      const float4 v = x[k4];
+      As[(4 * k4) * MX_R + lane] = v.x; As[(4 * k4 + 1) * MX_R + lane] = v.y;
+      As[(4 * k4 + 2) * MX_R + lane] = v.z; As[(4 * k4 + 3) * MX_R + lane] = v.w;
+    }
+  } else {
+    const float* __restrict__ x = A + (size_t)ba * MT_D + r;
+    for (int k = warp; k < MT_D; k += 8) As[k * MX_R + lane] = x[(size_t)k * na];
+  }
+}
+
+// Lines j0 .. j0 + 63 of side b (lines [bb, bb + nb)) into Bs, zeros past nb.
+__device__ __forceinline__ void mx_stage_chunk(float* Bs, const float* __restrict__ B, int layout, int bb, int nb, int j0,
+                                               int tid, int rb, int c) {
+  if (layout == 0) {
+    // 8 lanes read one line's 128 B run of float4s (coalesced), 4 lines per warp; padded transpose into Bs
+    for (int e = tid; e < MX_C * (MT_D / 4); e += 256) {
+      const int cc = (e >> 3) & (MX_C - 1), k4 = ((e >> 9) << 3) | (e & 7);
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (j0 + cc < nb) v = reinterpret_cast<const float4*>(B + (size_t)(bb + j0 + cc) * MT_D)[k4];
+      Bs[(4 * k4) * MX_BLD + cc] = v.x; Bs[(4 * k4 + 1) * MX_BLD + cc] = v.y;
+      Bs[(4 * k4 + 2) * MX_BLD + cc] = v.z; Bs[(4 * k4 + 3) * MX_BLD + cc] = v.w;
+    }
+  } else {
+    const float* __restrict__ y = B + (size_t)bb * MT_D + j0 + c;
+    const bool col = j0 + c < nb;
+    for (int k = rb; k < MT_D; k += 4) Bs[k * MX_BLD + c] = col ? y[(size_t)k * nb] : 0.f;
+  }
+}
+
+// acc[i] = ascending-k fmaf chain of row rb * 8 + i of As with column c of Bs (rows read as broadcast LDS.128).
+__device__ __forceinline__ void mx_dot8(const float* As, const float* Bs, int rb, int c, float acc[8]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  const float4* __restrict__ a4 = reinterpret_cast<const float4*>(As) + rb * 2;
+#pragma unroll 8
+  for (int k = 0; k < MT_D; ++k) {
+    const float4 x0 = a4[k * (MX_R / 4)], x1 = a4[k * (MX_R / 4) + 1];
+    const float y = Bs[k * MX_BLD + c];
+    acc[0] = fmaf(x0.x, y, acc[0]); acc[1] = fmaf(x0.y, y, acc[1]);
+    acc[2] = fmaf(x0.z, y, acc[2]); acc[3] = fmaf(x0.w, y, acc[3]);
+    acc[4] = fmaf(x1.x, y, acc[4]); acc[5] = fmaf(x1.y, y, acc[5]);
+    acc[6] = fmaf(x1.z, y, acc[6]); acc[7] = fmaf(x1.w, y, acc[7]);
+  }
+}
 
 // grid = (n_pairs, 2 sides, S), 256 threads.  CTA (pair, side, z) scans the windows w = z, z + S, ... of MX_WIN lines
 // of its side, compacts the lines whose slot cannot be trusted (side 0: ambiguous or within MATCH_EPS of the
@@ -466,21 +525,8 @@ __global__ void __launch_bounds__(256) match_exact_kernel(MatchExactArgs p) {
     __syncthreads();
     for (int g0 = 0; g0 < nf; g0 += MX_R) {
       const int nr = min(MX_R, nf - g0);
-      // ---- stage the group's rows k-major: lane -> row, warps split k into float4 steps (stores conflict-free)
-      if (lane < nr) {
-        const int r = list[g0 + lane];
-        if (p.layout == 0) {
-          const float4* __restrict__ x = reinterpret_cast<const float4*>(A + (size_t)(ba + r) * MT_D);
-          for (int k4 = warp; k4 < MT_D / 4; k4 += 8) {
-            const float4 v = x[k4];
-            As[(4 * k4) * MX_R + lane] = v.x; As[(4 * k4 + 1) * MX_R + lane] = v.y;
-            As[(4 * k4 + 2) * MX_R + lane] = v.z; As[(4 * k4 + 3) * MX_R + lane] = v.w;
-          }
-        } else {
-          const float* __restrict__ x = A + (size_t)ba * MT_D + r;
-          for (int k = warp; k < MT_D; k += 8) As[k * MX_R + lane] = x[(size_t)k * na];
-        }
-      }
+      // ---- stage the group's rows k-major (stores conflict-free)
+      if (lane < nr) mx_stage_row(As, A, p.layout, ba, na, list[g0 + lane], lane, warp);
       float sqa[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -494,35 +540,11 @@ __global__ void __launch_bounds__(256) match_exact_kernel(MatchExactArgs p) {
       for (int j0 = 0; j0 < nb; j0 += MX_C) {
         __syncthreads();   // As staged / the previous chunk consumed
         // ---- stage columns j0 .. j0 + 63 of the other side k-major (zeros past nb)
-        if (p.layout == 0) {
-          // 8 lanes read one line's 128 B run of float4s (coalesced), 4 lines per warp; padded transpose into Bs
-          for (int e = tid; e < MX_C * (MT_D / 4); e += 256) {
-            const int cc = (e >> 3) & (MX_C - 1), k4 = ((e >> 9) << 3) | (e & 7);
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (j0 + cc < nb) v = reinterpret_cast<const float4*>(B + (size_t)(bb + j0 + cc) * MT_D)[k4];
-            Bs[(4 * k4) * MX_BLD + cc] = v.x; Bs[(4 * k4 + 1) * MX_BLD + cc] = v.y;
-            Bs[(4 * k4 + 2) * MX_BLD + cc] = v.z; Bs[(4 * k4 + 3) * MX_BLD + cc] = v.w;
-          }
-        } else {
-          const float* __restrict__ y = B + (size_t)bb * MT_D + j0 + c;
-          const bool col = j0 + c < nb;
-          for (int k = rb; k < MT_D; k += 4) Bs[k * MX_BLD + c] = col ? y[(size_t)k * nb] : 0.f;
-        }
+        mx_stage_chunk(Bs, B, p.layout, bb, nb, j0, tid, rb, c);
         __syncthreads();
         if (rb * 8 < nr) {
           float acc[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) acc[i] = 0.f;
-          const float4* __restrict__ a4 = reinterpret_cast<const float4*>(As) + rb * 2;
-#pragma unroll 8
-          for (int k = 0; k < MT_D; ++k) {
-            const float4 x0 = a4[k * (MX_R / 4)], x1 = a4[k * (MX_R / 4) + 1];
-            const float y = Bs[k * MX_BLD + c];
-            acc[0] = fmaf(x0.x, y, acc[0]); acc[1] = fmaf(x0.y, y, acc[1]);
-            acc[2] = fmaf(x0.z, y, acc[2]); acc[3] = fmaf(x0.w, y, acc[3]);
-            acc[4] = fmaf(x1.x, y, acc[4]); acc[5] = fmaf(x1.y, y, acc[5]);
-            acc[6] = fmaf(x1.z, y, acc[6]); acc[7] = fmaf(x1.w, y, acc[7]);
-          }
+          mx_dot8(As, Bs, rb, c, acc);
           const int j = j0 + c;
           if (j < nb) {
             const float sqb = p.dist_mode == 1 ? sq_b[bb + j] : 0.f;
