@@ -667,6 +667,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
     }
   } else {
     // ---------------------------------------------------------------- consumers (2 warpgroups x 64 rows), as gemm_img_kernel
+    // except for the stage release (below)
     ptx::setmaxnreg_inc<232>();
     pdl_wait();   // residual / addend images of op 0 may come from the previous kernel
     const int wg = warp >> 2, q = warp & 3, half = warp >> 2;
@@ -694,13 +695,14 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
             ptx::wg_fence();
             mma_kblock<BN>(d, a_hi, a_hi + Cfg::A_TILE, w_hi, w_hi + Cfg::W_TILE, kb == 0);
             ptx::wg_commit();
-            ptx::wg_wait<1>();
+            // Release the stage as soon as its own MMAs are done, before waiting for the next one.  With two stages,
+            // keeping one k-block of MMAs in flight (wait_group 1) released stage it-1 only after full[it] had
+            // arrived, so the refill of a stage started only when the previous load had landed: one 96 KB load in
+            // flight at a time, and a k-block took a whole load latency (~4.4 us on H100 against ~1.6 us of MMA).
+            ptx::wg_wait<0>();
             ptx::wg_fence_regs(d);
-            if (kb > 0 && lane == 0) ptx::mbar_arrive(&empty[(it - 1) % Cfg::STAGES]);
+            if (lane == 0) ptx::mbar_arrive(&empty[s]);
           }
-          ptx::wg_wait<0>();
-          ptx::wg_fence_regs(d);
-          if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % Cfg::STAGES]);
           if (p.norm != NORM_NONE)
             epi_norm_tile(p, d, mt, q, half, lane, row_a, stg_all, stg, stgb, xch, ready);
           else
