@@ -26,6 +26,8 @@
  *                                 (evaluations/evaluate_pr.py:10-22) for a batch of pairs.
  *   ltr_triplet_loss           <- descriptor_loss.forward (evaluations/criteria.py:35-192) of the validation step
  *                                 (train.py:198-240) + Evaluate_PR.calc_TFPN, for groups of pairs.
+ *   ltr_homography             <- cv2.findHomography(RANSAC) per pair, as the reference's geometry helpers
+ *                                 (models/utils.py:291-412) verify matches, with line matches as well as points.
  *
  * Conventions: return 0 on success, a negative LTR_E_* code on failure (message via
  * ltr_last_error(), thread-local).  All device pointers are caller-owned and must live on
@@ -467,6 +469,70 @@ typedef struct {
 
 /* Asynchronous on `stream`; never synchronises.  n_pairs == 0 writes nothing. */
 int ltr_triplet_loss(const LtrTripletInput* in, const LtrTripletOutput* out, int32_t device, void* stream);
+
+/* RANSAC homographies (image 0 -> image 1) from point and line matches, for a batch of image pairs.  The reference
+ * verifies matches with one cv2.findHomography per pair, points only (models/utils.py:291-412 works the same way for
+ * poses); this is the project's own estimator, DESIGN.md "Homography estimation" states the model:
+ *   - correspondences of pair p: every matched side-0 keypoint row (match in [0, n_pts1[p])) in row order, then every
+ *     matched side-0 segment row in row order; each kind only when its switch is on;
+ *   - per pair and side, coordinates are normalised by the centre and half the larger extent of that side's bounding
+ *     box (points and segment end points);
+ *   - hypothesis k draws 4 distinct correspondences with the counter-based hash
+ *       s = splitmix64(seed + splitmix64((uint64)p << 32 | k)),  draw j = splitmix64(s + j) mod n,  j = 0, 1, ...
+ *     (a duplicate is redrawn with the next j; after 64 draws the hypothesis is rejected) and solves the 8 equations
+ *     (two DLT rows per point, l1^T H a0 = l1^T H b0 = 0 per line, l1 the unit-normal line through s1) with h33 = 1 by
+ *     fp64 Gaussian elimination with partial pivoting; a pivot below 1e-12, a non-finite result or |H33| < 1e-12
+ *     rejects it;
+ *   - residuals are fp64 pixels in image 1: point |pi(H x0) - x1|^2, line the larger squared distance of pi(H a0),
+ *     pi(H b0) to the line through s1; a projected |w| <= FLT_EPSILON makes an outlier; inlier iff residual <
+ *     thresh^2;
+ *   - the winner has the most inliers, the lowest k on a tie; it is refitted by least squares over its inliers
+ *     (smallest eigenvector of A^T A, cyclic Jacobi) and the refit is kept iff it has at least as many inliers.
+ * A pair with fewer than 4 correspondences or no accepted hypothesis is invalid: H is NaN and no row is an inlier.
+ *
+ * Capacity: one pair's correspondences are staged in shared memory, 18 bytes per keypoint row and 58 per segment row,
+ * counted over max_rows_p / max_rows_l of the kinds in use, at most 200 KiB: e.g. 8192 keypoints with 900 segments,
+ * 11377 keypoints alone or 3531 segments alone.  Beyond that the call returns LTR_E_UNSUPPORTED before any launch.
+ * Coordinates must be finite. */
+typedef struct {
+  const float* pts0;              /* device [*, 2] keypoint pool of side 0 */
+  const float* pts1;              /* device [*, 2] keypoint pool of side 1 */
+  const int32_t* pts_off0;        /* device [n_pairs]: pair p's side-0 keypoints start at pts0 row pts_off0[p] */
+  const int32_t* pts_off1;        /* device [n_pairs] */
+  const int32_t* n_pts1;          /* device [n_pairs]: side-1 keypoints of pair p */
+  const int32_t* matches_p;       /* device: local side-1 index or -1 per side-0 keypoint row */
+  const int32_t* cu_p;            /* device [n_pairs + 1]: pair p owns matches_p rows [cu_p[p], cu_p[p+1]) */
+  const float* segs0;             /* device [*, 2, 2] segment pools (start xy, end xy) */
+  const float* segs1;
+  const int32_t* seg_off0;        /* device [n_pairs] */
+  const int32_t* seg_off1;
+  const int32_t* n_segs1;         /* device [n_pairs] */
+  const int32_t* matches_l;       /* device: local side-1 index or -1 per side-0 segment row */
+  const int32_t* cu_l;            /* device [n_pairs + 1] */
+  int32_t n_pairs;
+  int32_t max_rows_p, max_rows_l; /* bounds of every pair's match rows (cu_p / cu_l differences); they size the
+                                     shared-memory staging, and a pair whose rows exceed them is invalid */
+  double thresh;                  /* pixels (3: OpenCV's default) */
+  int32_t n_hypotheses;           /* >= 1 (2048) */
+  uint64_t seed;
+  int32_t use_points, use_lines;  /* 0 / 1: which kinds of correspondence are used */
+} LtrHomographyInput;
+
+/* Outputs (device, caller-owned).  key [n_pairs] is workspace (winning (count << 32) | ~k, 0 = none). */
+typedef struct {
+  double* H;                      /* [n_pairs, 3, 3] */
+  uint8_t* valid;                 /* [n_pairs] */
+  uint8_t* inliers_p;             /* aligned with matches_p (0 for unmatched rows and unused kinds) */
+  uint8_t* inliers_l;             /* aligned with matches_l */
+  int32_t* n_inliers_p;           /* [n_pairs] */
+  int32_t* n_inliers_l;
+  int32_t* hypothesis;            /* [n_pairs] winning hypothesis index, -1 when invalid */
+  int32_t* hypothesis_inliers;    /* [n_pairs] its inlier count */
+  uint64_t* key;
+} LtrHomographyOutput;
+
+/* Asynchronous on `stream`; never synchronises.  n_pairs == 0 writes nothing. */
+int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out, int32_t device, void* stream);
 
 /* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
  * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */

@@ -8,6 +8,9 @@ Match quality against homography ground truth (eval_homography):
     line_assignment, get_precision_recall, homography_ground_truth, score_line_matches
 The validation step's descriptor loss and metrics (eval_criteria; drop-in eval_criteria.descriptor_loss):
     triplet_loss, validation_metrics
+Geometric verification (geometry): RANSAC homographies from line and point matches, batched on the GPU, and the
+homography-estimation metric:
+    estimate_homographies, homography_corner_error
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -35,6 +38,8 @@ _LAZY = {
     "score_line_matches": ("eval_homography", "score_line_matches"),
     "triplet_loss": ("eval_criteria", "triplet_loss"),
     "validation_metrics": ("eval_criteria", "validation_metrics"),
+    "estimate_homographies": ("geometry", "estimate_homographies"),
+    "homography_corner_error": ("geometry", "homography_corner_error"),
 }
 
 

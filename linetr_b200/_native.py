@@ -25,7 +25,7 @@ EXPORTED_SYMBOLS = (
     "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
-    "ltr_line_gt", "ltr_triplet_loss",
+    "ltr_line_gt", "ltr_triplet_loss", "ltr_homography",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
@@ -135,6 +135,21 @@ class LtrTripletOutput(C.Structure):
                 ("hardest_pos", C.c_void_p), ("hardest_neg", C.c_void_p), ("n_valid", C.c_void_p), ("tfpn", C.c_void_p)]
 
 
+class LtrHomographyInput(C.Structure):
+    _fields_ = [("pts0", C.c_void_p), ("pts1", C.c_void_p), ("pts_off0", C.c_void_p), ("pts_off1", C.c_void_p),
+                ("n_pts1", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("segs0", C.c_void_p),
+                ("segs1", C.c_void_p), ("seg_off0", C.c_void_p), ("seg_off1", C.c_void_p), ("n_segs1", C.c_void_p),
+                ("matches_l", C.c_void_p), ("cu_l", C.c_void_p), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32),
+                ("max_rows_l", C.c_int32), ("thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64),
+                ("use_points", C.c_int32), ("use_lines", C.c_int32)]
+
+
+class LtrHomographyOutput(C.Structure):
+    _fields_ = [("H", C.c_void_p), ("valid", C.c_void_p), ("inliers_p", C.c_void_p), ("inliers_l", C.c_void_p),
+                ("n_inliers_p", C.c_void_p), ("n_inliers_l", C.c_void_p), ("hypothesis", C.c_void_p),
+                ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
+
+
 def lib_path() -> str:
     return _LIB_PATH
 
@@ -184,6 +199,8 @@ def load():
     lib.ltr_line_gt.restype = C.c_int
     lib.ltr_triplet_loss.argtypes = [C.POINTER(LtrTripletInput), C.POINTER(LtrTripletOutput), C.c_int32, C.c_void_p]
     lib.ltr_triplet_loss.restype = C.c_int
+    lib.ltr_homography.argtypes = [C.POINTER(LtrHomographyInput), C.POINTER(LtrHomographyOutput), C.c_int32, C.c_void_p]
+    lib.ltr_homography.restype = C.c_int
     lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.ltr_gather_wait.restype = C.c_int
     lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,

@@ -354,6 +354,43 @@ def triplet_loss(desc0, desc1, layout, n_pairs, *, assign, assign_stride, pos, n
     N.check(rc, "ltr_triplet_loss")
 
 
+def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, segs0, segs1, seg_off0,
+               seg_off1, n_segs1, matches_l, cu_l, max_rows_l, H, valid, inliers_p, inliers_l, n_inliers_p, n_inliers_l,
+               hypothesis, hypothesis_inliers, key, thresh=3.0, n_hypotheses=2048, seed=0, use_points=True,
+               use_lines=True):
+    """ltr_homography into caller-allocated outputs: keypoint pools [*,2] / segment pools [*,2,2] fp32, per-pair pool
+    offsets and side-1 counts int32 [P], match rows int32 with offsets cu_p / cu_l [P+1]; H [P,3,3] fp64, valid [P]
+    uint8, inliers_p / inliers_l uint8 aligned with the match rows, counts / hypothesis int32 [P], key [P] int64
+    workspace."""
+    _req_cuda(H, "H")
+    dev = H.device
+    for nm, t, dt in (("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
+                      ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32),
+                      ("matches_p", matches_p, torch.int32), ("cu_p", cu_p, torch.int32), ("segs0", segs0, torch.float32),
+                      ("segs1", segs1, torch.float32), ("seg_off0", seg_off0, torch.int32),
+                      ("seg_off1", seg_off1, torch.int32), ("n_segs1", n_segs1, torch.int32),
+                      ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("H", H, torch.float64),
+                      ("valid", valid, torch.uint8), ("inliers_p", inliers_p, torch.uint8),
+                      ("inliers_l", inliers_l, torch.uint8), ("n_inliers_p", n_inliers_p, torch.int32),
+                      ("n_inliers_l", n_inliers_l, torch.int32), ("hypothesis", hypothesis, torch.int32),
+                      ("hypothesis_inliers", hypothesis_inliers, torch.int32), ("key", key, torch.int64)):
+        if t is None:
+            continue
+        if t.dtype != dt or not t.is_contiguous() or t.device != dev:
+            raise N.LtrError(f"homography: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    inp = _struct(N.LtrHomographyInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
+                  matches_p=matches_p, cu_p=cu_p, segs0=segs0, segs1=segs1, seg_off0=seg_off0, seg_off1=seg_off1,
+                  n_segs1=n_segs1, matches_l=matches_l, cu_l=cu_l, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
+                  max_rows_l=int(max_rows_l), thresh=float(thresh), n_hypotheses=int(n_hypotheses),
+                  seed=int(seed) & 0xFFFFFFFFFFFFFFFF, use_points=int(bool(use_points)), use_lines=int(bool(use_lines)))
+    out = _struct(N.LtrHomographyOutput, H=H, valid=valid, inliers_p=inliers_p, inliers_l=inliers_l,
+                  n_inliers_p=n_inliers_p, n_inliers_l=n_inliers_l, hypothesis=hypothesis,
+                  hypothesis_inliers=hypothesis_inliers, key=key)
+    with torch.cuda.device(dev):
+        rc = N.load().ltr_homography(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_homography")
+
+
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     """ltr_match_distmat on dist [P, n0, n1] (CUDA).  Returns dict(matches0 [P,n0], scores0, nn1, counts)."""
     _req_cuda(dist, "dist_mat")

@@ -41,6 +41,7 @@ enum KernelClass : int {
   KC_MATCH_TAIL,
   KC_LINE_GT,
   KC_TRIPLET,
+  KC_HOMOGRAPHY,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

@@ -21,6 +21,7 @@
 #include "match_tc.cuh"
 #include "line_gt.cuh"
 #include "triplet.cuh"
+#include "homography.cuh"
 
 namespace ltr {
 
@@ -39,7 +40,7 @@ const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
-                                         "triplet"};
+                                         "triplet", "homography"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1190,6 +1191,50 @@ int ltr_triplet_loss(const LtrTripletInput* in, const LtrTripletOutput* out, int
   r.loss = out->loss; r.hardest_pos = out->hardest_pos; r.hardest_neg = out->hardest_neg; r.n_valid = out->n_valid;
   LaunchScope ls(KC_TRIPLET, s);
   LTR_CUDA_TRY(launch_pdl(triplet_reduce_kernel, dim3(in->n_groups), dim3(256), 0, s, r));
+  return LTR_OK;
+}
+
+int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_homography: null argument");
+  if (in->n_pairs < 0 || in->max_rows_p < 0 || in->max_rows_l < 0)
+    return set_error(LTR_E_INVALID, "ltr_homography: negative count");
+  if (in->n_hypotheses < 1 || cdiv(in->n_hypotheses, HG_THREADS) > 65535)
+    return set_error(LTR_E_INVALID, "ltr_homography: n_hypotheses must be in [1, 65535 * 128]");
+  if (!(in->thresh > 0.0) || !std::isfinite(in->thresh)) return set_error(LTR_E_INVALID, "ltr_homography: thresh must be > 0");
+  const int rows_p = in->use_points ? in->max_rows_p : 0, rows_l = in->use_lines ? in->max_rows_l : 0;
+  const long long smem = hg_smem_bytes(rows_p, rows_l, true);
+  if (smem > HG_SMEM_MAX)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_homography: a pair's correspondences need " + std::to_string(smem) +
+                                             " bytes of shared memory (18 per keypoint row, 58 per segment row), over " +
+                                             std::to_string(HG_SMEM_MAX));
+  if (in->n_pairs == 0) return LTR_OK;
+  if (!out->H || !out->valid || !out->n_inliers_p || !out->n_inliers_l || !out->hypothesis || !out->hypothesis_inliers ||
+      !out->key)
+    return set_error(LTR_E_INVALID, "ltr_homography: null output");
+  if (!in->cu_p || !in->cu_l) return set_error(LTR_E_INVALID, "ltr_homography: null offsets");
+  if (in->max_rows_p > 0 && (!in->matches_p || !out->inliers_p)) return set_error(LTR_E_INVALID, "ltr_homography: null point matches");
+  if (in->max_rows_l > 0 && (!in->matches_l || !out->inliers_l)) return set_error(LTR_E_INVALID, "ltr_homography: null line matches");
+  if (rows_p > 0 && (!in->pts0 || !in->pts1 || !in->pts_off0 || !in->pts_off1 || !in->n_pts1))
+    return set_error(LTR_E_INVALID, "ltr_homography: null keypoint pools");
+  if (rows_l > 0 && (!in->segs0 || !in->segs1 || !in->seg_off0 || !in->seg_off1 || !in->n_segs1))
+    return set_error(LTR_E_INVALID, "ltr_homography: null segment pools");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  HomographyArgs a{in->pts0, in->pts1, in->pts_off0, in->pts_off1, in->n_pts1, in->matches_p, in->cu_p,
+                   in->segs0, in->segs1, in->seg_off0, in->seg_off1, in->n_segs1, in->matches_l, in->cu_l,
+                   rows_p, rows_l, in->use_points != 0, in->use_lines != 0, in->thresh * in->thresh, in->n_hypotheses, (unsigned long long)in->seed,
+                   reinterpret_cast<unsigned long long*>(out->key), out->H, out->valid, out->inliers_p, out->inliers_l,
+                   out->n_inliers_p, out->n_inliers_l, out->hypothesis, out->hypothesis_inliers};
+  LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_pairs, s));
+  LTR_CUDA_TRY(ensure_dynamic_smem(homography_hyp_kernel, HG_SMEM_MAX));
+  LTR_CUDA_TRY(ensure_dynamic_smem(homography_refit_kernel, HG_SMEM_MAX));
+  {
+    LaunchScope ls(KC_HOMOGRAPHY, s);
+    LTR_CUDA_TRY(launch_pdl(homography_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, HG_THREADS)), dim3(HG_THREADS),
+                            (size_t)hg_smem_bytes(rows_p, rows_l, false), s, a));
+  }
+  LaunchScope ls(KC_HOMOGRAPHY, s);
+  LTR_CUDA_TRY(launch_pdl(homography_refit_kernel, dim3(in->n_pairs), dim3(HG_REFIT_THREADS), (size_t)smem, s, a));
   return LTR_OK;
 }
 

@@ -262,3 +262,113 @@ def image_to(im: dict, device) -> dict:
     """Tensors of an image dict moved to `device` (klines and shapes untouched)."""
     import torch
     return {k: (v.to(device) if isinstance(v, torch.Tensor) else v) for k, v in im.items()}
+
+
+# ------------------------------------------------------------------ homography-related inputs (geometry)
+def random_homography(rng, w: int = 640, h: int = 480, strength: float = 0.1) -> np.ndarray:
+    """A homography (fp64 [3, 3], H[2, 2] = 1) that moves each image corner by up to strength * (w, h)."""
+    src = np.array([[0, 0], [w - 1, 0], [w - 1, h - 1], [0, h - 1]], dtype=np.float64)
+    dst = src + rng.uniform(-strength, strength, (4, 2)) * [w, h]
+    A = []
+    for (x, y), (u, v) in zip(src, dst):
+        A.append([x, y, 1, 0, 0, 0, -u * x, -u * y, u])
+        A.append([0, 0, 0, x, y, 1, -v * x, -v * y, v])
+    A = np.array(A)
+    hv = np.linalg.solve(A[:, :8], A[:, 8])
+    return np.append(hv, 1.0).reshape(3, 3)
+
+
+def warp_points(H, xy) -> np.ndarray:
+    """xy [..., 2] mapped by H (fp64)."""
+    p = np.asarray(xy, dtype=np.float64)
+    q = p @ np.asarray(H, dtype=np.float64)[:, :2].T + np.asarray(H, dtype=np.float64)[:, 2]
+    return q[..., :2] / q[..., 2:]
+
+
+def make_homography_correspondences(seed: int, n_points: int, n_lines: int, H, w: int = 640, h: int = 480,
+                                    noise_px: float = 0.3, outlier_frac: float = 0.5, min_outlier_px: float = 10.0):
+    """Point and line matches of an image pair related by H (image 0 -> image 1), with a fraction of outliers.
+
+    Row i of side 0 matches row i of side 1 (matches_p / matches_l are the identity).  Inlier keypoints are H(x0) plus
+    N(0, noise_px) per coordinate; inlier segments s1 are H of s0's end points slid along s0 (the line is what counts),
+    plus the same noise.  An outlier keypoint is moved 10 to 100 px (at least min_outlier_px) from H(x0); an outlier
+    segment is moved min_outlier_px + 2 to 60 px along its normal, so no outlier is within min_outlier_px of the true
+    model.  Returns dict kpts0, kpts1 [n, 2] / klines0, klines1 [n, 2, 2] float32, matches_p / matches_l int32 and the
+    true inlier masks true_p / true_l."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    x0 = rng.uniform([0, 0], [w - 1, h - 1], (n_points, 2))
+    x1 = warp_points(H, x0) + rng.normal(0, noise_px, (n_points, 2))
+    out_p = rng.random(n_points) < outlier_frac
+    ang = rng.uniform(0, 2 * np.pi, n_points)
+    r = rng.uniform(max(10.0, min_outlier_px), max(100.0, min_outlier_px + 1), n_points)
+    x1[out_p] = warp_points(H, x0[out_p]) + (r[:, None] * np.stack([np.cos(ang), np.sin(ang)], 1))[out_p]
+    a0 = rng.uniform([20, 20], [w - 21, h - 21], (n_lines, 2))
+    t = rng.uniform(0, 2 * np.pi, n_lines)
+    b0 = a0 + rng.uniform(40, 200, n_lines)[:, None] * np.stack([np.cos(t), np.sin(t)], 1)
+    slide = rng.uniform(-0.1, 0.1, (n_lines, 2))
+    a1 = warp_points(H, a0 + slide[:, :1] * (b0 - a0))
+    b1 = warp_points(H, b0 + slide[:, 1:] * (b0 - a0))
+    out_l = rng.random(n_lines) < outlier_frac
+    d = b1 - a1
+    nrm = np.stack([-d[:, 1], d[:, 0]], 1) / np.maximum(np.linalg.norm(d, axis=1, keepdims=True), 1e-9)
+    shift = (rng.uniform(min_outlier_px + 2, max(60.0, min_outlier_px + 3), n_lines)
+             * rng.choice([-1.0, 1.0], n_lines))[:, None] * nrm
+    a1[out_l] += shift[out_l]
+    b1[out_l] += shift[out_l]
+    a1 += rng.normal(0, noise_px, a1.shape)
+    b1 += rng.normal(0, noise_px, b1.shape)
+    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+    return {"kpts0": f32(x0), "kpts1": f32(x1), "matches_p": np.arange(n_points, dtype=np.int32),
+            "klines0": f32(np.stack([a0, b0], 1).reshape(-1, 2, 2)), "klines1": f32(np.stack([a1, b1], 1).reshape(-1, 2, 2)),
+            "matches_l": np.arange(n_lines, dtype=np.int32), "true_p": ~out_p, "true_l": ~out_l}
+
+
+def _warp_field(coarse, Hinv, xs, ys, w, h):
+    """A smooth scene field (bilinear over the coarse grid `coarse` [1, C, gh, gw] spread over the w x h image) read
+    at the scene positions Hinv(x, y) of the pixel positions xs [n], ys [m]: [1, C, m, n] float32."""
+    import torch
+    gx, gy = np.meshgrid(xs, ys)
+    q = warp_points(Hinv, np.stack([gx, gy], -1))
+    grid = np.stack([(q[..., 0] + 0.5) / w * 2 - 1, (q[..., 1] + 0.5) / h * 2 - 1], -1)[None]
+    return torch.nn.functional.grid_sample(torch.from_numpy(coarse), torch.from_numpy(grid.astype(np.float32)),
+                                           mode="bilinear", padding_mode="border", align_corners=False)
+
+
+def make_homography_set(seed: int, n_views: int, n_lines: int, n_points: int, w: int = 640, h: int = 480,
+                        strength: float = 0.06, jitter_px: float = 0.5, map_noise: float = 0.05, map_cell_px: int = 32):
+    """n_views views of one scene (image dicts as `make_image_set` returns) related by known homographies Hs[v] (scene
+    -> view): key lines and keypoints are the scene's mapped by Hs[v] plus N(0, jitter_px), point descriptors jittered
+    copies of the scene's.  The dense descriptor and score maps are the scene's maps warped by Hs[v] (plus map_noise),
+    so a scene line is sampled at the same scene positions in every view and its line descriptors correspond; the
+    scene maps are smooth (bilinear over a grid of map_cell_px cells) so that resampling at 8 px cells keeps them.  The
+    scene keeps a margin so no view clips it.  Returns (views, Hs [V, 3, 3]); view i -> view j is Hs[j] @ inv(Hs[i])."""
+    import torch
+    rng = np.random.Generator(np.random.PCG64(seed))
+    lo, hi = np.array([0.2 * w, 0.2 * h]), np.array([0.8 * w, 0.8 * h])
+    a = rng.uniform(lo, hi, (n_lines, 2))
+    ang, ln = rng.uniform(0, 2 * np.pi, n_lines), rng.uniform(30, 150, n_lines)
+    b = np.clip(a + ln[:, None] * np.stack([np.cos(ang), np.sin(ang)], 1), lo, hi)
+    octave = rng.integers(0, 2, n_lines)
+    kp = rng.uniform(lo, hi, (n_points, 2))
+    desc = _unit(rng.standard_normal((n_points, D_MODEL)).astype(np.float32))
+    gh, gw = -(-h // map_cell_px), -(-w // map_cell_px)
+    dense = rng.standard_normal((1, D_MODEL, gh, gw)).astype(np.float32)
+    score = rng.uniform(0, 1, (1, 1, gh, gw)).astype(np.float32)
+    cx, cy = np.arange(w // 8) * 8 + 3.5, np.arange(h // 8) * 8 + 3.5   # the pixel of each 8 px descriptor cell
+    views, Hs = [], []
+    for _ in range(n_views):
+        Hv = random_homography(rng, w, h, strength)
+        Hinv = np.linalg.inv(Hv)
+        e = np.concatenate([warp_points(Hv, a), warp_points(Hv, b)], 1) + rng.normal(0, jitter_px, (n_lines, 4))
+        k = (warp_points(Hv, kp) + rng.normal(0, jitter_px, kp.shape)).astype(np.float32)
+        d = _unit(desc + map_noise * rng.standard_normal(desc.shape).astype(np.float32))
+        dn = _warp_field(dense, Hinv, cx, cy, w, h)
+        dn = dn + map_noise * torch.from_numpy(rng.standard_normal(tuple(dn.shape)).astype(np.float32))
+        sm = _warp_field(score, Hinv, np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64), w, h)[0].numpy()
+        s = np.clip(sm + map_noise * rng.standard_normal(sm.shape), 0, 1).astype(np.float32)
+        views.append({"klines": [SyntheticKeyLine(*x, o) for x, o in zip(e, octave)], "image_shape": (1, 1, h, w),
+                      "keypoints": torch.from_numpy(k), "scores": torch.from_numpy(s.reshape(-1)[:len(k)].copy()),
+                      "descriptors": torch.from_numpy(np.ascontiguousarray(d.T)),
+                      "dense_descriptor": torch.nn.functional.normalize(dn, dim=1), "dense_score": torch.from_numpy(s)})
+        Hs.append(Hv)
+    return views, np.stack(Hs)
