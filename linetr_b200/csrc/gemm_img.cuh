@@ -94,7 +94,9 @@ __device__ __forceinline__ void epi_add_rows_f32(const float* __restrict__ X, in
   __syncwarp();
 }
 
-// C[row0 + lane][nbase .. nbase+32) = acc, 256-bit stores: 4 lanes cover one 128-byte row segment
+// C[row0 + lane][nbase .. nbase+32) = acc.  Eight lanes store one row's 128 contiguous bytes (4 rows per instruction),
+// so every 16-byte store instruction writes whole 32-byte sectors: with one lane writing 32 bytes as two 16-byte
+// stores, each instruction wrote half sectors and needed twice the L2 write requests.
 __device__ __forceinline__ void epi_store_rows_f32(float* __restrict__ C, int ldc, int row0, int nbase, int M, int lane,
                                                    float* stg, const float (&acc)[32]) {
 #pragma unroll
@@ -103,13 +105,10 @@ __device__ __forceinline__ void epi_store_rows_f32(float* __restrict__ C, int ld
         make_float4(acc[c4 * 4], acc[c4 * 4 + 1], acc[c4 * 4 + 2], acc[c4 * 4 + 3]);
   __syncwarp();
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int rl = i * 8 + (lane >> 2), c8 = lane & 3;
-    const float4 v0 = *reinterpret_cast<const float4*>(&stg[rl * 32 + (((2 * c8) ^ (rl & 7)) << 2)]);
-    const float4 v1 = *reinterpret_cast<const float4*>(&stg[rl * 32 + (((2 * c8 + 1) ^ (rl & 7)) << 2)]);
-    if (row0 + rl < M)
-      ptx::st_global_256(C + (long long)(row0 + rl) * ldc + nbase + c8 * 8, *reinterpret_cast<const uint4*>(&v0),
-                         *reinterpret_cast<const uint4*>(&v1));
+  for (int i = 0; i < 8; ++i) {
+    const int rl = i * 4 + (lane >> 3), c4 = lane & 7;
+    const float4 v = *reinterpret_cast<const float4*>(&stg[rl * 32 + ((c4 ^ (rl & 7)) << 2)]);
+    if (row0 + rl < M) *reinterpret_cast<float4*>(C + (long long)(row0 + rl) * ldc + nbase + c4 * 4) = v;
   }
   __syncwarp();
 }
@@ -132,27 +131,22 @@ __device__ __forceinline__ void epi_store_image(const ActImg& O, int kb0, int mt
   uint8_t* ohi = reinterpret_cast<uint8_t*>(O.hi + toff);
   uint8_t* olo = reinterpret_cast<uint8_t*>(O.lo + toff);
   const int gch0 = (nbase & 63) >> 3;   // first 16-byte chunk of these 32 columns inside the 64-wide k-block
-  // 256-bit stores: the 4 chunks of a row form one aligned 64-byte group of its 128-byte tile
-  // line; lane pair (2 x 32 B) per row and plane, 16 rows per instruction
+  // the 4 chunks of a row form one aligned 64-byte group of its 128-byte tile line; four lanes store a row's group
+  // (8 rows per instruction and plane), so every 16-byte store instruction writes whole 32-byte sectors
 #pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int rl = i * 16 + (lane >> 1), hp = lane & 1;     // hp: which 32-byte half of the 64-byte group
+  for (int i = 0; i < 4; ++i) {
+    const int rl = i * 8 + (lane >> 2), phys = lane & 3;    // phys: physical chunk (0..3) inside the 64-byte group
     const int r_in = q * 32 + rl;
     // physical chunk index inside the group = (gch0 + cc) ^ (r_in & 7) restricted to the group's 2 low bits
     const int base_phys = (gch0 ^ (r_in & 7)) & 4;          // which 64-byte half of the 128-byte line
-    uint4 vh[2], vl[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int phys = hp * 2 + e;                           // physical chunk (0..3) inside the group
-      const int cc = (phys ^ (r_in & 3));                    // logical chunk stored there (low two bits of the XOR)
-      const int slot = (rl * 4 + (cc ^ ((rl >> 1) & 3))) * 16;
-      vh[e] = *reinterpret_cast<const uint4*>(stgb + slot);
-      vl[e] = *reinterpret_cast<const uint4*>(stgb + 2048 + slot);
-    }
+    const int cc = phys ^ (r_in & 3);                       // logical chunk stored there (low two bits of the XOR)
+    const int slot = (rl * 4 + (cc ^ ((rl >> 1) & 3))) * 16;
+    const uint4 vh = *reinterpret_cast<const uint4*>(stgb + slot);
+    const uint4 vl = *reinterpret_cast<const uint4*>(stgb + 2048 + slot);
     if (row0 + rl < M) {
-      const uint32_t off = (r_in >> 3) * 1024u + (r_in & 7u) * 128u + (uint32_t)(base_phys + hp * 2) * 16u;
-      ptx::st_global_256(ohi + off, vh[0], vh[1]);
-      ptx::st_global_256(olo + off, vl[0], vl[1]);
+      const uint32_t off = (r_in >> 3) * 1024u + (r_in & 7u) * 128u + (uint32_t)(base_phys + phys) * 16u;
+      *reinterpret_cast<uint4*>(ohi + off) = vh;
+      *reinterpret_cast<uint4*>(olo + off) = vl;
     }
   }
   __syncwarp();
@@ -593,6 +587,16 @@ inline int launch_gemm_img(const GemmImgArgs& a, cudaStream_t s, int bn_hint = 0
 // pdl_wait.  BN = 256 only.
 constexpr int CHAIN_MAX_OPS = 4;
 constexpr int CHAIN_MAX_KB = 16;   // output k-blocks of an op that feeds the next one (N <= 1024)
+// k-block timeline of CTA 0 in g_dbg_trace when armed (ltr_debug_trace_arm; tools/gemm_chain_trace.py reads it).
+// k-block it < CHAIN_TRACE_KB of the CTA's walk: slot 3*it = producer has issued the k-block's loads (its empty-wait
+// ended), 3*it + 1 = the consumers' first thread sees its stage landed (full-wait returned), 3*it + 2 = its MMAs are
+// done (wgmma.wait_group 0).  Tile o * 4 + nb of the first m-tile: slot CHAIN_TRACE_EPI + o * 4 + nb = its epilogue
+// is done (an epilogue starts at its last k-block's 3*it + 2).  CHAIN_TRACE_T0 / + 1: producer / consumers past
+// pdl_wait.  Off (the default), a stamp costs its thread an `it` compare and, in the window, a load of g_dbg_on.
+constexpr int CHAIN_TRACE_KB = 36;
+constexpr int CHAIN_TRACE_EPI = 3 * CHAIN_TRACE_KB;
+constexpr int CHAIN_TRACE_T0 = CHAIN_TRACE_EPI + CHAIN_MAX_OPS * 4;
+static_assert(CHAIN_TRACE_T0 + 2 <= 128, "gemm_chain: trace slots");
 struct GemmChainArgs {
   GemmImgArgs op[CHAIN_MAX_OPS];
   int n_ops, m_tiles;
@@ -637,6 +641,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
         ptx::bulk_g2s(st + 2 * Cfg::A_TILE + Cfg::W_TILE, reinterpret_cast<const uint8_t*>(c.op[0].W.lo) + woff, Cfg::W_TILE, &full[kb]);
       }
       pdl_wait();   // the previous kernel's outputs (op 0's A image, residuals, addends) are complete from here on
+      LTR_DBG_STAMP(CHAIN_TRACE_T0);
       uint32_t it = 0, ph = 0;   // ph bit kb: parity of the next kb_ready[kb] phase to wait for
       for (int mt = blockIdx.x; mt < c.m_tiles; mt += gridDim.x)
         for (int o = 0; o < c.n_ops; ++o) {
@@ -655,6 +660,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
                 ptx::bulk_g2s(st + 2 * Cfg::A_TILE, whi + woff, Cfg::W_TILE, &full[s]);
                 ptx::bulk_g2s(st + 2 * Cfg::A_TILE + Cfg::W_TILE, wlo + woff, Cfg::W_TILE, &full[s]);
               }
+              if (it < CHAIN_TRACE_KB) LTR_DBG_STAMP(3 * it);
               if (o > 0 && nb == 0) {   // A k-block kb = output k-block kb of op o-1 for this m-tile
                 ptx::mbar_wait(&kb_ready[kb], (ph >> kb) & 1);
                 ph ^= 1u << kb;
@@ -670,6 +676,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
     // except for the stage release (below)
     ptx::setmaxnreg_inc<232>();
     pdl_wait();   // residual / addend images of op 0 may come from the previous kernel
+    if (tid == 0) LTR_DBG_STAMP(CHAIN_TRACE_T0 + 1);
     const int wg = warp >> 2, q = warp & 3, half = warp >> 2;
     const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);
     float* stg_all = reinterpret_cast<float*>(smem + Cfg::OFF_STG);
@@ -689,6 +696,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
           for (int kb = 0; kb < nk; ++kb, ++it) {
             const int s = it % Cfg::STAGES;
             ptx::mbar_wait(&full[s], (it / Cfg::STAGES) & 1);
+            if (it < CHAIN_TRACE_KB && tid == 0) LTR_DBG_STAMP(3 * it + 1);
             const uint32_t a_hi = ptx::smem_u32(smem + s * Cfg::STAGE) + wg * 8192;
             const uint32_t w_hi = ptx::smem_u32(smem + s * Cfg::STAGE + 2 * Cfg::A_TILE);
             ptx::wg_fence_regs(d);
@@ -702,11 +710,13 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
             ptx::wg_wait<0>();
             ptx::wg_fence_regs(d);
             if (lane == 0) ptx::mbar_arrive(&empty[s]);
+            if (it < CHAIN_TRACE_KB && tid == 0) LTR_DBG_STAMP(3 * it + 2);
           }
           if (p.norm != NORM_NONE)
             epi_norm_tile(p, d, mt, q, half, lane, row_a, stg_all, stg, stgb, xch, ready);
           else
             epi_plain_tile<BN>(p, d, mt, nb, q, half, lane, row_a, stg_all, stg, stgb, ready);
+          if (mt == (int)blockIdx.x && nb < 4 && tid == 0) LTR_DBG_STAMP(CHAIN_TRACE_EPI + o * 4 + nb);
         }
       }
   }
