@@ -28,6 +28,8 @@
  *                                 (train.py:198-240) + Evaluate_PR.calc_TFPN, for groups of pairs.
  *   ltr_homography             <- cv2.findHomography(RANSAC) per pair, as the reference's geometry helpers
  *                                 (models/utils.py:291-412) verify matches, with line matches as well as points.
+ *   ltr_warp_pairs             <- cv2.warpPerspective of the grey and colour images + the eroded valid mask of the
+ *                                 homography dataset builder (dataloaders/build_homography_dataset.py:164-184).
  *
  * Conventions: return 0 on success, a negative LTR_E_* code on failure (message via
  * ltr_last_error(), thread-local).  All device pointers are caller-owned and must live on
@@ -533,6 +535,32 @@ typedef struct {
 
 /* Asynchronous on `stream`; never synchronises.  n_pairs == 0 writes nothing. */
 int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out, int32_t device, void* stream);
+
+/* Homography image pairs <- the warp and valid mask of the homography dataset builder
+ * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where
+ * the warped colour image is 0 in every channel, eroded with a 5 x 5 kernel of ones.
+ *
+ * gray [n_images, height, width] and colour [n_images, height, width, channels] uint8 (device; channels 1 or 3: pass
+ * the grey image for grey-only data).  Pair p warps source image src_index[p] with inv_maps[p] (device fp64 [n_pairs,
+ * 9], row-major M = inv(H), H mapping image 0 to image 1); src_index_host is the same array in host memory, checked
+ * against n_images before any launch.  Outputs (device): warped and mask [n_pairs, height, width] uint8, mask 1 = valid.
+ *
+ * The warp is OpenCV's fixed-point INTER_LINEAR with BORDER_CONSTANT 0, bit for bit: with bw = min(1024 /
+ * min(16, height), width) and output column x = xb + j of the column block xb = x - x % bw, row y:
+ *   X0 = M0*xb + M1*y + M2, Y0 = M3*xb + M4*y + M5, W0 = M6*xb + M7*y + M8   (fp64, round to nearest, no FMA)
+ *   w = W0 + M6*j;  w = w != 0 ? 32 / w : 0;  X = rint(clamp((X0 + M0*j) * w)), Y = rint(clamp((Y0 + M3*j) * w))
+ *   cell (X >> 5, Y >> 5), sub-pixel (fx, fy) = (X & 31, Y & 31); neighbours (0,0) (0,1) (1,0) (1,1) weigh
+ *   (32-fx)(32-fy)*32, fx(32-fy)*32, (32-fx)fy*32, fx*fy*32; outside the image they are 0;
+ *   pixel = (sum of weight * value + 16384) >> 15.
+ * Before the erosion a pixel is valid iff an in-image neighbour with a nonzero weight has a nonzero channel; the 5 x 5
+ * erosion counts pixels outside the image as valid.
+ *
+ * Errors before any launch: LTR_E_INVALID for n_images < 1, n_pairs < 0, a null pointer or a src_index outside
+ * [0, n_images); LTR_E_UNSUPPORTED for a side outside [1, 32767] or channels other than 1 and 3.  n_pairs == 0 writes
+ * nothing.  Writes only warped and mask; asynchronous on `stream`, never synchronises. */
+int ltr_warp_pairs(const uint8_t* gray, const uint8_t* colour, int32_t n_images, int32_t height, int32_t width,
+                   int32_t channels, const int32_t* src_index_host, const int32_t* src_index, const double* inv_maps,
+                   int32_t n_pairs, uint8_t* warped, uint8_t* mask, int32_t device, void* stream);
 
 /* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
  * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */

@@ -11,6 +11,8 @@ The validation step's descriptor loss and metrics (eval_criteria; drop-in eval_c
 Geometric verification (geometry): RANSAC homographies from line and point matches, batched on the GPU, and the
 homography-estimation metric:
     estimate_homographies, homography_corner_error
+Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
+    sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -40,6 +42,10 @@ _LAZY = {
     "validation_metrics": ("eval_criteria", "validation_metrics"),
     "estimate_homographies": ("geometry", "estimate_homographies"),
     "homography_corner_error": ("geometry", "homography_corner_error"),
+    "sample_homographies": ("homography_pairs", "sample_homographies"),
+    "warp_pairs": ("homography_pairs", "warp_pairs"),
+    "homography_pairs": ("homography_pairs", "homography_pairs"),
+    "apply_valid_masks": ("homography_pairs", "apply_valid_masks"),
 }
 
 

@@ -25,7 +25,7 @@ EXPORTED_SYMBOLS = (
     "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
-    "ltr_line_gt", "ltr_triplet_loss", "ltr_homography",
+    "ltr_line_gt", "ltr_triplet_loss", "ltr_homography", "ltr_warp_pairs",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
@@ -201,6 +201,10 @@ def load():
     lib.ltr_triplet_loss.restype = C.c_int
     lib.ltr_homography.argtypes = [C.POINTER(LtrHomographyInput), C.POINTER(LtrHomographyOutput), C.c_int32, C.c_void_p]
     lib.ltr_homography.restype = C.c_int
+    lib.ltr_warp_pairs.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [c_int32_p, C.c_void_p, C.c_void_p,
+                                                                             C.c_int32, C.c_void_p, C.c_void_p,
+                                                                             C.c_int32, C.c_void_p]
+    lib.ltr_warp_pairs.restype = C.c_int
     lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.ltr_gather_wait.restype = C.c_int
     lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,

@@ -391,6 +391,30 @@ def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu
     N.check(rc, "ltr_homography")
 
 
+def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
+    """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
+    (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""
+    dev = gray.device
+    if gray.dim() != 3 or colour.dim() != 4 or tuple(colour.shape[:3]) != tuple(gray.shape):
+        raise N.LtrError(f"warp_pairs: gray must be [N,h,w] and colour [N,h,w,C], got {list(gray.shape)} and "
+                         f"{list(colour.shape)}")
+    P = len(src_index_host)
+    for nm, t, dt, shape in (("gray", gray, torch.uint8, None), ("colour", colour, torch.uint8, None),
+                             ("src_index", src_index, torch.int32, (P,)), ("inv_maps", inv_maps, torch.float64, (P, 9)),
+                             ("warped", warped, torch.uint8, (P, *gray.shape[1:])),
+                             ("mask", mask, torch.uint8, (P, *gray.shape[1:]))):
+        if t.dtype != dt or not t.is_contiguous() or t.device != dev or (shape is not None and tuple(t.shape) != shape):
+            raise N.LtrError(f"warp_pairs: '{nm}' must be a contiguous {dt} tensor on {dev}"
+                             + (f" of shape {list(shape)}" if shape is not None else ""))
+    n, h, w = (int(s) for s in gray.shape)
+    idx = np.ascontiguousarray(src_index_host, dtype=np.int32)
+    with torch.cuda.device(dev):
+        rc = N.load().ltr_warp_pairs(_ptr(gray), _ptr(colour), n, h, w, int(colour.shape[3]),
+                                     idx.ctypes.data_as(N.c_int32_p), _ptr(src_index), _ptr(inv_maps), P, _ptr(warped),
+                                     _ptr(mask), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_warp_pairs")
+
+
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     """ltr_match_distmat on dist [P, n0, n1] (CUDA).  Returns dict(matches0 [P,n0], scores0, nn1, counts)."""
     _req_cuda(dist, "dist_mat")

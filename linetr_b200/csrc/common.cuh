@@ -42,6 +42,7 @@ enum KernelClass : int {
   KC_LINE_GT,
   KC_TRIPLET,
   KC_HOMOGRAPHY,
+  KC_WARP,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

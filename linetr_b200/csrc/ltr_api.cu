@@ -22,6 +22,7 @@
 #include "line_gt.cuh"
 #include "triplet.cuh"
 #include "homography.cuh"
+#include "warp.cuh"
 
 namespace ltr {
 
@@ -40,7 +41,7 @@ const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
-                                         "triplet", "homography"};
+                                         "triplet", "homography", "warp"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1235,6 +1236,31 @@ int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out,
   }
   LaunchScope ls(KC_HOMOGRAPHY, s);
   LTR_CUDA_TRY(launch_pdl(homography_refit_kernel, dim3(in->n_pairs), dim3(HG_REFIT_THREADS), (size_t)smem, s, a));
+  return LTR_OK;
+}
+
+int ltr_warp_pairs(const uint8_t* gray, const uint8_t* colour, int32_t n_images, int32_t height, int32_t width,
+                   int32_t channels, const int32_t* src_index_host, const int32_t* src_index, const double* inv_maps,
+                   int32_t n_pairs, uint8_t* warped, uint8_t* mask, int32_t device, void* stream) {
+  if (n_images < 1 || n_pairs < 0) return set_error(LTR_E_INVALID, "ltr_warp_pairs: n_images must be >= 1 and n_pairs >= 0");
+  if (height < 1 || width < 1 || height > WP_MAX_SIDE || width > WP_MAX_SIDE)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_warp_pairs: height and width must be in [1, 32767]");
+  if (channels != 1 && channels != 3) return set_error(LTR_E_UNSUPPORTED, "ltr_warp_pairs: channels must be 1 or 3");
+  if (n_pairs == 0) return LTR_OK;
+  if (!gray || !colour || !src_index_host || !src_index || !inv_maps || !warped || !mask)
+    return set_error(LTR_E_INVALID, "ltr_warp_pairs: null argument");
+  for (int32_t p = 0; p < n_pairs; ++p)
+    if (src_index_host[p] < 0 || src_index_host[p] >= n_images)
+      return set_error(LTR_E_INVALID, "ltr_warp_pairs: src_index[" + std::to_string(p) + "] = " +
+                                          std::to_string(src_index_host[p]) + " is not an image index");
+  const int tiles_x = cdiv(width, WP_TW), tiles = tiles_x * cdiv(height, WP_TH);
+  if ((long long)tiles * n_pairs > INT_MAX) return set_error(LTR_E_UNSUPPORTED, "ltr_warp_pairs: too many output tiles");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  WarpArgs a{gray, colour, src_index, inv_maps, warped, mask, n_images, height, width, channels,
+             std::min(1024 / std::min(16, (int)height), (int)width), tiles_x, tiles};
+  LaunchScope ls(KC_WARP, s);
+  LTR_CUDA_TRY(launch_pdl(warp_pairs_kernel, dim3(tiles * n_pairs), dim3(WP_THREADS), 0, s, a));
   return LTR_OK;
 }
 

@@ -372,3 +372,26 @@ def make_homography_set(seed: int, n_views: int, n_lines: int, n_points: int, w:
                       "dense_descriptor": torch.nn.functional.normalize(dn, dim=1), "dense_score": torch.from_numpy(s)})
         Hs.append(Hv)
     return views, np.stack(Hs)
+
+
+def make_warp_images(seed: int, n: int, h: int, w: int):
+    """n seeded uint8 images for the homography warp: colour [n, h, w, 3] (gradients, rectangles with hard edges, noise
+    and regions that are black in every channel) and grey [n, h, w] from it (BT.601 weights, rounded)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    yy, xx = np.mgrid[0:h, 0:w].astype(np.float64)
+    colour = np.empty((n, h, w, 3), dtype=np.uint8)
+    for i in range(n):
+        img = np.stack([(xx * rng.uniform(0.2, 2) + yy * rng.uniform(-1, 1) + rng.uniform(0, 255)) % 256
+                        for _ in range(3)], -1)
+        for _ in range(6):
+            y0, x0 = rng.integers(0, h), rng.integers(0, w)
+            y1, x1 = y0 + rng.integers(1, h // 2 + 2), x0 + rng.integers(1, w // 2 + 2)
+            img[y0:y1, x0:x1] = rng.uniform(0, 255, 3)
+        img += rng.normal(0, 6, img.shape)
+        img = np.clip(np.rint(img), 0, 255)
+        for _ in range(2):
+            y0, x0 = rng.integers(0, h), rng.integers(0, w)
+            img[y0:y0 + rng.integers(1, h // 3 + 2), x0:x0 + rng.integers(1, w // 3 + 2)] = 0
+        colour[i] = img
+    gray = np.rint(colour.astype(np.float64) @ np.array([0.114, 0.587, 0.299])).astype(np.uint8)
+    return gray, colour
