@@ -28,6 +28,8 @@
  *                                 (train.py:198-240) + Evaluate_PR.calc_TFPN, for groups of pairs.
  *   ltr_homography             <- cv2.findHomography(RANSAC) per pair, as the reference's geometry helpers
  *                                 (models/utils.py:291-412) verify matches, with line matches as well as points.
+ *   ltr_essential              <- estimate_pose (models/utils.py:291-315): cv2.findEssentialMat(RANSAC) +
+ *                                 cv2.recoverPose per pair, batched.
  *   ltr_warp_pairs             <- cv2.warpPerspective of the grey and colour images + the eroded valid mask of the
  *                                 homography dataset builder (dataloaders/build_homography_dataset.py:164-184).
  *
@@ -535,6 +537,63 @@ typedef struct {
 
 /* Asynchronous on `stream`; never synchronises.  n_pairs == 0 writes nothing. */
 int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out, int32_t device, void* stream);
+
+/* Relative pose of calibrated image pairs <- estimate_pose (models/utils.py:291-315): cv2.findEssentialMat(RANSAC) +
+ * cv2.recoverPose per pair on the CPU.  Five-point RANSAC essential matrices and the pose, for a batch of pairs; DESIGN.md
+ * "Relative pose" states the model:
+ *   - correspondences of pair p: every matched side-0 keypoint row (match in [0, n_pts1[p])) in row order with its
+ *     partner, in normalised coordinates x = (k - c) / f per axis (K0[p] for side 0, K1[p] for side 1; fp64, correctly
+ *     rounded division);
+ *   - threshold as the reference: f_mean = (((K0[0,0] + K1[1,1]) + K0[0,0]) + K1[1,1]) / 4, t_n = thresh / f_mean; an
+ *     inlier has Sampson error (x1^T E x0)^2 / ((E x0)_0^2 + (E x0)_1^2 + (E^T x1)_0^2 + (E^T x1)_1^2) < t_n^2,
+ *     evaluated as (x1^T E x0)^2 < t_n^2 * (the denominator);
+ *   - hypothesis k draws 5 distinct correspondences with ltr_homography's hash and redraw rule and solves them with
+ *     Nister's five-point method (QR null space, 10 x 20 Gauss-Jordan, degree-10 determinant, Sturm chain and
+ *     bisection) in explicitly rounded fp64: up to 10 solutions j (real root j in ascending order);
+ *   - the winner has the most inliers, then the lowest k, then the lowest j; no refit;
+ *   - E is scaled to unit Frobenius norm with its largest-magnitude entry positive; of its four (R, t) candidates the
+ *     one with the most inliers of depth in (0, dist_thresh) in both cameras wins; |t| = 1.  X1 = R X0 + t.
+ * A pair with fewer than 5 correspondences, no finite solution, or more match rows than max_rows_p is invalid: E, R and
+ * t are NaN, no row is an inlier, hypothesis is -1.
+ *
+ * Capacity: one pair's correspondences are staged in shared memory, 33 bytes per keypoint row over max_rows_p, at most
+ * 200 KiB (6206 rows).  Beyond that the call returns LTR_E_UNSUPPORTED before any launch.  Coordinates and K must be
+ * finite, with fx, fy > 0. */
+typedef struct {
+  const float* pts0;              /* device [*, 2] keypoint pool of side 0 */
+  const float* pts1;              /* device [*, 2] keypoint pool of side 1 */
+  const int32_t* pts_off0;        /* device [n_pairs]: pair p's side-0 keypoints start at pts0 row pts_off0[p] */
+  const int32_t* pts_off1;        /* device [n_pairs] */
+  const int32_t* n_pts1;          /* device [n_pairs]: side-1 keypoints of pair p */
+  const int32_t* matches_p;       /* device: local side-1 index or -1 per side-0 keypoint row */
+  const int32_t* cu_p;            /* device [n_pairs + 1]: pair p owns matches_p rows [cu_p[p], cu_p[p+1]) */
+  const double* K0;               /* device [n_pairs, 3, 3] intrinsics of side 0 */
+  const double* K1;               /* device [n_pairs, 3, 3] intrinsics of side 1 */
+  int32_t n_pairs;
+  int32_t max_rows_p;             /* bound of every pair's match rows; sizes the staging, a pair over it is invalid */
+  double thresh;                  /* pixels (the reference's evaluation passes 1) */
+  double dist_thresh;             /* cheirality depth limit in units of |t| (1e9, as the reference's recoverPose) */
+  int32_t n_hypotheses;           /* >= 1 (1024) */
+  uint64_t seed;
+} LtrEssentialInput;
+
+/* Outputs (device, caller-owned).  key [n_pairs] is workspace (winning (count << 32) | ~(10 k + j), 0 = none). */
+typedef struct {
+  double* E;                      /* [n_pairs, 3, 3] essential matrix, x1^T E x0 = 0 in normalised coordinates */
+  double* R;                      /* [n_pairs, 3, 3] */
+  double* t;                      /* [n_pairs, 3] unit */
+  uint8_t* valid;                 /* [n_pairs] */
+  uint8_t* inliers_p;             /* aligned with matches_p (0 for unmatched rows) */
+  int32_t* n_inliers;             /* [n_pairs] */
+  int32_t* n_cheirality;          /* [n_pairs] inliers in front of both cameras under (R, t) */
+  int32_t* hypothesis;            /* [n_pairs] 10 k + j of the winning solution, -1 when invalid */
+  int32_t* hypothesis_inliers;    /* [n_pairs] its inlier count */
+  uint64_t* key;
+} LtrEssentialOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments, LTR_E_UNSUPPORTED over
+ * capacity) come before any launch.  n_pairs == 0 writes nothing. */
+int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, int32_t device, void* stream);
 
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where

@@ -11,6 +11,9 @@ The validation step's descriptor loss and metrics (eval_criteria; drop-in eval_c
 Geometric verification (geometry): RANSAC homographies from line and point matches, batched on the GPU, and the
 homography-estimation metric:
     estimate_homographies, homography_corner_error
+Relative pose (geometry): five-point RANSAC essential matrices and the pose of calibrated pairs, batched on the GPU, and
+the reference's pose metrics:
+    estimate_poses, compute_epipolar_error, compute_pose_error, pose_auc, pose_errors
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 `install_as_reference_models()` registers this package's modules under the reference's
@@ -42,6 +45,11 @@ _LAZY = {
     "validation_metrics": ("eval_criteria", "validation_metrics"),
     "estimate_homographies": ("geometry", "estimate_homographies"),
     "homography_corner_error": ("geometry", "homography_corner_error"),
+    "estimate_poses": ("geometry", "estimate_poses"),
+    "compute_epipolar_error": ("geometry", "compute_epipolar_error"),
+    "compute_pose_error": ("geometry", "compute_pose_error"),
+    "pose_auc": ("geometry", "pose_auc"),
+    "pose_errors": ("geometry", "pose_errors"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

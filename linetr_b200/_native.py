@@ -25,7 +25,7 @@ EXPORTED_SYMBOLS = (
     "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
-    "ltr_line_gt", "ltr_triplet_loss", "ltr_homography", "ltr_warp_pairs",
+    "ltr_line_gt", "ltr_triplet_loss", "ltr_homography", "ltr_warp_pairs", "ltr_essential",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
@@ -150,6 +150,19 @@ class LtrHomographyOutput(C.Structure):
                 ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
 
 
+class LtrEssentialInput(C.Structure):
+    _fields_ = [("pts0", C.c_void_p), ("pts1", C.c_void_p), ("pts_off0", C.c_void_p), ("pts_off1", C.c_void_p),
+                ("n_pts1", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("K0", C.c_void_p),
+                ("K1", C.c_void_p), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32), ("thresh", C.c_double),
+                ("dist_thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64)]
+
+
+class LtrEssentialOutput(C.Structure):
+    _fields_ = [("E", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("valid", C.c_void_p),
+                ("inliers_p", C.c_void_p), ("n_inliers", C.c_void_p), ("n_cheirality", C.c_void_p),
+                ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
+
+
 def lib_path() -> str:
     return _LIB_PATH
 
@@ -201,6 +214,8 @@ def load():
     lib.ltr_triplet_loss.restype = C.c_int
     lib.ltr_homography.argtypes = [C.POINTER(LtrHomographyInput), C.POINTER(LtrHomographyOutput), C.c_int32, C.c_void_p]
     lib.ltr_homography.restype = C.c_int
+    lib.ltr_essential.argtypes = [C.POINTER(LtrEssentialInput), C.POINTER(LtrEssentialOutput), C.c_int32, C.c_void_p]
+    lib.ltr_essential.restype = C.c_int
     lib.ltr_warp_pairs.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [c_int32_p, C.c_void_p, C.c_void_p,
                                                                              C.c_int32, C.c_void_p, C.c_void_p,
                                                                              C.c_int32, C.c_void_p]

@@ -391,6 +391,38 @@ def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu
     N.check(rc, "ltr_homography")
 
 
+def essential(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, K0, K1, E, R, t, valid,
+              inliers_p, n_inliers, n_cheirality, hypothesis, hypothesis_inliers, key, thresh=1.0, dist_thresh=1e9,
+              n_hypotheses=1024, seed=0):
+    """ltr_essential into caller-allocated outputs: keypoint pools [*,2] fp32, per-pair pool offsets and side-1 counts
+    int32 [P], match rows int32 with offsets cu_p [P+1], intrinsics K0 / K1 fp64 [P,3,3]; E / R [P,3,3] and t [P,3]
+    fp64, valid [P] uint8, inliers_p uint8 aligned with the match rows, counts / hypothesis int32 [P], key [P] int64
+    workspace."""
+    _req_cuda(E, "E")
+    dev = E.device
+    for nm, tt, dt in (("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
+                       ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32),
+                       ("matches_p", matches_p, torch.int32), ("cu_p", cu_p, torch.int32), ("K0", K0, torch.float64),
+                       ("K1", K1, torch.float64), ("E", E, torch.float64), ("R", R, torch.float64),
+                       ("t", t, torch.float64), ("valid", valid, torch.uint8), ("inliers_p", inliers_p, torch.uint8),
+                       ("n_inliers", n_inliers, torch.int32), ("n_cheirality", n_cheirality, torch.int32),
+                       ("hypothesis", hypothesis, torch.int32), ("hypothesis_inliers", hypothesis_inliers, torch.int32),
+                       ("key", key, torch.int64)):
+        if tt is None:
+            continue
+        if tt.dtype != dt or not tt.is_contiguous() or tt.device != dev:
+            raise N.LtrError(f"essential: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    inp = _struct(N.LtrEssentialInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
+                  matches_p=matches_p, cu_p=cu_p, K0=K0, K1=K1, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
+                  thresh=float(thresh), dist_thresh=float(dist_thresh), n_hypotheses=int(n_hypotheses),
+                  seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
+    out = _struct(N.LtrEssentialOutput, E=E, R=R, t=t, valid=valid, inliers_p=inliers_p, n_inliers=n_inliers,
+                  n_cheirality=n_cheirality, hypothesis=hypothesis, hypothesis_inliers=hypothesis_inliers, key=key)
+    with torch.cuda.device(dev):
+        rc = N.load().ltr_essential(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_essential")
+
+
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
     """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
     (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""

@@ -43,6 +43,7 @@ enum KernelClass : int {
   KC_TRIPLET,
   KC_HOMOGRAPHY,
   KC_WARP,
+  KC_ESSENTIAL,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

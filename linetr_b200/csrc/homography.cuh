@@ -25,6 +25,7 @@
 //   homography_refit_kernel  grid (pair): the winner again, A^T A, Jacobi, both inlier passes, the outputs.
 #pragma once
 #include "common.cuh"
+#include "ransac_common.cuh"
 
 namespace ltr {
 
@@ -33,7 +34,6 @@ constexpr int HG_REFIT_THREADS = 256;
 constexpr int HG_PT_BYTES = 16;         // shared bytes per point: x0, y0, x1, y1 fp32
 constexpr int HG_LN_BYTES = 56;         // per line: s0, s1 (4 fp32 each) and the pixel line through s1 (3 fp64)
 constexpr int HG_SMEM_MAX = 200 * 1024; // staging capacity of one pair (see hg_smem_bytes)
-constexpr int HG_MAX_DRAWS = 64;
 constexpr int HG_JACOBI_SWEEPS = 32;
 constexpr double HG_FLT_EPS = 1.1920928955078125e-07;
 
@@ -86,39 +86,6 @@ __device__ __forceinline__ HgStage hg_stage_ptrs(unsigned char* base, int rows_p
 #define HG_M __dmul_rn
 #define HG_A __dadd_rn
 #define HG_S __dsub_rn
-
-__device__ __forceinline__ unsigned long long hg_splitmix64(unsigned long long x) {
-  unsigned long long z = x + 0x9E3779B97F4A7C15ull;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-  return z ^ (z >> 31);
-}
-
-// Row-ordered compaction of the matched rows [b, e) of a match array: f(local row, match, compact index or -1) for
-// every row.  All threads of the block must call it.
-template <int NT, typename F>
-__device__ __forceinline__ int hg_compact(const int* __restrict__ match, int b, int e, int n1, int* warp_cnt, F f) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  int base = 0;
-  for (int r0 = b; r0 < e; r0 += NT) {
-    const int r = r0 + threadIdx.x;
-    const int m = r < e ? match[r] : -1;
-    const bool ok = r < e && m >= 0 && m < n1;
-    const unsigned bal = __ballot_sync(0xffffffffu, ok);
-    if (lane == 0) warp_cnt[w] = __popc(bal);
-    __syncthreads();
-    int off = base, tot = 0;
-#pragma unroll
-    for (int i = 0; i < NT / 32; ++i) {
-      off += i < w ? warp_cnt[i] : 0;
-      tot += warp_cnt[i];
-    }
-    if (r < e) f(r - b, m, ok ? off + __popc(bal & ((1u << lane) - 1u)) : -1);
-    __syncthreads();
-    base += tot;
-  }
-  return base;
-}
 
 // Stage pair p's correspondences and its normalisation.  Ends with __syncthreads.
 template <int NT>
@@ -267,16 +234,8 @@ __device__ __forceinline__ bool hg_to_pixels(const HgPair& sp, const double* h, 
 __device__ __noinline__ bool hg_hypothesis(const HgStage& st, const HgPair& sp, unsigned long long seed, int p, int k,
                                            double* H) {
   const int n = sp.np + sp.nl;
-  const unsigned long long s = hg_splitmix64(seed + hg_splitmix64(((unsigned long long)(unsigned)p << 32) | (unsigned)k));
   int idx[4];
-  int got = 0;
-  for (int j = 0; j < HG_MAX_DRAWS && got < 4; ++j) {
-    const int v = (int)(hg_splitmix64(s + (unsigned long long)j) % (unsigned long long)n);
-    bool dup = false;
-    for (int q = 0; q < got; ++q) dup |= idx[q] == v;
-    if (!dup) idx[got++] = v;
-  }
-  if (got < 4) return false;
+  if (!hg_draw<4>(seed, p, k, n, idx)) return false;
   double A[8][9];
   for (int q = 0; q < 4; ++q) {
     double r0[9], r1[9];

@@ -23,6 +23,7 @@
 #include "triplet.cuh"
 #include "homography.cuh"
 #include "warp.cuh"
+#include "essential.cuh"
 
 namespace ltr {
 
@@ -41,7 +42,7 @@ const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
-                                         "triplet", "homography", "warp"};
+                                         "triplet", "homography", "warp", "essential"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1236,6 +1237,45 @@ int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out,
   }
   LaunchScope ls(KC_HOMOGRAPHY, s);
   LTR_CUDA_TRY(launch_pdl(homography_refit_kernel, dim3(in->n_pairs), dim3(HG_REFIT_THREADS), (size_t)smem, s, a));
+  return LTR_OK;
+}
+
+int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_essential: null argument");
+  if (in->n_pairs < 0 || in->max_rows_p < 0) return set_error(LTR_E_INVALID, "ltr_essential: negative count");
+  if (in->n_hypotheses < 1 || cdiv(in->n_hypotheses, ESS_THREADS) > 65535)
+    return set_error(LTR_E_INVALID, "ltr_essential: n_hypotheses must be in [1, 65535 * 128]");
+  if (!(in->thresh > 0.0) || !std::isfinite(in->thresh)) return set_error(LTR_E_INVALID, "ltr_essential: thresh must be > 0");
+  if (!(in->dist_thresh > 0.0)) return set_error(LTR_E_INVALID, "ltr_essential: dist_thresh must be > 0");
+  const long long smem = ess_smem_bytes(in->max_rows_p, true);
+  if (smem > ESS_SMEM_MAX)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_essential: a pair's correspondences need " + std::to_string(smem) +
+                                            " bytes of shared memory (33 per keypoint row), over " +
+                                            std::to_string(ESS_SMEM_MAX));
+  if (in->n_pairs == 0) return LTR_OK;
+  if (!out->E || !out->R || !out->t || !out->valid || !out->n_inliers || !out->n_cheirality || !out->hypothesis ||
+      !out->hypothesis_inliers || !out->key)
+    return set_error(LTR_E_INVALID, "ltr_essential: null output");
+  if (!in->cu_p || !in->K0 || !in->K1) return set_error(LTR_E_INVALID, "ltr_essential: null offsets or intrinsics");
+  if (in->max_rows_p > 0 && (!in->matches_p || !out->inliers_p || !in->pts0 || !in->pts1 || !in->pts_off0 ||
+                             !in->pts_off1 || !in->n_pts1))
+    return set_error(LTR_E_INVALID, "ltr_essential: null keypoint pools or matches");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  EssentialArgs a{in->pts0, in->pts1, in->pts_off0, in->pts_off1, in->n_pts1, in->matches_p, in->cu_p, in->K0, in->K1,
+                  in->max_rows_p, in->thresh, in->dist_thresh, in->n_hypotheses, (unsigned long long)in->seed,
+                  reinterpret_cast<unsigned long long*>(out->key), out->E, out->R, out->t, out->valid, out->inliers_p,
+                  out->n_inliers, out->n_cheirality, out->hypothesis, out->hypothesis_inliers};
+  LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_pairs, s));
+  LTR_CUDA_TRY(ensure_dynamic_smem(essential_hyp_kernel, ESS_SMEM_MAX));
+  LTR_CUDA_TRY(ensure_dynamic_smem(essential_pose_kernel, ESS_SMEM_MAX));
+  {
+    LaunchScope ls(KC_ESSENTIAL, s);
+    LTR_CUDA_TRY(launch_pdl(essential_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, ESS_THREADS)),
+                            dim3(ESS_THREADS), (size_t)ess_smem_bytes(in->max_rows_p, false), s, a));
+  }
+  LaunchScope ls(KC_ESSENTIAL, s);
+  LTR_CUDA_TRY(launch_pdl(essential_pose_kernel, dim3(in->n_pairs), dim3(ESS_POSE_THREADS), (size_t)smem, s, a));
   return LTR_OK;
 }
 

@@ -1,4 +1,5 @@
-"""Geometric verification of matches: RANSAC homographies from line and point matches, and the corner-error metric.
+"""Geometric verification of matches: RANSAC homographies from line and point matches, the corner-error metric, and
+the relative pose of calibrated pairs with the reference's pose metrics.
 
     estimate_homographies(res: ImagePairMatches, thresh=3.0, n_hypotheses=2048, seed=0, use_lines=True,
                           use_points=True) -> HomographyResult
@@ -21,6 +22,28 @@ Residuals are in pixels of image 1: a point's |pi(H x0) - x1|^2 (OpenCV's reproj
 distance of pi(H a0), pi(H b0) to the line through s1; |w| <= FLT_EPSILON makes an outlier; inlier iff < thresh^2.
 The winner has the most inliers (lowest k on a tie) and is refitted by least squares over its inliers, kept iff the
 refit has at least as many inliers.
+
+    estimate_poses(res, K0, K1, thresh=1.0, n_hypotheses=1024, seed=0, dist_thresh=1e9) -> PoseResult
+        one `ltr_essential` call for every pair of a `match_images` / `match_sets` result; device outputs, no
+        synchronisation
+    ransac_essential_host(kpts0, kpts1, matches_p, K0, K1, pair=0, ...) -> dict
+        the same model for one pair in numpy: everything up to the winner is the kernels' operations in the kernels'
+        order (the winning sample, root and inlier count are the same bits); the decomposition uses np.linalg.svd
+    compute_epipolar_error, compute_pose_error, pose_auc: the reference's metrics (models/utils.py:358-412);
+    pose_errors(R, t, T_0to1): compute_pose_error over a batch of pairs
+
+The relative-pose model (DESIGN.md "Relative pose", include/linetr_b200.h `ltr_essential`): the correspondences of a
+pair are its matched side-0 keypoints in row order with their partners, in normalised coordinates (k - c) / f.
+t_n = thresh / f_mean with the reference's f_mean = mean(K0[0,0], K1[1,1], K0[0,0], K1[1,1]); an inlier has Sampson
+error < t_n^2, evaluated as (x1^T E x0)^2 < t_n^2 * den.  Hypothesis k draws 5 distinct correspondences
+(`draw_samples(..., size=5)`) and solves them with Nister's five-point method: the null basis of the 5 epipolar rows
+from a Householder QR, the 10 x 20 cubic constraints, Gauss-Jordan with partial pivoting, the degree-10 determinant
+of the hidden-variable matrix, its real roots by a Sturm chain and bisection (`sturm_roots`), (x, y) from the null
+vector; solution j is real root j.  Every operation is one explicitly rounded fp64 operation (no FMA).  The winner has
+the most inliers, then the lowest k, then the lowest j.  E is scaled to unit Frobenius norm (largest |entry| positive);
+of its four (R, t) candidates the one with the most inliers in front of both cameras wins (depths from the 2 x 2 normal
+equations of d1 x1 = d0 R x0 + t in (0, dist_thresh)).  No refit.  Fewer than 5 correspondences or no finite E makes
+the pair invalid.
 """
 from __future__ import annotations
 
@@ -50,24 +73,25 @@ def splitmix64(x) -> np.ndarray:
     return z ^ (z >> _U64(31))
 
 
-def draw_samples(seed: int, pair: int, n_hypotheses: int, n: int):
-    """The 4 correspondence indices of hypotheses 0..n_hypotheses-1 of `pair` among n: s = splitmix64(seed +
-    splitmix64(pair << 32 | k)), draw j = splitmix64(s + j) mod n for j = 0, 1, ..., a duplicate redrawn with the next
-    j.  -> (idx int64 [K, 4], ok [K]); ok is False where MAX_DRAWS draws did not give 4 distinct indices."""
+def draw_samples(seed: int, pair: int, n_hypotheses: int, n: int, size: int = 4):
+    """The `size` correspondence indices of hypotheses 0..n_hypotheses-1 of `pair` among n (4 for a homography, 5 for
+    an essential matrix): s = splitmix64(seed + splitmix64(pair << 32 | k)), draw j = splitmix64(s + j) mod n for
+    j = 0, 1, ..., a duplicate redrawn with the next j.  -> (idx int64 [K, size], ok [K]); ok is False where MAX_DRAWS
+    draws did not give `size` distinct indices."""
     k = np.arange(n_hypotheses, dtype=_U64)
     s = splitmix64(_U64(int(seed) & 0xFFFFFFFFFFFFFFFF) + splitmix64((_U64(pair) << _U64(32)) | k))
-    idx = np.full((n_hypotheses, 4), -1, dtype=np.int64)
+    idx = np.full((n_hypotheses, size), -1, dtype=np.int64)
     got = np.zeros(n_hypotheses, dtype=np.int64)
     rows = np.arange(n_hypotheses)
     for j in range(MAX_DRAWS):
-        active = got < 4
+        active = got < size
         if not active.any():
             break
         v = (splitmix64(s + _U64(j)) % _U64(n)).astype(np.int64)
         take = active & ~(idx == v[:, None]).any(1)
         idx[rows[take], got[take]] = v[take]
         got += take
-    return idx, got == 4
+    return idx, got == size
 
 
 @dataclass
@@ -373,4 +397,537 @@ def homography_corner_error(H_est, H_gt, shapes) -> dict:
     out = {"error": err, "mean_error": float(err[fin].mean()) if fin.any() else float("inf")}
     for t in (1, 3, 5):
         out[f"accuracy_{t}"] = float(np.mean(err <= t)) if P else 0.0
+    return out
+
+
+# ------------------------------------------------------------------ relative pose: the model in numpy
+# DESIGN.md "Relative pose"; the kernels are csrc/essential.cuh.  Every step up to the winner is one IEEE fp64 operation
+# per numpy elementwise operation (no FMA, no reductions whose order numpy chooses), in the kernels' order.
+ESS_SAMPLE = 5
+ESS_MAX_ROOTS = 10
+ESS_RANK_EPS = 1e-10      # a sample whose QR column norm falls below this times the first one's is rejected
+ESS_ROOT_BOUND = 1e8      # real roots are searched in [-B, B], B = min(Cauchy bound, ESS_ROOT_BOUND)
+ESS_BISECT_STEPS = 100
+# One pair's staging in shared memory (ltr_essential's capacity): 32 bytes of normalised fp64 coordinates plus one
+# inlier flag byte per keypoint row.
+SMEM_PER_ROW_E = 33
+
+# Products of the monomials in (x, y, z): degree 1 [x, y, z, 1], degree 2 [x^2, xy, xz, x, y^2, yz, y, z^2, z, 1],
+# degree 3 in the elimination order [x^3, y^3, x^2y, xy^2, x^2z, x^2, y^2z, y^2, xyz, xy | xz^2, xz, x, yz^2, yz, y,
+# z^3, z^2, z, 1] (csrc/essential.cuh ESS_MUL11 / ESS_MUL21).
+_MUL11 = ((0, 1, 2, 3), (1, 4, 5, 6), (2, 5, 7, 8), (3, 6, 8, 9))
+_MUL21 = ((0, 2, 4, 5), (2, 3, 8, 9), (4, 8, 10, 11), (5, 9, 11, 12), (3, 1, 6, 7), (8, 6, 13, 14), (9, 7, 14, 15),
+          (10, 13, 16, 17), (11, 14, 17, 18), (12, 15, 18, 19))
+
+
+def _normalised(kpts, K):
+    """Pixel keypoints (used as float32) -> normalised fp64 coordinates (k - c) / f per axis."""
+    k = np.asarray(kpts, dtype=np.float32).astype(np.float64).reshape(-1, 2)
+    K = np.asarray(K, dtype=np.float64)
+    return np.stack([(k[:, 0] - K[0, 2]) / K[0, 0], (k[:, 1] - K[1, 2]) / K[1, 1]], 1)
+
+
+def _f_mean(K0, K1):
+    """The reference's mean focal length (models/utils.py:295: K0[0,0], K1[1,1] twice each), summed in order."""
+    return (((K0[0, 0] + K1[1, 1]) + K0[0, 0]) + K1[1, 1]) / 4.0
+
+
+def _mul(a, b, table, n_out):
+    """Product of polynomials in (x, y, z) given as coefficient arrays [K, len] in the monomial orders above."""
+    out = np.zeros((a.shape[0], n_out))
+    for i in range(a.shape[1]):
+        for j in range(b.shape[1]):
+            m = table[i][j]
+            out[:, m] = out[:, m] + a[:, i] * b[:, j]
+    return out
+
+
+def _pmul(a, b):
+    """Product of polynomials in z, ascending coefficients [K, la] x [K, lb] -> [K, la + lb - 1]."""
+    out = np.zeros((a.shape[0], a.shape[1] + b.shape[1] - 1))
+    for i in range(a.shape[1]):
+        for j in range(b.shape[1]):
+            out[:, i + j] = out[:, i + j] + a[:, i] * b[:, j]
+    return out
+
+
+def _null_basis(q):
+    """Null-space basis of the 5 epipolar rows of each sample: q [K, 5, 4] normalised (a0, b0, a1, b1) -> (basis
+    [K, 4, 9] = Q e5 .. Q e8 of the Householder QR of the 9 x 5 transpose, ok [K])."""
+    K = q.shape[0]
+    a0, b0, a1, b1 = (q[:, :, i] for i in range(4))
+    M = np.stack([a1 * a0, a1 * b0, a1, b1 * a0, b1 * b0, b1, a0, b0, np.ones_like(a0)], 1)   # [K, 9, 5]
+    ok = np.ones(K, dtype=bool)
+    vs, betas, nrm0 = [], [], None
+    for c in range(5):
+        acc = np.zeros(K)
+        for i in range(c, 9):
+            acc = acc + M[:, i, c] * M[:, i, c]
+        nrm = np.sqrt(acc)
+        if c == 0:
+            nrm0 = nrm
+            ok &= nrm > 0
+        else:
+            ok &= nrm > ESS_RANK_EPS * nrm0
+        alpha = np.where(M[:, c, c] >= 0, -nrm, nrm)
+        v = M[:, c:, c].copy()
+        v[:, 0] = M[:, c, c] - alpha
+        vtv = np.zeros(K)
+        for i in range(9 - c):
+            vtv = vtv + v[:, i] * v[:, i]
+        beta = np.where(vtv > 0, 2.0 / np.where(vtv > 0, vtv, 1.0), 0.0)
+        for j in range(c + 1, 5):
+            s = np.zeros(K)
+            for i in range(9 - c):
+                s = s + v[:, i] * M[:, c + i, j]
+            g = s * beta
+            for i in range(9 - c):
+                M[:, c + i, j] = M[:, c + i, j] - g * v[:, i]
+        vs.append(v)
+        betas.append(beta)
+    basis = np.zeros((K, 4, 9))
+    for b in range(4):
+        y = np.zeros((K, 9))
+        y[:, 5 + b] = 1.0
+        for c in range(4, -1, -1):
+            v = vs[c]
+            s = np.zeros(K)
+            for i in range(9 - c):
+                s = s + v[:, i] * y[:, c + i]
+            g = s * betas[c]
+            for i in range(9 - c):
+                y[:, c + i] = y[:, c + i] - g * v[:, i]
+        basis[:, b] = y
+    return basis, ok
+
+
+def _constraints(basis):
+    """The 10 x 20 cubic constraints (det E = 0, then 2 E E^T E - tr(E E^T) E = 0 row-major) of E = x X + y Y + z Z + W
+    in the degree-3 monomial order: [K, 10, 20]."""
+    e = [basis[:, :, i] for i in range(9)]          # entry i of E as a polynomial [x, y, z, 1]: [K, 4]
+    m11 = lambda a, b: _mul(a, b, _MUL11, 10)
+    m21 = lambda a, b: _mul(a, b, _MUL21, 20)
+    det = (m21(m11(e[4], e[8]) - m11(e[5], e[7]), e[0]) - m21(m11(e[3], e[8]) - m11(e[5], e[6]), e[1])) \
+        + m21(m11(e[3], e[7]) - m11(e[4], e[6]), e[2])
+    eet = {}
+    for i in range(3):
+        for k in range(i, 3):
+            eet[i, k] = eet[k, i] = (m11(e[3 * i], e[3 * k]) + m11(e[3 * i + 1], e[3 * k + 1])) \
+                + m11(e[3 * i + 2], e[3 * k + 2])
+    tr = (eet[0, 0] + eet[1, 1]) + eet[2, 2]
+    L = {(i, k): eet[i, k] * 2.0 - tr if i == k else eet[i, k] * 2.0 for i in range(3) for k in range(3)}
+    rows = [det]
+    for i in range(3):
+        for j in range(3):
+            rows.append((m21(L[i, 0], e[j]) + m21(L[i, 1], e[3 + j])) + m21(L[i, 2], e[6 + j]))
+    return np.stack(rows, 1)
+
+
+def _gauss_jordan(C):
+    """Gauss-Jordan elimination of the first 10 columns with partial pivoting (first largest |pivot|): -> (the last 10
+    columns of the reduced rows [K, 10, 10], ok [K]: every pivot > 0)."""
+    C = C.copy()
+    K = C.shape[0]
+    ok = np.ones(K, dtype=bool)
+    ar = np.arange(K)
+    for c in range(10):
+        piv = np.full(K, c)
+        best = np.abs(C[:, c, c])
+        for r in range(c + 1, 10):
+            v = np.abs(C[:, r, c])
+            upd = v > best
+            best, piv = np.where(upd, v, best), np.where(upd, r, piv)
+        ok &= best > 0
+        rc, rp = C[ar, c].copy(), C[ar, piv].copy()
+        C[ar, c], C[ar, piv] = rp, rc
+        p = C[:, c, c].copy()
+        C[:, c, c + 1:] = C[:, c, c + 1:] / p[:, None]
+        for r in range(10):
+            if r != c:
+                f = C[:, r, c].copy()
+                C[:, r, c + 1:] = C[:, r, c + 1:] - f[:, None] * C[:, c, c + 1:]
+    return C[:, :, 10:], ok
+
+
+def _hidden_matrix(R):
+    """The 3 x 3 matrix of polynomials in z (ascending coefficients) whose null vector is (x, y, 1): rows from
+    x^2z - z x^2, y^2z - z y^2, xyz - z xy.  -> [[bx, by, b1] per row] with bx, by [K, 4] and b1 [K, 5]."""
+    B = []
+    for u, l in ((4, 5), (6, 7), (8, 9)):
+        ru, rl = R[:, u], R[:, l]
+        bx = np.stack([-ru[:, 2], rl[:, 2] - ru[:, 1], rl[:, 1] - ru[:, 0], rl[:, 0]], 1)
+        by = np.stack([-ru[:, 5], rl[:, 5] - ru[:, 4], rl[:, 4] - ru[:, 3], rl[:, 3]], 1)
+        b1 = np.stack([-ru[:, 9], rl[:, 9] - ru[:, 8], rl[:, 8] - ru[:, 7], rl[:, 7] - ru[:, 6], rl[:, 6]], 1)
+        B.append([bx, by, b1])
+    return B
+
+
+def _det_poly(B):
+    """det B(z), degree 10, ascending coefficients [K, 11]."""
+    t0 = _pmul(B[0][0], _pmul(B[1][1], B[2][2]) - _pmul(B[1][2], B[2][1]))
+    t1 = _pmul(B[0][1], _pmul(B[1][0], B[2][2]) - _pmul(B[1][2], B[2][0]))
+    t2 = _pmul(B[0][2], _pmul(B[1][0], B[2][1]) - _pmul(B[1][1], B[2][0]))
+    return (t0 - t1) + t2
+
+
+def _maxabs(p):
+    m = np.zeros(p.shape[0])
+    for i in range(p.shape[1]):
+        a = np.abs(p[:, i])
+        m = np.where(a > m, a, m)
+    return m
+
+
+def _horner(c, x):
+    """Polynomial with ascending coefficients c [K, n] at x [K, ...] (one multiply, then one add, per step)."""
+    sh = (-1,) + (1,) * (x.ndim - 1)
+    v = np.broadcast_to(c[:, -1].reshape(sh), x.shape).copy()
+    for i in range(c.shape[1] - 2, -1, -1):
+        v = v * x + c[:, i].reshape(sh)
+    return v
+
+
+def _sign_changes(chain, length, x):
+    """Sign changes of the Sturm chain at x [K, m] (zeros and NaNs skipped), over its first length[K] members."""
+    K = x.shape[0]
+    prev = np.zeros(x.shape, dtype=np.int8)
+    n = np.zeros(x.shape, dtype=np.int64)
+    for k, c in enumerate(chain):
+        v = _horner(c, x)
+        s = (v > 0).astype(np.int8) - (v < 0).astype(np.int8)
+        live = (s != 0) & (k < length.reshape(K, *([1] * (x.ndim - 1))))
+        n += live & (prev != 0) & (s != prev)
+        prev = np.where(live, s, prev)
+    return n
+
+
+def sturm_roots(p):
+    """The real roots of polynomials of degree 10 (ascending coefficients p [K, 11]) in [-B, B], B = min(Cauchy bound,
+    ESS_ROOT_BOUND), with the kernels' fixed operation sequence: the Sturm chain of p (each member divided by its
+    largest |coefficient|), then per root index i < (number of real roots) ESS_BISECT_STEPS bisection steps on
+    "roots below mid > i".  -> (roots [K, 10] ascending, NaN past the count, count [K])."""
+    p = np.asarray(p, dtype=np.float64)
+    K = p.shape[0]
+    with np.errstate(all="ignore"):
+        m = _maxabs(p)
+        ok = (m > 0) & (m < np.inf) & (p[:, 10] != 0)
+        s0 = p / np.where(ok, m, 1.0)[:, None]
+        bound = np.ones(K)
+        for i in range(10):
+            a = np.abs(s0[:, i] / s0[:, 10])
+            bound = np.where(a + 1.0 > bound, a + 1.0, bound)
+        bound = np.where(bound < ESS_ROOT_BOUND, bound, ESS_ROOT_BOUND)
+        ok &= bound == bound
+        d = np.stack([s0[:, i + 1] * float(i + 1) for i in range(10)], 1)
+        md = _maxabs(d)
+        length = np.where(ok, np.where(md > 0, 2, 1), 0)
+        chain = [s0, d / np.where(md > 0, md, 1.0)[:, None]]
+        for k in range(1, 10):
+            A, Bp = chain[k - 1], chain[k]
+            mdeg = 11 - k
+            lead = Bp[:, mdeg - 1]
+            go = (length == k + 1) & (lead != 0)
+            q1 = A[:, mdeg] / lead
+            T = A[:, :mdeg].copy()
+            for i in range(1, mdeg):
+                T[:, i] = A[:, i] - q1 * Bp[:, i - 1]
+            q0 = T[:, mdeg - 1] / lead
+            r = np.stack([-(T[:, i] - q0 * Bp[:, i]) for i in range(mdeg - 1)], 1)
+            mr = _maxabs(r)
+            go &= mr > 0
+            chain.append(r / np.where(go, mr, 1.0)[:, None])
+            length = np.where(go, k + 2, length)
+        lo0 = -bound
+        v_lo = _sign_changes(chain, length, lo0[:, None])[:, 0]
+        v_hi = _sign_changes(chain, length, bound[:, None])[:, 0]
+        count = np.clip(v_lo - v_hi, 0, 10)
+        count = np.where(ok, count, 0)
+        idx = np.arange(10)[None, :]
+        lo = np.broadcast_to(lo0[:, None], (K, 10)).copy()
+        hi = np.broadcast_to(bound[:, None], (K, 10)).copy()
+        live = idx < count[:, None]
+        for _ in range(ESS_BISECT_STEPS):
+            mid = (lo + hi) * 0.5
+            act = live & (mid > lo) & (mid < hi)
+            if not act.any():
+                break
+            below = v_lo[:, None] - _sign_changes(chain, length, mid)
+            up = below > idx
+            hi = np.where(act & up, mid, hi)
+            lo = np.where(act & ~up, mid, lo)
+        roots = np.where(live, (lo + hi) * 0.5, np.nan)
+    return roots, count
+
+
+def _back_substitute(B, basis, z):
+    """E of every root z [K, 10]: (x, y, 1) from the cross product of two rows of B(z) (the pair whose third component
+    is largest in magnitude, first on a tie), E = ((x X + y Y) + z Z) + W.  -> (E [K, 10, 9], ok [K, 10])."""
+    rows = [[_horner(B[r][c], z) for c in range(3)] for r in range(3)]
+
+    def cross(a, b):
+        return (a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0])
+
+    best = cross(rows[0], rows[1])
+    for a, b in ((0, 2), (1, 2)):
+        c = cross(rows[a], rows[b])
+        upd = np.abs(c[2]) > np.abs(best[2])
+        best = tuple(np.where(upd, c[i], best[i]) for i in range(3))
+    ok = np.abs(best[2]) > 0
+    x, y = best[0] / best[2], best[1] / best[2]
+    X, Y, Z, W = (basis[:, b, None, :] for b in range(4))
+    E = ((x[..., None] * X + y[..., None] * Y) + z[..., None] * Z) + W
+    return E, ok & np.isfinite(E).all(-1)
+
+
+def essential_solutions(q):
+    """The five-point solver (DESIGN.md "Relative pose") on samples q [K, 5, 4] of normalised correspondences
+    (a0, b0, a1, b1): -> (E [K, 10, 9] row-major, ok [K, 10]); solution j of sample k is real root j of det B(z)."""
+    q = np.asarray(q, dtype=np.float64)
+    with np.errstate(all="ignore"):
+        basis, ok = _null_basis(q)
+        R, okg = _gauss_jordan(_constraints(basis))
+        B = _hidden_matrix(R)
+        roots, count = sturm_roots(_det_poly(B))
+        E, oke = _back_substitute(B, basis, np.where(np.isnan(roots), 0.0, roots))
+    return E, oke & (ok & okg)[:, None] & ~np.isnan(roots)
+
+
+def sampson_inliers(E, q, t2, chunk=512):
+    """Inlier flags [M, n] of essential matrices E [M, 9] on normalised correspondences q [n, 4]: (x1^T E x0)^2 <
+    t2 * ((E x0)_0^2 + (E x0)_1^2 + (E^T x1)_0^2 + (E^T x1)_1^2), i.e. Sampson error < t2 without the division."""
+    a0, b0, a1, b1 = (q[None, :, i] for i in range(4))
+    out = np.empty((E.shape[0], q.shape[0]), dtype=bool)
+    with np.errstate(all="ignore"):
+        for s in range(0, E.shape[0], chunk):
+            e = [E[s:s + chunk, i:i + 1] for i in range(9)]
+            u0 = (e[0] * a0 + e[1] * b0) + e[2]
+            u1 = (e[3] * a0 + e[4] * b0) + e[5]
+            u2 = (e[6] * a0 + e[7] * b0) + e[8]
+            w0 = (e[0] * a1 + e[3] * b1) + e[6]
+            w1 = (e[1] * a1 + e[4] * b1) + e[7]
+            num = (a1 * u0 + b1 * u1) + u2
+            den = ((u0 * u0 + u1 * u1) + w0 * w0) + w1 * w1
+            out[s:s + chunk] = num * num < t2 * den
+    return out
+
+
+def sampson_error(E, q):
+    """Sampson error [n] of one essential matrix E [9] on normalised correspondences q [n, 4] (fp64)."""
+    E = np.asarray(E, dtype=np.float64).reshape(3, 3)
+    x0 = np.concatenate([q[:, :2], np.ones((len(q), 1))], 1)
+    x1 = np.concatenate([q[:, 2:], np.ones((len(q), 1))], 1)
+    Ex0, Etx1 = x0 @ E.T, x1 @ E
+    num = np.sum(x1 * Ex0, 1)
+    return num * num / (Ex0[:, 0] ** 2 + Ex0[:, 1] ** 2 + Etx1[:, 0] ** 2 + Etx1[:, 1] ** 2)
+
+
+def decompose_essential(E):
+    """The four (R, t) candidates of E [3, 3] in OpenCV's order (R1, t), (R2, t), (R1, -t), (R2, -t)."""
+    U, _, Vt = np.linalg.svd(np.asarray(E, dtype=np.float64).reshape(3, 3))
+    if np.linalg.det(U) < 0:
+        U = -U
+    if np.linalg.det(Vt) < 0:
+        Vt = -Vt
+    W = np.array([[0.0, 1.0, 0.0], [-1.0, 0.0, 0.0], [0.0, 0.0, 1.0]])
+    R1, R2, t = U @ W @ Vt, U @ W.T @ Vt, U[:, 2]
+    return [(R1, t), (R2, t), (R1, -t), (R2, -t)]
+
+
+def cheirality(R, t, q, dist_thresh=1e9):
+    """Rows of q [n, 4] in front of both cameras: depths (d0, d1) of d1 x1 = d0 R x0 + t from the 2 x 2 normal
+    equations, 0 < d0 < dist_thresh and 0 < d1 < dist_thresh."""
+    x0 = np.concatenate([q[:, :2], np.ones((len(q), 1))], 1)
+    x1 = np.concatenate([q[:, 2:], np.ones((len(q), 1))], 1)
+    a, b = x0 @ np.asarray(R).T, x1
+    aa, ab, bb = (a * a).sum(1), (a * b).sum(1), (b * b).sum(1)
+    at, bt = a @ t, b @ t
+    with np.errstate(all="ignore"):
+        det = ab * ab - aa * bb
+        d0, d1 = (at * bb - ab * bt) / det, (ab * at - aa * bt) / det
+    return (d0 > 0) & (d0 < dist_thresh) & (d1 > 0) & (d1 < dist_thresh)
+
+
+def unit_essential(E):
+    """E [9] scaled to unit Frobenius norm, the sign making its largest-magnitude entry (the first on a tie) positive."""
+    E = np.asarray(E, dtype=np.float64).reshape(9)
+    E = E / np.sqrt(np.sum(E * E))
+    return E if E[int(np.argmax(np.abs(E)))] > 0 else -E
+
+
+def ransac_essential_host(kpts0, kpts1, matches_p, K0, K1, pair=0, thresh=1.0, n_hypotheses=1024, seed=0,
+                          dist_thresh=1e9) -> dict:
+    """The relative-pose estimator's model for one pair in numpy (DESIGN.md "Relative pose").  kpts [N, 2] (used as
+    float32), matches_p [N0]: local side-1 index or -1 per side-0 row, K0 / K1 [3, 3] fp64; `pair` is the pair's index
+    in the batch (it seeds the samples).  Returns E [3, 3] (unit Frobenius norm), R [3, 3], t [3] (unit; all NaN when
+    invalid), valid, inliers_p uint8 [N0] aligned with the match rows, n_inliers, n_cheirality (inliers in front of
+    both cameras under the chosen (R, t)), hypothesis (10 k + j of the winning sample k and root j, or -1),
+    hypothesis_inliers and E_hypothesis (the winning solution before scaling)."""
+    k0 = np.asarray(kpts0, dtype=np.float32).reshape(-1, 2)
+    k1 = np.asarray(kpts1, dtype=np.float32).reshape(-1, 2)
+    mp = np.asarray(matches_p, dtype=np.int64).reshape(-1)
+    K0, K1 = np.asarray(K0, dtype=np.float64), np.asarray(K1, dtype=np.float64)
+    rp = np.flatnonzero((mp >= 0) & (mp < len(k1)))
+    out = dict(E=np.full((3, 3), np.nan), R=np.full((3, 3), np.nan), t=np.full(3, np.nan), valid=False,
+               inliers_p=np.zeros(len(mp), dtype=np.uint8), n_inliers=0, n_cheirality=0, hypothesis=-1,
+               hypothesis_inliers=0, E_hypothesis=np.full((3, 3), np.nan))
+    n = len(rp)
+    if n < ESS_SAMPLE:
+        return out
+    q = np.concatenate([_normalised(k0[rp], K0), _normalised(k1[mp[rp]], K1)], 1)
+    tn = float(thresh) / _f_mean(K0, K1)
+    t2 = tn * tn
+    idx, ok = draw_samples(seed, pair, n_hypotheses, n, ESS_SAMPLE)
+    E, oke = essential_solutions(q[np.maximum(idx, 0)])
+    oke &= ok[:, None]
+    flat = np.flatnonzero(oke.reshape(-1))
+    if not len(flat):
+        return out
+    cnt = sampson_inliers(E.reshape(-1, 9)[flat], q, t2).sum(1)
+    # the kernels' key: (count << 32) | ~(10 k + j); flat = 10 k + j
+    w = int(flat[np.lexsort((flat, -cnt))[0]])
+    Ew = E.reshape(-1, 9)[w]
+    fl = sampson_inliers(Ew[None], q, t2)[0]
+    Eu = unit_essential(Ew)
+    best, R, t = -1, None, None
+    for Rc, tc in decompose_essential(Eu):
+        c = int(cheirality(Rc, tc, q[fl], dist_thresh).sum())
+        if c > best:
+            best, R, t = c, Rc, tc
+    out["inliers_p"][rp] = fl
+    out.update(E=Eu.reshape(3, 3), R=R, t=t / np.linalg.norm(t), valid=True, n_inliers=int(fl.sum()),
+               n_cheirality=best, hypothesis=w, hypothesis_inliers=int(fl.sum()), E_hypothesis=Ew.reshape(3, 3).copy())
+    return out
+
+
+# ------------------------------------------------------------------ relative pose, batched on the GPU
+@dataclass
+class PoseResult:
+    """Result of `estimate_poses` (device tensors; nothing has been waited for).
+
+    E float64 [P, 3, 3] (x1^T E x0 = 0 in normalised coordinates, unit Frobenius norm), R float64 [P, 3, 3] and t
+    float64 [P, 3] (unit) with X1 = R X0 + t (all NaN where not valid), valid bool [P], inliers uint8 aligned with the
+    result's matches_p (0 for unmatched rows), n_inliers int32 [P], n_cheirality int32 [P] (inliers in front of both
+    cameras under (R, t)), hypothesis int32 [P] (10 k + j of the winning sample k and root j, -1 when not valid) and
+    hypothesis_inliers int32 [P]."""
+    E: torch.Tensor
+    R: torch.Tensor
+    t: torch.Tensor
+    valid: torch.Tensor
+    inliers: torch.Tensor
+    n_inliers: torch.Tensor
+    n_cheirality: torch.Tensor
+    hypothesis: torch.Tensor
+    hypothesis_inliers: torch.Tensor
+
+
+def _intrinsics(K, P, name):
+    K = np.asarray(K.cpu() if isinstance(K, torch.Tensor) else K, dtype=np.float64)
+    if K.shape not in ((3, 3), (P, 3, 3)):
+        raise N.LtrError(f"estimate_poses: {name} must be [3, 3] or [{P}, 3, 3], got {list(K.shape)}")
+    K = np.ascontiguousarray(np.broadcast_to(K, (P, 3, 3)))
+    if not np.isfinite(K).all() or not ((K[:, 0, 0] > 0) & (K[:, 1, 1] > 0)).all():
+        raise N.LtrError(f"estimate_poses: {name} must be finite with fx, fy > 0")
+    return K
+
+
+def estimate_poses(res, K0, K1, thresh=1.0, n_hypotheses=1024, seed=0, dist_thresh=1e9) -> PoseResult:
+    """Relative pose of every pair of an `ImagePairMatches` (`match_images`, `match_sets`) from its point matches
+    (res.keypoints0 / keypoints1 in pixels): five-point RANSAC essential matrices and the pose, in one `ltr_essential`
+    call (the batched form of the reference's estimate_pose, models/utils.py:291-315).  K0 / K1: intrinsics of side 0
+    / side 1, [3, 3] for every pair or [P, 3, 3]; thresh in pixels, scaled by the reference's mean focal length.  Host
+    arrays go up in one pinned copy; the call never waits for the device.  Raises LtrError for non-finite K or K with
+    fx / fy <= 0, and (LTR_E_UNSUPPORTED) when a pair has more match rows than one CTA can stage (SMEM_PER_ROW_E bytes
+    per row, SMEM_MAX in all)."""
+    P = res.n_pairs
+    dev = res.matches_p.device
+    op = np.asarray(res.offsets_p, dtype=np.int64)
+    if int(n_hypotheses) < 1:
+        raise N.LtrError("estimate_poses: n_hypotheses must be >= 1")
+    k0, k1 = _intrinsics(K0, P, "K0"), _intrinsics(K1, P, "K1")
+    pt_rows = lambda k: torch.as_tensor(k).to(device=dev, dtype=torch.float32).reshape(-1, 2)
+    p0, poff0, pn0 = _pool(res.keypoints0, P, pt_rows)
+    p1, poff1, pn1 = _pool(res.keypoints1, P, pt_rows)
+    if not np.array_equal(pn0, np.diff(op)):
+        raise N.LtrError("estimate_poses: side-0 keypoints and the match offsets disagree")
+    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
+    dv = _stage({"K0": k0, "K1": k1, "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1,
+                 "cu_p": np.ascontiguousarray(op, dtype=np.int32)}, dev)
+    f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
+    out = PoseResult(torch.empty((P, 3, 3), **f64), torch.empty((P, 3, 3), **f64), torch.empty((P, 3), **f64),
+                     torch.empty(P, dtype=torch.uint8, device=dev),
+                     torch.empty(res.matches_p.shape[0], dtype=torch.uint8, device=dev),
+                     torch.empty(P, **i32), torch.empty(P, **i32), torch.empty(P, **i32), torch.empty(P, **i32))
+    key = torch.empty(P, dtype=torch.int64, device=dev)
+    _ops.essential(P, pts0=cat_t(p0).contiguous(), pts1=cat_t(p1).contiguous(), pts_off0=dv["pts_off0"],
+                   pts_off1=dv["pts_off1"], n_pts1=dv["n_pts1"], matches_p=res.matches_p.contiguous(), cu_p=dv["cu_p"],
+                   max_rows_p=int(np.diff(op).max(initial=0)), K0=dv["K0"], K1=dv["K1"], E=out.E, R=out.R, t=out.t,
+                   valid=out.valid, inliers_p=out.inliers, n_inliers=out.n_inliers, n_cheirality=out.n_cheirality,
+                   hypothesis=out.hypothesis, hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh,
+                   dist_thresh=dist_thresh, n_hypotheses=n_hypotheses, seed=seed)
+    out.valid = out.valid.view(torch.bool)
+    return out
+
+
+# ------------------------------------------------------------------ pose metrics
+# The reference's evaluation metrics (models/utils.py:358-412), with its signatures and results.  pose_errors is the
+# batched form; compute_pose_error is its one-pair case.
+def _host64(a):
+    return np.asarray(a.cpu() if isinstance(a, torch.Tensor) else a, dtype=np.float64)
+
+
+def _pixels_to_rays(kpts, K):
+    """Pixel keypoints [n, 2] -> homogeneous normalised coordinates [n, 3] ((u - cx) / fx, (v - cy) / fy, 1)."""
+    K = _host64(K)
+    xy = (_host64(kpts).reshape(-1, 2) - np.array([K[0, 2], K[1, 2]])) / np.array([K[0, 0], K[1, 1]])
+    return np.concatenate([xy, np.ones((len(xy), 1))], 1)
+
+
+def compute_epipolar_error(kpts0, kpts1, T_0to1, K0, K1):
+    """Symmetric epipolar error [n] of matched keypoints under the true relative pose T_0to1 [4, 4] (X1 = R X0 + t):
+    with E = [t]x R and normalised rays x0, x1, the squared residual x1^T E x0 divided by the squared normal length of
+    each epipolar line, E x0 in image 1 and E^T x1 in image 0, summed over both images."""
+    T = _host64(T_0to1)
+    E = np.cross(T[:3, 3], T[:3, :3].T).T            # column j of [t]x R is t x R[:, j]
+    x0, x1 = _pixels_to_rays(kpts0, K0), _pixels_to_rays(kpts1, K1)
+    line1, line0 = x0 @ E.T, x1 @ E                   # epipolar lines in image 1 and image 0
+    r2 = np.einsum("ni,ni->n", x1, line1) ** 2
+    return r2 / (line1[:, 0] ** 2 + line1[:, 1] ** 2) + r2 / (line0[:, 0] ** 2 + line0[:, 1] ** 2)
+
+
+def pose_errors(R, t, T_0to1):
+    """Pose errors of P estimates in degrees: R [P, 3, 3] and t [P, 3] (tensors or arrays) against T_0to1 [P, 4, 4]
+    or [4, 4] -> (error_t [P], error_R [P]).  error_R is the angle of the rotation R_gt^T R; error_t is the angle
+    between t and t_gt folded to [0, 90] (E fixes t only up to sign).  A pair whose R or t is not finite (an invalid
+    estimate) gets inf in both, as the reference's evaluation scores a failed estimate_pose."""
+    R, t = _host64(R).reshape(-1, 3, 3), _host64(t).reshape(-1, 3)
+    T = np.broadcast_to(_host64(T_0to1).reshape(-1, 4, 4), (len(R), 4, 4))
+    ok = np.isfinite(R).all((1, 2)) & np.isfinite(t).all(1)
+    with np.errstate(all="ignore"):
+        cos_r = ((T[:, :3, :3] * R).sum((1, 2)) - 1.0) / 2.0        # trace(R_gt^T R) = sum of the elementwise product
+        err_R = np.degrees(np.arccos(np.clip(cos_r, -1.0, 1.0)))
+        t_gt = T[:, :3, 3]
+        cos_t = (t * t_gt).sum(1) / (np.linalg.norm(t, axis=1) * np.linalg.norm(t_gt, axis=1))
+        ang = np.degrees(np.arccos(np.clip(cos_t, -1.0, 1.0)))
+    err_t = np.minimum(ang, 180.0 - ang)
+    return np.where(ok, err_t, np.inf), np.where(ok, err_R, np.inf)
+
+
+def compute_pose_error(T_0to1, R, t):
+    """(translation error, rotation error) in degrees of one estimate: `pose_errors` for one pair."""
+    et, eR = pose_errors(np.asarray(R)[None], np.asarray(t).reshape(1, 3), T_0to1)
+    return et[0], eR[0]
+
+
+def pose_auc(errors, thresholds):
+    """Normalised area under the cumulative error curve, one value per threshold: the curve rises linearly from (0, 0)
+    through (e_i, i / n) for the sorted errors e_1 <= ... <= e_n and stays flat after the last error below the
+    threshold; its area up to the threshold is divided by the threshold."""
+    e = np.sort(_host64(errors).reshape(-1))
+    x = np.concatenate([[0.0], e])
+    y = np.arange(len(x)) / max(len(e), 1)
+    seg = np.diff(x) * (y[1:] + y[:-1]) / 2.0           # trapezoid between consecutive curve points
+    out = []
+    for thr in thresholds:
+        k = int(np.searchsorted(x, thr))                  # curve points strictly below thr (x[0] = 0 included)
+        out.append(float((seg[:k - 1].sum() + (thr - x[k - 1]) * y[k - 1]) / thr))
     return out

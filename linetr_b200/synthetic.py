@@ -395,3 +395,97 @@ def make_warp_images(seed: int, n: int, h: int, w: int):
         colour[i] = img
     gray = np.rint(colour.astype(np.float64) @ np.array([0.114, 0.587, 0.299])).astype(np.uint8)
     return gray, colour
+
+
+# ------------------------------------------------------------------ calibrated two-view inputs (relative pose)
+DEFAULT_K = np.array([[500.0, 0.0, 319.5], [0.0, 500.0, 239.5], [0.0, 0.0, 1.0]])
+
+
+def random_pose(rng, max_angle_deg: float = 15.0, translation=None) -> tuple:
+    """A random relative pose (R [3, 3], t [3] with |t| = 1; X1 = R X0 + t): a rotation about a random axis by up to
+    max_angle_deg, and a random unit translation unless `translation` is given (normalised)."""
+    ax = rng.normal(size=3)
+    ax /= np.linalg.norm(ax)
+    a = np.deg2rad(max_angle_deg) * rng.uniform(0.2, 1.0)
+    S = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
+    R = np.eye(3) + np.sin(a) * S + (1 - np.cos(a)) * S @ S
+    t = rng.normal(size=3) if translation is None else np.asarray(translation, dtype=np.float64)
+    return R, t / np.linalg.norm(t)
+
+
+def _project(K, X):
+    x = X @ np.asarray(K, dtype=np.float64).T
+    return x[:, :2] / x[:, 2:]
+
+
+def make_pose_correspondences(seed: int, n: int, R, t, K0=DEFAULT_K, K1=DEFAULT_K, noise_px: float = 0.5,
+                              outlier_frac: float = 0.5, w: int = 640, h: int = 480, min_outlier_px: float = 10.0):
+    """Point matches of a calibrated pair with relative pose (R, t) (X1 = R X0 + t): 3D points in front of both cameras
+    (depth 2 to 8 in camera 0, seen inside image 0, depth > 0.5 in camera 1), projected with K0 / K1, plus N(0,
+    noise_px) per coordinate on both sides.  An outlier's side-1 keypoint is moved min_outlier_px to 60 px across its
+    epipolar line (and up to 30 px along it), so no outlier is within min_outlier_px of the true model.  Row i of side
+    0 matches row i of side 1.  Returns dict kpts0, kpts1 [n, 2] float32, matches_p int32 and the true inlier mask
+    true_p."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    R, t = np.asarray(R, dtype=np.float64), np.asarray(t, dtype=np.float64)
+    X = np.zeros((0, 3))
+    while len(X) < n:
+        m = 2 * (n - len(X)) + 8
+        x = np.stack([rng.uniform(0, w - 1, m), rng.uniform(0, h - 1, m), np.ones(m)], 1)
+        Xc = (x @ np.linalg.inv(K0).T) * rng.uniform(2.0, 8.0, (m, 1))
+        X = np.concatenate([X, Xc[(Xc @ R.T + t)[:, 2] > 0.5]])
+    X = X[:n]
+    x0 = _project(K0, X) + rng.normal(0, noise_px, (n, 2))
+    x1 = _project(K1, X @ R.T + t)
+    out = rng.random(n) < outlier_frac
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    F = np.linalg.inv(K1).T @ tx @ R @ np.linalg.inv(K0)
+    l = np.concatenate([_project(K0, X), np.ones((n, 1))], 1) @ F.T
+    nrm = l[:, :2] / np.maximum(np.linalg.norm(l[:, :2], axis=1, keepdims=True), 1e-12)
+    tan = np.stack([-nrm[:, 1], nrm[:, 0]], 1)
+    shift = (rng.uniform(min_outlier_px, max(60.0, min_outlier_px + 1), n) * rng.choice([-1.0, 1.0], n))[:, None] * nrm \
+        + rng.uniform(-30, 30, (n, 1)) * tan
+    x1[out] += shift[out]
+    x1 += rng.normal(0, noise_px, (n, 2))
+    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+    return {"kpts0": f32(x0), "kpts1": f32(x1), "matches_p": np.arange(n, dtype=np.int32), "true_p": ~out}
+
+
+def make_pose_set(seed: int, n_views: int, n_lines: int, n_points: int, K=DEFAULT_K, w: int = 640, h: int = 480,
+                  max_angle_deg: float = 4.0, max_shift: float = 0.8, jitter_px: float = 0.3, map_noise: float = 0.02):
+    """n_views calibrated views (intrinsics K) of one 3D point cloud (image dicts as `make_image_set` returns): camera v
+    has pose T[v] (world -> camera, [4, 4]): a rotation of up to max_angle_deg and a centre within max_shift of the
+    origin, looking down +z at n_points points 4 to 8 units away, chosen so every view sees all of them.  Keypoints are
+    the projections plus N(0, jitter_px); point descriptors are per 3D point plus map_noise, as `make_image_set` makes
+    them; key lines and dense maps are `make_image_set`'s (line matches carry no two-view constraint for the pose).
+    Returns (views, T [V, 4, 4]); the pose of view i -> view j is T[j] @ inv(T[i])."""
+    import torch
+    rng = np.random.Generator(np.random.PCG64(seed))
+    K = np.asarray(K, dtype=np.float64)
+    Ts = []
+    for _ in range(n_views):
+        R, _ = random_pose(rng, max_angle_deg)
+        c = rng.uniform(-max_shift, max_shift, 3)
+        T = np.eye(4)
+        T[:3, :3], T[:3, 3] = R, -R @ c
+        Ts.append(T)
+    X = np.zeros((0, 3))
+    while len(X) < n_points:
+        m = 2 * n_points
+        x = np.stack([rng.uniform(0.15 * w, 0.85 * w, m), rng.uniform(0.15 * h, 0.85 * h, m), np.ones(m)], 1)
+        Xc = (x @ np.linalg.inv(K).T) * rng.uniform(4.0, 8.0, (m, 1))
+        keep = np.ones(m, dtype=bool)
+        for T in Ts:
+            q = Xc @ T[:3, :3].T + T[:3, 3]
+            p = _project(K, q)
+            keep &= (q[:, 2] > 1.0) & (p[:, 0] >= 0) & (p[:, 0] <= w - 1) & (p[:, 1] >= 0) & (p[:, 1] <= h - 1)
+        X = np.concatenate([X, Xc[keep]])
+    X = X[:n_points]
+    base = make_image_set(seed + 1, n_views, n_lines, n_points, w, h, jitter_px, map_noise)
+    desc = _unit(rng.standard_normal((n_points, D_MODEL)).astype(np.float32))
+    for v, T in zip(base, Ts):
+        k = _project(K, X @ T[:3, :3].T + T[:3, 3]) + rng.normal(0, jitter_px, (n_points, 2))
+        d = _unit(desc + map_noise * rng.standard_normal(desc.shape).astype(np.float32))
+        v["keypoints"] = torch.from_numpy(np.clip(k, 0, [w - 1, h - 1]).astype(np.float32))
+        v["descriptors"] = torch.from_numpy(np.ascontiguousarray(d.T))
+    return base, np.stack(Ts)
