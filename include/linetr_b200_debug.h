@@ -31,6 +31,14 @@ const unsigned long long* ltr_gemm_trace(void);
 void ltr_debug_trace_arm(int32_t on);
 int ltr_debug_trace_read(unsigned long long* out128);
 
+/* Where ltr_encode leaves each stage's activation in `workspace` (the pointer given to ltr_encode) for a batch of
+ * n_lines lines, so that tests can read every stage's real inputs and outputs after an encode.  Slot i of hi / lo /
+ * kblocks: 0 z, 1 ctx, 2 l128, 3 l256, 4 lpos, 5 y1i, 6 g, 7 xm, 8 hm, 9 qkv: split-bf16 activation images (hi and lo
+ * planes, kblocks 64-wide k-blocks per 128-row block); 10 yf: fp32 rows [n_lines, 256] in hi, lo = NULL, kblocks 0.
+ * Returns 0, or LTR_E_INVALID on a null argument. */
+int ltr_debug_encode_images(const struct LtrModel* model, int32_t n_lines, void* workspace, void* hi[11], void* lo[11],
+                            int32_t kblocks[11]);
+
 #ifdef __cplusplus
 }
 #endif

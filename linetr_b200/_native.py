@@ -28,7 +28,10 @@ EXPORTED_SYMBOLS = (
     "ltr_line_gt", "ltr_triplet_loss", "ltr_homography", "ltr_warp_pairs", "ltr_essential",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
-DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read")
+DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read",
+                 "ltr_debug_encode_images")
+# slots of ltr_debug_encode_images, in order
+ENCODE_IMAGES = ("z", "ctx", "l128", "l256", "lpos", "y1i", "g", "xm", "hm", "qkv", "yf")
 ABI_VERSION = 3
 
 
@@ -254,6 +257,9 @@ def load():
     lib.ltr_debug_trace_arm.restype = None
     lib.ltr_debug_trace_read.argtypes = [C.POINTER(C.c_uint64)]
     lib.ltr_debug_trace_read.restype = C.c_int
+    lib.ltr_debug_encode_images.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p),
+                                            C.POINTER(C.c_void_p), c_int32_p]
+    lib.ltr_debug_encode_images.restype = C.c_int
     lib.ltr_launch_count.restype = C.c_int64
     lib.ltr_reset_launch_count.restype = None
     lib.ltr_profile_begin.restype = None
@@ -269,6 +275,15 @@ def check(rc: int, what: str):
     if rc != 0:
         msg = load().ltr_last_error()
         raise LtrError(f"{what} failed (code {rc}): {msg.decode() if msg else ''}")
+
+
+def encode_images(model_ptr, n_lines: int, workspace_ptr: int) -> dict:
+    """ltr_debug_encode_images: {name: (hi address, lo address, kblocks)} of the activations ltr_encode leaves in a
+    workspace (names ENCODE_IMAGES; 'yf' is fp32 rows with lo = 0, kblocks = 0)."""
+    hi, lo, kb = (C.c_void_p * 11)(), (C.c_void_p * 11)(), (C.c_int32 * 11)()
+    check(load().ltr_debug_encode_images(model_ptr, int(n_lines), C.c_void_p(workspace_ptr), hi, lo, kb),
+          "ltr_debug_encode_images")
+    return {n: (hi[i] or 0, lo[i] or 0, int(kb[i])) for i, n in enumerate(ENCODE_IMAGES)}
 
 
 def launch_count() -> int:

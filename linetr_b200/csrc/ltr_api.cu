@@ -1391,6 +1391,24 @@ int ltr_debug_trace_read(unsigned long long* out128) {
   return cudaMemcpyFromSymbol(out128, g_dbg_trace, 128 * sizeof(unsigned long long)) == cudaSuccess ? 0 : -2;
 }
 
+int ltr_debug_encode_images(const LtrModel* m, int32_t n_lines, void* workspace, void* hi[11], void* lo[11],
+                            int32_t kblocks[11]) {
+  if (!m || n_lines < 0 || !workspace || !hi || !lo || !kblocks)
+    return set_error(LTR_E_INVALID, "ltr_debug_encode_images: bad argument");
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(workspace), 256));   // as ltr_encode
+  const EncodeWs w = carve(m, n_lines, 1, base);
+  const ActImg* img[10] = {&w.z, &w.ctx, &w.l128, &w.l256, &w.lpos, &w.y1i, &w.g, &w.xm, &w.hm, &w.qkv};
+  for (int i = 0; i < 10; ++i) {
+    hi[i] = img[i]->hi;
+    lo[i] = img[i]->lo;
+    kblocks[i] = img[i]->kblocks;
+  }
+  hi[10] = w.yf;
+  lo[10] = nullptr;
+  kblocks[10] = 0;
+  return LTR_OK;
+}
+
 static unsigned long long g_trace_host[64];
 const unsigned long long* ltr_gemm_trace(void) { return g_trace_host; }
 
