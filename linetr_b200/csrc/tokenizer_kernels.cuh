@@ -8,9 +8,14 @@
 // clipped end point, n_tokens = ceil(length / token_distance), first subline index, image index.
 // One launch pair covers many images (ltr_tokenize_batch); each image has its own maps, sizes and
 // token_distance, and its sublines land at its rows of the concatenated output.  Token
-// positions are computed in float64 exactly as the reference's numpy code does (IEEE sqrt/div),
-// then rounded to fp32, so positions, sublines, masks and responses are bit-identical; sampled
-// descriptors agree to fp32 rounding.
+// positions, subline cut points and responses are computed in float64 in the CPU glue's numpy order,
+// one explicitly rounded operation per numpy operation (__dmul_rn / __dadd_rn / __ddiv_rn / __dsqrt_rn, so
+// nvcc cannot contract a product and a sum into one fma; squares are products, as in the glue, where the
+// reference's scalar m ** 2 goes through libm pow), then rounded once to fp32: they, the masks and the
+// score lookups are bit-identical to the CPU glue.  That order is part of the contract.  Sampled
+// descriptors agree to fp32 rounding (bound: tests/tokenizer_model.py).  Key lines must have finite,
+// non-negative coordinates and run left to right (start x <= end x, as change_cv2_T_np orders them), so no
+// token rounds to a negative score row or column; the host refuses other lines (keyline_geometry).
 #pragma once
 #include "common.cuh"
 
@@ -50,26 +55,28 @@ __device__ __forceinline__ const TokImage& image_of_line(const TokLines& L, cons
   return I.im[L.line_image ? L.line_image[k] - I.first : 0];
 }
 
-// point at distance d from sp along the line (reference point_on_line, line_process.py:43-59)
+// point at distance d from sp along the line (reference point_on_line, line_process.py:43-59), every operation
+// rounded as numpy rounds it: m = vy / vx, dx = sqrt(d**2 / (1 + m**2)), dy = m * dx, then + sp.  Explicit
+// intrinsics keep nvcc from contracting 1 + m * m into one fma, which rounds once less than numpy.
 __device__ __forceinline__ void point_on_line_f64(double spx, double spy, double epx, double epy, double d, double& x, double& y) {
-  const double vx = epx - spx, vy = epy - spy;
+  const double vx = __dsub_rn(epx, spx), vy = __dsub_rn(epy, spy);
   double dx, dy;
   if (vx != 0.0) {
-    const double m = vy / vx;
-    dx = sqrt(d * d / (1.0 + m * m));
-    dy = m * dx;
+    const double m = __ddiv_rn(vy, vx);
+    dx = __dsqrt_rn(__ddiv_rn(__dmul_rn(d, d), __dadd_rn(1.0, __dmul_rn(m, m))));
+    dy = __dmul_rn(m, dx);
   } else {
     dx = 0.0;
     dy = (vy > 0.0) ? d : -d;
   }
-  x = dx + spx;
-  y = dy + spy;
+  x = __dadd_rn(dx, spx);
+  y = __dadd_rn(dy, spy);
 }
 
 // token i of key line k (i < n_tok): i < n_tok-1 -> point at i*token_distance, last -> clipped end point
 __device__ __forceinline__ void token_of_line(const TokLines& L, double token_distance, int k, int i, double& x, double& y) {
   if (i < L.n_tok[k] - 1) {
-    point_on_line_f64(L.sp[2 * k], L.sp[2 * k + 1], L.ep[2 * k], L.ep[2 * k + 1], (double)i * token_distance, x, y);
+    point_on_line_f64(L.sp[2 * k], L.sp[2 * k + 1], L.ep[2 * k], L.ep[2 * k + 1], __dmul_rn((double)i, token_distance), x, y);
   } else {
     x = L.epc[2 * k];
     y = L.epc[2 * k + 1];
@@ -103,8 +110,10 @@ tok_points_kernel(TokLines L, const __grid_constant__ TokImages<NI> I, int s_beg
     if (sl == n_sub - 1) { bx = L.epc[2 * k]; by = L.epc[2 * k + 1]; } else token_of_line(L, td, k, (sl + 1) * L.T - 1, bx, by);
     sublines[4 * s + 0] = (float)ax; sublines[4 * s + 1] = (float)ay;
     sublines[4 * s + 2] = (float)bx; sublines[4 * s + 3] = (float)by;
-    const double dxx = bx - ax, dyy = by - ay;
-    resp[s] = (float)(sqrt(dxx * dxx + dyy * dyy) / (td * (double)L.T));
+    // numpy: sqrt(((b - a) ** 2).sum()) / (token_distance * max_tokens), both squares rounded before the sum
+    const double dxx = __dsub_rn(bx, ax), dyy = __dsub_rn(by, ay);
+    resp[s] = (float)__ddiv_rn(__dsqrt_rn(__dadd_rn(__dmul_rn(dxx, dxx), __dmul_rn(dyy, dyy))),
+                               __dmul_rn(td, (double)L.T));
     angle[2 * s] = L.angle[2 * k];
     angle[2 * s + 1] = L.angle[2 * k + 1];
   }

@@ -9,6 +9,13 @@ quirks (in-place end-point clipping, `index[:max_keylines]` dropping the shortes
 max_keylines == -1, the torch-version dependent `align_corners`) - and is the pin the GPU
 tokeniser is tested against.  The cheap per-image filters (`remove_borders`,
 `filter_by_length`, cv2 KeyLine conversion) stay vectorised numpy.
+
+One deliberate difference: the reference squares the slope and the token distance as scalars
+(`m ** 2`, `dist_px ** 2`), which numpy and Python evaluate with libm's pow.  pow is not correctly
+rounded (glibc's differs from m * m for about 1 in 1200 random slopes), so its result depends on the
+platform.  The glue squares with one correctly rounded product (m * m, d * d), which the GPU
+reproduces exactly; a token differs from the reference only where pow's last bit differs and that
+bit moves the fp32 rounding of the position.
 """
 from __future__ import annotations
 
@@ -44,9 +51,22 @@ def keyline_geometry(kl, length, token_distance, max_tokens, width, height):
     has its end points clipped IN PLACE to (width-0.6, height-0.6), as the reference does; token_distance,
     width and height are scalars or per-key-line arrays.  -> dict of n_tok, n_sub [K] int64, sub0 [K+1]
     (first subline of every key line, the key-line CSR), sub2line [S], and the float64 start point sp,
-    end point ep (before the clip) and epc (after it), each [K,2]."""
+    end point ep (before the clip) and epc (after it), each [K,2].
+
+    Key lines must have finite, non-negative coordinates (`remove_borders` keeps only such lines) and run left
+    to right (start x <= end x), as `change_cv2_T_np` orders them: tokens step from the start in +x, so on a
+    reversed line they would move away from it, and a token left of or above the image would look up a score
+    before the start of the map (the reference wraps the negative index).  Any other line raises LtrError."""
+    from . import _native as N
     T = int(max_tokens)
     K = len(kl)
+    ends = lambda i: f"(start {tuple(kl[i, 0].tolist())}, end {tuple(kl[i, 1].tolist())})"
+    for bad, why in ((~np.isfinite(kl).all(axis=(1, 2)), "has a non-finite coordinate"),
+                     ((kl < 0).any(axis=(1, 2)), "has a negative coordinate: key lines must lie in the image"),
+                     (kl[:, 0, 0] > kl[:, 1, 0], "runs right to left: key lines must have start x <= end x")):
+        if bad.any():
+            i = int(np.flatnonzero(bad)[0])
+            raise N.LtrError(f"key line {i} {why} {ends(i)}")
     length = np.asarray(length, dtype=np.float64)
     n_tok = np.ceil(length / token_distance).astype(np.int64)
     n_sub = -(-n_tok // T)
@@ -228,7 +248,7 @@ def _tokens_on_line(kline, n_tokens, token_distance, width, height):
     vec = ep - sp
     if vec[0] != 0:
         m = vec[1] / vec[0]
-        dx = np.sqrt(dists ** 2 / (1 + m ** 2))
+        dx = np.sqrt(dists * dists / (1 + m * m))   # correctly rounded squares, not pow (module docstring)
         dy = m * dx
     else:
         dx = np.zeros_like(dists)
@@ -319,8 +339,9 @@ def line_tokenizer(klines, token_distance, max_tokens, pred_superpoint, image_sh
 
 def line_tokenizer_gpu(klines, token_distance, max_tokens, pred_superpoint, image_shape):
     """`line_tokenizer` on the GPU (ltr_tokenize): same inputs, same output dict, no Python loops.
-    Token positions, sublines, masks, responses and the adjacency are bit-identical to the CPU
-    version (float64 arithmetic, rounded once to fp32); sampled descriptors agree to fp32 rounding."""
+    Token positions, sublines, masks, responses, scores and the adjacency are bit-identical to the CPU
+    version (float64 arithmetic in numpy's operation order, rounded once to fp32); sampled descriptors
+    agree to fp32 rounding.  Key lines must lie in the image and run left to right (see `keyline_geometry`)."""
     import ctypes as C
     from . import _native as N
     dense = pred_superpoint["dense_descriptor"]
