@@ -32,6 +32,8 @@
  *                                 cv2.recoverPose per pair, batched.
  *   ltr_warp_pairs             <- cv2.warpPerspective of the grey and colour images + the eroded valid mask of the
  *                                 homography dataset builder (dataloaders/build_homography_dataset.py:164-184).
+ *   ltr_photometric            <- imgPhotometric of the homography dataset builder (ImgAugTransform +
+ *                                 customizedTransform.additive_shade, dataloaders/utils/photometric.py).
  *
  * Conventions: return 0 on success, a negative LTR_E_* code on failure (message via
  * ltr_last_error(), thread-local).  All device pointers are caller-owned and must live on
@@ -620,6 +622,45 @@ int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, in
 int ltr_warp_pairs(const uint8_t* gray, const uint8_t* colour, int32_t n_images, int32_t height, int32_t width,
                    int32_t channels, const int32_t* src_index_host, const int32_t* src_index, const double* inv_maps,
                    int32_t n_pairs, uint8_t* warped, uint8_t* mask, int32_t device, void* stream);
+
+/* Photometric augmentation <- imgPhotometric of the homography dataset builder
+ * (dataloaders/build_homography_dataset.py:105-121, dataloaders/utils/photometric.py) for the yaml's primitives, on
+ * n_images uint8 images [n_images, height, width] (device).  `out` may equal `in` (in place).
+ *
+ * Per image, params[i * LTR_PHOTOMETRIC_PARAMS + slot] (fp64; params_host is the same array in host memory, checked
+ * before any launch):
+ *    0- 2  brightness: application count (0-2), integer delta of application 0, of application 1
+ *    3- 5  contrast: count, float32 alpha 0, alpha 1        6- 8  Gaussian noise: count, stddev 0, stddev 1
+ *    9-11  impulse noise: count, p 0, p 1                   12    motion blur on (1) / off (0)
+ *   13-21  the 3 x 3 float32 motion-blur kernel, row-major  22    shade on / off
+ *   23     transparency (used as float32)   24  odd Gaussian kernel size <= 149   25, 26  noise key low / high 32 bits
+ *   27     number of shade ellipses (<= max_ellipses)
+ * ellipses [n_images, max_ellipses, 5] int32 (device): ax, ay, x, y, integer angle in degrees, each inside the image as
+ * sample_photometric draws them (max(ax, ay) <= x < width - max(ax, ay), likewise y); others are not drawn.
+ * taps [n_images, 149] float32 (device): the first ksize are the image's Gaussian taps.
+ *
+ * The arithmetic (DESIGN.md "Photometric augmentation"; linetr_b200/photometric.py is its numpy model):
+ *   brightness a = clip(a + d); contrast a = trunc(clip(fl32(127.5 + fl32(alpha * fl32(a - 127.5)))));
+ *   Gaussian noise a = clip(a + clip(rint(s * z), -255, 255)); impulse noise a = rint(255 sin^2(pi u / 2)) where
+ *   u' < p; z, u, u' from Philox4x64-10 with key (key, 0) and counter (y * width + x, application, 0, 0);
+ *   motion blur: fp32 FMAs over the kernel in row-major order from 0, BORDER_REFLECT_101, rint and saturate;
+ *   shade: cv2.ellipse's filled ellipses into a 0/255 mask, the separable fp32 Gaussian (rows, then columns, each
+ *   acc = fl32(acc + fl32(tap_k * v_k)), BORDER_REFLECT_101 reflected as often as needed), then
+ *   out = trunc(double(fl32(clip(fl32(x * fl32(1 - fl32(fl32(t * m) / 255))), 0, 255) / 255)) * 255) with
+ *   x = fl32(fl32(a / 255) * 255).  Without the shade, out is the stage-1 byte.
+ *
+ * workspace: device, at least LTR_PHOTOMETRIC_WORKSPACE_BYTES(n_images, height, width) bytes, 256-byte aligned.
+ * Errors before any launch: LTR_E_INVALID for a negative count, a null pointer, n_params != LTR_PHOTOMETRIC_PARAMS or
+ * a parameter outside the ranges above; LTR_E_UNSUPPORTED for a side outside [1, 32767] or more than 65535 images;
+ * LTR_E_WORKSPACE for a short workspace.  n_images == 0 writes nothing.  Writes out and the workspace; asynchronous on
+ * `stream`, never synchronises. */
+#define LTR_PHOTOMETRIC_PARAMS 28
+#define LTR_PHOTOMETRIC_MAX_KSIZE 149
+#define LTR_PHOTOMETRIC_WORKSPACE_BYTES(n, h, w) ((int64_t)(n) * (h) * (w) * 6 + 512)
+int ltr_photometric(const uint8_t* in, uint8_t* out, int32_t n_images, int32_t height, int32_t width,
+                    const double* params_host, const double* params, int32_t n_params, const int32_t* ellipses,
+                    int32_t max_ellipses, const float* taps, void* workspace, int64_t workspace_bytes, int32_t device,
+                    void* stream);
 
 /* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
  * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */

@@ -16,6 +16,9 @@ the reference's pose metrics:
     estimate_poses, compute_epipolar_error, compute_pose_error, pose_auc, pose_errors
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
+Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
+batched on the GPU, and pairs built from augmented images:
+    sample_photometric, photometric_augment, photometric_homography_pairs
 `install_as_reference_models()` registers this package's modules under the reference's
 module names (`models.line_transformer`, `models.nn_matcher`, `models.line_process`) so that
 the reference's own `models/matching.py` / `match_line_pairs.py` run unchanged on top of it.
@@ -54,6 +57,9 @@ _LAZY = {
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),
     "apply_valid_masks": ("homography_pairs", "apply_valid_masks"),
+    "sample_photometric": ("photometric", "sample_photometric"),
+    "photometric_augment": ("photometric", "photometric_augment"),
+    "photometric_homography_pairs": ("photometric", "photometric_homography_pairs"),
 }
 
 

@@ -26,6 +26,7 @@ EXPORTED_SYMBOLS = (
     "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
     "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
     "ltr_line_gt", "ltr_triplet_loss", "ltr_homography", "ltr_warp_pairs", "ltr_essential",
+    "ltr_photometric",
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read",
@@ -33,6 +34,13 @@ DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "lt
 # slots of ltr_debug_encode_images, in order
 ENCODE_IMAGES = ("z", "ctx", "l128", "l256", "lpos", "y1i", "g", "xm", "hm", "qkv", "yf")
 ABI_VERSION = 3
+PHOTOMETRIC_PARAMS = 28      # LTR_PHOTOMETRIC_PARAMS
+PHOTOMETRIC_MAX_KSIZE = 149  # LTR_PHOTOMETRIC_MAX_KSIZE
+
+
+def photometric_workspace_bytes(n, h, w) -> int:
+    """LTR_PHOTOMETRIC_WORKSPACE_BYTES(n, h, w)."""
+    return int(n) * int(h) * int(w) * 6 + 512
 
 
 class LtrError(RuntimeError):
@@ -223,6 +231,11 @@ def load():
                                                                              C.c_int32, C.c_void_p, C.c_void_p,
                                                                              C.c_int32, C.c_void_p]
     lib.ltr_warp_pairs.restype = C.c_int
+    lib.ltr_photometric.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, C.c_int32,
+                                                                                C.c_void_p, C.c_int32, C.c_void_p,
+                                                                                C.c_void_p, C.c_int64, C.c_int32,
+                                                                                C.c_void_p]
+    lib.ltr_photometric.restype = C.c_int
     lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.ltr_gather_wait.restype = C.c_int
     lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,

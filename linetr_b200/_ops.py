@@ -447,6 +447,33 @@ def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, wa
     N.check(rc, "ltr_warp_pairs")
 
 
+def photometric(src, dst, params_host: np.ndarray, params, ellipses, taps, workspace):
+    """ltr_photometric into a caller-allocated output: src / dst uint8 [N,h,w] (dst may be src), params fp64
+    [N, PHOTOMETRIC_PARAMS] (host copy and device copy), ellipses int32 [N,E,5], taps float32 [N,149], workspace uint8
+    of at least photometric_workspace_bytes(N, h, w)."""
+    dev = src.device
+    if src.dim() != 3:
+        raise N.LtrError(f"photometric: images must be [N,h,w], got {list(src.shape)}")
+    n, h, w = (int(s) for s in src.shape)
+    ph = np.ascontiguousarray(params_host, dtype=np.float64)
+    if ph.ndim != 2 or ph.shape[0] != n:
+        raise N.LtrError(f"photometric: params must be [{n}, {N.PHOTOMETRIC_PARAMS}], got {list(ph.shape)}")
+    E = int(ellipses.shape[1]) if ellipses.dim() == 3 else -1
+    for nm, t, dt, shape in (("src", src, torch.uint8, None), ("dst", dst, torch.uint8, (n, h, w)),
+                             ("params", params, torch.float64, tuple(ph.shape)),
+                             ("ellipses", ellipses, torch.int32, (n, E, 5)),
+                             ("taps", taps, torch.float32, (n, N.PHOTOMETRIC_MAX_KSIZE)),
+                             ("workspace", workspace, torch.uint8, None)):
+        if t.dtype != dt or not t.is_contiguous() or t.device != dev or (shape is not None and tuple(t.shape) != shape):
+            raise N.LtrError(f"photometric: '{nm}' must be a contiguous {dt} tensor on {dev}"
+                             + (f" of shape {list(shape)}" if shape is not None else ""))
+    with torch.cuda.device(dev):
+        rc = N.load().ltr_photometric(_ptr(src), _ptr(dst), n, h, w, ph.ctypes.data_as(C.c_void_p), _ptr(params),
+                                      int(ph.shape[1]), _ptr(ellipses), E, _ptr(taps), _ptr(workspace),
+                                      int(workspace.numel()), dev.index, _stream_ptr(dev))
+    N.check(rc, "ltr_photometric")
+
+
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     """ltr_match_distmat on dist [P, n0, n1] (CUDA).  Returns dict(matches0 [P,n0], scores0, nn1, counts)."""
     _req_cuda(dist, "dist_mat")

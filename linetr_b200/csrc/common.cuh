@@ -44,6 +44,7 @@ enum KernelClass : int {
   KC_HOMOGRAPHY,
   KC_WARP,
   KC_ESSENTIAL,
+  KC_PHOTOMETRIC,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

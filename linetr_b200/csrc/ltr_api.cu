@@ -24,6 +24,7 @@
 #include "homography.cuh"
 #include "warp.cuh"
 #include "essential.cuh"
+#include "photometric.cuh"
 
 namespace ltr {
 
@@ -42,7 +43,7 @@ const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
-                                         "triplet", "homography", "warp", "essential"};
+                                         "triplet", "homography", "warp", "essential", "photometric"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1301,6 +1302,80 @@ int ltr_warp_pairs(const uint8_t* gray, const uint8_t* colour, int32_t n_images,
              std::min(1024 / std::min(16, (int)height), (int)width), tiles_x, tiles};
   LaunchScope ls(KC_WARP, s);
   LTR_CUDA_TRY(launch_pdl(warp_pairs_kernel, dim3(tiles * n_pairs), dim3(WP_THREADS), 0, s, a));
+  return LTR_OK;
+}
+
+static bool ph_is_int(double v, double lo, double hi) { return std::isfinite(v) && v == std::floor(v) && v >= lo && v <= hi; }
+
+// Host check of one image's parameter vector; an empty string when it is inside the contract.
+static std::string ph_check_params(const double* p, int32_t max_ellipses) {
+  for (int s : {PH_P_BRIGHT, PH_P_CONTRAST, PH_P_NOISE, PH_P_SPECKLE})
+    if (!ph_is_int(p[s], 0, 2)) return "an application count must be 0, 1 or 2";
+  for (int j = 0; j < 2; ++j) {
+    if (!ph_is_int(p[PH_P_BRIGHT + 1 + j], -255, 255)) return "a brightness delta must be an integer in [-255, 255]";
+    if (!std::isfinite(p[PH_P_CONTRAST + 1 + j])) return "a contrast alpha is not finite";
+    if (!(p[PH_P_NOISE + 1 + j] >= 0 && std::isfinite(p[PH_P_NOISE + 1 + j]))) return "a noise stddev must be finite and >= 0";
+    if (!(p[PH_P_SPECKLE + 1 + j] >= 0 && p[PH_P_SPECKLE + 1 + j] <= 1)) return "an impulse probability must lie in [0, 1]";
+  }
+  if (!ph_is_int(p[PH_P_BLUR], 0, 1) || !ph_is_int(p[PH_P_SHADE], 0, 1)) return "the blur and shade flags must be 0 or 1";
+  for (int k = 0; k < 9; ++k)
+    if (!std::isfinite(p[PH_P_KERNEL + k])) return "a motion-blur tap is not finite";
+  if (!ph_is_int(p[PH_P_KEY_LO], 0, 4294967295.0) || !ph_is_int(p[PH_P_KEY_HI], 0, 4294967295.0))
+    return "the noise key halves must be integers in [0, 2^32)";
+  if (p[PH_P_SHADE] != 0) {
+    if (!ph_is_int(p[PH_P_KSIZE], 1, PH_MAX_KSIZE) || ((int)p[PH_P_KSIZE] % 2) == 0)
+      return "the shade's kernel size must be odd and in [1, 149]";
+    if (!std::isfinite(p[PH_P_TRANSPARENCY])) return "the transparency is not finite";
+    if (!ph_is_int(p[PH_P_N_ELLIPSES], 0, max_ellipses)) return "the ellipse count must lie in [0, max_ellipses]";
+  }
+  return "";
+}
+
+int ltr_photometric(const uint8_t* in, uint8_t* out, int32_t n_images, int32_t height, int32_t width,
+                    const double* params_host, const double* params, int32_t n_params, const int32_t* ellipses,
+                    int32_t max_ellipses, const float* taps, void* workspace, int64_t workspace_bytes, int32_t device,
+                    void* stream) {
+  if (n_images < 0 || max_ellipses < 0)
+    return set_error(LTR_E_INVALID, "ltr_photometric: n_images and max_ellipses must be >= 0");
+  if (n_params != PH_NPARAM)
+    return set_error(LTR_E_INVALID, "ltr_photometric: n_params must be LTR_PHOTOMETRIC_PARAMS (" +
+                                        std::to_string(PH_NPARAM) + "), got " + std::to_string(n_params));
+  if (height < 1 || width < 1 || height > 32767 || width > 32767)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_photometric: height and width must be in [1, 32767]");
+  if (n_images > 65535) return set_error(LTR_E_UNSUPPORTED, "ltr_photometric: at most 65535 images per call");
+  if (n_images == 0) return LTR_OK;
+  if (!in || !out || !params_host || !params || !taps || !workspace || (max_ellipses > 0 && !ellipses))
+    return set_error(LTR_E_INVALID, "ltr_photometric: null argument");
+  const int64_t plane = (int64_t)n_images * height * width, a1 = align_up(plane, 256);
+  if (workspace_bytes < 2 * a1 + 4 * plane)
+    return set_error(LTR_E_WORKSPACE, "ltr_photometric: the workspace needs LTR_PHOTOMETRIC_WORKSPACE_BYTES(n, h, w)");
+  for (int32_t i = 0; i < n_images; ++i) {
+    const std::string why = ph_check_params(params_host + (size_t)i * PH_NPARAM, max_ellipses);
+    if (!why.empty()) return set_error(LTR_E_INVALID, "ltr_photometric: image " + std::to_string(i) + ": " + why);
+  }
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  PhotoArgs a{in, out, params, ellipses, taps, ws, ws + a1, reinterpret_cast<float*>(ws + 2 * a1),
+              height, width, max_ellipses};
+  LTR_CUDA_TRY(cudaMemsetAsync(a.mask, 0, (size_t)plane, s));
+  {
+    LaunchScope ls(KC_PHOTOMETRIC, s);
+    LTR_CUDA_TRY(launch_pdl(photo_stage1_kernel, dim3(cdiv(width, PS_TW), cdiv(height, PS_TH), n_images),
+                            dim3(PS_THREADS), 0, s, a));
+  }
+  if (max_ellipses > 0) {
+    LaunchScope ls(KC_PHOTOMETRIC, s);
+    LTR_CUDA_TRY(launch_pdl(photo_ellipse_kernel, dim3(max_ellipses, n_images), dim3(PE_THREADS), 0, s, a));
+  }
+  {
+    LaunchScope ls(KC_PHOTOMETRIC, s);
+    LTR_CUDA_TRY(launch_pdl(photo_blur_row_kernel, dim3(cdiv(width, PR_W), cdiv(height, PR_ROWS), n_images),
+                            dim3(PR_ROWS * 32), 0, s, a));
+  }
+  LaunchScope ls(KC_PHOTOMETRIC, s);
+  LTR_CUDA_TRY(launch_pdl(photo_blur_col_kernel, dim3(cdiv(width, PC_W), cdiv(height, PC_H), n_images),
+                          dim3(PC_W * (PC_H / PC_Q)), 0, s, a));
   return LTR_OK;
 }
 
