@@ -36,6 +36,14 @@ int ltr_debug_trace_read(unsigned long long* out128);
  * kblocks: 0 z, 1 ctx, 2 l128, 3 l256, 4 lpos, 5 y1i, 6 g, 7 xm, 8 hm, 9 qkv: split-bf16 activation images (hi and lo
  * planes, kblocks 64-wide k-blocks per 128-row block); 10 yf: fp32 rows [n_lines, 256] in hi, lo = NULL, kblocks 0.
  * Returns 0, or LTR_E_INVALID on a null argument. */
+/* ltr_linear_img with its residual read from a split-bf16 image: res [m, n] (device, row stride n) is split into an
+ * image first, and the GEMM adds hi + lo of it after the activation, as mlp2's x += delta does.  y_from_image given:
+ * the output image is written in place over the residual image (y must be NULL), then read back as hi + lo.  Else y
+ * gets the fp32 rows.  Test hook of the two image-residual epilogues. */
+int ltr_debug_linear_img_res(const float* x, int32_t ldx, const float* w_host, const float* bias, const float* res,
+                             float* y, float* y_from_image, int32_t m, int32_t n, int32_t k, int32_t act,
+                             int32_t bn_hint, int32_t device, void* stream);
+
 int ltr_debug_encode_images(const struct LtrModel* model, int32_t n_lines, void* workspace, void* hi[11], void* lo[11],
                             int32_t kblocks[11]);
 

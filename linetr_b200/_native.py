@@ -30,7 +30,7 @@ EXPORTED_SYMBOLS = (
 )
 # include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
 DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read",
-                 "ltr_debug_encode_images")
+                 "ltr_debug_encode_images", "ltr_debug_linear_img_res")
 # slots of ltr_debug_encode_images, in order
 ENCODE_IMAGES = ("z", "ctx", "l128", "l256", "lpos", "y1i", "g", "xm", "hm", "qkv", "yf")
 ABI_VERSION = 3
@@ -257,6 +257,10 @@ def load():
                                    C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, C.c_void_p]
     lib.ltr_linear_img.restype = C.c_int
+    lib.ltr_debug_linear_img_res.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.c_void_p]
+    lib.ltr_debug_linear_img_res.restype = C.c_int
     lib.ltr_linear_img_norm.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
                                         C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
                                         C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]

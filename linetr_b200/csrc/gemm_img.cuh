@@ -11,10 +11,12 @@
 //
 // The main loop is pure TMA + wgmma:  warp 8 (of a producer warpgroup) streams A and W tiles through an mbarrier ring,
 // two consumer warpgroups (64 rows each) issue 3 MMAs per k-step (lo*hi + hi*lo + hi*hi, fp32
-// accumulate in registers), then stage the accumulator through shared memory so that a thread
-// owns one row of 32 columns, apply bias / activation / residual and write fp32 rows and/or the
-// split-bf16 image of the result.  CTAs are persistent (one per SM) and walk the tile list
-// round-robin; the producer fetches the next tile's k-blocks while the epilogue runs.
+// accumulate in registers), then apply bias / activation / residual and write fp32 rows and/or the
+// split-bf16 image of the result.  A plain tile that writes only an image does that on the
+// accumulator fragment and bulk-stores each warp's rows (epi_frag_tile); the others stage the
+// accumulator through shared memory so that a thread owns one row of 32 columns.  CTAs are
+// persistent (one per SM) and walk the tile list round-robin; the producer fetches the next
+// tile's k-blocks while the epilogue runs.
 #pragma once
 #include "common.cuh"
 #include "linear_f32.cuh"
@@ -258,6 +260,14 @@ __device__ __forceinline__ void load_stage(const float* stg, int lane, float (&a
   __syncwarp();
 }
 
+// v, opaque to the compiler: what a staged epilogue derives from it (stage_acc64's sixteen staging addresses) is formed
+// per chunk.  Hoisted out of the tile loop, those addresses stayed live through the whole chained kernel, next to the
+// fragment epilogue's working set, and were spilled.
+__device__ __forceinline__ int opaque(int v) {
+  asm volatile("" : "+r"(v));
+  return v;
+}
+
 // Row-normalising epilogue of one 128 x 256 tile (see GemmImgArgs::norm).  A row's 256 columns sit in two
 // threads (column halves of every 64-column chunk, different warps); partial sums are exchanged through `xch`.
 // The accumulator stays in registers and is staged again for every pass.  ready: see publish_kblock.
@@ -265,10 +275,11 @@ template <int NR>
 __device__ __forceinline__ void epi_norm_tile(const GemmImgArgs& p, const float (&d)[NR], int mt, int q, int half, int lane,
                                               int row_a, float* stg_all, float* stg, uint8_t* stgb, float* xch,
                                               uint64_t* ready = nullptr) {
+  if (lane == 0) ptx::bulk_wait_read_all();   // a chain's fragment epilogues may still be bulk-storing from the staging
   const int row0 = mt * 128 + q * 32, r_in = q * 32 + lane;
   auto chunk = [&](int ch, float (&v)[32]) {
     epi_bar();
-    stage_acc64(d, ch, stg_all, row_a, lane);
+    stage_acc64(d, ch, stg_all, opaque(row_a), lane);
     epi_bar();
     load_stage(stg, lane, v);
     const int c0 = ch * 64 + half * 32;
@@ -356,12 +367,13 @@ __device__ __forceinline__ void epi_norm_tile(const GemmImgArgs& p, const float 
 template <int BN, int NR>
 __device__ __forceinline__ void epi_plain_tile(const GemmImgArgs& p, const float (&d)[NR], int mt, int nb, int q, int half, int lane,
                                                int row_a, float* stg_all, float* stg, uint8_t* stgb, uint64_t* ready = nullptr) {
+  if (lane == 0) ptx::bulk_wait_read_all();   // a chain's fragment epilogues may still be bulk-storing from the staging
   const int row0 = mt * 128 + q * 32;   // first row of this warp
 #pragma unroll 1
   for (int ch = 0; ch < BN / 64; ++ch) {
     float acc[32];
     epi_bar();
-    stage_acc64(d, ch, stg_all, row_a, lane);
+    stage_acc64(d, ch, stg_all, opaque(row_a), lane);
     epi_bar();
     load_stage(stg, lane, acc);
     const int nbase = nb * BN + ch * 64 + half * 32;
@@ -393,6 +405,141 @@ __device__ __forceinline__ void epi_plain_tile(const GemmImgArgs& p, const float
   publish_kblock(ready, nb * (BN / 64) + BN / 64 - 1, lane);
 }
 
+// ---------------------------------------------------------------- fragment epilogue: plain tiles that write only an image
+// Warp q of consumer warpgroup wg holds tile rows frow + lane / 4 + {0, 8}, frow = 64 wg + 16 q (ptx::wg_*), and row r
+// of an image tile is the 128-byte line at byte 128 r.  So the warp's 16 rows of one 64-column chunk are one contiguous
+// 2 KB piece of each plane's tile: the warp splits its fragment into its 4 KB staging block (hi piece, then lo piece, in
+// the tile's own SWIZZLE_128B layout) and lane 0 writes each piece with one bulk copy.  No barrier spans warps, and no
+// lane waits for its global stores.  Every element gets the staged path's operations in its order (acc + bias,
+// activation, acc + (hi + lo) of the residual, split), so the image is bit-identical to the split of its fp32 rows.
+// Ordering (all of it lane 0's bulk groups and the warp's residual mbarrier):
+//  - the staging block is rewritten only after the previous bulk store has read it (wait_group.read 0, then the warp
+//    syncs, or the residual load issued after that wait has landed);
+//  - chained GEMMs: output k-block kb is published once its stores have completed: wait_group 1 after the next
+//    chunk's commit, wait_group 0 after the tile's last one (publish_bulk);
+//  - an image residual (mlp2's in-place x += delta) is bulk-loaded into the staging block: chunk 0 before the tile's
+//    main loop (epi_frag_prefetch), chunk c + 1 once chunk c's store has read the block.  A lane reads the residual
+//    words at the positions it then overwrites with its output, and a chunk's store is issued after its residual
+//    has landed, so an in-place update reads the old values.
+__host__ __device__ __forceinline__ bool epi_frag(const GemmImgArgs& p) { return p.norm == NORM_NONE && p.O.hi && !p.C && !p.R; }
+
+// bytes of the warp's 16-row piece (first tile row frow) that lie above row M; rows >= M stay unwritten
+__device__ __forceinline__ uint32_t frag_piece_bytes(int M, int mt, int frow) {
+  return 128u * (uint32_t)min(max(M - (mt * 128 + frow), 0), 16);
+}
+
+// lane 0: this warp's piece of residual k-block r_kb0 + kb -> its staging block, completing on rbar
+__device__ __forceinline__ void frag_load_res(const GemmImgArgs& p, int mt, int kb, int frow, uint32_t bytes, uint8_t* stgb,
+                                              uint64_t* rbar) {
+  const size_t toff = ((size_t)mt * p.Rimg.kblocks + p.r_kb0 + kb) * IMG_TILE_ELEMS;
+  ptx::mbar_arrive_expect_tx(rbar, 2 * bytes);
+  ptx::bulk_g2s(stgb, reinterpret_cast<const uint8_t*>(p.Rimg.hi + toff) + 128 * frow, bytes, rbar);
+  ptx::bulk_g2s(stgb + 2048, reinterpret_cast<const uint8_t*>(p.Rimg.lo + toff) + 128 * frow, bytes, rbar);
+}
+
+// before a fragment tile's main loop: start loading its first chunk's residual, once the staging block is free
+__device__ __forceinline__ void epi_frag_prefetch(const GemmImgArgs& p, int mt, int kb0, int frow, int lane, uint8_t* stgb,
+                                                  uint64_t* rbar) {
+  if (lane != 0 || !p.Rimg.hi) return;
+  const uint32_t bytes = frag_piece_bytes(p.M, mt, frow);
+  if (!bytes) return;
+  ptx::bulk_wait_read_all();
+  frag_load_res(p, mt, kb0, frow, bytes, stgb, rbar);
+}
+
+// Chained GEMMs, lane 0: all but its newest N bulk groups have completed, and with them every store of output k-block
+// kb; fence them to the async proxy (the next op's TMA reads) and count the warp on kb_ready[kb] (as publish_kblock).
+template <int N>
+__device__ __forceinline__ void publish_bulk(uint64_t* ready, int kb) {
+  ptx::bulk_wait<N>();
+  ptx::fence_proxy_async_global();
+  ptx::mbar_arrive(&ready[kb]);
+}
+
+// The fragment epilogue of one 128 x BN tile for this warp (d is consumed in place).  ph0: parity of the residual
+// barrier's phase that completes with this tile's first load.  The barrier completes one phase per load, a tile issues
+// BN / 64 loads when its piece has rows below M and none otherwise, and the m-tile never decreases along a CTA's walk,
+// so tiles without loads come last: after tl tiles, ph0 = (tl BN / 64) & 1, which is 0 for BN = 256 whatever the walk.
+// ready: chained GEMMs publish k-blocks up to the tile's second-to-last one here; the caller publishes the last one
+// (publish_bulk<0>).
+template <int BN, int NR>
+__device__ __forceinline__ void epi_frag_tile(const GemmImgArgs& p, float (&d)[NR], int mt, int nb, int frow, int lane,
+                                              uint8_t* stgb, uint64_t* rbar, uint32_t ph0, uint64_t* ready) {
+  constexpr int NCH = BN / 64;
+  const uint32_t bytes = frag_piece_bytes(p.M, mt, frow);
+  const bool res = p.Rimg.hi && bytes;
+  const int r8 = lane >> 2, cq = 2 * (lane & 3);   // fragment row mod 8 (also its swizzle key), first column of a pair
+  // word of (row r8, columns 8 j + cq) in the hi piece: 128 r8 + 16 (j ^ r8) + 2 cq = sbase ^ 16 j (the staging block is
+  // 4 KB aligned, so the fields occupy disjoint bits); row r8 + 8 is 1024 bytes further, the lo piece 2048
+  const uint32_t sbase = ptx::smem_u32(stgb) + 144u * r8 + 2u * cq;
+#pragma unroll
+  for (int c = 0; c < NCH; ++c) {
+    const int kb = nb * NCH + c;
+    if (p.bias) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const float2 b = *reinterpret_cast<const float2*>(p.bias + kb * 64 + 8 * j + cq);
+        const int e = 32 * c + 4 * j;
+        d[e] += b.x; d[e + 1] += b.y; d[e + 2] += b.x; d[e + 3] += b.y;
+      }
+    }
+    // the activation is uniform per op: branch once per chunk
+    if (p.act == ACT_RELU) {
+#pragma unroll
+      for (int e = 32 * c; e < 32 * c + 32; ++e) d[e] = fmaxf(d[e], 0.f);
+    } else if (p.act == ACT_GELU) {
+#pragma unroll
+      for (int e = 32 * c; e < 32 * c + 32; e += 2) {
+        const float2 g = gelu_erf2(make_float2(d[e], d[e + 1]));
+        d[e] = g.x; d[e + 1] = g.y;
+      }
+    }
+    if (res) {
+      ptx::mbar_wait(rbar, (ph0 + c) & 1);
+    } else {
+      if (lane == 0) ptx::bulk_wait_read_all();
+      __syncwarp();
+    }
+    // opaque to the compiler, so that the eight addresses below are formed per chunk: hoisted out of the tile loop, they
+    // stayed live through the whole kernel and were spilled
+    uint32_t sb = sbase;
+    asm volatile("" : "+r"(sb));
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        // the 32 lanes of one (j, h) write 32 distinct banks: word lane & 3 of 16-byte chunk j ^ r8 (8 distinct r8)
+        const uint32_t wh = (sb ^ (16u * j)) + 1024u * h, wl = wh + 2048u;
+        const int e = 32 * c + 4 * j + 2 * h;
+        float a = d[e], b = d[e + 1];
+        if (res) {
+          const uint32_t rh = ptx::ld_shared_u32(wh), rl = ptx::ld_shared_u32(wl);
+          a += __uint_as_float(rh << 16) + __uint_as_float(rl << 16);
+          b += __uint_as_float(rh & 0xFFFF0000u) + __uint_as_float(rl & 0xFFFF0000u);
+        }
+        uint32_t hi, lo;
+        ptx::split2_bf16(a, b, hi, lo);
+        ptx::st_shared_u32(wh, hi);
+        ptx::st_shared_u32(wl, lo);
+      }
+    ptx::fence_proxy_async_smem();
+    __syncwarp();
+    if (lane == 0) {
+      if (bytes) {
+        const size_t toff = ((size_t)mt * p.O.kblocks + p.o_kb0 + kb) * IMG_TILE_ELEMS;
+        ptx::bulk_s2g(reinterpret_cast<uint8_t*>(p.O.hi + toff) + 128 * frow, stgb, bytes);
+        ptx::bulk_s2g(reinterpret_cast<uint8_t*>(p.O.lo + toff) + 128 * frow, stgb + 2048, bytes);
+      }
+      ptx::bulk_commit();
+      if (ready && c > 0) publish_bulk<1>(ready, kb - 1);
+      if (res && c + 1 < NCH) {
+        ptx::bulk_wait_read_all();
+        frag_load_res(p, mt, kb + 1, frow, bytes, stgb, rbar);
+      }
+    }
+  }
+}
+
 // One k-block (64 deep) of a warpgroup's 64 x BN accumulator: three split products per K = 16 step
 // (lo*hi + hi*lo + hi*hi).  a_hi / a_lo: this warpgroup's 64 rows of the A tile planes; w_hi / w_lo: the W tile planes.
 template <int BN>
@@ -415,15 +562,20 @@ __device__ __forceinline__ void mma_kblock(float (&d)[BN / 2], uint32_t a_hi, ui
   }
 }
 
-template <int BN>
+// FRAG: the launch's op takes the fragment epilogue (epi_frag, chosen on the host).  The two epilogues are separate
+// instantiations so that neither one's registers are allocated around the other's: in one kernel, the staged
+// epilogue's hoisted staging addresses and the fragment epilogue together spilled into the main loop.
+template <int BN, bool FRAG>
 __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
   using Cfg = GemmImgCfg<BN>;
+  static_assert((2 * Cfg::STAGES + 8) * 8 <= Cfg::OFF_XCH - Cfg::OFF_BAR, "gemm_img: barrier area");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
+  uint64_t* res_bar = bars + 2 * Cfg::STAGES;   // one per consumer warp (epi_frag_tile's residual loads)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nk = p.W.K / 64;
@@ -435,6 +587,7 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
       ptx::mbar_init(&full[s], 1);
       ptx::mbar_init(&empty[s], 8);
     }
+    for (int w = 0; w < 8; ++w) ptx::mbar_init(&res_bar[w], 1);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -468,12 +621,14 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
   } else {
     // ---------------------------------------------------------------- consumers (2 warpgroups x 64 rows)
     // Main loop: wgmma with the accumulator in registers, one k-block in flight behind the one being issued.
-    // Epilogue: 64-column chunks of the accumulator go through the staging blocks so that a thread owns one
+    // Epilogue: image-only plain tiles work on the fragment and bulk-store each warp's rows (epi_frag_tile).
+    // Otherwise 64-column chunks of the accumulator go through the staging blocks so that a thread owns one
     // row (lane = row) of 32 columns; global traffic then goes through the warp's 4 KB block so that every
     // global load/store instruction touches whole 32-byte sectors of a few rows.
     ptx::setmaxnreg_inc<232>();
     const int wg = warp >> 2, q = warp & 3, half = warp >> 2;
     const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int frow = 16 * warp;   // first tile row of the warp's fragment (64 wg + 16 q)
     float* stg_all = reinterpret_cast<float*>(smem + Cfg::OFF_STG);
     float* stg = stg_all + warp * (Cfg::STG_WARP / 4);
     uint8_t* stgb = reinterpret_cast<uint8_t*>(stg);
@@ -483,6 +638,7 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
       float d[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      if constexpr (FRAG) epi_frag_prefetch(p, mt, nb * (BN / 64), frow, lane, stgb, &res_bar[warp]);
       if (tl < 4 && tid == 0) LTR_STAMP(tl * 16 + 0);
       for (int kb = 0; kb < nk; ++kb, ++it) {
         const int s = it % Cfg::STAGES;
@@ -501,14 +657,21 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
       ptx::wg_fence_regs(d);
       if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % Cfg::STAGES]);
       if (tl < 4 && tid == 0) LTR_STAMP(tl * 16 + 2);
-      if constexpr (BN == 256) {
-        if (p.norm != NORM_NONE) {
-          epi_norm_tile(p, d, mt, q, half, lane, row_a, stg_all, stg, stgb, reinterpret_cast<float*>(smem + Cfg::OFF_XCH));
-          continue;
+      if constexpr (FRAG) {
+        epi_frag_tile<BN>(p, d, mt, nb, frow, lane, stgb, &res_bar[warp], (tl * (BN / 64)) & 1, nullptr);
+      } else {
+        if constexpr (BN == 256) {
+          if (p.norm != NORM_NONE) {
+            epi_norm_tile(p, d, mt, q, half, lane, row_a, stg_all, stg, stgb, reinterpret_cast<float*>(smem + Cfg::OFF_XCH));
+            continue;
+          }
         }
+        epi_plain_tile<BN>(p, d, mt, nb, q, half, lane, row_a, stg_all, stg, stgb);
       }
-      epi_plain_tile<BN>(p, d, mt, nb, q, half, lane, row_a, stg_all, stg, stgb);
       if (tl < 4 && tid == 0) LTR_STAMP(tl * 16 + 5);
+    }
+    if constexpr (FRAG) {
+      if (lane == 0) ptx::bulk_wait<0>();   // the staging stays allocated, and the writes done, until the stores complete
     }
   }
 }
@@ -527,16 +690,16 @@ inline int device_sm_count() {
   return v;
 }
 
-template <int BN>
+template <int BN, bool FRAG>
 static int launch_gemm_img_bn(GemmImgArgs a, cudaStream_t s) {
   using Cfg = GemmImgCfg<BN>;
-  LTR_CUDA_TRY(ensure_dynamic_smem(gemm_img_kernel<BN>, Cfg::SMEM));
+  LTR_CUDA_TRY(ensure_dynamic_smem(gemm_img_kernel<BN, FRAG>, Cfg::SMEM));
   a.m_tiles = cdiv(a.M, 128);
   a.n_blks = a.W.N / BN;
   const int tiles = a.m_tiles * a.n_blks;
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
   LaunchScope ls(KC_LINEAR, s);
-  LTR_CUDA_TRY(launch_pdl(gemm_img_kernel<BN>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, a));
+  LTR_CUDA_TRY(launch_pdl(gemm_img_kernel<BN, FRAG>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, a));
   return 0;
 }
 
@@ -559,16 +722,17 @@ inline int launch_gemm_img(const GemmImgArgs& a, cudaStream_t s, int bn_hint = 0
         (a.R && a.Rimg.hi) || (a.nadd && a.NaddImg.hi) ||
         (a.NaddImg.hi && (a.nadd_kb0 < 0 || a.nadd_kb0 + 4 > a.NaddImg.kblocks)))
       return set_error(-1, "gemm_img: the row-norm epilogue needs N == 256, no activation, fp32 residual");
-    return launch_gemm_img_bn<256>(a, s);
+    return launch_gemm_img_bn<256, false>(a, s);
   }
-  if (bn_hint == 64 || a.W.N % 128) return launch_gemm_img_bn<64>(a, s);
+  const bool frag = epi_frag(a);
+  if (bn_hint == 64 || a.W.N % 128) return frag ? launch_gemm_img_bn<64, true>(a, s) : launch_gemm_img_bn<64, false>(a, s);
   int bn = bn_hint;
   if (!bn) {
     bn = 128;
     if (a.W.N % 256 == 0 && (long long)cdiv(a.M, 128) * (a.W.N / 256) >= device_sm_count()) bn = 256;
   }
-  if (bn == 256 && a.W.N % 256 == 0) return launch_gemm_img_bn<256>(a, s);
-  return launch_gemm_img_bn<128>(a, s);
+  if (bn == 256 && a.W.N % 256 == 0) return frag ? launch_gemm_img_bn<256, true>(a, s) : launch_gemm_img_bn<256, false>(a, s);
+  return frag ? launch_gemm_img_bn<128, true>(a, s) : launch_gemm_img_bn<128, false>(a, s);
 }
 
 // ---------------------------------------------------------------- chained GEMMs (one launch, several row-local layers)
@@ -591,7 +755,8 @@ constexpr int CHAIN_MAX_KB = 16;   // output k-blocks of an op that feeds the ne
 // k-block it < CHAIN_TRACE_KB of the CTA's walk: slot 3*it = producer has issued the k-block's loads (its empty-wait
 // ended), 3*it + 1 = the consumers' first thread sees its stage landed (full-wait returned), 3*it + 2 = its MMAs are
 // done (wgmma.wait_group 0).  Tile o * 4 + nb of the first m-tile: slot CHAIN_TRACE_EPI + o * 4 + nb = its epilogue
-// is done (an epilogue starts at its last k-block's 3*it + 2).  CHAIN_TRACE_T0 / + 1: producer / consumers past
+// is done (an epilogue starts at its last k-block's 3*it + 2; a fragment epilogue is done when the first thread's warp
+// has committed its last bulk store, before the wait that publishes that k-block).  CHAIN_TRACE_T0 / + 1: producer / consumers past
 // pdl_wait.  Off (the default), a stamp costs its thread an `it` compare and, in the window, a load of g_dbg_on.
 constexpr int CHAIN_TRACE_KB = 36;
 constexpr int CHAIN_TRACE_EPI = 3 * CHAIN_TRACE_KB;
@@ -605,7 +770,7 @@ struct GemmChainArgs {
 __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constant__ GemmChainArgs c) {
   constexpr int BN = 256;
   using Cfg = GemmImgCfg<BN>;
-  static_assert((2 * Cfg::STAGES + CHAIN_MAX_KB) * 8 <= Cfg::OFF_XCH - Cfg::OFF_BAR, "gemm_chain: barrier area");
+  static_assert((2 * Cfg::STAGES + CHAIN_MAX_KB + 8) * 8 <= Cfg::OFF_XCH - Cfg::OFF_BAR, "gemm_chain: barrier area");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t raw = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
@@ -613,6 +778,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
   uint64_t* kb_ready = bars + 2 * Cfg::STAGES;
+  uint64_t* res_bar = kb_ready + CHAIN_MAX_KB;   // one per consumer warp (epi_frag_tile's residual loads)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   pdl_launch_dependents();
@@ -623,6 +789,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
       ptx::mbar_init(&empty[s], 8);
     }
     for (int k = 0; k < CHAIN_MAX_KB; ++k) ptx::mbar_init(&kb_ready[k], 8);
+    for (int w = 0; w < 8; ++w) ptx::mbar_init(&res_bar[w], 1);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -679,6 +846,7 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
     if (tid == 0) LTR_DBG_STAMP(CHAIN_TRACE_T0 + 1);
     const int wg = warp >> 2, q = warp & 3, half = warp >> 2;
     const int row_a = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int frow = 16 * warp;   // first tile row of the warp's fragment (64 wg + 16 q)
     float* stg_all = reinterpret_cast<float*>(smem + Cfg::OFF_STG);
     float* stg = stg_all + warp * (Cfg::STG_WARP / 4);
     uint8_t* stgb = reinterpret_cast<uint8_t*>(stg);
@@ -688,11 +856,13 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
       for (int o = 0; o < c.n_ops; ++o) {
         const GemmImgArgs& p = c.op[o];
         const int nk = p.W.K / 64;
+        const bool frag = epi_frag(p);
         uint64_t* ready = o + 1 < c.n_ops ? kb_ready : nullptr;
         for (int nb = 0; nb < p.n_blks; ++nb) {
           float d[BN / 2];
 #pragma unroll
           for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+          if (frag) epi_frag_prefetch(p, mt, nb * (BN / 64), frow, lane, stgb, &res_bar[warp]);
           for (int kb = 0; kb < nk; ++kb, ++it) {
             const int s = it % Cfg::STAGES;
             ptx::mbar_wait(&full[s], (it / Cfg::STAGES) & 1);
@@ -714,11 +884,15 @@ __global__ void __launch_bounds__(384, 1) gemm_chain_kernel(const __grid_constan
           }
           if (p.norm != NORM_NONE)
             epi_norm_tile(p, d, mt, q, half, lane, row_a, stg_all, stg, stgb, xch, ready);
+          else if (frag)
+            epi_frag_tile<BN>(p, d, mt, nb, frow, lane, stgb, &res_bar[warp], 0, ready);
           else
             epi_plain_tile<BN>(p, d, mt, nb, q, half, lane, row_a, stg_all, stg, stgb, ready);
           if (mt == (int)blockIdx.x && nb < 4 && tid == 0) LTR_DBG_STAMP(CHAIN_TRACE_EPI + o * 4 + nb);
+          if (frag && ready && lane == 0) publish_bulk<0>(ready, nb * (BN / 64) + BN / 64 - 1);
         }
       }
+    if (lane == 0) ptx::bulk_wait<0>();   // the staging stays allocated, and the writes done, until the stores complete
   }
 }
 

@@ -1388,9 +1388,11 @@ int ltr_linear(const float* x, int32_t ldx, const float* w, const float* bias, c
 
 struct NormSpec { int norm; float eps; const float* g; const float* beta; const float* add; int ldadd; };
 
+// res_image: the residual res [m, n] (row stride ldr) is split into the output image first and read from there (Rimg);
+// the output image, if any, is then written in place over it
 static int linear_img_impl(const float* x, int32_t ldx, const float* w_host, const float* bias, const float* res, int32_t ldr,
                            float* y, int32_t ldy, float* y_from_image, int32_t m, int32_t n, int32_t k, int32_t act,
-                           int32_t bn_hint, int32_t device, void* stream, const NormSpec& ns) {
+                           int32_t bn_hint, int32_t device, void* stream, const NormSpec& ns, bool res_image = false) {
   if (!x || !w_host || (!y && !y_from_image)) return set_error(LTR_E_INVALID, "ltr_linear_img: null argument");
   if (n % 64 || k % 64) return set_error(LTR_E_UNSUPPORTED, "ltr_linear_img: n and k must be multiples of 64");
   LTR_CUDA_TRY(cudaSetDevice(device));
@@ -1414,8 +1416,13 @@ static int linear_img_impl(const float* x, int32_t ldx, const float* w_host, con
       LaunchScope ls(KC_IMG_CONVERT, s);
       to_image_kernel<<<cdiv((long long)m * (k / 8), 256), 256, 0, s>>>(x, ldx, m, k, A, 0);
     }
+    if (res_image) {
+      LaunchScope ls(KC_IMG_CONVERT, s);
+      to_image_kernel<<<cdiv((long long)m * (n / 8), 256), 256, 0, s>>>(res, ldr, m, n, O, 0);
+    }
     GemmImgArgs a{};
-    a.A = A; a.a_kb0 = 0; a.bias = bias; a.R = res; a.ldr = ldr; a.C = y; a.ldc = ldy; a.M = m; a.act = act;
+    a.A = A; a.a_kb0 = 0; a.bias = bias; a.C = y; a.ldc = ldy; a.M = m; a.act = act;
+    if (res_image) { a.Rimg = O; a.r_kb0 = 0; } else { a.R = res; a.ldr = ldr; }
     a.W.hi = reinterpret_cast<const __nv_bfloat16*>(dw);
     a.W.lo = reinterpret_cast<const __nv_bfloat16*>(dw + (size_t)n * k);
     a.W.N = n; a.W.K = k;
@@ -1439,6 +1446,15 @@ int ltr_linear_img(const float* x, int32_t ldx, const float* w_host, const float
                    int32_t bn_hint, int32_t device, void* stream) {
   return linear_img_impl(x, ldx, w_host, bias, res, ldr, y, ldy, y_from_image, m, n, k, act, bn_hint, device, stream,
                          NormSpec{NORM_NONE, 0.f, nullptr, nullptr, nullptr, 0});
+}
+
+int ltr_debug_linear_img_res(const float* x, int32_t ldx, const float* w_host, const float* bias, const float* res,
+                             float* y, float* y_from_image, int32_t m, int32_t n, int32_t k, int32_t act,
+                             int32_t bn_hint, int32_t device, void* stream) {
+  if (!res || (y != nullptr) == (y_from_image != nullptr))
+    return set_error(LTR_E_INVALID, "ltr_debug_linear_img_res: res and exactly one of y, y_from_image required");
+  return linear_img_impl(x, ldx, w_host, bias, res, n, y, n, y_from_image, m, n, k, act, bn_hint, device, stream,
+                         NormSpec{NORM_NONE, 0.f, nullptr, nullptr, nullptr, 0}, true);
 }
 
 int ltr_linear_img_norm(const float* x, int32_t ldx, const float* w_host, const float* bias, const float* res, int32_t ldr,

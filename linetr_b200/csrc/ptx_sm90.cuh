@@ -74,6 +74,19 @@ __device__ __forceinline__ void bulk_s2g(void* gmem_dst, const void* smem_src, u
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all bulk groups of this thread have finished READING their shared-memory source
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// all but the newest N bulk groups of this thread have completed: their global writes are performed
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
+// 32-bit shared-memory access at a shared-window address (smem_u32)
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
 
 // Ampere-style 16-byte asynchronous copy global -> shared (no register staging); src_bytes = 0
 // zero-fills the destination.
