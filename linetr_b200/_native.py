@@ -18,19 +18,6 @@ c_int32_p = C.POINTER(C.c_int32)
 LAYOUT_ROWS = 0
 LAYOUT_CHANNEL_FIRST = 1
 
-# Every symbol include/linetr_b200.h declares (tests check the library exports all of them).
-EXPORTED_SYMBOLS = (
-    "ltr_abi_version", "ltr_last_error", "ltr_create", "ltr_destroy", "ltr_encode_workspace_bytes",
-    "ltr_desc_tiles_bytes", "ltr_encode", "ltr_match_workspace_bytes", "ltr_match", "ltr_gather_wait", "ltr_match_distmat",
-    "ltr_merge_sublines", "ltr_tokenize", "ltr_tokenize_batch", "ltr_linear", "ltr_linear_img", "ltr_linear_img_norm",
-    "ltr_launch_count", "ltr_reset_launch_count", "ltr_profile_begin", "ltr_profile_end",
-    "ltr_image_tiles_bytes", "ltr_image_tiles", "ltr_match_indexed_workspace_bytes", "ltr_match_indexed",
-    "ltr_line_gt", "ltr_triplet_loss", "ltr_homography", "ltr_warp_pairs", "ltr_essential",
-    "ltr_photometric",
-)
-# include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
-DEBUG_SYMBOLS = ("ltr_gemm_bench", "ltr_gemm_chain_bench", "ltr_gemm_trace", "ltr_debug_trace_arm", "ltr_debug_trace_read",
-                 "ltr_debug_encode_images", "ltr_debug_linear_img_res")
 # slots of ltr_debug_encode_images, in order
 ENCODE_IMAGES = ("z", "ctx", "l128", "l256", "lpos", "y1i", "g", "xm", "hm", "qkv", "yf")
 ABI_VERSION = 3
@@ -174,6 +161,57 @@ class LtrEssentialOutput(C.Structure):
                 ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
 
 
+_P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
+# {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
+# of them, and each entry against its C prototype)
+PROTOTYPES = {
+    "ltr_abi_version": (C.c_int, []),
+    "ltr_last_error": (C.c_char_p, []),
+    "ltr_create": (C.c_int, [_ptr(LtrTensor), _I32, _ptr(LtrConfig), _I32, _ptr(_P)]),
+    "ltr_destroy": (None, [_P]),
+    "ltr_encode_workspace_bytes": (_I64, [_P, _I32, _I32, _I32]),
+    "ltr_desc_tiles_bytes": (_I64, [_I32]),
+    "ltr_encode": (C.c_int, [_P, _ptr(LtrEncodeInput), _ptr(LtrEncodeOutput), _P, _I64, _P]),
+    "ltr_match_workspace_bytes": (_I64, [_ptr(LtrMatchInput)]),
+    "ltr_match": (C.c_int, [_ptr(LtrMatchInput), _ptr(LtrMatchOutput), _I32, _P]),
+    "ltr_gather_wait": (C.c_int, [_P, _I32, _I32, _I32, _I32, _P, _I32, _P]),
+    "ltr_image_tiles_bytes": (_I64, [_I32, c_int32_p]),
+    "ltr_image_tiles": (C.c_int, [_P, _I32, _P, _P, _I32, _I32, _I32, _P, _I32, _P]),
+    "ltr_match_indexed_workspace_bytes": (_I64, [_ptr(LtrMatchInput), _ptr(LtrPairIndex)]),
+    "ltr_match_indexed": (C.c_int, [_ptr(LtrMatchInput), _ptr(LtrPairIndex), _ptr(LtrMatchOutput), _I32, _P]),
+    "ltr_match_distmat": (C.c_int, [_P, _I32, _I32, _I32, _I64, _F32, _I32, _P, _P, _P, _P, _I32, _P]),
+    "ltr_merge_sublines": (C.c_int, [_P, _I64, _I32, _P, _P, _P, _P, _I32, _I32, _P, _I64, _I32, _P]),
+    "ltr_tokenize": (C.c_int, [_ptr(LtrTokenizeInput)] + [_P] * 7 + [_I32, _P]),
+    "ltr_tokenize_batch": (C.c_int, [_ptr(LtrTokenizeBatchInput)] + [_P] * 7 + [_I32, _P]),
+    "ltr_line_gt": (C.c_int, [_ptr(LtrLineGtInput), _ptr(LtrLineGtOutput), _I32, _P]),
+    "ltr_triplet_loss": (C.c_int, [_ptr(LtrTripletInput), _ptr(LtrTripletOutput), _I32, _P]),
+    "ltr_homography": (C.c_int, [_ptr(LtrHomographyInput), _ptr(LtrHomographyOutput), _I32, _P]),
+    "ltr_essential": (C.c_int, [_ptr(LtrEssentialInput), _ptr(LtrEssentialOutput), _I32, _P]),
+    "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
+    "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
+    "ltr_linear": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P] + [_I32] * 6 + [_P]),
+    "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),
+    "ltr_linear_img_norm": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _I32, _F32, _P, _P, _P, _I32, _P, _I32, _P, _I32,
+                                      _I32, _I32, _P]),
+    "ltr_launch_count": (_I64, []),
+    "ltr_reset_launch_count": (None, []),
+    "ltr_profile_begin": (None, []),
+    "ltr_profile_end": (C.c_int, [_ptr(C.c_char_p), c_float_p, c_int32_p, _I32]),
+}
+# include/linetr_b200_debug.h (micro-benchmark / tracing hooks; not part of the drop-in boundary)
+DEBUG_PROTOTYPES = {
+    "ltr_gemm_bench": (_F32, [_I32] * 7),
+    "ltr_gemm_chain_bench": (_F32, [_I32] * 4),
+    "ltr_gemm_trace": (_ptr(C.c_uint64), []),
+    "ltr_debug_trace_arm": (None, [_I32]),
+    "ltr_debug_trace_read": (C.c_int, [_ptr(C.c_uint64)]),
+    "ltr_debug_linear_img_res": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P] + [_I32] * 6 + [_P]),
+    "ltr_debug_encode_images": (C.c_int, [_P, _I32, _P, _ptr(_P), _ptr(_P), c_int32_p]),
+}
+EXPORTED_SYMBOLS = tuple(PROTOTYPES)
+DEBUG_SYMBOLS = tuple(DEBUG_PROTOTYPES)
+
+
 def lib_path() -> str:
     return _LIB_PATH
 
@@ -191,97 +229,9 @@ def load():
     missing = [s for s in EXPORTED_SYMBOLS if not hasattr(lib, s)]
     if missing:
         raise LtrError(f"linetr_b200: the native library predates this binding (missing {', '.join(missing)}); rebuild it")
-    lib.ltr_abi_version.restype = C.c_int
-    lib.ltr_last_error.restype = C.c_char_p
-    lib.ltr_create.argtypes = [C.POINTER(LtrTensor), C.c_int32, C.POINTER(LtrConfig), C.c_int32,
-                               C.POINTER(C.c_void_p)]
-    lib.ltr_create.restype = C.c_int
-    lib.ltr_destroy.argtypes = [C.c_void_p]
-    lib.ltr_destroy.restype = None
-    lib.ltr_encode_workspace_bytes.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32]
-    lib.ltr_encode_workspace_bytes.restype = C.c_int64
-    lib.ltr_desc_tiles_bytes.argtypes = [C.c_int32]
-    lib.ltr_desc_tiles_bytes.restype = C.c_int64
-    lib.ltr_encode.argtypes = [C.c_void_p, C.POINTER(LtrEncodeInput), C.POINTER(LtrEncodeOutput), C.c_void_p,
-                               C.c_int64, C.c_void_p]
-    lib.ltr_encode.restype = C.c_int
-    lib.ltr_match_workspace_bytes.argtypes = [C.POINTER(LtrMatchInput)]
-    lib.ltr_match_workspace_bytes.restype = C.c_int64
-    lib.ltr_match.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrMatchOutput), C.c_int32, C.c_void_p]
-    lib.ltr_match.restype = C.c_int
-    lib.ltr_image_tiles_bytes.argtypes = [C.c_int32, c_int32_p]
-    lib.ltr_image_tiles_bytes.restype = C.c_int64
-    lib.ltr_image_tiles.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
-                                    C.c_void_p, C.c_int32, C.c_void_p]
-    lib.ltr_image_tiles.restype = C.c_int
-    lib.ltr_match_indexed_workspace_bytes.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrPairIndex)]
-    lib.ltr_match_indexed_workspace_bytes.restype = C.c_int64
-    lib.ltr_match_indexed.argtypes = [C.POINTER(LtrMatchInput), C.POINTER(LtrPairIndex), C.POINTER(LtrMatchOutput),
-                                      C.c_int32, C.c_void_p]
-    lib.ltr_match_indexed.restype = C.c_int
-    lib.ltr_line_gt.argtypes = [C.POINTER(LtrLineGtInput), C.POINTER(LtrLineGtOutput), C.c_int32, C.c_void_p]
-    lib.ltr_line_gt.restype = C.c_int
-    lib.ltr_triplet_loss.argtypes = [C.POINTER(LtrTripletInput), C.POINTER(LtrTripletOutput), C.c_int32, C.c_void_p]
-    lib.ltr_triplet_loss.restype = C.c_int
-    lib.ltr_homography.argtypes = [C.POINTER(LtrHomographyInput), C.POINTER(LtrHomographyOutput), C.c_int32, C.c_void_p]
-    lib.ltr_homography.restype = C.c_int
-    lib.ltr_essential.argtypes = [C.POINTER(LtrEssentialInput), C.POINTER(LtrEssentialOutput), C.c_int32, C.c_void_p]
-    lib.ltr_essential.restype = C.c_int
-    lib.ltr_warp_pairs.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [c_int32_p, C.c_void_p, C.c_void_p,
-                                                                             C.c_int32, C.c_void_p, C.c_void_p,
-                                                                             C.c_int32, C.c_void_p]
-    lib.ltr_warp_pairs.restype = C.c_int
-    lib.ltr_photometric.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int32] * 3 + [C.c_void_p, C.c_void_p, C.c_int32,
-                                                                                C.c_void_p, C.c_int32, C.c_void_p,
-                                                                                C.c_void_p, C.c_int64, C.c_int32,
-                                                                                C.c_void_p]
-    lib.ltr_photometric.restype = C.c_int
-    lib.ltr_gather_wait.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
-    lib.ltr_gather_wait.restype = C.c_int
-    lib.ltr_match_distmat.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_float,
-                                      C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                                      C.c_void_p]
-    lib.ltr_match_distmat.restype = C.c_int
-    lib.ltr_merge_sublines.argtypes = [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                       C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int32,
-                                       C.c_void_p]
-    lib.ltr_merge_sublines.restype = C.c_int
-    lib.ltr_tokenize.argtypes = [C.POINTER(LtrTokenizeInput)] + [C.c_void_p] * 7 + [C.c_int32, C.c_void_p]
-    lib.ltr_tokenize.restype = C.c_int
-    lib.ltr_tokenize_batch.argtypes = [C.POINTER(LtrTokenizeBatchInput)] + [C.c_void_p] * 7 + [C.c_int32, C.c_void_p]
-    lib.ltr_tokenize_batch.restype = C.c_int
-    lib.ltr_linear.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                               C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-    lib.ltr_linear.restype = C.c_int
-    lib.ltr_linear_img.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                                   C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                   C.c_int32, C.c_void_p]
-    lib.ltr_linear_img.restype = C.c_int
-    lib.ltr_debug_linear_img_res.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                             C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                                             C.c_void_p]
-    lib.ltr_debug_linear_img_res.restype = C.c_int
-    lib.ltr_linear_img_norm.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
-                                        C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32,
-                                        C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
-    lib.ltr_linear_img_norm.restype = C.c_int
-    lib.ltr_gemm_bench.argtypes = [C.c_int32] * 7
-    lib.ltr_gemm_bench.restype = C.c_float
-    lib.ltr_gemm_chain_bench.argtypes = [C.c_int32] * 4
-    lib.ltr_gemm_chain_bench.restype = C.c_float
-    lib.ltr_gemm_trace.restype = C.POINTER(C.c_uint64)
-    lib.ltr_debug_trace_arm.argtypes = [C.c_int32]
-    lib.ltr_debug_trace_arm.restype = None
-    lib.ltr_debug_trace_read.argtypes = [C.POINTER(C.c_uint64)]
-    lib.ltr_debug_trace_read.restype = C.c_int
-    lib.ltr_debug_encode_images.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.POINTER(C.c_void_p),
-                                            C.POINTER(C.c_void_p), c_int32_p]
-    lib.ltr_debug_encode_images.restype = C.c_int
-    lib.ltr_launch_count.restype = C.c_int64
-    lib.ltr_reset_launch_count.restype = None
-    lib.ltr_profile_begin.restype = None
-    lib.ltr_profile_end.argtypes = [C.POINTER(C.c_char_p), c_float_p, c_int32_p, C.c_int32]
-    lib.ltr_profile_end.restype = C.c_int
+    for name, (restype, argtypes) in {**PROTOTYPES, **DEBUG_PROTOTYPES}.items():
+        f = getattr(lib, name)
+        f.restype, f.argtypes = restype, argtypes
     if lib.ltr_abi_version() != ABI_VERSION:
         raise LtrError("linetr_b200: ABI version mismatch between _native.py and the shared library")
     _lib = lib

@@ -47,6 +47,54 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
+def _call(entry: str, dev, *args):
+    """C-ABI entry point `entry`(*args, device, stream) on the current stream of `dev`; raises on a non-zero return
+    code."""
+    with torch.cuda.device(dev):
+        rc = getattr(N.load(), entry)(*args, dev.index, _stream_ptr(dev))
+    N.check(rc, entry)
+
+
+def _check_tensors(who: str, dev, specs):
+    """Raises unless every tensor of `specs`, (name, tensor or None, dtype[, shape]), is None or a contiguous tensor
+    of that dtype (and shape) on `dev`."""
+    for nm, t, dt, *shape in specs:
+        shape = shape[0] if shape else None
+        if t is None:
+            continue
+        if t.dtype != dt or not t.is_contiguous() or t.device != dev or (shape is not None and tuple(t.shape) != shape):
+            raise N.LtrError(f"{who}: '{nm}' must be a contiguous {dt} tensor on {dev}"
+                             + (f" of shape {list(shape)}" if shape is not None else ""))
+
+
+_staging = []   # (pinned host buffer, event behind its copy) until the copy has finished
+_TORCH_DTYPE = {np.dtype(np.float64): torch.float64, np.dtype(np.float32): torch.float32,
+                np.dtype(np.int32): torch.int32}
+
+
+def stage(arrays: dict, device) -> dict:
+    """One pinned staging buffer, one non-blocking H2D copy on the current stream of `device`: -> device views of the
+    host arrays (float64, float32 or int32).  The buffer is held (with an event behind the copy) until the copy has
+    finished, so it is never reused early."""
+    global _staging
+    _staging = [(b, e) for b, e in _staging if not e.query()]
+    layout, total = {}, 0
+    for k, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        total = (total + 15) // 16 * 16
+        layout[k] = (total, a)
+        total += a.nbytes
+    host = torch.empty(max(total, 16), dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    for o, a in layout.values():
+        hv[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
+    dev = host.to(device, non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(device))
+    _staging.append((host, ev))
+    return {k: dev[o:o + a.nbytes].view(_TORCH_DTYPE[a.dtype]).view(a.shape) for k, (o, a) in layout.items()}
+
+
 class ModelHandle:
     """Owns one LtrModel* (packed weights on one GPU)."""
 
@@ -141,7 +189,7 @@ def encode(handle: ModelHandle, sublines, resp, angle, pnt, desc, score, image_w
     outp = N.LtrEncodeOutput(out_cf.data_ptr() if out_cf is not None else None,
                              out_rows.data_ptr() if out_rows is not None else None,
                              out_tiles.data_ptr() if out_tiles is not None else None)
-    with torch.cuda.device(dev):
+    with torch.cuda.device(dev):   # ltr_encode takes no device argument, so it does not go through _call
         rc = handle._lib.ltr_encode(handle.ptr, C.byref(inp), C.byref(outp), _ptr(ws), ws.numel(), _stream_ptr(dev))
     N.check(rc, "ltr_encode")
     return (out_cf, out_rows, out_tiles) if want_tiles else (out_cf, out_rows)
@@ -180,9 +228,7 @@ def _match(entry: str, dev, inp: dict, out: dict, idx=None, gather=None):
     ws = _match_workspace(dev, need)
     o = _struct(N.LtrMatchOutput, workspace=ws, workspace_bytes=ws.numel(),
                 gather=C.pointer(gather) if gather is not None else None, **out)
-    with torch.cuda.device(dev):
-        rc = getattr(lib, entry)(*args, C.byref(o), dev.index, _stream_ptr(dev))
-    N.check(rc, entry)
+    _call(entry, dev, *args, C.byref(o))
 
 
 def match_descriptors(desc0, desc1, layout, n_pairs, nn_thresh, mutual=True, *, n0=0, n1=0, cu0=None, cu1=None,
@@ -260,10 +306,8 @@ def image_tiles(desc: torch.Tensor, layout: int, cu_host: np.ndarray, cu_dev: to
     if nbytes < 0:
         N.check(nbytes, "ltr_image_tiles_bytes")
     out = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        rc = lib.ltr_image_tiles(_ptr(desc), int(layout), _ptr(cu_dev), _ptr(tile_off_dev), n,
-                                 int(np.diff(cu_host).max(initial=0)), int(n_tiles), _ptr(out), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_image_tiles")
+    _call("ltr_image_tiles", dev, _ptr(desc), int(layout), _ptr(cu_dev), _ptr(tile_off_dev), n,
+          int(np.diff(cu_host).max(initial=0)), int(n_tiles), _ptr(out))
     return out
 
 
@@ -306,24 +350,21 @@ def line_gt(segs0, segs1, n_pairs, *, cu0, cu1, max_n0, max_n1, homography, homo
     _req_cuda(segs0, "segs0")
     _req_cuda(segs1, "segs1")
     dev = segs0.device
-    for nm, t, dt in (("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32), ("cu0", cu0, torch.int32),
-                      ("cu1", cu1, torch.int32), ("homography", homography, torch.float64),
-                      ("homography_inv", homography_inv, torch.float64), ("n_gt", n_gt, torch.int32),
-                      ("assign", assign, torch.float32), ("pred0", pred0, torch.int32), ("tfpn", tfpn, torch.int32),
-                      ("proj0", proj0, torch.float32), ("proj1", proj1, torch.float32)):
-        if t is None:
-            continue
-        _req_cuda(t, nm)
-        if t.dtype != dt or not t.is_contiguous() or t.device != dev:
-            raise N.LtrError(f"line_gt: '{nm}' must be a contiguous {dt} tensor on {dev}")
-    inp = N.LtrLineGtInput(_ptr(segs0).value, _ptr(segs1).value, _ptr(cu0).value, _ptr(cu1).value, _ptr(homography).value,
-                           _ptr(homography_inv).value, _ptr(proj0).value, _ptr(proj1).value, _ptr(pred0).value,
-                           int(n_pairs), int(max_n0), int(max_n1), float(thres_reprojected), float(thres_angdiff),
-                           float(min_overlap_ratio))
-    out = N.LtrLineGtOutput(_ptr(assign).value, int(assign_stride), _ptr(n_gt).value, _ptr(tfpn).value)
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_line_gt(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_line_gt")
+    specs = (("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32), ("cu0", cu0, torch.int32),
+             ("cu1", cu1, torch.int32), ("homography", homography, torch.float64),
+             ("homography_inv", homography_inv, torch.float64), ("n_gt", n_gt, torch.int32),
+             ("assign", assign, torch.float32), ("pred0", pred0, torch.int32), ("tfpn", tfpn, torch.int32),
+             ("proj0", proj0, torch.float32), ("proj1", proj1, torch.float32))
+    for nm, t, _ in specs:
+        if t is not None:
+            _req_cuda(t, nm)
+    _check_tensors("line_gt", dev, specs)
+    inp = _struct(N.LtrLineGtInput, segs0=segs0, segs1=segs1, cu0=cu0, cu1=cu1, homography=homography,
+                  homography_inv=homography_inv, proj0=proj0, proj1=proj1, pred0=pred0, n_pairs=int(n_pairs),
+                  max_n0=int(max_n0), max_n1=int(max_n1), thres_reprojected=float(thres_reprojected),
+                  thres_angdiff=float(thres_angdiff), min_overlap_ratio=float(min_overlap_ratio))
+    out = _struct(N.LtrLineGtOutput, assign=assign, assign_stride=int(assign_stride), n_gt=n_gt, tfpn=tfpn)
+    _call("ltr_line_gt", dev, C.byref(inp), C.byref(out))
 
 
 def triplet_loss(desc0, desc1, layout, n_pairs, *, assign, assign_stride, pos, neg, state, loss, hardest_pos,
@@ -334,24 +375,19 @@ def triplet_loss(desc0, desc1, layout, n_pairs, *, assign, assign_stride, pos, n
     _req_cuda(desc0, "desc0")
     _req_cuda(desc1, "desc1")
     dev = desc0.device
-    for nm, t, dt in (("desc0", desc0, torch.float32), ("desc1", desc1, torch.float32), ("assign", assign, torch.float32),
-                      ("cu0", cu0, torch.int32), ("cu1", cu1, torch.int32), ("pred0", pred0, torch.int32),
-                      ("group_off", group_off, torch.int32), ("pos", pos, torch.float32), ("neg", neg, torch.float32),
-                      ("state", state, torch.int32), ("loss", loss, torch.float32), ("hardest_pos", hardest_pos, torch.float32),
-                      ("hardest_neg", hardest_neg, torch.float32), ("n_valid", n_valid, torch.int32), ("tfpn", tfpn, torch.int32)):
-        if t is None:
-            continue
-        if t.dtype != dt or not t.is_contiguous() or t.device != dev:
-            raise N.LtrError(f"triplet_loss: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    _check_tensors("triplet_loss", dev, (
+        ("desc0", desc0, torch.float32), ("desc1", desc1, torch.float32), ("assign", assign, torch.float32),
+        ("cu0", cu0, torch.int32), ("cu1", cu1, torch.int32), ("pred0", pred0, torch.int32),
+        ("group_off", group_off, torch.int32), ("pos", pos, torch.float32), ("neg", neg, torch.float32),
+        ("state", state, torch.int32), ("loss", loss, torch.float32), ("hardest_pos", hardest_pos, torch.float32),
+        ("hardest_neg", hardest_neg, torch.float32), ("n_valid", n_valid, torch.int32), ("tfpn", tfpn, torch.int32)))
     inp = _struct(N.LtrTripletInput, desc0=desc0, desc1=desc1, layout=int(layout), d=256, n_pairs=int(n_pairs), n0=int(n0),
                   n1=int(n1), cu0=cu0, cu1=cu1, max_n0=int(max_n0), max_n1=int(max_n1), assign=assign,
                   assign_stride=int(assign_stride), assign_ld=int(assign_ld), match_thr=float(match_thr),
                   unmatch_thr=float(unmatch_thr), pred0=pred0, n_groups=int(n_groups), group_off=group_off)
     out = _struct(N.LtrTripletOutput, pos=pos, neg=neg, state=state, loss=loss, hardest_pos=hardest_pos,
                   hardest_neg=hardest_neg, n_valid=n_valid, tfpn=tfpn)
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_triplet_loss(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_triplet_loss")
+    _call("ltr_triplet_loss", dev, C.byref(inp), C.byref(out))
 
 
 def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, segs0, segs1, seg_off0,
@@ -364,20 +400,16 @@ def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu
     workspace."""
     _req_cuda(H, "H")
     dev = H.device
-    for nm, t, dt in (("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
-                      ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32),
-                      ("matches_p", matches_p, torch.int32), ("cu_p", cu_p, torch.int32), ("segs0", segs0, torch.float32),
-                      ("segs1", segs1, torch.float32), ("seg_off0", seg_off0, torch.int32),
-                      ("seg_off1", seg_off1, torch.int32), ("n_segs1", n_segs1, torch.int32),
-                      ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("H", H, torch.float64),
-                      ("valid", valid, torch.uint8), ("inliers_p", inliers_p, torch.uint8),
-                      ("inliers_l", inliers_l, torch.uint8), ("n_inliers_p", n_inliers_p, torch.int32),
-                      ("n_inliers_l", n_inliers_l, torch.int32), ("hypothesis", hypothesis, torch.int32),
-                      ("hypothesis_inliers", hypothesis_inliers, torch.int32), ("key", key, torch.int64)):
-        if t is None:
-            continue
-        if t.dtype != dt or not t.is_contiguous() or t.device != dev:
-            raise N.LtrError(f"homography: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    _check_tensors("homography", dev, (
+        ("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
+        ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32), ("matches_p", matches_p, torch.int32),
+        ("cu_p", cu_p, torch.int32), ("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32),
+        ("seg_off0", seg_off0, torch.int32), ("seg_off1", seg_off1, torch.int32), ("n_segs1", n_segs1, torch.int32),
+        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("H", H, torch.float64),
+        ("valid", valid, torch.uint8), ("inliers_p", inliers_p, torch.uint8), ("inliers_l", inliers_l, torch.uint8),
+        ("n_inliers_p", n_inliers_p, torch.int32), ("n_inliers_l", n_inliers_l, torch.int32),
+        ("hypothesis", hypothesis, torch.int32), ("hypothesis_inliers", hypothesis_inliers, torch.int32),
+        ("key", key, torch.int64)))
     inp = _struct(N.LtrHomographyInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
                   matches_p=matches_p, cu_p=cu_p, segs0=segs0, segs1=segs1, seg_off0=seg_off0, seg_off1=seg_off1,
                   n_segs1=n_segs1, matches_l=matches_l, cu_l=cu_l, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
@@ -386,9 +418,7 @@ def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu
     out = _struct(N.LtrHomographyOutput, H=H, valid=valid, inliers_p=inliers_p, inliers_l=inliers_l,
                   n_inliers_p=n_inliers_p, n_inliers_l=n_inliers_l, hypothesis=hypothesis,
                   hypothesis_inliers=hypothesis_inliers, key=key)
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_homography(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_homography")
+    _call("ltr_homography", dev, C.byref(inp), C.byref(out))
 
 
 def essential(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, K0, K1, E, R, t, valid,
@@ -400,27 +430,21 @@ def essential(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_
     workspace."""
     _req_cuda(E, "E")
     dev = E.device
-    for nm, tt, dt in (("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
-                       ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32),
-                       ("matches_p", matches_p, torch.int32), ("cu_p", cu_p, torch.int32), ("K0", K0, torch.float64),
-                       ("K1", K1, torch.float64), ("E", E, torch.float64), ("R", R, torch.float64),
-                       ("t", t, torch.float64), ("valid", valid, torch.uint8), ("inliers_p", inliers_p, torch.uint8),
-                       ("n_inliers", n_inliers, torch.int32), ("n_cheirality", n_cheirality, torch.int32),
-                       ("hypothesis", hypothesis, torch.int32), ("hypothesis_inliers", hypothesis_inliers, torch.int32),
-                       ("key", key, torch.int64)):
-        if tt is None:
-            continue
-        if tt.dtype != dt or not tt.is_contiguous() or tt.device != dev:
-            raise N.LtrError(f"essential: '{nm}' must be a contiguous {dt} tensor on {dev}")
+    _check_tensors("essential", dev, (
+        ("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
+        ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32), ("matches_p", matches_p, torch.int32),
+        ("cu_p", cu_p, torch.int32), ("K0", K0, torch.float64), ("K1", K1, torch.float64), ("E", E, torch.float64),
+        ("R", R, torch.float64), ("t", t, torch.float64), ("valid", valid, torch.uint8),
+        ("inliers_p", inliers_p, torch.uint8), ("n_inliers", n_inliers, torch.int32),
+        ("n_cheirality", n_cheirality, torch.int32), ("hypothesis", hypothesis, torch.int32),
+        ("hypothesis_inliers", hypothesis_inliers, torch.int32), ("key", key, torch.int64)))
     inp = _struct(N.LtrEssentialInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
                   matches_p=matches_p, cu_p=cu_p, K0=K0, K1=K1, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
                   thresh=float(thresh), dist_thresh=float(dist_thresh), n_hypotheses=int(n_hypotheses),
                   seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
     out = _struct(N.LtrEssentialOutput, E=E, R=R, t=t, valid=valid, inliers_p=inliers_p, n_inliers=n_inliers,
                   n_cheirality=n_cheirality, hypothesis=hypothesis, hypothesis_inliers=hypothesis_inliers, key=key)
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_essential(C.byref(inp), C.byref(out), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_essential")
+    _call("ltr_essential", dev, C.byref(inp), C.byref(out))
 
 
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
@@ -431,20 +455,15 @@ def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, wa
         raise N.LtrError(f"warp_pairs: gray must be [N,h,w] and colour [N,h,w,C], got {list(gray.shape)} and "
                          f"{list(colour.shape)}")
     P = len(src_index_host)
-    for nm, t, dt, shape in (("gray", gray, torch.uint8, None), ("colour", colour, torch.uint8, None),
-                             ("src_index", src_index, torch.int32, (P,)), ("inv_maps", inv_maps, torch.float64, (P, 9)),
-                             ("warped", warped, torch.uint8, (P, *gray.shape[1:])),
-                             ("mask", mask, torch.uint8, (P, *gray.shape[1:]))):
-        if t.dtype != dt or not t.is_contiguous() or t.device != dev or (shape is not None and tuple(t.shape) != shape):
-            raise N.LtrError(f"warp_pairs: '{nm}' must be a contiguous {dt} tensor on {dev}"
-                             + (f" of shape {list(shape)}" if shape is not None else ""))
+    _check_tensors("warp_pairs", dev, (("gray", gray, torch.uint8), ("colour", colour, torch.uint8),
+                                       ("src_index", src_index, torch.int32, (P,)),
+                                       ("inv_maps", inv_maps, torch.float64, (P, 9)),
+                                       ("warped", warped, torch.uint8, (P, *gray.shape[1:])),
+                                       ("mask", mask, torch.uint8, (P, *gray.shape[1:]))))
     n, h, w = (int(s) for s in gray.shape)
     idx = np.ascontiguousarray(src_index_host, dtype=np.int32)
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_warp_pairs(_ptr(gray), _ptr(colour), n, h, w, int(colour.shape[3]),
-                                     idx.ctypes.data_as(N.c_int32_p), _ptr(src_index), _ptr(inv_maps), P, _ptr(warped),
-                                     _ptr(mask), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_warp_pairs")
+    _call("ltr_warp_pairs", dev, _ptr(gray), _ptr(colour), n, h, w, int(colour.shape[3]),
+          idx.ctypes.data_as(N.c_int32_p), _ptr(src_index), _ptr(inv_maps), P, _ptr(warped), _ptr(mask))
 
 
 def photometric(src, dst, params_host: np.ndarray, params, ellipses, taps, workspace):
@@ -459,19 +478,13 @@ def photometric(src, dst, params_host: np.ndarray, params, ellipses, taps, works
     if ph.ndim != 2 or ph.shape[0] != n:
         raise N.LtrError(f"photometric: params must be [{n}, {N.PHOTOMETRIC_PARAMS}], got {list(ph.shape)}")
     E = int(ellipses.shape[1]) if ellipses.dim() == 3 else -1
-    for nm, t, dt, shape in (("src", src, torch.uint8, None), ("dst", dst, torch.uint8, (n, h, w)),
-                             ("params", params, torch.float64, tuple(ph.shape)),
-                             ("ellipses", ellipses, torch.int32, (n, E, 5)),
-                             ("taps", taps, torch.float32, (n, N.PHOTOMETRIC_MAX_KSIZE)),
-                             ("workspace", workspace, torch.uint8, None)):
-        if t.dtype != dt or not t.is_contiguous() or t.device != dev or (shape is not None and tuple(t.shape) != shape):
-            raise N.LtrError(f"photometric: '{nm}' must be a contiguous {dt} tensor on {dev}"
-                             + (f" of shape {list(shape)}" if shape is not None else ""))
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_photometric(_ptr(src), _ptr(dst), n, h, w, ph.ctypes.data_as(C.c_void_p), _ptr(params),
-                                      int(ph.shape[1]), _ptr(ellipses), E, _ptr(taps), _ptr(workspace),
-                                      int(workspace.numel()), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_photometric")
+    _check_tensors("photometric", dev, (("src", src, torch.uint8), ("dst", dst, torch.uint8, (n, h, w)),
+                                        ("params", params, torch.float64, tuple(ph.shape)),
+                                        ("ellipses", ellipses, torch.int32, (n, E, 5)),
+                                        ("taps", taps, torch.float32, (n, N.PHOTOMETRIC_MAX_KSIZE)),
+                                        ("workspace", workspace, torch.uint8)))
+    _call("ltr_photometric", dev, _ptr(src), _ptr(dst), n, h, w, ph.ctypes.data_as(C.c_void_p), _ptr(params),
+          int(ph.shape[1]), _ptr(ellipses), E, _ptr(taps), _ptr(workspace), int(workspace.numel()))
 
 
 def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
@@ -489,11 +502,8 @@ def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     }
     if P == 0 or n0 == 0:
         return out
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_match_distmat(_ptr(dist), P, n0, n1, 0, float(nn_thresh), int(bool(mutual)),
-                                        _ptr(out["matches0"]), _ptr(out["scores0"]), _ptr(out["nn1"]),
-                                        _ptr(out["counts"]), dev.index, _stream_ptr(dev))
-    N.check(rc, "ltr_match_distmat")
+    _call("ltr_match_distmat", dev, _ptr(dist), P, n0, n1, 0, float(nn_thresh), int(bool(mutual)),
+          _ptr(out["matches0"]), _ptr(out["scores0"]), _ptr(out["nn1"]), _ptr(out["counts"]))
     return out
 
 
@@ -507,10 +517,7 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias=None, res=None, act=0) -> torc
     y = torch.empty((M, Nn), dtype=torch.float32, device=x.device)
     bias = _f32c(bias) if bias is not None else None
     res = _f32c(res) if res is not None else None
-    with torch.cuda.device(x.device):
-        rc = N.load().ltr_linear(_ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), Nn, _ptr(y), Nn, M, Nn, K, int(act),
-                                 x.device.index, _stream_ptr(x.device))
-    N.check(rc, "ltr_linear")
+    _call("ltr_linear", x.device, _ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), Nn, _ptr(y), Nn, M, Nn, K, int(act))
     return y
 
 
@@ -525,10 +532,8 @@ def linear_img(x: torch.Tensor, w: torch.Tensor, bias=None, res=None, act=0, bn_
     y2 = torch.empty((M, Nn), dtype=torch.float32, device=x.device)
     bias = _f32c(bias) if bias is not None else None
     res = _f32c(res) if res is not None else None
-    with torch.cuda.device(x.device):
-        rc = N.load().ltr_linear_img(_ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), Nn, _ptr(y), Nn, _ptr(y2), M, Nn, K,
-                                     int(act), int(bn_hint), x.device.index, _stream_ptr(x.device))
-    N.check(rc, "ltr_linear_img")
+    _call("ltr_linear_img", x.device, _ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), Nn, _ptr(y), Nn, _ptr(y2), M, Nn, K,
+          int(act), int(bn_hint))
     return y, y2
 
 
@@ -545,9 +550,6 @@ def linear_img_norm(x: torch.Tensor, w: torch.Tensor, bias=None, res=None, norm=
     y2 = torch.empty((M, 256), dtype=torch.float32, device=x.device)
     f = lambda t: _f32c(t) if t is not None else None
     bias, res, gamma, beta, add = map(f, (bias, res, gamma, beta, add))
-    with torch.cuda.device(x.device):
-        rc = N.load().ltr_linear_img_norm(_ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), 256, int(norm), float(eps), _ptr(gamma),
-                                          _ptr(beta), _ptr(add), 256, _ptr(y), 256, _ptr(y2), M, K, x.device.index,
-                                          _stream_ptr(x.device))
-    N.check(rc, "ltr_linear_img_norm")
+    _call("ltr_linear_img_norm", x.device, _ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), 256, int(norm), float(eps),
+          _ptr(gamma), _ptr(beta), _ptr(add), 256, _ptr(y), 256, _ptr(y2), M, K)
     return y, y2

@@ -138,11 +138,8 @@ def merge_sublines(dist_sub: torch.Tensor, sub_off0: torch.Tensor, sub_off1: tor
     cuk1 = torch.tensor([0, K1], dtype=torch.int32, device=dev)
     out = torch.empty((K0, K1), dtype=torch.float32, device=dev)
     p = lambda t: C.c_void_p(t.data_ptr())
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_merge_sublines(p(dist_sub), 0, 1, p(cuk0), p(cuk1), p(sub_off0.int().contiguous()),
-                                         p(sub_off1.int().contiguous()), K0, K1, p(out), 0, dev.index,
-                                         C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    N.check(rc, "ltr_merge_sublines")
+    _ops._call("ltr_merge_sublines", dev, p(dist_sub), 0, 1, p(cuk0), p(cuk1), p(sub_off0.int().contiguous()),
+               p(sub_off1.int().contiguous()), K0, K1, p(out), 0)
     return out
 
 
@@ -427,27 +424,6 @@ class PairEngine:
                            out["dist_key"], out["stride"], d0 if keep_desc else None, d1 if keep_desc else None)
 
     # ------------------------------------------------------------------ image-level front-end
-    def _stage(self, arrays: dict) -> dict:
-        """One pinned staging buffer, one non-blocking H2D copy: -> device views of the host arrays.  The buffer
-        is held (with an event behind the copy) until the copy has finished, so it is never reused early."""
-        self._staging = [(b, e) for b, e in getattr(self, "_staging", []) if not e.query()]
-        layout, total = {}, 0
-        for k, a in arrays.items():
-            a = np.ascontiguousarray(a)
-            total = (total + 15) // 16 * 16
-            layout[k] = (total, a)
-            total += a.nbytes
-        host = torch.empty(max(total, 16), dtype=torch.uint8, pin_memory=True)
-        hv = host.numpy()
-        for o, a in layout.values():
-            hv[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
-        dev = host.to(self.device, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream(self.device))
-        self._staging.append((host, ev))
-        tdt = {np.dtype(np.float64): torch.float64, np.dtype(np.float32): torch.float32, np.dtype(np.int32): torch.int32}
-        return {k: dev[o:o + a.nbytes].view(tdt[a.dtype]).view(a.shape) for k, (o, a) in layout.items()}
-
     def _image_specs(self, images, auto_min_length):
         specs = [(im["klines"], tuple(im["image_shape"]), im.get("valid_mask")) for im in images]
         return specs, [LP.tokenizer_config(self.model.config, sh, auto_min_length) for _, sh, _ in specs]
@@ -477,10 +453,7 @@ class PairEngine:
                                       1 if int(torch.__version__[2]) > 2 else 0, tab,
                                       cu.ctypes.data_as(N.c_int32_p))
         p = lambda t: C.c_void_p(t.data_ptr())
-        with torch.cuda.device(self.device):
-            rc = N.load().ltr_tokenize_batch(C.byref(inp), *[p(t) for t in out], self.device.index,
-                                             C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
-        N.check(rc, "ltr_tokenize_batch")
+        _ops._call("ltr_tokenize_batch", self.device, C.byref(inp), *[p(t) for t in out])
         batch = LineBatch(slines, resp, ang, pnt, desc, score, cu, host.sub0 if host.split else None,
                           host.cuk if host.split else None)
         batch._dev_cache[("cu_lines", str(self.device))] = dv["cu_lines"]
@@ -506,7 +479,7 @@ class PairEngine:
     def tokenize_prepared(self, host: "LP.TokenizerBatch", images: Sequence[dict]) -> LineBatch:
         """`tokenize_images` for a batch already prepared on the host (`line_process.prepare_tokenizer_batch`,
         whose per-image settings may differ except for max_tokens); `images` supply the SuperPoint maps."""
-        return self._tokenize(host, images, self._stage(self._tok_arrays(host)))
+        return self._tokenize(host, images, _ops.stage(self._tok_arrays(host), self.device))
 
     def match_images(self, images0: Sequence[dict], images1: Sequence[dict], line_thresh: Optional[float] = None,
                      point_thresh: float = 0.7, want_scores: bool = False, auto_min_length: bool = True) -> ImagePairMatches:
@@ -537,7 +510,7 @@ class PairEngine:
         arrays.update(cu0=i32(cu[:P + 1]), cu1=i32(cu[P:] - R0), p_cu0=i32(cup[:P + 1]), p_cu1=i32(cup[P:] - cup[P]))
         if host.split:
             arrays.update(cuk0=i32(cuk[:P + 1]), cuk1=i32(cuk[P:] - K0), sub_off0=i32(so[:K0 + 1]), sub_off1=i32(so[K0:] - R0))
-        dv = self._stage(arrays)
+        dv = _ops.stage(arrays, self.device)
         batch = self._tokenize(host, images, dv)
         mx = lambda a: int(np.diff(a).max(initial=0))
         i32d = dict(dtype=torch.int32, device=self.device)
@@ -582,7 +555,7 @@ class PairEngine:
         to_l, to_p = _ops.tile_offsets(cu), _ops.tile_offsets(cup)
         arrays = self._tok_arrays(host)
         arrays.update(cuk=i32(host.cuk), tile_off_l=to_l, cu_points=cup, tile_off_p=to_p)
-        dv = self._stage(arrays)
+        dv = _ops.stage(arrays, self.device)
         batch = self._tokenize(host, images, dv)
         rows = self.encode(batch)
         tiles_l = _ops.image_tiles(rows, N.LAYOUT_ROWS, cu, dv["cu_lines"], dv["tile_off_l"], int(to_l[-1]))
@@ -621,7 +594,8 @@ class PairEngine:
         merge = bool((n0 != k0).any() or (n1 != k1).any())
         pref = lambda c: np.concatenate([[0], np.cumsum(c)]).astype(np.int32)
         ol0, ol1, op0, op1 = pref(k0), pref(k1), pref(q0), pref(q1)
-        dv = self._stage({"img0": pr[:, 0].copy(), "img1": pr[:, 1].copy(), "ol0": ol0, "ol1": ol1, "op0": op0, "op1": op1})
+        dv = _ops.stage({"img0": pr[:, 0].copy(), "img1": pr[:, 1].copy(), "ol0": ol0, "ol1": ol1, "op0": op0,
+                         "op1": op1}, self.device)
         i32d = dict(dtype=torch.int32, device=self.device)
         f32d = dict(dtype=torch.float32, device=self.device)
         alloc = lambda n, kw: torch.empty(max(int(n), 1), **kw)[:int(n)]   # never a null pointer
@@ -800,11 +774,8 @@ class PeerCounts:
         e = self._collected
         self._collected += 1
         out = torch.empty(self.world * self.n_pairs, dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            rc = N.load().ltr_gather_wait(C.c_void_p(self.buf.data_ptr()), self.world, self.n_pairs, e % N.GATHER_SLOTS,
-                                          e // N.GATHER_SLOTS + 1, C.c_void_p(out.data_ptr()), self.device.index,
-                                          C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream))
-        N.check(rc, "ltr_gather_wait")
+        _ops._call("ltr_gather_wait", self.device, C.c_void_p(self.buf.data_ptr()), self.world, self.n_pairs,
+                   e % N.GATHER_SLOTS, e // N.GATHER_SLOTS + 1, C.c_void_p(out.data_ptr()))
         return out
 
     def collect_async(self) -> "PeerCountsHandle":

@@ -34,7 +34,7 @@ import torch
 
 from . import _native as N
 from . import _ops
-from .eval_homography import LineGroundTruth, _stage, precision_recall_from_counts
+from .eval_homography import LineGroundTruth, precision_recall_from_counts
 
 MATCH_THR_F32 = float(np.float32(0.3))   # criteria.py:63 `overlap_gt > 0.3` on a float32 tensor
 FAR = np.float32(10000.0)                # criteria.py:95 max_dist
@@ -191,7 +191,7 @@ def _prepare(desc0, desc1, assign, cu0, cu1, layout, assign_ld, groups):
     host = {"groups": g}
     if c0 is not None:
         host.update(cu0=c0, cu1=c1)
-    dv = _stage(host, d0.device) if (c0 is not None or groups is not None) else {}
+    dv = _ops.stage(host, d0.device) if (c0 is not None or groups is not None) else {}
     return dict(d0=d0, d1=d1, P=P, u0=u0, u1=u1, n0=n0, n1=n1, mx0=mx0, mx1=mx1, assign=a, stride=stride, ld=ld, groups=g,
                 cu0=dv.get("cu0"), cu1=dv.get("cu1"), group_off=dv.get("groups") if groups is not None else None)
 

@@ -156,31 +156,6 @@ def get_precision_recall(score, score_gt):
 
 
 # ------------------------------------------------------------------ batched on the GPU
-_staging = []   # (pinned host buffer, event behind its copy) until the copy has finished
-
-
-def _stage(arrays: dict, device) -> dict:
-    """One pinned staging buffer, one non-blocking H2D copy: -> device views of the host arrays."""
-    global _staging
-    _staging = [(b, e) for b, e in _staging if not e.query()]
-    layout, total = {}, 0
-    for k, a in arrays.items():
-        a = np.ascontiguousarray(a)
-        total = (total + 15) // 16 * 16
-        layout[k] = (total, a)
-        total += a.nbytes
-    host = torch.empty(max(total, 16), dtype=torch.uint8, pin_memory=True)
-    hv = host.numpy()
-    for o, a in layout.values():
-        hv[o:o + a.nbytes] = a.reshape(-1).view(np.uint8)
-    dev = host.to(device, non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record(torch.cuda.current_stream(device))
-    _staging.append((host, ev))
-    tdt = {np.dtype(np.float64): torch.float64, np.dtype(np.float32): torch.float32, np.dtype(np.int32): torch.int32}
-    return {k: dev[o:o + a.nbytes].view(tdt[a.dtype]).view(a.shape) for k, (o, a) in layout.items()}
-
-
 def _check_offsets(cu, n_pairs, n_segs, name) -> np.ndarray:
     cu = np.asarray(cu)
     if cu.ndim != 1 or len(cu) != n_pairs + 1 or not np.issubdtype(cu.dtype, np.integer):
@@ -264,7 +239,7 @@ def homography_ground_truth(segs0, segs1, cu0, cu1, homographies, pred0=None, wa
     if device is None:
         device = next((t.device for t in devs.values()), None) or _ops.current_cuda_device()
     device = torch.device(device)
-    dv = _stage({**host, "cu0": c0, "cu1": c1, "H": hs, "Hinv": np.ascontiguousarray(hinv)}, device)
+    dv = _ops.stage({**host, "cu0": c0, "cu1": c1, "H": hs, "Hinv": np.ascontiguousarray(hinv)}, device)
     dv.update(devs)
     n0, n1 = np.diff(c0), np.diff(c1)
     mx0, mx1 = int(n0.max(initial=0)), int(n1.max(initial=0))

@@ -54,7 +54,6 @@ import torch
 
 from . import _native as N
 from . import _ops
-from .eval_homography import _stage
 
 FLT_EPSILON = float(np.finfo(np.float32).eps)
 MAX_DRAWS = 64          # draws per hypothesis before it is rejected (HG_MAX_DRAWS)
@@ -349,8 +348,8 @@ def estimate_homographies(res, thresh=3.0, n_hypotheses=2048, seed=0, use_lines=
     cat_np = lambda parts: np.concatenate(parts) if parts else np.zeros((0, 4), dtype=np.float32)
     cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
     i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
-    dv = _stage({"segs0": cat_np(s0), "segs1": cat_np(s1), "seg_off0": soff0, "seg_off1": soff1, "n_segs1": sn1,
-                 "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1, "cu_p": i32(op), "cu_l": i32(ol)}, dev)
+    dv = _ops.stage({"segs0": cat_np(s0), "segs1": cat_np(s1), "seg_off0": soff0, "seg_off1": soff1, "n_segs1": sn1,
+                      "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1, "cu_p": i32(op), "cu_l": i32(ol)}, dev)
     u8, i32d = dict(dtype=torch.uint8, device=dev), dict(dtype=torch.int32, device=dev)
     out = HomographyResult(torch.empty((P, 3, 3), dtype=torch.float64, device=dev), torch.empty(P, **u8),
                            torch.empty(res.matches_l.shape[0], **u8), torch.empty(res.matches_p.shape[0], **u8),
@@ -850,8 +849,8 @@ def estimate_poses(res, K0, K1, thresh=1.0, n_hypotheses=1024, seed=0, dist_thre
     if not np.array_equal(pn0, np.diff(op)):
         raise N.LtrError("estimate_poses: side-0 keypoints and the match offsets disagree")
     cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
-    dv = _stage({"K0": k0, "K1": k1, "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1,
-                 "cu_p": np.ascontiguousarray(op, dtype=np.int32)}, dev)
+    dv = _ops.stage({"K0": k0, "K1": k1, "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1,
+                      "cu_p": np.ascontiguousarray(op, dtype=np.int32)}, dev)
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
     out = PoseResult(torch.empty((P, 3, 3), **f64), torch.empty((P, 3, 3), **f64), torch.empty((P, 3), **f64),
                      torch.empty(P, dtype=torch.uint8, device=dev),

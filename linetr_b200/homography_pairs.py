@@ -31,7 +31,6 @@ import torch
 
 from . import _native as N
 from . import _ops
-from .eval_homography import _stage
 
 INT_MIN, INT_MAX = -2147483648.0, 2147483647.0
 MAX_SIDE = 32767      # OpenCV's remap keeps source cells in int16
@@ -253,7 +252,7 @@ def warp_pairs(gray, colour, src_index, H):
         raise N.LtrError(f"warp_pairs: src_index must lie in [0, {gray.shape[0]})")
     P, dev = len(idx), gray.device
     idx = np.ascontiguousarray(idx, dtype=np.int32)
-    dv = _stage({"src_index": idx, "inv_maps": _inverse_maps(H, P)}, dev)
+    dv = _ops.stage({"src_index": idx, "inv_maps": _inverse_maps(H, P)}, dev)
     warped = torch.empty((P, *gray.shape[1:]), dtype=torch.uint8, device=dev)
     mask = torch.empty_like(warped)
     _ops.warp_pairs(gray.contiguous(), colour.contiguous(), idx, dv["src_index"], dv["inv_maps"], warped, mask)

@@ -343,7 +343,7 @@ def line_tokenizer_gpu(klines, token_distance, max_tokens, pred_superpoint, imag
     version (float64 arithmetic in numpy's operation order, rounded once to fp32); sampled descriptors
     agree to fp32 rounding.  Key lines must lie in the image and run left to right (see `keyline_geometry`)."""
     import ctypes as C
-    from . import _native as N
+    from . import _native as N, _ops
     dense = pred_superpoint["dense_descriptor"]
     if not dense.is_cuda:
         raise N.LtrError("line_tokenizer_gpu needs the SuperPoint outputs on a CUDA device")
@@ -375,10 +375,8 @@ def line_tokenizer_gpu(klines, token_distance, max_tokens, pred_superpoint, imag
                              dense_c.data_ptr(), c, hc, wc, score_map.data_ptr(), score_map.shape[-2], score_map.shape[-1],
                              1 if int(torch.__version__[2]) > 2 else 0)
     p = lambda t: C.c_void_p(t.data_ptr())
-    with torch.cuda.device(dev):
-        rc = N.load().ltr_tokenize(C.byref(inp), p(slines), p(tokens), p(masks), p(responses), p(ang), p(desc), p(scores),
-                                   dev.index, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-    N.check(rc, "ltr_tokenize")
+    _ops._call("ltr_tokenize", dev, C.byref(inp), p(slines), p(tokens), p(masks), p(responses), p(ang), p(desc),
+               p(scores))
     adj = np.zeros((K, S), dtype=np.float32)
     w = (1.0 / n_sub).astype(np.float64)
     adj[sub2line, np.arange(S)] = w[sub2line]

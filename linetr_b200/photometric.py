@@ -522,8 +522,6 @@ def photometric_augment(gray, record):
     """The builder's photometric augmentation of every image of gray (uint8 CUDA [N, h, w]) with the draws of
     `record` (sample_photometric(N, (h, w), ...)), in one `ltr_photometric` call.  Returns a new uint8 CUDA tensor
     [N, h, w], equal to photometric_host(gray, record); the call never waits for the device."""
-    from .eval_homography import _stage
-
     if not isinstance(gray, torch.Tensor):
         raise N.LtrError("photometric_augment: 'gray' must be a torch tensor")
     _ops._req_cuda(gray, "gray")
@@ -537,8 +535,8 @@ def photometric_augment(gray, record):
     _check_ellipses(ell, h, w)
     ph = params_array(record)
     dev = gray.device
-    dv = _stage({"params": ph, "ellipses": ell.reshape(n, -1, 5),
-                 "taps": np.ascontiguousarray(record["taps"], dtype=np.float32)}, dev)
+    dv = _ops.stage({"params": ph, "ellipses": ell.reshape(n, -1, 5),
+                      "taps": np.ascontiguousarray(record["taps"], dtype=np.float32)}, dev)
     out = torch.empty_like(gray)
     ws = torch.empty(N.photometric_workspace_bytes(n, h, w), dtype=torch.uint8, device=dev)
     _ops.photometric(gray.contiguous(), out, ph, dv["params"], dv["ellipses"], dv["taps"], ws)

@@ -3,9 +3,6 @@ between two encoded sets (`ltr_image_tiles` + `ltr_match_indexed`), against `mat
 `ltr_match` on descriptors gathered per pair."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -16,7 +13,6 @@ from linetr_b200.match_io import dense_to_indices
 from tests import helpers as H
 from tests.test_image_pairs import DIST_TOL, _glue, _model, _reference_superpoint
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DEV = torch.device("cuda", 0)
 
 
@@ -73,43 +69,6 @@ def test_make_image_set_deterministic():
         assert [vars(l) for l in x["klines"]] == [vars(l) for l in y["klines"]]
     assert not torch.equal(a[0]["descriptors"], c[0]["descriptors"])
     assert not torch.equal(a[0]["descriptors"], a[1]["descriptors"])   # the views differ from each other
-
-
-def _header_struct(name):
-    hdr = open(os.path.join(ROOT, "include", "linetr_b200.h")).read()
-    body = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + ";", hdr).group(1)
-    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-    fields = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if not decl:
-            continue
-        m = re.match(r"(const\s+)?(\w+)\s*(\**)\s*(.*)", decl)
-        for nm in m.group(4).split(","):
-            fields.append((nm.strip().lstrip("*"), "*" in m.group(3) + nm))
-    return fields
-
-
-def test_pair_index_layout_matches_header():
-    fields = _header_struct("LtrPairIndex")
-    assert [f for f, _ in fields] == [f for f, _ in N.LtrPairIndex._fields_]
-    for (f, is_ptr), (g, ct) in zip(fields, N.LtrPairIndex._fields_):
-        assert ctypes.sizeof(ct) == (8 if is_ptr else 4), f
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no host C compiler for the offsetof check")
-    import tempfile
-    with tempfile.TemporaryDirectory() as td:
-        src, exe = os.path.join(td, "off.c"), os.path.join(td, "off")
-        with open(src, "w") as f:
-            f.write('#include <stdio.h>\n#include <stddef.h>\n#include "linetr_b200.h"\nint main(void){\n')
-            for nm, _ in fields:
-                f.write(f'  printf("%zu\\n", offsetof(LtrPairIndex, {nm}));\n')
-            f.write('  printf("%zu\\n", sizeof(LtrPairIndex));\n  return 0;\n}\n')
-        subprocess.check_call([cc, "-I", os.path.join(ROOT, "include"), "-o", exe, src])
-        got = [int(x) for x in subprocess.check_output([exe]).split()]
-    want = [getattr(N.LtrPairIndex, nm).offset for nm, _ in fields] + [ctypes.sizeof(N.LtrPairIndex)]
-    assert got == want
 
 
 # ------------------------------------------------------------------ GPU helpers

@@ -3,10 +3,6 @@ reference's find_line_matches / calculate_line_overlaps / Evaluate_PR outputs in
 (tests/golden/make_line_gt_golden.py) and against the host restatement."""
 import ctypes
 import os
-import re
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -132,42 +128,6 @@ def test_argument_validation():
     assert call(assign=16, stride=15) == -1          # stride < max_n0 * max_n1
     assert call() == -1                               # null n_gt and inputs
     assert call(n_pairs=0) == 0
-
-
-def _header_struct(name):
-    hdr = open(os.path.join(ROOT, "include", "linetr_b200.h")).read()
-    body = re.search(r"typedef struct \{([^{}]*)\}\s*" + name + ";", hdr).group(1)
-    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
-    fields = []
-    for decl in body.split(";"):
-        decl = decl.strip()
-        if decl:
-            m = re.match(r"(const\s+)?(\w+)\s*(\**)\s*(.*)", decl)
-            fields += [(nm.strip().lstrip("*"), m.group(2), "*" in m.group(3) + nm) for nm in m.group(4).split(",")]
-    return fields
-
-
-@pytest.mark.parametrize("name", ["LtrLineGtInput", "LtrLineGtOutput"])
-def test_struct_layout_matches_header(name):
-    st = getattr(N, name)
-    fields = _header_struct(name)
-    assert [f for f, _, _ in fields] == [f for f, _ in st._fields_]
-    size = {"int32_t": 4, "float": 4, "int64_t": 8, "double": 8}
-    for (f, ty, is_ptr), (g, ct) in zip(fields, st._fields_):
-        assert ctypes.sizeof(ct) == (8 if is_ptr else size[ty]), f
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no host C compiler for the offsetof check")
-    with tempfile.TemporaryDirectory() as td:
-        src, exe = os.path.join(td, "off.c"), os.path.join(td, "off")
-        with open(src, "w") as f:
-            f.write('#include <stdio.h>\n#include <stddef.h>\n#include "linetr_b200.h"\nint main(void){\n')
-            for nm, _, _ in fields:
-                f.write(f'  printf("%zu\\n", offsetof({name}, {nm}));\n')
-            f.write(f'  printf("%zu\\n", sizeof({name}));\n  return 0;\n}}\n')
-        subprocess.check_call([cc, "-I", os.path.join(ROOT, "include"), "-o", exe, src])
-        got = [int(x) for x in subprocess.check_output([exe]).split()]
-    assert got == [getattr(st, nm).offset for nm, _, _ in fields] + [ctypes.sizeof(st)]
 
 
 # ------------------------------------------------------------------ GPU

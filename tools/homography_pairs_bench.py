@@ -25,7 +25,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from linetr_b200 import _ops, synthetic as syn   # noqa: E402
-from linetr_b200.eval_homography import _stage   # noqa: E402
+from linetr_b200._ops import stage   # noqa: E402
 from linetr_b200.homography_pairs import sample_homographies, warp_pairs   # noqa: E402
 
 W, H = 640, 480
@@ -92,7 +92,7 @@ def main():
     for P in args.pairs:
         Hs, _ = sample_homographies(P, (H, W), rng)
         src = np.arange(P, dtype=np.int32) % args.images
-        dv = _stage({"src_index": src, "inv_maps": np.linalg.inv(Hs).reshape(P, 9)}, dev)
+        dv = stage({"src_index": src, "inv_maps": np.linalg.inv(Hs).reshape(P, 9)}, dev)
         warped = torch.empty((P, H, W), dtype=torch.uint8, device=dev)
         mask = torch.empty_like(warped)
         kern = time_windows(lambda: _ops.warp_pairs(g, c, src, dv["src_index"], dv["inv_maps"], warped, mask),

@@ -25,7 +25,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from linetr_b200 import _native as N, _ops, synthetic as syn   # noqa: E402
 from linetr_b200 import photometric as PH   # noqa: E402
-from linetr_b200.eval_homography import _stage   # noqa: E402
+from linetr_b200._ops import stage   # noqa: E402
 
 W, H = 640, 480
 
@@ -88,7 +88,7 @@ def main():
         g, c = (torch.from_numpy(a).to(dev) for a in (gray, colour))
         rec = PH.sample_photometric(n, (H, W), np.random.default_rng(n), **PH.HOMOGRAPHY_PHOTOMETRIC)
         ph = PH.params_array(rec)
-        dv = _stage({"params": ph, "ellipses": rec["ellipses"], "taps": rec["taps"]}, dev)
+        dv = stage({"params": ph, "ellipses": rec["ellipses"], "taps": rec["taps"]}, dev)
         out = torch.empty_like(g)
         ws = torch.empty(N.photometric_workspace_bytes(n, H, W), dtype=torch.uint8, device=dev)
         kern = time_windows(lambda: _ops.photometric(g, out, ph, dv["params"], dv["ellipses"], dv["taps"], ws),
