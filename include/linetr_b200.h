@@ -51,7 +51,7 @@
 extern "C" {
 #endif
 
-#define LTR_ABI_VERSION 3
+#define LTR_ABI_VERSION 4
 
 #define LTR_OK 0
 #define LTR_E_INVALID (-1)   /* bad argument / missing checkpoint tensor / shape mismatch */
@@ -292,43 +292,21 @@ int ltr_merge_sublines(const float* dist_sub, int64_t stride_sub, int32_t n_pair
                        int64_t stride_key, int32_t device, void* stream);
 
 /* GPU line tokenizer - the step that feeds ltr_encode (reference line_tokenizer +
- * sample_descriptors, models/line_process.py:86-196).  The host supplies per key line (device
- * arrays): start point, end point before and after the in-place clip to (W-0.6, H-0.6) [K,2]
- * float64, detector length [K] float64, angle code [K,2] float32, n_tok = ceil(length /
- * token_distance) [K], first subline index sub0 [K+1] and the key line of every subline [S].
- * Outputs (device, fp32) in the tokenizer's layout: sublines [S,2,2], pnt [S,T,2], mask
- * [S,T+1,1], resp [S,1], angle [S,2], desc [S,T,256] (bilinear grid_sample of dense_desc
- * [256,desc_h,desc_w] + L2 normalisation), score [S,T,1] (dense_score [score_h,score_w] at the
- * rounded token position). */
-typedef struct {
-  const double* sp;
-  const double* ep;
-  const double* ep_clipped;
-  const double* length;
-  const float* angle;
-  const int32_t* n_tok;
-  const int32_t* sub0;
-  const int32_t* sub2line;
-  int32_t n_keylines, n_sublines, n_tokens;
-  double token_distance;
-  const float* dense_desc;
-  int32_t desc_channels, desc_h, desc_w;
-  const float* dense_score;
-  int32_t score_h, score_w;
-  int32_t align_corners;   /* the reference keys this on the torch version (line_process.py:93) */
-} LtrTokenizeInput;
-
-int ltr_tokenize(const LtrTokenizeInput* in, float* sublines, float* pnt, float* mask, float* resp,
-                 float* angle, float* desc, float* score, int32_t device, void* stream);
-
-/* ltr_tokenize over many images in one call (the same kernels; a batch equals per-image calls bit
- * for bit).  Key lines of all images are concatenated, image by image: sub0 [K+1] and sub2line [S]
- * use global subline numbering and line_image [K] (device) names the image of every key line.
+ * sample_descriptors, models/line_process.py:86-196), over many images in one call.  The host supplies
+ * per key line (device arrays): start point, end point before and after the in-place clip to
+ * (W-0.6, H-0.6) [K,2] float64, detector length [K] float64, angle code [K,2] float32, n_tok =
+ * ceil(length / token_distance) [K], first subline index sub0 [K+1], the key line of every subline [S]
+ * and the image of every key line line_image [K].  Key lines of all images are concatenated, image by
+ * image, and sub0 / sub2line use global subline numbering.
  * images [n_images] and cu_sublines [n_images+1] are HOST arrays read during the call only: image i
  * owns output rows [cu_sublines[i], cu_sublines[i+1]) of the packed outputs (the LineBatch layout)
  * and is tokenised with its own token_distance and sampled from its own maps, whose sizes may
- * differ between images.  An image without key lines is an empty range; its maps may be NULL (and
- * so may the outputs of a batch without any key line).
+ * differ between images; a batch equals per-image calls bit for bit.  An image without key lines is
+ * an empty range; its maps may be NULL (and so may the outputs of a batch without any key line).
+ * Outputs (device, fp32) in the tokenizer's layout: sublines [S,2,2], pnt [S,T,2], mask [S,T+1,1],
+ * resp [S,1], angle [S,2], desc [S,T,256] (bilinear grid_sample of the image's dense_desc
+ * [256,desc_h,desc_w] + L2 normalisation), score [S,T,1] (its dense_score [score_h,score_w] at the
+ * rounded token position).
  * n_tokens must be 1..128 (the encoder's limit) and desc_channels 256.  Nothing synchronises. */
 typedef struct {
   const float* dense_desc;     /* device [256, desc_h, desc_w] */
@@ -662,15 +640,9 @@ int ltr_photometric(const uint8_t* in, uint8_t* out, int32_t n_images, int32_t h
                     int32_t max_ellipses, const float* taps, void* workspace, int64_t workspace_bytes, int32_t device,
                     void* stream);
 
-/* Generic row-major linear layer Y = act(X W^T + b) (+ R) on the library's GEMM engine;
- * exported so the engine can be unit-tested in isolation.  act: 0 none, 1 relu, 2 gelu(erf). */
-int ltr_linear(const float* x, int32_t ldx, const float* w, const float* bias, const float* res,
-               int32_t ldr, float* y, int32_t ldy, int32_t m, int32_t n, int32_t k, int32_t act,
-               int32_t device, void* stream);
-
-/* The same on the tensor-core engine (gemm_img.cuh: persistent, TMA-fed split-bf16 tile images,
- * wgmma): x is converted to a
- * split-bf16 tile image, the GEMM writes fp32 rows into `y` (may be NULL) and - when
+/* Row-major linear layer Y = act(X W^T + b) (+ R) on the tensor-core engine (gemm_img.cuh:
+ * persistent, TMA-fed split-bf16 tile images, wgmma), exported so the engine can be unit-tested in
+ * isolation; act: 0 none, 1 relu, 2 gelu(erf).  x is converted to a split-bf16 tile image, the GEMM writes fp32 rows into `y` (may be NULL) and - when
  * `y_from_image` is given - also the split-bf16 image of the result, which is converted back
  * to fp32 rows [m, n] there so that both outputs can be checked.  n % 64 == 0, k % 64 == 0;
  * bn_hint: 0 (auto), 64, 128 or 256.  Synchronous; unit-test hook only. */

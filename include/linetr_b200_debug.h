@@ -21,13 +21,11 @@ float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t o
  * -1 on failure. */
 float ltr_gemm_chain_bench(int32_t m, int32_t chained, int32_t iters, int32_t device);
 
-/* clock64 stamps of CTA 0 recorded by the last ltr_gemm_bench call (64 slots, 16 per tile:
- * 0 MMA acc_empty ok, 1 first operands landed, 2 MMAs issued, 3 epilogue acc_full ok, 4 first
- * accumulator complete, 5 epilogue done, 6 producer slot free). */
-const unsigned long long* ltr_gemm_trace(void);
-
 /* Kernels instrumented with LTR_DBG_STAMP store clock64 stamps of their first CTA into a
- * 128-slot device array while tracing is armed. */
+ * 128-slot device array while tracing is armed.  gemm_img_kernel (as ltr_gemm_bench launches it)
+ * stamps the first 4 tiles of CTA 0, 16 slots per tile, slot 16 * i + j: j = 0 consumers start tile i,
+ * 2 its MMAs are done, 5 its epilogue is done; j = 6 the producer got a ring slot for its i-th k-block
+ * (counted across tiles).  gemm_chain_kernel's layout is CHAIN_TRACE_* in csrc/gemm_img.cuh. */
 void ltr_debug_trace_arm(int32_t on);
 int ltr_debug_trace_read(unsigned long long* out128);
 

@@ -20,7 +20,7 @@ LAYOUT_CHANNEL_FIRST = 1
 
 # slots of ltr_debug_encode_images, in order
 ENCODE_IMAGES = ("z", "ctx", "l128", "l256", "lpos", "y1i", "g", "xm", "hm", "qkv", "yf")
-ABI_VERSION = 3
+ABI_VERSION = 4
 PHOTOMETRIC_PARAMS = 28      # LTR_PHOTOMETRIC_PARAMS
 PHOTOMETRIC_MAX_KSIZE = 149  # LTR_PHOTOMETRIC_MAX_KSIZE
 
@@ -85,15 +85,6 @@ class LtrMatchOutput(C.Structure):
     _fields_ = [("matches0", C.c_void_p), ("scores0", C.c_void_p), ("nn1", C.c_void_p),
                 ("counts", C.c_void_p), ("dist_key", C.c_void_p), ("dist_sub", C.c_void_p),
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64), ("gather", C.POINTER(LtrPeerGather))]
-
-
-class LtrTokenizeInput(C.Structure):
-    _fields_ = [("sp", C.c_void_p), ("ep", C.c_void_p), ("ep_clipped", C.c_void_p), ("length", C.c_void_p),
-                ("angle", C.c_void_p), ("n_tok", C.c_void_p), ("sub0", C.c_void_p), ("sub2line", C.c_void_p),
-                ("n_keylines", C.c_int32), ("n_sublines", C.c_int32), ("n_tokens", C.c_int32),
-                ("token_distance", C.c_double), ("dense_desc", C.c_void_p), ("desc_channels", C.c_int32),
-                ("desc_h", C.c_int32), ("desc_w", C.c_int32), ("dense_score", C.c_void_p), ("score_h", C.c_int32),
-                ("score_w", C.c_int32), ("align_corners", C.c_int32)]
 
 
 class LtrTokenizeImage(C.Structure):
@@ -181,7 +172,6 @@ PROTOTYPES = {
     "ltr_match_indexed": (C.c_int, [_ptr(LtrMatchInput), _ptr(LtrPairIndex), _ptr(LtrMatchOutput), _I32, _P]),
     "ltr_match_distmat": (C.c_int, [_P, _I32, _I32, _I32, _I64, _F32, _I32, _P, _P, _P, _P, _I32, _P]),
     "ltr_merge_sublines": (C.c_int, [_P, _I64, _I32, _P, _P, _P, _P, _I32, _I32, _P, _I64, _I32, _P]),
-    "ltr_tokenize": (C.c_int, [_ptr(LtrTokenizeInput)] + [_P] * 7 + [_I32, _P]),
     "ltr_tokenize_batch": (C.c_int, [_ptr(LtrTokenizeBatchInput)] + [_P] * 7 + [_I32, _P]),
     "ltr_line_gt": (C.c_int, [_ptr(LtrLineGtInput), _ptr(LtrLineGtOutput), _I32, _P]),
     "ltr_triplet_loss": (C.c_int, [_ptr(LtrTripletInput), _ptr(LtrTripletOutput), _I32, _P]),
@@ -189,7 +179,6 @@ PROTOTYPES = {
     "ltr_essential": (C.c_int, [_ptr(LtrEssentialInput), _ptr(LtrEssentialOutput), _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
-    "ltr_linear": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P] + [_I32] * 6 + [_P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),
     "ltr_linear_img_norm": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _I32, _F32, _P, _P, _P, _I32, _P, _I32, _P, _I32,
                                       _I32, _I32, _P]),
@@ -202,7 +191,6 @@ PROTOTYPES = {
 DEBUG_PROTOTYPES = {
     "ltr_gemm_bench": (_F32, [_I32] * 7),
     "ltr_gemm_chain_bench": (_F32, [_I32] * 4),
-    "ltr_gemm_trace": (_ptr(C.c_uint64), []),
     "ltr_debug_trace_arm": (None, [_I32]),
     "ltr_debug_trace_read": (C.c_int, [_ptr(C.c_uint64)]),
     "ltr_debug_linear_img_res": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P] + [_I32] * 6 + [_P]),

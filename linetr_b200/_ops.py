@@ -340,6 +340,36 @@ def match_indexed(desc0, desc1, layout, n_pairs, nn_thresh, *, cu0, cu1, max_n0,
                     total_out1=total_out1))
 
 
+def tokenize(dv: dict, maps, cu_lines: np.ndarray, max_tokens: int, dev) -> list:
+    """ltr_tokenize_batch of the key lines staged in `dv` (device arrays sp, ep, epc, length, angle, n_tok, sub0,
+    sub2line, line_image of `line_process.keyline_geometry`, image by image) -> sublines [S,2,2], pnt [S,T,2],
+    mask [S,T+1,1], resp [S,1], angle [S,2], desc [S,T,256], score [S,T,1].  maps: per image (dense descriptor
+    map, dense score map, token_distance), or None for an image without key lines; cu_lines [n+1]: host subline
+    offsets."""
+    S, T, n = int(cu_lines[-1]), int(max_tokens), len(maps)
+    f32 = dict(dtype=torch.float32, device=dev)
+    out = [torch.empty(shape, **f32) for shape in ((S, 2, 2), (S, T, 2), (S, T + 1, 1), (S, 1), (S, 2), (S, T, 256), (S, T, 1))]
+    keep, tab = [], (N.LtrTokenizeImage * max(n, 1))()
+    for i, m in enumerate(maps):
+        if m is None:
+            continue
+        dense, smap = m[0].float().contiguous(), m[1].float().contiguous()
+        if dense.shape[-3] != 256:
+            raise N.LtrError(f"ltr_tokenize_batch: image {i} has {dense.shape[-3]} descriptor channels, 256 required")
+        keep += [dense, smap]
+        tab[i] = N.LtrTokenizeImage(dense.data_ptr(), smap.data_ptr(), float(m[2]), dense.shape[-2], dense.shape[-1],
+                                    smap.shape[-2], smap.shape[-1])
+    cu = np.ascontiguousarray(cu_lines, dtype=np.int32)
+    ptr = lambda k: dv[k].data_ptr()   # noqa: E731
+    # the reference keys grid_sample's align_corners on the third character of torch.__version__ (line_process.py:93)
+    align = 1 if int(torch.__version__[2]) > 2 else 0
+    inp = N.LtrTokenizeBatchInput(ptr("sp"), ptr("ep"), ptr("epc"), ptr("length"), ptr("angle"), ptr("n_tok"),
+                                  ptr("sub0"), ptr("sub2line"), ptr("line_image"), n, len(dv["n_tok"]), S, T, 256, align,
+                                  tab, cu.ctypes.data_as(N.c_int32_p))
+    _call("ltr_tokenize_batch", dev, C.byref(inp), *[_ptr(t) for t in out])
+    return out
+
+
 def line_gt(segs0, segs1, n_pairs, *, cu0, cu1, max_n0, max_n1, homography, homography_inv, n_gt, assign=None,
             assign_stride=0, pred0=None, tfpn=None, proj0=None, proj1=None, thres_reprojected=3.0, thres_angdiff=2.0,
             min_overlap_ratio=0.3):
@@ -505,20 +535,6 @@ def match_distmat(dist: torch.Tensor, nn_thresh: float, mutual=True):
     _call("ltr_match_distmat", dev, _ptr(dist), P, n0, n1, 0, float(nn_thresh), int(bool(mutual)),
           _ptr(out["matches0"]), _ptr(out["scores0"]), _ptr(out["nn1"]), _ptr(out["counts"]))
     return out
-
-
-def linear(x: torch.Tensor, w: torch.Tensor, bias=None, res=None, act=0) -> torch.Tensor:
-    """ltr_linear: act(x @ w.T + bias) (+ res) on the fp32 CUDA-core engine (unit-test hook and
-    numerics yardstick of the tensor-core engine)."""
-    _req_cuda(x, "x")
-    x, w = _f32c(x), _f32c(w)
-    M, K = x.shape
-    Nn = w.shape[0]
-    y = torch.empty((M, Nn), dtype=torch.float32, device=x.device)
-    bias = _f32c(bias) if bias is not None else None
-    res = _f32c(res) if res is not None else None
-    _call("ltr_linear", x.device, _ptr(x), K, _ptr(w), _ptr(bias), _ptr(res), Nn, _ptr(y), Nn, M, Nn, K, int(act))
-    return y
 
 
 def linear_img(x: torch.Tensor, w: torch.Tensor, bias=None, res=None, act=0, bn_hint=0):

@@ -19,7 +19,6 @@
 // tile's k-blocks while the epilogue runs.
 #pragma once
 #include "common.cuh"
-#include "linear_f32.cuh"
 #include "tc_weight.cuh"
 #include "act_img.cuh"
 #include "ptx_sm90.cuh"
@@ -44,12 +43,10 @@ struct GemmImgArgs {
   const float* nadd; int ldadd;   // fp32 rows added AFTER the normalisation or nullptr
   ActImg NaddImg; int nadd_kb0;   // OR: the same addend read from a split-bf16 image
   int m_tiles, n_blks;
-  unsigned long long* trace;   // debug: clock64 stamps of CTA 0 (nullptr = off)
 };
 
+enum Act : int { ACT_NONE = 0, ACT_RELU = 1, ACT_GELU = 2 };
 enum { NORM_NONE = 0, NORM_LAYER = 1, NORM_L2 = 2 };
-
-#define LTR_STAMP(slot) do { if (p.trace && blockIdx.x == 0) p.trace[slot] = clock64(); } while (0)
 
 // GELU(x) = x * Phi(x) with the erf form the reference uses (F.gelu default, models/line_attention.py:92).
 // erfc(u) = P(t) exp(-u^2), t = 1 / (1 + 0.3275911 u)  (Abramowitz-Stegun 7.1.26, |error| <= 1.5e-7 - the
@@ -580,6 +577,8 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int nk = p.W.K / 64;
   const int n_tiles = p.m_tiles * p.n_blks;
+  // Only CTA 0 reads the debug-trace switch, once: a global load at every stamp sits on each CTA's critical path.
+  const bool trace = blockIdx.x == 0 && g_dbg_on;
   pdl_launch_dependents();
 
   if (tid == 0) {
@@ -606,7 +605,7 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
           const int s = it % Cfg::STAGES;
           const uint32_t ph = (it / Cfg::STAGES) & 1;
           ptx::mbar_wait(&empty[s], ph ^ 1);
-          if (it < 4) LTR_STAMP(it * 16 + 6);
+          if (trace && it < 4) LTR_DBG_STAMP(it * 16 + 6);
           uint8_t* st = smem + s * Cfg::STAGE;
           const size_t aoff = ((size_t)mt * p.A.kblocks + p.a_kb0 + nb * p.a_kb_nb + kb) * IMG_TILE_ELEMS;
           const size_t woff = ((size_t)kb * (p.W.N / 8) + (size_t)nb * (BN / 8)) * 1024;
@@ -639,7 +638,7 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
       if constexpr (FRAG) epi_frag_prefetch(p, mt, nb * (BN / 64), frow, lane, stgb, &res_bar[warp]);
-      if (tl < 4 && tid == 0) LTR_STAMP(tl * 16 + 0);
+      if (trace && tl < 4 && tid == 0) LTR_DBG_STAMP(tl * 16 + 0);
       for (int kb = 0; kb < nk; ++kb, ++it) {
         const int s = it % Cfg::STAGES;
         ptx::mbar_wait(&full[s], (it / Cfg::STAGES) & 1);
@@ -656,7 +655,7 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
       ptx::wg_wait<0>();
       ptx::wg_fence_regs(d);
       if (lane == 0) ptx::mbar_arrive(&empty[(it - 1) % Cfg::STAGES]);
-      if (tl < 4 && tid == 0) LTR_STAMP(tl * 16 + 2);
+      if (trace && tl < 4 && tid == 0) LTR_DBG_STAMP(tl * 16 + 2);
       if constexpr (FRAG) {
         epi_frag_tile<BN>(p, d, mt, nb, frow, lane, stgb, &res_bar[warp], (tl * (BN / 64)) & 1, nullptr);
       } else {
@@ -668,7 +667,7 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
         }
         epi_plain_tile<BN>(p, d, mt, nb, q, half, lane, row_a, stg_all, stg, stgb);
       }
-      if (tl < 4 && tid == 0) LTR_STAMP(tl * 16 + 5);
+      if (trace && tl < 4 && tid == 0) LTR_DBG_STAMP(tl * 16 + 5);
     }
     if constexpr (FRAG) {
       if (lane == 0) ptx::bulk_wait<0>();   // the staging stays allocated, and the writes done, until the stores complete
@@ -936,7 +935,6 @@ inline int launch_gemm_chain(const GemmImgArgs* ops, int n_ops, cudaStream_t s) 
     c.op[i] = ops[i];
     c.op[i].m_tiles = c.m_tiles;
     c.op[i].n_blks = ops[i].W.N / 256;
-    c.op[i].trace = nullptr;
   }
   using Cfg = GemmImgCfg<256>;
   LTR_CUDA_TRY(ensure_dynamic_smem(gemm_chain_kernel, Cfg::SMEM));

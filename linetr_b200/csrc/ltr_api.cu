@@ -11,7 +11,6 @@
 
 #include "common.cuh"
 #include "encoder_kernels.cuh"
-#include "linear_f32.cuh"
 #include "tc_weight.cuh"
 #include "gemm_img.cuh"
 #include "token_fused.cuh"
@@ -65,10 +64,15 @@ struct Lin {
   TcWeight tw;
 };
 
-struct MlpTail {  // positional encoder: narrow head + the two wide layers (128->256 relu, 256->256)
-  SmallMlpWeights head;
-  Lin l2;           // 32 -> 64 as a tensor-core image with K zero-padded to one 64-wide k-block (token stage)
+// Positional encoders (IN -> 32 -> 64 -> 128 -> 256 -> 256), each packed in the form its kernels read.
+struct WordPosEnc {   // token_fused_kernel: first layer on CUDA cores, the other four as tensor-core images
+  const float *w1 = nullptr, *b1 = nullptr;
+  Lin l2;             // 32 -> 64 with K zero-padded to one 64-wide k-block; l2.b is the kernel's fp32 b2
   Lin l3, l4, l5;
+};
+struct LinePosEnc {   // small_mlp_kernel (narrow head), then two image GEMMs (128 -> 256 relu, 256 -> 256)
+  SmallMlpWeights head;
+  Lin l4, l5;
 };
 
 struct SigLayer {
@@ -85,7 +89,8 @@ struct LtrModel {
   float* arena = nullptr;
   uint16_t* tc_arena = nullptr;
   size_t arena_floats = 0;
-  ltr::MlpTail wpe{}, lpe{};
+  ltr::WordPosEnc wpe{};
+  ltr::LinePosEnc lpe{};
   float *U = nullptr, *s_cls = nullptr, *cls = nullptr;
   ltr::Lin wv, wfc, w1, w2, wf;  // wv: 4 heads of [64,256]; wfc bias includes the CLS residual
   float *ln1g = nullptr, *ln1b = nullptr, *ln2g = nullptr, *ln2b = nullptr;
@@ -107,27 +112,23 @@ struct HostPack {
     for (size_t i = 0; i < v.size(); ++i) buf[off + i] = (float)v[i];
     return off;
   }
-  // wide layer [N,K]: bias + tensor-core image.  `groups` > 1 packs row groups of N/groups
-  // rows as independent matrices.
-  LinOff add_lin(const std::vector<double>& W, const std::vector<double>& b, int N, int K, int groups = 1) {
+  // wide layer [N,K]: bias + tensor-core image
+  LinOff add_lin(const std::vector<double>& W, const std::vector<double>& b, int N, int K) {
     LinOff o{add(b), 0, N, K};
     size_t off = (tc.size() + 511) / 512 * 512;  // 1024-byte alignment
     tc.resize(off + 2 * (size_t)N * K);
-    const int gn = N / groups;
-    for (int g = 0; g < groups; ++g)
-      pack_tc_weight(W.data() + (size_t)g * gn * K, gn, K, tc.data() + off + (size_t)g * gn * K,
-                     tc.data() + off + (size_t)N * K + (size_t)g * gn * K);
+    pack_tc_weight(W.data(), N, K, tc.data() + off, tc.data() + off + (size_t)N * K);
     o.tc = off;
     return o;
   }
 };
 
-static Lin bind_lin(const LinOff& o, float* fbase, uint16_t* tbase, int groups = 1) {
+static Lin bind_lin(const LinOff& o, float* fbase, uint16_t* tbase) {
   Lin l;
   l.b = fbase + o.b;
   l.tw.hi = reinterpret_cast<const __nv_bfloat16*>(tbase + o.tc);
   l.tw.lo = reinterpret_cast<const __nv_bfloat16*>(tbase + o.tc + (size_t)o.N * o.K);
-  l.tw.N = o.N / groups;
+  l.tw.N = o.N;
   l.tw.K = o.K;
   return l;
 }
@@ -167,43 +168,46 @@ static bool fold_layer(const TensorMap& tm, const std::string& conv, const std::
   return true;
 }
 
-struct MlpOffsets { size_t w[3], b[3]; LinOff l2, l3, l4, l5; };
-
-static bool pack_pos_encoder(const TensorMap& tm, const std::string& prefix, int in, HostPack& hp, MlpOffsets& off,
-                             std::string& err) {
+// The five layers of a positional encoder, eval-BatchNorm folded into the first four.
+static bool fold_pos_encoder(const TensorMap& tm, const std::string& prefix, int in, std::vector<double> (&W)[5],
+                             std::vector<double> (&b)[5], std::string& err) {
   const int ch[6] = {in, 32, 64, 128, 256, 256};
   for (int l = 0; l < 5; ++l) {
     std::string conv = prefix + "." + std::to_string(3 * l);
     std::string bn = (l < 4) ? prefix + "." + std::to_string(3 * l + 1) : std::string();
-    std::vector<double> W, b;
-    if (!fold_layer(tm, conv, bn, ch[l + 1], ch[l], W, b, err)) return false;
-    if (l < 3) {
-      off.w[l] = hp.add(W);
-      off.b[l] = hp.add(b);
-      if (l == 1) {   // 32 -> 64 also as a tensor-core image, K padded to 64
-        std::vector<double> Wp((size_t)64 * 64, 0.0);
-        for (int o = 0; o < 64; ++o)
-          for (int i = 0; i < 32; ++i) Wp[(size_t)o * 64 + i] = W[(size_t)o * 32 + i];
-        off.l2 = hp.add_lin(Wp, b, 64, 64);
-      }
-      if (l == 2) off.l3 = hp.add_lin(W, b, ch[l + 1], ch[l]);  // 64 -> 128 also as a tensor-core image
-    } else if (l == 3) {
-      off.l4 = hp.add_lin(W, b, ch[l + 1], ch[l]);
-    } else {
-      off.l5 = hp.add_lin(W, b, ch[l + 1], ch[l]);
-    }
+    if (!fold_layer(tm, conv, bn, ch[l + 1], ch[l], W[l], b[l], err)) return false;
   }
   return true;
 }
 
-static void bind_mlp(MlpTail& m, float* base, uint16_t* tbase, const MlpOffsets& o) {
-  m.head.w1 = base + o.w[0]; m.head.b1 = base + o.b[0];
-  m.head.w2 = base + o.w[1]; m.head.b2 = base + o.b[1];
-  m.head.w3 = base + o.w[2]; m.head.b3 = base + o.b[2];
-  m.l2 = bind_lin(o.l2, base, tbase);
-  m.l3 = bind_lin(o.l3, base, tbase);
-  m.l4 = bind_lin(o.l4, base, tbase);
-  m.l5 = bind_lin(o.l5, base, tbase);
+struct WordPosOff { size_t w1, b1; LinOff l2, l3, l4, l5; };
+struct LinePosOff { size_t w[3], b[3]; LinOff l4, l5; };
+
+static bool pack_word_pos(const TensorMap& tm, HostPack& hp, WordPosOff& o, std::string& err) {
+  std::vector<double> W[5], b[5];
+  if (!fold_pos_encoder(tm, "klenc.word_position_enc.encoder", 3, W, b, err)) return false;
+  std::vector<double> W2((size_t)64 * 64, 0.0);
+  for (int r = 0; r < 64; ++r)
+    for (int i = 0; i < 32; ++i) W2[(size_t)r * 64 + i] = W[1][(size_t)r * 32 + i];
+  o.w1 = hp.add(W[0]);
+  o.b1 = hp.add(b[0]);
+  o.l2 = hp.add_lin(W2, b[1], 64, 64);
+  o.l3 = hp.add_lin(W[2], b[2], 128, 64);
+  o.l4 = hp.add_lin(W[3], b[3], 256, 128);
+  o.l5 = hp.add_lin(W[4], b[4], 256, 256);
+  return true;
+}
+
+static bool pack_line_pos(const TensorMap& tm, HostPack& hp, LinePosOff& o, std::string& err) {
+  std::vector<double> W[5], b[5];
+  if (!fold_pos_encoder(tm, "klenc.line_position_enc.encoder", 5, W, b, err)) return false;
+  for (int l = 0; l < 3; ++l) {
+    o.w[l] = hp.add(W[l]);
+    o.b[l] = hp.add(b[l]);
+  }
+  o.l4 = hp.add_lin(W[3], b[3], 256, 128);
+  o.l5 = hp.add_lin(W[4], b[4], 256, 256);
+  return true;
 }
 
 static cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
@@ -219,7 +223,7 @@ struct EncodeWs {
   int64_t bytes;
 };
 
-static EncodeWs carve(const LtrModel* m, int n_lines, int T, char* base) {
+static EncodeWs carve(const LtrModel* m, int n_lines, char* base) {
   EncodeWs w{};
   int64_t off = 0;
   auto take = [&](int64_t bytes) {
@@ -236,7 +240,6 @@ static EncodeWs carve(const LtrModel* m, int n_lines, int T, char* base) {
     a.kblocks = K / 64;
     return a;
   };
-  (void)T;
   const int64_t R = n_lines;
   w.z = takei(R, 1024);
   w.ctx = takei(R, 256);
@@ -251,14 +254,6 @@ static EncodeWs carve(const LtrModel* m, int n_lines, int T, char* base) {
   w.yf = takef(R * 256);
   w.bytes = off;
   return w;
-}
-
-static LinearArgs lin(const float* A, int lda, const float* W, const float* b, float* C, int ldc, int M, int N, int K,
-                      int act, const float* R = nullptr, int ldr = 0) {
-  LinearArgs a{};
-  a.A = A; a.lda = lda; a.W = W; a.bias = b; a.R = R; a.ldr = ldr; a.C = C; a.ldc = ldc;
-  a.M = M; a.N = N; a.K = K; a.act = act; a.nz = 1;
-  return a;
 }
 
 // One wide layer on the tensor-core engine: A image k-blocks [a_kb0, a_kb0 + K/64) -> fp32 rows C
@@ -280,19 +275,17 @@ static int gemm(const Lin& L, const ActImg& A, int a_kb0, int M, int act, cudaSt
   return launch_gemm_img(gemm_args(L, A, a_kb0, M, act, C, ldc, O, o_kb0, R, ldr, Rimg, r_kb0, a_kb_nb), s, bn_hint);
 }
 
-template <bool TOKEN>
 static int launch_small_mlp(const SmallMlpWeights& w, const float* in0, const float* in1, const float* in2, ActImg out,
                             int rows, float width, float height, cudaStream_t s) {
   if (rows <= 0) return 0;
-  constexpr int IN = TOKEN ? 3 : 5;
-  const int smem = (int)sizeof(SmallMlpSmem<IN>);
-  LTR_CUDA_TRY(ensure_dynamic_smem(small_mlp_kernel<TOKEN>, smem));
+  const int smem = (int)sizeof(SmallMlpSmem);
+  LTR_CUDA_TRY(ensure_dynamic_smem(small_mlp_kernel, smem));
   const int groups = cdiv(rows, SM_ROWS);
   int grid = cdiv(groups, SM_WARPS);
   if (grid > 132 * 3) grid = 132 * 3;
   const float scale = fmaxf(width, height) * 0.7f;
   LaunchScope ls(KC_SMALL_MLP, s);
-  LTR_CUDA_TRY(launch_pdl(small_mlp_kernel<TOKEN>, dim3(grid), dim3(SM_WARPS * 32), (size_t)smem, s, w, in0, in1, in2, out, rows,
+  LTR_CUDA_TRY(launch_pdl(small_mlp_kernel, dim3(grid), dim3(SM_WARPS * 32), (size_t)smem, s, w, in0, in1, in2, out, rows,
                           width / 2.f, height / 2.f, scale));
   return 0;
 }
@@ -334,7 +327,7 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
   {
     TokenFusedArgs a{};
     a.pnt = in.pnt; a.score = in.score; a.desc = in.desc;
-    a.w1 = m->wpe.head.w1; a.b1 = m->wpe.head.b1; a.b2 = m->wpe.head.b2;
+    a.w1 = m->wpe.w1; a.b1 = m->wpe.b1; a.b2 = m->wpe.l2.b;
     a.W2 = m->wpe.l2.tw; a.W3 = m->wpe.l3.tw; a.W4 = m->wpe.l4.tw; a.W5 = m->wpe.l5.tw;
     a.b3 = m->wpe.l3.b; a.b4 = m->wpe.l4.b; a.b5 = m->wpe.l5.b;
     a.U = m->U; a.s_cls = m->s_cls; a.cls = m->cls;
@@ -346,8 +339,7 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
   // ---- line stage: V projection (block diagonal over heads), fc + CLS residual, LN, FFN, LN, + line pos ----
   LTR_TRY(gemm(m->wv, w.z, 0, R, ACT_NONE, s, nullptr, 0, &w.ctx, 0, nullptr, 0, nullptr, 0, 64, 4));
   // line positional encoder first (its output is added in the w_2 epilogue)
-  LTR_TRY(launch_small_mlp<false>(m->lpe.head, in.sublines, in.resp, in.angle, w.l128, R, in.image_width,
-                                  in.image_height, s));
+  LTR_TRY(launch_small_mlp(m->lpe.head, in.sublines, in.resp, in.angle, w.l128, R, in.image_width, in.image_height, s));
   LTR_TRY(gemm(m->lpe.l4, w.l128, 0, R, ACT_RELU, s, nullptr, 0, &w.l256, 0));
   LTR_TRY(gemm(m->lpe.l5, w.l256, 0, R, ACT_NONE, s, nullptr, 0, &w.lpos, 0));
   // The row-local GEMM runs fc -> w_1 -> w_2 -> qkv(0) and, per signature layer, mlp1 -> mlp2 -> qkv(l+1) (or
@@ -522,10 +514,9 @@ int ltr_create(const LtrTensor* tensors, int32_t n_tensors, const LtrConfig* cfg
   std::string err;
   HostPack hp;
   const int D = 256, DI = cfg->d_inner;
-  MlpOffsets wpe_o{}, lpe_o{};
-  if (!pack_pos_encoder(tm, "klenc.word_position_enc.encoder", 3, hp, wpe_o, err) ||
-      !pack_pos_encoder(tm, "klenc.line_position_enc.encoder", 5, hp, lpe_o, err))
-    return set_error(LTR_E_INVALID, err);
+  WordPosOff wpe_o{};
+  LinePosOff lpe_o{};
+  if (!pack_word_pos(tm, hp, wpe_o, err) || !pack_line_pos(tm, hp, lpe_o, err)) return set_error(LTR_E_INVALID, err);
 
   // ---- descriptive layer (only the last one is live) ----
   const std::string dl = "klenc.desc_layers." + std::to_string(cfg->n_desc_layers - 1);
@@ -640,8 +631,11 @@ int ltr_create(const LtrTensor* tensors, int32_t n_tensors, const LtrConfig* cfg
   }
   float* B = m->arena;
   uint16_t* TB = m->tc_arena;
-  bind_mlp(m->wpe, B, TB, wpe_o);
-  bind_mlp(m->lpe, B, TB, lpe_o);
+  m->wpe = {B + wpe_o.w1, B + wpe_o.b1, bind_lin(wpe_o.l2, B, TB), bind_lin(wpe_o.l3, B, TB), bind_lin(wpe_o.l4, B, TB),
+            bind_lin(wpe_o.l5, B, TB)};
+  m->lpe.head = {B + lpe_o.w[0], B + lpe_o.b[0], B + lpe_o.w[1], B + lpe_o.b[1], B + lpe_o.w[2], B + lpe_o.b[2]};
+  m->lpe.l4 = bind_lin(lpe_o.l4, B, TB);
+  m->lpe.l5 = bind_lin(lpe_o.l5, B, TB);
   m->U = B + oU; m->s_cls = B + oS; m->cls = B + oC;
   m->wv = bind_lin(oWv, B, TB);
   m->wfc = bind_lin(oWfc, B, TB);
@@ -667,7 +661,7 @@ void ltr_destroy(LtrModel* m) {
 int64_t ltr_encode_workspace_bytes(const LtrModel* m, int32_t n_images, int32_t n_lines, int32_t n_tokens) {
   (void)n_images;
   if (!m || n_lines < 0 || n_tokens < 1) return set_error(LTR_E_INVALID, "ltr_encode_workspace_bytes: bad argument");
-  return carve(m, n_lines, n_tokens, nullptr).bytes + 256;
+  return carve(m, n_lines, nullptr).bytes + 256;
 }
 
 int64_t ltr_desc_tiles_bytes(int32_t n_lines) {
@@ -695,7 +689,7 @@ int ltr_encode(LtrModel* m, const LtrEncodeInput* in, const LtrEncodeOutput* out
     return set_error(LTR_E_INVALID, "ltr_encode: desc_tiles must be 16-byte aligned");
   LTR_CUDA_TRY(cudaSetDevice(m->device));
   char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(workspace), 256));
-  EncodeWs w = carve(m, in->n_lines, in->n_tokens, base);
+  EncodeWs w = carve(m, in->n_lines, base);
   if (!workspace || (base - (char*)workspace) + w.bytes > workspace_bytes)
     return set_error(LTR_E_WORKSPACE, "ltr_encode: workspace too small, need " + std::to_string(w.bytes + 256));
   return encode_impl(m, *in, out->desc_cf, out->desc_rows, out->desc_tiles, w, as_stream(stream));
@@ -1061,25 +1055,6 @@ int ltr_merge_sublines(const float* dist_sub, int64_t stride_sub, int32_t n_pair
                         as_stream(stream));
 }
 
-int ltr_tokenize(const LtrTokenizeInput* in, float* sublines, float* pnt, float* mask, float* resp, float* angle,
-                 float* desc, float* score, int32_t device, void* stream) {
-  if (!in || !sublines || !pnt || !mask || !resp || !angle || !desc || !score)
-    return set_error(LTR_E_INVALID, "ltr_tokenize: null argument");
-  if (in->n_sublines <= 0 || in->n_keylines <= 0) return LTR_OK;
-  if (in->n_tokens < 1 || in->desc_channels != 256)
-    return set_error(LTR_E_UNSUPPORTED, "ltr_tokenize: n_tokens >= 1 and 256 descriptor channels required");
-  if (!in->sp || !in->ep || !in->ep_clipped || !in->length || !in->angle || !in->n_tok || !in->sub0 || !in->sub2line ||
-      !in->dense_desc || !in->dense_score)
-    return set_error(LTR_E_INVALID, "ltr_tokenize: null input array");
-  LTR_CUDA_TRY(cudaSetDevice(device));
-  TokLines L{in->sp, in->ep, in->ep_clipped, in->length, in->angle, in->n_tok, in->sub0, in->sub2line, nullptr,
-             in->n_keylines, in->n_sublines, in->n_tokens};
-  TokImages<1> I{};
-  I.im[0] = TokImage{in->dense_desc, in->dense_score, in->token_distance, in->desc_h, in->desc_w, in->score_h, in->score_w};
-  return launch_tokenize(L, I, 0, in->n_sublines, in->align_corners, sublines, pnt, mask, resp, angle, desc, score,
-                         as_stream(stream));
-}
-
 int ltr_tokenize_batch(const LtrTokenizeBatchInput* in, float* sublines, float* pnt, float* mask, float* resp,
                        float* angle, float* desc, float* score, int32_t device, void* stream) {
   if (!in) return set_error(LTR_E_INVALID, "ltr_tokenize_batch: null argument");
@@ -1106,14 +1081,18 @@ int ltr_tokenize_batch(const LtrTokenizeBatchInput* in, float* sublines, float* 
   cudaStream_t s = as_stream(stream);
   TokLines L{in->sp, in->ep, in->ep_clipped, in->length, in->angle, in->n_tok, in->sub0, in->sub2line, in->line_image,
              in->n_keylines, in->n_sublines, in->n_tokens};
+  const auto image = [](const LtrTokenizeImage& g) {
+    return TokImage{g.dense_desc, g.dense_score, g.token_distance, g.desc_h, g.desc_w, g.score_h, g.score_w};
+  };
+  if (in->n_images == 1) {   // one image: a 40-byte table, and every line is in it
+    TokImages<1> I{{image(in->images[0])}, 0};
+    return launch_tokenize(L, I, 0, in->n_sublines, in->align_corners, sublines, pnt, mask, resp, angle, desc, score, s);
+  }
   for (int i0 = 0; i0 < in->n_images; i0 += kTokImagesPerLaunch) {
     const int i1 = std::min(in->n_images, i0 + kTokImagesPerLaunch);
     TokImages<kTokImagesPerLaunch> I{};
     I.first = i0;
-    for (int i = i0; i < i1; ++i) {
-      const LtrTokenizeImage& g = in->images[i];
-      I.im[i - i0] = TokImage{g.dense_desc, g.dense_score, g.token_distance, g.desc_h, g.desc_w, g.score_h, g.score_w};
-    }
+    for (int i = i0; i < i1; ++i) I.im[i - i0] = image(in->images[i]);
     LTR_TRY(launch_tokenize(L, I, cu[i0], cu[i1], in->align_corners, sublines, pnt, mask, resp, angle, desc, score, s));
   }
   return LTR_OK;
@@ -1379,13 +1358,6 @@ int ltr_photometric(const uint8_t* in, uint8_t* out, int32_t n_images, int32_t h
   return LTR_OK;
 }
 
-int ltr_linear(const float* x, int32_t ldx, const float* w, const float* bias, const float* res, int32_t ldr, float* y,
-               int32_t ldy, int32_t m, int32_t n, int32_t k, int32_t act, int32_t device, void* stream) {
-  if (!x || !w || !y) return set_error(LTR_E_INVALID, "ltr_linear: null argument");
-  LTR_CUDA_TRY(cudaSetDevice(device));
-  return launch_linear_f32(lin(x, ldx, w, bias, y, ldy, m, n, k, act, res, ldr), as_stream(stream));
-}
-
 struct NormSpec { int norm; float eps; const float* g; const float* beta; const float* add; int ldadd; };
 
 // res_image: the residual res [m, n] (row stride ldr) is split into the output image first and read from there (Rimg);
@@ -1487,7 +1459,7 @@ int ltr_debug_encode_images(const LtrModel* m, int32_t n_lines, void* workspace,
   if (!m || n_lines < 0 || !workspace || !hi || !lo || !kblocks)
     return set_error(LTR_E_INVALID, "ltr_debug_encode_images: bad argument");
   char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<int64_t>(workspace), 256));   // as ltr_encode
-  const EncodeWs w = carve(m, n_lines, 1, base);
+  const EncodeWs w = carve(m, n_lines, base);
   const ActImg* img[10] = {&w.z, &w.ctx, &w.l128, &w.l256, &w.lpos, &w.y1i, &w.g, &w.xm, &w.hm, &w.qkv};
   for (int i = 0; i < 10; ++i) {
     hi[i] = img[i]->hi;
@@ -1499,9 +1471,6 @@ int ltr_debug_encode_images(const LtrModel* m, int32_t n_lines, void* workspace,
   kblocks[10] = 0;
   return LTR_OK;
 }
-
-static unsigned long long g_trace_host[64];
-const unsigned long long* ltr_gemm_trace(void) { return g_trace_host; }
 
 float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t out_mode, int32_t iters, int32_t device) {
   if (cudaSetDevice(device) != cudaSuccess) return -1.f;
@@ -1521,17 +1490,9 @@ float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t o
   a.W.N = n; a.W.K = k; a.M = m; a.act = 1;
   if (out_mode == 0 || out_mode == 2) { a.C = dc; a.ldc = n; }
   if (out_mode == 1 || out_mode == 2) a.O = ActImg{reinterpret_cast<__nv_bfloat16*>(dout), reinterpret_cast<__nv_bfloat16*>(dout + mpad * n), n / 64};
-  unsigned long long* dtrace = nullptr;
-  cudaMalloc(&dtrace, 64 * 8);
-  cudaMemset(dtrace, 0, 64 * 8);
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   for (int i = 0; i < 3; ++i) launch_gemm_img(a, 0, bn_hint);
-  a.trace = dtrace;
-  launch_gemm_img(a, 0, bn_hint);
-  a.trace = nullptr;
-  cudaMemcpy(g_trace_host, dtrace, 64 * 8, cudaMemcpyDeviceToHost);
-  cudaFree(dtrace);
   cudaEventRecord(e0, 0);
   for (int i = 0; i < iters; ++i) launch_gemm_img(a, 0, bn_hint);
   cudaEventRecord(e1, 0);

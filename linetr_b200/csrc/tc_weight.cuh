@@ -6,7 +6,6 @@
 #pragma once
 #include <cstring>
 #include "common.cuh"
-#include "linear_f32.cuh"
 #include "ptx_sm90.cuh"
 
 namespace ltr {

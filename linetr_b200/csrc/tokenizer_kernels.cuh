@@ -30,7 +30,7 @@ struct TokImage {
 };
 
 // The images of one launch, passed by value (__grid_constant__: indexed in place, never copied to local
-// memory).  Key line k belongs to im[line_image[k] - first]; line_image == nullptr means one image.
+// memory).  Key line k belongs to im[line_image[k] - first]; a one-image table (NI = 1) holds every line.
 template <int NI>
 struct TokImages {
   TokImage im[NI];
@@ -46,13 +46,14 @@ struct TokLines {
   const int* n_tok;       // [K]
   const int* sub0;        // [K+1] first subline of each key line (prefix sum of n_sub, over all images)
   const int* sub2line;    // [S]
-  const int* line_image;  // [K] image of each key line, or nullptr (one image)
+  const int* line_image;  // [K] image of each key line
   int K, S, T;
 };
 
 template <int NI>
 __device__ __forceinline__ const TokImage& image_of_line(const TokLines& L, const TokImages<NI>& I, int k) {
-  return I.im[L.line_image ? L.line_image[k] - I.first : 0];
+  if constexpr (NI == 1) return I.im[0];
+  else return I.im[L.line_image[k] - I.first];
 }
 
 // point at distance d from sp along the line (reference point_on_line, line_process.py:43-59), every operation

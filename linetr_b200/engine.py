@@ -430,30 +430,17 @@ class PairEngine:
 
     def _tokenize(self, host: "LP.TokenizerBatch", images: Sequence[dict], dv: dict) -> LineBatch:
         """ltr_tokenize_batch of `host` (its per-key-line arrays already staged in `dv`) -> the packed LineBatch."""
-        S, T, K, n = host.n_sublines, host.max_tokens, host.n_keylines, host.n_images
-        f32 = dict(dtype=torch.float32, device=self.device)
-        out = [torch.empty(shape, **f32) for shape in ((S, 2, 2), (S, T, 2), (S, T + 1, 1), (S, 1), (S, 2), (S, T, 256), (S, T, 1))]
-        slines, pnt, mask, resp, ang, desc, score = out
-        keep, tab = [], (N.LtrTokenizeImage * max(n, 1))()
-        for i, im in enumerate(images):
+        maps = []
+        for i, im in enumerate(images[:host.n_images]):
             if host.cu_lines[i + 1] == host.cu_lines[i]:
+                maps.append(None)
                 continue
             dense = im["dense_descriptor"]
             if not dense.is_cuda or dense.device != self.device:
                 raise N.LtrError(f"match_images: SuperPoint maps must be on {self.device} (there is no CPU fallback)")
-            dense = dense.float().contiguous()
-            smap = im["dense_score"].float().contiguous()
-            keep += [dense, smap]
-            tab[i] = N.LtrTokenizeImage(dense.data_ptr(), smap.data_ptr(), float(host.token_distance[i]),
-                                        dense.shape[-2], dense.shape[-1], smap.shape[-2], smap.shape[-1])
+            maps.append((dense, im["dense_score"], host.token_distance[i]))
         cu = np.ascontiguousarray(host.cu_lines, dtype=np.int32)
-        ptr = lambda k: dv[k].data_ptr()
-        inp = N.LtrTokenizeBatchInput(ptr("sp"), ptr("ep"), ptr("epc"), ptr("length"), ptr("angle"), ptr("n_tok"),
-                                      ptr("sub0"), ptr("sub2line"), ptr("line_image"), n, K, S, T, 256,
-                                      1 if int(torch.__version__[2]) > 2 else 0, tab,
-                                      cu.ctypes.data_as(N.c_int32_p))
-        p = lambda t: C.c_void_p(t.data_ptr())
-        _ops._call("ltr_tokenize_batch", self.device, C.byref(inp), *[p(t) for t in out])
+        slines, pnt, mask, resp, ang, desc, score = _ops.tokenize(dv, maps, cu, host.max_tokens, self.device)
         batch = LineBatch(slines, resp, ang, pnt, desc, score, cu, host.sub0 if host.split else None,
                           host.cuk if host.split else None)
         batch._dev_cache[("cu_lines", str(self.device))] = dv["cu_lines"]

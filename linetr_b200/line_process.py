@@ -2,7 +2,7 @@
 
 `get_dist_matrix` is on the hot path (reference models/line_process.py:198-201) and runs on
 the GPU through `ltr_match`.  The tokeniser (reference models/line_process.py:6-196; SURVEY.md
-§8f row 1, the first "next" row) exists twice: `line_tokenizer_gpu` (CUDA, `ltr_tokenize`; used by
+§8f row 1, the first "next" row) exists twice: `line_tokenizer_gpu` (CUDA, `ltr_tokenize_batch`; used by
 `LineTransformer.preprocess` whenever the SuperPoint outputs live on a CUDA device) and
 `line_tokenizer`, numpy/PyTorch glue that reproduces the reference bit for bit - including its
 quirks (in-place end-point clipping, `index[:max_keylines]` dropping the shortest line when
@@ -338,45 +338,29 @@ def line_tokenizer(klines, token_distance, max_tokens, pred_superpoint, image_sh
 
 
 def line_tokenizer_gpu(klines, token_distance, max_tokens, pred_superpoint, image_shape):
-    """`line_tokenizer` on the GPU (ltr_tokenize): same inputs, same output dict, no Python loops.
-    Token positions, sublines, masks, responses, scores and the adjacency are bit-identical to the CPU
-    version (float64 arithmetic in numpy's operation order, rounded once to fp32); sampled descriptors
-    agree to fp32 rounding.  Key lines must lie in the image and run left to right (see `keyline_geometry`)."""
-    import ctypes as C
+    """`line_tokenizer` on the GPU (`ltr_tokenize_batch` with one image): same inputs, same output dict, no Python
+    loops.  Token positions, sublines, masks, responses, scores and the adjacency are bit-identical to the CPU
+    version (float64 arithmetic in numpy's operation order, rounded once to fp32); sampled descriptors agree to fp32
+    rounding.  Key lines must lie in the image and run left to right (see `keyline_geometry`), and max_tokens must
+    be 1..128 (the encoder's limit)."""
     from . import _native as N, _ops
     dense = pred_superpoint["dense_descriptor"]
     if not dense.is_cuda:
         raise N.LtrError("line_tokenizer_gpu needs the SuperPoint outputs on a CUDA device")
     dev = dense.device
     height, width = image_shape
-    T = int(max_tokens)
     K = len(klines["klines"])
     length = np.ascontiguousarray(klines["length_klines"], dtype=np.float64)
-    g = keyline_geometry(klines["klines"], length, token_distance, T, width, height)
-    n_tok, n_sub, sub0, sub2line, sp, ep, epc = (g[k] for k in ("n_tok", "n_sub", "sub0", "sub2line", "sp", "ep", "epc"))
-    S = int(sub0[-1])
-    angles = np.ascontiguousarray(klines["angles"], dtype=np.float32)
-    up = lambda a, dt: torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
-    d_sp, d_ep, d_epc, d_len = up(sp, np.float64), up(ep, np.float64), up(epc, np.float64), up(length, np.float64)
-    d_ang, d_ntok, d_sub0, d_s2l = up(angles, np.float32), up(n_tok, np.int32), up(sub0, np.int32), up(sub2line, np.int32)
-    f32 = dict(dtype=torch.float32, device=dev)
-    slines = torch.empty((S, 2, 2), **f32)
-    tokens = torch.empty((S, T, 2), **f32)
-    masks = torch.empty((S, T + 1, 1), **f32)
-    responses = torch.empty((S, 1), **f32)
-    ang = torch.empty((S, 2), **f32)
-    desc = torch.empty((S, T, 256), **f32)
-    scores = torch.empty((S, T, 1), **f32)
-    dense_c = dense.float().contiguous()
-    score_map = pred_superpoint["dense_score"].float().contiguous()
-    b, c, hc, wc = dense_c.shape
-    inp = N.LtrTokenizeInput(d_sp.data_ptr(), d_ep.data_ptr(), d_epc.data_ptr(), d_len.data_ptr(), d_ang.data_ptr(),
-                             d_ntok.data_ptr(), d_sub0.data_ptr(), d_s2l.data_ptr(), K, S, T, float(token_distance),
-                             dense_c.data_ptr(), c, hc, wc, score_map.data_ptr(), score_map.shape[-2], score_map.shape[-1],
-                             1 if int(torch.__version__[2]) > 2 else 0)
-    p = lambda t: C.c_void_p(t.data_ptr())
-    _ops._call("ltr_tokenize", dev, C.byref(inp), p(slines), p(tokens), p(masks), p(responses), p(ang), p(desc),
-               p(scores))
+    g = keyline_geometry(klines["klines"], length, token_distance, max_tokens, width, height)
+    n_sub, sub2line = g["n_sub"], g["sub2line"]
+    S = int(g["sub0"][-1])
+    i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)   # noqa: E731
+    dv = _ops.stage({"sp": g["sp"], "ep": g["ep"], "epc": g["epc"], "length": length,
+                     "angle": np.ascontiguousarray(klines["angles"], dtype=np.float32).reshape(K, 2),
+                     "n_tok": i32(g["n_tok"]), "sub0": i32(g["sub0"]), "sub2line": i32(sub2line),
+                     "line_image": np.zeros(K, dtype=np.int32)}, dev)
+    maps = [(dense, pred_superpoint["dense_score"], token_distance)]
+    slines, tokens, masks, responses, ang, desc, scores = _ops.tokenize(dv, maps, np.array([0, S]), max_tokens, dev)
     adj = np.zeros((K, S), dtype=np.float32)
     w = (1.0 / n_sub).astype(np.float64)
     adj[sub2line, np.arange(S)] = w[sub2line]

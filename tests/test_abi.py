@@ -137,13 +137,13 @@ def test_prototype_matches_header(name):
         assert _ctype_kind(t) == k, f"{name}: argument {i} is {_ctype_kind(t)} in the binding, {k} in the header"
 
 
-def test_call_sites_take_device_and_stream():
+def test_routed_entries_take_device_and_stream():
     """_ops._call appends (device, stream) to its arguments, and ctypes passes surplus arguments without complaint, so
     every entry routed through it must end its prototype with them."""
     pkg = os.path.join(ROOT, "linetr_b200")
     src = "".join(open(os.path.join(pkg, f)).read() for f in sorted(os.listdir(pkg)) if f.endswith(".py"))
     routed = set(re.findall(r"\b_(?:call|match)\(\s*\"(ltr_\w+)\"", src))
-    assert {"ltr_match", "ltr_tokenize", "ltr_gather_wait"} <= routed
+    assert {"ltr_match", "ltr_tokenize_batch", "ltr_gather_wait"} <= routed
     decls = "".join(_declarations("linetr_b200.h"))
     for name in routed:
         args = re.search(r"\b" + name + r"\s*\(([^()]*)\)", decls).group(1)

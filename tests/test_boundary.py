@@ -24,7 +24,7 @@ def _model(nd=1):
     return LineTransformer({"mode": "train", "n_line_descriptive_layers": nd})
 
 
-def test_header_symbols_exported():
+def test_header_symbols_exported_at_abi_version():
     hdr = open(os.path.join(ROOT, "include", "linetr_b200.h")).read()
     declared = set(re.findall(r"\b(ltr_[a-z_0-9]+)\s*\(", hdr))
     assert declared == set(N.EXPORTED_SYMBOLS), declared ^ set(N.EXPORTED_SYMBOLS)
@@ -36,7 +36,7 @@ def test_header_symbols_exported():
     assert declared_dbg == set(N.DEBUG_SYMBOLS)
     for s in declared_dbg:
         assert hasattr(lib, s), f"{s} not exported"
-    assert N.load().ltr_abi_version() == N.ABI_VERSION == 3
+    assert N.load().ltr_abi_version() == N.ABI_VERSION == 4
 
 
 def test_header_constants_match_binding_and_kernels():

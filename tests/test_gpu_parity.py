@@ -49,20 +49,6 @@ def fwd(model, data_np):
 
 
 # ------------------------------------------------------------------ GEMM engine
-@pytest.mark.parametrize("M,N_,K,act", [(1, 64, 16, 0), (127, 256, 128, 1), (300, 768, 256, 0), (513, 1024, 256, 2),
-                                        (64, 256, 1024, 0), (2816, 256, 256, 0)])
-def test_linear_engine_vs_torch_fp32(M, N_, K, act):
-    g = torch.Generator().manual_seed(M * 7 + K)
-    x = torch.randn(M, K, generator=g)
-    w = torch.randn(N_, K, generator=g) / K ** 0.5
-    b = torch.randn(N_, generator=g)
-    r = torch.randn(M, N_, generator=g)
-    want = torch.nn.functional.linear(x.double(), w.double(), b.double())
-    want = [want, torch.relu(want), torch.nn.functional.gelu(want)][act] + r.double()
-    got = _ops.linear(x.to(DEV), w.to(DEV), b.to(DEV), r.to(DEV), act).cpu().double()
-    assert (got - want).abs().max().item() < 2e-5
-
-
 @pytest.mark.parametrize("M,N_,K,act,bn", [(1, 128, 64, 0, 0), (128, 128, 64, 0, 128), (127, 256, 128, 1, 256),
                                            (300, 768, 256, 0, 256), (513, 1024, 256, 2, 0), (64, 256, 1024, 0, 128),
                                            (40000, 256, 256, 0, 256), (20000, 512, 512, 1, 0), (1000, 256, 512, 0, 128),
@@ -564,7 +550,7 @@ def test_encoder_tiles_equal_converted_tiles():
 
 @pytest.mark.parametrize("cfg", [{}, {"max_tokens": 8, "token_distance": 12}, {"min_length": 40, "max_keylines": 20}])
 def test_gpu_tokenizer_equals_cpu_glue(cfg):
-    """ltr_tokenize (GPU) vs the committed outputs of the REFERENCE tokeniser (tests/golden/tokenizer_outputs.npz,
+    """ltr_tokenize_batch (GPU, one image) vs the committed outputs of the REFERENCE tokeniser (tests/golden/tokenizer_outputs.npz,
     generated by make_plumbing_golden.py from models/line_process.py:100-196) and vs the CPU glue:
     geometry/masks/adjacency identical, sampled descriptors to fp32 rounding."""
     from tests.test_tokenizer import CFGS, fake_lines, fake_superpoint

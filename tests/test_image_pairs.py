@@ -102,7 +102,7 @@ def _dev(im):
 @pytest.mark.gpu
 def test_tokenize_batch_equals_per_image_gpu_calls():
     """Sizes 640x480, 320x240 and 800x600 (token_distance 8, 8, 10 under auto_min_length), one image without key
-    lines, vertical and split lines: the batch equals per-image ltr_tokenize calls bit for bit."""
+    lines, vertical and split lines: the batch equals per-image GPU calls bit for bit."""
     model, _ = _model()
     eng = engine.PairEngine(model, DEV)
     sets = [(7, 60, 640, 480), (5, 30, 320, 240), (9, 0, 800, 600), (11, 50, 800, 600)]

@@ -3,8 +3,8 @@
 Every GPU case checks that token positions, sublines, masks, responses, angles and scores equal the CPU glue
 (`line_process.line_tokenizer`, pinned to the reference by tests/golden/tokenizer_outputs.npz) bit for bit, that the
 scores equal the model's (round half to even, clipped to the score map's own size), that every descriptor is within
-the element-wise bound of tests/tokenizer_model.py, and that `ltr_tokenize` (one image) equals `ltr_tokenize_batch`
-bit for bit.  The maps are shaped as SuperPoint shapes them: descriptors [256, H//8, W//8], scores
+the element-wise bound of tests/tokenizer_model.py, and that a one-image `ltr_tokenize_batch` equals the image's rows
+of the batch bit for bit.  The maps are shaped as SuperPoint shapes them: descriptors [256, H//8, W//8], scores
 [H//8*8, W//8*8], so at sizes that are not multiples of 8 tokens near the right and bottom edges take the score
 clip and bilinear taps outside the descriptor grid.  Both align_corners modes are run through the C ABI.
 
@@ -268,24 +268,12 @@ class Batch:
 
 
 def tokenize_one(im, T, align):
-    """ltr_tokenize of one image -> outputs."""
-    kl = im["kd"]["klines"].copy()
-    length = np.ascontiguousarray(im["kd"]["length_klines"], dtype=np.float64)
-    g = LP.keyline_geometry(kl, length, float(im["td"]), T, im["W"], im["H"])
-    S = int(g["sub0"][-1])
-    keep = [_f64(g["sp"]), _f64(g["ep"]), _f64(g["epc"]), _f64(length),
-            torch.from_numpy(np.asarray(im["kd"]["angles"], np.float32).reshape(-1, 2)).to(DEV), _i32(g["n_tok"]),
-            _i32(g["sub0"]), _i32(g["sub2line"])]
-    dense, score = im["dense"], im["score"]
-    inp = N.LtrTokenizeInput(*[t.data_ptr() for t in keep], len(kl), S, T, float(im["td"]), dense.data_ptr(), 256,
-                             dense.shape[1], dense.shape[2], score.data_ptr(), score.shape[0], score.shape[1], align)
-    out = _outputs(S, T)
-    N.check(N.load().ltr_tokenize(C.byref(inp), *_ptrs(out), DEV.index, _stream()), "ltr_tokenize")
-    return out
+    """ltr_tokenize_batch of one image -> outputs."""
+    return Batch([im], T).run(align)
 
 
 def check_image(im, T, align, rows, tag):
-    """One image's rows of a GPU run against the glue, the model and ltr_tokenize."""
+    """One image's rows of a GPU run against the glue, the model and a one-image batch."""
     kd = {k: np.array(v, copy=True) for k, v in im["kd"].items()}
     dense, score = im["dense"].cpu(), im["score"].cpu()
     want = LP.line_tokenizer(kd, float(im["td"]), T, {"dense_descriptor": dense[None], "dense_score": score[None]},
@@ -295,7 +283,7 @@ def check_image(im, T, align, rows, tag):
         assert torch.equal(got[k], want[g][0]), (tag, k)
     one = tokenize_one(im, T, align)
     for k in FIELDS:
-        assert torch.equal(one[k].cpu(), got[k]), (tag, "ltr_tokenize", k)
+        assert torch.equal(one[k].cpu(), got[k]), (tag, "one image", k)
     pnt = got["pnt"].numpy().reshape(-1, 2)
     assert np.array_equal(M.scores(pnt, score.numpy()), got["score"].numpy().reshape(-1)), tag
     d = got["desc"].numpy().reshape(-1, 256)
@@ -334,7 +322,7 @@ def _check_batch(images, T, align, tag):
 # ------------------------------------------------------------------ GPU cases
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", range(len(CONSTRUCTED)))
-def test_constructed_geometry_is_numpy_order(case):
+def test_constructed_lines_take_numpy_order_on_the_gpu(case):
     """Positions, cut points, a score pixel and a response that the fma-contracted order rounds differently, and a
     position where a pow-evaluated square of the slope would."""
     T, td, sp, ep, i, what = CONSTRUCTED[case]
@@ -345,7 +333,7 @@ def test_constructed_geometry_is_numpy_order(case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("W,H,td,T", SHAPES)
 @pytest.mark.parametrize("align", [0, 1])
-def test_shapes_and_edge_lines(W, H, td, T, align):
+def test_map_shapes_and_edge_lines(W, H, td, T, align):
     """SuperPoint-shaped maps at sizes that are and are not multiples of 8, lines along every branch, a zero
     descriptor patch under some tokens (the 1e-12 norm floor) and a second image of the same size in the batch."""
     lines = edge_lines(W, H, td, T)
@@ -358,7 +346,7 @@ def test_shapes_and_edge_lines(W, H, td, T, align):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("T", [1, 7, 21, 128])
-def test_token_counts(T):
+def test_token_slot_counts(T):
     """Per T: n_tok = 1, n_tok a multiple of T, one token short and past it, and lines cut into more than 10
     sublines (T <= 21)."""
     W, H, td = 1600, 1200, 4.0
@@ -372,9 +360,9 @@ def test_token_counts(T):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("align", [0, 1])
-def test_batch_of_300_images(align):
+def test_batch_of_300_images_equals_one_image_batches(align):
     """300 images (3 launches of up to 128) of mixed sizes and token distances; the images at 0, 127, 128, 255 and
-    299 have no key lines.  Each image's rows against its own glue and model."""
+    299 have no key lines.  Each image's rows against its own glue, its model and its one-image batch."""
     rng = np.random.Generator(np.random.PCG64(11))
     images = []
     for i in range(300):
@@ -427,6 +415,9 @@ def test_batch_refusals_come_before_any_launch():
         _refused(call(b.input(0, **{k: -1})), "negative count")
     out_ok = b.run(0)                                          # the unmodified batch still runs
     assert not torch.isnan(out_ok["desc"]).any()
+    sp = {"dense_descriptor": ims[0]["dense"][None], "dense_score": ims[0]["score"][None]}
+    kd = {k: v.copy() for k, v in ims[0]["kd"].items()}
+    _refused(lambda: LP.line_tokenizer_gpu(kd, 4.0, 129, sp, (48, 64)), "n_tokens in 1..128")
 
 
 @pytest.mark.gpu

@@ -63,7 +63,7 @@ for mode in ("eager", "cuda_graph"):
     if mode == "eager":
         out["engine_match_pairs_1_pair"] = timeit(lambda: eng.match_pairs(ba, bb, 0.8).counts)
 # ---- the same pair starting where `Matching` starts the plugin: SuperPoint's dense maps already on the device + detected key
-#      lines (host objects) -> GPU tokeniser (LineTransformer.preprocess -> ltr_tokenize) -> forward x2 -> matcher calls
+#      lines (host objects) -> GPU tokeniser (LineTransformer.preprocess -> ltr_tokenize_batch) -> forward x2 -> matcher calls
 try:
     from tests.test_tokenizer import fake_lines, fake_superpoint
     m = LineTransformer({"mode": "test"})
