@@ -45,6 +45,17 @@ int ltr_debug_linear_img_res(const float* x, int32_t ldx, const float* w_host, c
 int ltr_debug_encode_images(const struct LtrModel* model, int32_t n_lines, void* workspace, void* hi[11], void* lo[11],
                             int32_t kblocks[11]);
 
+/* The relative-pose estimator's fp64 root finder on its own, one thread per polynomial: poly [n, 11] ascending
+ * coefficients (device) -> roots [n, 10] ascending, NaN past the count, and count [n] (device).  The estimator's own
+ * __device__ function (Sturm chain and bisection). */
+int ltr_debug_sturm_roots(const double* poly, int32_t n, double* roots, int32_t* count, int32_t device, void* stream);
+
+/* The estimator's five-point solver on its own, one thread per sample: q [n, 5, 4] normalised correspondences
+ * (a0, b0, a1, b1; device) -> E [n, 10, 9] row-major, root_index [n, 10] (the real root each solution came from) and
+ * n_solutions [n] (device); entries past n_solutions are NaN / -1.  The same compiled function the estimator runs. */
+int ltr_debug_essential_solve(const double* q, int32_t n, double* E, int32_t* root_index, int32_t* n_solutions,
+                              int32_t device, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

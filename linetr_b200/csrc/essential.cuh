@@ -140,8 +140,15 @@ __device__ __forceinline__ double ess_maxabs(const double* c, int n) {
   return m;
 }
 
-// Member k of the Sturm chain (degree 10 - k) starts at chain + ESS_CHAIN_OFF(k).
+// Member k of the Sturm chain starts at chain + ESS_CHAIN_OFF(k) and has 11 - k coefficients: its degree is at most
+// 10 - k (degrees strictly decrease along the chain), the coefficients above its degree are 0.
 #define ESS_CHAIN_OFF(k) (11 * (k) - ((k) * ((k) - 1)) / 2)
+
+// Degree of c (coefficients 0..top): the highest index with a non-zero coefficient, 0 for a constant.
+__device__ __forceinline__ int ess_degree(const double* c, int top) {
+  while (top > 0 && c[top] == 0.0) --top;
+  return top;
+}
 
 __device__ __forceinline__ int ess_sign_changes(const double* chain, int len, double x) {
   int prev = 0, n = 0;
@@ -156,42 +163,52 @@ __device__ __forceinline__ int ess_sign_changes(const double* chain, int len, do
   return n;
 }
 
-// Real roots of the degree-10 polynomial p (ascending) in [-B, B]: Sturm chain and bisection.  -> root count.
+// Real roots of the polynomial p (ascending, 11 coefficients, degree 1 to 10 once exact-zero leading coefficients are
+// stripped) in [-B, B]: Sturm chain and bisection.  -> root count; 0 for a constant or a non-finite coefficient.
 __device__ int ess_roots(const double* p, double* roots) {
   double chain[66];
+  bool fin = true;
+  for (int i = 0; i < 11; ++i) fin &= isfinite(p[i]);
   const double m = ess_maxabs(p, 11);
-  if (!(m > 0.0 && m < INFINITY && p[10] != 0.0)) return 0;
+  if (!(fin && m > 0.0)) return 0;
   for (int i = 0; i < 11; ++i) chain[i] = ES_D(p[i], m);
+  const int n = ess_degree(chain, 10);
+  if (n == 0) return 0;
   double bound = 1.0;
-  for (int i = 0; i < 10; ++i) {
-    const double v = ES_A(fabs(ES_D(chain[i], chain[10])), 1.0);
+  for (int i = 0; i < n; ++i) {
+    const double v = ES_A(fabs(ES_D(chain[i], chain[n])), 1.0);
     bound = v > bound ? v : bound;
   }
   bound = bound < ESS_ROOT_BOUND ? bound : ESS_ROOT_BOUND;
   if (!(bound == bound)) return 0;
   double* d = chain + ESS_CHAIN_OFF(1);
   for (int i = 0; i < 10; ++i) d[i] = ES_M(chain[i + 1], (double)(i + 1));
-  const double md = ess_maxabs(d, 10);
-  int len = md > 0.0 ? 2 : 1;
-  if (md > 0.0)
-    for (int i = 0; i < 10; ++i) d[i] = ES_D(d[i], md);
-  for (int k = 1; k < 10 && len == k + 1; ++k) {
-    const double* A = chain + ESS_CHAIN_OFF(k - 1);
-    const double* Bp = chain + ESS_CHAIN_OFF(k);
-    double* r = chain + ESS_CHAIN_OFF(k + 1);
-    const int mdeg = 11 - k;
-    const double lead = Bp[mdeg - 1];
-    if (!(lead != 0.0)) break;
-    const double q1 = ES_D(A[mdeg], lead);
-    double T[10];
-    T[0] = A[0];
-    for (int i = 1; i < mdeg; ++i) T[i] = ES_S(A[i], ES_M(q1, Bp[i - 1]));
-    const double q0 = ES_D(T[mdeg - 1], lead);
-    for (int i = 0; i < mdeg - 1; ++i) r[i] = -ES_S(T[i], ES_M(q0, Bp[i]));
-    const double mr = ess_maxabs(r, mdeg - 1);
+  const double md = ess_maxabs(d, 10);   // > 0: d[n - 1] = n chain[n]
+  for (int i = 0; i < 10; ++i) d[i] = ES_D(d[i], md);
+  // Members len - 2 (A, degree da) and len - 1 (Bp, degree db < da) give the next member: the remainder of A / Bp by
+  // long division, negated, stripped of exact-zero leading coefficients and divided by its largest |coefficient|.
+  // The chain ends at a constant, or before a zero remainder (Bp is then the gcd of p and p').  Where every degree
+  // drops by one this is the two-step division q1 = A[da] / lead, q0 = T[db] / lead.
+  int len = 2, da = n, db = ess_degree(d, n - 1);
+  while (db > 0) {
+    const double* A = chain + ESS_CHAIN_OFF(len - 2);
+    const double* Bp = chain + ESS_CHAIN_OFF(len - 1);
+    double* r = chain + ESS_CHAIN_OFF(len);
+    const double lead = Bp[db];
+    double T[11];
+    for (int i = 0; i <= da; ++i) T[i] = A[i];
+    for (int j = da; j >= db; --j) {
+      const double q = ES_D(T[j], lead);
+      for (int i = 0; i < db; ++i) T[j - db + i] = ES_S(T[j - db + i], ES_M(q, Bp[i]));
+    }
+    for (int i = 0; i < db; ++i) r[i] = -T[i];
+    const double mr = ess_maxabs(r, db);
     if (!(mr > 0.0)) break;
-    for (int i = 0; i < mdeg - 1; ++i) r[i] = ES_D(r[i], mr);
-    len = k + 2;
+    for (int i = 0; i < db; ++i) r[i] = ES_D(r[i], mr);
+    for (int i = db; i < 11 - len; ++i) r[i] = 0.0;
+    da = db;
+    db = ess_degree(r, db - 1);
+    ++len;
   }
   const int v_lo = ess_sign_changes(chain, len, -bound);
   int count = v_lo - ess_sign_changes(chain, len, bound);

@@ -1472,6 +1472,51 @@ int ltr_debug_encode_images(const LtrModel* m, int32_t n_lines, void* workspace,
   return LTR_OK;
 }
 
+// Test hooks of the relative-pose estimator's fp64 pieces: one thread per item, the estimator's __device__ functions.
+static __global__ void debug_sturm_roots_kernel(const double* poly, int n, double* roots, int* count) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double p[11], r[10];
+  for (int j = 0; j < 11; ++j) p[j] = poly[11ll * i + j];
+  const int c = ess_roots(p, r);
+  for (int j = 0; j < 10; ++j) roots[10ll * i + j] = j < c ? r[j] : __longlong_as_double(0x7ff8000000000000ll);
+  count[i] = c;
+}
+
+static __global__ void debug_essential_solve_kernel(const double* q, int n, double* E, int* root_index, int* n_sol) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double4 s[5];
+  for (int j = 0; j < 5; ++j)
+    s[j] = make_double4(q[20ll * i + 4 * j], q[20ll * i + 4 * j + 1], q[20ll * i + 4 * j + 2], q[20ll * i + 4 * j + 3]);
+  double Es[90];
+  int jr[10];
+  const int ns = ess_solve(s, Es, jr);
+  for (int j = 0; j < 90; ++j) E[90ll * i + j] = j < 9 * ns ? Es[j] : __longlong_as_double(0x7ff8000000000000ll);
+  for (int j = 0; j < 10; ++j) root_index[10ll * i + j] = j < ns ? jr[j] : -1;
+  n_sol[i] = ns;
+}
+
+int ltr_debug_sturm_roots(const double* poly, int32_t n, double* roots, int32_t* count, int32_t device, void* stream) {
+  if (n < 0 || (n > 0 && (!poly || !roots || !count))) return set_error(LTR_E_INVALID, "ltr_debug_sturm_roots: bad argument");
+  if (n == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  debug_sturm_roots_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(poly, n, roots, count);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
+int ltr_debug_essential_solve(const double* q, int32_t n, double* E, int32_t* root_index, int32_t* n_solutions,
+                              int32_t device, void* stream) {
+  if (n < 0 || (n > 0 && (!q || !E || !root_index || !n_solutions)))
+    return set_error(LTR_E_INVALID, "ltr_debug_essential_solve: bad argument");
+  if (n == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  debug_essential_solve_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(q, n, E, root_index, n_solutions);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
 float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t out_mode, int32_t iters, int32_t device) {
   if (cudaSetDevice(device) != cudaSuccess) return -1.f;
   const size_t mpad = (size_t)cdiv(m, 256) * 256;

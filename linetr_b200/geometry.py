@@ -600,42 +600,61 @@ def _sign_changes(chain, length, x):
     return n
 
 
+def _degree(c):
+    """Degree of each polynomial c [K, n] (ascending): the highest index with a non-zero coefficient, 0 for a
+    constant."""
+    nz = c != 0
+    return np.where(nz.any(1), c.shape[1] - 1 - np.argmax(nz[:, ::-1], 1), 0)
+
+
 def sturm_roots(p):
-    """The real roots of polynomials of degree 10 (ascending coefficients p [K, 11]) in [-B, B], B = min(Cauchy bound,
-    ESS_ROOT_BOUND), with the kernels' fixed operation sequence: the Sturm chain of p (each member divided by its
-    largest |coefficient|), then per root index i < (number of real roots) ESS_BISECT_STEPS bisection steps on
-    "roots below mid > i".  -> (roots [K, 10] ascending, NaN past the count, count [K])."""
+    """The real roots of polynomials of degree 1 to 10 (ascending coefficients p [K, 11], exact-zero leading
+    coefficients stripped) in [-B, B], B = min(Cauchy bound, ESS_ROOT_BOUND), with the kernels' operation sequence:
+    the Sturm chain of p (each member's remainder by long division, stripped of exact-zero leading coefficients and
+    divided by its largest |coefficient|; the chain ends at a constant or before a zero remainder), then per root
+    index i < (number of distinct real roots) ESS_BISECT_STEPS bisection steps on "roots below mid > i".  A constant
+    or a non-finite coefficient has no roots.  -> (roots [K, 10] ascending, NaN past the count, count [K])."""
     p = np.asarray(p, dtype=np.float64)
     K = p.shape[0]
+    ar = np.arange(K)
     with np.errstate(all="ignore"):
         m = _maxabs(p)
-        ok = (m > 0) & (m < np.inf) & (p[:, 10] != 0)
+        ok = (m > 0) & np.isfinite(p).all(1)
         s0 = p / np.where(ok, m, 1.0)[:, None]
+        n = _degree(s0)
+        ok &= n > 0
+        lead = s0[ar, n]
         bound = np.ones(K)
         for i in range(10):
-            a = np.abs(s0[:, i] / s0[:, 10])
-            bound = np.where(a + 1.0 > bound, a + 1.0, bound)
+            a = np.abs(s0[:, i] / lead)
+            bound = np.where((i < n) & (a + 1.0 > bound), a + 1.0, bound)
         bound = np.where(bound < ESS_ROOT_BOUND, bound, ESS_ROOT_BOUND)
         ok &= bound == bound
         d = np.stack([s0[:, i + 1] * float(i + 1) for i in range(10)], 1)
         md = _maxabs(d)
-        length = np.where(ok, np.where(md > 0, 2, 1), 0)
         chain = [s0, d / np.where(md > 0, md, 1.0)[:, None]]
+        length = np.where(ok, 2, 0)
+        # members k - 1 (degree da) and k (degree db < da) give member k + 1 (csrc/essential.cuh ess_roots)
+        da, db = n, _degree(chain[1])
         for k in range(1, 10):
             A, Bp = chain[k - 1], chain[k]
-            mdeg = 11 - k
-            lead = Bp[:, mdeg - 1]
-            go = (length == k + 1) & (lead != 0)
-            q1 = A[:, mdeg] / lead
-            T = A[:, :mdeg].copy()
-            for i in range(1, mdeg):
-                T[:, i] = A[:, i] - q1 * Bp[:, i - 1]
-            q0 = T[:, mdeg - 1] / lead
-            r = np.stack([-(T[:, i] - q0 * Bp[:, i]) for i in range(mdeg - 1)], 1)
+            go = (length == k + 1) & (db > 0)
+            lead = Bp[ar, np.minimum(db, 10 - k)]      # (rows whose chain has ended read any coefficient)
+            T = np.zeros((K, 11))
+            T[:, :A.shape[1]] = A
+            for j in range(10, 0, -1):
+                act = go & (j <= da) & (j >= db)
+                q = T[ar, j] / lead
+                for i in range(10 - k):
+                    col = np.where(act & (i < db), j - db + i, 0)
+                    upd = T[ar, col] - q * Bp[:, i]
+                    T[ar, col] = np.where(act & (i < db), upd, T[ar, col])
+            r = np.stack([np.where(i < db, -T[:, i], 0.0) for i in range(10 - k)], 1)
             mr = _maxabs(r)
             go &= mr > 0
             chain.append(r / np.where(go, mr, 1.0)[:, None])
             length = np.where(go, k + 2, length)
+            da, db = np.where(go, db, da), np.where(go, _degree(chain[-1]), db)
         lo0 = -bound
         v_lo = _sign_changes(chain, length, lo0[:, None])[:, 0]
         v_hi = _sign_changes(chain, length, bound[:, None])[:, 0]
