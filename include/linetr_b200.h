@@ -147,7 +147,8 @@ typedef struct {
   int32_t layout;          /* LTR_LAYOUT_* of desc0/desc1 */
   int32_t d;               /* descriptor dim, multiple of 16 (others: LTR_E_UNSUPPORTED, from
                               ltr_match_workspace_bytes too) */
-  int32_t n_pairs;
+  int32_t n_pairs;         /* at most 65535 (the pair is a grid dimension); more: LTR_E_UNSUPPORTED, from
+                              ltr_match_workspace_bytes too - split the pairs into calls */
   int32_t n0, n1;          /* sublines per image when cu0/cu1 are NULL */
   const int32_t* cu0;      /* device [n_pairs+1] or NULL */
   const int32_t* cu1;
@@ -156,7 +157,8 @@ typedef struct {
   const int32_t* cuk0;     /* device [n_pairs+1] keyline offsets, required iff sub_off0 != NULL */
   const int32_t* cuk1;
   int32_t max_n0, max_n1;  /* max sublines per image on each side (grid sizing; var-len only) */
-  int32_t max_k0, max_k1;  /* max keylines per image on each side (keyline merging only) */
+  int32_t max_k0, max_k1;  /* max keylines per image on each side (keyline merging only; max_k0 above
+                              8 * 65535: LTR_E_UNSUPPORTED) */
   int64_t dist_pair_stride; /* elements between consecutive pairs' matrices in `dist_key`;
                                0 = max_k0*max_k1 (or max_n0*max_n1 without merging) */
   float nn_thresh;         /* strict '<' (models/nn_matcher.py:18) */
@@ -277,7 +279,7 @@ int ltr_match_indexed(const LtrMatchInput* in, const LtrPairIndex* idx, const Lt
 
 /* nn_matcher_distmat on caller-supplied distance matrices (device, row-major [n0, n1],
  * pair p at p*dist_pair_stride, 0 = n0*n1); negative entries are clipped to 0 as the
- * reference does (models/nn_matcher.py:12). */
+ * reference does (models/nn_matcher.py:12).  At most 65535 pairs (more: LTR_E_UNSUPPORTED). */
 int ltr_match_distmat(const float* dist, int32_t n_pairs, int32_t n0, int32_t n1,
                       int64_t dist_pair_stride, float nn_thresh, int32_t mutual,
                       int32_t* matches0, float* scores0, int32_t* nn1, int32_t* counts,
@@ -285,7 +287,8 @@ int ltr_match_distmat(const float* dist, int32_t n_pairs, int32_t n0, int32_t n1
 
 /* LineTransformer.subline2keyline alone: dist_key[p] = A0_p @ dist_sub[p] @ A1_p^T with the
  * adjacencies given as CSR offsets (see LtrMatchInput).  dist_sub: pair p at p*stride_sub,
- * row-major [S0_p, S1_p]; dist_key: pair p at p*stride_key, row-major [K0_p, K1_p]. */
+ * row-major [S0_p, S1_p]; dist_key: pair p at p*stride_key, row-major [K0_p, K1_p].  At most
+ * 65535 pairs and max_k0 <= 8 * 65535 (more: LTR_E_UNSUPPORTED). */
 int ltr_merge_sublines(const float* dist_sub, int64_t stride_sub, int32_t n_pairs,
                        const int32_t* cuk0, const int32_t* cuk1, const int32_t* sub_off0,
                        const int32_t* sub_off1, int32_t max_k0, int32_t max_k1, float* dist_key,

@@ -765,6 +765,20 @@ static const char* check_match_input(const LtrMatchInput* in) {
 // a descriptor dimension that is not a multiple of 16 is a valid request the kernels do not serve
 static int match_input_code(const LtrMatchInput* in) { return in->d > 0 && in->d % 16 ? LTR_E_UNSUPPORTED : LTR_E_INVALID; }
 
+// The matcher kernels put the pair count in grid y or z, and segmean_kernel covers side 0's key lines with grid y in
+// blocks of 8: counts above what those grid dimensions hold are valid requests the kernels do not serve, refused
+// (LTR_E_UNSUPPORTED) before any CUDA call.  Callers with more pairs split them into calls (engine.plan_chunks).
+constexpr int kMaxGridYZ = 65535;
+static int check_grid_limits(const char* who, int64_t n_pairs, bool seg, int64_t max_k0) {
+  if (n_pairs > kMaxGridYZ) return set_error(LTR_E_UNSUPPORTED, std::string(who) + ": at most 65535 pairs per call");
+  if (seg && max_k0 > 8LL * kMaxGridYZ)
+    return set_error(LTR_E_UNSUPPORTED, std::string(who) + ": key-line merging takes at most 8 * 65535 side-0 key lines per pair");
+  return LTR_OK;
+}
+static int check_match_limits(const char* who, const LtrMatchInput* in) {
+  return check_grid_limits(who, in->n_pairs, in->sub_off0 != nullptr, in->max_k0);
+}
+
 }  // extern "C"
 
 // launch sequence of the tensor-core matcher; returns 0 or an error code.  ix != nullptr: pair list over image
@@ -934,6 +948,7 @@ extern "C" {
 int64_t ltr_match_workspace_bytes(const LtrMatchInput* in) {
   if (!in) return set_error(LTR_E_INVALID, "ltr_match_workspace_bytes: null argument");
   if (const char* e = check_match_input(in)) return set_error(match_input_code(in), e);
+  if (int rc = check_match_limits("ltr_match_workspace_bytes", in)) return rc;
   if (in->n_pairs <= 0 || in->d != MT_D) return 0;
   return plan_match(*in, nullptr, nullptr).bytes + 1024;
 }
@@ -942,6 +957,7 @@ int ltr_match(const LtrMatchInput* in, const LtrMatchOutput* out, int32_t device
   if (!in || !out) return set_error(LTR_E_INVALID, "ltr_match: null argument");
   if (in->n_pairs <= 0) return LTR_OK;
   if (const char* e = check_match_input(in)) return set_error(match_input_code(in), e);
+  LTR_TRY(check_match_limits("ltr_match", in));
   LTR_TRY(check_match_output("ltr_match", *in, *out));
   const bool seg = in->sub_off0 != nullptr;
   const bool tc = in->d == MT_D;
@@ -1003,6 +1019,7 @@ static const char* check_match_indexed(const LtrMatchInput* in, const LtrPairInd
 int64_t ltr_match_indexed_workspace_bytes(const LtrMatchInput* in, const LtrPairIndex* idx) {
   if (!in || !idx) return set_error(LTR_E_INVALID, "ltr_match_indexed_workspace_bytes: null argument");
   if (const char* e = check_match_indexed(in, idx)) return set_error(LTR_E_INVALID, e);
+  if (int rc = check_match_limits("ltr_match_indexed_workspace_bytes", in)) return rc;
   if (in->n_pairs <= 0) return 0;
   return plan_match(*in, idx, nullptr).bytes + 1024;
 }
@@ -1014,6 +1031,7 @@ int ltr_match_indexed(const LtrMatchInput* in, const LtrPairIndex* idx, const Lt
   if (out->gather && out->gather->world > 1) return set_error(LTR_E_UNSUPPORTED, "ltr_match_indexed: gather is not supported");
   if (in->n_pairs <= 0) return LTR_OK;
   if (const char* e = check_match_indexed(in, idx)) return set_error(LTR_E_INVALID, e);
+  LTR_TRY(check_match_limits("ltr_match_indexed", in));
   LTR_TRY(check_match_output("ltr_match_indexed", *in, *out));
   return run_match("ltr_match_indexed", *in, idx, *out, device, stream);
 }
@@ -1034,6 +1052,7 @@ int ltr_match_distmat(const float* dist, int32_t n_pairs, int32_t n0, int32_t n1
                       int32_t mutual, int32_t* matches0, float* scores0, int32_t* nn1, int32_t* counts, int32_t device,
                       void* stream) {
   if (n_pairs <= 0) return LTR_OK;
+  LTR_TRY(check_grid_limits("ltr_match_distmat", n_pairs, false, 0));
   if (!matches0 || !scores0 || !nn1 || !counts) return set_error(LTR_E_INVALID, "ltr_match_distmat: null output");
   if (n0 > 0 && n1 > 0 && !dist) return set_error(LTR_E_INVALID, "ltr_match_distmat: null distance matrix");
   LTR_CUDA_TRY(cudaSetDevice(device));
@@ -1048,6 +1067,7 @@ int ltr_merge_sublines(const float* dist_sub, int64_t stride_sub, int32_t n_pair
                        const int32_t* cuk1, const int32_t* sub_off0, const int32_t* sub_off1, int32_t max_k0,
                        int32_t max_k1, float* dist_key, int64_t stride_key, int32_t device, void* stream) {
   if (n_pairs <= 0 || max_k0 <= 0 || max_k1 <= 0) return LTR_OK;
+  LTR_TRY(check_grid_limits("ltr_merge_sublines", n_pairs, true, max_k0));
   if (!dist_sub || !cuk0 || !cuk1 || !sub_off0 || !sub_off1 || !dist_key)
     return set_error(LTR_E_INVALID, "ltr_merge_sublines: null argument");
   LTR_CUDA_TRY(cudaSetDevice(device));
