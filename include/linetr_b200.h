@@ -30,6 +30,8 @@
  *                                 (models/utils.py:291-412) verify matches, with line matches as well as points.
  *   ltr_essential              <- estimate_pose (models/utils.py:291-315): cv2.findEssentialMat(RANSAC) +
  *                                 cv2.recoverPose per pair, batched.
+ *   ltr_fundamental            <- cv2.findFundamentalMat(FM_RANSAC) per pair, batched, for pairs without intrinsics,
+ *                                 with an epipolar check of the line matches.
  *   ltr_warp_pairs             <- cv2.warpPerspective of the grey and colour images + the eroded valid mask of the
  *                                 homography dataset builder (dataloaders/build_homography_dataset.py:164-184).
  *   ltr_photometric            <- imgPhotometric of the homography dataset builder (ImgAugTransform +
@@ -577,6 +579,75 @@ typedef struct {
 /* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments, LTR_E_UNSUPPORTED over
  * capacity) come before any launch.  n_pairs == 0 writes nothing. */
 int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, int32_t device, void* stream);
+
+/* Fundamental matrices of uncalibrated image pairs, as one cv2.findFundamentalMat(FM_RANSAC) per pair would verify
+ * them, plus an epipolar check of the line matches; DESIGN.md "Fundamental matrices" states the model:
+ *   - F maps image 0 to image 1: x1^T F x0 = 0 in pixels;
+ *   - correspondences of pair p: every matched side-0 keypoint row (match in [0, n_pts1[p])) in row order with its
+ *     partner; per side, coordinates are normalised by the centre and half the larger extent of that side's bounding
+ *     box (as ltr_homography's points);
+ *   - hypothesis k draws 7 distinct correspondences with ltr_homography's hash and redraw rule and solves them with the
+ *     seven-point method (QR null space F1, F2, the cubic det(F2 + a (F1 - F2)), its real roots by a Sturm chain and
+ *     bisection) in explicitly rounded fp64: up to 3 solutions j (real root j in ascending order; the solution at
+ *     a = infinity is not returned), denormalised and scaled to unit Frobenius norm, largest |entry| positive;
+ *   - inlier iff cv2's FM error, max((x1^T F x0)^2 / |(F x0)_xy|^2, (x1^T F x0)^2 / |(F^T x1)_xy|^2), is below
+ *     thresh^2, evaluated without the division; a zero line normal makes an outlier;
+ *   - the winner has the most inliers, then the lowest k, then the lowest j; with at least 8 inliers it is refitted by
+ *     the normalised eight-point method over them (smallest eigenvector of A^T A, rank 2 through the SVD), and the
+ *     refit is kept iff it has at least as many inliers;
+ *   - line check (lines_consistent, aligned with matches_l): for a matched key-line pair s0 = (a0, b0), s1 = (a1, b1),
+ *     the epipolar lines F a0, F b0 cut the line through s1 at positions ta, tb (a1 at 0, b1 at 1); the overlap ratio
+ *     is |[min, max] n [0, 1]| / min(max - min, 1); the same with F^T on s0.  A side whose intersection has |w| <=
+ *     FLT_EPSILON |X|, or whose two positions coincide, cannot reject.  Consistent iff no side's ratio is below
+ *     min_overlap.  Lines take no part in the fit.
+ * A pair with fewer than 7 correspondences, no finite solution, or more match rows than max_rows_p is invalid: F is NaN,
+ * no row is an inlier or consistent, hypothesis is -1.  A planar scene is degenerate for F: use ltr_homography there.
+ *
+ * Capacity: one pair's correspondences are staged in shared memory, 18 bytes per keypoint row over max_rows_p, at most
+ * 200 KiB (11377 rows).  Beyond that the call returns LTR_E_UNSUPPORTED before any launch.  Line rows are read from
+ * global memory and have no bound.  Coordinates must be finite. */
+typedef struct {
+  const float* pts0;              /* device [*, 2] keypoint pool of side 0 */
+  const float* pts1;              /* device [*, 2] keypoint pool of side 1 */
+  const int32_t* pts_off0;        /* device [n_pairs]: pair p's side-0 keypoints start at pts0 row pts_off0[p] */
+  const int32_t* pts_off1;        /* device [n_pairs] */
+  const int32_t* n_pts1;          /* device [n_pairs]: side-1 keypoints of pair p */
+  const int32_t* matches_p;       /* device: local side-1 index or -1 per side-0 keypoint row */
+  const int32_t* cu_p;            /* device [n_pairs + 1]: pair p owns matches_p rows [cu_p[p], cu_p[p+1]) */
+  const float* segs0;             /* device [*, 2, 2] segment pools (start xy, end xy) */
+  const float* segs1;
+  const int32_t* seg_off0;        /* device [n_pairs]: pair p's side-0 segments start at segs0 row seg_off0[p] */
+  const int32_t* seg_off1;
+  const int32_t* n_segs1;         /* device [n_pairs] */
+  const int32_t* matches_l;       /* device: local side-1 index or -1 per side-0 segment row */
+  const int32_t* cu_l;            /* device [n_pairs + 1] */
+  int32_t n_pairs;
+  int32_t max_rows_p;             /* bound of every pair's keypoint match rows; sizes the staging, a pair over it is
+                                     invalid */
+  int32_t max_rows_l;             /* bound of every pair's segment match rows (0: no line matches) */
+  double thresh;                  /* pixels (3: OpenCV's default) */
+  double min_overlap;             /* in [0, 1] (0.5) */
+  int32_t n_hypotheses;           /* >= 1 (2048) */
+  uint64_t seed;
+} LtrFundamentalInput;
+
+/* Outputs (device, caller-owned).  key [n_pairs] is workspace (winning (count << 32) | ~(3 k + j), 0 = none). */
+typedef struct {
+  double* F;                      /* [n_pairs, 3, 3] x1^T F x0 = 0 in pixels, unit Frobenius norm */
+  uint8_t* valid;                 /* [n_pairs] */
+  uint8_t* refit;                 /* [n_pairs] 1 where F is the eight-point refit */
+  uint8_t* inliers_p;             /* aligned with matches_p (0 for unmatched rows) */
+  uint8_t* lines_consistent;      /* aligned with matches_l (0 for unmatched rows and invalid pairs) */
+  int32_t* n_inliers;             /* [n_pairs] */
+  int32_t* n_lines_consistent;    /* [n_pairs] */
+  int32_t* hypothesis;            /* [n_pairs] 3 k + j of the winning solution, -1 when invalid */
+  int32_t* hypothesis_inliers;    /* [n_pairs] its inlier count */
+  uint64_t* key;
+} LtrFundamentalOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments, LTR_E_UNSUPPORTED over
+ * capacity) come before any launch.  n_pairs == 0 writes nothing. */
+int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* out, int32_t device, void* stream);
 
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where

@@ -14,6 +14,9 @@ homography-estimation metric:
 Relative pose (geometry): five-point RANSAC essential matrices and the pose of calibrated pairs, batched on the GPU, and
 the reference's pose metrics:
     estimate_poses, compute_epipolar_error, compute_pose_error, pose_auc, pose_errors
+Fundamental matrices (geometry): seven-point RANSAC with an eight-point refit for uncalibrated pairs, and an epipolar
+check of the line matches, batched on the GPU:
+    estimate_fundamentals
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
@@ -53,6 +56,7 @@ _LAZY = {
     "compute_pose_error": ("geometry", "compute_pose_error"),
     "pose_auc": ("geometry", "pose_auc"),
     "pose_errors": ("geometry", "pose_errors"),
+    "estimate_fundamentals": ("geometry", "estimate_fundamentals"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

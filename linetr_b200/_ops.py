@@ -477,6 +477,37 @@ def essential(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_
     _call("ltr_essential", dev, C.byref(inp), C.byref(out))
 
 
+def fundamental(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, segs0, segs1,
+                seg_off0, seg_off1, n_segs1, matches_l, cu_l, max_rows_l, F, valid, refit, inliers_p, lines_consistent,
+                n_inliers, n_lines_consistent, hypothesis, hypothesis_inliers, key, thresh=3.0, min_overlap=0.5,
+                n_hypotheses=2048, seed=0):
+    """ltr_fundamental into caller-allocated outputs: keypoint pools [*,2] / segment pools [*,2,2] fp32, per-pair pool
+    offsets and side-1 counts int32 [P], match rows int32 with offsets cu_p / cu_l [P+1]; F [P,3,3] fp64, valid / refit
+    [P] uint8, inliers_p / lines_consistent uint8 aligned with the match rows, counts / hypothesis int32 [P], key [P]
+    int64 workspace."""
+    _req_cuda(F, "F")
+    dev = F.device
+    _check_tensors("fundamental", dev, (
+        ("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
+        ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32), ("matches_p", matches_p, torch.int32),
+        ("cu_p", cu_p, torch.int32), ("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32),
+        ("seg_off0", seg_off0, torch.int32), ("seg_off1", seg_off1, torch.int32), ("n_segs1", n_segs1, torch.int32),
+        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("F", F, torch.float64),
+        ("valid", valid, torch.uint8), ("refit", refit, torch.uint8), ("inliers_p", inliers_p, torch.uint8),
+        ("lines_consistent", lines_consistent, torch.uint8), ("n_inliers", n_inliers, torch.int32),
+        ("n_lines_consistent", n_lines_consistent, torch.int32), ("hypothesis", hypothesis, torch.int32),
+        ("hypothesis_inliers", hypothesis_inliers, torch.int32), ("key", key, torch.int64)))
+    inp = _struct(N.LtrFundamentalInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
+                  matches_p=matches_p, cu_p=cu_p, segs0=segs0, segs1=segs1, seg_off0=seg_off0, seg_off1=seg_off1,
+                  n_segs1=n_segs1, matches_l=matches_l, cu_l=cu_l, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
+                  max_rows_l=int(max_rows_l), thresh=float(thresh), min_overlap=float(min_overlap),
+                  n_hypotheses=int(n_hypotheses), seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
+    out = _struct(N.LtrFundamentalOutput, F=F, valid=valid, refit=refit, inliers_p=inliers_p,
+                  lines_consistent=lines_consistent, n_inliers=n_inliers, n_lines_consistent=n_lines_consistent,
+                  hypothesis=hypothesis, hypothesis_inliers=hypothesis_inliers, key=key)
+    _call("ltr_fundamental", dev, C.byref(inp), C.byref(out))
+
+
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
     """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
     (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""

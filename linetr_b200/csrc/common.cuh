@@ -45,6 +45,7 @@ enum KernelClass : int {
   KC_WARP,
   KC_ESSENTIAL,
   KC_PHOTOMETRIC,
+  KC_FUNDAMENTAL,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

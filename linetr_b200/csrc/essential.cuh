@@ -30,10 +30,6 @@ constexpr int ESS_THREADS = 128;          // hypotheses per CTA
 constexpr int ESS_POSE_THREADS = 256;
 constexpr int ESS_ROW_BYTES = 32;         // shared bytes per correspondence: a0, b0, a1, b1 fp64
 constexpr int ESS_SMEM_MAX = 200 * 1024;
-constexpr int ESS_BISECT_STEPS = 100;
-constexpr double ESS_RANK_EPS = 1e-10;
-constexpr double ESS_ROOT_BOUND = 1e8;
-constexpr int ESS_JACOBI_SWEEPS = 30;
 
 struct EssentialArgs {
   const float* pts0; const float* pts1;   // [*, 2] keypoint pools
@@ -118,167 +114,12 @@ __device__ __forceinline__ void ess_mul21(const double* x, const double* y, doub
     for (int j = 0; j < 4; ++j) out[ESS_MUL21[i][j]] = ES_A(out[ESS_MUL21[i][j]], ES_M(x[i], y[j]));
 }
 
-// Polynomials in z, ascending coefficients: out (la + lb - 1) = x (la) * y (lb)
-__device__ __forceinline__ void ess_pmul(const double* x, int la, const double* y, int lb, double* out) {
-  for (int i = 0; i < la + lb - 1; ++i) out[i] = 0.0;
-  for (int i = 0; i < la; ++i)
-    for (int j = 0; j < lb; ++j) out[i + j] = ES_A(out[i + j], ES_M(x[i], y[j]));
-}
-
-__device__ __forceinline__ double ess_horner(const double* c, int deg, double x) {
-  double v = c[deg];
-  for (int i = deg - 1; i >= 0; --i) v = ES_A(ES_M(v, x), c[i]);
-  return v;
-}
-
-__device__ __forceinline__ double ess_maxabs(const double* c, int n) {
-  double m = 0.0;
-  for (int i = 0; i < n; ++i) {
-    const double v = fabs(c[i]);
-    m = v > m ? v : m;
-  }
-  return m;
-}
-
-// Member k of the Sturm chain starts at chain + ESS_CHAIN_OFF(k) and has 11 - k coefficients: its degree is at most
-// 10 - k (degrees strictly decrease along the chain), the coefficients above its degree are 0.
-#define ESS_CHAIN_OFF(k) (11 * (k) - ((k) * ((k) - 1)) / 2)
-
-// Degree of c (coefficients 0..top): the highest index with a non-zero coefficient, 0 for a constant.
-__device__ __forceinline__ int ess_degree(const double* c, int top) {
-  while (top > 0 && c[top] == 0.0) --top;
-  return top;
-}
-
-__device__ __forceinline__ int ess_sign_changes(const double* chain, int len, double x) {
-  int prev = 0, n = 0;
-  for (int k = 0; k < len; ++k) {
-    const double v = ess_horner(chain + ESS_CHAIN_OFF(k), 10 - k, x);
-    const int s = (v > 0.0) - (v < 0.0);
-    if (s != 0) {
-      n += prev != 0 && s != prev;
-      prev = s;
-    }
-  }
-  return n;
-}
-
-// Real roots of the polynomial p (ascending, 11 coefficients, degree 1 to 10 once exact-zero leading coefficients are
-// stripped) in [-B, B]: Sturm chain and bisection.  -> root count; 0 for a constant or a non-finite coefficient.
-__device__ int ess_roots(const double* p, double* roots) {
-  double chain[66];
-  bool fin = true;
-  for (int i = 0; i < 11; ++i) fin &= isfinite(p[i]);
-  const double m = ess_maxabs(p, 11);
-  if (!(fin && m > 0.0)) return 0;
-  for (int i = 0; i < 11; ++i) chain[i] = ES_D(p[i], m);
-  const int n = ess_degree(chain, 10);
-  if (n == 0) return 0;
-  double bound = 1.0;
-  for (int i = 0; i < n; ++i) {
-    const double v = ES_A(fabs(ES_D(chain[i], chain[n])), 1.0);
-    bound = v > bound ? v : bound;
-  }
-  bound = bound < ESS_ROOT_BOUND ? bound : ESS_ROOT_BOUND;
-  if (!(bound == bound)) return 0;
-  double* d = chain + ESS_CHAIN_OFF(1);
-  for (int i = 0; i < 10; ++i) d[i] = ES_M(chain[i + 1], (double)(i + 1));
-  const double md = ess_maxabs(d, 10);   // > 0: d[n - 1] = n chain[n]
-  for (int i = 0; i < 10; ++i) d[i] = ES_D(d[i], md);
-  // Members len - 2 (A, degree da) and len - 1 (Bp, degree db < da) give the next member: the remainder of A / Bp by
-  // long division, negated, stripped of exact-zero leading coefficients and divided by its largest |coefficient|.
-  // The chain ends at a constant, or before a zero remainder (Bp is then the gcd of p and p').  Where every degree
-  // drops by one this is the two-step division q1 = A[da] / lead, q0 = T[db] / lead.
-  int len = 2, da = n, db = ess_degree(d, n - 1);
-  while (db > 0) {
-    const double* A = chain + ESS_CHAIN_OFF(len - 2);
-    const double* Bp = chain + ESS_CHAIN_OFF(len - 1);
-    double* r = chain + ESS_CHAIN_OFF(len);
-    const double lead = Bp[db];
-    double T[11];
-    for (int i = 0; i <= da; ++i) T[i] = A[i];
-    for (int j = da; j >= db; --j) {
-      const double q = ES_D(T[j], lead);
-      for (int i = 0; i < db; ++i) T[j - db + i] = ES_S(T[j - db + i], ES_M(q, Bp[i]));
-    }
-    for (int i = 0; i < db; ++i) r[i] = -T[i];
-    const double mr = ess_maxabs(r, db);
-    if (!(mr > 0.0)) break;
-    for (int i = 0; i < db; ++i) r[i] = ES_D(r[i], mr);
-    for (int i = db; i < 11 - len; ++i) r[i] = 0.0;
-    da = db;
-    db = ess_degree(r, db - 1);
-    ++len;
-  }
-  const int v_lo = ess_sign_changes(chain, len, -bound);
-  int count = v_lo - ess_sign_changes(chain, len, bound);
-  count = count < 0 ? 0 : (count > 10 ? 10 : count);
-  for (int i = 0; i < count; ++i) {
-    double lo = -bound, hi = bound;
-    for (int s = 0; s < ESS_BISECT_STEPS; ++s) {
-      const double mid = ES_M(ES_A(lo, hi), 0.5);
-      if (!(mid > lo && mid < hi)) break;   // converged: further steps change nothing
-      if (v_lo - ess_sign_changes(chain, len, mid) > i) hi = mid; else lo = mid;
-    }
-    roots[i] = ES_M(ES_A(lo, hi), 0.5);
-  }
-  return count;
-}
-
-__device__ __forceinline__ void ess_cross(const double* x, const double* y, double* c) {
-  c[0] = ES_S(ES_M(x[1], y[2]), ES_M(x[2], y[1]));
-  c[1] = ES_S(ES_M(x[2], y[0]), ES_M(x[0], y[2]));
-  c[2] = ES_S(ES_M(x[0], y[1]), ES_M(x[1], y[0]));
-}
-
 // The five-point solver on 5 normalised correspondences q[s] = (a0, b0, a1, b1): up to 10 E (row-major, Es[9 s]) with
 // their root indices jr[s].  -> solution count.
 __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
-  // Householder QR of the 9 x 5 transpose of the epipolar rows
-  double M[9][5];
-  for (int c = 0; c < 5; ++c) {
-    const double a0 = q[c].x, b0 = q[c].y, a1 = q[c].z, b1 = q[c].w;
-    M[0][c] = ES_M(a1, a0); M[1][c] = ES_M(a1, b0); M[2][c] = a1;
-    M[3][c] = ES_M(b1, a0); M[4][c] = ES_M(b1, b0); M[5][c] = b1;
-    M[6][c] = a0; M[7][c] = b0; M[8][c] = 1.0;
-  }
-  double V[5][9], beta[5], nrm0 = 0.0;   // reflector c is V[c][c..8] (v_c = M[c][c] - alpha, then M[c+1..8][c])
-  for (int c = 0; c < 5; ++c) {
-    double acc = 0.0;
-    for (int i = c; i < 9; ++i) acc = ES_A(acc, ES_M(M[i][c], M[i][c]));
-    const double nrm = __dsqrt_rn(acc);
-    if (c == 0) {
-      nrm0 = nrm;
-      if (!(nrm > 0.0)) return 0;
-    } else if (!(nrm > ES_M(ESS_RANK_EPS, nrm0))) {
-      return 0;   // rank-deficient sample
-    }
-    const double alpha = M[c][c] >= 0.0 ? -nrm : nrm;
-    for (int i = c + 1; i < 9; ++i) V[c][i] = M[i][c];
-    V[c][c] = ES_S(M[c][c], alpha);
-    double vtv = 0.0;
-    for (int i = c; i < 9; ++i) vtv = ES_A(vtv, ES_M(V[c][i], V[c][i]));
-    beta[c] = vtv > 0.0 ? ES_D(2.0, vtv) : 0.0;
-    for (int j = c + 1; j < 5; ++j) {
-      double s = 0.0;
-      for (int i = c; i < 9; ++i) s = ES_A(s, ES_M(V[c][i], M[i][j]));
-      const double g = ES_M(s, beta[c]);
-      for (int i = c; i < 9; ++i) M[i][j] = ES_S(M[i][j], ES_M(g, V[c][i]));
-    }
-  }
-  // null basis X, Y, Z, W = Q e5 .. Q e8; e[i] = entry i of E as a polynomial [x, y, z, 1]
+  // null basis X, Y, Z, W of the 5 epipolar rows; e[i] = entry i of E as a polynomial [x, y, z, 1]
   double e[9][4];
-  for (int b = 0; b < 4; ++b) {
-    double y[9];
-    for (int i = 0; i < 9; ++i) y[i] = i == 5 + b ? 1.0 : 0.0;
-    for (int c = 4; c >= 0; --c) {
-      double s = 0.0;
-      for (int i = c; i < 9; ++i) s = ES_A(s, ES_M(V[c][i], y[i]));
-      const double g = ES_M(s, beta[c]);
-      for (int i = c; i < 9; ++i) y[i] = ES_S(y[i], ES_M(g, V[c][i]));
-    }
-    for (int i = 0; i < 9; ++i) e[i][b] = y[i];
-  }
+  if (!rc_null_basis<5>(q, e)) return 0;
   // the 10 x 20 constraints: det E, then (2 E E^T - tr(E E^T) I) E row-major
   double C[10][20];
   {
@@ -453,34 +294,7 @@ __device__ __noinline__ void ess_decompose(const double* E, double (*cand)[12]) 
       S[i][k] = E[i] * E[k] + E[3 + i] * E[3 + k] + E[6 + i] * E[6 + k];
       V[i][k] = i == k ? 1.0 : 0.0;
     }
-  const double fro = S[0][0] * S[0][0] + S[1][1] * S[1][1] + S[2][2] * S[2][2];
-  for (int sweep = 0; sweep < ESS_JACOBI_SWEEPS; ++sweep) {
-    const double off = S[0][1] * S[0][1] + S[0][2] * S[0][2] + S[1][2] * S[1][2];
-    if (!(off > 1e-32 * fro)) break;
-    for (int p = 0; p < 2; ++p)
-      for (int q = p + 1; q < 3; ++q) {
-        const double apq = S[p][q];
-        if (apq == 0.0) continue;
-        const double theta = (S[q][q] - S[p][p]) / (2.0 * apq);
-        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-        for (int k = 0; k < 3; ++k) {
-          const double skp = S[k][p], skq = S[k][q];
-          S[k][p] = c * skp - s * skq;
-          S[k][q] = s * skp + c * skq;
-        }
-        for (int k = 0; k < 3; ++k) {
-          const double spk = S[p][k], sqk = S[q][k];
-          S[p][k] = c * spk - s * sqk;
-          S[q][k] = s * spk + c * sqk;
-        }
-        for (int k = 0; k < 3; ++k) {
-          const double vkp = V[k][p], vkq = V[k][q];
-          V[k][p] = c * vkp - s * vkq;
-          V[k][q] = s * vkp + c * vkq;
-        }
-      }
-  }
+  rc_jacobi3(S, V);
   int i0 = 0, i2 = 0;
   for (int i = 1; i < 3; ++i) {
     if (S[i][i] > S[i0][i0]) i0 = i;
@@ -645,6 +459,5 @@ __global__ void __launch_bounds__(ESS_POSE_THREADS) essential_pose_kernel(Essent
 #undef ES_A
 #undef ES_S
 #undef ES_D
-#undef ESS_CHAIN_OFF
 
 }  // namespace ltr

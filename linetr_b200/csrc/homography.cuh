@@ -34,7 +34,6 @@ constexpr int HG_REFIT_THREADS = 256;
 constexpr int HG_PT_BYTES = 16;         // shared bytes per point: x0, y0, x1, y1 fp32
 constexpr int HG_LN_BYTES = 56;         // per line: s0, s1 (4 fp32 each) and the pixel line through s1 (3 fp64)
 constexpr int HG_SMEM_MAX = 200 * 1024; // staging capacity of one pair (see hg_smem_bytes)
-constexpr int HG_JACOBI_SWEEPS = 32;
 constexpr double HG_FLT_EPS = 1.1920928955078125e-07;
 
 struct HomographyArgs {
@@ -354,47 +353,6 @@ __device__ __forceinline__ int2 hg_mark(const HgStage& st, const HgPair& sp, con
   int2 t = make_int2(0, 0);
   for (int i = 0; i < NT / 32; ++i) { t.x += red[i].x; t.y += red[i].y; }
   return t;
-}
-
-// Eigenvector of the smallest eigenvalue of the symmetric 9x9 M (cyclic Jacobi; M is destroyed).
-__device__ __noinline__ void hg_smallest_eigvec(double* M, double* h) {
-  double V[81];
-  for (int i = 0; i < 81; ++i) V[i] = (i % 10 == 0) ? 1.0 : 0.0;
-  double fro = 0.0;
-  for (int i = 0; i < 81; ++i) fro += M[i] * M[i];
-  for (int sweep = 0; sweep < HG_JACOBI_SWEEPS; ++sweep) {
-    double off = 0.0;
-    for (int i = 0; i < 9; ++i)
-      for (int j = i + 1; j < 9; ++j) off += M[9 * i + j] * M[9 * i + j];
-    if (!(off > 1e-32 * fro)) break;
-    for (int p = 0; p < 8; ++p)
-      for (int q = p + 1; q < 9; ++q) {
-        const double apq = M[9 * p + q];
-        if (apq == 0.0) continue;
-        const double theta = (M[9 * q + q] - M[9 * p + p]) / (2.0 * apq);
-        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-        for (int k = 0; k < 9; ++k) {
-          const double mkp = M[9 * k + p], mkq = M[9 * k + q];
-          M[9 * k + p] = c * mkp - s * mkq;
-          M[9 * k + q] = s * mkp + c * mkq;
-        }
-        for (int k = 0; k < 9; ++k) {
-          const double mpk = M[9 * p + k], mqk = M[9 * q + k];
-          M[9 * p + k] = c * mpk - s * mqk;
-          M[9 * q + k] = s * mpk + c * mqk;
-        }
-        for (int k = 0; k < 9; ++k) {
-          const double vkp = V[9 * k + p], vkq = V[9 * k + q];
-          V[9 * k + p] = c * vkp - s * vkq;
-          V[9 * k + q] = s * vkp + c * vkq;
-        }
-      }
-  }
-  int m = 0;
-  for (int i = 1; i < 9; ++i)
-    if (M[10 * i] < M[10 * m]) m = i;
-  for (int k = 0; k < 9; ++k) h[k] = V[9 * k + m];
 }
 
 __global__ void __launch_bounds__(HG_REFIT_THREADS) homography_refit_kernel(HomographyArgs a) {

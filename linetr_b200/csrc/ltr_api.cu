@@ -23,6 +23,7 @@
 #include "homography.cuh"
 #include "warp.cuh"
 #include "essential.cuh"
+#include "fundamental.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -42,7 +43,8 @@ const char* kernel_class_name(int kc) {
   static const char* names[KC_COUNT] = {"small_mlp", "linear", "img_convert", "sig_attention", "final_norm",
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
-                                         "triplet", "homography", "warp", "essential", "photometric"};
+                                         "triplet", "homography", "warp", "essential", "photometric",
+                                         "fundamental"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1276,6 +1278,51 @@ int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, in
   }
   LaunchScope ls(KC_ESSENTIAL, s);
   LTR_CUDA_TRY(launch_pdl(essential_pose_kernel, dim3(in->n_pairs), dim3(ESS_POSE_THREADS), (size_t)smem, s, a));
+  return LTR_OK;
+}
+
+int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_fundamental: null argument");
+  if (in->n_pairs < 0 || in->max_rows_p < 0) return set_error(LTR_E_INVALID, "ltr_fundamental: negative count");
+  if (in->n_hypotheses < 1 || cdiv(in->n_hypotheses, FM_THREADS) > 65535)
+    return set_error(LTR_E_INVALID, "ltr_fundamental: n_hypotheses must be in [1, 65535 * 128]");
+  if (!(in->thresh > 0.0) || !std::isfinite(in->thresh)) return set_error(LTR_E_INVALID, "ltr_fundamental: thresh must be > 0");
+  if (!(in->min_overlap >= 0.0 && in->min_overlap <= 1.0))
+    return set_error(LTR_E_INVALID, "ltr_fundamental: min_overlap must be in [0, 1]");
+  const long long smem = fm_smem_bytes(in->max_rows_p, true);
+  if (smem > FM_SMEM_MAX)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_fundamental: a pair's correspondences need " + std::to_string(smem) +
+                                            " bytes of shared memory (18 per keypoint row), over " +
+                                            std::to_string(FM_SMEM_MAX));
+  if (in->n_pairs == 0) return LTR_OK;
+  if (!out->F || !out->valid || !out->refit || !out->n_inliers || !out->n_lines_consistent || !out->hypothesis ||
+      !out->hypothesis_inliers || !out->key)
+    return set_error(LTR_E_INVALID, "ltr_fundamental: null output");
+  if (!in->cu_p || !in->cu_l) return set_error(LTR_E_INVALID, "ltr_fundamental: null offsets");
+  if (in->max_rows_p > 0 && (!in->matches_p || !out->inliers_p || !in->pts0 || !in->pts1 || !in->pts_off0 ||
+                             !in->pts_off1 || !in->n_pts1))
+    return set_error(LTR_E_INVALID, "ltr_fundamental: null keypoint pools or matches");
+  if (in->max_rows_l > 0 && (!in->matches_l || !out->lines_consistent || !in->segs0 || !in->segs1 || !in->seg_off0 ||
+                             !in->seg_off1 || !in->n_segs1))
+    return set_error(LTR_E_INVALID, "ltr_fundamental: null segment pools or line matches");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  FundamentalArgs a{in->pts0, in->pts1, in->pts_off0, in->pts_off1, in->n_pts1, in->matches_p, in->cu_p,
+                    in->segs0, in->segs1, in->seg_off0, in->seg_off1, in->n_segs1, in->matches_l, in->cu_l,
+                    in->max_rows_p, in->thresh * in->thresh, in->min_overlap, in->n_hypotheses,
+                    (unsigned long long)in->seed, reinterpret_cast<unsigned long long*>(out->key), out->F, out->valid,
+                    out->inliers_p, out->lines_consistent, out->refit, out->n_inliers, out->n_lines_consistent,
+                    out->hypothesis, out->hypothesis_inliers};
+  LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_pairs, s));
+  LTR_CUDA_TRY(ensure_dynamic_smem(fundamental_hyp_kernel, FM_SMEM_MAX));
+  LTR_CUDA_TRY(ensure_dynamic_smem(fundamental_fit_kernel, FM_SMEM_MAX));
+  {
+    LaunchScope ls(KC_FUNDAMENTAL, s);
+    LTR_CUDA_TRY(launch_pdl(fundamental_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, FM_THREADS)),
+                            dim3(FM_THREADS), (size_t)fm_smem_bytes(in->max_rows_p, false), s, a));
+  }
+  LaunchScope ls(KC_FUNDAMENTAL, s);
+  LTR_CUDA_TRY(launch_pdl(fundamental_fit_kernel, dim3(in->n_pairs), dim3(FM_FIT_THREADS), (size_t)smem, s, a));
   return LTR_OK;
 }
 

@@ -44,6 +44,24 @@ the most inliers, then the lowest k, then the lowest j.  E is scaled to unit Fro
 of its four (R, t) candidates the one with the most inliers in front of both cameras wins (depths from the 2 x 2 normal
 equations of d1 x1 = d0 R x0 + t in (0, dist_thresh)).  No refit.  Fewer than 5 correspondences or no finite E makes
 the pair invalid.
+
+    estimate_fundamentals(res, thresh=3.0, n_hypotheses=2048, seed=0, min_overlap=0.5) -> FundamentalResult
+        one `ltr_fundamental` call for every pair of a `match_images` / `match_sets` result, for pairs without
+        intrinsics; device outputs, no synchronisation
+    ransac_fundamental_host(kpts0, kpts1, matches_p, klines0, klines1, matches_l, pair=0, ...) -> dict
+        the same model for one pair in numpy: everything up to the winner is the kernels' operations in the kernels'
+        order; the refit uses np.linalg.eigh / svd
+
+The fundamental-matrix model (DESIGN.md "Fundamental matrices", include/linetr_b200.h `ltr_fundamental`): x1^T F x0 = 0
+in pixels.  The correspondences are the pair's matched side-0 keypoints in row order with their partners, normalised
+per side as the homography's points.  Hypothesis k draws 7 distinct correspondences (`draw_samples(..., size=7)`) and
+solves them with the seven-point method: the null basis F1, F2 of the 7 epipolar rows (the essential solver's QR), the
+cubic det(F2 + a (F1 - F2)), its real roots by `sturm_roots`; solution j is real root j, denormalised and scaled to
+unit Frobenius norm (largest |entry| positive).  A row is an inlier iff cv2's FM error (the larger squared distance to
+the two epipolar lines) is below thresh^2.  The winner has the most inliers, then the lowest k, then the lowest j; with
+at least 8 inliers it is refitted by the normalised eight-point method (rank 2 through the SVD), kept iff the refit has
+at least as many inliers.  Matched key lines are then checked against the kept F (`lines_consistent`): the epipolar
+band of each segment must overlap its partner by at least min_overlap of the shorter extent, on both sides.
 """
 from __future__ import annotations
 
@@ -451,14 +469,15 @@ def _pmul(a, b):
 
 
 def _null_basis(q):
-    """Null-space basis of the 5 epipolar rows of each sample: q [K, 5, 4] normalised (a0, b0, a1, b1) -> (basis
-    [K, 4, 9] = Q e5 .. Q e8 of the Householder QR of the 9 x 5 transpose, ok [K])."""
-    K = q.shape[0]
+    """Null-space basis of the S epipolar rows of each sample (S = 5 for an essential matrix, 7 for a fundamental
+    matrix): q [K, S, 4] normalised (a0, b0, a1, b1) -> (basis [K, 9 - S, 9] = Q e_S .. Q e_8 of the Householder QR of
+    the 9 x S transpose, ok [K]) (csrc/ransac_common.cuh rc_null_basis)."""
+    K, S = q.shape[0], q.shape[1]
     a0, b0, a1, b1 = (q[:, :, i] for i in range(4))
-    M = np.stack([a1 * a0, a1 * b0, a1, b1 * a0, b1 * b0, b1, a0, b0, np.ones_like(a0)], 1)   # [K, 9, 5]
+    M = np.stack([a1 * a0, a1 * b0, a1, b1 * a0, b1 * b0, b1, a0, b0, np.ones_like(a0)], 1)   # [K, 9, S]
     ok = np.ones(K, dtype=bool)
     vs, betas, nrm0 = [], [], None
-    for c in range(5):
+    for c in range(S):
         acc = np.zeros(K)
         for i in range(c, 9):
             acc = acc + M[:, i, c] * M[:, i, c]
@@ -475,7 +494,7 @@ def _null_basis(q):
         for i in range(9 - c):
             vtv = vtv + v[:, i] * v[:, i]
         beta = np.where(vtv > 0, 2.0 / np.where(vtv > 0, vtv, 1.0), 0.0)
-        for j in range(c + 1, 5):
+        for j in range(c + 1, S):
             s = np.zeros(K)
             for i in range(9 - c):
                 s = s + v[:, i] * M[:, c + i, j]
@@ -484,11 +503,11 @@ def _null_basis(q):
                 M[:, c + i, j] = M[:, c + i, j] - g * v[:, i]
         vs.append(v)
         betas.append(beta)
-    basis = np.zeros((K, 4, 9))
-    for b in range(4):
+    basis = np.zeros((K, 9 - S, 9))
+    for b in range(9 - S):
         y = np.zeros((K, 9))
-        y[:, 5 + b] = 1.0
-        for c in range(4, -1, -1):
+        y[:, S + b] = 1.0
+        for c in range(S - 1, -1, -1):
             v = vs[c]
             s = np.zeros(K)
             for i in range(9 - c):
@@ -883,6 +902,288 @@ def estimate_poses(res, K0, K1, thresh=1.0, n_hypotheses=1024, seed=0, dist_thre
                    hypothesis=out.hypothesis, hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh,
                    dist_thresh=dist_thresh, n_hypotheses=n_hypotheses, seed=seed)
     out.valid = out.valid.view(torch.bool)
+    return out
+
+
+# ------------------------------------------------------------------ fundamental matrices: the model in numpy
+# DESIGN.md "Fundamental matrices"; the kernels are csrc/fundamental.cuh.  As for the essential model, every step up to
+# the winner is one IEEE fp64 operation per numpy elementwise operation, in the kernels' order.
+FM_SAMPLE = 7
+FM_MAX_SOLUTIONS = 3
+FM_MIN_REFIT = 8          # winner inliers needed for the eight-point refit
+# One pair's staging in shared memory (ltr_fundamental's capacity): 16 bytes of fp32 pixel coordinates plus two inlier
+# flag bytes per keypoint row.
+SMEM_PER_ROW_F = 18
+
+
+def fundamental_cubic(basis):
+    """det(F2 + a (F1 - F2)) of null bases [K, 2, 9] (F1, F2 row-major) as ascending coefficients [K, 4], expanded
+    along the first row: (c0 (c4 c8 - c5 c7) - c1 (c3 c8 - c5 c6)) + c2 (c3 c7 - c4 c6), with c_i = [F2_i, F1_i - F2_i]
+    the entries as polynomials in a.  -> (coefficients, F2 [K, 9], F1 - F2 [K, 9])."""
+    F1, F2 = basis[:, 0], basis[:, 1]
+    D = F1 - F2
+    c = [np.stack([F2[:, i], D[:, i]], 1) for i in range(9)]
+    t0 = _pmul(c[0], _pmul(c[4], c[8]) - _pmul(c[5], c[7]))
+    t1 = _pmul(c[1], _pmul(c[3], c[8]) - _pmul(c[5], c[6]))
+    t2 = _pmul(c[2], _pmul(c[3], c[7]) - _pmul(c[4], c[6]))
+    return (t0 - t1) + t2, F2, D
+
+
+def fundamental_solutions(q):
+    """The seven-point solver (DESIGN.md "Fundamental matrices") on samples q [K, 7, 4] of normalised correspondences
+    (x0, y0, x1, y1): -> (F^ [K, 3, 9] row-major in normalised coordinates, ok [K, 3]); solution j of sample k is
+    F2 + a_j (F1 - F2) for real root a_j (ascending) of the cubic.  The solution at a = infinity (F1 - F2 singular on
+    its own) is not returned."""
+    q = np.asarray(q, dtype=np.float64)
+    K = q.shape[0]
+    with np.errstate(all="ignore"):
+        basis, ok = _null_basis(q)
+        cubic, F2, D = fundamental_cubic(basis)
+        p = np.zeros((K, 11))
+        p[:, :4] = cubic
+        roots, _ = sturm_roots(p)
+        a = roots[:, :FM_MAX_SOLUTIONS]
+        F = F2[:, None, :] + np.where(np.isnan(a), 0.0, a)[..., None] * D[:, None, :]
+    return F, ok[:, None] & ~np.isnan(a) & np.isfinite(F).all(-1)
+
+
+def _fundamental_to_pixels(f, nm: _Norm):
+    """Normalised F^ [..., 9] -> pixel F = T1^T F^ T0 scaled to unit Frobenius norm, its largest |entry| (the first on a
+    tie) positive; ok is False for a zero or non-finite norm."""
+    t0x, t0y = -(nm.c0x * nm.i0), -(nm.c0y * nm.i0)
+    t1x, t1y = -(nm.c1x * nm.i1), -(nm.c1y * nm.i1)
+    M, G = np.empty_like(f), np.empty_like(f)
+    for i in range(3):
+        M[..., 3 * i] = f[..., 3 * i] * nm.i0
+        M[..., 3 * i + 1] = f[..., 3 * i + 1] * nm.i0
+        M[..., 3 * i + 2] = (f[..., 3 * i] * t0x + f[..., 3 * i + 1] * t0y) + f[..., 3 * i + 2]
+    for j in range(3):
+        G[..., j] = M[..., j] * nm.i1
+        G[..., 3 + j] = M[..., 3 + j] * nm.i1
+        G[..., 6 + j] = (t1x * M[..., j] + t1y * M[..., 3 + j]) + M[..., 6 + j]
+    s = np.zeros(f.shape[:-1])
+    for j in range(9):
+        s = s + G[..., j] * G[..., j]
+    with np.errstate(all="ignore"):
+        nrm = np.sqrt(s)
+        ok = (nrm > 0) & np.isfinite(nrm)
+        F = G / np.where(ok, nrm, 1.0)[..., None]
+    neg = np.take_along_axis(G, np.argmax(np.abs(G), -1)[..., None], -1) < 0
+    return np.where(neg, -F, F), ok
+
+
+def _fm_terms(F, pts):
+    """x1^T F x0, |(F x0)_xy|^2 and |(F^T x1)_xy|^2 of pixel F [M, 9] on correspondences pts [n, 4]: [M, n] each."""
+    x0, y0, x1, y1 = (np.asarray(pts[:, i], dtype=np.float64)[None, :] for i in range(4))
+    f = [F[:, i:i + 1] for i in range(9)]
+    u0 = (f[0] * x0 + f[1] * y0) + f[2]
+    u1 = (f[3] * x0 + f[4] * y0) + f[5]
+    u2 = (f[6] * x0 + f[7] * y0) + f[8]
+    w0 = (f[0] * x1 + f[3] * y1) + f[6]
+    w1 = (f[1] * x1 + f[4] * y1) + f[7]
+    return (x1 * u0 + y1 * u1) + u2, u0 * u0 + u1 * u1, w0 * w0 + w1 * w1
+
+
+def fundamental_inliers(F, pts, t2, chunk=512):
+    """Inlier flags [M, n] of pixel F [M, 9] on correspondences pts [n, 4] (x0, y0, x1, y1): cv2's FM error below t2,
+    evaluated as (x1^T F x0)^2 < t2 min(|(F x0)_xy|^2, |(F^T x1)_xy|^2); a zero line normal is an outlier."""
+    F = np.asarray(F, dtype=np.float64).reshape(-1, 9)
+    out = np.empty((F.shape[0], len(pts)), dtype=bool)
+    with np.errstate(all="ignore"):
+        for s in range(0, F.shape[0], chunk):
+            num, a, b = _fm_terms(F[s:s + chunk], pts)
+            m = np.where(a < b, a, b)
+            out[s:s + chunk] = (m > 0) & (num * num < t2 * m)
+    return out
+
+
+def fundamental_error(F, pts):
+    """cv2's FM error [n] of one pixel F [3, 3] on correspondences pts [n, 4]: the larger squared distance of x1 to the
+    epipolar line F x0 and of x0 to F^T x1, in pixels^2."""
+    num, a, b = _fm_terms(np.asarray(F, dtype=np.float64).reshape(1, 9), pts)
+    with np.errstate(all="ignore"):
+        return np.maximum(num * num / a, num * num / b)[0]
+
+
+def _side_ratio(la, lb, px, py, qx, qy):
+    """Overlap ratio of one side: the lines la, lb (3 arrays each) cut the line through (p, q) at positions ta, tb (p at
+    0, q at 1) -> |[min, max] n [0, 1]| / min(max - min, 1), NaN where the side cannot reject (an intersection with
+    |w| <= FLT_EPSILON |X|, or ta == tb)."""
+    l0, l1, l2 = py - qy, qx - px, px * qy - qx * py
+    dx, dy = qx - px, qy - py
+    len2 = dx * dx + dy * dy
+    ok, t = np.ones(px.shape, dtype=bool), []
+    for m in (la, lb):
+        X0, X1, X2 = m[1] * l2 - m[2] * l1, m[2] * l0 - m[0] * l2, m[0] * l1 - m[1] * l0
+        nrm = np.sqrt((X0 * X0 + X1 * X1) + X2 * X2)
+        ok &= np.abs(X2) > FLT_EPSILON * nrm
+        x, y = X0 / X2, X1 / X2
+        t.append(((x - px) * dx + (y - py) * dy) / len2)
+    lo, hi = np.where(t[0] < t[1], t[0], t[1]), np.where(t[0] < t[1], t[1], t[0])
+    ok &= hi > lo
+    a, b = np.where(lo > 0, lo, 0.0), np.where(hi < 1, hi, 1.0)
+    ov = np.where(b > a, b - a, 0.0)
+    span = hi - lo
+    return np.where(ok, ov / np.where(span < 1, span, 1.0), np.nan)
+
+
+def line_overlap_ratios(F, seg0, seg1):
+    """The epipolar overlap ratios of matched key-line pairs under pixel F [3, 3] (x1^T F x0 = 0): seg0 / seg1 [m, 2, 2]
+    (start xy, end xy; used as float32).  -> (ratio in image 1 of F a0, F b0 against s1, ratio in image 0 of F^T a1,
+    F^T b1 against s0), [m] each, NaN where that side cannot reject (DESIGN.md "Fundamental matrices")."""
+    F = np.asarray(F, dtype=np.float64).reshape(9)
+    s0 = np.asarray(seg0, dtype=np.float32).reshape(-1, 4).astype(np.float64)
+    s1 = np.asarray(seg1, dtype=np.float32).reshape(-1, 4).astype(np.float64)
+    a0x, a0y, b0x, b0y = (s0[:, i] for i in range(4))
+    a1x, a1y, b1x, b1y = (s1[:, i] for i in range(4))
+    with np.errstate(all="ignore"):
+        img1 = [[(F[3 * r] * x + F[3 * r + 1] * y) + F[3 * r + 2] for r in range(3)] for x, y in ((a0x, a0y), (b0x, b0y))]
+        r1 = _side_ratio(img1[0], img1[1], a1x, a1y, b1x, b1y)
+        img0 = [[(F[c] * x + F[3 + c] * y) + F[6 + c] for c in range(3)] for x, y in ((a1x, a1y), (b1x, b1y))]
+        r0 = _side_ratio(img0[0], img0[1], a0x, a0y, b0x, b0y)
+    return r1, r0
+
+
+def lines_consistent(F, seg0, seg1, min_overlap=0.5):
+    """The epipolar check of matched key-line pairs [m]: True iff no side's overlap ratio (`line_overlap_ratios`) is
+    below min_overlap."""
+    r1, r0 = line_overlap_ratios(F, seg0, seg1)
+    return ~(r1 < min_overlap) & ~(r0 < min_overlap)
+
+
+def _epipolar_rows(q):
+    """The normalised epipolar rows (x1 x0, x1 y0, x1, y1 x0, y1 y0, y1, x0, y0, 1) of q [n, 4]: [n, 9]."""
+    x0, y0, x1, y1 = (q[:, i] for i in range(4))
+    return np.stack([x1 * x0, x1 * y0, x1, y1 * x0, y1 * y0, y1, x0, y0, np.ones_like(x0)], 1)
+
+
+def ransac_fundamental_host(kpts0, kpts1, matches_p, klines0=None, klines1=None, matches_l=None, pair=0, thresh=3.0,
+                            n_hypotheses=2048, seed=0, min_overlap=0.5) -> dict:
+    """The fundamental-matrix estimator's model for one pair in numpy (DESIGN.md "Fundamental matrices").  kpts [N, 2]
+    and klines [K, 2, 2] are used as float32; matches_p [N0] / matches_l [K0]: local side-1 index or -1 per side-0 row;
+    `pair` is the pair's index in the batch (it seeds the samples).  Everything up to the winner is the kernels'
+    operations in the kernels' order (the winning sample, root and inlier count are the same bits); the refit uses
+    np.linalg.eigh / svd instead of the kernels' Jacobi solves.  Returns F [3, 3] (pixels, unit Frobenius norm, NaN when
+    invalid), valid, inliers_p uint8 [N0], lines_consistent uint8 [K0] (aligned with the match rows), n_inliers,
+    n_lines_consistent, hypothesis (3 k + j of the winning sample k and root j, or -1), hypothesis_inliers,
+    F_hypothesis (the winning solution) and refit (whether the eight-point refit was kept)."""
+    l0 = np.zeros((0, 2, 2), np.float32) if klines0 is None else klines0
+    l1 = np.zeros((0, 2, 2), np.float32) if klines1 is None else klines1
+    ml = np.zeros(0, np.int64) if matches_l is None else matches_l
+    pts, _, _, rp, _ = _correspondences(kpts0, kpts1, matches_p, l0, l1, ml, True, False)
+    ml = np.asarray(ml, dtype=np.int64).reshape(-1)
+    out = dict(F=np.full((3, 3), np.nan), valid=False, inliers_p=np.zeros(len(np.ravel(matches_p)), dtype=np.uint8),
+               lines_consistent=np.zeros(len(ml), dtype=np.uint8), n_inliers=0, n_lines_consistent=0, hypothesis=-1,
+               hypothesis_inliers=0, F_hypothesis=np.full((3, 3), np.nan), refit=False)
+    n = len(pts)
+    if n < FM_SAMPLE:
+        return out
+    t2 = float(thresh) * float(thresh)
+    e = np.zeros((0, 2, 2), np.float32)
+    nm = _normalisation(pts, e, e)
+    f = lambda a: np.asarray(a, dtype=np.float64)
+    q = np.stack([(f(pts[:, 0]) - nm.c0x) * nm.i0, (f(pts[:, 1]) - nm.c0y) * nm.i0,
+                  (f(pts[:, 2]) - nm.c1x) * nm.i1, (f(pts[:, 3]) - nm.c1y) * nm.i1], 1)
+    idx, ok = draw_samples(seed, pair, n_hypotheses, n, FM_SAMPLE)
+    Fh, okf = fundamental_solutions(q[np.maximum(idx, 0)])
+    Fp, okp = _fundamental_to_pixels(Fh, nm)
+    flat = np.flatnonzero((okf & okp & ok[:, None]).reshape(-1))
+    if not len(flat):
+        return out
+    cnt = fundamental_inliers(Fp.reshape(-1, 9)[flat], pts, t2).sum(1)
+    # the kernels' key: (count << 32) | ~(3 k + j); flat = 3 k + j
+    w = int(flat[np.lexsort((flat, -cnt))[0]])
+    F = Fp.reshape(-1, 9)[w]
+    fl = fundamental_inliers(F, pts, t2)[0]
+    out.update(hypothesis=w, hypothesis_inliers=int(fl.sum()), F_hypothesis=F.reshape(3, 3).copy())
+    if fl.sum() >= FM_MIN_REFIT:
+        A = _epipolar_rows(q[fl])
+        _, V = np.linalg.eigh(A.T @ A)
+        U, S, Vt = np.linalg.svd(V[:, 0].reshape(3, 3))
+        S[2] = 0.0
+        Fr, okr = _fundamental_to_pixels(((U * S) @ Vt).reshape(1, 9), nm)
+        if okr[0]:
+            flr = fundamental_inliers(Fr[0], pts, t2)[0]
+            if flr.sum() >= fl.sum():
+                F, fl = Fr[0], flr
+                out["refit"] = True
+    out["inliers_p"][rp] = fl
+    k1 = np.asarray(l1, dtype=np.float32).reshape(-1, 2, 2)
+    rl = np.flatnonzero((ml >= 0) & (ml < len(k1)))
+    if len(rl):
+        k0 = np.asarray(l0, dtype=np.float32).reshape(-1, 2, 2)
+        out["lines_consistent"][rl] = lines_consistent(F, k0[rl], k1[ml[rl]], min_overlap)
+    out.update(F=F.reshape(3, 3).copy(), valid=True, n_inliers=int(fl.sum()),
+               n_lines_consistent=int(out["lines_consistent"].sum()))
+    return out
+
+
+# ------------------------------------------------------------------ fundamental matrices, batched on the GPU
+@dataclass
+class FundamentalResult:
+    """Result of `estimate_fundamentals` (device tensors; nothing has been waited for).
+
+    F float64 [P, 3, 3] (x1^T F x0 = 0 in pixels, unit Frobenius norm, NaN where not valid), valid bool [P], inliers_p
+    uint8 aligned with the result's matches_p (0 for unmatched rows), n_inliers int32 [P], hypothesis int32 [P] (3 k + j
+    of the winning sample k and root j, -1 when not valid), hypothesis_inliers int32 [P], refit bool [P] (F is the
+    eight-point refit), lines_consistent uint8 aligned with matches_l (1 where the line match passes the epipolar
+    check, 0 for unmatched rows and invalid pairs) and n_lines_consistent int32 [P]."""
+    F: torch.Tensor
+    valid: torch.Tensor
+    inliers_p: torch.Tensor
+    n_inliers: torch.Tensor
+    hypothesis: torch.Tensor
+    hypothesis_inliers: torch.Tensor
+    refit: torch.Tensor
+    lines_consistent: torch.Tensor
+    n_lines_consistent: torch.Tensor
+
+
+def estimate_fundamentals(res, thresh=3.0, n_hypotheses=2048, seed=0, min_overlap=0.5) -> FundamentalResult:
+    """Fundamental matrices (x1^T F x0 = 0 in pixels) of every pair of an `ImagePairMatches` (`match_images`,
+    `match_sets`) from its point matches (res.keypoints0 / keypoints1), for pairs without intrinsics: seven-point RANSAC
+    with an eight-point refit, and the epipolar check of its line matches (res.klines0 / klines1 as float32 segments),
+    in one `ltr_fundamental` call.  thresh in pixels (cv2's default 3); 2048 hypotheses leave about e^-16 chance of no
+    all-inlier sample at 50 % outliers; min_overlap is the line check's bound.  A planar scene is degenerate for F:
+    `estimate_homographies` is the tool there.  Host arrays go up in one pinned copy; the call never waits for the
+    device.  Raises LtrError (LTR_E_UNSUPPORTED) when a pair has more point match rows than one CTA can stage
+    (SMEM_PER_ROW_F bytes per row, SMEM_MAX in all)."""
+    P = res.n_pairs
+    dev = res.matches_p.device
+    op, ol = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
+    if int(n_hypotheses) < 1:
+        raise N.LtrError("estimate_fundamentals: n_hypotheses must be >= 1")
+    seg_rows = lambda k: np.asarray(k, dtype=np.float32).reshape(-1, 4)
+    pt_rows = lambda k: torch.as_tensor(k).to(device=dev, dtype=torch.float32).reshape(-1, 2)
+    s0, soff0, sn0 = _pool(res.klines0, P, seg_rows)
+    s1, soff1, sn1 = _pool(res.klines1, P, seg_rows)
+    p0, poff0, pn0 = _pool(res.keypoints0, P, pt_rows)
+    p1, poff1, pn1 = _pool(res.keypoints1, P, pt_rows)
+    if not (np.array_equal(sn0, np.diff(ol)) and np.array_equal(pn0, np.diff(op))):
+        raise N.LtrError("estimate_fundamentals: side-0 key lines / keypoints and the match offsets disagree")
+    cat_np = lambda parts: np.concatenate(parts) if parts else np.zeros((0, 4), dtype=np.float32)
+    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
+    i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
+    dv = _ops.stage({"segs0": cat_np(s0), "segs1": cat_np(s1), "seg_off0": soff0, "seg_off1": soff1, "n_segs1": sn1,
+                      "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1, "cu_p": i32(op), "cu_l": i32(ol)}, dev)
+    u8, i32d = dict(dtype=torch.uint8, device=dev), dict(dtype=torch.int32, device=dev)
+    out = FundamentalResult(torch.empty((P, 3, 3), dtype=torch.float64, device=dev), torch.empty(P, **u8),
+                            torch.empty(res.matches_p.shape[0], **u8), torch.empty(P, **i32d), torch.empty(P, **i32d),
+                            torch.empty(P, **i32d), torch.empty(P, **u8), torch.empty(res.matches_l.shape[0], **u8),
+                            torch.empty(P, **i32d))
+    key = torch.empty(P, dtype=torch.int64, device=dev)
+    mx = lambda a: int(np.diff(a).max(initial=0))
+    _ops.fundamental(P, pts0=cat_t(p0).contiguous(), pts1=cat_t(p1).contiguous(), pts_off0=dv["pts_off0"],
+                     pts_off1=dv["pts_off1"], n_pts1=dv["n_pts1"], matches_p=res.matches_p.contiguous(),
+                     cu_p=dv["cu_p"], max_rows_p=mx(op), segs0=dv["segs0"], segs1=dv["segs1"], seg_off0=dv["seg_off0"],
+                     seg_off1=dv["seg_off1"], n_segs1=dv["n_segs1"], matches_l=res.matches_l.contiguous(),
+                     cu_l=dv["cu_l"], max_rows_l=mx(ol), F=out.F, valid=out.valid, refit=out.refit,
+                     inliers_p=out.inliers_p, lines_consistent=out.lines_consistent, n_inliers=out.n_inliers,
+                     n_lines_consistent=out.n_lines_consistent, hypothesis=out.hypothesis,
+                     hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh, min_overlap=min_overlap,
+                     n_hypotheses=n_hypotheses, seed=seed)
+    out.valid = out.valid.view(torch.bool)
+    out.refit = out.refit.view(torch.bool)
     return out
 
 

@@ -489,3 +489,87 @@ def make_pose_set(seed: int, n_views: int, n_lines: int, n_points: int, K=DEFAUL
         v["keypoints"] = torch.from_numpy(np.clip(k, 0, [w - 1, h - 1]).astype(np.float32))
         v["descriptors"] = torch.from_numpy(np.ascontiguousarray(d.T))
     return base, np.stack(Ts)
+
+
+# ------------------------------------------------------------------ uncalibrated two-view inputs (fundamental matrices)
+def fundamental_from_pose(K0, K1, R, t) -> np.ndarray:
+    """F = K1^-T [t]x R K0^-1 (x1^T F x0 = 0 in pixels) scaled to unit Frobenius norm, its largest |entry| positive."""
+    t = np.asarray(t, dtype=np.float64)
+    tx = np.array([[0, -t[2], t[1]], [t[2], 0, -t[0]], [-t[1], t[0], 0]])
+    F = np.linalg.inv(K1).T @ tx @ np.asarray(R, dtype=np.float64) @ np.linalg.inv(K0)
+    F = F / np.linalg.norm(F)
+    return F if F.flat[int(np.argmax(np.abs(F)))] > 0 else -F
+
+
+def random_intrinsics(rng, w: int = 640, h: int = 480) -> np.ndarray:
+    """A pinhole K with focal lengths 0.6 to 1.6 times the image width (fx, fy within 5 % of each other) and the
+    principal point within 5 % of the image size of its centre."""
+    f = w * rng.uniform(0.6, 1.6)
+    c = np.array([(w - 1) / 2, (h - 1) / 2]) + rng.uniform(-0.05, 0.05, 2) * [w, h]
+    return np.array([[f, 0.0, c[0]], [0.0, f * rng.uniform(0.95, 1.05), c[1]], [0.0, 0.0, 1.0]])
+
+
+def make_fundamental_correspondences(seed: int, n_points: int, n_lines: int, noise_px: float = 0.5,
+                                     outlier_frac: float = 0.5, line_outlier_frac: float = 0.3, K0=None, K1=None,
+                                     w: int = 640, h: int = 480, min_outlier_px: float = 10.0,
+                                     min_epipolar_angle_deg: float = 30.0, min_length_px: float = 40.0):
+    """Point and line matches of an uncalibrated pair: two views with different intrinsics (random_intrinsics unless
+    K0 / K1 are given) and a random relative pose (up to 15 degrees, unit translation).  Points are
+    `make_pose_correspondences`': N(0, noise_px) on both sides, an outlier's side-1 keypoint moved min_outlier_px to
+    60 px across its epipolar line.  Lines are 3D segments (one end point at depth 2 to 8 in camera 0, 0.3 to 1.5 units
+    long) seen inside both images, at least min_length_px long and at least min_epipolar_angle_deg from the epipolar
+    line through their midpoint in both images (so end-point noise moves the epipolar intersections little), with
+    N(0, noise_px) per end point.  A line outlier's side-1 segment is moved along itself by 1.2 to 2.5 of its lengths,
+    off its epipolar band.  Row i of side 0 matches row i of side 1.  Returns dict kpts0 / kpts1 [n, 2], klines0 /
+    klines1 [m, 2, 2] float32, matches_p / matches_l int32, the true masks true_p / true_l, the true F (unit norm,
+    largest |entry| positive), K0, K1, R, t."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    K0 = random_intrinsics(rng, w, h) if K0 is None else np.asarray(K0, dtype=np.float64)
+    K1 = random_intrinsics(rng, w, h) if K1 is None else np.asarray(K1, dtype=np.float64)
+    R, t = random_pose(rng)
+    d = make_pose_correspondences(seed + 1, n_points, R, t, K0, K1, noise_px, outlier_frac, w, h, min_outlier_px)
+    F = fundamental_from_pose(K0, K1, R, t)
+
+    def angle_ok(F, a, b):   # the segments a -> b [m, 2] against the epipolar lines F^T / F of their partner images
+        mid = np.concatenate([(a + b) / 2, np.ones((len(a), 1))], 1)
+        l = mid @ F.T
+        n = l[:, :2] / np.maximum(np.linalg.norm(l[:, :2], axis=1, keepdims=True), 1e-300)
+        u = (b - a) / np.maximum(np.linalg.norm(b - a, axis=1, keepdims=True), 1e-300)
+        return np.abs((u * n).sum(1)) > np.sin(np.deg2rad(min_epipolar_angle_deg))
+
+    segs0, segs1 = np.zeros((0, 2, 2)), np.zeros((0, 2, 2))
+    for _ in range(200):
+        if len(segs0) >= n_lines:
+            break
+        m = 4 * (n_lines - len(segs0)) + 16
+        x = np.stack([rng.uniform(0, w - 1, m), rng.uniform(0, h - 1, m), np.ones(m)], 1)
+        Xa = (x @ np.linalg.inv(K0).T) * rng.uniform(2.0, 8.0, (m, 1))
+        u = rng.normal(size=(m, 3))
+        Xb = Xa + u / np.linalg.norm(u, axis=1, keepdims=True) * rng.uniform(0.3, 1.5, (m, 1))
+        keep = np.ones(m, dtype=bool)
+        ends = []
+        for Kc, Rc, tc in ((K0, np.eye(3), np.zeros(3)), (K1, R, t)):
+            e = []
+            for X in (Xa, Xb):
+                q = X @ Rc.T + tc
+                p = _project(Kc, q)
+                keep &= (q[:, 2] > 0.5) & (p[:, 0] >= 0) & (p[:, 0] <= w - 1) & (p[:, 1] >= 0) & (p[:, 1] <= h - 1)
+                e.append(p)
+            keep &= np.linalg.norm(e[1] - e[0], axis=1) >= min_length_px
+            ends.append(e)
+        with np.errstate(all="ignore"):
+            # side 1 against F x0 (epipolar lines of image 1 are F x0; those of image 0 are F^T x1)
+            keep &= angle_ok(F, ends[1][0], ends[1][1]) & angle_ok(F.T, ends[0][0], ends[0][1])
+        segs0 = np.concatenate([segs0, np.stack(ends[0], 1)[keep]])
+        segs1 = np.concatenate([segs1, np.stack(ends[1], 1)[keep]])
+    segs0, segs1 = segs0[:n_lines], segs1[:n_lines]
+    m = len(segs0)
+    out_l = rng.random(m) < line_outlier_frac
+    shift = (segs1[:, 1] - segs1[:, 0]) * (rng.uniform(1.2, 2.5, m) * rng.choice([-1.0, 1.0], m))[:, None]
+    segs1[out_l] += shift[out_l][:, None, :]
+    segs0 = segs0 + rng.normal(0, noise_px, segs0.shape)
+    segs1 = segs1 + rng.normal(0, noise_px, segs1.shape)
+    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+    d.update(klines0=f32(segs0), klines1=f32(segs1), matches_l=np.arange(m, dtype=np.int32), true_l=~out_l, F=F,
+             K0=K0, K1=K1, R=R, t=t)
+    return d
