@@ -32,6 +32,8 @@
  *                                 cv2.recoverPose per pair, batched.
  *   ltr_fundamental            <- cv2.findFundamentalMat(FM_RANSAC) per pair, batched, for pairs without intrinsics,
  *                                 with an epipolar check of the line matches.
+ *   ltr_absolute_pose          <- cv2.solvePnPRansac per query, batched, with the line matches scored and refined too
+ *                                 (PL-Loc's localization step).
  *   ltr_warp_pairs             <- cv2.warpPerspective of the grey and colour images + the eroded valid mask of the
  *                                 homography dataset builder (dataloaders/build_homography_dataset.py:164-184).
  *   ltr_photometric            <- imgPhotometric of the homography dataset builder (ImgAugTransform +
@@ -648,6 +650,81 @@ typedef struct {
 /* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments, LTR_E_UNSUPPORTED over
  * capacity) come before any launch.  n_pairs == 0 writes nothing. */
 int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* out, int32_t device, void* stream);
+
+/* Absolute pose of query images, as cv2.solvePnPRansac per query would localize them from 2D-3D point matches, with
+ * the line matches scored and refined too; DESIGN.md "Absolute pose" states the model:
+ *   - side 0 is the query, side 1 a database image with 3D: X1 rows (fp64 [*, 3]) are aligned with pair p's side-1
+ *     keypoints from x_off1[p], L1 rows (fp64 [*, 2, 3], the two end points) with its side-1 segments from l_off1[p];
+ *     a row with a non-finite coordinate has no 3D.  The pose maps world to query camera: X_cam = R X + t;
+ *   - group g is the run of pairs [groups[g], groups[g+1]), which share one side-0 (query) image; its correspondences
+ *     are its pairs' point rows in pair and row order (a side-0 keypoint row with a match in [0, n_x1[p]) whose 3D is
+ *     finite), then, with use_lines, its line rows (a side-0 segment row with a match in [0, n_l1[p]) whose two end
+ *     points are finite); query pixels are normalised as ((x - cx) / fx, (y - cy) / fy) with K0[g] (skew ignored);
+ *   - world coordinates are shifted by the midpoint c of the bounding box of the group's staged 3D coordinates;
+ *   - hypothesis k draws 3 distinct point rows with ltr_homography's hash and redraw rule (pair index = group index) and
+ *     solves them with Grunert's P3P in explicitly rounded fp64: the quartic in the distance ratio, its real roots by
+ *     a Sturm chain and bisection, positive distances only, R from the triads of the camera and world points,
+ *     t = P1 - R X1.  Up to 4 solutions j (real root j in ascending order); a sample whose world points are collinear
+ *     (cross-product norm <= 1e-10 times the product of the edge lengths) has none;
+ *   - a point is an inlier iff its depth is > 0 and its reprojection error through K0 is below thresh pixels; a line
+ *     iff both end points have depth > 0 and lie within thresh pixels of the infinite line through the query segment;
+ *     without use_lines only points are scored.  Lines never take part in sampling;
+ *   - the winner has the most inliers (points plus lines), then the lowest k, then the lowest j.  With at least 3
+ *     inliers it is refined by Levenberg-Marquardt over them (20 steps, R <- cay(w) R, t <- t + dt, damping 1e-3 times
+ *     0.1 after a step that lowers the cost and 10 after one that does not), kept iff it has at least as many inliers.
+ * A group with fewer than 3 point rows, no finite solution, or more match rows than max_rows_p / max_rows_l is
+ * invalid: R and t are NaN, no row is an inlier, hypothesis is -1.
+ *
+ * Capacity: one group's correspondences are staged in shared memory, 32 bytes per keypoint row over max_rows_p and 64
+ * per segment row over max_rows_l (with use_lines), at most 200 KiB.  Beyond that the call returns LTR_E_UNSUPPORTED
+ * before any launch.  K0 must be finite with fx, fy > 0. */
+typedef struct {
+  const float* pts0;              /* device [*, 2] query keypoint pool */
+  const int32_t* pts_off0;        /* device [n_pairs]: pair p's query keypoints start at pts0 row pts_off0[p] */
+  const int32_t* matches_p;       /* device: local side-1 index or -1 per query keypoint row */
+  const int32_t* cu_p;            /* device [n_pairs + 1]: pair p owns matches_p rows [cu_p[p], cu_p[p+1]) */
+  const double* X1;               /* device [*, 3] world points of the database keypoints */
+  const int32_t* x_off1;          /* device [n_pairs]: pair p's side-1 rows start at X1 row x_off1[p] */
+  const int32_t* n_x1;            /* device [n_pairs]: side-1 keypoints of pair p */
+  const float* segs0;             /* device [*, 2, 2] query segment pool (start xy, end xy) */
+  const int32_t* seg_off0;        /* device [n_pairs] */
+  const int32_t* matches_l;       /* device: local side-1 index or -1 per query segment row */
+  const int32_t* cu_l;            /* device [n_pairs + 1] */
+  const double* L1;               /* device [*, 2, 3] world end points of the database segments */
+  const int32_t* l_off1;          /* device [n_pairs] */
+  const int32_t* n_l1;            /* device [n_pairs] */
+  const int32_t* groups;          /* device [n_groups + 1]: pair offsets, non-decreasing from 0 to n_pairs */
+  const double* K0;               /* device [n_groups, 3, 3] query intrinsics */
+  int32_t n_pairs;
+  int32_t n_groups;
+  int32_t max_rows_p;             /* bound of every group's keypoint match rows; sizes the staging, a group over it is
+                                     invalid */
+  int32_t max_rows_l;             /* bound of every group's segment match rows */
+  double thresh;                  /* pixels (8: cv2.solvePnPRansac's default) */
+  int32_t n_hypotheses;           /* >= 1 (1024) */
+  uint64_t seed;
+  int32_t use_lines;              /* 0: score points only */
+} LtrAbsPoseInput;
+
+/* Outputs (device, caller-owned).  key [n_groups] is workspace (winning (count << 32) | ~(4 k + j), 0 = none). */
+typedef struct {
+  double* R;                      /* [n_groups, 3, 3] world -> query camera */
+  double* t;                      /* [n_groups, 3] */
+  uint8_t* valid;                 /* [n_groups] */
+  uint8_t* refit;                 /* [n_groups] 1 where the pose is the Levenberg-Marquardt refit */
+  uint8_t* inliers_p;             /* aligned with matches_p (0 for rows without a correspondence) */
+  uint8_t* inliers_l;             /* aligned with matches_l (0 for rows without a correspondence, and without use_lines) */
+  int32_t* n_inliers_p;           /* [n_groups] */
+  int32_t* n_inliers_l;           /* [n_groups] */
+  int32_t* hypothesis;            /* [n_groups] 4 k + j of the winning solution, -1 when invalid */
+  int32_t* hypothesis_inliers;    /* [n_groups] its inlier count (points and lines) */
+  uint64_t* key;
+} LtrAbsPoseOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments, LTR_E_UNSUPPORTED over
+ * capacity) come before any launch.  n_groups == 0 writes nothing.  Writes the masks of the rows of pairs in
+ * [groups[0], groups[n_groups]). */
+int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream);
 
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where

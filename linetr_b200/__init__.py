@@ -17,6 +17,9 @@ the reference's pose metrics:
 Fundamental matrices (geometry): seven-point RANSAC with an eight-point refit for uncalibrated pairs, and an epipolar
 check of the line matches, batched on the GPU:
     estimate_fundamentals
+Visual localization (localization): the absolute pose of query images from 2D-3D point and line matches (P3P RANSAC
+and a Levenberg-Marquardt refit), batched on the GPU, and the localization metrics:
+    estimate_absolute_poses, absolute_pose_errors, localization_recall, lift_to_3d
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
@@ -57,6 +60,11 @@ _LAZY = {
     "pose_auc": ("geometry", "pose_auc"),
     "pose_errors": ("geometry", "pose_errors"),
     "estimate_fundamentals": ("geometry", "estimate_fundamentals"),
+    "estimate_absolute_poses": ("localization", "estimate_absolute_poses"),
+    "AbsolutePoseResult": ("localization", "AbsolutePoseResult"),
+    "absolute_pose_errors": ("localization", "absolute_pose_errors"),
+    "localization_recall": ("localization", "localization_recall"),
+    "lift_to_3d": ("localization", "lift_to_3d"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

@@ -167,6 +167,22 @@ class LtrFundamentalOutput(C.Structure):
                 ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
 
 
+class LtrAbsPoseInput(C.Structure):
+    _fields_ = [("pts0", C.c_void_p), ("pts_off0", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p),
+                ("X1", C.c_void_p), ("x_off1", C.c_void_p), ("n_x1", C.c_void_p), ("segs0", C.c_void_p),
+                ("seg_off0", C.c_void_p), ("matches_l", C.c_void_p), ("cu_l", C.c_void_p), ("L1", C.c_void_p),
+                ("l_off1", C.c_void_p), ("n_l1", C.c_void_p), ("groups", C.c_void_p), ("K0", C.c_void_p),
+                ("n_pairs", C.c_int32), ("n_groups", C.c_int32), ("max_rows_p", C.c_int32), ("max_rows_l", C.c_int32),
+                ("thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64), ("use_lines", C.c_int32)]
+
+
+class LtrAbsPoseOutput(C.Structure):
+    _fields_ = [("R", C.c_void_p), ("t", C.c_void_p), ("valid", C.c_void_p), ("refit", C.c_void_p),
+                ("inliers_p", C.c_void_p), ("inliers_l", C.c_void_p), ("n_inliers_p", C.c_void_p),
+                ("n_inliers_l", C.c_void_p), ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p),
+                ("key", C.c_void_p)]
+
+
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
 # {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
 # of them, and each entry against its C prototype)
@@ -193,6 +209,7 @@ PROTOTYPES = {
     "ltr_homography": (C.c_int, [_ptr(LtrHomographyInput), _ptr(LtrHomographyOutput), _I32, _P]),
     "ltr_essential": (C.c_int, [_ptr(LtrEssentialInput), _ptr(LtrEssentialOutput), _I32, _P]),
     "ltr_fundamental": (C.c_int, [_ptr(LtrFundamentalInput), _ptr(LtrFundamentalOutput), _I32, _P]),
+    "ltr_absolute_pose": (C.c_int, [_ptr(LtrAbsPoseInput), _ptr(LtrAbsPoseOutput), _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),

@@ -508,6 +508,39 @@ def fundamental(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, c
     _call("ltr_fundamental", dev, C.byref(inp), C.byref(out))
 
 
+def absolute_pose(n_pairs, n_groups, *, pts0, pts_off0, matches_p, cu_p, X1, x_off1, n_x1, segs0, seg_off0, matches_l,
+                  cu_l, L1, l_off1, n_l1, groups, K0, max_rows_p, max_rows_l, R, t, valid, refit, inliers_p, inliers_l,
+                  n_inliers_p, n_inliers_l, hypothesis, hypothesis_inliers, key, thresh=8.0, n_hypotheses=1024, seed=0,
+                  use_lines=True):
+    """ltr_absolute_pose into caller-allocated outputs: query keypoint pool [*,2] / segment pool [*,2,2] fp32 with
+    per-pair first rows, world points X1 [*,3] / end points L1 [*,2,3] fp64 with per-pair first rows and counts int32
+    [P], match rows int32 with offsets cu_p / cu_l [P+1], group offsets int32 [G+1], K0 fp64 [G,3,3]; R [G,3,3] / t
+    [G,3] fp64, valid / refit [G] uint8, inliers_p / inliers_l uint8 aligned with the match rows, counts / hypothesis
+    int32 [G], key [G] int64 workspace."""
+    _req_cuda(R, "R")
+    dev = R.device
+    _check_tensors("absolute_pose", dev, (
+        ("pts0", pts0, torch.float32), ("pts_off0", pts_off0, torch.int32), ("matches_p", matches_p, torch.int32),
+        ("cu_p", cu_p, torch.int32), ("X1", X1, torch.float64), ("x_off1", x_off1, torch.int32),
+        ("n_x1", n_x1, torch.int32), ("segs0", segs0, torch.float32), ("seg_off0", seg_off0, torch.int32),
+        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("L1", L1, torch.float64),
+        ("l_off1", l_off1, torch.int32), ("n_l1", n_l1, torch.int32), ("groups", groups, torch.int32),
+        ("K0", K0, torch.float64), ("R", R, torch.float64), ("t", t, torch.float64), ("valid", valid, torch.uint8),
+        ("refit", refit, torch.uint8), ("inliers_p", inliers_p, torch.uint8), ("inliers_l", inliers_l, torch.uint8),
+        ("n_inliers_p", n_inliers_p, torch.int32), ("n_inliers_l", n_inliers_l, torch.int32),
+        ("hypothesis", hypothesis, torch.int32), ("hypothesis_inliers", hypothesis_inliers, torch.int32),
+        ("key", key, torch.int64)))
+    inp = _struct(N.LtrAbsPoseInput, pts0=pts0, pts_off0=pts_off0, matches_p=matches_p, cu_p=cu_p, X1=X1,
+                  x_off1=x_off1, n_x1=n_x1, segs0=segs0, seg_off0=seg_off0, matches_l=matches_l, cu_l=cu_l, L1=L1,
+                  l_off1=l_off1, n_l1=n_l1, groups=groups, K0=K0, n_pairs=int(n_pairs), n_groups=int(n_groups),
+                  max_rows_p=int(max_rows_p), max_rows_l=int(max_rows_l), thresh=float(thresh),
+                  n_hypotheses=int(n_hypotheses), seed=int(seed) & 0xFFFFFFFFFFFFFFFF, use_lines=int(bool(use_lines)))
+    out = _struct(N.LtrAbsPoseOutput, R=R, t=t, valid=valid, refit=refit, inliers_p=inliers_p, inliers_l=inliers_l,
+                  n_inliers_p=n_inliers_p, n_inliers_l=n_inliers_l, hypothesis=hypothesis,
+                  hypothesis_inliers=hypothesis_inliers, key=key)
+    _call("ltr_absolute_pose", dev, C.byref(inp), C.byref(out))
+
+
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
     """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
     (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""

@@ -46,6 +46,7 @@ enum KernelClass : int {
   KC_ESSENTIAL,
   KC_PHOTOMETRIC,
   KC_FUNDAMENTAL,
+  KC_ABSOLUTE_POSE,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

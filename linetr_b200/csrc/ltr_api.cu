@@ -24,6 +24,7 @@
 #include "warp.cuh"
 #include "essential.cuh"
 #include "fundamental.cuh"
+#include "absolute_pose.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -44,7 +45,7 @@ const char* kernel_class_name(int kc) {
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
-                                         "fundamental"};
+                                         "fundamental", "absolute_pose"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1323,6 +1324,51 @@ int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* o
   }
   LaunchScope ls(KC_FUNDAMENTAL, s);
   LTR_CUDA_TRY(launch_pdl(fundamental_fit_kernel, dim3(in->n_pairs), dim3(FM_FIT_THREADS), (size_t)smem, s, a));
+  return LTR_OK;
+}
+
+int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_absolute_pose: null argument");
+  if (in->n_pairs < 0 || in->n_groups < 0 || in->max_rows_p < 0 || in->max_rows_l < 0)
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: negative count");
+  if (in->n_hypotheses < 1 || cdiv(in->n_hypotheses, AP_THREADS) > 65535)
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: n_hypotheses must be in [1, 65535 * 128]");
+  if (!(in->thresh > 0.0) || !std::isfinite(in->thresh))
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: thresh must be finite and > 0");
+  const int rows_l = in->use_lines ? in->max_rows_l : 0;
+  const long long smem = ap_smem_bytes(in->max_rows_p, rows_l);
+  if (smem > AP_SMEM_MAX)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_absolute_pose: a group's correspondences need " + std::to_string(smem) +
+                                            " bytes of shared memory (32 per keypoint row, 64 per segment row), over " +
+                                            std::to_string(AP_SMEM_MAX));
+  if (in->n_groups == 0) return LTR_OK;
+  if (!out->R || !out->t || !out->valid || !out->refit || !out->n_inliers_p || !out->n_inliers_l || !out->hypothesis ||
+      !out->hypothesis_inliers || !out->key)
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null output");
+  if (!in->groups || !in->K0 || !in->cu_p || !in->cu_l || !out->inliers_p || !out->inliers_l)
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null groups, intrinsics, offsets or masks");
+  if (in->max_rows_p > 0 && (!in->pts0 || !in->pts_off0 || !in->matches_p || !in->X1 || !in->x_off1 || !in->n_x1))
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null keypoint pools, 3D points or matches");
+  if (rows_l > 0 && (!in->segs0 || !in->seg_off0 || !in->matches_l || !in->L1 || !in->l_off1 || !in->n_l1))
+    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null segment pools, 3D segments or line matches");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  AbsPoseArgs a{in->pts0, in->pts_off0, in->matches_p, in->cu_p, in->X1, in->x_off1, in->n_x1,
+                in->segs0, in->seg_off0, in->matches_l, in->cu_l, in->L1, in->l_off1, in->n_l1,
+                in->groups, in->K0, in->max_rows_p, rows_l, in->thresh * in->thresh, in->n_hypotheses,
+                (unsigned long long)in->seed, reinterpret_cast<unsigned long long*>(out->key), out->R, out->t,
+                out->valid, out->refit, out->inliers_p, out->inliers_l, out->n_inliers_p, out->n_inliers_l,
+                out->hypothesis, out->hypothesis_inliers};
+  LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_groups, s));
+  LTR_CUDA_TRY(ensure_dynamic_smem(abspose_hyp_kernel, AP_SMEM_MAX));
+  LTR_CUDA_TRY(ensure_dynamic_smem(abspose_fit_kernel, AP_SMEM_MAX));
+  {
+    LaunchScope ls(KC_ABSOLUTE_POSE, s);
+    LTR_CUDA_TRY(launch_pdl(abspose_hyp_kernel, dim3(in->n_groups, cdiv(in->n_hypotheses, AP_THREADS)),
+                            dim3(AP_THREADS), (size_t)smem, s, a));
+  }
+  LaunchScope ls(KC_ABSOLUTE_POSE, s);
+  LTR_CUDA_TRY(launch_pdl(abspose_fit_kernel, dim3(in->n_groups), dim3(AP_FIT_THREADS), (size_t)smem, s, a));
   return LTR_OK;
 }
 

@@ -1,7 +1,7 @@
-// RANSAC scaffolding shared by the homography (homography.cuh), essential-matrix (essential.cuh) and fundamental-matrix
-// (fundamental.cuh) estimators: the counter-based sample hash, the row-ordered compaction of a pair's match rows into
-// shared memory, the draw of one hypothesis' distinct correspondences (geometry.draw_samples restates it in numpy), and
-// the fp64 solver pieces: the null basis of a minimal sample's epipolar rows (Householder QR), the Sturm-chain root
+// RANSAC scaffolding shared by the homography (homography.cuh), essential-matrix (essential.cuh), fundamental-matrix
+// (fundamental.cuh) and absolute-pose (absolute_pose.cuh) estimators: the counter-based sample hash, the row-ordered
+// compaction of a pair's match rows into shared memory, the draw of one hypothesis' distinct correspondences
+// (geometry.draw_samples restates it in numpy), and the fp64 solver pieces: the null basis of a minimal sample's epipolar rows (Householder QR), the Sturm-chain root
 // finder (geometry.sturm_roots) and the cyclic Jacobi eigen-solvers of the refits and decompositions.
 #pragma once
 #include "common.cuh"
@@ -22,16 +22,16 @@ __device__ __forceinline__ unsigned long long hg_splitmix64(unsigned long long x
   return z ^ (z >> 31);
 }
 
-// Row-ordered compaction of the matched rows [b, e) of a match array: f(local row, match, compact index or -1) for
-// every row.  All threads of the block must call it.
-template <int NT, typename F>
-__device__ __forceinline__ int hg_compact(const int* __restrict__ match, int b, int e, int n1, int* warp_cnt, F f) {
+// Row-ordered compaction of the rows [b, e) of a match array whose match m passes keep(m): f(local row, match, compact
+// index or -1) for every row.  All threads of the block must call it.
+template <int NT, typename K, typename F>
+__device__ __forceinline__ int rc_compact_if(const int* __restrict__ match, int b, int e, int* warp_cnt, K keep, F f) {
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   int base = 0;
   for (int r0 = b; r0 < e; r0 += NT) {
     const int r = r0 + threadIdx.x;
     const int m = r < e ? match[r] : -1;
-    const bool ok = r < e && m >= 0 && m < n1;
+    const bool ok = r < e && keep(m);
     const unsigned bal = __ballot_sync(0xffffffffu, ok);
     if (lane == 0) warp_cnt[w] = __popc(bal);
     __syncthreads();
@@ -46,6 +46,12 @@ __device__ __forceinline__ int hg_compact(const int* __restrict__ match, int b, 
     base += tot;
   }
   return base;
+}
+
+// The matched rows (match in [0, n1)) of [b, e): rc_compact_if with that test.
+template <int NT, typename F>
+__device__ __forceinline__ int hg_compact(const int* __restrict__ match, int b, int e, int n1, int* warp_cnt, F f) {
+  return rc_compact_if<NT>(match, b, e, warp_cnt, [n1](int m) { return m >= 0 && m < n1; }, f);
 }
 
 // The S distinct correspondence indices of hypothesis k of pair p among n: s = splitmix64(seed + splitmix64(p << 32 |

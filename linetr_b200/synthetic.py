@@ -452,13 +452,15 @@ def make_pose_correspondences(seed: int, n: int, R, t, K0=DEFAULT_K, K1=DEFAULT_
 
 
 def make_pose_set(seed: int, n_views: int, n_lines: int, n_points: int, K=DEFAULT_K, w: int = 640, h: int = 480,
-                  max_angle_deg: float = 4.0, max_shift: float = 0.8, jitter_px: float = 0.3, map_noise: float = 0.02):
+                  max_angle_deg: float = 4.0, max_shift: float = 0.8, jitter_px: float = 0.3, map_noise: float = 0.02,
+                  return_points: bool = False):
     """n_views calibrated views (intrinsics K) of one 3D point cloud (image dicts as `make_image_set` returns): camera v
     has pose T[v] (world -> camera, [4, 4]): a rotation of up to max_angle_deg and a centre within max_shift of the
     origin, looking down +z at n_points points 4 to 8 units away, chosen so every view sees all of them.  Keypoints are
     the projections plus N(0, jitter_px); point descriptors are per 3D point plus map_noise, as `make_image_set` makes
     them; key lines and dense maps are `make_image_set`'s (line matches carry no two-view constraint for the pose).
-    Returns (views, T [V, 4, 4]); the pose of view i -> view j is T[j] @ inv(T[i])."""
+    Returns (views, T [V, 4, 4]); the pose of view i -> view j is T[j] @ inv(T[i]).  With return_points, also the
+    world points X [n_points, 3] (fp64): row i of every view's keypoints is the projection of X[i]."""
     import torch
     rng = np.random.Generator(np.random.PCG64(seed))
     K = np.asarray(K, dtype=np.float64)
@@ -488,7 +490,7 @@ def make_pose_set(seed: int, n_views: int, n_lines: int, n_points: int, K=DEFAUL
         d = _unit(desc + map_noise * rng.standard_normal(desc.shape).astype(np.float32))
         v["keypoints"] = torch.from_numpy(np.clip(k, 0, [w - 1, h - 1]).astype(np.float32))
         v["descriptors"] = torch.from_numpy(np.ascontiguousarray(d.T))
-    return base, np.stack(Ts)
+    return (base, np.stack(Ts), X) if return_points else (base, np.stack(Ts))
 
 
 # ------------------------------------------------------------------ uncalibrated two-view inputs (fundamental matrices)
@@ -573,3 +575,68 @@ def make_fundamental_correspondences(seed: int, n_points: int, n_lines: int, noi
     d.update(klines0=f32(segs0), klines1=f32(segs1), matches_l=np.arange(m, dtype=np.int32), true_l=~out_l, F=F,
              K0=K0, K1=K1, R=R, t=t)
     return d
+
+
+# ------------------------------------------------------------------ 2D-3D inputs (absolute pose)
+def random_rotation(rng) -> np.ndarray:
+    """A rotation drawn uniformly (QR of a Gaussian matrix, signs fixed, determinant +1)."""
+    Q, Rr = np.linalg.qr(rng.normal(size=(3, 3)))
+    Q = Q * np.sign(np.diag(Rr))
+    if np.linalg.det(Q) < 0:
+        Q[:, 0] = -Q[:, 0]
+    return Q
+
+
+def make_localization_correspondences(seed: int, n_points: int, n_lines: int, noise_px: float = 0.5,
+                                      outlier_frac: float = 0.5, line_outlier_frac: float = 0.3, K=DEFAULT_K,
+                                      w: int = 640, h: int = 480, min_outlier_px: float = 10.0,
+                                      min_length_px: float = 40.0, origin_scale: float = 10.0):
+    """2D-3D point and line matches of one query: a query camera with a uniformly random rotation and a centre within
+    origin_scale of the world origin (X_cam = R X + t), 3D points at depth 2 to 8 seen inside the image, and 3D segments
+    (0.3 to 1.5 units, both end points at depth > 0.5 and inside the image, at least min_length_px long in it).  Query
+    keypoints / segment end points are the projections plus N(0, noise_px) per coordinate.  A point outlier's keypoint
+    is moved min_outlier_px to 60 px off its projection in a random direction; a line outlier's query segment is moved
+    min_outlier_px to 60 px along its normal (both end points, so both are that far from the projected line).  Row i of
+    the query matches row i of the 3D arrays.  Returns dict kpts0 [n, 2] / klines0 [m, 2, 2] float32, points3d1 [n, 3]
+    / lines3d1 [m, 2, 3] fp64, matches_p / matches_l int32, the true masks true_p / true_l, R, t and K."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    K = np.asarray(K, dtype=np.float64)
+    Ki = np.linalg.inv(K)
+    R = random_rotation(rng)
+    centre = rng.uniform(-origin_scale, origin_scale, 3)
+    t = -R @ centre
+    to_world = lambda Xc: (Xc - t) @ R          # R^T (X_cam - t)
+    x = np.stack([rng.uniform(0, w - 1, n_points), rng.uniform(0, h - 1, n_points), np.ones(n_points)], 1)
+    Xc = (x @ Ki.T) * rng.uniform(2.0, 8.0, (n_points, 1))
+    kp = _project(K, Xc)
+    out_p = rng.random(n_points) < outlier_frac
+    ang = rng.uniform(0, 2 * np.pi, n_points)
+    mag = rng.uniform(min_outlier_px, max(60.0, min_outlier_px + 1), n_points)
+    kp[out_p] += (mag[:, None] * np.stack([np.cos(ang), np.sin(ang)], 1))[out_p]
+    kp += rng.normal(0, noise_px, kp.shape)
+    segs, ends = np.zeros((0, 2, 2)), np.zeros((0, 2, 3))
+    for _ in range(200):
+        if len(segs) >= n_lines:
+            break
+        m = 4 * (n_lines - len(segs)) + 16
+        xa = np.stack([rng.uniform(0, w - 1, m), rng.uniform(0, h - 1, m), np.ones(m)], 1)
+        A = (xa @ Ki.T) * rng.uniform(2.0, 8.0, (m, 1))
+        u = rng.normal(size=(m, 3))
+        B = A + u / np.linalg.norm(u, axis=1, keepdims=True) * rng.uniform(0.3, 1.5, (m, 1))
+        pa, pb = _project(K, A), _project(K, np.where(B[:, 2:] > 0, B, 1.0))
+        keep = (B[:, 2] > 0.5) & (pb[:, 0] >= 0) & (pb[:, 0] <= w - 1) & (pb[:, 1] >= 0) & (pb[:, 1] <= h - 1)
+        keep &= np.linalg.norm(pb - pa, axis=1) >= min_length_px
+        segs = np.concatenate([segs, np.stack([pa, pb], 1)[keep]])
+        ends = np.concatenate([ends, np.stack([A, B], 1)[keep]])
+    segs, ends = segs[:n_lines], ends[:n_lines]
+    m = len(segs)
+    out_l = rng.random(m) < line_outlier_frac
+    d = segs[:, 1] - segs[:, 0]
+    nrm = np.stack([-d[:, 1], d[:, 0]], 1) / np.maximum(np.linalg.norm(d, axis=1, keepdims=True), 1e-12)
+    shift = nrm * (rng.uniform(min_outlier_px, max(60.0, min_outlier_px + 1), m) * rng.choice([-1.0, 1.0], m))[:, None]
+    segs[out_l] += shift[out_l][:, None, :]
+    segs = segs + rng.normal(0, noise_px, segs.shape)
+    f32 = lambda a: np.ascontiguousarray(a, dtype=np.float32)
+    return {"kpts0": f32(kp), "points3d1": to_world(Xc), "matches_p": np.arange(n_points, dtype=np.int32),
+            "klines0": f32(segs.reshape(-1, 2, 2)), "lines3d1": to_world(ends.reshape(-1, 3)).reshape(-1, 2, 3),
+            "matches_l": np.arange(m, dtype=np.int32), "true_p": ~out_p, "true_l": ~out_l, "R": R, "t": t, "K": K}
