@@ -56,6 +56,27 @@ int ltr_debug_sturm_roots(const double* poly, int32_t n, double* roots, int32_t*
 int ltr_debug_essential_solve(const double* q, int32_t n, double* E, int32_t* root_index, int32_t* n_solutions,
                               int32_t device, void* stream);
 
+/* The fundamental-matrix estimator's seven-point solver on its own, one thread per sample: q [n, 7, 4] normalised
+ * correspondences (x0, y0, x1, y1; device) -> F [n, 3, 9] normalised F^ row-major, root_index [n, 3] (the real root of
+ * the cubic each solution came from) and n_solutions [n] (device); entries past n_solutions are NaN / -1.  The same
+ * compiled function the estimator runs. */
+int ltr_debug_fundamental_solve(const double* q, int32_t n, double* F, int32_t* root_index, int32_t* n_solutions,
+                                int32_t device, void* stream);
+
+/* The absolute-pose estimator's P3P solver on its own, one thread per sample: j [n, 3, 3] unit bearings and X [n, 3, 3]
+ * world points of the sample's three points (device) -> R [n, 4, 9] row-major, t [n, 4, 3] (X_cam = R X + t),
+ * root_index [n, 4] (the real root of the quartic each pose came from) and n_solutions [n] (device); entries past
+ * n_solutions are NaN / -1.  The same compiled function the estimator runs. */
+int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double* t, int32_t* root_index,
+                  int32_t* n_solutions, int32_t device, void* stream);
+
+/* The fundamental-matrix estimator's line check on its own, one thread per key-line pair: F [n, 9] pixel F (row-major,
+ * fp64), s0 / s1 [n, 4] the matched segments (a, b; fp32) -> r1 [n] (the overlap ratio in image 1), r0 [n] (in
+ * image 0; NaN where the side cannot reject) and ok [n] (1 iff consistent at min_overlap in [0, 1]; device).  The same
+ * compiled functions the fit kernel runs. */
+int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s1, int32_t n, double min_overlap,
+                                double* r1, double* r0, uint8_t* ok, int32_t device, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -230,6 +230,9 @@ DEBUG_PROTOTYPES = {
     "ltr_debug_encode_images": (C.c_int, [_P, _I32, _P, _ptr(_P), _ptr(_P), c_int32_p]),
     "ltr_debug_sturm_roots": (C.c_int, [_P, _I32, _P, _P, _I32, _P]),
     "ltr_debug_essential_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),
+    "ltr_debug_fundamental_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),
+    "ltr_debug_p3p": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _I32, _P]),
+    "ltr_debug_fundamental_lines": (C.c_int, [_P, _P, _P, _I32, C.c_double, _P, _P, _P, _I32, _P]),
 }
 EXPORTED_SYMBOLS = tuple(PROTOTYPES)
 DEBUG_SYMBOLS = tuple(DEBUG_PROTOTYPES)

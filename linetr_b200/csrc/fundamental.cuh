@@ -300,8 +300,10 @@ __device__ __forceinline__ double fm_side_ratio(const double* la, const double* 
   return FM_D(ov, span < 1.0 ? span : 1.0);
 }
 
-// The line check of one matched key-line pair under F: false iff a side's ratio is below min_overlap.
-__device__ __forceinline__ bool fm_line_consistent(const double* F, const float* s0, const float* s1, double min_overlap) {
+// Both side ratios of one matched key-line pair under F: r1 in image 1 (F a0, F b0 against s1), r0 in image 0
+// (F^T a1, F^T b1 against s0); NaN where the side cannot reject.
+__device__ __forceinline__ void fm_line_ratios(const double* F, const float* s0, const float* s1, double& r1,
+                                               double& r0) {
   const double a0x = s0[0], a0y = s0[1], b0x = s0[2], b0y = s0[3];
   const double a1x = s1[0], a1y = s1[1], b1x = s1[2], b1y = s1[3];
   double la[3], lb[3];
@@ -311,15 +313,26 @@ __device__ __forceinline__ bool fm_line_consistent(const double* F, const float*
     la[r] = FM_A(FM_A(FM_M(F[3 * r], a0x), FM_M(F[3 * r + 1], a0y)), F[3 * r + 2]);
     lb[r] = FM_A(FM_A(FM_M(F[3 * r], b0x), FM_M(F[3 * r + 1], b0y)), F[3 * r + 2]);
   }
-  const double r1 = fm_side_ratio(la, lb, a1x, a1y, b1x, b1y);
+  r1 = fm_side_ratio(la, lb, a1x, a1y, b1x, b1y);
   // image 0: F^T a1, F^T b1 against s0
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
     la[c] = FM_A(FM_A(FM_M(F[c], a1x), FM_M(F[3 + c], a1y)), F[6 + c]);
     lb[c] = FM_A(FM_A(FM_M(F[c], b1x), FM_M(F[3 + c], b1y)), F[6 + c]);
   }
-  const double r0 = fm_side_ratio(la, lb, a0x, a0y, b0x, b0y);
+  r0 = fm_side_ratio(la, lb, a0x, a0y, b0x, b0y);
+}
+
+// The decision on the two ratios: consistent iff no side's ratio is below min_overlap (a NaN side cannot reject).
+__device__ __forceinline__ bool fm_ratios_consistent(double r1, double r0, double min_overlap) {
   return !(r1 < min_overlap) && !(r0 < min_overlap);
+}
+
+// The line check of one matched key-line pair under F: false iff a side's ratio is below min_overlap.
+__device__ __forceinline__ bool fm_line_consistent(const double* F, const float* s0, const float* s1, double min_overlap) {
+  double r1, r0;
+  fm_line_ratios(F, s0, s1, r1, r0);
+  return fm_ratios_consistent(r1, r0, min_overlap);
 }
 
 __global__ void __launch_bounds__(FM_FIT_THREADS) fundamental_fit_kernel(FundamentalArgs a) {

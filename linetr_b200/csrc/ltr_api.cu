@@ -1610,6 +1610,54 @@ static __global__ void debug_essential_solve_kernel(const double* q, int n, doub
   n_sol[i] = ns;
 }
 
+// Test hooks of the fundamental-matrix and absolute-pose estimators' fp64 pieces, in the same form.
+static __global__ void debug_fundamental_solve_kernel(const double* q, int n, double* F, int* root_index, int* n_sol) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double4 s[FM_SAMPLE];
+  for (int j = 0; j < FM_SAMPLE; ++j)
+    s[j] = make_double4(q[28ll * i + 4 * j], q[28ll * i + 4 * j + 1], q[28ll * i + 4 * j + 2], q[28ll * i + 4 * j + 3]);
+  double Fs[9 * FM_MAX_SOLUTIONS];
+  int jr[FM_MAX_SOLUTIONS];
+  const int ns = fm_solve(s, Fs, jr);
+  for (int j = 0; j < 9 * FM_MAX_SOLUTIONS; ++j)
+    F[27ll * i + j] = j < 9 * ns ? Fs[j] : __longlong_as_double(0x7ff8000000000000ll);
+  for (int j = 0; j < FM_MAX_SOLUTIONS; ++j) root_index[3ll * i + j] = j < ns ? jr[j] : -1;
+  n_sol[i] = ns;
+}
+
+static __global__ void debug_p3p_kernel(const double* jb, const double* X, int n, double* R, double* t, int* root_index,
+                                        int* n_sol) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double j[9], x[9];
+  for (int e = 0; e < 9; ++e) {
+    j[e] = jb[9ll * i + e];
+    x[e] = X[9ll * i + e];
+  }
+  double Rs[9 * AP_MAX_SOLUTIONS], ts[3 * AP_MAX_SOLUTIONS];
+  int jr[AP_MAX_SOLUTIONS];
+  const int ns = ap_p3p(j, x, Rs, ts, jr);
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  for (int e = 0; e < 9 * AP_MAX_SOLUTIONS; ++e) R[36ll * i + e] = e < 9 * ns ? Rs[e] : nan;
+  for (int e = 0; e < 3 * AP_MAX_SOLUTIONS; ++e) t[12ll * i + e] = e < 3 * ns ? ts[e] : nan;
+  for (int e = 0; e < AP_MAX_SOLUTIONS; ++e) root_index[4ll * i + e] = e < ns ? jr[e] : -1;
+  n_sol[i] = ns;
+}
+
+static __global__ void debug_fundamental_lines_kernel(const double* F, const float* s0, const float* s1, int n,
+                                                      double min_overlap, double* r1, double* r0, uint8_t* ok) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double f[9];
+  for (int e = 0; e < 9; ++e) f[e] = F[9ll * i + e];
+  double a, b;
+  fm_line_ratios(f, s0 + 4ll * i, s1 + 4ll * i, a, b);
+  r1[i] = a;
+  r0[i] = b;
+  ok[i] = fm_ratios_consistent(a, b, min_overlap);
+}
+
 int ltr_debug_sturm_roots(const double* poly, int32_t n, double* roots, int32_t* count, int32_t device, void* stream) {
   if (n < 0 || (n > 0 && (!poly || !roots || !count))) return set_error(LTR_E_INVALID, "ltr_debug_sturm_roots: bad argument");
   if (n == 0) return LTR_OK;
@@ -1626,6 +1674,39 @@ int ltr_debug_essential_solve(const double* q, int32_t n, double* E, int32_t* ro
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
   debug_essential_solve_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(q, n, E, root_index, n_solutions);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
+int ltr_debug_fundamental_solve(const double* q, int32_t n, double* F, int32_t* root_index, int32_t* n_solutions,
+                                int32_t device, void* stream) {
+  if (n < 0 || (n > 0 && (!q || !F || !root_index || !n_solutions)))
+    return set_error(LTR_E_INVALID, "ltr_debug_fundamental_solve: bad argument");
+  if (n == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  debug_fundamental_solve_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(q, n, F, root_index, n_solutions);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
+int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double* t, int32_t* root_index,
+                  int32_t* n_solutions, int32_t device, void* stream) {
+  if (n < 0 || (n > 0 && (!j || !X || !R || !t || !root_index || !n_solutions)))
+    return set_error(LTR_E_INVALID, "ltr_debug_p3p: bad argument");
+  if (n == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  debug_p3p_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(j, X, n, R, t, root_index, n_solutions);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
+int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s1, int32_t n, double min_overlap,
+                                double* r1, double* r0, uint8_t* ok, int32_t device, void* stream) {
+  if (n < 0 || (n > 0 && (!F || !s0 || !s1 || !r1 || !r0 || !ok)) || !(min_overlap >= 0.0 && min_overlap <= 1.0))
+    return set_error(LTR_E_INVALID, "ltr_debug_fundamental_lines: bad argument");
+  if (n == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  debug_fundamental_lines_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(F, s0, s1, n, min_overlap, r1, r0, ok);
   LTR_CUDA_TRY(cudaGetLastError());
   return LTR_OK;
 }

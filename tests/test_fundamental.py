@@ -242,6 +242,107 @@ def _ragged_cases(n_pairs=200, seed=0):
 
 FIELDS = ("F", "valid", "inliers_p", "n_inliers", "hypothesis", "hypothesis_inliers", "refit", "lines_consistent",
           "n_lines_consistent")
+U = 2.0 ** -53
+# The refit's A^T A is summed in another order than numpy's (and nvcc may contract its products to FMA), its smallest
+# eigenvector comes from Jacobi instead of eigh, and the rank-2 step from Jacobi on F^T F instead of an SVD.  So the
+# refitted F^ differs from the host's by about u times the conditioning of both steps: lambda_max / (lambda_2 -
+# lambda_1) of A^T A (Davis-Kahan) plus sigma_1 / (sigma_2 - sigma_3) of F^ (the rank-2 direction).  Denormalising and
+# the unit scaling keep that relative size.  Measured on an H100 80GB HBM3 (700 W limit) over the 162 kept refits of
+# test_kernels_match_host_model and the 1290 of test_estimator_edges' every-hypothesis runs: at most 29.8 u cond.
+# FM_REFIT_C leaves a factor 4 above that.
+FM_REFIT_C = 120.0
+
+
+def refit_condition(res, p, h, t2):
+    """lambda_max / (lambda_2 - lambda_1) of the refit's A^T A plus sigma_1 / (sigma_2 - sigma_3) of its F^."""
+    a, b = res.offsets_p[p:p + 2]
+    pts, _, _, _, _ = G._correspondences(res.keypoints0[p].cpu().numpy(), res.keypoints1[p].cpu().numpy(),
+                                         res.matches_p[a:b].cpu().numpy(), E22, E22, np.zeros(0, np.int64), True, False)
+    nm = G._normalisation(pts, E22, E22)
+    f = lambda v: np.asarray(v, dtype=np.float64)
+    q = np.stack([(f(pts[:, 0]) - nm.c0x) * nm.i0, (f(pts[:, 1]) - nm.c0y) * nm.i0,
+                  (f(pts[:, 2]) - nm.c1x) * nm.i1, (f(pts[:, 3]) - nm.c1y) * nm.i1], 1)
+    fl = G.fundamental_inliers(h["F_hypothesis"].reshape(1, 9), pts, t2)[0]
+    A = G._epipolar_rows(q[fl])
+    w, V = np.linalg.eigh(A.T @ A)
+    s = np.linalg.svd(V[:, 0].reshape(3, 3), compute_uv=False)
+    return float(w[-1] / (w[1] - w[0]) + s[0] / (s[1] - s[2]))
+
+
+def _masks_at(res, p, F, thresh, min_overlap):
+    """The host model's point mask and line decisions of pair p under a given pixel F: -> (inliers_p, lines, pts, rp)
+    with pts the correspondences and rp their match rows."""
+    a, b = res.offsets_p[p:p + 2]
+    c, e = res.offsets_l[p:p + 2]
+    pts, _, _, rp, _ = G._correspondences(res.keypoints0[p].cpu().numpy(), res.keypoints1[p].cpu().numpy(),
+                                          res.matches_p[a:b].cpu().numpy(), E22, E22, np.zeros(0, np.int64), True,
+                                          False)
+    mp = np.zeros(b - a, np.uint8)
+    mp[rp] = G.fundamental_inliers(F.reshape(1, 9), pts, thresh * thresh)[0]
+    ml = res.matches_l[c:e].cpu().numpy().astype(np.int64)
+    k1 = np.asarray(res.klines1[p], np.float32).reshape(-1, 2, 2)
+    rl = np.flatnonzero((ml >= 0) & (ml < len(k1)))
+    lines = np.zeros(e - c, np.uint8)
+    if len(rl):
+        k0 = np.asarray(res.klines0[p], np.float32).reshape(-1, 2, 2)
+        lines[rl] = G.lines_consistent(F, k0[rl], k1[ml[rl]], min_overlap)
+    return mp, lines, pts, rp
+
+
+def _residual_band(F, pts, tol):
+    """How far a relative F error of tol (entrywise, relative to max |F|) can move the FM residual r = |x1^T F x0| /
+    |n| of each correspondence (n the smaller epipolar line normal, (F x0)_xy or (F^T x1)_xy).  With |dF_ij| <= eps =
+    tol max |F|: |d(x1^T F x0)| <= eps |x1|_1 |x0|_1 and |d|n|| <= sqrt(2) eps |x|_1 (x the point the normal is taken
+    at, homogeneous), so to first order |dr| <= (eps |x1|_1 |x0|_1 + r sqrt(2) eps |x|_1) / |n|, taking the larger of the
+    two normals' bounds.  Twice that covers the second-order terms and r being taken at one of the two F."""
+    F = np.asarray(F, dtype=np.float64).reshape(1, 9)
+    num, na, nb = (v[0] for v in G._fm_terms(F, pts))
+    eps = tol * np.abs(F).max()
+    h0 = np.abs(pts[:, 0]) + np.abs(pts[:, 1]) + 1.0
+    h1 = np.abs(pts[:, 2]) + np.abs(pts[:, 3]) + 1.0
+    with np.errstate(all="ignore"):
+        r = np.abs(num) / np.sqrt(np.minimum(na, nb))
+        band = np.maximum((eps * h1 * h0 + r * np.sqrt(2.0) * eps * h0) / np.sqrt(na),
+                          (eps * h1 * h0 + r * np.sqrt(2.0) * eps * h1) / np.sqrt(nb))
+    return r, 2.0 * band
+
+
+def check_pair(res, got, p, thresh=3.0, stats=None, **kw):
+    """Pair p of an estimate_fundamentals result (numpy fields) against the host model: validity, the hypothesis and
+    its inlier count exactly; F bit for bit unless the refit was kept, else within FM_REFIT_C u refit_condition of the
+    host's (relative to its largest entry).  The masks: bit for bit without a kept refit; with one, the point mask and
+    line decisions must be exactly the host model's at the kernel's F (the inlier test and the line check are
+    explicitly rounded, so no band is needed there), and a point row may differ from the host's own mask only where
+    its residual lies within `_residual_band` of the threshold.  Counts equal to the masks."""
+    h = _host_pair(res, p, thresh=thresh, **kw)
+    assert bool(got["valid"][p]) == h["valid"], p
+    assert got["hypothesis"][p] == h["hypothesis"] and got["hypothesis_inliers"][p] == h["hypothesis_inliers"], p
+    a, b = res.offsets_p[p:p + 2]
+    c, e = res.offsets_l[p:p + 2]
+    gm, gl = got["inliers_p"][a:b], got["lines_consistent"][c:e]
+    if not h["valid"]:
+        assert np.isnan(got["F"][p]).all() and not gm.any() and not gl.any() and got["n_lines_consistent"][p] == 0
+        assert got["n_inliers"][p] == 0 and not got["refit"][p], p
+        return h
+    assert bool(got["refit"][p]) == h["refit"], p
+    assert got["n_inliers"][p] == gm.sum() and got["n_lines_consistent"][p] == gl.sum(), p
+    if not h["refit"]:
+        assert np.array_equal(got["F"][p].reshape(9).view(np.int64), h["F"].reshape(9).view(np.int64)), p
+        assert np.array_equal(gm, h["inliers_p"]) and np.array_equal(gl, h["lines_consistent"]), p
+        return h
+    cond = refit_condition(res, p, h, thresh * thresh)
+    err = float(np.abs(got["F"][p] - h["F"]).max() / np.abs(h["F"]).max())
+    if stats is not None:
+        stats.append(err / (U * cond))
+    tol = FM_REFIT_C * U * cond
+    assert err <= tol, (p, err, cond, tol)
+    mp, ml, pts, rp = _masks_at(res, p, got["F"][p], thresh, kw.get("min_overlap", 0.5))
+    assert np.array_equal(gm, mp) and np.array_equal(gl, ml), p
+    diff = np.flatnonzero(gm[rp] != h["inliers_p"][rp])
+    if len(diff):
+        r, band = _residual_band(h["F"], pts[diff].astype(np.float64), tol)
+        assert np.all(np.abs(r - thresh) <= band), (p, r, band)
+    return h
 
 
 @pytest.mark.gpu
@@ -251,28 +352,11 @@ def test_kernels_match_host_model():
     Kh, seed = 256, 5
     out = G.estimate_fundamentals(res, n_hypotheses=Kh, seed=seed)
     got = {f: getattr(out, f).cpu().numpy() for f in FIELDS}
-    diff_p = diff_l = total_p = total_l = 0
+    ratios = []
     for p in range(res.n_pairs):
-        h = _host_pair(res, p, n_hypotheses=Kh, seed=seed)
-        assert bool(got["valid"][p]) == h["valid"], p
-        assert got["hypothesis"][p] == h["hypothesis"] and got["hypothesis_inliers"][p] == h["hypothesis_inliers"], p
-        a, b = res.offsets_p[p:p + 2]
-        c, e = res.offsets_l[p:p + 2]
-        gm, gl = got["inliers_p"][a:b], got["lines_consistent"][c:e]
-        total_p += b - a
-        total_l += e - c
-        if not h["valid"]:
-            assert np.isnan(got["F"][p]).all() and not gm.any() and not gl.any() and got["n_lines_consistent"][p] == 0
-            continue
-        assert bool(got["refit"][p]) == h["refit"], p
-        assert np.abs(got["F"][p] - h["F"]).max() < 1e-9, (p, got["F"][p], h["F"])
-        diff_p += int((gm != h["inliers_p"]).sum())
-        diff_l += int((gl != h["lines_consistent"]).sum())
-        assert got["n_inliers"][p] == gm.sum() and got["n_lines_consistent"][p] == gl.sum()
-    print(f"{res.n_pairs} pairs, {int(got['valid'].sum())} valid, {int(got['refit'].sum())} refitted; {diff_p} of "
-          f"{total_p} point mask rows and {diff_l} of {total_l} line rows differ")
-    # the refit F agrees to 1e-9, so only rows within ~1e-9 relative of a threshold could differ
-    assert diff_p * 10000 <= total_p and diff_l * 1000 <= max(total_l, 1)
+        check_pair(res, got, p, stats=ratios, n_hypotheses=Kh, seed=seed)
+    print(f"{res.n_pairs} pairs, {int(got['valid'].sum())} valid, {int(got['refit'].sum())} refitted; worst refit "
+          f"|dF| / (u cond) {max(ratios, default=0.0):.3g}")
     assert not got["valid"][::10].any()                       # the pairs below 7 correspondences
 
 

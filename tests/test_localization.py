@@ -328,7 +328,9 @@ def test_kernels_match_host_model():
             continue
         n_valid += 1
         assert bool(got["refit"][g]) == h["refit"], g
-        assert np.abs(got["R"][g] - h["R"]).max() < 1e-9 and np.abs(got["t"][g] - h["t"]).max() < 1e-9, g
+        for f in ("R", "t"):                                                  # bit for bit
+            assert np.array_equal(np.ascontiguousarray(got[f][g]).view(np.int64),
+                                  np.ascontiguousarray(h[f]).view(np.int64)), (g, f, got[f][g], h[f])
         diff += int((gm != h["inliers_p"]).sum() + (gl != h["inliers_l"]).sum())
         assert got["n_inliers_p"][g] == gm.sum() and got["n_inliers_l"][g] == gl.sum()
     print(f"{len(groups) - 1} groups, {n_valid} valid, {int(got['refit'].sum())} refitted; {diff} of {rows} mask rows "
