@@ -45,6 +45,13 @@ int ltr_debug_linear_img_res(const float* x, int32_t ldx, const float* w_host, c
 int ltr_debug_encode_images(const struct LtrModel* model, int32_t n_lines, void* workspace, void* hi[11], void* lo[11],
                             int32_t kblocks[11]);
 
+/* `launches` back-to-back signature-attention launches as ltr_encode issues them for n_images images of 128 lines
+ * (uniform batch): qkv image (12 k-blocks per 128-row block, hi / lo planes, device) -> columns 256..511 of an
+ * 8-k-block output image.  The kernel is chosen as an encode chooses it, LTR_ATTN_PIPE included.  Returns 0, LTR_E_INVALID on a
+ * bad argument, or the launch error. */
+int ltr_debug_sig_attention(const void* qkv_hi, const void* qkv_lo, void* out_hi, void* out_lo, int32_t n_images,
+                            int32_t launches, void* stream);
+
 /* The relative-pose estimator's fp64 root finder on its own, one thread per polynomial: poly [n, 11] ascending
  * coefficients (device) -> roots [n, 10] ascending, NaN past the count, and count [n] (device).  The estimator's own
  * __device__ function (Sturm chain and bisection). */

@@ -228,6 +228,7 @@ DEBUG_PROTOTYPES = {
     "ltr_debug_trace_read": (C.c_int, [_ptr(C.c_uint64)]),
     "ltr_debug_linear_img_res": (C.c_int, [_P, _I32, _P, _P, _P, _P, _P] + [_I32] * 6 + [_P]),
     "ltr_debug_encode_images": (C.c_int, [_P, _I32, _P, _ptr(_P), _ptr(_P), c_int32_p]),
+    "ltr_debug_sig_attention": (C.c_int, [_P, _P, _P, _P, _I32, _I32, _P]),
     "ltr_debug_sturm_roots": (C.c_int, [_P, _I32, _P, _P, _I32, _P]),
     "ltr_debug_essential_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),
     "ltr_debug_fundamental_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),

@@ -155,6 +155,21 @@ inline cudaError_t ensure_dynamic_smem(K kernel, int bytes) {
   return e;
 }
 
+// SMs of the current device (persistent grids size themselves by it)
+inline int device_sm_count() {
+  static std::atomic<int> sms[64];   // zero-initialised; benign duplicate queries, no torn state
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64) return 132;
+  int v = sms[dev].load(std::memory_order_relaxed);
+  if (!v) {
+    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
+    if (v <= 0) v = 132;
+    sms[dev].store(v, std::memory_order_relaxed);
+  }
+  return v;
+}
+
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline int64_t align_up(int64_t x, int64_t a) { return (x + a - 1) / a * a; }
 

@@ -675,20 +675,6 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
   }
 }
 
-inline int device_sm_count() {
-  static std::atomic<int> sms[64];   // zero-initialised; benign duplicate queries, no torn state
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return 132;
-  int v = sms[dev].load(std::memory_order_relaxed);
-  if (!v) {
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    if (v <= 0) v = 132;
-    sms[dev].store(v, std::memory_order_relaxed);
-  }
-  return v;
-}
-
 template <int BN, bool FRAG>
 static int launch_gemm_img_bn(GemmImgArgs a, cudaStream_t s) {
   using Cfg = GemmImgCfg<BN>;

@@ -1585,6 +1585,19 @@ int ltr_debug_encode_images(const LtrModel* m, int32_t n_lines, void* workspace,
   return LTR_OK;
 }
 
+int ltr_debug_sig_attention(const void* qkv_hi, const void* qkv_lo, void* out_hi, void* out_lo, int32_t n_images,
+                            int32_t launches, void* stream) {
+  if (!qkv_hi || !qkv_lo || !out_hi || !out_lo || n_images <= 0 || launches < 0)
+    return set_error(LTR_E_INVALID, "ltr_debug_sig_attention: bad argument");
+  auto img = [](const void* hi, const void* lo, int kb) {
+    return ActImg{reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(hi)), reinterpret_cast<__nv_bfloat16*>(const_cast<void*>(lo)), kb};
+  };
+  const ActImg qkv = img(qkv_hi, qkv_lo, 12), out = img(out_hi, out_lo, 8);
+  for (int i = 0; i < launches; ++i)
+    LTR_TRY(launch_sig_attention_tc(qkv, out, 256, nullptr, 128, 128, n_images, static_cast<cudaStream_t>(stream)));
+  return LTR_OK;
+}
+
 // Test hooks of the relative-pose estimator's fp64 pieces: one thread per item, the estimator's __device__ functions.
 static __global__ void debug_sturm_roots_kernel(const double* poly, int n, double* roots, int* count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -20,6 +20,8 @@
 // rescaling of the accumulator is ever needed.  Output: columns [out_k0, out_k0+256) of a split-bf16
 // activation image (the second half of the signature MLP input; the `merge` projection is folded into W1).
 #pragma once
+#include <cstdlib>
+#include <cstring>
 #include "act_img.cuh"
 #include "common.cuh"
 #include "ptx_sm90.cuh"
@@ -286,9 +288,194 @@ __global__ void __launch_bounds__(256) sig_attention_tc_kernel(ActImg qkv, ActIm
   if (tid == 0) LTR_DBG_STAMP(38);
 }
 
+// ------------------------------------------------------------------ uniform batches of 128-line images
+// Image i is exactly tile i of the qkv image, so one (image, head) unit is six 16 KB bulk copies and one 128-query tile.
+// One persistent CTA per SM walks its images (b, b + grid, ...) and all four heads of each, 384 threads:
+//   * a producer warpgroup (one lane issues the copies) fills a two-stage ring, so head h + 1 - or the next image's
+//     head 0 - lands while head h computes; q and k complete on full_qk, v on full_v (S does not wait for v);
+//   * two consumer warpgroups of 64 query rows each run S -> softmax -> PV on their own: the split P is the register A
+//     fragment of the PV wgmma (the S accumulator layout is the A-fragment layout), so nothing is written to shared
+//     memory and there is no barrier across warpgroups.  A stage is released (8 warp arrivals on empty) as soon as
+//     its PV MMAs have completed;
+//   * each consumer warp stages its 16 output rows x 64 head dims - one contiguous 2 KB piece of the output tile per
+//     plane - and bulk-stores them itself.
+// Per element this is the instruction sequence of sig_attention_tc_kernel's single-key-tile path (same MMA products in
+// the same order, same softmax and split), so the output is bit-identical to it.
+struct SigAttnPipeSmem {
+  static constexpr int TILE = 16384;             // [128 x 64] bf16, one plane
+  static constexpr int STAGE = 6 * TILE;         // q hi/lo, k hi/lo, v hi/lo
+  static constexpr int STAGES = 2;
+  static constexpr int STG_WARP = 2 * 2048;      // 16 rows x 64 dims, hi and lo
+  static constexpr int OFF_STG = STAGES * STAGE;
+  static constexpr int OFF_BAR = OFF_STG + 8 * STG_WARP;
+  static constexpr int TOTAL = OFF_BAR + 64 + 1024;   // + alignment slack
+};
+
+__global__ void __launch_bounds__(384, 1) sig_attention_pipe_kernel(ActImg qkv, ActImg out, int out_k0, int n_images) {
+  using S = SigAttnPipeSmem;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  const uint32_t raw = ptx::smem_u32(smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (raw & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::OFF_BAR);
+  uint64_t* full_qk = bars;        // [2] q and k of the stage have landed
+  uint64_t* full_v = bars + 2;     // [2] v of the stage has landed
+  uint64_t* empty = bars + 4;      // [2] the stage's MMAs are done (8 consumer warps)
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  pdl_launch_dependents();
+  if (tid == 0) {
+    for (int s = 0; s < S::STAGES; ++s) {
+      ptx::mbar_init(&full_qk[s], 1);
+      ptx::mbar_init(&full_v[s], 1);
+      ptx::mbar_init(&empty[s], 8);
+    }
+    ptx::fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // ---------------------------------------------------------------- TMA producer
+    ptx::setmaxnreg_dec<40>();
+    if (warp == 8 && lane == 0) {
+      pdl_wait();   // qkv of this layer is complete
+      uint32_t it = 0;
+      for (int img = blockIdx.x; img < n_images; img += gridDim.x)
+        for (int h = 0; h < 4; ++h, ++it) {
+          const int s = it & 1;
+          ptx::mbar_wait(&empty[s], ((it >> 1) & 1) ^ 1);
+          uint8_t* st = smem + s * S::STAGE;
+          const size_t t0 = (size_t)img * qkv.kblocks * IMG_TILE_ELEMS;
+          const size_t tq = t0 + (size_t)h * IMG_TILE_ELEMS, tk = t0 + (size_t)(4 + h) * IMG_TILE_ELEMS,
+                       tv = t0 + (size_t)(8 + h) * IMG_TILE_ELEMS;
+          ptx::mbar_arrive_expect_tx(&full_qk[s], 4 * S::TILE);
+          ptx::bulk_g2s(st, qkv.hi + tq, S::TILE, &full_qk[s]);
+          ptx::bulk_g2s(st + S::TILE, qkv.lo + tq, S::TILE, &full_qk[s]);
+          ptx::bulk_g2s(st + 2 * S::TILE, qkv.hi + tk, S::TILE, &full_qk[s]);
+          ptx::bulk_g2s(st + 3 * S::TILE, qkv.lo + tk, S::TILE, &full_qk[s]);
+          ptx::mbar_arrive_expect_tx(&full_v[s], 2 * S::TILE);
+          ptx::bulk_g2s(st + 4 * S::TILE, qkv.hi + tv, S::TILE, &full_v[s]);
+          ptx::bulk_g2s(st + 5 * S::TILE, qkv.lo + tv, S::TILE, &full_v[s]);
+        }
+    }
+  } else {
+    // ---------------------------------------------------------------- consumers (2 warpgroups x 64 query rows)
+    ptx::setmaxnreg_inc<232>();
+    pdl_wait();   // the previous kernel may still read the output image's columns this kernel writes
+    const int wg = warp >> 2;
+    const int r0 = lane >> 2, cq = 2 * (lane & 3);   // rows 16 warp + r0 and + 8 of the tile, columns 8 j + cq, + 1
+    uint8_t* stg = smem + S::OFF_STG + warp * S::STG_WARP;   // hi plane, lo plane 2 KB on
+    constexpr float LOG2E = 1.4426950408889634f;
+    uint32_t it = 0;
+    for (int img = blockIdx.x; img < n_images; img += gridDim.x)
+      for (int h = 0; h < 4; ++h, ++it) {
+        const int s = it & 1;
+        const uint32_t par = (it >> 1) & 1;
+        const uint32_t sb = ptx::smem_u32(smem + s * S::STAGE);
+        float sd[64];
+        ptx::mbar_wait(&full_qk[s], par);
+        attn_qk(sd, sb + wg * 8192, sb + S::TILE + wg * 8192, sb + 2 * S::TILE, sb + 3 * S::TILE);
+        float m0 = -INFINITY, m1 = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            m0 = fmaxf(m0, sd[4 * j + e]);
+            m1 = fmaxf(m1, sd[4 * j + 2 + e]);
+          }
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {
+          m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, o));
+          m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, o));
+        }
+        // p = exp(s - m) -> A fragments of the PV MMA: K = 16 step kk takes the accumulator groups 2 kk (a[0], a[1])
+        // and 2 kk + 1 (a[2], a[3]), rows r0 and r0 + 8 each
+        float l0 = 0.f, l1 = 0.f;
+        uint32_t ah[8][4], al[8][4];
+        const float mb0 = m0 * LOG2E, mb1 = m1 * LOG2E;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          const float p00 = ptx::ex2_approx(fmaf(sd[4 * j], LOG2E, -mb0));
+          const float p01 = ptx::ex2_approx(fmaf(sd[4 * j + 1], LOG2E, -mb0));
+          const float p10 = ptx::ex2_approx(fmaf(sd[4 * j + 2], LOG2E, -mb1));
+          const float p11 = ptx::ex2_approx(fmaf(sd[4 * j + 3], LOG2E, -mb1));
+          l0 += p00 + p01;
+          l1 += p10 + p11;
+          ptx::split2_bf16(p00, p01, ah[j >> 1][2 * (j & 1)], al[j >> 1][2 * (j & 1)]);
+          ptx::split2_bf16(p10, p11, ah[j >> 1][2 * (j & 1) + 1], al[j >> 1][2 * (j & 1) + 1]);
+        }
+        // O = P V    (B = V as an MN-major operand: [K = keys][N = 64 dims], 16 key rows of 128 bytes per K step)
+        // The accumulator starts from +0 held in registers, as in sig_attention_tc_kernel.  With a literal 0 ptxas drops
+        // the C input of the first MMA, which would turn an output whose products are all -0 into -0 instead of +0.
+        const float zero = 0.f * l0;   // l0 >= 1
+        float od[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) od[i] = zero;
+        const uint32_t vh = sb + 4 * S::TILE, vl = sb + 5 * S::TILE;
+        ptx::mbar_wait(&full_v[s], par);
+        ptx::wg_fence_regs(od);
+        ptx::wg_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const uint32_t va = kk * 2048;
+          ptx::wgmma_rs_n64_tb(od, al[kk], ptx::make_sw128_mnmajor_desc(vh + va, 1024, 1024), 1);
+          ptx::wgmma_rs_n64_tb(od, ah[kk], ptx::make_sw128_mnmajor_desc(vl + va, 1024, 1024), 1);
+          ptx::wgmma_rs_n64_tb(od, ah[kk], ptx::make_sw128_mnmajor_desc(vh + va, 1024, 1024), 1);
+        }
+        ptx::wg_commit();
+        ptx::wg_wait<0>();
+        ptx::wg_fence_regs(od);
+        if (lane == 0) ptx::mbar_arrive(&empty[s]);   // this warpgroup is done reading the stage
+        // ---- o / l -> this warp's 16 rows of output tile (img, out_k0 / 64 + h)
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {
+          l0 += __shfl_xor_sync(0xffffffffu, l0, o);
+          l1 += __shfl_xor_sync(0xffffffffu, l1, o);
+        }
+        const float inv0 = 1.f / l0, inv1 = 1.f / l1;
+        if (lane == 0) ptx::bulk_wait_read_all();   // the previous head's store is done reading the staging block
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          uint32_t hh, ll;
+          ptx::split2_bf16(od[4 * j] * inv0, od[4 * j + 1] * inv0, hh, ll);
+          *reinterpret_cast<uint32_t*>(stg + ptx::sw128_offset(r0, 8 * j + cq)) = hh;
+          *reinterpret_cast<uint32_t*>(stg + 2048 + ptx::sw128_offset(r0, 8 * j + cq)) = ll;
+          ptx::split2_bf16(od[4 * j + 2] * inv1, od[4 * j + 3] * inv1, hh, ll);
+          *reinterpret_cast<uint32_t*>(stg + ptx::sw128_offset(r0 + 8, 8 * j + cq)) = hh;
+          *reinterpret_cast<uint32_t*>(stg + 2048 + ptx::sw128_offset(r0 + 8, 8 * j + cq)) = ll;
+        }
+        ptx::fence_proxy_async_smem();
+        __syncwarp();
+        if (lane == 0) {
+          // rows 16 warp .. + 15 of a SWIZZLE_128B tile are its bytes [2048 warp, 2048 warp + 2048)
+          const size_t toff = ((size_t)img * out.kblocks + (out_k0 >> 6) + h) * IMG_TILE_ELEMS + (size_t)warp * 1024;
+          ptx::bulk_s2g(out.hi + toff, stg, 2048);
+          ptx::bulk_s2g(out.lo + toff, stg + 2048, 2048);
+          ptx::bulk_commit();
+        }
+      }
+    if (lane == 0) ptx::bulk_wait<0>();   // the staging stays allocated, and the writes done, until the stores complete
+  }
+}
+
+// LTR_ATTN_PIPE=0 keeps every batch on sig_attention_tc_kernel (A/B runs and the bit-identity tests); read at every
+// call so that one process can run both kernels.
+inline bool attn_pipe_enabled() {
+  const char* e = std::getenv("LTR_ATTN_PIPE");
+  return !(e && std::strcmp(e, "0") == 0);
+}
+
 inline int launch_sig_attention_tc(ActImg qkv, ActImg out, int out_k0, const int* cu, int lpi, int max_l,
                                    int n_images, cudaStream_t s) {
   if (max_l <= 0 || n_images <= 0) return 0;
+  if (!cu && lpi == 128 && attn_pipe_enabled()) {
+    LTR_CUDA_TRY(ensure_dynamic_smem(sig_attention_pipe_kernel, SigAttnPipeSmem::TOTAL));
+    const int grid = std::min(n_images, device_sm_count());
+    LaunchScope ls(KC_SIG_ATTN, s);
+    LTR_CUDA_TRY(launch_pdl(sig_attention_pipe_kernel, dim3(grid), dim3(384), SigAttnPipeSmem::TOTAL, s, qkv, out, out_k0,
+                            n_images));
+    return 0;
+  }
   LTR_CUDA_TRY(ensure_dynamic_smem(sig_attention_tc_kernel, SigAttnSmem::TOTAL));
   dim3 grid(cdiv(max_l, 128), 4, n_images);
   LaunchScope ls(KC_SIG_ATTN, s);
