@@ -34,6 +34,8 @@
  *                                 with an epipolar check of the line matches.
  *   ltr_absolute_pose          <- cv2.solvePnPRansac per query, batched, with the line matches scored and refined too
  *                                 (PL-Loc's localization step).
+ *   ltr_triangulate            <- cv2.triangulatePoints per pair, batched over every image of a posed set, multi-view
+ *                                 with outlier rejection, and for the key lines' end points too.
  *   ltr_warp_pairs             <- cv2.warpPerspective of the grey and colour images + the eroded valid mask of the
  *                                 homography dataset builder (dataloaders/build_homography_dataset.py:164-184).
  *   ltr_photometric            <- imgPhotometric of the homography dataset builder (ImgAugTransform +
@@ -725,6 +727,77 @@ typedef struct {
  * capacity) come before any launch.  n_groups == 0 writes nothing.  Writes the masks of the rows of pairs in
  * [groups[0], groups[n_groups]). */
 int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream);
+
+/* Triangulation of posed images: a world point for every keypoint and two world end points for every key line of every
+ * image, from the pair matches of the set (ltr_match_indexed / match_set); DESIGN.md "Triangulation" states the model:
+ *   - image i has intrinsics K[i] (zero skew: fx, fy, cx, cy are read) and the world -> camera pose X_cam = R[i] X +
+ *     t[i], centre C = -R^T t.  A row of image a (the anchor) is lifted along its own ray by its depth s,
+ *     X = C_a + s R_a^T K_a^-1 (x, y, 1): a keypoint's ray, or each end point's ray of a key line;
+ *   - observations: every pair that contains a gives at most one partner row, in the order of views[view_off[a] ..
+ *     view_off[a+1]) (pair << 1 | side of a; pair order): matches_*[cu_*[p] + k] when a is side 0 of pair p, the
+ *     lowest side-0 row that matched k when a is side 1 (found by an atomicMin scatter into inv_*); a match outside
+ *     [0, rows of the partner) is no observation;
+ *   - residuals in pixels: a point's reprojection error into the partner; an end point's signed distance of its
+ *     projection to the infinite line through the partner segment (the partner's back-projected plane);
+ *   - candidates: each observation's two-view depth (a point's least-squares root of its two residual numerators, an
+ *     end point's plane intersection), kept iff depth > 0 and the triangulation angle >= min_angle degrees (a point:
+ *     the angle between the two rays at X; a key line: between each end point's ray and the partner plane);
+ *   - support: an observation supports a depth iff its own depth is > 0 and its residual is <= thresh (a key line at
+ *     both end points).  The winner has the most supporters, ties to the lowest observation;
+ *   - refit: 5 one-dimensional Gauss-Newton steps over the supporters' residuals (a key line's end points separately),
+ *     kept iff its depth is > 0 and it has at least as many supporters;
+ *   - valid iff 1 + supporters >= min_views: n_views = 1 + supporters, else NaN coordinates and n_views = 0.
+ * Every operation is explicitly rounded fp64 in a fixed order.
+ *
+ * Capacity: at most LTR_TRI_MAX_VIEWS pairs per image (max_views), else LTR_E_UNSUPPORTED before any launch.  Pairs
+ * must be distinct unordered pairs of two different images (checked by the caller: the kernels take them as given). */
+#define LTR_TRI_MAX_VIEWS 64
+typedef struct {
+  const float* kpts;              /* device [*, 2] keypoints, image i's rows from kp_off[i] */
+  const int32_t* kp_off;          /* device [n_images + 1] */
+  const float* segs;              /* device [*, 2, 2] key lines (start xy, end xy), image i's rows from seg_off[i] */
+  const int32_t* seg_off;         /* device [n_images + 1] */
+  const double* K;                /* device [n_images, 3, 3] */
+  const double* R;                /* device [n_images, 3, 3] world -> camera */
+  const double* t;                /* device [n_images, 3] */
+  const int32_t* pairs;           /* device [n_pairs, 2] image indices */
+  const int32_t* matches_p;       /* device: local side-1 keypoint index or -1 per side-0 keypoint row */
+  const int32_t* cu_p;            /* device [n_pairs + 1]: pair p owns matches_p rows [cu_p[p], cu_p[p+1]), as many as
+                                     image pairs[p][0] has keypoints */
+  const int32_t* matches_l;       /* device: the same for key lines */
+  const int32_t* cu_l;            /* device [n_pairs + 1] */
+  const int32_t* views;           /* device: image i's observations [view_off[i], view_off[i+1]), pair << 1 | side */
+  const int32_t* view_off;        /* device [n_images + 1] */
+  const int32_t* block_off;       /* device [2 n_images + 1]: prefix sum of ceil(rows / 128) over the images'
+                                     keypoints, then over their key lines */
+  const int32_t* inv_off_p;       /* device [n_pairs + 1]: prefix sum of the keypoint counts of images pairs[p][1] */
+  const int32_t* inv_off_l;       /* device [n_pairs + 1]: the same for key lines */
+  int32_t n_images;
+  int32_t n_pairs;
+  int32_t total_p;                /* cu_p[n_pairs] (host value) */
+  int32_t total_l;                /* cu_l[n_pairs] */
+  int32_t n_inv_p;                /* inv_off_p[n_pairs] */
+  int32_t n_inv_l;                /* inv_off_l[n_pairs] */
+  int32_t n_blocks;               /* block_off[2 n_images] */
+  int32_t max_views;              /* the largest view_off[i+1] - view_off[i], at most LTR_TRI_MAX_VIEWS */
+  double thresh;                  /* pixels (4) */
+  double min_angle;               /* degrees in [0, 90) (1.5) */
+  int32_t min_views;              /* >= 1 (2) */
+} LtrTriangulateInput;
+
+/* Outputs (device, caller-owned), aligned with kpts / segs.  inv_p [n_inv_p] / inv_l [n_inv_l] int32 are workspace. */
+typedef struct {
+  double* points3d;               /* [*, 3] */
+  double* lines3d;                /* [*, 2, 3] */
+  int32_t* n_views_p;             /* [*] */
+  int32_t* n_views_l;             /* [*] */
+  int32_t* inv_p;
+  int32_t* inv_l;
+} LtrTriangulateOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments, LTR_E_UNSUPPORTED over
+ * capacity) come before any launch.  Two launches: the scatter of the side-1 index, then one thread per row. */
+int ltr_triangulate(const LtrTriangulateInput* in, const LtrTriangulateOutput* out, int32_t device, void* stream);
 
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where

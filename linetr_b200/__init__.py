@@ -20,6 +20,9 @@ check of the line matches, batched on the GPU:
 Visual localization (localization): the absolute pose of query images from 2D-3D point and line matches (P3P RANSAC
 and a Levenberg-Marquardt refit), batched on the GPU, and the localization metrics:
     estimate_absolute_poses, absolute_pose_errors, localization_recall, lift_to_3d
+Triangulation (triangulation): world points of every keypoint and world end points of every key line of posed images
+from their pair matches (multi-view, with outlier rejection and a Gauss-Newton refit), batched on the GPU:
+    triangulate, TriangulationResult
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
@@ -65,6 +68,8 @@ _LAZY = {
     "absolute_pose_errors": ("localization", "absolute_pose_errors"),
     "localization_recall": ("localization", "localization_recall"),
     "lift_to_3d": ("localization", "lift_to_3d"),
+    "triangulate": ("triangulation", "triangulate"),
+    "TriangulationResult": ("triangulation", "TriangulationResult"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

@@ -23,6 +23,7 @@ ENCODE_IMAGES = ("z", "ctx", "l128", "l256", "lpos", "y1i", "g", "xm", "hm", "qk
 ABI_VERSION = 4
 PHOTOMETRIC_PARAMS = 28      # LTR_PHOTOMETRIC_PARAMS
 PHOTOMETRIC_MAX_KSIZE = 149  # LTR_PHOTOMETRIC_MAX_KSIZE
+TRI_MAX_VIEWS = 64           # LTR_TRI_MAX_VIEWS
 
 
 def photometric_workspace_bytes(n, h, w) -> int:
@@ -183,6 +184,21 @@ class LtrAbsPoseOutput(C.Structure):
                 ("key", C.c_void_p)]
 
 
+class LtrTriangulateInput(C.Structure):
+    _fields_ = [("kpts", C.c_void_p), ("kp_off", C.c_void_p), ("segs", C.c_void_p), ("seg_off", C.c_void_p),
+                ("K", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("pairs", C.c_void_p),
+                ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("matches_l", C.c_void_p), ("cu_l", C.c_void_p),
+                ("views", C.c_void_p), ("view_off", C.c_void_p), ("block_off", C.c_void_p), ("inv_off_p", C.c_void_p),
+                ("inv_off_l", C.c_void_p), ("n_images", C.c_int32), ("n_pairs", C.c_int32), ("total_p", C.c_int32),
+                ("total_l", C.c_int32), ("n_inv_p", C.c_int32), ("n_inv_l", C.c_int32), ("n_blocks", C.c_int32),
+                ("max_views", C.c_int32), ("thresh", C.c_double), ("min_angle", C.c_double), ("min_views", C.c_int32)]
+
+
+class LtrTriangulateOutput(C.Structure):
+    _fields_ = [("points3d", C.c_void_p), ("lines3d", C.c_void_p), ("n_views_p", C.c_void_p), ("n_views_l", C.c_void_p),
+                ("inv_p", C.c_void_p), ("inv_l", C.c_void_p)]
+
+
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
 # {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
 # of them, and each entry against its C prototype)
@@ -210,6 +226,7 @@ PROTOTYPES = {
     "ltr_essential": (C.c_int, [_ptr(LtrEssentialInput), _ptr(LtrEssentialOutput), _I32, _P]),
     "ltr_fundamental": (C.c_int, [_ptr(LtrFundamentalInput), _ptr(LtrFundamentalOutput), _I32, _P]),
     "ltr_absolute_pose": (C.c_int, [_ptr(LtrAbsPoseInput), _ptr(LtrAbsPoseOutput), _I32, _P]),
+    "ltr_triangulate": (C.c_int, [_ptr(LtrTriangulateInput), _ptr(LtrTriangulateOutput), _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),

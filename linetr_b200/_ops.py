@@ -541,6 +541,37 @@ def absolute_pose(n_pairs, n_groups, *, pts0, pts_off0, matches_p, cu_p, X1, x_o
     _call("ltr_absolute_pose", dev, C.byref(inp), C.byref(out))
 
 
+def triangulate(*, kpts, kp_off, segs, seg_off, K, R, t, pairs, matches_p, cu_p, matches_l, cu_l, views, view_off,
+                block_off, inv_off_p, inv_off_l, n_images, n_pairs, total_p, total_l, n_inv_p, n_inv_l, n_blocks,
+                max_views, points3d, lines3d, n_views_p, n_views_l, inv_p, inv_l, thresh=4.0, min_angle=1.5,
+                min_views=2):
+    """ltr_triangulate into caller-allocated outputs: keypoint pool [*,2] / key-line pool [*,2,2] fp32 with image
+    offsets [n+1], K / R [n,3,3] and t [n,3] fp64, pairs [P,2] and match rows int32 with offsets cu_p / cu_l [P+1],
+    the observation lists (views, view_off), the block table block_off [2n+1] and the side-1 index offsets inv_off_*
+    [P+1] int32; points3d [*,3] / lines3d [*,2,3] fp64, n_views_p / n_views_l int32, inv_p / inv_l int32 workspace."""
+    _req_cuda(points3d, "points3d")
+    dev = points3d.device
+    _check_tensors("triangulate", dev, (
+        ("kpts", kpts, torch.float32), ("kp_off", kp_off, torch.int32), ("segs", segs, torch.float32),
+        ("seg_off", seg_off, torch.int32), ("K", K, torch.float64), ("R", R, torch.float64), ("t", t, torch.float64),
+        ("pairs", pairs, torch.int32), ("matches_p", matches_p, torch.int32), ("cu_p", cu_p, torch.int32),
+        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("views", views, torch.int32),
+        ("view_off", view_off, torch.int32), ("block_off", block_off, torch.int32),
+        ("inv_off_p", inv_off_p, torch.int32), ("inv_off_l", inv_off_l, torch.int32),
+        ("points3d", points3d, torch.float64), ("lines3d", lines3d, torch.float64),
+        ("n_views_p", n_views_p, torch.int32), ("n_views_l", n_views_l, torch.int32), ("inv_p", inv_p, torch.int32),
+        ("inv_l", inv_l, torch.int32)))
+    inp = _struct(N.LtrTriangulateInput, kpts=kpts, kp_off=kp_off, segs=segs, seg_off=seg_off, K=K, R=R, t=t,
+                  pairs=pairs, matches_p=matches_p, cu_p=cu_p, matches_l=matches_l, cu_l=cu_l, views=views,
+                  view_off=view_off, block_off=block_off, inv_off_p=inv_off_p, inv_off_l=inv_off_l,
+                  n_images=int(n_images), n_pairs=int(n_pairs), total_p=int(total_p), total_l=int(total_l),
+                  n_inv_p=int(n_inv_p), n_inv_l=int(n_inv_l), n_blocks=int(n_blocks), max_views=int(max_views),
+                  thresh=float(thresh), min_angle=float(min_angle), min_views=int(min_views))
+    out = _struct(N.LtrTriangulateOutput, points3d=points3d, lines3d=lines3d, n_views_p=n_views_p, n_views_l=n_views_l,
+                  inv_p=inv_p, inv_l=inv_l)
+    _call("ltr_triangulate", dev, C.byref(inp), C.byref(out))
+
+
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
     """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
     (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""

@@ -47,6 +47,7 @@ enum KernelClass : int {
   KC_PHOTOMETRIC,
   KC_FUNDAMENTAL,
   KC_ABSOLUTE_POSE,
+  KC_TRIANGULATE,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

@@ -25,6 +25,7 @@
 #include "essential.cuh"
 #include "fundamental.cuh"
 #include "absolute_pose.cuh"
+#include "triangulation.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -45,7 +46,7 @@ const char* kernel_class_name(int kc) {
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
-                                         "fundamental", "absolute_pose"};
+                                         "fundamental", "absolute_pose", "triangulate"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1369,6 +1370,54 @@ int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, in
   }
   LaunchScope ls(KC_ABSOLUTE_POSE, s);
   LTR_CUDA_TRY(launch_pdl(abspose_fit_kernel, dim3(in->n_groups), dim3(AP_FIT_THREADS), (size_t)smem, s, a));
+  return LTR_OK;
+}
+
+static_assert(LTR_TRI_MAX_VIEWS == ltr::TRI_MAX_VIEWS, "LTR_TRI_MAX_VIEWS and the kernels' bound differ");
+
+int ltr_triangulate(const LtrTriangulateInput* in, const LtrTriangulateOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_triangulate: null argument");
+  if (in->n_images < 0 || in->n_pairs < 0 || in->total_p < 0 || in->total_l < 0 || in->n_inv_p < 0 ||
+      in->n_inv_l < 0 || in->n_blocks < 0 || in->max_views < 0)
+    return set_error(LTR_E_INVALID, "ltr_triangulate: negative count");
+  if (in->max_views > LTR_TRI_MAX_VIEWS)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_triangulate: an image takes part in " + std::to_string(in->max_views) +
+                                            " pairs, over " + std::to_string(LTR_TRI_MAX_VIEWS));
+  if (!(in->thresh > 0.0) || !std::isfinite(in->thresh))
+    return set_error(LTR_E_INVALID, "ltr_triangulate: thresh must be finite and > 0");
+  if (!(in->min_angle >= 0.0 && in->min_angle < 90.0))
+    return set_error(LTR_E_INVALID, "ltr_triangulate: min_angle must be in [0, 90) degrees");
+  if (in->min_views < 1 || in->min_views > LTR_TRI_MAX_VIEWS + 1)
+    return set_error(LTR_E_INVALID, "ltr_triangulate: min_views must be in [1, LTR_TRI_MAX_VIEWS + 1]");
+  if (in->n_images == 0 || in->n_blocks == 0) return LTR_OK;
+  if (!in->kp_off || !in->seg_off || !in->K || !in->R || !in->t || !in->view_off || !in->block_off)
+    return set_error(LTR_E_INVALID, "ltr_triangulate: null offsets or cameras");
+  if (!out->points3d || !out->lines3d || !out->n_views_p || !out->n_views_l)
+    return set_error(LTR_E_INVALID, "ltr_triangulate: null output");
+  if (in->n_pairs > 0 && (!in->pairs || !in->views || !in->cu_p || !in->cu_l || !in->inv_off_p || !in->inv_off_l))
+    return set_error(LTR_E_INVALID, "ltr_triangulate: null pairs, observations or match offsets");
+  if ((in->total_p > 0 && !in->matches_p) || (in->total_l > 0 && !in->matches_l) || (in->n_inv_p > 0 && !out->inv_p) ||
+      (in->n_inv_l > 0 && !out->inv_l))
+    return set_error(LTR_E_INVALID, "ltr_triangulate: null matches or index workspace");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  const double rad = in->min_angle * (M_PI / 180.0), sn = std::sin(rad);
+  TriArgs a{in->kpts, in->kp_off, in->segs, in->seg_off, in->K, in->R, in->t, in->pairs, in->matches_p, in->cu_p,
+            in->matches_l, in->cu_l, in->views, in->view_off, in->block_off, in->inv_off_p, in->inv_off_l, out->inv_p,
+            out->inv_l, in->n_images, in->n_pairs, in->total_p, in->total_l, in->thresh * in->thresh, std::cos(rad),
+            sn * sn, in->min_views, out->points3d, out->lines3d, out->n_views_p, out->n_views_l};
+  if (in->n_inv_p > 0) LTR_CUDA_TRY(cudaMemsetAsync(out->inv_p, 0x7f, sizeof(int32_t) * in->n_inv_p, s));
+  if (in->n_inv_l > 0) LTR_CUDA_TRY(cudaMemsetAsync(out->inv_l, 0x7f, sizeof(int32_t) * in->n_inv_l, s));
+  const long long rows = (long long)in->total_p + in->total_l;
+  if (rows > 0) {
+    LaunchScope ls(KC_TRIANGULATE, s);
+    LTR_CUDA_TRY(launch_pdl(tri_scatter_kernel, dim3(cdiv(rows, TRI_SCATTER_THREADS)), dim3(TRI_SCATTER_THREADS), 0,
+                            s, a));
+  }
+  const int smem = (in->max_views > 0 ? in->max_views : 1) * TRI_THREADS * (int)sizeof(float4);
+  LTR_CUDA_TRY(ensure_dynamic_smem(tri_kernel, TRI_MAX_VIEWS * TRI_THREADS * (int)sizeof(float4)));
+  LaunchScope ls(KC_TRIANGULATE, s);
+  LTR_CUDA_TRY(launch_pdl(tri_kernel, dim3(in->n_blocks), dim3(TRI_THREADS), (size_t)smem, s, a));
   return LTR_OK;
 }
 

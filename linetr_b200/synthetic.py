@@ -640,3 +640,89 @@ def make_localization_correspondences(seed: int, n_points: int, n_lines: int, no
     return {"kpts0": f32(kp), "points3d1": to_world(Xc), "matches_p": np.arange(n_points, dtype=np.int32),
             "klines0": f32(segs.reshape(-1, 2, 2)), "lines3d1": to_world(ends.reshape(-1, 3)).reshape(-1, 2, 3),
             "matches_l": np.arange(m, dtype=np.int32), "true_p": ~out_p, "true_l": ~out_l, "R": R, "t": t, "K": K}
+
+
+# ------------------------------------------------------------------ posed views of points and segments (triangulation)
+def make_line_map_set(seed: int, n_views: int, n_points: int, n_lines: int, K=DEFAULT_K, w: int = 640, h: int = 480,
+                      jitter_px: float = 0.0, outlier_frac: float = 0.0, max_angle_deg: float = 6.0,
+                      max_shift: float = 1.2, min_length_px: float = 40.0, min_outlier_px: float = 10.0):
+    """n_views posed views (intrinsics K, world -> camera R [V, 3, 3], t [V, 3] with X_cam = R X + t: a rotation of up
+    to max_angle_deg and a centre within max_shift of the origin, looking down +z) of one scene of n_points 3D points
+    and n_lines 3D segments, 4 to 9 units away, every one seen inside every view.  A segment is at least min_length_px
+    long in every view.  Each view holds its own clipped part of every segment: the sub-segment between parameters
+    a ~ U(0, 0.2) and b ~ U(0.8, 1) of the 3D segment, drawn per view, so partner extents differ.  Row i of every
+    view's keypoints is point i and row l of its key lines is segment l: the ground-truth matches of any pair are the
+    identity.  Keypoints and segment end points are the projections plus N(0, jitter_px); with probability
+    outlier_frac an observation is moved min_outlier_px to 60 px (a keypoint in a random direction, a segment along its
+    normal).  Returns dict keypoints (list of float32 [n_points, 2]), klines (list of float32 [n_lines, 2, 2]), K, R,
+    t, points3d [n_points, 3], segments3d [n_lines, 2, 3], lines3d [V, n_lines, 2, 3] (each view's end points on the
+    true segment), outlier_p [V, n_points] and outlier_l [V, n_lines] (bool)."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    K = np.asarray(K, dtype=np.float64)
+    Ki = np.linalg.inv(K)
+    Rs, ts = [], []
+    for _ in range(n_views):
+        R, _ = random_pose(rng, max_angle_deg)
+        c = rng.uniform(-max_shift, max_shift, 3)
+        Rs.append(R)
+        ts.append(-R @ c)
+    Rs, ts = np.stack(Rs) if n_views else np.zeros((0, 3, 3)), np.stack(ts) if n_views else np.zeros((0, 3))
+
+    def seen(X, margin=0.05):   # [m] inside every view with a margin, depth > 1
+        keep = np.ones(len(X), dtype=bool)
+        for R, t in zip(Rs, ts):
+            q = X @ R.T + t
+            p = _project(K, np.where(q[:, 2:] > 0, q, 1.0))
+            keep &= (q[:, 2] > 1.0) & (p[:, 0] >= margin * w) & (p[:, 0] <= (1 - margin) * w - 1) \
+                & (p[:, 1] >= margin * h) & (p[:, 1] <= (1 - margin) * h - 1)
+        return keep
+
+    def sample(m):
+        x = np.stack([rng.uniform(0.1 * w, 0.9 * w, m), rng.uniform(0.1 * h, 0.9 * h, m), np.ones(m)], 1)
+        return (x @ Ki.T) * rng.uniform(4.0, 9.0, (m, 1))
+
+    X = np.zeros((0, 3))
+    for _ in range(200):
+        if len(X) >= n_points:
+            break
+        Xc = sample(2 * n_points + 8)
+        X = np.concatenate([X, Xc[seen(Xc)]])
+    X = X[:n_points]
+    S = np.zeros((0, 2, 3))
+    for _ in range(400):
+        if len(S) >= n_lines:
+            break
+        m = 4 * (n_lines - len(S)) + 16
+        A = sample(m)
+        u = rng.normal(size=(m, 3))
+        B = A + u / np.linalg.norm(u, axis=1, keepdims=True) * rng.uniform(0.8, 2.5, (m, 1))
+        keep = seen(A) & seen(B)
+        for R, t in zip(Rs, ts):
+            pa, pb = _project(K, A @ R.T + t), _project(K, np.where((B @ R.T + t)[:, 2:] > 0, B @ R.T + t, 1.0))
+            keep &= np.linalg.norm(pb - pa, axis=1) >= min_length_px
+        S = np.concatenate([S, np.stack([A, B], 1)[keep]])
+    S = S[:n_lines]
+    kps, kls, L3 = [], [], []
+    out_p = rng.random((n_views, len(X))) < outlier_frac
+    out_l = rng.random((n_views, len(S))) < outlier_frac
+    for v, (R, t) in enumerate(zip(Rs, ts)):
+        k = _project(K, X @ R.T + t)
+        ang = rng.uniform(0, 2 * np.pi, len(X))
+        mag = rng.uniform(min_outlier_px, max(60.0, min_outlier_px + 1), len(X))
+        k[out_p[v]] += (mag[:, None] * np.stack([np.cos(ang), np.sin(ang)], 1))[out_p[v]]
+        k += rng.normal(0, jitter_px, k.shape) if jitter_px > 0 else 0.0
+        ab = np.stack([rng.uniform(0.0, 0.2, len(S)), rng.uniform(0.8, 1.0, len(S))], 1)
+        E = S[:, :1] + ab[:, :, None] * (S[:, 1:] - S[:, :1])        # [m, 2, 3] this view's end points
+        seg = _project(K, E.reshape(-1, 3) @ R.T + t).reshape(-1, 2, 2)
+        d = seg[:, 1] - seg[:, 0]
+        nrm = np.stack([-d[:, 1], d[:, 0]], 1) / np.maximum(np.linalg.norm(d, axis=1, keepdims=True), 1e-12)
+        shift = nrm * (rng.uniform(min_outlier_px, max(60.0, min_outlier_px + 1), len(S))
+                       * rng.choice([-1.0, 1.0], len(S)))[:, None]
+        seg[out_l[v]] += shift[out_l[v]][:, None, :]
+        seg += rng.normal(0, jitter_px, seg.shape) if jitter_px > 0 else 0.0
+        kps.append(np.ascontiguousarray(k, dtype=np.float32))
+        kls.append(np.ascontiguousarray(seg, dtype=np.float32))
+        L3.append(E)
+    return {"keypoints": kps, "klines": kls, "K": K, "R": Rs, "t": ts, "points3d": X, "segments3d": S,
+            "lines3d": np.stack(L3) if n_views else np.zeros((0, len(S), 2, 3)), "outlier_p": out_p,
+            "outlier_l": out_l}
