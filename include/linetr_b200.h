@@ -799,6 +799,95 @@ typedef struct {
  * capacity) come before any launch.  Two launches: the scatter of the side-1 index, then one thread per row. */
 int ltr_triangulate(const LtrTriangulateInput* in, const LtrTriangulateOutput* out, int32_t device, void* stream);
 
+/* Tracks of posed images: the pair matches that agree with the poses join the rows of all images into point and line
+ * tracks, and each track gets one world point or world line; DESIGN.md "Tracks" states the model:
+ *   - nodes: image i's keypoint k is point node kp_off[i] + k, its key line k line node seg_off[i] + k (two graphs);
+ *   - edges: a match row of pair p = (i, j) whose match m lies in [0, rows of j) and agrees with F[p], the pixel
+ *     fundamental matrix of the poses (x_j^T F x_i = 0, computed by the caller): a point under cv2's FM error below
+ *     epi_thresh, a key line under the epipolar overlap check of ltr_fundamental with min_overlap;
+ *   - tracks: connected components of >= 2 nodes (lock-free union-find, each labelled by its minimum node), numbered in
+ *     ascending order of that node; a track's observations obs[track_off[t] .. track_off[t+1]) ascend by node;
+ *   - candidates (tracks of at most LTR_TRK_MAX_OBS observations): every pair (i, j), i < j in track order, gives
+ *     ltr_triangulate's two-view estimate along observation i's ray(s) from j (depth > 0, triangulation angle >=
+ *     min_angle);
+ *   - support: observation q supports a world point iff its depth is > 0 and its reprojection error is <= thresh (a key
+ *     line: the distance of both world end points to q's infinite line).  The winner has the most supporters, ties to
+ *     the lowest i * LTR_TRK_MAX_OBS + j;
+ *   - refit: 5 Gauss-Newton steps on the 3D point (a key line: each of the anchor's world end points, with the anchor's
+ *     own pixel residuals and the supporters' line distances) over the winner's supporters, kept iff every supporter
+ *     keeps depth > 0 and the supporter count does not fall; the inliers are the supporters of the kept estimate;
+ *   - status: LTR_TRK_OK iff inliers >= min_views; LTR_TRK_TOO_LONG (more than LTR_TRK_MAX_OBS observations),
+ *     LTR_TRK_NO_CANDIDATE, LTR_TRK_TOO_FEW give NaN coordinates.  An inlier row of a valid track gets its track's point
+ *     (a key line: the points of the track's line closest to its own two end-point rays) and n_views = inliers; every
+ *     other row NaN and 0.
+ * Every operation is explicitly rounded fp64 in a fixed order, so the outputs do not depend on the atomics' order. */
+#define LTR_TRK_MAX_OBS 64
+#define LTR_TRK_OK 0
+#define LTR_TRK_TOO_LONG 1
+#define LTR_TRK_NO_CANDIDATE 2
+#define LTR_TRK_TOO_FEW 3
+typedef struct {
+  const float* kpts;              /* device [n_kp, 2] keypoints, image i's rows from kp_off[i] */
+  const int32_t* kp_off;          /* device [n_images + 1] */
+  const float* segs;              /* device [n_kl, 2, 2] key lines (start xy, end xy), image i's rows from seg_off[i] */
+  const int32_t* seg_off;         /* device [n_images + 1] */
+  const double* K;                /* device [n_images, 3, 3] */
+  const double* R;                /* device [n_images, 3, 3] world -> camera */
+  const double* t;                /* device [n_images, 3] */
+  const double* F;                /* device [n_pairs, 3, 3] pixel fundamental matrix of pair p, image pairs[p][0] -> 1 */
+  const int32_t* pairs;           /* device [n_pairs, 2] image indices */
+  const int32_t* matches_p;       /* device: local side-1 keypoint index or -1 per side-0 keypoint row */
+  const int32_t* cu_p;            /* device [n_pairs + 1] */
+  const int32_t* matches_l;       /* device: the same for key lines */
+  const int32_t* cu_l;            /* device [n_pairs + 1] */
+  int32_t n_images;
+  int32_t n_pairs;
+  int32_t total_p;                /* cu_p[n_pairs] (host value) */
+  int32_t total_l;                /* cu_l[n_pairs] */
+  int32_t n_kp;                   /* kp_off[n_images] (host value) */
+  int32_t n_kl;                   /* seg_off[n_images] */
+  double thresh;                  /* pixels (4) */
+  double min_angle;               /* degrees in [0, 90) (1.5) */
+  int32_t min_views;              /* >= 1 (2) */
+  double epi_thresh;              /* pixels (4) */
+  double min_overlap;             /* (0.5) */
+} LtrTracksInput;
+
+/* Outputs (device, caller-owned).  T_p = max(n_kp / 2, 1) and T_l = max(n_kl / 2, 1) bound the track counts; entries
+ * of tracks at or past *n_tracks_* are not written.  workspace: int32 [5 (n_kp + n_kl)]. */
+typedef struct {
+  int32_t* track_p;               /* [n_kp] track of each keypoint row, -1 for none */
+  int32_t* track_l;               /* [n_kl] */
+  int32_t* n_tracks_p;            /* [1] */
+  int32_t* n_tracks_l;            /* [1] */
+  int32_t* track_off_p;           /* [T_p + 1] */
+  int32_t* track_off_l;           /* [T_l + 1] */
+  int32_t* obs_p;                 /* [n_kp] keypoint rows of track t: obs_p[track_off_p[t] .. track_off_p[t+1]) */
+  int32_t* obs_l;                 /* [n_kl] */
+  double* points3d;               /* [T_p, 3] */
+  double* lines3d;                /* [T_l, 2, 3] the anchor observation's two world end points */
+  int32_t* n_obs_p;               /* [T_p] */
+  int32_t* n_obs_l;               /* [T_l] */
+  int32_t* n_inliers_p;           /* [T_p] */
+  int32_t* n_inliers_l;           /* [T_l] */
+  int32_t* n_images_p;            /* [T_p] distinct images among the observations */
+  int32_t* n_images_l;            /* [T_l] */
+  int32_t* status_p;              /* [T_p] LTR_TRK_* */
+  int32_t* status_l;              /* [T_l] */
+  uint8_t* inlier_p;              /* [n_kp] 1 for a supporter of its track's kept estimate */
+  uint8_t* inlier_l;              /* [n_kl] */
+  double* row_points3d;           /* [n_kp, 3] */
+  double* row_lines3d;            /* [n_kl, 2, 3] */
+  int32_t* n_views_p;             /* [n_kp] */
+  int32_t* n_views_l;             /* [n_kl] */
+  int32_t* workspace;
+} LtrTracksOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors (LTR_E_INVALID for bad arguments) come before any launch.  Six
+ * launches: initialisation, edges and unions, path compression, the prefix sum over the roots, the observation slots,
+ * then one persistent grid over the tracks up to the device track count. */
+int ltr_tracks(const LtrTracksInput* in, const LtrTracksOutput* out, int32_t device, void* stream);
+
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where
  * the warped colour image is 0 in every channel, eroded with a 5 x 5 kernel of ones.

@@ -23,6 +23,9 @@ and a Levenberg-Marquardt refit), batched on the GPU, and the localization metri
 Triangulation (triangulation): world points of every keypoint and world end points of every key line of posed images
 from their pair matches (multi-view, with outlier rejection and a Gauss-Newton refit), batched on the GPU:
     triangulate, TriangulationResult
+Tracks (tracks): the pair matches that agree with the poses joined into point and line tracks across a posed image
+set, and one robust multi-view world point or world line per track, batched on the GPU:
+    triangulate_tracks, TrackResult
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
@@ -70,6 +73,8 @@ _LAZY = {
     "lift_to_3d": ("localization", "lift_to_3d"),
     "triangulate": ("triangulation", "triangulate"),
     "TriangulationResult": ("triangulation", "TriangulationResult"),
+    "triangulate_tracks": ("tracks", "triangulate_tracks"),
+    "TrackResult": ("tracks", "TrackResult"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

@@ -24,6 +24,8 @@ ABI_VERSION = 4
 PHOTOMETRIC_PARAMS = 28      # LTR_PHOTOMETRIC_PARAMS
 PHOTOMETRIC_MAX_KSIZE = 149  # LTR_PHOTOMETRIC_MAX_KSIZE
 TRI_MAX_VIEWS = 64           # LTR_TRI_MAX_VIEWS
+TRK_MAX_OBS = 64             # LTR_TRK_MAX_OBS
+TRK_OK, TRK_TOO_LONG, TRK_NO_CANDIDATE, TRK_TOO_FEW = 0, 1, 2, 3   # LTR_TRK_OK .. LTR_TRK_TOO_FEW
 
 
 def photometric_workspace_bytes(n, h, w) -> int:
@@ -199,6 +201,22 @@ class LtrTriangulateOutput(C.Structure):
                 ("inv_p", C.c_void_p), ("inv_l", C.c_void_p)]
 
 
+class LtrTracksInput(C.Structure):
+    _fields_ = [("kpts", C.c_void_p), ("kp_off", C.c_void_p), ("segs", C.c_void_p), ("seg_off", C.c_void_p),
+                ("K", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("F", C.c_void_p), ("pairs", C.c_void_p),
+                ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("matches_l", C.c_void_p), ("cu_l", C.c_void_p),
+                ("n_images", C.c_int32), ("n_pairs", C.c_int32), ("total_p", C.c_int32), ("total_l", C.c_int32),
+                ("n_kp", C.c_int32), ("n_kl", C.c_int32), ("thresh", C.c_double), ("min_angle", C.c_double),
+                ("min_views", C.c_int32), ("epi_thresh", C.c_double), ("min_overlap", C.c_double)]
+
+
+class LtrTracksOutput(C.Structure):
+    _fields_ = [(nm, C.c_void_p) for nm in (
+        "track_p", "track_l", "n_tracks_p", "n_tracks_l", "track_off_p", "track_off_l", "obs_p", "obs_l", "points3d",
+        "lines3d", "n_obs_p", "n_obs_l", "n_inliers_p", "n_inliers_l", "n_images_p", "n_images_l", "status_p",
+        "status_l", "inlier_p", "inlier_l", "row_points3d", "row_lines3d", "n_views_p", "n_views_l", "workspace")]
+
+
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
 # {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
 # of them, and each entry against its C prototype)
@@ -227,6 +245,7 @@ PROTOTYPES = {
     "ltr_fundamental": (C.c_int, [_ptr(LtrFundamentalInput), _ptr(LtrFundamentalOutput), _I32, _P]),
     "ltr_absolute_pose": (C.c_int, [_ptr(LtrAbsPoseInput), _ptr(LtrAbsPoseOutput), _I32, _P]),
     "ltr_triangulate": (C.c_int, [_ptr(LtrTriangulateInput), _ptr(LtrTriangulateOutput), _I32, _P]),
+    "ltr_tracks": (C.c_int, [_ptr(LtrTracksInput), _ptr(LtrTracksOutput), _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),

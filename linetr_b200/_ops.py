@@ -572,6 +572,43 @@ def triangulate(*, kpts, kp_off, segs, seg_off, K, R, t, pairs, matches_p, cu_p,
     _call("ltr_triangulate", dev, C.byref(inp), C.byref(out))
 
 
+_TRACK_OUTPUTS = (("track_p", torch.int32), ("track_l", torch.int32), ("n_tracks_p", torch.int32),
+                  ("n_tracks_l", torch.int32), ("track_off_p", torch.int32), ("track_off_l", torch.int32),
+                  ("obs_p", torch.int32), ("obs_l", torch.int32), ("points3d", torch.float64),
+                  ("lines3d", torch.float64), ("n_obs_p", torch.int32), ("n_obs_l", torch.int32),
+                  ("n_inliers_p", torch.int32), ("n_inliers_l", torch.int32), ("n_images_p", torch.int32),
+                  ("n_images_l", torch.int32), ("status_p", torch.int32), ("status_l", torch.int32),
+                  ("inlier_p", torch.uint8), ("inlier_l", torch.uint8), ("row_points3d", torch.float64),
+                  ("row_lines3d", torch.float64), ("n_views_p", torch.int32), ("n_views_l", torch.int32),
+                  ("workspace", torch.int32))
+
+
+def tracks(*, kpts, kp_off, segs, seg_off, K, R, t, F, pairs, matches_p, cu_p, matches_l, cu_l, n_images, n_pairs,
+           total_p, total_l, n_kp, n_kl, outputs: dict, thresh=4.0, min_angle=1.5, min_views=2, epi_thresh=4.0,
+           min_overlap=0.5):
+    """ltr_tracks into caller-allocated outputs: keypoint pool [*,2] / key-line pool [*,2,2] fp32 with image offsets
+    [n+1], K / R [n,3,3], t [n,3] and the pairs' pixel fundamental matrices F [P,3,3] fp64, pairs [P,2] and match rows
+    int32 with offsets cu_p / cu_l [P+1]; outputs {name: tensor} holds every LtrTracksOutput field (int32 workspace of
+    5 (n_kp + n_kl))."""
+    dev = outputs["workspace"].device
+    _req_cuda(outputs["workspace"], "workspace")
+    _check_tensors("tracks", dev, (
+        ("kpts", kpts, torch.float32), ("kp_off", kp_off, torch.int32), ("segs", segs, torch.float32),
+        ("seg_off", seg_off, torch.int32), ("K", K, torch.float64), ("R", R, torch.float64), ("t", t, torch.float64),
+        ("F", F, torch.float64), ("pairs", pairs, torch.int32), ("matches_p", matches_p, torch.int32),
+        ("cu_p", cu_p, torch.int32), ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32))
+        + tuple((nm, outputs[nm], dt) for nm, dt in _TRACK_OUTPUTS))
+    if outputs["workspace"].numel() < 5 * (int(n_kp) + int(n_kl)):
+        raise N.LtrError("tracks: the workspace must hold 5 (n_kp + n_kl) int32")
+    inp = _struct(N.LtrTracksInput, kpts=kpts, kp_off=kp_off, segs=segs, seg_off=seg_off, K=K, R=R, t=t, F=F,
+                  pairs=pairs, matches_p=matches_p, cu_p=cu_p, matches_l=matches_l, cu_l=cu_l, n_images=int(n_images),
+                  n_pairs=int(n_pairs), total_p=int(total_p), total_l=int(total_l), n_kp=int(n_kp), n_kl=int(n_kl),
+                  thresh=float(thresh), min_angle=float(min_angle), min_views=int(min_views),
+                  epi_thresh=float(epi_thresh), min_overlap=float(min_overlap))
+    out = _struct(N.LtrTracksOutput, **{nm: outputs[nm] for nm, _ in _TRACK_OUTPUTS})
+    _call("ltr_tracks", dev, C.byref(inp), C.byref(out))
+
+
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
     """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
     (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""

@@ -48,6 +48,7 @@ enum KernelClass : int {
   KC_FUNDAMENTAL,
   KC_ABSOLUTE_POSE,
   KC_TRIANGULATE,
+  KC_TRACKS,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

@@ -26,6 +26,7 @@
 #include "fundamental.cuh"
 #include "absolute_pose.cuh"
 #include "triangulation.cuh"
+#include "tracks.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -46,7 +47,7 @@ const char* kernel_class_name(int kc) {
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
-                                         "fundamental", "absolute_pose", "triangulate"};
+                                         "fundamental", "absolute_pose", "triangulate", "tracks"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1418,6 +1419,78 @@ int ltr_triangulate(const LtrTriangulateInput* in, const LtrTriangulateOutput* o
   LTR_CUDA_TRY(ensure_dynamic_smem(tri_kernel, TRI_MAX_VIEWS * TRI_THREADS * (int)sizeof(float4)));
   LaunchScope ls(KC_TRIANGULATE, s);
   LTR_CUDA_TRY(launch_pdl(tri_kernel, dim3(in->n_blocks), dim3(TRI_THREADS), (size_t)smem, s, a));
+  return LTR_OK;
+}
+
+static_assert(LTR_TRK_MAX_OBS == ltr::TRK_MAX_OBS && LTR_TRK_OK == ltr::TRK_OK && LTR_TRK_TOO_LONG == ltr::TRK_TOO_LONG &&
+                  LTR_TRK_NO_CANDIDATE == ltr::TRK_NO_CANDIDATE && LTR_TRK_TOO_FEW == ltr::TRK_TOO_FEW,
+              "the LTR_TRK_* constants and the kernels' differ");
+
+int ltr_tracks(const LtrTracksInput* in, const LtrTracksOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_tracks: null argument");
+  if (in->n_images < 0 || in->n_pairs < 0 || in->total_p < 0 || in->total_l < 0 || in->n_kp < 0 || in->n_kl < 0)
+    return set_error(LTR_E_INVALID, "ltr_tracks: negative count");
+  if ((long long)in->n_kp + in->n_kl > INT_MAX / 5)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_tracks: too many rows for 32-bit node indices");
+  if (!(in->thresh > 0.0) || !std::isfinite(in->thresh) || !(in->epi_thresh > 0.0) || !std::isfinite(in->epi_thresh))
+    return set_error(LTR_E_INVALID, "ltr_tracks: thresh and epi_thresh must be finite and > 0");
+  if (!(in->min_angle >= 0.0 && in->min_angle < 90.0))
+    return set_error(LTR_E_INVALID, "ltr_tracks: min_angle must be in [0, 90) degrees");
+  if (!std::isfinite(in->min_overlap)) return set_error(LTR_E_INVALID, "ltr_tracks: min_overlap must be finite");
+  if (in->min_views < 1) return set_error(LTR_E_INVALID, "ltr_tracks: min_views must be >= 1");
+  if (in->n_images == 0 || (in->n_kp == 0 && in->n_kl == 0)) return LTR_OK;
+  if (!in->kp_off || !in->seg_off || !in->K || !in->R || !in->t)
+    return set_error(LTR_E_INVALID, "ltr_tracks: null offsets or cameras");
+  if (in->n_pairs > 0 && (!in->pairs || !in->F || !in->cu_p || !in->cu_l))
+    return set_error(LTR_E_INVALID, "ltr_tracks: null pairs, fundamental matrices or match offsets");
+  if ((in->total_p > 0 && (!in->matches_p || !in->kpts)) || (in->total_l > 0 && (!in->matches_l || !in->segs)))
+    return set_error(LTR_E_INVALID, "ltr_tracks: null matches or rows");
+  if (!out->track_p || !out->track_l || !out->n_tracks_p || !out->n_tracks_l || !out->track_off_p ||
+      !out->track_off_l || !out->obs_p || !out->obs_l || !out->points3d || !out->lines3d || !out->n_obs_p ||
+      !out->n_obs_l || !out->n_inliers_p || !out->n_inliers_l || !out->n_images_p || !out->n_images_l ||
+      !out->status_p || !out->status_l || !out->inlier_p || !out->inlier_l || !out->row_points3d ||
+      !out->row_lines3d || !out->n_views_p || !out->n_views_l || !out->workspace)
+    return set_error(LTR_E_INVALID, "ltr_tracks: null output or workspace");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  const double rad = in->min_angle * (M_PI / 180.0), sn = std::sin(rad);
+  const int nodes = in->n_kp + in->n_kl;
+  int* ws = out->workspace;
+  TrkArgs a{in->kpts, in->kp_off, in->segs, in->seg_off, in->K, in->R, in->t, in->F, in->pairs, in->matches_p,
+            in->cu_p, in->matches_l, in->cu_l, in->n_images, in->n_pairs, in->total_p, in->total_l,
+            {in->n_kp, in->n_kl}, in->thresh * in->thresh, in->epi_thresh * in->epi_thresh, in->min_overlap,
+            std::cos(rad), sn * sn, in->min_views, ws, ws + nodes, ws + 2 * nodes, ws + 3 * nodes, ws + 4 * nodes,
+            {out->track_p, out->track_l}, {out->n_tracks_p, out->n_tracks_l}, {out->track_off_p, out->track_off_l},
+            {out->obs_p, out->obs_l}, {out->n_obs_p, out->n_obs_l}, {out->n_inliers_p, out->n_inliers_l},
+            {out->n_images_p, out->n_images_l}, {out->status_p, out->status_l}, out->points3d, out->lines3d,
+            out->row_points3d, out->row_lines3d, {out->inlier_p, out->inlier_l}, {out->n_views_p, out->n_views_l}};
+  const dim3 node_grid(cdiv(nodes, TRK_ROW_THREADS)), rows(TRK_ROW_THREADS);
+  {
+    LaunchScope ls(KC_TRACKS, s);
+    LTR_CUDA_TRY(launch_pdl(trk_init_kernel, node_grid, rows, 0, s, a));
+  }
+  const long long edges = (long long)in->total_p + in->total_l;
+  if (edges > 0) {
+    LaunchScope ls(KC_TRACKS, s);
+    LTR_CUDA_TRY(launch_pdl(trk_edge_kernel, dim3(cdiv(edges, TRK_ROW_THREADS)), rows, 0, s, a));
+  }
+  {
+    LaunchScope ls(KC_TRACKS, s);
+    LTR_CUDA_TRY(launch_pdl(trk_root_kernel, node_grid, rows, 0, s, a));
+  }
+  {
+    LaunchScope ls(KC_TRACKS, s);
+    LTR_CUDA_TRY(launch_pdl(trk_scan_kernel, dim3(2), dim3(TRK_SCAN_THREADS), 0, s, a));
+  }
+  {
+    LaunchScope ls(KC_TRACKS, s);
+    LTR_CUDA_TRY(launch_pdl(trk_assign_kernel, node_grid, rows, 0, s, a));
+  }
+  // persistent: enough CTAs for the larger bound, at most 8 per SM
+  const int bound = std::max(in->n_kp / 2, in->n_kl / 2);
+  const int ctas = std::max(1, std::min(bound, 8 * device_sm_count()));
+  LaunchScope ls(KC_TRACKS, s);
+  LTR_CUDA_TRY(launch_pdl(trk_kernel, dim3(ctas, 2), dim3(TRK_THREADS), 0, s, a));
   return LTR_OK;
 }
 

@@ -54,65 +54,71 @@ class _Set:
     view_off: np.ndarray     # int32 [n + 1]
 
 
-def _rows(items, width, what):
+def _rows(items, width, what, who="triangulate"):
     n = []
     for i, k in enumerate(items):
         shape = tuple(k.shape) if hasattr(k, "shape") else np.shape(k)
         m = shape[0] if len(shape) else 0
         if int(np.prod(shape)) != m * width:
-            raise N.LtrError(f"triangulate: {what}[{i}] must hold {width} coordinates per row, got shape {list(shape)}")
+            raise N.LtrError(f"{who}: {what}[{i}] must hold {width} coordinates per row, got shape {list(shape)}")
         n.append(m)
     return np.array(n, dtype=np.int64)
 
 
-def _check(keypoints, klines, pairs, res, K, R, t) -> _Set:
-    """The argument checks of `triangulate` (all on the host, before any device work) -> the set's host tables."""
+def _check(keypoints, klines, pairs, res, K, R, t, who="triangulate") -> _Set:
+    """The argument checks shared by `triangulate` and `tracks.triangulate_tracks` (all on the host, before any device
+    work; messages start with `who`) -> the set's host tables."""
     n = len(keypoints)
     if len(klines) != n:
-        raise N.LtrError(f"triangulate: {n} keypoint arrays but {len(klines)} key-line arrays")
-    n_kp, n_kl = _rows(keypoints, 2, "keypoints"), _rows(klines, 4, "klines")
+        raise N.LtrError(f"{who}: {n} keypoint arrays but {len(klines)} key-line arrays")
+    n_kp, n_kl = _rows(keypoints, 2, "keypoints", who), _rows(klines, 4, "klines", who)
     pr = _host(pairs, np.int64)
     if pr.size == 0:
         pr = pr.reshape(0, 2)
     if pr.ndim != 2 or pr.shape[1] != 2:
-        raise N.LtrError(f"triangulate: pairs must be [P, 2], got {list(pr.shape)}")
+        raise N.LtrError(f"{who}: pairs must be [P, 2], got {list(pr.shape)}")
     P = len(pr)
     if P != res.n_pairs:
-        raise N.LtrError(f"triangulate: {P} pairs but the matches hold {res.n_pairs}")
+        raise N.LtrError(f"{who}: {P} pairs but the matches hold {res.n_pairs}")
     if P and (pr.min() < 0 or pr.max() >= n):
-        raise N.LtrError(f"triangulate: pair indices must lie in [0, {n})")
+        raise N.LtrError(f"{who}: pair indices must lie in [0, {n})")
     if (pr[:, 0] == pr[:, 1]).any():
-        raise N.LtrError(f"triangulate: pair {int(np.flatnonzero(pr[:, 0] == pr[:, 1])[0])} is a self pair")
+        raise N.LtrError(f"{who}: pair {int(np.flatnonzero(pr[:, 0] == pr[:, 1])[0])} is a self pair")
     key = np.sort(pr, 1)
     if len(np.unique(key[:, 0] * max(n, 1) + key[:, 1])) != P:
-        raise N.LtrError("triangulate: an unordered pair is listed twice")
+        raise N.LtrError(f"{who}: an unordered pair is listed twice")
     op, ol = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
     for nm, off, cnt0, side1, cnt1 in (("keypoint", op, n_kp, res.keypoints1, n_kp), ("key-line", ol, n_kl, res.klines1, n_kl)):
         bad = np.flatnonzero(np.diff(off) != cnt0[pr[:, 0]])
         if len(bad):
-            raise N.LtrError(f"triangulate: pair {int(bad[0])} has {int(np.diff(off)[bad[0]])} {nm} match rows for "
+            raise N.LtrError(f"{who}: pair {int(bad[0])} has {int(np.diff(off)[bad[0]])} {nm} match rows for "
                              f"{int(cnt0[pr[bad[0], 0]])} {nm}s of image {int(pr[bad[0], 0])}")
         for p in range(P):
             if len(side1[p]) != cnt1[pr[p, 1]]:
-                raise N.LtrError(f"triangulate: side 1 of pair {p} has {len(side1[p])} {nm}s, image {int(pr[p, 1])} "
+                raise N.LtrError(f"{who}: side 1 of pair {p} has {len(side1[p])} {nm}s, image {int(pr[p, 1])} "
                                  f"{int(cnt1[pr[p, 1]])}")
     Kn = _intrinsics(K, n, "K")
     Rn, tn = _host(R, np.float64), _host(t, np.float64)
     if Rn.shape != (n, 3, 3) or tn.shape != (n, 3):
-        raise N.LtrError(f"triangulate: R must be [{n}, 3, 3] and t [{n}, 3], got {list(Rn.shape)} and {list(tn.shape)}")
+        raise N.LtrError(f"{who}: R must be [{n}, 3, 3] and t [{n}, 3], got {list(Rn.shape)} and {list(tn.shape)}")
     if not (np.isfinite(Rn).all() and np.isfinite(tn).all()):
-        raise N.LtrError("triangulate: R and t must be finite")
+        raise N.LtrError(f"{who}: R and t must be finite")
     img = np.concatenate([pr[:, 0], pr[:, 1]])
     code = np.concatenate([2 * np.arange(P), 2 * np.arange(P) + 1])
     order = np.lexsort((code, img))
     cnt = np.bincount(img, minlength=n)
-    if n and cnt.max(initial=0) > TRI_MAX_VIEWS:
-        bad = int(np.argmax(cnt))
-        raise N.LtrError(f"triangulate: image {bad} takes part in {int(cnt[bad])} pairs, more than LTR_TRI_MAX_VIEWS "
-                         f"({TRI_MAX_VIEWS})")
     view_off = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int32)
     return _Set(pr.astype(np.int32), Kn, np.ascontiguousarray(Rn), np.ascontiguousarray(tn), n_kp, n_kl,
                 code[order].astype(np.int32), view_off)
+
+
+def _check_views(S: _Set):
+    """`triangulate`'s capacity: at most LTR_TRI_MAX_VIEWS pairs per image (tracks have no such limit)."""
+    cnt = np.diff(S.view_off)
+    if len(cnt) and cnt.max(initial=0) > TRI_MAX_VIEWS:
+        bad = int(np.argmax(cnt))
+        raise N.LtrError(f"triangulate: image {bad} takes part in {int(cnt[bad])} pairs, more than LTR_TRI_MAX_VIEWS "
+                         f"({TRI_MAX_VIEWS})")
 
 
 # ------------------------------------------------------------------ the model in numpy
@@ -252,6 +258,7 @@ def triangulate_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_ang
     depth_l, NaN where not valid) and refit_p / refit_l (the Gauss-Newton refit was kept); views / view_off list each
     image's observations (pair << 1 | side) in order."""
     S = _check(keypoints, klines, pairs, res, K, R, t)
+    _check_views(S)
     if not (float(thresh) > 0 and math.isfinite(float(thresh))) or not (0 <= float(min_angle) < 90) or int(min_views) < 1:
         raise N.LtrError("triangulate: thresh must be finite and > 0, min_angle in [0, 90) and min_views >= 1")
     n = len(keypoints)
@@ -397,6 +404,7 @@ def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.
     Raises LtrError before any device work for bad K, R or t, a pair list that disagrees with res, self or duplicate
     pairs, and an image in more than LTR_TRI_MAX_VIEWS pairs."""
     S = _check(keypoints, klines, pairs, res, K, R, t)
+    _check_views(S)
     n, P = len(keypoints), len(S.pairs)
     dev = res.matches_p.device
     op, ol = _offsets(S.n_kp), _offsets(S.n_kl)
