@@ -888,6 +888,100 @@ typedef struct {
  * then one persistent grid over the tracks up to the device track count. */
 int ltr_tracks(const LtrTracksInput* in, const LtrTracksOutput* out, int32_t device, void* stream);
 
+/* Bundle adjustment of a posed image set over the tracks of ltr_tracks: the camera poses, the world points of the
+ * point tracks and the world lines of the line tracks refined together; DESIGN.md "Bundle adjustment" states the model:
+ *   - participation: a track takes part (LTR_BA_IN) iff its ltr_tracks status is LTR_TRK_OK, its inlier rows lie in
+ *     distinct images (else LTR_BA_SAME_IMAGE) and every pivot of the Cholesky of its undamped initial landmark block is
+ *     > 1e-12 times its diagonal entry (else LTR_BA_DEGENERATE); any other track is LTR_BA_NOT_VALID.  Its inlier rows
+ *     are its residual blocks;
+ *   - residuals (pixels): a point row's two reprojection errors, a key-line row the signed distances n . P / P_z of the
+ *     track's two world end points to the row's infinite line; the cost is their sum of squares;
+ *   - parameters: camera R <- cay(w) R, C <- C + dC (t = -R C); point 3 DoF; line 4 DoF, each end point moving in the
+ *     plane orthogonal to the line's direction;
+ *   - gauge: images with fixed[i] != 0 keep their input bits; with n_fixed == 1, the lowest free image k with a
+ *     participating row also holds its centre coordinate hold[k] (the caller's choice: the first-largest |C_k - C_f|);
+ *   - solver: Levenberg-Marquardt (A + lambda diag A, lambda from 1e-3, x0.1 after an accepted step, x10 after a
+ *     rejected one) with a Schur complement onto the cameras, a dense Cholesky of the reduced camera matrix in one CTA;
+ *     a step is accepted iff every factorization succeeds, every participating depth stays > 0 and the cost falls; the
+ *     adjustment stops after an accepted step with relative decrease <= ftol, when lambda > 1e32 or after max_iters
+ *     iterations.
+ * Every operation is explicitly rounded fp64 in a fixed order, so two calls give the same bits. */
+#define LTR_BA_MAX_IMAGES 128
+#define LTR_BA_MAX_ITERS 1000
+#define LTR_BA_IN 0
+#define LTR_BA_NOT_VALID 1
+#define LTR_BA_SAME_IMAGE 2
+#define LTR_BA_DEGENERATE 3
+#define LTR_BA_STOP_ITERS 0
+#define LTR_BA_STOP_FTOL 1
+#define LTR_BA_STOP_LAMBDA 2
+#define LTR_BA_STATS 8
+typedef struct {
+  const float* kpts;              /* device [n_kp, 2], as ltr_tracks */
+  const int32_t* kp_off;          /* device [n_images + 1] */
+  const float* segs;              /* device [n_kl, 2, 2] */
+  const int32_t* seg_off;         /* device [n_images + 1] */
+  const double* K;                /* device [n_images, 3, 3] */
+  const double* R;                /* device [n_images, 3, 3] world -> camera */
+  const double* t;                /* device [n_images, 3] */
+  const int32_t* hold;            /* device [n_images] the held centre coordinate (0..2) of each image (n_fixed == 1) */
+  const int32_t* fixed;           /* device [n_images] 1 = the pose is held */
+  const int32_t* n_tracks_p;      /* device [1]: the ltr_tracks outputs of the same set */
+  const int32_t* n_tracks_l;
+  const int32_t* track_off_p;
+  const int32_t* track_off_l;
+  const int32_t* obs_p;
+  const int32_t* obs_l;
+  const int32_t* status_p;        /* LTR_TRK_* */
+  const int32_t* status_l;
+  const uint8_t* inlier_p;
+  const uint8_t* inlier_l;
+  const int32_t* track_p;
+  const int32_t* track_l;
+  const int32_t* n_views_p;
+  const int32_t* n_views_l;
+  const double* points3d;         /* [t_p, 3] */
+  const double* lines3d;          /* [t_l, 2, 3] */
+  int32_t n_images;               /* <= LTR_BA_MAX_IMAGES */
+  int32_t n_fixed;                /* >= 1: images with fixed[i] != 0 */
+  int32_t n_kp;                   /* kp_off[n_images] (host value) */
+  int32_t n_kl;                   /* seg_off[n_images] */
+  int32_t t_p;                    /* the ltr_tracks bounds max(n_kp / 2, 1), max(n_kl / 2, 1) */
+  int32_t t_l;
+  int32_t max_iters;              /* in [0, LTR_BA_MAX_ITERS] (50): 5 launches each are enqueued, whatever the stop */
+  double ftol;                    /* finite, >= 0 (1e-10) */
+} LtrBundleInput;
+
+/* Outputs (device, caller-owned).  Entries of tracks at or past *n_tracks_* are not written.  stats fp64
+ * [LTR_BA_STATS]: initial cost, final cost, final lambda, iterations, accepted steps, stop reason (LTR_BA_STOP_*),
+ * participating observations, participating tracks.  workspace: LTR_BA_WORKSPACE_BYTES(n_images, n_kp, n_kl, t_p, t_l)
+ * bytes, 8-byte aligned. */
+#define LTR_BA_WORKSPACE_BYTES(n, n_kp, n_kl, t_p, t_l)                                                            \
+  (8 * (64 * ((int64_t)(n_kp) + (n_kl)) + 40 * ((int64_t)(t_p) + (t_l)) + 36 * (int64_t)(n) * (n) + 60 * (int64_t)(n) + \
+        16) +                                                                                                        \
+   4 * (2 * ((int64_t)(n_kp) + (n_kl)) + 4 * ((int64_t)(t_p) + (t_l)) + 7 * (int64_t)(n) + 24) + (int64_t)(n))
+typedef struct {
+  double* R;                      /* [n_images, 3, 3]: the input bits for an image whose pose did not move */
+  double* t;                      /* [n_images, 3] */
+  double* points3d;               /* [t_p, 3]: refined for LTR_BA_IN tracks, the input otherwise */
+  double* lines3d;                /* [t_l, 2, 3] */
+  int32_t* status_p;              /* [t_p] LTR_BA_* */
+  int32_t* status_l;              /* [t_l] */
+  double* residual_p;             /* [n_kp] a participating row's reprojection error after the adjustment, else NaN */
+  double* residual_l;             /* [n_kl] the larger end-point distance of a participating key-line row, else NaN */
+  double* row_points3d;           /* [n_kp, 3] as ltr_tracks' rows, under the refined poses */
+  double* row_lines3d;            /* [n_kl, 2, 3] */
+  int32_t* n_views_p;             /* [n_kp] */
+  int32_t* n_views_l;             /* [n_kl] */
+  double* stats;                  /* [LTR_BA_STATS] */
+  void* workspace;
+} LtrBundleOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors come before any launch: LTR_E_INVALID for bad arguments,
+ * LTR_E_UNSUPPORTED for more than LTR_BA_MAX_IMAGES images.  Three set-up launches, five per iteration (max_iters of
+ * them; each returns at once after the stop) and one for the outputs. */
+int ltr_bundle_adjust(const LtrBundleInput* in, const LtrBundleOutput* out, int32_t device, void* stream);
+
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where
  * the warped colour image is 0 in every channel, eroded with a 5 x 5 kernel of ones.

@@ -26,6 +26,9 @@ from their pair matches (multi-view, with outlier rejection and a Gauss-Newton r
 Tracks (tracks): the pair matches that agree with the poses joined into point and line tracks across a posed image
 set, and one robust multi-view world point or world line per track, batched on the GPU:
     triangulate_tracks, TrackResult
+Bundle adjustment (bundle): the poses of a posed image set and the world points and lines of its tracks refined
+together (Levenberg-Marquardt with a Schur complement onto the cameras), on the GPU:
+    bundle_adjust, BundleResult
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
@@ -75,6 +78,8 @@ _LAZY = {
     "TriangulationResult": ("triangulation", "TriangulationResult"),
     "triangulate_tracks": ("tracks", "triangulate_tracks"),
     "TrackResult": ("tracks", "TrackResult"),
+    "bundle_adjust": ("bundle", "bundle_adjust"),
+    "BundleResult": ("bundle", "BundleResult"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

@@ -26,6 +26,17 @@ PHOTOMETRIC_MAX_KSIZE = 149  # LTR_PHOTOMETRIC_MAX_KSIZE
 TRI_MAX_VIEWS = 64           # LTR_TRI_MAX_VIEWS
 TRK_MAX_OBS = 64             # LTR_TRK_MAX_OBS
 TRK_OK, TRK_TOO_LONG, TRK_NO_CANDIDATE, TRK_TOO_FEW = 0, 1, 2, 3   # LTR_TRK_OK .. LTR_TRK_TOO_FEW
+BA_MAX_IMAGES = 128          # LTR_BA_MAX_IMAGES
+BA_MAX_ITERS = 1000          # LTR_BA_MAX_ITERS
+BA_IN, BA_NOT_VALID, BA_SAME_IMAGE, BA_DEGENERATE = 0, 1, 2, 3     # LTR_BA_IN .. LTR_BA_DEGENERATE
+BA_STOP_ITERS, BA_STOP_FTOL, BA_STOP_LAMBDA = 0, 1, 2              # LTR_BA_STOP_ITERS .. LTR_BA_STOP_LAMBDA
+BA_STATS = 8                 # LTR_BA_STATS
+
+
+def ba_workspace_bytes(n_images, n_kp, n_kl, t_p, t_l) -> int:
+    """LTR_BA_WORKSPACE_BYTES(n_images, n_kp, n_kl, t_p, t_l)."""
+    n, rows, trk = int(n_images), int(n_kp) + int(n_kl), int(t_p) + int(t_l)
+    return 8 * (64 * rows + 40 * trk + 36 * n * n + 60 * n + 16) + 4 * (2 * rows + 4 * trk + 7 * n + 24) + n
 
 
 def photometric_workspace_bytes(n, h, w) -> int:
@@ -217,6 +228,21 @@ class LtrTracksOutput(C.Structure):
         "status_l", "inlier_p", "inlier_l", "row_points3d", "row_lines3d", "n_views_p", "n_views_l", "workspace")]
 
 
+class LtrBundleInput(C.Structure):
+    _fields_ = [(nm, C.c_void_p) for nm in (
+        "kpts", "kp_off", "segs", "seg_off", "K", "R", "t", "hold", "fixed", "n_tracks_p", "n_tracks_l", "track_off_p",
+        "track_off_l", "obs_p", "obs_l", "status_p", "status_l", "inlier_p", "inlier_l", "track_p", "track_l",
+        "n_views_p", "n_views_l", "points3d", "lines3d")] + [
+        (nm, C.c_int32) for nm in ("n_images", "n_fixed", "n_kp", "n_kl", "t_p", "t_l", "max_iters")] + [
+        ("ftol", C.c_double)]
+
+
+class LtrBundleOutput(C.Structure):
+    _fields_ = [(nm, C.c_void_p) for nm in (
+        "R", "t", "points3d", "lines3d", "status_p", "status_l", "residual_p", "residual_l", "row_points3d",
+        "row_lines3d", "n_views_p", "n_views_l", "stats", "workspace")]
+
+
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
 # {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
 # of them, and each entry against its C prototype)
@@ -246,6 +272,7 @@ PROTOTYPES = {
     "ltr_absolute_pose": (C.c_int, [_ptr(LtrAbsPoseInput), _ptr(LtrAbsPoseOutput), _I32, _P]),
     "ltr_triangulate": (C.c_int, [_ptr(LtrTriangulateInput), _ptr(LtrTriangulateOutput), _I32, _P]),
     "ltr_tracks": (C.c_int, [_ptr(LtrTracksInput), _ptr(LtrTracksOutput), _I32, _P]),
+    "ltr_bundle_adjust": (C.c_int, [_ptr(LtrBundleInput), _ptr(LtrBundleOutput), _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),

@@ -609,6 +609,38 @@ def tracks(*, kpts, kp_off, segs, seg_off, K, R, t, F, pairs, matches_p, cu_p, m
     _call("ltr_tracks", dev, C.byref(inp), C.byref(out))
 
 
+_BUNDLE_INPUTS = (("kpts", torch.float32), ("kp_off", torch.int32), ("segs", torch.float32), ("seg_off", torch.int32),
+                  ("K", torch.float64), ("R", torch.float64), ("t", torch.float64), ("hold", torch.int32),
+                  ("fixed", torch.int32), ("n_tracks_p", torch.int32), ("n_tracks_l", torch.int32),
+                  ("track_off_p", torch.int32), ("track_off_l", torch.int32), ("obs_p", torch.int32),
+                  ("obs_l", torch.int32), ("status_p", torch.int32), ("status_l", torch.int32),
+                  ("inlier_p", torch.uint8), ("inlier_l", torch.uint8), ("track_p", torch.int32),
+                  ("track_l", torch.int32), ("n_views_p", torch.int32), ("n_views_l", torch.int32),
+                  ("points3d", torch.float64), ("lines3d", torch.float64))
+_BUNDLE_OUTPUTS = (("R", torch.float64), ("t", torch.float64), ("points3d", torch.float64), ("lines3d", torch.float64),
+                   ("status_p", torch.int32), ("status_l", torch.int32), ("residual_p", torch.float64),
+                   ("residual_l", torch.float64), ("row_points3d", torch.float64), ("row_lines3d", torch.float64),
+                   ("n_views_p", torch.int32), ("n_views_l", torch.int32), ("stats", torch.float64),
+                   ("workspace", torch.float64))
+
+
+def bundle_adjust(*, inputs: dict, outputs: dict, n_images, n_fixed, n_kp, n_kl, t_p, t_l, max_iters=50, ftol=1e-10):
+    """ltr_bundle_adjust into caller-allocated outputs: inputs {name: tensor} holds every LtrBundleInput pointer field
+    (the set's rows and cameras, the held coordinates and fixed flags, and the ltr_tracks outputs), outputs every
+    LtrBundleOutput field (an fp64 workspace of at least LTR_BA_WORKSPACE_BYTES)."""
+    dev = outputs["workspace"].device
+    _req_cuda(outputs["workspace"], "workspace")
+    _check_tensors("bundle_adjust", dev, tuple((nm, inputs[nm], dt) for nm, dt in _BUNDLE_INPUTS)
+                   + tuple((nm, outputs[nm], dt) for nm, dt in _BUNDLE_OUTPUTS))
+    if outputs["workspace"].numel() * 8 < N.ba_workspace_bytes(n_images, n_kp, n_kl, t_p, t_l):
+        raise N.LtrError("bundle_adjust: the workspace is smaller than LTR_BA_WORKSPACE_BYTES")
+    inp = _struct(N.LtrBundleInput, **{nm: inputs[nm] for nm, _ in _BUNDLE_INPUTS}, n_images=int(n_images),
+                  n_fixed=int(n_fixed), n_kp=int(n_kp), n_kl=int(n_kl), t_p=int(t_p), t_l=int(t_l),
+                  max_iters=int(max_iters), ftol=float(ftol))
+    out = _struct(N.LtrBundleOutput, **{nm: outputs[nm] for nm, _ in _BUNDLE_OUTPUTS})
+    _call("ltr_bundle_adjust", dev, C.byref(inp), C.byref(out))
+
+
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):
     """ltr_warp_pairs into caller-allocated outputs: gray uint8 [N,h,w], colour uint8 [N,h,w,C], src_index int32 [P]
     (host copy and device copy), inv_maps fp64 [P,9] on the device; warped / mask uint8 [P,h,w]."""

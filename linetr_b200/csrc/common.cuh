@@ -49,6 +49,7 @@ enum KernelClass : int {
   KC_ABSOLUTE_POSE,
   KC_TRIANGULATE,
   KC_TRACKS,
+  KC_BUNDLE,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

@@ -27,6 +27,7 @@
 #include "absolute_pose.cuh"
 #include "triangulation.cuh"
 #include "tracks.cuh"
+#include "bundle.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -47,7 +48,8 @@ const char* kernel_class_name(int kc) {
                                          "dist", "segmean", "argmin", "mutual", "token_fused",
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
-                                         "fundamental", "absolute_pose", "triangulate", "tracks"};
+                                         "fundamental", "absolute_pose", "triangulate", "tracks",
+                                         "bundle"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1491,6 +1493,89 @@ int ltr_tracks(const LtrTracksInput* in, const LtrTracksOutput* out, int32_t dev
   const int ctas = std::max(1, std::min(bound, 8 * device_sm_count()));
   LaunchScope ls(KC_TRACKS, s);
   LTR_CUDA_TRY(launch_pdl(trk_kernel, dim3(ctas, 2), dim3(TRK_THREADS), 0, s, a));
+  return LTR_OK;
+}
+
+static_assert(LTR_BA_MAX_IMAGES == ltr::BA_MAX_IMAGES && LTR_BA_IN == ltr::BA_IN &&
+                  LTR_BA_NOT_VALID == ltr::BA_NOT_VALID && LTR_BA_SAME_IMAGE == ltr::BA_SAME_IMAGE &&
+                  LTR_BA_DEGENERATE == ltr::BA_DEGENERATE && LTR_BA_STOP_ITERS == ltr::BA_STOP_ITERS &&
+                  LTR_BA_STOP_FTOL == ltr::BA_STOP_FTOL && LTR_BA_STOP_LAMBDA == ltr::BA_STOP_LAMBDA,
+              "the LTR_BA_* constants and the kernels' differ");
+
+int ltr_bundle_adjust(const LtrBundleInput* in, const LtrBundleOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_bundle_adjust: null argument");
+  if (in->n_images < 1 || in->n_kp < 0 || in->n_kl < 0 || in->t_p < 1 || in->t_l < 1)
+    return set_error(LTR_E_INVALID, "ltr_bundle_adjust: n_images and the track bounds must be >= 1, rows >= 0");
+  if (in->n_images > LTR_BA_MAX_IMAGES)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_bundle_adjust: more than LTR_BA_MAX_IMAGES images");
+  if ((long long)in->n_kp + in->n_kl > INT_MAX / 64)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_bundle_adjust: too many rows");
+  if (in->n_fixed < 1 || in->n_fixed > in->n_images)
+    return set_error(LTR_E_INVALID, "ltr_bundle_adjust: at least one image must be fixed");
+  if (in->max_iters < 0 || in->max_iters > LTR_BA_MAX_ITERS)
+    return set_error(LTR_E_INVALID, "ltr_bundle_adjust: max_iters must lie in [0, LTR_BA_MAX_ITERS]");
+  if (!std::isfinite(in->ftol) || !(in->ftol >= 0.0))
+    return set_error(LTR_E_INVALID, "ltr_bundle_adjust: ftol must be finite and >= 0");
+  if (!in->kp_off || !in->seg_off || !in->K || !in->R || !in->t || !in->hold || !in->fixed || !in->n_tracks_p ||
+      !in->n_tracks_l || !in->track_off_p || !in->track_off_l || !in->status_p || !in->status_l || !in->points3d ||
+      !in->lines3d || !in->kpts || !in->segs || !in->obs_p || !in->obs_l || !in->inlier_p || !in->inlier_l ||
+      !in->track_p || !in->track_l || !in->n_views_p || !in->n_views_l)
+    return set_error(LTR_E_INVALID, "ltr_bundle_adjust: null input");
+  if (!out->R || !out->t || !out->points3d || !out->lines3d || !out->status_p || !out->status_l || !out->residual_p ||
+      !out->residual_l || !out->row_points3d || !out->row_lines3d || !out->n_views_p || !out->n_views_l ||
+      !out->stats || !out->workspace)
+    return set_error(LTR_E_INVALID, "ltr_bundle_adjust: null output or workspace");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  const int n = in->n_images, rows = in->n_kp + in->n_kl, trk = in->t_p + in->t_l;
+  char* w = static_cast<char*>(out->workspace);
+  auto take = [&](size_t bytes) {
+    char* p = w;
+    w += bytes;
+    return p;
+  };
+  BaArgs a{};
+  a.kpts = in->kpts; a.kp_off = in->kp_off; a.segs = in->segs; a.seg_off = in->seg_off;
+  a.K = in->K; a.R0 = in->R; a.t0 = in->t; a.hold = in->hold; a.fixed = in->fixed;
+  a.n_images = n; a.n_fixed = in->n_fixed; a.n_nodes[0] = in->n_kp; a.n_nodes[1] = in->n_kl;
+  a.t_bound[0] = in->t_p; a.t_bound[1] = in->t_l; a.max_iters = in->max_iters; a.ftol = in->ftol;
+  a.n_tracks[0] = in->n_tracks_p; a.n_tracks[1] = in->n_tracks_l;
+  a.track_off[0] = in->track_off_p; a.track_off[1] = in->track_off_l; a.obs[0] = in->obs_p; a.obs[1] = in->obs_l;
+  a.trk_status[0] = in->status_p; a.trk_status[1] = in->status_l; a.inlier[0] = in->inlier_p;
+  a.inlier[1] = in->inlier_l; a.track_row[0] = in->track_p; a.track_row[1] = in->track_l;
+  a.n_views_in[0] = in->n_views_p; a.n_views_in[1] = in->n_views_l; a.X_in[0] = in->points3d;
+  a.X_in[1] = in->lines3d;
+  a.R = out->R; a.t = out->t; a.X_out[0] = out->points3d; a.X_out[1] = out->lines3d; a.status[0] = out->status_p;
+  a.status[1] = out->status_l; a.residual[0] = out->residual_p; a.residual[1] = out->residual_l;
+  a.row_points = out->row_points3d; a.row_lines = out->row_lines3d; a.n_views[0] = out->n_views_p;
+  a.n_views[1] = out->n_views_l; a.stats = out->stats;
+  a.row = reinterpret_cast<double*>(take(8ull * BA_ROW * rows));
+  a.trk = reinterpret_cast<double*>(take(8ull * BA_TRK * trk));
+  a.A = reinterpret_cast<double*>(take(8ull * 36 * n * n));
+  a.cam = reinterpret_cast<double*>(take(8ull * BA_CAM * n));
+  a.rhs = reinterpret_cast<double*>(take(8ull * 12 * n));
+  a.sd = reinterpret_cast<double*>(take(8ull * 16));
+  a.list = reinterpret_cast<int*>(take(4ull * 2 * rows));
+  a.mask = reinterpret_cast<unsigned*>(take(4ull * 4 * trk));
+  a.list_off = reinterpret_cast<int*>(take(4ull * (n + 1)));
+  a.col = reinterpret_cast<int*>(take(4ull * 6 * n));
+  a.si = reinterpret_cast<int*>(take(4ull * 23));
+  a.part = reinterpret_cast<uint8_t*>(take(n));
+  const int sms = device_sm_count();
+  const dim3 tg(std::max(1, std::min(cdiv(trk, BA_THREADS), 4 * sms))), tb(BA_THREADS);
+  LaunchScope ls(KC_BUNDLE, s);
+  LTR_CUDA_TRY(launch_pdl(ba_start_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
+  LTR_CUDA_TRY(launch_pdl(ba_init_kernel, tg, tb, 0, s, a));
+  LTR_CUDA_TRY(launch_pdl(ba_setup_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
+  for (int it = 0; it < in->max_iters; ++it) {
+    LTR_CUDA_TRY(launch_pdl(ba_track_kernel, tg, tb, 0, s, a));
+    LTR_CUDA_TRY(launch_pdl(ba_reduce_kernel, dim3(n, n), dim3(64), 0, s, a));
+    LTR_CUDA_TRY(launch_pdl(ba_solve_kernel, dim3(1), dim3(BA_CTA_THREADS), 0, s, a));
+    LTR_CUDA_TRY(launch_pdl(ba_update_kernel, tg, tb, 0, s, a));
+    LTR_CUDA_TRY(launch_pdl(ba_accept_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
+  }
+  const dim3 fg(std::max(1, std::min(cdiv(std::max(rows, trk), BA_THREADS), 4 * sms)));
+  LTR_CUDA_TRY(launch_pdl(ba_finish_kernel, fg, tb, 0, s, a));
   return LTR_OK;
 }
 
