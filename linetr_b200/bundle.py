@@ -30,16 +30,16 @@ import torch
 
 from . import _native as N
 from . import _ops
-from .localization import _block_sum
-from .triangulation import TriangulationResult, _host, _offsets, _pool_rows, _rows
-from .geometry import _intrinsics
+from ._posed import (block_sum, cayley, centre, check_poses, closest_on_line, cross3, dot3, line_normal, offsets,
+                     pool64, ray, row_counts, stage_with_pools)
+from .triangulation import TriangulationResult
 
 BA_MAX_IMAGES, BA_MAX_ITERS = N.BA_MAX_IMAGES, N.BA_MAX_ITERS
 BA_IN, BA_NOT_VALID, BA_SAME_IMAGE, BA_DEGENERATE = N.BA_IN, N.BA_NOT_VALID, N.BA_SAME_IMAGE, N.BA_DEGENERATE
 BA_STOP_ITERS, BA_STOP_FTOL, BA_STOP_LAMBDA = N.BA_STOP_ITERS, N.BA_STOP_FTOL, N.BA_STOP_LAMBDA
 BA_LAMBDA0, BA_ACCEPT, BA_REJECT, BA_LAMBDA_MAX = 1e-3, 0.1, 10.0, 1e32
 BA_DEGENERATE_PIVOT = 1e-12   # relative pivot of the undamped initial landmark block below which a track is left out
-BA_COST_THREADS = 256         # the cost reduction's thread count (localization._block_sum)
+BA_COST_THREADS = 256         # the cost reduction's thread count (_posed.block_sum)
 STATS = ("initial_cost", "final_cost", "lambda", "iterations", "accepted", "stop_reason", "n_obs", "n_tracks")
 _WHO = "bundle_adjust"
 
@@ -57,17 +57,12 @@ def _check(keypoints, klines, K, R, t, tracks, fixed, max_iters, ftol):
         raise N.LtrError(f"{_WHO}: {n} keypoint arrays but {len(klines)} key-line arrays")
     if n > BA_MAX_IMAGES:
         raise N.LtrError(f"{_WHO}: {n} images exceed LTR_BA_MAX_IMAGES = {BA_MAX_IMAGES}")
-    n_kp, n_kl = _rows(keypoints, 2, "keypoints", _WHO), _rows(klines, 4, "klines", _WHO)
+    n_kp, n_kl = row_counts(keypoints, 2, "keypoints", _WHO), row_counts(klines, 4, "klines", _WHO)
     for nm, cnt in (("offsets_p", n_kp), ("offsets_l", n_kl)):
         off = np.asarray(tracks[nm] if isinstance(tracks, dict) else getattr(tracks, nm), dtype=np.int64)
         if off.shape != (n + 1,) or not np.array_equal(np.diff(off), cnt):
             raise N.LtrError(f"{_WHO}: the tracks' {nm} disagree with the rows of keypoints / klines")
-    Kn = _intrinsics(K, n, "K")
-    Rn, tn = _host(R, np.float64), _host(t, np.float64)
-    if Rn.shape != (n, 3, 3) or tn.shape != (n, 3):
-        raise N.LtrError(f"{_WHO}: R must be [{n}, 3, 3] and t [{n}, 3], got {list(Rn.shape)} and {list(tn.shape)}")
-    if not (np.isfinite(Rn).all() and np.isfinite(tn).all()):
-        raise N.LtrError(f"{_WHO}: R and t must be finite")
+    Kn, Rn, tn = check_poses(K, R, t, n, _WHO)
     fx = sorted({int(f) for f in fixed})
     if not fx:
         raise N.LtrError(f"{_WHO}: at least one image must be fixed")
@@ -77,12 +72,12 @@ def _check(keypoints, klines, K, R, t, tracks, fixed, max_iters, ftol):
         raise N.LtrError(f"{_WHO}: max_iters must lie in [0, LTR_BA_MAX_ITERS = {BA_MAX_ITERS}]")
     if not (math.isfinite(float(ftol)) and float(ftol) >= 0):
         raise N.LtrError(f"{_WHO}: ftol must be finite and >= 0")
-    return n, Kn, np.ascontiguousarray(Rn), np.ascontiguousarray(tn), fx
+    return n, Kn, Rn, tn, fx
 
 
 def _centres(R, t):
     """C = -R^T t per image in the tracks' order: [n, 3]."""
-    return np.stack([-((R[:, 0, j] * t[:, 0] + R[:, 1, j] * t[:, 1]) + R[:, 2, j] * t[:, 2]) for j in range(3)], 1)
+    return np.stack(centre(R.reshape(-1, 9), t.T), 1)
 
 
 def _hold(R, t, fixed):
@@ -97,14 +92,6 @@ def _hold(R, t, fixed):
 
 
 # ------------------------------------------------------------------ the model in numpy
-def _dot3(a, b):
-    return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]
-
-
-def _cross(a, b):
-    return [a[1] * b[2] - a[2] * b[1], a[2] * b[0] - a[0] * b[2], a[0] * b[1] - a[1] * b[0]]
-
-
 def _basis(X):
     """u1, u2 (3 arrays each) of lines X (6 arrays)."""
     d = [X[3 + k] - X[k] for k in range(3)]
@@ -112,11 +99,11 @@ def _basis(X):
     k = np.where(ad[1] < ad[0], 1, 0)
     k = np.where(ad[2] < np.where(k == 1, ad[1], ad[0]), 2, k)
     e = [np.where(k == j, 1.0, 0.0) for j in range(3)]
-    v = _cross(d, e)
-    nv = np.sqrt(_dot3(v, v))
+    v = cross3(d, e)
+    nv = np.sqrt(dot3(v, v))
     u1 = [x / nv for x in v]
-    w = _cross(d, u1)
-    nw = np.sqrt(_dot3(w, w))
+    w = cross3(d, u1)
+    nw = np.sqrt(dot3(w, w))
     return u1, [x / nw for x in w]
 
 
@@ -140,7 +127,7 @@ def _residual(R, C, X, cam, ob, line):
 def _jac(R, P, g):
     """Camera Jacobian [6] (w, C) and world Jacobian [3] of a residual with dr/dP = g."""
     gX = [(R[..., k] * g[0] + R[..., 3 + k] * g[1]) + R[..., 6 + k] * g[2] for k in range(3)]
-    c = _cross(P, g)
+    c = cross3(P, g)
     return [2.0 * c[0], 2.0 * c[1], 2.0 * c[2], -gX[0], -gX[1], -gX[2]], gX
 
 
@@ -154,15 +141,10 @@ class _Kind:
         Ki = K[img]
         self.cam = (Ki[..., 0, 0], Ki[..., 1, 1], Ki[..., 0, 2], Ki[..., 1, 2])
         px = pool[np.where(self.mask, rows, 0)]
-        fx, fy, cx, cy = self.cam
         if line:
-            x0, y0, x1, y1 = px[..., 0], px[..., 1], px[..., 2], px[..., 3]
-            a, b, c = y0 - y1, x1 - x0, x0 * y1 - x1 * y0
-            rn = 1.0 / np.sqrt(a * a + b * b)
-            la, lb, lc = a * rn, b * rn, c * rn
-            self.ob = [la * fx, lb * fy, (la * cx + lb * cy) + lc]
+            self.ob = line_normal(*self.cam, px)
         else:
-            self.ob = (px[..., 0] - cx, px[..., 1] - cy)
+            self.ob = (px[..., 0] - self.cam[2], px[..., 1] - self.cam[3])
         self.k = 4 if line else 3
 
     def terms(self, Rs, Cs, X):
@@ -187,7 +169,7 @@ class _Kind:
             res, P = _residual(R, C, Xb[3 * e:3 * e + 3], self.cam, self.ob, True)
             rq, g = res[0]
             jc, gX = _jac(R, P, g)
-            a, b = _dot3(gX, u1), _dot3(gX, u2)
+            a, b = dot3(gX, u1), dot3(gX, u2)
             z = np.zeros_like(a)
             r.append(rq)
             Jc.append(jc)
@@ -273,20 +255,6 @@ def _seq_sum(acc, group, key, vals, sign):
     return acc
 
 
-def _cayley_rot(w, R):
-    """cay(w) R for w (3 arrays [m]), R [m, 9] -> [m, 9] (localization.cayley's operations)."""
-    ww = (w[0] * w[0] + w[1] * w[1]) + w[2] * w[2]
-    den, s = 1.0 + ww, 1.0 - ww
-    z = np.zeros_like(ww)
-    wx = [[z, -w[2], w[1]], [w[2], z, -w[0]], [-w[1], w[0], z]]
-    Cm = [[(((s if i == k else z) + 2.0 * (w[i] * w[k])) + 2.0 * wx[i][k]) / den for k in range(3)] for i in range(3)]
-    out = np.empty_like(R)
-    for i in range(3):
-        for k in range(3):
-            out[:, 3 * i + k] = (Cm[i][0] * R[:, k] + Cm[i][1] * R[:, 3 + k]) + Cm[i][2] * R[:, 6 + k]
-    return out
-
-
 def _tracks_of(tr, line, n, off):
     """Participating-row layout of one kind of a TrackResult / triangulate_tracks_host dict -> (T bound, T, status,
     rows [T, Vm], cnt [T], img [T, Vm], X [T, 3|6], trk_status)."""
@@ -330,10 +298,7 @@ def bundle_adjust_host(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters
     n, Kn, R0, t0, fixed = _check(keypoints, klines, K, R, t, tracks, fixed, max_iters, ftol)
     op = np.asarray(_get(tracks, "offsets_p"), dtype=np.int64)
     ol = np.asarray(_get(tracks, "offsets_l"), dtype=np.int64)
-    kp = [_host(k, np.float32).reshape(-1, 2) for k in keypoints]
-    kl = [_host(k, np.float32).reshape(-1, 4) for k in klines]
-    kp_pool = (np.concatenate(kp) if n else np.zeros((0, 2), np.float32)).astype(np.float64)
-    kl_pool = (np.concatenate(kl) if n else np.zeros((0, 4), np.float32)).astype(np.float64)
+    kp_pool, kl_pool = pool64(keypoints, 2), pool64(klines, 4)
     hold = _hold(R0, t0, fixed)
     Rs, Cs = R0.reshape(n, 9).copy(), _centres(R0, t0)
     free = np.ones(n, bool)
@@ -383,7 +348,7 @@ def bundle_adjust_host(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters
                     fr = fr and bool((front[:, o] | ~mk).all())
                 costs.append(c)
             cc = np.concatenate(costs)
-            return (_block_sum(cc[:, None], BA_COST_THREADS)[0] if len(cc) else 0.0), fr
+            return (block_sum(cc[:, None], BA_COST_THREADS)[0] if len(cc) else 0.0), fr
 
         cost, _ = cost_of(Rs, Cs, Xs)
         init_cost = cost
@@ -480,7 +445,8 @@ def bundle_adjust_host(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters
             Rn, Cn = Rs.copy(), Cs.copy()
             si = np.flatnonzero(sysimg)
             if len(si):
-                Rn[si] = _cayley_rot([dcam[si, 0], dcam[si, 1], dcam[si, 2]], Rs[si])
+                Q, Rc = cayley([dcam[si, 0], dcam[si, 1], dcam[si, 2]]), Rs[si]
+                Rn[si] = np.stack([dot3(Q[i], Rc[:, k::3].T) for i in range(3) for k in range(3)], 1)
                 Cn[si] = Cs[si] + dcam[si, 3:]
             Xn = []
             for (r, Jc, W, Y, g, L, okl), kd, X in zip(per, kinds, Xs):
@@ -559,11 +525,8 @@ def bundle_adjust_host(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters
                 d = [Xb_[k] - Xa_[k] for k in range(3)]
                 w = [Xa_[k] - Cf[im, k] for k in range(3)]
                 for e in range(2):
-                    nx, ny = (seg[:, 2 * e] - cx) / fx, (seg[:, 2 * e + 1] - cy) / fy
-                    ray = [(Ri[:, k] * nx + Ri[:, 3 + k] * ny) + Ri[:, 6 + k] for k in range(3)]
-                    aa, bb, cc, dd, ee = _dot3(d, d), _dot3(d, ray), _dot3(ray, ray), _dot3(d, w), _dot3(ray, w)
-                    uu = (bb * ee - cc * dd) / (aa * cc - bb * bb)
-                    rowX[rowsel, 3 * e:3 * e + 3] = np.stack([Xa_[k] + uu * d[k] for k in range(3)], 1)
+                    r_e = ray(Ri, fx, fy, cx, cy, seg[:, 2 * e], seg[:, 2 * e + 1])
+                    rowX[rowsel, 3 * e:3 * e + 3] = np.stack(closest_on_line(Xa_, d, w, r_e), 1)
             out["row_lines3d" if kd.line else "row_points3d"] = rowX.reshape(Nr, 2, 3) if kd.line else rowX
             out[f"n_views_{s}"] = nv
     out["stats"] = dict(initial_cost=float(init_cost), final_cost=float(cost), **{"lambda": float(lam)},
@@ -634,16 +597,9 @@ def bundle_adjust(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters=50, 
              row_points3d=torch.empty((rp, 3), **f64), row_lines3d=torch.empty((rl, 2, 3), **f64),
              n_views_p=torch.empty(rp, **i32), n_views_l=torch.empty(rl, **i32), stats=torch.empty(8, **f64),
              workspace=torch.empty(-(-N.ba_workspace_bytes(n, Np, Nl, Tp, Tl) // 8), **f64))
-    kpts, segs = _pool_rows(keypoints, 2, dev), _pool_rows(klines, 4, dev)
-    arrays = {"K": Kn, "R": Rn, "t": tn, "kp_off": _offsets(np.diff(op)), "seg_off": _offsets(np.diff(ol)),
+    arrays = {"K": Kn, "R": Rn, "t": tn, "kp_off": offsets(np.diff(op)), "seg_off": offsets(np.diff(ol)),
               "hold": np.maximum(_hold(Rn, tn, fixed), 0).astype(np.int32), "fixed": fx}
-    for nm, a in (("kpts", kpts), ("segs", segs)):
-        if isinstance(a, np.ndarray):
-            arrays[nm] = a if len(a) else np.zeros((1, a.shape[1]), np.float32)
-    dv = _ops.stage(arrays, dev)
-    for nm, a in (("kpts", kpts), ("segs", segs)):
-        if isinstance(a, torch.Tensor):
-            dv[nm] = a
+    dv = stage_with_pools(arrays, keypoints, klines, dev)
     for nm in ("n_tracks_p", "n_tracks_l", "track_off_p", "track_off_l", "obs_p", "obs_l", "status_p", "status_l",
                "inlier_p", "inlier_l", "track_p", "track_l", "n_views_p", "n_views_l", "points3d", "lines3d"):
         dv[nm] = getattr(tracks, nm).contiguous()

@@ -27,6 +27,7 @@
 //   abspose_fit_kernel  grid (group): the winner again, the block-parallel refit, the masks, counts and pose.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 #include "ransac_common.cuh"
 
 namespace ltr {
@@ -88,15 +89,6 @@ __device__ __forceinline__ ApStage ap_stage_ptrs(unsigned char* base, int rows_p
   st.X = reinterpret_cast<double*>(st.k + rows_p);
   st.E = st.X + 3 * rows_p;
   return st;
-}
-
-#define AP_M __dmul_rn
-#define AP_A __dadd_rn
-#define AP_S __dsub_rn
-#define AP_D __ddiv_rn
-
-__device__ __forceinline__ double ap_dot(const double* a, const double* b) {
-  return AP_A(AP_A(AP_M(a[0], b[0]), AP_M(a[1], b[1])), AP_M(a[2], b[2]));
 }
 
 // Stage group g's rows and its frame.  Ends with __syncthreads.
@@ -174,7 +166,7 @@ __device__ void ap_stage_group(const AbsPoseArgs& a, int g, const ApStage& st, A
   if (threadIdx.x == 0) {
     for (int i = 1; i < NT / 32; ++i)
       for (int e = 0; e < 6; ++e) red[e] = fmin(red[e], red[i * 6 + e]);
-    for (int e = 0; e < 3; ++e) sg.c[e] = np + nl ? AP_M(AP_A(red[e], -red[3 + e]), 0.5) : 0.0;
+    for (int e = 0; e < 3; ++e) sg.c[e] = np + nl ? RC_M(RC_A(red[e], -red[3 + e]), 0.5) : 0.0;
     const double* K = a.K0 + 9ll * g;
     sg.fx = K[0]; sg.cx = K[2]; sg.fy = K[4]; sg.cy = K[5];
     sg.np = np;
@@ -183,14 +175,14 @@ __device__ void ap_stage_group(const AbsPoseArgs& a, int g, const ApStage& st, A
   __syncthreads();
   const double c0 = sg.c[0], c1 = sg.c[1], c2 = sg.c[2];
   for (int i = threadIdx.x; i < np; i += NT) {
-    st.X[3 * i] = AP_S(st.X[3 * i], c0);
-    st.X[3 * i + 1] = AP_S(st.X[3 * i + 1], c1);
-    st.X[3 * i + 2] = AP_S(st.X[3 * i + 2], c2);
+    st.X[3 * i] = RC_S(st.X[3 * i], c0);
+    st.X[3 * i + 1] = RC_S(st.X[3 * i + 1], c1);
+    st.X[3 * i + 2] = RC_S(st.X[3 * i + 2], c2);
   }
   for (int i = threadIdx.x; i < 2 * nl; i += NT) {
-    st.E[3 * i] = AP_S(st.E[3 * i], c0);
-    st.E[3 * i + 1] = AP_S(st.E[3 * i + 1], c1);
-    st.E[3 * i + 2] = AP_S(st.E[3 * i + 2], c2);
+    st.E[3 * i] = RC_S(st.E[3 * i], c0);
+    st.E[3 * i + 1] = RC_S(st.E[3 * i + 1], c1);
+    st.E[3 * i + 2] = RC_S(st.E[3 * i + 2], c2);
   }
   __syncthreads();
 }
@@ -201,66 +193,66 @@ __device__ __noinline__ int ap_p3p(const double* j, const double* X, double* Rs,
   double d1[3], d2[3], d3[3];
 #pragma unroll
   for (int e = 0; e < 3; ++e) {
-    d1[e] = AP_S(X[3 + e], X[e]);
-    d2[e] = AP_S(X[6 + e], X[e]);
-    d3[e] = AP_S(X[6 + e], X[3 + e]);
+    d1[e] = RC_S(X[3 + e], X[e]);
+    d2[e] = RC_S(X[6 + e], X[e]);
+    d3[e] = RC_S(X[6 + e], X[3 + e]);
   }
-  const double c2 = ap_dot(d1, d1), b2 = ap_dot(d2, d2), a2 = ap_dot(d3, d3);
+  const double c2 = rc_dot3(d1, d1), b2 = rc_dot3(d2, d2), a2 = rc_dot3(d3, d3);
   double cr[3];
-  ess_cross(d1, d2, cr);
-  const double n1 = __dsqrt_rn(c2), n2 = __dsqrt_rn(b2), ncr = __dsqrt_rn(ap_dot(cr, cr));
-  if (!(ncr > AP_M(AP_M(AP_COLLINEAR_EPS, n1), n2))) return 0;   // collinear world points
-  const double ca = ap_dot(j + 3, j + 6), cb = ap_dot(j, j + 6), cg = ap_dot(j, j + 3);
-  const double p = AP_D(AP_S(a2, c2), b2), q = AP_D(AP_A(a2, c2), b2);
-  const double rc = AP_D(c2, b2), ra = AP_D(a2, b2), rbc = AP_D(AP_S(b2, c2), b2), rba = AP_D(AP_S(b2, a2), b2);
-  const double ca2 = AP_M(ca, ca), cb2 = AP_M(cb, cb), cg2 = AP_M(cg, cg);
-  const double pm1 = AP_S(p, 1.0), pp1 = AP_A(p, 1.0), omq = AP_S(1.0, q);
+  rc_cross3(d1, d2, cr);
+  const double n1 = __dsqrt_rn(c2), n2 = __dsqrt_rn(b2), ncr = __dsqrt_rn(rc_dot3(cr, cr));
+  if (!(ncr > RC_M(RC_M(AP_COLLINEAR_EPS, n1), n2))) return 0;   // collinear world points
+  const double ca = rc_dot3(j + 3, j + 6), cb = rc_dot3(j, j + 6), cg = rc_dot3(j, j + 3);
+  const double p = RC_D(RC_S(a2, c2), b2), q = RC_D(RC_A(a2, c2), b2);
+  const double rc = RC_D(c2, b2), ra = RC_D(a2, b2), rbc = RC_D(RC_S(b2, c2), b2), rba = RC_D(RC_S(b2, a2), b2);
+  const double ca2 = RC_M(ca, ca), cb2 = RC_M(cb, cb), cg2 = RC_M(cg, cg);
+  const double pm1 = RC_S(p, 1.0), pp1 = RC_A(p, 1.0), omq = RC_S(1.0, q);
   double poly[11];
-  poly[4] = AP_S(AP_M(pm1, pm1), AP_M(AP_M(4.0, rc), ca2));
-  poly[3] = AP_M(4.0, AP_A(AP_S(AP_M(AP_M(p, AP_S(1.0, p)), cb), AP_M(AP_M(omq, ca), cg)),
-                           AP_M(AP_M(AP_M(2.0, rc), ca2), cb)));
-  poly[2] = AP_M(2.0, AP_A(AP_S(AP_A(AP_A(AP_S(AP_M(p, p), 1.0), AP_M(AP_M(2.0, AP_M(p, p)), cb2)),
-                                     AP_M(AP_M(2.0, rbc), ca2)),
-                                AP_M(AP_M(AP_M(AP_M(4.0, q), ca), cb), cg)),
-                           AP_M(AP_M(2.0, rba), cg2)));
-  poly[1] = AP_M(4.0, AP_S(AP_A(-AP_M(AP_M(p, pp1), cb), AP_M(AP_M(AP_M(2.0, ra), cg2), cb)), AP_M(AP_M(omq, ca), cg)));
-  poly[0] = AP_S(AP_M(pp1, pp1), AP_M(AP_M(4.0, ra), cg2));
+  poly[4] = RC_S(RC_M(pm1, pm1), RC_M(RC_M(4.0, rc), ca2));
+  poly[3] = RC_M(4.0, RC_A(RC_S(RC_M(RC_M(p, RC_S(1.0, p)), cb), RC_M(RC_M(omq, ca), cg)),
+                           RC_M(RC_M(RC_M(2.0, rc), ca2), cb)));
+  poly[2] = RC_M(2.0, RC_A(RC_S(RC_A(RC_A(RC_S(RC_M(p, p), 1.0), RC_M(RC_M(2.0, RC_M(p, p)), cb2)),
+                                     RC_M(RC_M(2.0, rbc), ca2)),
+                                RC_M(RC_M(RC_M(RC_M(4.0, q), ca), cb), cg)),
+                           RC_M(RC_M(2.0, rba), cg2)));
+  poly[1] = RC_M(4.0, RC_S(RC_A(-RC_M(RC_M(p, pp1), cb), RC_M(RC_M(RC_M(2.0, ra), cg2), cb)), RC_M(RC_M(omq, ca), cg)));
+  poly[0] = RC_S(RC_M(pp1, pp1), RC_M(RC_M(4.0, ra), cg2));
   for (int i = 5; i < 11; ++i) poly[i] = 0.0;
   double roots[10];
   const int nr = ess_roots(poly, roots);
   double e1[3], e2[3], e3[3];
 #pragma unroll
   for (int e = 0; e < 3; ++e) {
-    e1[e] = AP_D(d1[e], n1);
-    e3[e] = AP_D(cr[e], ncr);
+    e1[e] = RC_D(d1[e], n1);
+    e3[e] = RC_D(cr[e], ncr);
   }
-  ess_cross(e3, e1, e2);
+  rc_cross3(e3, e1, e2);
   int ns = 0;
   for (int r = 0; r < nr && r < AP_MAX_SOLUTIONS; ++r) {
-    const double v = roots[r], v2 = AP_M(v, v);
-    const double num = AP_A(AP_S(AP_M(pm1, v2), AP_M(AP_M(AP_M(2.0, p), cb), v)), pp1);
-    const double den = AP_M(2.0, AP_S(cg, AP_M(v, ca)));
-    const double den1 = AP_S(AP_A(1.0, v2), AP_M(AP_M(2.0, v), cb));
+    const double v = roots[r], v2 = RC_M(v, v);
+    const double num = RC_A(RC_S(RC_M(pm1, v2), RC_M(RC_M(RC_M(2.0, p), cb), v)), pp1);
+    const double den = RC_M(2.0, RC_S(cg, RC_M(v, ca)));
+    const double den1 = RC_S(RC_A(1.0, v2), RC_M(RC_M(2.0, v), cb));
     if (den == 0.0 || !(den1 > 0.0)) continue;
-    const double u = AP_D(num, den);
+    const double u = RC_D(num, den);
     if (!(u > 0.0) || !(v > 0.0)) continue;
-    const double s1 = __dsqrt_rn(AP_D(b2, den1)), s2 = AP_M(u, s1), s3 = AP_M(v, s1);
+    const double s1 = __dsqrt_rn(RC_D(b2, den1)), s2 = RC_M(u, s1), s3 = RC_M(v, s1);
     double P1[3], f1[3], f2[3];
 #pragma unroll
     for (int e = 0; e < 3; ++e) {
-      P1[e] = AP_M(s1, j[e]);
-      f1[e] = AP_S(AP_M(s2, j[3 + e]), P1[e]);
-      f2[e] = AP_S(AP_M(s3, j[6 + e]), P1[e]);
+      P1[e] = RC_M(s1, j[e]);
+      f1[e] = RC_S(RC_M(s2, j[3 + e]), P1[e]);
+      f2[e] = RC_S(RC_M(s3, j[6 + e]), P1[e]);
     }
     double cc[3], g1[3], g2[3], g3[3];
-    ess_cross(f1, f2, cc);
-    const double m1 = __dsqrt_rn(ap_dot(f1, f1)), mc = __dsqrt_rn(ap_dot(cc, cc));
+    rc_cross3(f1, f2, cc);
+    const double m1 = __dsqrt_rn(rc_dot3(f1, f1)), mc = __dsqrt_rn(rc_dot3(cc, cc));
 #pragma unroll
     for (int e = 0; e < 3; ++e) {
-      g1[e] = AP_D(f1[e], m1);
-      g3[e] = AP_D(cc[e], mc);
+      g1[e] = RC_D(f1[e], m1);
+      g3[e] = RC_D(cc[e], mc);
     }
-    ess_cross(g3, g1, g2);
+    rc_cross3(g3, g1, g2);
     double* R = Rs + 9 * ns;
     double* t = ts + 3 * ns;
     bool fin = true;
@@ -268,12 +260,12 @@ __device__ __noinline__ int ap_p3p(const double* j, const double* X, double* Rs,
     for (int i = 0; i < 3; ++i)
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        R[3 * i + k] = AP_A(AP_A(AP_M(g1[i], e1[k]), AP_M(g2[i], e2[k])), AP_M(g3[i], e3[k]));
+        R[3 * i + k] = RC_A(RC_A(RC_M(g1[i], e1[k]), RC_M(g2[i], e2[k])), RC_M(g3[i], e3[k]));
         fin &= isfinite(R[3 * i + k]);
       }
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
-      t[i] = AP_S(P1[i], AP_A(AP_A(AP_M(R[3 * i], X[0]), AP_M(R[3 * i + 1], X[1])), AP_M(R[3 * i + 2], X[2])));
+      t[i] = RC_S(P1[i], RC_A(RC_A(RC_M(R[3 * i], X[0]), RC_M(R[3 * i + 1], X[1])), RC_M(R[3 * i + 2], X[2])));
       fin &= isfinite(t[i]);
     }
     if (fin) jr[ns++] = r;
@@ -289,11 +281,11 @@ __device__ __forceinline__ int ap_hypothesis(const ApStage& st, const ApGroup& s
   double j[9], X[9];
   for (int s = 0; s < AP_SAMPLE; ++s) {
     const float2 kk = st.k[idx[s]];
-    const double qx = AP_D(AP_S(kk.x, sg.cx), sg.fx), qy = AP_D(AP_S(kk.y, sg.cy), sg.fy);
-    const double nb = __dsqrt_rn(AP_A(AP_A(AP_M(qx, qx), AP_M(qy, qy)), 1.0));
-    j[3 * s] = AP_D(qx, nb);
-    j[3 * s + 1] = AP_D(qy, nb);
-    j[3 * s + 2] = AP_D(1.0, nb);
+    const double qx = RC_D(RC_S(kk.x, sg.cx), sg.fx), qy = RC_D(RC_S(kk.y, sg.cy), sg.fy);
+    const double nb = __dsqrt_rn(RC_A(RC_A(RC_M(qx, qx), RC_M(qy, qy)), 1.0));
+    j[3 * s] = RC_D(qx, nb);
+    j[3 * s + 1] = RC_D(qy, nb);
+    j[3 * s + 2] = RC_D(1.0, nb);
 #pragma unroll
     for (int e = 0; e < 3; ++e) X[3 * s + e] = st.X[3 * idx[s] + e];
   }
@@ -304,21 +296,9 @@ __device__ __forceinline__ int ap_hypothesis(const ApStage& st, const ApGroup& s
 __device__ __forceinline__ void ap_cam(const double* C, const double* X, double* Y, double* P) {
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
-    Y[i] = AP_A(AP_A(AP_M(C[3 * i], X[0]), AP_M(C[3 * i + 1], X[1])), AP_M(C[3 * i + 2], X[2]));
-    P[i] = AP_A(Y[i], C[9 + i]);
+    Y[i] = RC_A(RC_A(RC_M(C[3 * i], X[0]), RC_M(C[3 * i + 1], X[1])), RC_M(C[3 * i + 2], X[2]));
+    P[i] = RC_A(Y[i], C[9 + i]);
   }
-}
-
-// The query line through s0 in camera-ray form: the pixel line scaled to a^2 + b^2 = 1, then (a fx, b fy, a cx + b cy
-// + c).
-__device__ __forceinline__ void ap_line_normal(const float4 s, const ApGroup& sg, double* n) {
-  const double ax = s.x, ay = s.y, bx = s.z, by = s.w;
-  const double a = AP_S(ay, by), b = AP_S(bx, ax), c = AP_S(AP_M(ax, by), AP_M(bx, ay));
-  const double rn = __drcp_rn(__dsqrt_rn(AP_A(AP_M(a, a), AP_M(b, b))));
-  const double la = AP_M(a, rn), lb = AP_M(b, rn), lc = AP_M(c, rn);
-  n[0] = AP_M(la, sg.fx);
-  n[1] = AP_M(lb, sg.fy);
-  n[2] = AP_A(AP_A(AP_M(la, sg.cx), AP_M(lb, sg.cy)), lc);
 }
 
 // Staged row d (points, then lines) is an inlier of pose C.
@@ -327,19 +307,20 @@ __device__ __forceinline__ bool ap_inlier(const ApStage& st, const ApGroup& sg, 
   if (d < sg.np) {
     ap_cam(C, st.X + 3 * d, Y, P);
     const float2 k = st.k[d];
-    const double ex = AP_S(AP_M(sg.fx, P[0]), AP_M(AP_S(k.x, sg.cx), P[2]));
-    const double ey = AP_S(AP_M(sg.fy, P[1]), AP_M(AP_S(k.y, sg.cy), P[2]));
-    return P[2] > 0.0 && AP_A(AP_M(ex, ex), AP_M(ey, ey)) < AP_M(t2, AP_M(P[2], P[2]));
+    const double ex = RC_S(RC_M(sg.fx, P[0]), RC_M(RC_S(k.x, sg.cx), P[2]));
+    const double ey = RC_S(RC_M(sg.fy, P[1]), RC_M(RC_S(k.y, sg.cy), P[2]));
+    return P[2] > 0.0 && RC_A(RC_M(ex, ex), RC_M(ey, ey)) < RC_M(t2, RC_M(P[2], P[2]));
   }
   const int i = d - sg.np;
   double n[3];
-  ap_line_normal(st.s0[i], sg, n);
+  const double cam[4] = {sg.fx, sg.fy, sg.cx, sg.cy};
+  rc_line_normal(cam, st.s0[i], n);
   bool ok = true;
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     ap_cam(C, st.E + 6 * i + 3 * e, Y, P);
-    const double dd = AP_A(AP_A(AP_M(n[0], P[0]), AP_M(n[1], P[1])), AP_M(n[2], P[2]));
-    ok &= P[2] > 0.0 && AP_M(dd, dd) < AP_M(t2, AP_M(P[2], P[2]));
+    const double dd = RC_A(RC_A(RC_M(n[0], P[0]), RC_M(n[1], P[1])), RC_M(n[2], P[2]));
+    ok &= P[2] > 0.0 && RC_M(dd, dd) < RC_M(t2, RC_M(P[2], P[2]));
   }
   return ok;
 }
@@ -422,10 +403,10 @@ __device__ __forceinline__ void ap_residual(const ApStage& st, const ApGroup& sg
   double Y[3], P[3], g[3];
   auto jac = [&](double* Jr) {
     double c[3];
-    ess_cross(Y, g, c);
+    rc_cross3(Y, g, c);
 #pragma unroll
     for (int e = 0; e < 3; ++e) {
-      Jr[e] = AP_M(2.0, c[e]);
+      Jr[e] = RC_M(2.0, c[e]);
       Jr[3 + e] = g[e];
     }
   };
@@ -433,27 +414,28 @@ __device__ __forceinline__ void ap_residual(const ApStage& st, const ApGroup& sg
     ap_cam(C, st.X + 3 * d, Y, P);
     const float2 k = st.k[d];
     const double iz = __drcp_rn(P[2]);
-    const double xn = AP_M(P[0], iz), yn = AP_M(P[1], iz);
-    r[0] = AP_S(AP_M(sg.fx, xn), AP_S(k.x, sg.cx));
-    r[1] = AP_S(AP_M(sg.fy, yn), AP_S(k.y, sg.cy));
+    const double xn = RC_M(P[0], iz), yn = RC_M(P[1], iz);
+    r[0] = RC_S(RC_M(sg.fx, xn), RC_S(k.x, sg.cx));
+    r[1] = RC_S(RC_M(sg.fy, yn), RC_S(k.y, sg.cy));
     if (JAC) {
-      g[0] = AP_M(sg.fx, iz); g[1] = 0.0; g[2] = -AP_M(AP_M(sg.fx, xn), iz);
+      g[0] = RC_M(sg.fx, iz); g[1] = 0.0; g[2] = -RC_M(RC_M(sg.fx, xn), iz);
       jac(J[0]);
-      g[0] = 0.0; g[1] = AP_M(sg.fy, iz); g[2] = -AP_M(AP_M(sg.fy, yn), iz);
+      g[0] = 0.0; g[1] = RC_M(sg.fy, iz); g[2] = -RC_M(RC_M(sg.fy, yn), iz);
       jac(J[1]);
     }
     return;
   }
   const int i = d - sg.np;
   double n[3];
-  ap_line_normal(st.s0[i], sg, n);
+  const double cam[4] = {sg.fx, sg.fy, sg.cx, sg.cy};
+  rc_line_normal(cam, st.s0[i], n);
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     ap_cam(C, st.E + 6 * i + 3 * e, Y, P);
     const double iz = __drcp_rn(P[2]);
-    r[e] = AP_M(AP_A(AP_A(AP_M(n[0], P[0]), AP_M(n[1], P[1])), AP_M(n[2], P[2])), iz);
+    r[e] = RC_M(RC_A(RC_A(RC_M(n[0], P[0]), RC_M(n[1], P[1])), RC_M(n[2], P[2])), iz);
     if (JAC) {
-      g[0] = AP_M(n[0], iz); g[1] = AP_M(n[1], iz); g[2] = -AP_M(AP_S(r[e], n[2]), iz);
+      g[0] = RC_M(n[0], iz); g[1] = RC_M(n[1], iz); g[2] = -RC_M(RC_S(r[e], n[2]), iz);
       jac(J[e]);
     }
   }
@@ -484,16 +466,16 @@ __device__ void ap_sums(const ApStage& st, const ApGroup& sg, const double* sH, 
       for (int i = 0; i < 6; ++i)
 #pragma unroll
         for (int k = i; k < 6; ++k, ++e)
-          acc[e] = AP_A(acc[e], AP_A(AP_M(J[0][i], J[0][k]), AP_M(J[1][i], J[1][k])));
+          acc[e] = RC_A(acc[e], RC_A(RC_M(J[0][i], J[0][k]), RC_M(J[1][i], J[1][k])));
 #pragma unroll
-      for (int i = 0; i < 6; ++i) acc[21 + i] = AP_A(acc[21 + i], AP_A(AP_M(J[0][i], r[0]), AP_M(J[1][i], r[1])));
+      for (int i = 0; i < 6; ++i) acc[21 + i] = RC_A(acc[21 + i], RC_A(RC_M(J[0][i], r[0]), RC_M(J[1][i], r[1])));
     }
-    acc[M - 1] = AP_A(acc[M - 1], AP_A(AP_M(r[0], r[0]), AP_M(r[1], r[1])));
+    acc[M - 1] = RC_A(acc[M - 1], RC_A(RC_M(r[0], r[0]), RC_M(r[1], r[1])));
   }
 #pragma unroll
   for (int e = 0; e < M; ++e)
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc[e] = AP_A(acc[e], __shfl_xor_sync(0xffffffffu, acc[e], o));
+    for (int o = 16; o > 0; o >>= 1) acc[e] = RC_A(acc[e], __shfl_xor_sync(0xffffffffu, acc[e], o));
   if ((threadIdx.x & 31) == 0)
 #pragma unroll
     for (int e = 0; e < M; ++e) red[(threadIdx.x >> 5) * M + e] = acc[e];
@@ -501,7 +483,7 @@ __device__ void ap_sums(const ApStage& st, const ApGroup& sg, const double* sH, 
   if (threadIdx.x == 0)
     for (int e = 0; e < M; ++e) {
       double v = 0.0;
-      for (int w = 0; w < NT / 32; ++w) v = AP_A(v, red[w * M + e]);
+      for (int w = 0; w < NT / 32; ++w) v = RC_A(v, red[w * M + e]);
       out[e] = v;
     }
   __syncthreads();
@@ -515,7 +497,7 @@ __device__ __noinline__ bool ap_lm_step(const double* S, double lam, const doubl
   for (int i = 0; i < 6; ++i)
     for (int k = i; k < 6; ++k, ++e) A[i][k] = A[k][i] = S[e];
   for (int i = 0; i < 6; ++i) {
-    A[i][i] = AP_A(A[i][i], AP_M(lam, A[i][i]));
+    A[i][i] = RC_A(A[i][i], RC_M(lam, A[i][i]));
     A[i][6] = -S[21 + i];
   }
   for (int c = 0; c < 6; ++c) {
@@ -527,32 +509,26 @@ __device__ __noinline__ bool ap_lm_step(const double* S, double lam, const doubl
     if (piv != c)
       for (int k = c; k < 7; ++k) { const double t = A[c][k]; A[c][k] = A[piv][k]; A[piv][k] = t; }
     for (int r = c + 1; r < 6; ++r) {
-      const double f = AP_D(A[r][c], A[c][c]);
-      for (int k = c + 1; k < 7; ++k) A[r][k] = AP_S(A[r][k], AP_M(f, A[c][k]));
+      const double f = RC_D(A[r][c], A[c][c]);
+      for (int k = c + 1; k < 7; ++k) A[r][k] = RC_S(A[r][k], RC_M(f, A[c][k]));
     }
   }
   double x[6];
   for (int i = 5; i >= 0; --i) {
     double acc = A[i][6];
-    for (int k = i + 1; k < 6; ++k) acc = AP_S(acc, AP_M(A[i][k], x[k]));
-    x[i] = AP_D(acc, A[i][i]);
+    for (int k = i + 1; k < 6; ++k) acc = RC_S(acc, RC_M(A[i][k], x[k]));
+    x[i] = RC_D(acc, A[i][i]);
     if (!isfinite(x[i])) return false;
   }
-  // Cayley map ((1 - w.w) I + 2 [w]x + 2 w w^T) / (1 + w.w)
-  const double ww = AP_A(AP_A(AP_M(x[0], x[0]), AP_M(x[1], x[1])), AP_M(x[2], x[2]));
-  const double den = AP_A(1.0, ww), s = AP_S(1.0, ww);
-  const double wx[9] = {0.0, -x[2], x[1], x[2], 0.0, -x[0], -x[1], x[0], 0.0};
   double Q[9];
-  for (int i = 0; i < 3; ++i)
-    for (int k = 0; k < 3; ++k)
-      Q[3 * i + k] = AP_D(AP_A(AP_A(i == k ? s : 0.0, AP_M(2.0, AP_M(x[i], x[k]))), AP_M(2.0, wx[3 * i + k])), den);
+  rc_cayley(x, Q);
   bool fin = true;
   for (int i = 0; i < 3; ++i) {
     for (int k = 0; k < 3; ++k) {
-      Cn[3 * i + k] = AP_A(AP_A(AP_M(Q[3 * i], C[k]), AP_M(Q[3 * i + 1], C[3 + k])), AP_M(Q[3 * i + 2], C[6 + k]));
+      Cn[3 * i + k] = RC_A(RC_A(RC_M(Q[3 * i], C[k]), RC_M(Q[3 * i + 1], C[3 + k])), RC_M(Q[3 * i + 2], C[6 + k]));
       fin &= isfinite(Cn[3 * i + k]);
     }
-    Cn[9 + i] = AP_A(C[9 + i], x[3 + i]);
+    Cn[9 + i] = RC_A(C[9 + i], x[3 + i]);
     fin &= isfinite(Cn[9 + i]);
   }
   return fin;
@@ -607,9 +583,9 @@ __global__ void __launch_bounds__(AP_FIT_THREADS) abspose_fit_kernel(AbsPoseArgs
           s_ok[2] = s_ok[1] && s_cost < sS[AP_TERMS - 1];
           if (s_ok[2]) {
             for (int i = 0; i < 12; ++i) sC[1][i] = sC[2][i];
-            lam = AP_M(lam, AP_LM_ACCEPT);
+            lam = RC_M(lam, AP_LM_ACCEPT);
           } else {
-            lam = AP_M(lam, AP_LM_REJECT);
+            lam = RC_M(lam, AP_LM_REJECT);
           }
         }
         __syncthreads();
@@ -676,8 +652,8 @@ __global__ void __launch_bounds__(AP_FIT_THREADS) abspose_fit_kernel(AbsPoseArgs
   if (threadIdx.x < 9) a.R[9ll * g + threadIdx.x] = valid ? C[threadIdx.x] : nan;
   if (threadIdx.x < 3) {
     const int i = threadIdx.x;
-    const double rc = AP_A(AP_A(AP_M(C[3 * i], sg.c[0]), AP_M(C[3 * i + 1], sg.c[1])), AP_M(C[3 * i + 2], sg.c[2]));
-    a.t[3ll * g + i] = valid ? AP_S(C[9 + i], rc) : nan;
+    const double rc = RC_A(RC_A(RC_M(C[3 * i], sg.c[0]), RC_M(C[3 * i + 1], sg.c[1])), RC_M(C[3 * i + 2], sg.c[2]));
+    a.t[3ll * g + i] = valid ? RC_S(C[9 + i], rc) : nan;
   }
   if (threadIdx.x == 0) {
     int2 t = make_int2(0, 0);
@@ -690,10 +666,5 @@ __global__ void __launch_bounds__(AP_FIT_THREADS) abspose_fit_kernel(AbsPoseArgs
     a.hyp_inliers[g] = valid ? (int)(key >> 32) : 0;
   }
 }
-
-#undef AP_M
-#undef AP_A
-#undef AP_S
-#undef AP_D
 
 }  // namespace ltr

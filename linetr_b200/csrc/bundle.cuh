@@ -32,6 +32,7 @@
 //   ba_finish_kernel   outputs: poses, per-track coordinates and status, per-row residuals and rows(), stats.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 #include "triangulation.cuh"
 #include "tracks.cuh"
 
@@ -40,7 +41,7 @@ namespace ltr {
 constexpr int BA_MAX_IMAGES = 128;       // LTR_BA_MAX_IMAGES: a track's image set is a 128-bit mask
 constexpr int BA_THREADS = 128;
 constexpr int BA_CTA_THREADS = 1024;     // the one-CTA solve
-constexpr int BA_COST_THREADS = 256;     // the cost reduction (localization._block_sum)
+constexpr int BA_COST_THREADS = 256;     // the cost reduction (_posed.block_sum)
 constexpr int BA_ROW = 64;               // doubles per row: r (2), Jc (2 x 6), W (6 x 4), Y (6 x 4)
 constexpr int BA_TRK = 40;               // doubles per track: X (6), X_new (6), g (4), L (16), cost (1)
 constexpr int BA_CAM = 48;               // doubles per image: R (9), C (3), R_new (9), C_new (3), dcam (6)
@@ -70,11 +71,6 @@ struct BaArgs {
   int* list; int* list_off; int* col; uint8_t* part; unsigned* mask; int* si;
 };
 
-#define RC_M __dmul_rn
-#define RC_A __dadd_rn
-#define RC_S __dsub_rn
-#define RC_D __ddiv_rn
-
 __device__ __forceinline__ int ba_width(int g) { return g ? 6 : 3; }
 __device__ __forceinline__ int ba_k(int g) { return g ? 4 : 3; }
 
@@ -92,7 +88,7 @@ __device__ __forceinline__ double* ba_rowp(const BaArgs& a, int g, int row) {
   return a.row + (size_t)BA_ROW * (g ? a.n_nodes[0] + row : row);
 }
 __device__ __forceinline__ int ba_image(const BaArgs& a, int g, int row) {
-  return tri_segment(g ? a.seg_off : a.kp_off, a.n_images, row);
+  return rc_segment(g ? a.seg_off : a.kp_off, a.n_images, row);
 }
 
 // A row's observation: fx fy cx cy, then (x - cx, y - cy) of a keypoint or the pixel line normal of a key line.
@@ -104,7 +100,7 @@ __device__ __forceinline__ BaObs ba_obs(const BaArgs& a, int g, int row, int img
   o.fx = Kv[0]; o.fy = Kv[4]; o.cx = Kv[2]; o.cy = Kv[5];
   if (g) {
     const double c[4] = {o.fx, o.fy, o.cx, o.cy};
-    tri_line_normal(c, reinterpret_cast<const float4*>(a.segs)[row], o.ob);
+    rc_line_normal(c, reinterpret_cast<const float4*>(a.segs)[row], o.ob);
   } else {
     const float2 q = reinterpret_cast<const float2*>(a.kpts)[row];
     o.ob[0] = RC_S((double)q.x, o.cx);
@@ -112,12 +108,6 @@ __device__ __forceinline__ BaObs ba_obs(const BaArgs& a, int g, int row, int img
     o.ob[2] = 0.0;
   }
   return o;
-}
-
-__device__ __forceinline__ void ba_cross(const double* a, const double* b, double* o) {
-  o[0] = RC_S(RC_M(a[1], b[2]), RC_M(a[2], b[1]));
-  o[1] = RC_S(RC_M(a[2], b[0]), RC_M(a[0], b[2]));
-  o[2] = RC_S(RC_M(a[0], b[1]), RC_M(a[1], b[0]));
 }
 
 // The in-plane basis u1, u2 of a line's end points X [6].
@@ -128,11 +118,11 @@ __device__ __forceinline__ void ba_basis(const double* X, double* u1, double* u2
   if (fabs(d[1]) < fabs(d[k])) k = 1;
   if (fabs(d[2]) < fabs(d[k])) k = 2;
   e[k] = 1.0;
-  ba_cross(d, e, v);
-  const double nv = __dsqrt_rn(tri_dot(v, v));
+  rc_cross3(d, e, v);
+  const double nv = __dsqrt_rn(rc_dot3(v, v));
   for (int j = 0; j < 3; ++j) u1[j] = RC_D(v[j], nv);
-  ba_cross(d, u1, v);
-  const double nw = __dsqrt_rn(tri_dot(v, v));
+  rc_cross3(d, u1, v);
+  const double nw = __dsqrt_rn(rc_dot3(v, v));
   for (int j = 0; j < 3; ++j) u2[j] = RC_D(v[j], nw);
 }
 
@@ -140,7 +130,7 @@ __device__ __forceinline__ void ba_basis(const double* X, double* u1, double* u2
 __device__ __forceinline__ void ba_jac(const double* R, const double* P, const double* gp, double* Jc, double* gX) {
   for (int k = 0; k < 3; ++k) gX[k] = RC_A(RC_A(RC_M(R[k], gp[0]), RC_M(R[3 + k], gp[1])), RC_M(R[6 + k], gp[2]));
   double c[3];
-  ba_cross(P, gp, c);
+  rc_cross3(P, gp, c);
   for (int k = 0; k < 3; ++k) {
     Jc[k] = RC_M(2.0, c[k]);
     Jc[3 + k] = -gX[k];
@@ -156,15 +146,15 @@ __device__ __forceinline__ bool ba_terms(const double* R, const double* C, const
   for (int e = 0; e < (g ? 2 : 1); ++e) {
     double D[3], P[3];
     for (int k = 0; k < 3; ++k) D[k] = RC_S(X[3 * e + k], C[k]);
-    tri_mv(R, D, P);
+    rc_mv3(R, D, P);
     front = front && P[2] > 0.0;
     if (g) {
-      const double rr = RC_D(tri_dot(o.ob, P), P[2]);
+      const double rr = RC_D(rc_dot3(o.ob, P), P[2]);
       const double gp[3] = {RC_D(o.ob[0], P[2]), RC_D(o.ob[1], P[2]), RC_D(RC_S(o.ob[2], rr), P[2])};
       double gX[3];
       ba_jac(R, P, gp, Jc[e], gX);
       r[e] = rr;
-      const double ja = tri_dot(gX, u1), jb = tri_dot(gX, u2);
+      const double ja = rc_dot3(gX, u1), jb = rc_dot3(gX, u2);
       Jl[e][0] = e ? 0.0 : ja;
       Jl[e][1] = e ? 0.0 : jb;
       Jl[e][2] = e ? ja : 0.0;
@@ -295,7 +285,7 @@ __global__ void __launch_bounds__(BA_COST_THREADS) ba_start_kernel(const BaArgs 
     const double* R = a.R0 + 9 * i;
     const double* t = a.t0 + 3 * i;
     for (int e = 0; e < 9; ++e) cm[e] = R[e];
-    for (int j = 0; j < 3; ++j) cm[9 + j] = -RC_A(RC_A(RC_M(R[j], t[0]), RC_M(R[3 + j], t[1])), RC_M(R[6 + j], t[2]));
+    rc_centre(R, t, cm + 9);
     for (int e = 24; e < 30; ++e) cm[e] = 0.0;
     a.part[i] = 0;
   }
@@ -562,16 +552,12 @@ __global__ void __launch_bounds__(BA_CTA_THREADS) ba_solve_kernel(const BaArgs a
       cm[24 + e] = w[e];
     }
     if (a.col[6 * tid] >= 0) {
-      const double ww = RC_A(RC_A(RC_M(w[0], w[0]), RC_M(w[1], w[1])), RC_M(w[2], w[2]));
-      const double den = RC_A(1.0, ww), sd = RC_S(1.0, ww);
-      const double wx[3][3] = {{0.0, -w[2], w[1]}, {w[2], 0.0, -w[0]}, {-w[1], w[0], 0.0}};
-      double Cm[3][3];
+      double Q[9];
+      rc_cayley(w, Q);
       for (int i = 0; i < 3; ++i)
         for (int k = 0; k < 3; ++k)
-          Cm[i][k] = RC_D(RC_A(RC_A(i == k ? sd : 0.0, RC_M(2.0, RC_M(w[i], w[k]))), RC_M(2.0, wx[i][k])), den);
-      for (int i = 0; i < 3; ++i)
-        for (int k = 0; k < 3; ++k)
-          cm[12 + 3 * i + k] = RC_A(RC_A(RC_M(Cm[i][0], cm[k]), RC_M(Cm[i][1], cm[3 + k])), RC_M(Cm[i][2], cm[6 + k]));
+          cm[12 + 3 * i + k] =
+              RC_A(RC_A(RC_M(Q[3 * i], cm[k]), RC_M(Q[3 * i + 1], cm[3 + k])), RC_M(Q[3 * i + 2], cm[6 + k]));
       for (int k = 0; k < 3; ++k) cm[21 + k] = RC_A(cm[9 + k], w[3 + k]);
     } else {
       for (int e = 0; e < 12; ++e) cm[12 + e] = cm[e];
@@ -680,7 +666,7 @@ __device__ __forceinline__ void ba_pose(const BaArgs& a, int i, double* R, doubl
   const double* cm = a.cam + (size_t)BA_CAM * i;
   if (a.col[6 * i] >= 0 && a.si[BA_I_ACC] > 0) {
     for (int e = 0; e < 9; ++e) R[e] = cm[e];
-    for (int e = 0; e < 3; ++e) t[e] = -tri_dot(cm + 3 * e, cm + 9);
+    for (int e = 0; e < 3; ++e) t[e] = -rc_dot3(cm + 3 * e, cm + 9);
   } else {
     for (int e = 0; e < 9; ++e) R[e] = a.R0[9 * i + e];
     for (int e = 0; e < 3; ++e) t[e] = a.t0[3 * i + e];
@@ -745,7 +731,7 @@ __global__ void __launch_bounds__(BA_THREADS) ba_finish_kernel(const BaArgs a) {
     const int img = ba_image(a, 1, row);
     double R[9], t[3], C[3], d[3], w[3];
     ba_pose(a, img, R, t);
-    for (int j = 0; j < 3; ++j) C[j] = -RC_A(RC_A(RC_M(R[j], t[0]), RC_M(R[3 + j], t[1])), RC_M(R[6 + j], t[2]));
+    rc_centre(R, t, C);
     for (int k = 0; k < 3; ++k) {
       d[k] = RC_S(Xf[3 + k], Xf[k]);
       w[k] = RC_S(Xf[k], C[k]);
@@ -754,17 +740,10 @@ __global__ void __launch_bounds__(BA_THREADS) ba_finish_kernel(const BaArgs a) {
     const float4 s = reinterpret_cast<const float4*>(a.segs)[row];
     for (int e = 0; e < 2; ++e) {
       double rr[3];
-      tri_ray(R, Kv[0], Kv[4], Kv[2], Kv[5], e ? s.z : s.x, e ? s.w : s.y, rr);
-      const double aa = tri_dot(d, d), b = tri_dot(d, rr), cc = tri_dot(rr, rr), dd = tri_dot(d, w), ee = tri_dot(rr, w);
-      const double u = RC_D(RC_S(RC_M(b, ee), RC_M(cc, dd)), RC_S(RC_M(aa, cc), RC_M(b, b)));
-      for (int k = 0; k < 3; ++k) a.row_lines[6ll * row + 3 * e + k] = RC_A(Xf[k], RC_M(u, d[k]));
+      rc_ray(R, Kv[0], Kv[4], Kv[2], Kv[5], e ? s.z : s.x, e ? s.w : s.y, rr);
+      rc_closest_on_line(Xf, d, w, rr, a.row_lines + 6ll * row + 3 * e);
     }
   }
 }
-
-#undef RC_M
-#undef RC_A
-#undef RC_S
-#undef RC_D
 
 }  // namespace ltr

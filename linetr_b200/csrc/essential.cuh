@@ -22,6 +22,7 @@
 //   essential_pose_kernel  grid (pair): the winner again, inlier flags, decomposition, cheirality, the outputs.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 #include "ransac_common.cuh"
 
 namespace ltr {
@@ -48,11 +49,6 @@ struct EssentialArgs {
 // Dynamic shared memory of one pair: the rows, plus one flag byte per row in the pose kernel.
 static inline long long ess_smem_bytes(long long rows, bool pose) { return rows * (ESS_ROW_BYTES + (pose ? 1 : 0)); }
 
-#define ES_M __dmul_rn
-#define ES_A __dadd_rn
-#define ES_S __dsub_rn
-#define ES_D __ddiv_rn
-
 // Products of monomials in (x, y, z): degree 1 [x, y, z, 1], degree 2 [x^2, xy, xz, x, y^2, yz, y, z^2, z, 1], degree 3
 // [x^3, y^3, x^2y, xy^2, x^2z, x^2, y^2z, y^2, xyz, xy | xz^2, xz, x, yz^2, yz, y, z^3, z^2, z, 1].
 __constant__ unsigned char ESS_MUL11[4][4] = {{0, 1, 2, 3}, {1, 4, 5, 6}, {2, 5, 7, 8}, {3, 6, 8, 9}};
@@ -76,8 +72,8 @@ __device__ int ess_stage_pair(const EssentialArgs& a, int p, double4* rows, int*
   const float* __restrict__ x1 = a.pts1 + 2ll * a.pts_off1[p];
   const int n = hg_compact<NT>(a.matches_p, a.cu_p[p], a.cu_p[p + 1], a.n_pts1[p], warp_cnt, [&](int i, int m, int ci) {
     if (ci < 0) return;
-    rows[ci] = make_double4(ES_D(ES_S((double)x0[2 * i], c0x), f0x), ES_D(ES_S((double)x0[2 * i + 1], c0y), f0y),
-                            ES_D(ES_S((double)x1[2 * m], c1x), f1x), ES_D(ES_S((double)x1[2 * m + 1], c1y), f1y));
+    rows[ci] = make_double4(RC_D(RC_S((double)x0[2 * i], c0x), f0x), RC_D(RC_S((double)x0[2 * i + 1], c0y), f0y),
+                            RC_D(RC_S((double)x1[2 * m], c1x), f1x), RC_D(RC_S((double)x1[2 * m + 1], c1y), f1y));
   });
   if (threadIdx.x == 0) *s_n = n;
   __syncthreads();
@@ -88,9 +84,9 @@ __device__ int ess_stage_pair(const EssentialArgs& a, int p, double4* rows, int*
 __device__ __forceinline__ double ess_t2(const EssentialArgs& a, int p) {
   const double* K0 = a.K0 + 9ll * p;
   const double* K1 = a.K1 + 9ll * p;
-  const double fm = ES_D(ES_A(ES_A(ES_A(K0[0], K1[4]), K0[0]), K1[4]), 4.0);
-  const double tn = ES_D(a.thresh, fm);
-  return ES_M(tn, tn);
+  const double fm = RC_D(RC_A(RC_A(RC_A(K0[0], K1[4]), K0[0]), K1[4]), 4.0);
+  const double tn = RC_D(a.thresh, fm);
+  return RC_M(tn, tn);
 }
 
 __device__ __forceinline__ void ess_mul11(const double* x, const double* y, double* out) {
@@ -99,11 +95,11 @@ __device__ __forceinline__ void ess_mul11(const double* x, const double* y, doub
 #pragma unroll
   for (int i = 0; i < 4; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) out[ESS_MUL11[i][j]] = ES_A(out[ESS_MUL11[i][j]], ES_M(x[i], y[j]));
+    for (int j = 0; j < 4; ++j) out[ESS_MUL11[i][j]] = RC_A(out[ESS_MUL11[i][j]], RC_M(x[i], y[j]));
 }
 
 __device__ __forceinline__ void ess_sub(double* x, const double* y, int n) {
-  for (int i = 0; i < n; ++i) x[i] = ES_S(x[i], y[i]);
+  for (int i = 0; i < n; ++i) x[i] = RC_S(x[i], y[i]);
 }
 
 // out (20) = x (degree 2) * y (degree 1)
@@ -111,7 +107,7 @@ __device__ __forceinline__ void ess_mul21(const double* x, const double* y, doub
   for (int m = 0; m < 20; ++m) out[m] = 0.0;
   for (int i = 0; i < 10; ++i)
 #pragma unroll
-    for (int j = 0; j < 4; ++j) out[ESS_MUL21[i][j]] = ES_A(out[ESS_MUL21[i][j]], ES_M(x[i], y[j]));
+    for (int j = 0; j < 4; ++j) out[ESS_MUL21[i][j]] = RC_A(out[ESS_MUL21[i][j]], RC_M(x[i], y[j]));
 }
 
 // The five-point solver on 5 normalised correspondences q[s] = (a0, b0, a1, b1): up to 10 E (row-major, Es[9 s]) with
@@ -128,22 +124,22 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
     ess_mul11(e[3], e[8], t1); ess_mul11(e[5], e[6], t2); ess_sub(t1, t2, 10); ess_mul21(t1, e[1], u);
     ess_sub(C[0], u, 20);
     ess_mul11(e[3], e[7], t1); ess_mul11(e[4], e[6], t2); ess_sub(t1, t2, 10); ess_mul21(t1, e[2], u);
-    for (int m = 0; m < 20; ++m) C[0][m] = ES_A(C[0][m], u[m]);
+    for (int m = 0; m < 20; ++m) C[0][m] = RC_A(C[0][m], u[m]);
     double L[6][10];   // (0,0) (0,1) (0,2) (1,1) (1,2) (2,2) of E E^T, then 2 E E^T - tr I
     int w = 0;
     for (int i = 0; i < 3; ++i)
       for (int k = i; k < 3; ++k, ++w) {
         ess_mul11(e[3 * i], e[3 * k], L[w]);
         ess_mul11(e[3 * i + 1], e[3 * k + 1], t1);
-        for (int m = 0; m < 10; ++m) L[w][m] = ES_A(L[w][m], t1[m]);
+        for (int m = 0; m < 10; ++m) L[w][m] = RC_A(L[w][m], t1[m]);
         ess_mul11(e[3 * i + 2], e[3 * k + 2], t1);
-        for (int m = 0; m < 10; ++m) L[w][m] = ES_A(L[w][m], t1[m]);
+        for (int m = 0; m < 10; ++m) L[w][m] = RC_A(L[w][m], t1[m]);
       }
     double tr[10];
-    for (int m = 0; m < 10; ++m) tr[m] = ES_A(ES_A(L[0][m], L[3][m]), L[5][m]);
+    for (int m = 0; m < 10; ++m) tr[m] = RC_A(RC_A(L[0][m], L[3][m]), L[5][m]);
     for (int w2 = 0; w2 < 6; ++w2) {
       const bool diag = w2 == 0 || w2 == 3 || w2 == 5;
-      for (int m = 0; m < 10; ++m) L[w2][m] = diag ? ES_S(ES_M(L[w2][m], 2.0), tr[m]) : ES_M(L[w2][m], 2.0);
+      for (int m = 0; m < 10; ++m) L[w2][m] = diag ? RC_S(RC_M(L[w2][m], 2.0), tr[m]) : RC_M(L[w2][m], 2.0);
     }
     const int li[3][3] = {{0, 1, 2}, {1, 3, 4}, {2, 4, 5}};
     for (int i = 0; i < 3; ++i)
@@ -151,9 +147,9 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
         double* row = C[1 + 3 * i + j];
         ess_mul21(L[li[i][0]], e[j], row);
         ess_mul21(L[li[i][1]], e[3 + j], u);
-        for (int m = 0; m < 20; ++m) row[m] = ES_A(row[m], u[m]);
+        for (int m = 0; m < 20; ++m) row[m] = RC_A(row[m], u[m]);
         ess_mul21(L[li[i][2]], e[6 + j], u);
-        for (int m = 0; m < 20; ++m) row[m] = ES_A(row[m], u[m]);
+        for (int m = 0; m < 20; ++m) row[m] = RC_A(row[m], u[m]);
       }
   }
   // Gauss-Jordan on the first 10 columns
@@ -166,11 +162,11 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
     if (piv != c)
       for (int j = 0; j < 20; ++j) { const double tmp = C[c][j]; C[c][j] = C[piv][j]; C[piv][j] = tmp; }
     const double pv = C[c][c];
-    for (int j = c + 1; j < 20; ++j) C[c][j] = ES_D(C[c][j], pv);
+    for (int j = c + 1; j < 20; ++j) C[c][j] = RC_D(C[c][j], pv);
     for (int r = 0; r < 10; ++r) {
       if (r == c) continue;
       const double f = C[r][c];
-      for (int j = c + 1; j < 20; ++j) C[r][j] = ES_S(C[r][j], ES_M(f, C[c][j]));
+      for (int j = c + 1; j < 20; ++j) C[r][j] = RC_S(C[r][j], RC_M(f, C[c][j]));
     }
   }
   // hidden-variable matrix B(z): rows x^2z - z x^2, y^2z - z y^2, xyz - z xy; B[r] = bx (4), by (4), b1 (5)
@@ -179,9 +175,9 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
     const double* ru = C[4 + 2 * r] + 10;
     const double* rl = C[5 + 2 * r] + 10;
     double* b = B[r];
-    b[0] = -ru[2]; b[1] = ES_S(rl[2], ru[1]); b[2] = ES_S(rl[1], ru[0]); b[3] = rl[0];
-    b[4] = -ru[5]; b[5] = ES_S(rl[5], ru[4]); b[6] = ES_S(rl[4], ru[3]); b[7] = rl[3];
-    b[8] = -ru[9]; b[9] = ES_S(rl[9], ru[8]); b[10] = ES_S(rl[8], ru[7]); b[11] = ES_S(rl[7], ru[6]); b[12] = rl[6];
+    b[0] = -ru[2]; b[1] = RC_S(rl[2], ru[1]); b[2] = RC_S(rl[1], ru[0]); b[3] = rl[0];
+    b[4] = -ru[5]; b[5] = RC_S(rl[5], ru[4]); b[6] = RC_S(rl[4], ru[3]); b[7] = rl[3];
+    b[8] = -ru[9]; b[9] = RC_S(rl[9], ru[8]); b[10] = RC_S(rl[8], ru[7]); b[11] = RC_S(rl[7], ru[6]); b[12] = rl[6];
   }
   double poly[11];
   {
@@ -196,7 +192,7 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
     // t2 = B02 (B10 B21 - B11 B20)
     ess_pmul(B[1], 4, B[2] + 4, 4, x8); ess_pmul(B[1] + 4, 4, B[2], 4, y8); ess_sub(x8, y8, 7);
     ess_pmul(B[0] + 8, 5, x8, 7, t);
-    for (int i = 0; i < 11; ++i) poly[i] = ES_A(poly[i], t[i]);
+    for (int i = 0; i < 11; ++i) poly[i] = RC_A(poly[i], t[i]);
   }
   double roots[10];
   const int nr = ess_roots(poly, roots);
@@ -210,17 +206,17 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
       rw[r][2] = ess_horner(B[r] + 8, 4, z);
     }
     double best[3], c[3];
-    ess_cross(rw[0], rw[1], best);
-    ess_cross(rw[0], rw[2], c);
+    rc_cross3(rw[0], rw[1], best);
+    rc_cross3(rw[0], rw[2], c);
     if (fabs(c[2]) > fabs(best[2])) { best[0] = c[0]; best[1] = c[1]; best[2] = c[2]; }
-    ess_cross(rw[1], rw[2], c);
+    rc_cross3(rw[1], rw[2], c);
     if (fabs(c[2]) > fabs(best[2])) { best[0] = c[0]; best[1] = c[1]; best[2] = c[2]; }
     if (!(fabs(best[2]) > 0.0)) continue;
-    const double x = ES_D(best[0], best[2]), y = ES_D(best[1], best[2]);
+    const double x = RC_D(best[0], best[2]), y = RC_D(best[1], best[2]);
     double* E = Es + 9 * ns;
     bool fin = true;
     for (int i = 0; i < 9; ++i) {
-      E[i] = ES_A(ES_A(ES_A(ES_M(x, e[i][0]), ES_M(y, e[i][1])), ES_M(z, e[i][2])), e[i][3]);
+      E[i] = RC_A(RC_A(RC_A(RC_M(x, e[i][0]), RC_M(y, e[i][1])), RC_M(z, e[i][2])), e[i][3]);
       fin &= isfinite(E[i]);
     }
     if (!fin) continue;
@@ -230,14 +226,14 @@ __device__ __noinline__ int ess_solve(const double4* q, double* Es, int* jr) {
 }
 
 __device__ __forceinline__ bool ess_inlier(const double* e, const double4 q, double t2) {
-  const double u0 = ES_A(ES_A(ES_M(e[0], q.x), ES_M(e[1], q.y)), e[2]);
-  const double u1 = ES_A(ES_A(ES_M(e[3], q.x), ES_M(e[4], q.y)), e[5]);
-  const double u2 = ES_A(ES_A(ES_M(e[6], q.x), ES_M(e[7], q.y)), e[8]);
-  const double w0 = ES_A(ES_A(ES_M(e[0], q.z), ES_M(e[3], q.w)), e[6]);
-  const double w1 = ES_A(ES_A(ES_M(e[1], q.z), ES_M(e[4], q.w)), e[7]);
-  const double num = ES_A(ES_A(ES_M(q.z, u0), ES_M(q.w, u1)), u2);
-  const double den = ES_A(ES_A(ES_A(ES_M(u0, u0), ES_M(u1, u1)), ES_M(w0, w0)), ES_M(w1, w1));
-  return ES_M(num, num) < ES_M(t2, den);
+  const double u0 = RC_A(RC_A(RC_M(e[0], q.x), RC_M(e[1], q.y)), e[2]);
+  const double u1 = RC_A(RC_A(RC_M(e[3], q.x), RC_M(e[4], q.y)), e[5]);
+  const double u2 = RC_A(RC_A(RC_M(e[6], q.x), RC_M(e[7], q.y)), e[8]);
+  const double w0 = RC_A(RC_A(RC_M(e[0], q.z), RC_M(e[3], q.w)), e[6]);
+  const double w1 = RC_A(RC_A(RC_M(e[1], q.z), RC_M(e[4], q.w)), e[7]);
+  const double num = RC_A(RC_A(RC_M(q.z, u0), RC_M(q.w, u1)), u2);
+  const double den = RC_A(RC_A(RC_A(RC_M(u0, u0), RC_M(u1, u1)), RC_M(w0, w0)), RC_M(w1, w1));
+  return RC_M(num, num) < RC_M(t2, den);
 }
 
 __global__ void __launch_bounds__(ESS_THREADS) essential_hyp_kernel(EssentialArgs a) {
@@ -304,7 +300,7 @@ __device__ __noinline__ void ess_decompose(const double* E, double (*cand)[12]) 
   const int i1 = 3 - i0 - i2;
   double v1[3], v2[3], v3[3], u1[3], u2[3], u3[3];
   for (int k = 0; k < 3; ++k) { v1[k] = V[k][i0]; v2[k] = V[k][i1]; }
-  ess_cross(v1, v2, v3);
+  rc_cross3(v1, v2, v3);
   for (int r = 0; r < 3; ++r) {
     u1[r] = E[3 * r] * v1[0] + E[3 * r + 1] * v1[1] + E[3 * r + 2] * v1[2];
     u2[r] = E[3 * r] * v2[0] + E[3 * r + 1] * v2[1] + E[3 * r + 2] * v2[2];
@@ -315,7 +311,7 @@ __device__ __noinline__ void ess_decompose(const double* E, double (*cand)[12]) 
   for (int r = 0; r < 3; ++r) u2[r] -= d * u1[r];
   const double n2 = sqrt(u2[0] * u2[0] + u2[1] * u2[1] + u2[2] * u2[2]);
   for (int r = 0; r < 3; ++r) u2[r] /= n2;
-  ess_cross(u1, u2, u3);
+  rc_cross3(u1, u2, u3);
   // R1 = U W V^T = -u2 v1^T + u1 v2^T + u3 v3^T, R2 = U W^T V^T = u2 v1^T - u1 v2^T + u3 v3^T, t = u3
   for (int r = 0; r < 3; ++r)
     for (int c = 0; c < 3; ++c) {
@@ -331,17 +327,17 @@ __device__ __noinline__ void ess_decompose(const double* E, double (*cand)[12]) 
 
 // Depths of d1 x1 = d0 R x0 + t from the 2 x 2 normal equations; true when both lie in (0, dist).
 __device__ __forceinline__ bool ess_in_front(const double* c, const double4 q, double dist) {
-  const double ax = ES_A(ES_A(ES_M(c[0], q.x), ES_M(c[1], q.y)), c[2]);
-  const double ay = ES_A(ES_A(ES_M(c[3], q.x), ES_M(c[4], q.y)), c[5]);
-  const double az = ES_A(ES_A(ES_M(c[6], q.x), ES_M(c[7], q.y)), c[8]);
-  const double aa = ES_A(ES_A(ES_M(ax, ax), ES_M(ay, ay)), ES_M(az, az));
-  const double ab = ES_A(ES_A(ES_M(ax, q.z), ES_M(ay, q.w)), az);
-  const double bb = ES_A(ES_A(ES_M(q.z, q.z), ES_M(q.w, q.w)), 1.0);
-  const double at = ES_A(ES_A(ES_M(ax, c[9]), ES_M(ay, c[10])), ES_M(az, c[11]));
-  const double bt = ES_A(ES_A(ES_M(q.z, c[9]), ES_M(q.w, c[10])), c[11]);
-  const double det = ES_S(ES_M(ab, ab), ES_M(aa, bb));
-  const double d0 = ES_D(ES_S(ES_M(at, bb), ES_M(ab, bt)), det);
-  const double d1 = ES_D(ES_S(ES_M(ab, at), ES_M(aa, bt)), det);
+  const double ax = RC_A(RC_A(RC_M(c[0], q.x), RC_M(c[1], q.y)), c[2]);
+  const double ay = RC_A(RC_A(RC_M(c[3], q.x), RC_M(c[4], q.y)), c[5]);
+  const double az = RC_A(RC_A(RC_M(c[6], q.x), RC_M(c[7], q.y)), c[8]);
+  const double aa = RC_A(RC_A(RC_M(ax, ax), RC_M(ay, ay)), RC_M(az, az));
+  const double ab = RC_A(RC_A(RC_M(ax, q.z), RC_M(ay, q.w)), az);
+  const double bb = RC_A(RC_A(RC_M(q.z, q.z), RC_M(q.w, q.w)), 1.0);
+  const double at = RC_A(RC_A(RC_M(ax, c[9]), RC_M(ay, c[10])), RC_M(az, c[11]));
+  const double bt = RC_A(RC_A(RC_M(q.z, c[9]), RC_M(q.w, c[10])), c[11]);
+  const double det = RC_S(RC_M(ab, ab), RC_M(aa, bb));
+  const double d0 = RC_D(RC_S(RC_M(at, bb), RC_M(ab, bt)), det);
+  const double d1 = RC_D(RC_S(RC_M(ab, at), RC_M(aa, bt)), det);
   return d0 > 0.0 && d0 < dist && d1 > 0.0 && d1 < dist;
 }
 
@@ -454,10 +450,5 @@ __global__ void __launch_bounds__(ESS_POSE_THREADS) essential_pose_kernel(Essent
     for (int r = pb + threadIdx.x; r < pe; r += NT) a.inl[r] = 0;
   }
 }
-
-#undef ES_M
-#undef ES_A
-#undef ES_S
-#undef ES_D
 
 }  // namespace ltr

@@ -29,6 +29,7 @@
 //                           check of the pair's match rows (row-parallel, from global memory).
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 #include "ransac_common.cuh"
 #include "homography.cuh"
 
@@ -60,11 +61,6 @@ struct FundamentalArgs {
 // Dynamic shared memory of one pair: the pixel rows (16 bytes each), plus two flag bytes per row in the fit kernel.
 static inline long long fm_smem_bytes(long long rows, bool fit) { return hg_smem_bytes(rows, 0, fit); }
 
-#define FM_M __dmul_rn
-#define FM_A __dadd_rn
-#define FM_S __dsub_rn
-#define FM_D __ddiv_rn
-
 // The point-only view of the arguments that the homography's staging reads (same compaction and normalisation).
 __device__ __forceinline__ HomographyArgs fm_point_args(const FundamentalArgs& a) {
   HomographyArgs h{};
@@ -83,21 +79,21 @@ __device__ __noinline__ int fm_solve(const double4* q, double* Fs, int* jr) {
   double c[9][2];
   for (int i = 0; i < 9; ++i) {
     c[i][0] = e[i][1];
-    c[i][1] = FM_S(e[i][0], e[i][1]);
+    c[i][1] = RC_S(e[i][0], e[i][1]);
   }
   // det F(a) = (c0 (c4 c8 - c5 c7) - c1 (c3 c8 - c5 c6)) + c2 (c3 c7 - c4 c6), ascending coefficients
   double poly[11], x3[3], y3[3], t[4];
   ess_pmul(c[4], 2, c[8], 2, x3); ess_pmul(c[5], 2, c[7], 2, y3);
-  for (int i = 0; i < 3; ++i) x3[i] = FM_S(x3[i], y3[i]);
+  for (int i = 0; i < 3; ++i) x3[i] = RC_S(x3[i], y3[i]);
   ess_pmul(c[0], 2, x3, 3, poly);
   ess_pmul(c[3], 2, c[8], 2, x3); ess_pmul(c[5], 2, c[6], 2, y3);
-  for (int i = 0; i < 3; ++i) x3[i] = FM_S(x3[i], y3[i]);
+  for (int i = 0; i < 3; ++i) x3[i] = RC_S(x3[i], y3[i]);
   ess_pmul(c[1], 2, x3, 3, t);
-  for (int i = 0; i < 4; ++i) poly[i] = FM_S(poly[i], t[i]);
+  for (int i = 0; i < 4; ++i) poly[i] = RC_S(poly[i], t[i]);
   ess_pmul(c[3], 2, c[7], 2, x3); ess_pmul(c[4], 2, c[6], 2, y3);
-  for (int i = 0; i < 3; ++i) x3[i] = FM_S(x3[i], y3[i]);
+  for (int i = 0; i < 3; ++i) x3[i] = RC_S(x3[i], y3[i]);
   ess_pmul(c[2], 2, x3, 3, t);
-  for (int i = 0; i < 4; ++i) poly[i] = FM_A(poly[i], t[i]);
+  for (int i = 0; i < 4; ++i) poly[i] = RC_A(poly[i], t[i]);
   for (int i = 4; i < 11; ++i) poly[i] = 0.0;
   double roots[10];
   const int nr = ess_roots(poly, roots);
@@ -106,7 +102,7 @@ __device__ __noinline__ int fm_solve(const double4* q, double* Fs, int* jr) {
     double* F = Fs + 9 * ns;
     bool fin = true;
     for (int i = 0; i < 9; ++i) {
-      F[i] = FM_A(c[i][0], FM_M(roots[j], c[i][1]));
+      F[i] = RC_A(c[i][0], RC_M(roots[j], c[i][1]));
       fin &= isfinite(F[i]);
     }
     if (fin) jr[ns++] = j;
@@ -117,26 +113,26 @@ __device__ __noinline__ int fm_solve(const double4* q, double* Fs, int* jr) {
 // Normalised f (9) -> pixel F = T1^T F^ T0, scaled to unit Frobenius norm with its largest |entry| (the first on a
 // tie) positive; false for a zero or non-finite result.
 __device__ __forceinline__ bool fm_to_pixels(const HgPair& sp, const double* f, double* F) {
-  const double t0x = -FM_M(sp.c0x, sp.i0), t0y = -FM_M(sp.c0y, sp.i0);
-  const double t1x = -FM_M(sp.c1x, sp.i1), t1y = -FM_M(sp.c1y, sp.i1);
+  const double t0x = -RC_M(sp.c0x, sp.i0), t0y = -RC_M(sp.c0y, sp.i0);
+  const double t1x = -RC_M(sp.c1x, sp.i1), t1y = -RC_M(sp.c1y, sp.i1);
   double M[9], G[9];
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
-    M[3 * i] = FM_M(f[3 * i], sp.i0);
-    M[3 * i + 1] = FM_M(f[3 * i + 1], sp.i0);
-    M[3 * i + 2] = FM_A(FM_A(FM_M(f[3 * i], t0x), FM_M(f[3 * i + 1], t0y)), f[3 * i + 2]);
+    M[3 * i] = RC_M(f[3 * i], sp.i0);
+    M[3 * i + 1] = RC_M(f[3 * i + 1], sp.i0);
+    M[3 * i + 2] = RC_A(RC_A(RC_M(f[3 * i], t0x), RC_M(f[3 * i + 1], t0y)), f[3 * i + 2]);
   }
 #pragma unroll
   for (int j = 0; j < 3; ++j) {
-    G[j] = FM_M(M[j], sp.i1);
-    G[3 + j] = FM_M(M[3 + j], sp.i1);
-    G[6 + j] = FM_A(FM_A(FM_M(t1x, M[j]), FM_M(t1y, M[3 + j])), M[6 + j]);
+    G[j] = RC_M(M[j], sp.i1);
+    G[3 + j] = RC_M(M[3 + j], sp.i1);
+    G[6 + j] = RC_A(RC_A(RC_M(t1x, M[j]), RC_M(t1y, M[3 + j])), M[6 + j]);
   }
   double s = 0.0;
   int im = 0;
 #pragma unroll
   for (int j = 0; j < 9; ++j) {
-    s = FM_A(s, FM_M(G[j], G[j]));
+    s = RC_A(s, RC_M(G[j], G[j]));
     if (fabs(G[j]) > fabs(G[im])) im = j;
   }
   const double nrm = __dsqrt_rn(s);
@@ -144,7 +140,7 @@ __device__ __forceinline__ bool fm_to_pixels(const HgPair& sp, const double* f, 
   const bool neg = G[im] < 0.0;
 #pragma unroll
   for (int j = 0; j < 9; ++j) {
-    const double v = FM_D(G[j], nrm);
+    const double v = RC_D(G[j], nrm);
     F[j] = neg ? -v : v;
   }
   return true;
@@ -158,8 +154,8 @@ __device__ __forceinline__ int fm_hypothesis(const HgStage& st, const HgPair& sp
   double4 q[FM_SAMPLE];
   for (int s = 0; s < FM_SAMPLE; ++s) {
     const float4 r = st.pt[idx[s]];
-    q[s] = make_double4(FM_M(FM_S(r.x, sp.c0x), sp.i0), FM_M(FM_S(r.y, sp.c0y), sp.i0),
-                        FM_M(FM_S(r.z, sp.c1x), sp.i1), FM_M(FM_S(r.w, sp.c1y), sp.i1));
+    q[s] = make_double4(RC_M(RC_S(r.x, sp.c0x), sp.i0), RC_M(RC_S(r.y, sp.c0y), sp.i0),
+                        RC_M(RC_S(r.z, sp.c1x), sp.i1), RC_M(RC_S(r.w, sp.c1y), sp.i1));
   }
   double Fh[9 * FM_MAX_SOLUTIONS];
   int jh[FM_MAX_SOLUTIONS];
@@ -173,15 +169,15 @@ __device__ __forceinline__ int fm_hypothesis(const HgStage& st, const HgPair& sp
 // cv2's FM error below t2, without the division: (x1^T F x0)^2 < t2 min(|(F x0)_xy|^2, |(F^T x1)_xy|^2).
 __device__ __forceinline__ bool fm_inlier(const double* F, const float4 q, double t2) {
   const double x0 = q.x, y0 = q.y, x1 = q.z, y1 = q.w;
-  const double u0 = FM_A(FM_A(FM_M(F[0], x0), FM_M(F[1], y0)), F[2]);
-  const double u1 = FM_A(FM_A(FM_M(F[3], x0), FM_M(F[4], y0)), F[5]);
-  const double u2 = FM_A(FM_A(FM_M(F[6], x0), FM_M(F[7], y0)), F[8]);
-  const double w0 = FM_A(FM_A(FM_M(F[0], x1), FM_M(F[3], y1)), F[6]);
-  const double w1 = FM_A(FM_A(FM_M(F[1], x1), FM_M(F[4], y1)), F[7]);
-  const double num = FM_A(FM_A(FM_M(x1, u0), FM_M(y1, u1)), u2);
-  const double a = FM_A(FM_M(u0, u0), FM_M(u1, u1)), b = FM_A(FM_M(w0, w0), FM_M(w1, w1));
+  const double u0 = RC_A(RC_A(RC_M(F[0], x0), RC_M(F[1], y0)), F[2]);
+  const double u1 = RC_A(RC_A(RC_M(F[3], x0), RC_M(F[4], y0)), F[5]);
+  const double u2 = RC_A(RC_A(RC_M(F[6], x0), RC_M(F[7], y0)), F[8]);
+  const double w0 = RC_A(RC_A(RC_M(F[0], x1), RC_M(F[3], y1)), F[6]);
+  const double w1 = RC_A(RC_A(RC_M(F[1], x1), RC_M(F[4], y1)), F[7]);
+  const double num = RC_A(RC_A(RC_M(x1, u0), RC_M(y1, u1)), u2);
+  const double a = RC_A(RC_M(u0, u0), RC_M(u1, u1)), b = RC_A(RC_M(w0, w0), RC_M(w1, w1));
   const double m = a < b ? a : b;
-  return m > 0.0 && FM_M(num, num) < FM_M(t2, m);
+  return m > 0.0 && RC_M(num, num) < RC_M(t2, m);
 }
 
 __global__ void __launch_bounds__(FM_THREADS) fundamental_hyp_kernel(FundamentalArgs a) {
@@ -277,27 +273,27 @@ __device__ __noinline__ void fm_rank2(double* f) {
 __device__ __forceinline__ double fm_side_ratio(const double* la, const double* lb, double px, double py, double qx,
                                                 double qy) {
   const double nan = __longlong_as_double(0x7ff8000000000000ll);
-  const double l0 = FM_S(py, qy), l1 = FM_S(qx, px), l2 = FM_S(FM_M(px, qy), FM_M(qx, py));
-  const double dx = FM_S(qx, px), dy = FM_S(qy, py);
-  const double len2 = FM_A(FM_M(dx, dx), FM_M(dy, dy));
+  const double l0 = RC_S(py, qy), l1 = RC_S(qx, px), l2 = RC_S(RC_M(px, qy), RC_M(qx, py));
+  const double dx = RC_S(qx, px), dy = RC_S(qy, py);
+  const double len2 = RC_A(RC_M(dx, dx), RC_M(dy, dy));
   double t[2];
 #pragma unroll
   for (int e = 0; e < 2; ++e) {
     const double* m = e ? lb : la;
-    const double X0 = FM_S(FM_M(m[1], l2), FM_M(m[2], l1));
-    const double X1 = FM_S(FM_M(m[2], l0), FM_M(m[0], l2));
-    const double X2 = FM_S(FM_M(m[0], l1), FM_M(m[1], l0));
-    const double nrm = __dsqrt_rn(FM_A(FM_A(FM_M(X0, X0), FM_M(X1, X1)), FM_M(X2, X2)));
-    if (!(fabs(X2) > FM_M(HG_FLT_EPS, nrm))) return nan;
-    const double x = FM_D(X0, X2), y = FM_D(X1, X2);
-    t[e] = FM_D(FM_A(FM_M(FM_S(x, px), dx), FM_M(FM_S(y, py), dy)), len2);
+    const double X0 = RC_S(RC_M(m[1], l2), RC_M(m[2], l1));
+    const double X1 = RC_S(RC_M(m[2], l0), RC_M(m[0], l2));
+    const double X2 = RC_S(RC_M(m[0], l1), RC_M(m[1], l0));
+    const double nrm = __dsqrt_rn(RC_A(RC_A(RC_M(X0, X0), RC_M(X1, X1)), RC_M(X2, X2)));
+    if (!(fabs(X2) > RC_M(HG_FLT_EPS, nrm))) return nan;
+    const double x = RC_D(X0, X2), y = RC_D(X1, X2);
+    t[e] = RC_D(RC_A(RC_M(RC_S(x, px), dx), RC_M(RC_S(y, py), dy)), len2);
   }
   const double lo = t[0] < t[1] ? t[0] : t[1], hi = t[0] < t[1] ? t[1] : t[0];
   if (!(hi > lo)) return nan;
   const double a = lo > 0.0 ? lo : 0.0, b = hi < 1.0 ? hi : 1.0;
-  const double ov = b > a ? FM_S(b, a) : 0.0;
-  const double span = FM_S(hi, lo);
-  return FM_D(ov, span < 1.0 ? span : 1.0);
+  const double ov = b > a ? RC_S(b, a) : 0.0;
+  const double span = RC_S(hi, lo);
+  return RC_D(ov, span < 1.0 ? span : 1.0);
 }
 
 // Both side ratios of one matched key-line pair under F: r1 in image 1 (F a0, F b0 against s1), r0 in image 0
@@ -310,15 +306,15 @@ __device__ __forceinline__ void fm_line_ratios(const double* F, const float* s0,
   // image 1: F a0, F b0 against s1
 #pragma unroll
   for (int r = 0; r < 3; ++r) {
-    la[r] = FM_A(FM_A(FM_M(F[3 * r], a0x), FM_M(F[3 * r + 1], a0y)), F[3 * r + 2]);
-    lb[r] = FM_A(FM_A(FM_M(F[3 * r], b0x), FM_M(F[3 * r + 1], b0y)), F[3 * r + 2]);
+    la[r] = RC_A(RC_A(RC_M(F[3 * r], a0x), RC_M(F[3 * r + 1], a0y)), F[3 * r + 2]);
+    lb[r] = RC_A(RC_A(RC_M(F[3 * r], b0x), RC_M(F[3 * r + 1], b0y)), F[3 * r + 2]);
   }
   r1 = fm_side_ratio(la, lb, a1x, a1y, b1x, b1y);
   // image 0: F^T a1, F^T b1 against s0
 #pragma unroll
   for (int c = 0; c < 3; ++c) {
-    la[c] = FM_A(FM_A(FM_M(F[c], a1x), FM_M(F[3 + c], a1y)), F[6 + c]);
-    lb[c] = FM_A(FM_A(FM_M(F[c], b1x), FM_M(F[3 + c], b1y)), F[6 + c]);
+    la[c] = RC_A(RC_A(RC_M(F[c], a1x), RC_M(F[3 + c], a1y)), F[6 + c]);
+    lb[c] = RC_A(RC_A(RC_M(F[c], b1x), RC_M(F[3 + c], b1y)), F[6 + c]);
   }
   r0 = fm_side_ratio(la, lb, a0x, a0y, b0x, b0y);
 }
@@ -385,8 +381,8 @@ __global__ void __launch_bounds__(FM_FIT_THREADS) fundamental_fit_kernel(Fundame
       for (int d = threadIdx.x; d < n; d += NT) {
         if (!flh[d]) continue;
         const float4 q = st.pt[d];
-        const double x = FM_M(FM_S(q.x, sp.c0x), sp.i0), y = FM_M(FM_S(q.y, sp.c0y), sp.i0);
-        const double u = FM_M(FM_S(q.z, sp.c1x), sp.i1), v = FM_M(FM_S(q.w, sp.c1y), sp.i1);
+        const double x = RC_M(RC_S(q.x, sp.c0x), sp.i0), y = RC_M(RC_S(q.y, sp.c0y), sp.i0);
+        const double u = RC_M(RC_S(q.z, sp.c1x), sp.i1), v = RC_M(RC_S(q.w, sp.c1y), sp.i1);
         const double r[9] = {u * x, u * y, u, v * x, v * y, v, x, y, 1.0};
         int e = 0;
 #pragma unroll
@@ -478,10 +474,5 @@ __global__ void __launch_bounds__(FM_FIT_THREADS) fundamental_fit_kernel(Fundame
     a.n_lines_ok[p] = t;
   }
 }
-
-#undef FM_M
-#undef FM_A
-#undef FM_S
-#undef FM_D
 
 }  // namespace ltr

@@ -25,6 +25,7 @@
 //   homography_refit_kernel  grid (pair): the winner again, A^T A, Jacobi, both inlier passes, the outputs.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 #include "ransac_common.cuh"
 
 namespace ltr {
@@ -82,10 +83,6 @@ __device__ __forceinline__ HgStage hg_stage_ptrs(unsigned char* base, int rows_p
   return st;
 }
 
-#define HG_M __dmul_rn
-#define HG_A __dadd_rn
-#define HG_S __dsub_rn
-
 // Stage pair p's correspondences and its normalisation.  Ends with __syncthreads.
 template <int NT>
 __device__ void hg_stage_pair(const HomographyArgs& a, int p, const HgStage& st, HgPair& sp, int* warp_cnt, float* red) {
@@ -113,11 +110,11 @@ __device__ void hg_stage_pair(const HomographyArgs& a, int p, const HgStage& st,
       st.a[ci] = make_float4(l0[4 * i], l0[4 * i + 1], l0[4 * i + 2], l0[4 * i + 3]);
       st.b[ci] = s1;
       const double ax = s1.x, ay = s1.y, bx = s1.z, by = s1.w;
-      const double la = HG_S(ay, by), lb = HG_S(bx, ax), lc = HG_S(HG_M(ax, by), HG_M(bx, ay));
-      const double r = __drcp_rn(__dsqrt_rn(HG_A(HG_M(la, la), HG_M(lb, lb))));
-      st.l[3 * ci] = HG_M(la, r);
-      st.l[3 * ci + 1] = HG_M(lb, r);
-      st.l[3 * ci + 2] = HG_M(lc, r);
+      const double la = RC_S(ay, by), lb = RC_S(bx, ax), lc = RC_S(RC_M(ax, by), RC_M(bx, ay));
+      const double r = __drcp_rn(__dsqrt_rn(RC_A(RC_M(la, la), RC_M(lb, lb))));
+      st.l[3 * ci] = RC_M(la, r);
+      st.l[3 * ci + 1] = RC_M(lb, r);
+      st.l[3 * ci + 2] = RC_M(lc, r);
     });
   }
   // bounding boxes: min x0, min y0, -max x0, -max y0, then side 1
@@ -157,10 +154,10 @@ __device__ void hg_stage_pair(const HomographyArgs& a, int p, const HgStage& st,
     double c[2][2], s[2];
     for (int side = 0; side < 2; ++side) {
       const double lx = red[4 * side], ly = red[4 * side + 1], hx = -red[4 * side + 2], hy = -red[4 * side + 3];
-      c[side][0] = HG_M(HG_A(lx, hx), 0.5);
-      c[side][1] = HG_M(HG_A(ly, hy), 0.5);
-      const double wx = HG_S(hx, lx), wy = HG_S(hy, ly);
-      double sc = HG_M(wx > wy ? wx : wy, 0.5);
+      c[side][0] = RC_M(RC_A(lx, hx), 0.5);
+      c[side][1] = RC_M(RC_A(ly, hy), 0.5);
+      const double wx = RC_S(hx, lx), wy = RC_S(hy, ly);
+      double sc = RC_M(wx > wy ? wx : wy, 0.5);
       if (!(sc > 0.0)) sc = 1.0;   // one point, or no correspondence
       s[side] = sc;
     }
@@ -176,47 +173,47 @@ __device__ void hg_stage_pair(const HomographyArgs& a, int p, const HgStage& st,
 __device__ __forceinline__ void hg_rows(const HgStage& st, const HgPair& sp, int d, double* r0, double* r1) {
   if (d < sp.np) {
     const float4 q = st.pt[d];
-    const double x = HG_M(HG_S(q.x, sp.c0x), sp.i0), y = HG_M(HG_S(q.y, sp.c0y), sp.i0);
-    const double u = HG_M(HG_S(q.z, sp.c1x), sp.i1), v = HG_M(HG_S(q.w, sp.c1y), sp.i1);
+    const double x = RC_M(RC_S(q.x, sp.c0x), sp.i0), y = RC_M(RC_S(q.y, sp.c0y), sp.i0);
+    const double u = RC_M(RC_S(q.z, sp.c1x), sp.i1), v = RC_M(RC_S(q.w, sp.c1y), sp.i1);
     r0[0] = x; r0[1] = y; r0[2] = 1.0; r0[3] = 0.0; r0[4] = 0.0; r0[5] = 0.0;
-    r0[6] = -HG_M(u, x); r0[7] = -HG_M(u, y); r0[8] = -u;
+    r0[6] = -RC_M(u, x); r0[7] = -RC_M(u, y); r0[8] = -u;
     r1[0] = 0.0; r1[1] = 0.0; r1[2] = 0.0; r1[3] = x; r1[4] = y; r1[5] = 1.0;
-    r1[6] = -HG_M(v, x); r1[7] = -HG_M(v, y); r1[8] = -v;
+    r1[6] = -RC_M(v, x); r1[7] = -RC_M(v, y); r1[8] = -v;
   } else {
     const int i = d - sp.np;
     const float4 q = st.a[i], t = st.b[i];
-    const double ua = HG_M(HG_S(t.x, sp.c1x), sp.i1), va = HG_M(HG_S(t.y, sp.c1y), sp.i1);
-    const double ub = HG_M(HG_S(t.z, sp.c1x), sp.i1), vb = HG_M(HG_S(t.w, sp.c1y), sp.i1);
-    const double la = HG_S(va, vb), lb = HG_S(ub, ua), lc = HG_S(HG_M(ua, vb), HG_M(ub, va));
-    const double r = __drcp_rn(__dsqrt_rn(HG_A(HG_M(la, la), HG_M(lb, lb))));
-    const double A = HG_M(la, r), B = HG_M(lb, r), C = HG_M(lc, r);
+    const double ua = RC_M(RC_S(t.x, sp.c1x), sp.i1), va = RC_M(RC_S(t.y, sp.c1y), sp.i1);
+    const double ub = RC_M(RC_S(t.z, sp.c1x), sp.i1), vb = RC_M(RC_S(t.w, sp.c1y), sp.i1);
+    const double la = RC_S(va, vb), lb = RC_S(ub, ua), lc = RC_S(RC_M(ua, vb), RC_M(ub, va));
+    const double r = __drcp_rn(__dsqrt_rn(RC_A(RC_M(la, la), RC_M(lb, lb))));
+    const double A = RC_M(la, r), B = RC_M(lb, r), C = RC_M(lc, r);
     double* rr[2] = {r0, r1};
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const double x = HG_M(HG_S(e ? q.z : q.x, sp.c0x), sp.i0), y = HG_M(HG_S(e ? q.w : q.y, sp.c0y), sp.i0);
+      const double x = RC_M(RC_S(e ? q.z : q.x, sp.c0x), sp.i0), y = RC_M(RC_S(e ? q.w : q.y, sp.c0y), sp.i0);
       double* o = rr[e];
-      o[0] = HG_M(A, x); o[1] = HG_M(A, y); o[2] = A;
-      o[3] = HG_M(B, x); o[4] = HG_M(B, y); o[5] = B;
-      o[6] = HG_M(C, x); o[7] = HG_M(C, y); o[8] = C;
+      o[0] = RC_M(A, x); o[1] = RC_M(A, y); o[2] = A;
+      o[3] = RC_M(B, x); o[4] = RC_M(B, y); o[5] = B;
+      o[6] = RC_M(C, x); o[7] = RC_M(C, y); o[8] = C;
     }
   }
 }
 
 // Normalised h (9) -> pixel H = T1^-1 H^ T0 / H33; false when |H33| < 1e-12 or a result is not finite.
 __device__ __forceinline__ bool hg_to_pixels(const HgPair& sp, const double* h, double* H) {
-  const double t0x = -HG_M(sp.c0x, sp.i0), t0y = -HG_M(sp.c0y, sp.i0);
+  const double t0x = -RC_M(sp.c0x, sp.i0), t0y = -RC_M(sp.c0y, sp.i0);
   double M[9];
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
-    M[3 * i] = HG_M(h[3 * i], sp.i0);
-    M[3 * i + 1] = HG_M(h[3 * i + 1], sp.i0);
-    M[3 * i + 2] = HG_A(HG_A(HG_M(h[3 * i], t0x), HG_M(h[3 * i + 1], t0y)), h[3 * i + 2]);
+    M[3 * i] = RC_M(h[3 * i], sp.i0);
+    M[3 * i + 1] = RC_M(h[3 * i + 1], sp.i0);
+    M[3 * i + 2] = RC_A(RC_A(RC_M(h[3 * i], t0x), RC_M(h[3 * i + 1], t0y)), h[3 * i + 2]);
   }
   double G[9];
 #pragma unroll
   for (int j = 0; j < 3; ++j) {
-    G[j] = HG_A(HG_M(sp.s1, M[j]), HG_M(sp.c1x, M[6 + j]));
-    G[3 + j] = HG_A(HG_M(sp.s1, M[3 + j]), HG_M(sp.c1y, M[6 + j]));
+    G[j] = RC_A(RC_M(sp.s1, M[j]), RC_M(sp.c1x, M[6 + j]));
+    G[3 + j] = RC_A(RC_M(sp.s1, M[3 + j]), RC_M(sp.c1y, M[6 + j]));
     G[6 + j] = M[6 + j];
   }
   if (!(fabs(G[8]) >= 1e-12)) return false;
@@ -256,14 +253,14 @@ __device__ __noinline__ bool hg_hypothesis(const HgStage& st, const HgPair& sp, 
       for (int j = 0; j < 9; ++j) { const double t = A[c][j]; A[c][j] = A[piv][j]; A[piv][j] = t; }
     for (int r = c + 1; r < 8; ++r) {
       const double f = __ddiv_rn(A[r][c], A[c][c]);
-      for (int j = c + 1; j < 9; ++j) A[r][j] = HG_S(A[r][j], HG_M(f, A[c][j]));
+      for (int j = c + 1; j < 9; ++j) A[r][j] = RC_S(A[r][j], RC_M(f, A[c][j]));
     }
   }
   double h[9];
   h[8] = 1.0;
   for (int i = 7; i >= 0; --i) {
     double acc = A[i][8];
-    for (int j = i + 1; j < 8; ++j) acc = HG_S(acc, HG_M(A[i][j], h[j]));
+    for (int j = i + 1; j < 8; ++j) acc = RC_S(acc, RC_M(A[i][j], h[j]));
     h[i] = __ddiv_rn(acc, A[i][i]);
     if (!isfinite(h[i])) return false;
   }
@@ -271,11 +268,11 @@ __device__ __noinline__ bool hg_hypothesis(const HgStage& st, const HgPair& sp, 
 }
 
 __device__ __forceinline__ bool hg_project(const double* H, double x, double y, double& px, double& py) {
-  const double w = HG_A(HG_A(HG_M(H[6], x), HG_M(H[7], y)), H[8]);
+  const double w = RC_A(RC_A(RC_M(H[6], x), RC_M(H[7], y)), H[8]);
   if (!(fabs(w) > HG_FLT_EPS)) return false;
   const double r = __drcp_rn(w);
-  px = HG_M(HG_A(HG_A(HG_M(H[0], x), HG_M(H[1], y)), H[2]), r);
-  py = HG_M(HG_A(HG_A(HG_M(H[3], x), HG_M(H[4], y)), H[5]), r);
+  px = RC_M(RC_A(RC_A(RC_M(H[0], x), RC_M(H[1], y)), H[2]), r);
+  py = RC_M(RC_A(RC_A(RC_M(H[3], x), RC_M(H[4], y)), H[5]), r);
   return true;
 }
 
@@ -284,16 +281,16 @@ __device__ __forceinline__ bool hg_inlier(const HgStage& st, const HgPair& sp, c
     const float4 q = st.pt[d];
     double px, py;
     if (!hg_project(H, q.x, q.y, px, py)) return false;
-    const double dx = HG_S(px, q.z), dy = HG_S(py, q.w);
-    return HG_A(HG_M(dx, dx), HG_M(dy, dy)) < t2;
+    const double dx = RC_S(px, q.z), dy = RC_S(py, q.w);
+    return RC_A(RC_M(dx, dx), RC_M(dy, dy)) < t2;
   }
   const int i = d - sp.np;
   const float4 q = st.a[i];
   const double la = st.l[3 * i], lb = st.l[3 * i + 1], lc = st.l[3 * i + 2];
   double ax, ay, bx, by;
   if (!hg_project(H, q.x, q.y, ax, ay) || !hg_project(H, q.z, q.w, bx, by)) return false;
-  const double da = HG_A(HG_A(HG_M(la, ax), HG_M(lb, ay)), lc), db = HG_A(HG_A(HG_M(la, bx), HG_M(lb, by)), lc);
-  const double ea = HG_M(da, da), eb = HG_M(db, db);
+  const double da = RC_A(RC_A(RC_M(la, ax), RC_M(lb, ay)), lc), db = RC_A(RC_A(RC_M(la, bx), RC_M(lb, by)), lc);
+  const double ea = RC_M(da, da), eb = RC_M(db, db);
   return (ea > eb ? ea : eb) < t2;
 }
 
@@ -462,9 +459,5 @@ __global__ void __launch_bounds__(HG_REFIT_THREADS) homography_refit_kernel(Homo
     for (int r = lb + threadIdx.x; r < le; r += NT) a.inl_l[r] = 0;
   }
 }
-
-#undef HG_M
-#undef HG_A
-#undef HG_S
 
 }  // namespace ltr

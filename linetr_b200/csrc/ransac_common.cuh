@@ -5,6 +5,7 @@
 // finder (geometry.sturm_roots) and the cyclic Jacobi eigen-solvers of the refits and decompositions.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 
 namespace ltr {
 
@@ -68,11 +69,6 @@ __device__ __forceinline__ bool hg_draw(unsigned long long seed, int p, int k, i
   }
   return got == S;
 }
-
-#define RC_M __dmul_rn
-#define RC_A __dadd_rn
-#define RC_S __dsub_rn
-#define RC_D __ddiv_rn
 
 // Null basis of the S epipolar rows (x1 x0, x1 y0, x1, y1 x0, y1 y0, y1, x0, y0, 1) of q[c] = (x0, y0, x1, y1), S = 5
 // (essential) or 7 (fundamental): the Householder QR of the 9 x S transpose (reflector c zeroes column c below the
@@ -232,12 +228,6 @@ __device__ int ess_roots(const double* p, double* roots) {
   return count;
 }
 
-__device__ __forceinline__ void ess_cross(const double* x, const double* y, double* c) {
-  c[0] = RC_S(RC_M(x[1], y[2]), RC_M(x[2], y[1]));
-  c[1] = RC_S(RC_M(x[2], y[0]), RC_M(x[0], y[2]));
-  c[2] = RC_S(RC_M(x[0], y[1]), RC_M(x[1], y[0]));
-}
-
 // Cyclic Jacobi eigen-decomposition of the symmetric 3 x 3 S (diagonalised in place; V accumulates the rotations and
 // must start as the identity).
 __device__ __forceinline__ void rc_jacobi3(double (*S)[3], double (*V)[3]) {
@@ -312,10 +302,6 @@ __device__ __noinline__ void hg_smallest_eigvec(double* M, double* h) {
   for (int k = 0; k < 9; ++k) h[k] = V[9 * k + m];
 }
 
-#undef RC_M
-#undef RC_A
-#undef RC_S
-#undef RC_D
 #undef ESS_CHAIN_OFF
 
 }  // namespace ltr

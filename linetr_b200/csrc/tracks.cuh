@@ -32,6 +32,7 @@
 //                      track's observations, then candidates, winner, refit and the outputs.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 #include "fundamental.cuh"
 #include "triangulation.cuh"
 
@@ -64,11 +65,6 @@ struct TrkArgs {
   double* row_points; double* row_lines;     // [n_nodes[0], 3], [n_nodes[1], 2, 3]
   uint8_t* inlier[2]; int* n_views[2];
 };
-
-#define RC_M __dmul_rn
-#define RC_A __dadd_rn
-#define RC_S __dsub_rn
-#define RC_D __ddiv_rn
 
 __device__ __forceinline__ int trk_find(const int* par, int x) {
   int p = __ldcg(par + x);
@@ -119,7 +115,7 @@ __global__ void __launch_bounds__(TRK_ROW_THREADS) trk_edge_kernel(const TrkArgs
   if (r >= (long long)a.total_p + a.total_l) return;
   const int* cu = lines ? a.cu_l : a.cu_p;
   const int* off = lines ? a.seg_off : a.kp_off;
-  const int p = tri_segment(cu, a.n_pairs, row);
+  const int p = rc_segment(cu, a.n_pairs, row);
   const int i = a.pairs[2 * p], j = a.pairs[2 * p + 1];
   const int k = row - cu[p], m = (lines ? a.matches_l : a.matches_p)[row];
   if (!(m >= 0 && m < off[j + 1] - off[j])) return;
@@ -222,7 +218,7 @@ __global__ void __launch_bounds__(TRK_ROW_THREADS) trk_assign_kernel(const TrkAr
 // Observation q supports the world point X: depth P_z > 0 (P = R_q X + t_q) and squared reprojection error <= t2.
 __device__ __forceinline__ bool trk_point_supports(const double* c, float2 px, const double* X, double t2) {
   double P[3];
-  tri_mv(c + 4, X, P);
+  rc_mv3(c + 4, X, P);
   for (int e = 0; e < 3; ++e) P[e] = RC_A(P[e], c[13 + e]);
   const double dx = RC_S((double)px.x, c[2]), dy = RC_S((double)px.y, c[3]);
   const double ex = RC_S(RC_M(c[0], P[0]), RC_M(dx, P[2])), ey = RC_S(RC_M(c[1], P[1]), RC_M(dy, P[2]));
@@ -232,21 +228,21 @@ __device__ __forceinline__ bool trk_point_supports(const double* c, float2 px, c
 // Observation q supports the world end point X: P_z > 0 and (n_q . P)^2 <= t2 P_z^2 (q's line normal at c + 25).
 __device__ __forceinline__ bool trk_end_supports(const double* c, const double* X, double t2) {
   double P[3];
-  tri_mv(c + 4, X, P);
+  rc_mv3(c + 4, X, P);
   for (int e = 0; e < 3; ++e) P[e] = RC_A(P[e], c[13 + e]);
-  const double v = tri_dot(c + 25, P);
+  const double v = rc_dot3(c + 25, P);
   return P[2] > 0.0 && RC_M(v, v) <= RC_M(t2, RC_M(P[2], P[2]));
 }
 
 // The depth P_z of world point X in observation q.
 __device__ __forceinline__ double trk_depth(const double* c, const double* X) {
-  return RC_A(tri_dot(c + 10, X), c[15]);
+  return RC_A(rc_dot3(c + 10, X), c[15]);
 }
 
 // Partner j as ltr_triangulate's camera relative to anchor i (TRI_CAM doubles: fx fy cx cy, R_j, A = R_j C_i + t_j).
 __device__ __forceinline__ void trk_partner(const double* ci, const double* cj, double* o) {
   for (int e = 0; e < 13; ++e) o[e] = cj[e];
-  tri_mv(cj + 4, ci + 16, o + 13);
+  rc_mv3(cj + 4, ci + 16, o + 13);
   for (int e = 0; e < 3; ++e) o[13 + e] = RC_A(o[13 + e], cj[13 + e]);
 }
 
@@ -261,7 +257,7 @@ __device__ __forceinline__ bool trk_point_candidate(const double (*cam)[TRK_CAM]
   if (!(s > 0.0)) return false;
   double P[3];
   for (int e = 0; e < 3; ++e) P[e] = RC_A(c[13 + e], RC_M(s, t.B[e]));
-  if (!(tri_dot(t.B, P) <= RC_M(cos_min, __dsqrt_rn(RC_M(tri_dot(t.B, t.B), tri_dot(P, P)))))) return false;
+  if (!(rc_dot3(t.B, P) <= RC_M(cos_min, __dsqrt_rn(RC_M(rc_dot3(t.B, t.B), rc_dot3(P, P)))))) return false;
   for (int e = 0; e < 3; ++e) X[e] = RC_A(cam[i][16 + e], RC_M(s, r[e]));
   return true;
 }
@@ -274,7 +270,7 @@ __device__ __forceinline__ bool trk_line_candidate(const double (*cam)[TRK_CAM],
   const double* n = cam[j] + 25;
   const double* r0 = cam[i] + 19;
   const double* r1 = cam[i] + 22;
-  const double alpha = tri_dot(n, c + 13), nn = tri_dot(n, n);
+  const double alpha = rc_dot3(n, c + 13), nn = rc_dot3(n, n);
   const TriEnd e0 = tri_end_terms(c, n, r0), e1 = tri_end_terms(c, n, r1);
   const double s0 = -RC_D(alpha, e0.beta), s1 = -RC_D(alpha, e1.beta);
   if (!(s0 > 0.0 && s1 > 0.0)) return false;
@@ -308,7 +304,7 @@ __device__ __forceinline__ void trk_gn_term(double num, double den, const double
 __device__ __forceinline__ void trk_pixel_terms(const double* c, const double* A, float2 px, const double* Y, double* h,
                                                 double* g) {
   double P[3];
-  tri_mv(c + 4, Y, P);
+  rc_mv3(c + 4, Y, P);
   for (int e = 0; e < 3; ++e) P[e] = RC_A(P[e], A[e]);
   const double dx = RC_S((double)px.x, c[2]), dy = RC_S((double)px.y, c[3]);
   const double* R = c + 4;
@@ -322,13 +318,13 @@ __device__ __forceinline__ void trk_pixel_terms(const double* c, const double* A
 // The signed-distance residual n . P / P_z of observation c at Y.
 __device__ __forceinline__ void trk_line_term(const double* c, const double* A, const double* Y, double* h, double* g) {
   double P[3];
-  tri_mv(c + 4, Y, P);
+  rc_mv3(c + 4, Y, P);
   for (int e = 0; e < 3; ++e) P[e] = RC_A(P[e], A[e]);
   const double* R = c + 4;
   const double* n = c + 25;
   double b[3];
   for (int k = 0; k < 3; ++k) b[k] = RC_A(RC_A(RC_M(n[0], R[k]), RC_M(n[1], R[3 + k])), RC_M(n[2], R[6 + k]));
-  trk_gn_term(tri_dot(n, P), P[2], b, R + 6, h, g);
+  trk_gn_term(rc_dot3(n, P), P[2], b, R + 6, h, g);
 }
 
 // Y -= H^-1 g by Gaussian elimination with first-largest partial pivoting; false (Y unchanged) on a zero pivot or a
@@ -398,8 +394,8 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_kernel(const TrkArgs a) {
     }
     __syncthreads();
     for (int q = tid; q < V; q += TRK_THREADS) {
-      const int img = tri_segment(off, a.n_images, obs[q]);
-      if (q == 0 || img != tri_segment(off, a.n_images, obs[q - 1])) atomicAdd(&s_nimg, 1);
+      const int img = rc_segment(off, a.n_images, obs[q]);
+      if (q == 0 || img != rc_segment(off, a.n_images, obs[q - 1])) atomicAdd(&s_nimg, 1);
     }
     __syncthreads();
     if (tid == 0) {
@@ -418,25 +414,24 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_kernel(const TrkArgs a) {
     }
     // stage each observation's camera, centre, ray(s) and pixel / line normal
     if (tid < V) {
-      const int node = s_node[tid], v = tri_segment(off, a.n_images, node);
+      const int node = s_node[tid], v = rc_segment(off, a.n_images, node);
       double* c = s_cam[tid];
       const double* Kv = a.K + 9 * v;
       c[0] = Kv[0]; c[1] = Kv[4]; c[2] = Kv[2]; c[3] = Kv[5];
       for (int e = 0; e < 9; ++e) c[4 + e] = a.R[9 * v + e];
       for (int e = 0; e < 3; ++e) c[13 + e] = a.t[3 * v + e];
       const double* Rv = c + 4;
-      for (int j = 0; j < 3; ++j)
-        c[16 + j] = -RC_A(RC_A(RC_M(Rv[j], c[13]), RC_M(Rv[3 + j], c[14])), RC_M(Rv[6 + j], c[15]));
+      rc_centre(Rv, c + 13, c + 16);
       if (lines) {
         const float4 s = sg[node];
         s_px[tid] = s;
-        tri_ray(Rv, c[0], c[1], c[2], c[3], s.x, s.y, c + 19);
-        tri_ray(Rv, c[0], c[1], c[2], c[3], s.z, s.w, c + 22);
-        tri_line_normal(c, s, c + 25);
+        rc_ray(Rv, c[0], c[1], c[2], c[3], s.x, s.y, c + 19);
+        rc_ray(Rv, c[0], c[1], c[2], c[3], s.z, s.w, c + 22);
+        rc_line_normal(c, s, c + 25);
       } else {
         const float2 q = kp[node];
         s_px[tid] = make_float4(q.x, q.y, 0.f, 0.f);
-        tri_ray(Rv, c[0], c[1], c[2], c[3], q.x, q.y, c + 19);
+        rc_ray(Rv, c[0], c[1], c[2], c[3], q.x, q.y, c + 19);
       }
     }
     __syncthreads();
@@ -486,12 +481,12 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_kernel(const TrkArgs a) {
             const float2 pe = e ? make_float2(s_px[i].z, s_px[i].w) : make_float2(s_px[i].x, s_px[i].y);
             for (int it = 0; it < TRK_GN_ITERS; ++it) {
               double h[6] = {0, 0, 0, 0, 0, 0}, gr[3] = {0, 0, 0};
-              tri_mv(ci + 4, ci + 16, A);
+              rc_mv3(ci + 4, ci + 16, A);
               for (int k = 0; k < 3; ++k) A[k] = RC_A(A[k], ci[13 + k]);
               trk_pixel_terms(ci, A, pe, Y, h, gr);
               for (int q = 0; q < V; ++q) {
                 if (q == i || !((mask >> q) & 1ull)) continue;
-                tri_mv(s_cam[q] + 4, ci + 16, A);
+                rc_mv3(s_cam[q] + 4, ci + 16, A);
                 for (int k = 0; k < 3; ++k) A[k] = RC_A(A[k], s_cam[q][13 + k]);
                 trk_line_term(s_cam[q], A, Y, h, gr);
               }
@@ -519,7 +514,7 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_kernel(const TrkArgs a) {
             double h[6] = {0, 0, 0, 0, 0, 0}, gr[3] = {0, 0, 0};
             for (int q = 0; q < V; ++q) {
               if (!((mask >> q) & 1ull)) continue;
-              tri_mv(s_cam[q] + 4, ci + 16, A);
+              rc_mv3(s_cam[q] + 4, ci + 16, A);
               for (int k = 0; k < 3; ++k) A[k] = RC_A(A[k], s_cam[q][13 + k]);
               trk_pixel_terms(s_cam[q], A, make_float2(s_px[q].x, s_px[q].y), Y, h, gr);
             }
@@ -566,13 +561,7 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_kernel(const TrkArgs a) {
             d[k] = RC_S(s_X[3 + k], s_X[k]);
             w[k] = RC_S(s_X[k], c[16 + k]);
           }
-          for (int e = 0; e < 2; ++e) {
-            const double* r = c + 19 + 3 * e;
-            const double aa = tri_dot(d, d), b = tri_dot(d, r), cc = tri_dot(r, r), dd = tri_dot(d, w),
-                         ee = tri_dot(r, w);
-            const double u = RC_D(RC_S(RC_M(b, ee), RC_M(cc, dd)), RC_S(RC_M(aa, cc), RC_M(b, b)));
-            for (int k = 0; k < 3; ++k) a.row_lines[6ll * row + 3 * e + k] = RC_A(s_X[k], RC_M(u, d[k]));
-          }
+          for (int e = 0; e < 2; ++e) rc_closest_on_line(s_X, d, w, c + 19 + 3 * e, a.row_lines + 6ll * row + 3 * e);
         } else {
           for (int k = 0; k < 3; ++k) a.row_points[3ll * row + k] = s_X[k];
         }
@@ -581,10 +570,5 @@ __global__ void __launch_bounds__(TRK_THREADS) trk_kernel(const TrkArgs a) {
     __syncthreads();
   }
 }
-
-#undef RC_M
-#undef RC_A
-#undef RC_S
-#undef RC_D
 
 }  // namespace ltr

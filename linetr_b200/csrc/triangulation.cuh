@@ -29,6 +29,7 @@
 //                       and each thread's partner pixels in dynamic shared memory.
 #pragma once
 #include "common.cuh"
+#include "rn_fp64.cuh"
 
 namespace ltr {
 
@@ -56,44 +57,13 @@ struct TriArgs {
   double* points3d; double* lines3d; int* n_views_p; int* n_views_l;
 };
 
-#define RC_M __dmul_rn
-#define RC_A __dadd_rn
-#define RC_S __dsub_rn
-#define RC_D __ddiv_rn
-
-// Largest g in [0, n) with off[g] <= x (off non-decreasing, off[0] <= x < off[n]).
-__device__ __forceinline__ int tri_segment(const int* __restrict__ off, int n, int x) {
-  int lo = 0, hi = n - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (off[mid] <= x) lo = mid; else hi = mid - 1;
-  }
-  return lo;
-}
-
-__device__ __forceinline__ double tri_dot(const double* a, const double* b) {
-  return RC_A(RC_A(RC_M(a[0], b[0]), RC_M(a[1], b[1])), RC_M(a[2], b[2]));
-}
-
-// M v for a row-major 3 x 3 M
-__device__ __forceinline__ void tri_mv(const double* M, const double* v, double* o) {
-  for (int i = 0; i < 3; ++i) o[i] = tri_dot(M + 3 * i, v);
-}
-
-// The anchor ray r = R^T ((x - cx) / fx, (y - cy) / fy, 1) of pixel (x, y).
-__device__ __forceinline__ void tri_ray(const double* R, double fx, double fy, double cx, double cy, float x, float y,
-                                        double* r) {
-  const double nx = RC_D(RC_S((double)x, cx), fx), ny = RC_D(RC_S((double)y, cy), fy);
-  for (int k = 0; k < 3; ++k) r[k] = RC_A(RC_A(RC_M(R[k], nx), RC_M(R[3 + k], ny)), R[6 + k]);
-}
-
 // A point observation's residual terms in partner camera c (TRI_CAM doubles): x numerator ax + s bx, y numerator
 // ay + s by, denominator A[2] + s B[2]; B = R_v r.
 struct TriPt { double ax, bx, ay, by, B[3]; };
 
 __device__ __forceinline__ TriPt tri_point_terms(const double* c, const double* r, float2 px) {
   TriPt o;
-  tri_mv(c + 4, r, o.B);
+  rc_mv3(c + 4, r, o.B);
   const double* A = c + 13;
   const double dx = RC_S((double)px.x, c[2]), dy = RC_S((double)px.y, c[3]);
   o.ax = RC_S(RC_M(c[0], A[0]), RC_M(dx, A[2]));
@@ -109,25 +79,13 @@ __device__ __forceinline__ bool tri_point_supports(const TriPt& o, double Az, do
   return pz > 0.0 && RC_A(RC_M(ex, ex), RC_M(ey, ey)) <= RC_M(t2, RC_M(pz, pz));
 }
 
-// The partner segment (x0, y0, x1, y1) as a unit pixel line in camera-ray form through partner camera c: n . P / Pz is
-// the signed pixel distance of the projection of the camera point P.
-__device__ __forceinline__ void tri_line_normal(const double* c, float4 s, double* n) {
-  const double x0 = s.x, y0 = s.y, x1 = s.z, y1 = s.w;
-  const double a = RC_S(y0, y1), b = RC_S(x1, x0), cc = RC_S(RC_M(x0, y1), RC_M(x1, y0));
-  const double rn = RC_D(1.0, __dsqrt_rn(RC_A(RC_M(a, a), RC_M(b, b))));
-  const double la = RC_M(a, rn), lb = RC_M(b, rn), lc = RC_M(cc, rn);
-  n[0] = RC_M(la, c[0]);
-  n[1] = RC_M(lb, c[1]);
-  n[2] = RC_A(RC_A(RC_M(la, c[2]), RC_M(lb, c[3])), lc);
-}
-
 // An end point's residual terms: numerator alpha + s beta, denominator A[2] + s delta.
 struct TriEnd { double beta, delta, BB; };
 
 __device__ __forceinline__ TriEnd tri_end_terms(const double* c, const double* n, const double* r) {
   double B[3];
-  tri_mv(c + 4, r, B);
-  return TriEnd{tri_dot(n, B), B[2], tri_dot(B, B)};
+  rc_mv3(c + 4, r, B);
+  return TriEnd{rc_dot3(n, B), B[2], rc_dot3(B, B)};
 }
 
 __device__ __forceinline__ bool tri_end_supports(double alpha, const TriEnd& e, double Az, double s, double t2) {
@@ -162,7 +120,7 @@ __global__ void __launch_bounds__(TRI_SCATTER_THREADS) tri_scatter_kernel(const 
   if (r >= (long long)a.total_p + a.total_l) return;
   const int* cu = lines ? a.cu_l : a.cu_p;
   const int* inv_off = lines ? a.inv_off_l : a.inv_off_p;
-  const int p = tri_segment(cu, a.n_pairs, row);
+  const int p = rc_segment(cu, a.n_pairs, row);
   const int m = (lines ? a.matches_l : a.matches_p)[row];
   if (m >= 0 && m < inv_off[p + 1] - inv_off[p]) atomicMin((lines ? a.inv_l : a.inv_p) + inv_off[p] + m, row - cu[p]);
 }
@@ -173,7 +131,7 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
   extern __shared__ float4 s_px[];             // [V][TRI_THREADS] each thread's partner pixel / segment
   pdl_launch_dependents();
   const int tid = threadIdx.x;
-  const int g = tri_segment(a.block_off, 2 * a.n_images, blockIdx.x);
+  const int g = rc_segment(a.block_off, 2 * a.n_images, blockIdx.x);
   const bool lines = g >= a.n_images;
   const int img = lines ? g - a.n_images : g;
   const int* off = lines ? a.seg_off : a.kp_off;
@@ -182,7 +140,7 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
   const double* Ra = a.R + 9 * img;
   const double* ta = a.t + 3 * img;
   double C[3];
-  for (int j = 0; j < 3; ++j) C[j] = -RC_A(RC_A(RC_M(Ra[j], ta[0]), RC_M(Ra[3 + j], ta[1])), RC_M(Ra[6 + j], ta[2]));
+  rc_centre(Ra, ta, C);
   for (int o = tid; o < V; o += TRI_THREADS) {
     const int code = a.views[vb + o], p = code >> 1, side = code & 1;
     const int v = a.pairs[2 * p + 1 - side];
@@ -190,7 +148,7 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
     double* c = s_cam[o];
     c[0] = Kv[0]; c[1] = Kv[4]; c[2] = Kv[2]; c[3] = Kv[5];
     for (int e = 0; e < 9; ++e) c[4 + e] = a.R[9 * v + e];
-    tri_mv(c + 4, C, c + 13);
+    rc_mv3(c + 4, C, c + 13);
     for (int e = 0; e < 3; ++e) c[13 + e] = RC_A(c[13 + e], a.t[3 * v + e]);
     s_obs[o][0] = code;
     s_obs[o][1] = v;
@@ -226,7 +184,7 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
   if (!lines) {
     const float2 q = reinterpret_cast<const float2*>(a.kpts)[off[img] + k];
     double r[3];
-    tri_ray(Ra, fx, fy, cx, cy, q.x, q.y, r);
+    rc_ray(Ra, fx, fy, cx, cy, q.x, q.y, r);
     int best = -1;
     double s_best = 0.0;
     unsigned long long mask = 0ull;
@@ -238,7 +196,7 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
       if (!(s > 0.0)) continue;
       double P[3];
       for (int e = 0; e < 3; ++e) P[e] = RC_A(c[13 + e], RC_M(s, t.B[e]));
-      if (!(tri_dot(t.B, P) <= RC_M(a.cos_min, __dsqrt_rn(RC_M(tri_dot(t.B, t.B), tri_dot(P, P)))))) continue;
+      if (!(rc_dot3(t.B, P) <= RC_M(a.cos_min, __dsqrt_rn(RC_M(rc_dot3(t.B, t.B), rc_dot3(P, P)))))) continue;
       unsigned long long m = 0ull;
       int cnt = 0;
       for (int q = 0; q < V; ++q) {
@@ -292,16 +250,16 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
   } else {
     const float4 sg = reinterpret_cast<const float4*>(a.segs)[off[img] + k];
     double r0[3], r1[3];
-    tri_ray(Ra, fx, fy, cx, cy, sg.x, sg.y, r0);
-    tri_ray(Ra, fx, fy, cx, cy, sg.z, sg.w, r1);
+    rc_ray(Ra, fx, fy, cx, cy, sg.x, sg.y, r0);
+    rc_ray(Ra, fx, fy, cx, cy, sg.z, sg.w, r1);
     int best = -1;
     double b0 = 0.0, b1 = 0.0;
     unsigned long long mask = 0ull;
     for (int o = 0; o < V; ++o) {
       const double* c = s_cam[o];
       double n[3];
-      tri_line_normal(c, s_px[o * TRI_THREADS + tid], n);
-      const double alpha = tri_dot(n, c + 13), nn = tri_dot(n, n);
+      rc_line_normal(c, s_px[o * TRI_THREADS + tid], n);
+      const double alpha = rc_dot3(n, c + 13), nn = rc_dot3(n, n);
       const TriEnd e0 = tri_end_terms(c, n, r0), e1 = tri_end_terms(c, n, r1);
       const double s0 = -RC_D(alpha, e0.beta), s1 = -RC_D(alpha, e1.beta);
       if (!(s0 > 0.0 && s1 > 0.0)) continue;
@@ -313,8 +271,8 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
       for (int q = 0; q < V; ++q) {
         const double* cq = s_cam[q];
         double nq[3];
-        tri_line_normal(cq, s_px[q * TRI_THREADS + tid], nq);
-        const double aq = tri_dot(nq, cq + 13);
+        rc_line_normal(cq, s_px[q * TRI_THREADS + tid], nq);
+        const double aq = rc_dot3(nq, cq + 13);
         const bool sup = tri_end_supports(aq, tri_end_terms(cq, nq, r0), cq[15], s0, t2) &&
                          tri_end_supports(aq, tri_end_terms(cq, nq, r1), cq[15], s1, t2);
         m |= (unsigned long long)sup << q;
@@ -341,9 +299,9 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
             if (!((mask >> q) & 1ull)) continue;
             const double* cq = s_cam[q];
             double nq[3];
-            tri_line_normal(cq, s_px[q * TRI_THREADS + tid], nq);
+            rc_line_normal(cq, s_px[q * TRI_THREADS + tid], nq);
             const TriEnd t = tri_end_terms(cq, nq, r);
-            tri_gn_term(tri_dot(nq, cq + 13), t.beta, cq[15], t.delta, s[e], jj, jr);
+            tri_gn_term(rc_dot3(nq, cq + 13), t.beta, cq[15], t.delta, s[e], jj, jr);
           }
           if (!tri_gn_step(jj, jr, s[e])) break;
         }
@@ -353,8 +311,8 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
         for (int q = 0; q < V; ++q) {
           const double* cq = s_cam[q];
           double nq[3];
-          tri_line_normal(cq, s_px[q * TRI_THREADS + tid], nq);
-          const double aq = tri_dot(nq, cq + 13);
+          rc_line_normal(cq, s_px[q * TRI_THREADS + tid], nq);
+          const double aq = rc_dot3(nq, cq + 13);
           cnt += tri_end_supports(aq, tri_end_terms(cq, nq, r0), cq[15], s[0], t2) &&
                  tri_end_supports(aq, tri_end_terms(cq, nq, r1), cq[15], s[1], t2);
         }
@@ -377,10 +335,5 @@ __global__ void __launch_bounds__(TRI_THREADS) tri_kernel(const TriArgs a) {
     a.n_views_l[row] = nvw;
   }
 }
-
-#undef RC_M
-#undef RC_A
-#undef RC_S
-#undef RC_D
 
 }  // namespace ltr

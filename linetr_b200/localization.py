@@ -34,6 +34,8 @@ import torch
 
 from . import _native as N
 from . import _ops
+from . import _posed
+from ._posed import block_sum
 from .geometry import SMEM_MAX, _intrinsics, _pool, draw_samples, sturm_roots
 
 AP_SAMPLE = 3
@@ -148,13 +150,8 @@ def line_normals(seg0, K):
     (a, b, c) through s0 scaled to a^2 + b^2 = 1, then n = (a fx, b fy, (a cx + b cy) + c), so that n . P / Pz is the
     signed pixel distance of the projection of the camera point P to the line."""
     s = np.asarray(seg0, dtype=np.float32).reshape(-1, 4).astype(np.float64)
-    ax, ay, bx, by = s[:, 0], s[:, 1], s[:, 2], s[:, 3]
-    fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
     with np.errstate(all="ignore"):
-        a, b, c = ay - by, bx - ax, ax * by - bx * ay
-        rn = 1.0 / np.sqrt(a * a + b * b)
-        la, lb, lc = a * rn, b * rn, c * rn
-    return np.stack([la * fx, lb * fy, (la * cx + lb * cy) + lc], 1)
+        return np.stack(_posed.line_normal(K[0, 0], K[1, 1], K[0, 2], K[1, 2], s), 1)
 
 
 @dataclass
@@ -236,38 +233,9 @@ def _row_terms(g: _Group, R, t, rows):
     return out
 
 
-def _block_sum(terms, nt=AP_FIT_THREADS):
-    """The refit kernel's reduction of per-row terms [n, m]: thread t sums rows t, t + nt, ... in order, each warp
-    folds its 32 lanes with the xor butterfly (16, 8, 4, 2, 1), then lane 0 of every warp is added in warp order."""
-    n, m = terms.shape
-    R = -(-n // nt)
-    pad = np.zeros((R * nt, m))
-    pad[:n] = terms
-    pad = pad.reshape(R, nt, m)
-    acc = np.zeros((nt, m))
-    for r in range(R):
-        acc = acc + pad[r]
-    acc = acc.reshape(nt // 32, 32, m)
-    lanes = np.arange(32)
-    for o in (16, 8, 4, 2, 1):
-        acc = acc + acc[:, lanes ^ o]
-    out = np.zeros(m)
-    for w in range(nt // 32):
-        out = out + acc[w, 0]
-    return out
-
-
 def cayley(w):
     """The Cayley map ((1 - w.w) I + 2 [w]x + 2 w w^T) / (1 + w.w) of w [3], explicitly rounded: [3, 3]."""
-    w = np.asarray(w, dtype=np.float64)
-    ww = (w[0] * w[0] + w[1] * w[1]) + w[2] * w[2]
-    den, s = 1.0 + ww, 1.0 - ww
-    wx = np.array([[0.0, -w[2], w[1]], [w[2], 0.0, -w[0]], [-w[1], w[0], 0.0]])
-    C = np.empty((3, 3))
-    for i in range(3):
-        for k in range(3):
-            C[i, k] = (((s if i == k else 0.0) + 2.0 * (w[i] * w[k])) + 2.0 * wx[i, k]) / den
-    return C
+    return np.array(_posed.cayley(np.asarray(w, dtype=np.float64)), dtype=np.float64)
 
 
 def _lm_step(S, lam, R, t):
@@ -314,14 +282,14 @@ def refine_pose_host(g: _Group, R, t, rows):
     frame: AP_LM_ITERS steps with damping AP_LM_LAMBDA0, multiplied by AP_LM_ACCEPT after a step that lowers the cost
     and by AP_LM_REJECT otherwise.  -> (R, t, cost, number of accepted steps)."""
     R, t = np.array(R, dtype=np.float64), np.array(t, dtype=np.float64)
-    S = _block_sum(_row_terms(g, R, t, rows))
+    S = block_sum(_row_terms(g, R, t, rows), AP_FIT_THREADS)
     lam, acc = AP_LM_LAMBDA0, 0
     for _ in range(AP_LM_ITERS):
         Rn, tn, ok = _lm_step(S, lam, R, t)
-        cost = _block_sum(_row_terms(g, Rn, tn, rows)[:, 27:])[0] if ok else np.nan
+        cost = block_sum(_row_terms(g, Rn, tn, rows)[:, 27:], AP_FIT_THREADS)[0] if ok else np.nan
         if ok and cost < S[27]:
             R, t, lam, acc = Rn, tn, lam * AP_LM_ACCEPT, acc + 1
-            S = _block_sum(_row_terms(g, R, t, rows))
+            S = block_sum(_row_terms(g, R, t, rows), AP_FIT_THREADS)
         else:
             lam = lam * AP_LM_REJECT
     return R, t, float(S[27]), acc

@@ -31,7 +31,9 @@ import torch
 from . import _native as N
 from . import _ops
 from .geometry import fundamental_inliers, lines_consistent
-from .triangulation import TriangulationResult, _check, _host, _offsets, _pool_rows
+from ._posed import (centre, check_set, closest_on_line, dot3, host, line_normal, mv3, offsets, pool64, ray,
+                     stage_with_pools)
+from .triangulation import TriangulationResult
 
 TRK_MAX_OBS = N.TRK_MAX_OBS
 TRK_GN_ITERS = 5           # Gauss-Newton steps of the refits (fixed budget)
@@ -80,15 +82,6 @@ def pair_fundamentals(S) -> np.ndarray:
 
 
 # ------------------------------------------------------------------ the model in numpy
-def _dot(a, b):
-    return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]
-
-
-def _mv(R, v):
-    """R [..., 9] row-major times v (3 arrays)."""
-    return [(R[..., 3 * e] * v[0] + R[..., 3 * e + 1] * v[1]) + R[..., 3 * e + 2] * v[2] for e in range(3)]
-
-
 class _Obs:
     """The staged observations of a group of tracks of V observations each: every field [T, V] (vectors: lists)."""
 
@@ -98,23 +91,14 @@ class _Obs:
         self.fx, self.fy, self.cx, self.cy = K[..., 0, 0], K[..., 1, 1], K[..., 0, 2], K[..., 1, 2]
         self.R = S.R[img].reshape(*nodes.shape, 9)
         self.t = [S.t[img][..., e] for e in range(3)]
-        R = self.R
-        self.C = [-((R[..., j] * self.t[0] + R[..., 3 + j] * self.t[1]) + R[..., 6 + j] * self.t[2]) for j in range(3)]
+        self.C = centre(self.R, self.t)
         px = pool[nodes]
         self.px = px
-        self.r0 = self._ray(px[..., 0], px[..., 1])
+        cam = (self.R, self.fx, self.fy, self.cx, self.cy)
+        self.r0 = ray(*cam, px[..., 0], px[..., 1])
         if lines:
-            self.r1 = self._ray(px[..., 2], px[..., 3])
-            x0, y0, x1, y1 = px[..., 0], px[..., 1], px[..., 2], px[..., 3]
-            a, b, c = y0 - y1, x1 - x0, x0 * y1 - x1 * y0
-            rn = 1.0 / np.sqrt(a * a + b * b)
-            la, lb, lc = a * rn, b * rn, c * rn
-            self.n = [la * self.fx, lb * self.fy, (la * self.cx + lb * self.cy) + lc]
-
-    def _ray(self, x, y):
-        nx, ny = (x - self.cx) / self.fx, (y - self.cy) / self.fy
-        R = self.R
-        return [(R[..., k] * nx + R[..., 3 + k] * ny) + R[..., 6 + k] for k in range(3)]
+            self.r1 = ray(*cam, px[..., 2], px[..., 3])
+            self.n = line_normal(self.fx, self.fy, self.cx, self.cy, px)
 
     def at(self, field, q):
         v = getattr(self, field)
@@ -122,14 +106,14 @@ class _Obs:
 
     def camera_P(self, X):
         """P = R_q X + t_q of world points X (3 arrays [T]) in every observation: 3 arrays [T, V]."""
-        P = _mv(self.R, [x[:, None] for x in X])
+        P = mv3(self.R, [x[:, None] for x in X])
         return [P[e] + self.t[e] for e in range(3)]
 
     def A(self, i, q):
         """R_q C_i + t_q of anchor column i for observation column q: 3 arrays [T]."""
         Ci = self.at("C", i)
         Rq = self.R[:, q]
-        return [x + self.t[e][:, q] for e, x in enumerate(_mv(Rq, Ci))]
+        return [x + self.t[e][:, q] for e, x in enumerate(mv3(Rq, Ci))]
 
 
 def _point_support(o: _Obs, X, t2):
@@ -141,7 +125,7 @@ def _point_support(o: _Obs, X, t2):
 
 def _end_support(o: _Obs, X, t2):
     P = o.camera_P(X)
-    v = _dot(o.n, P)
+    v = dot3(o.n, P)
     return (P[2] > 0) & ((v * v) <= t2 * (P[2] * P[2]))
 
 
@@ -153,14 +137,14 @@ def _point_candidate(o: _Obs, i, j, cos_min):
     A = o.A(i, j)
     r = o.at("r0", i)
     Rj = o.R[:, j]
-    B = _mv(Rj, r)
+    B = mv3(Rj, r)
     dx, dy = o.px[:, j, 0] - o.cx[:, j], o.px[:, j, 1] - o.cy[:, j]
     fx, fy = o.fx[:, j], o.fy[:, j]
     ax, bx = fx * A[0] - dx * A[2], fx * B[0] - dx * B[2]
     ay, by = fy * A[1] - dy * A[2], fy * B[1] - dy * B[2]
     s = -((ax * bx + ay * by) / (bx * bx + by * by))
     P = [A[e] + s * B[e] for e in range(3)]
-    ok = (s > 0) & (_dot(B, P) <= cos_min * np.sqrt(_dot(B, B) * _dot(P, P)))
+    ok = (s > 0) & (dot3(B, P) <= cos_min * np.sqrt(dot3(B, B) * dot3(P, P)))
     Ci = o.at("C", i)
     return ok, [Ci[e] + s * r[e] for e in range(3)]
 
@@ -169,12 +153,12 @@ def _line_candidate(o: _Obs, i, j, sin2_min):
     A = o.A(i, j)
     n = o.at("n", j)
     Rj = o.R[:, j]
-    alpha, nn = _dot(n, A), _dot(n, n)
+    alpha, nn = dot3(n, A), dot3(n, n)
     Ci = o.at("C", i)
     ok, X = None, []
     for r in (o.at("r0", i), o.at("r1", i)):
-        B = _mv(Rj, r)
-        beta, BB = _dot(n, B), _dot(B, B)
+        B = mv3(Rj, r)
+        beta, BB = dot3(n, B), dot3(B, B)
         s = -(alpha / beta)
         okr = (s > 0, beta * beta >= sin2_min * (nn * BB))
         ok = okr if ok is None else (ok[0] & okr[0], ok[1] & okr[1])
@@ -192,9 +176,11 @@ def _gn_term(num, den, b, d, h, g, sel):
 
 
 def _pixel_terms(o: _Obs, q, A, px, Y, h, g, sel):
-    R = o.R[:, q]
-    P = [x + A[e] for e, x in enumerate(_mv(R, Y))]
-    fx, fy, cx, cy = o.fx[:, q], o.fy[:, q], o.cx[:, q], o.cy[:, q]
+    """The two pixel residuals of observation column q, or per track of column q[track] (the anchor's)."""
+    col = lambda a: a[np.arange(len(sel)), q]
+    R = col(o.R)
+    P = [x + A[e] for e, x in enumerate(mv3(R, Y))]
+    fx, fy, cx, cy = col(o.fx), col(o.fy), col(o.cx), col(o.cy)
     dx, dy = px[0] - cx, px[1] - cy
     d = [R[:, 6], R[:, 7], R[:, 8]]
     _gn_term(fx * P[0] - dx * P[2], P[2], [fx * R[:, k] - dx * R[:, 6 + k] for k in range(3)], d, h, g, sel)
@@ -204,9 +190,9 @@ def _pixel_terms(o: _Obs, q, A, px, Y, h, g, sel):
 def _line_term(o: _Obs, q, A, Y, h, g, sel):
     R = o.R[:, q]
     n = o.at("n", q)
-    P = [x + A[e] for e, x in enumerate(_mv(R, Y))]
+    P = [x + A[e] for e, x in enumerate(mv3(R, Y))]
     b = [(n[0] * R[:, k] + n[1] * R[:, 3 + k]) + n[2] * R[:, 6 + k] for k in range(3)]
-    _gn_term(_dot(n, P), P[2], b, [R[:, 6], R[:, 7], R[:, 8]], h, g, sel)
+    _gn_term(dot3(n, P), P[2], b, [R[:, 6], R[:, 7], R[:, 8]], h, g, sel)
 
 
 def _solve_step(h, g, Y, active):
@@ -277,8 +263,8 @@ def _estimate(o: _Obs, V, T, lines, t2, cos_min, sin2_min):
     pick = lambda a: np.take_along_axis(a, ai[:, None], 1)[:, 0]
     Ci = [pick(c) for c in o.C]
     Ra, ta = o.R[np.arange(T), ai], [pick(x) for x in o.t]
-    Aa = [x + ta[e] for e, x in enumerate(_mv(Ra, Ci))]
-    Aq = [[x + o.t[e][:, q] for e, x in enumerate(_mv(o.R[:, q], Ci))] for q in range(V)]
+    Aa = [x + ta[e] for e, x in enumerate(mv3(Ra, Ci))]
+    Aq = [[x + o.t[e][:, q] for e, x in enumerate(mv3(o.R[:, q], Ci))] for q in range(V)]
     ends = 2 if lines else 1
     Xr = []
     for e in range(ends):
@@ -289,7 +275,7 @@ def _estimate(o: _Obs, V, T, lines, t2, cos_min, sin2_min):
         for _ in range(TRK_GN_ITERS):
             h, g = [np.zeros(T) for _ in range(6)], [np.zeros(T) for _ in range(3)]
             if lines:
-                _pixel_terms_anchor(o, ai, Ra, Aa, pe, Y, h, g)
+                _pixel_terms(o, ai, Aa, pe, Y, h, g, np.ones(T, bool))
                 for q in range(V):
                     _line_term(o, q, Aq[q], Y, h, g, bits[q] & (ai != q))
             else:
@@ -313,20 +299,6 @@ def _estimate(o: _Obs, V, T, lines, t2, cos_min, sin2_min):
                 support=np.where(have, mask, np.uint64(0)), refit=keep, X=np.stack(Xf, 1), mask=mask_f)
 
 
-def _pixel_terms_anchor(o: _Obs, ai, Ra, Aa, pe, Y, h, g):
-    """The anchor end point's own two pixel residuals (the anchor column differs per track)."""
-    T = len(ai)
-    pick = lambda a: a[np.arange(T), ai]
-    fx, fy, cx, cy = pick(o.fx), pick(o.fy), pick(o.cx), pick(o.cy)
-    R = Ra
-    P = [x + Aa[e] for e, x in enumerate(_mv(R, Y))]
-    dx, dy = pe[0] - cx, pe[1] - cy
-    d = [R[:, 6], R[:, 7], R[:, 8]]
-    sel = np.ones(T, bool)
-    _gn_term(fx * P[0] - dx * P[2], P[2], [fx * R[:, k] - dx * R[:, 6 + k] for k in range(3)], d, h, g, sel)
-    _gn_term(fy * P[1] - dy * P[2], P[2], [fy * R[:, 3 + k] - dy * R[:, 6 + k] for k in range(3)], d, h, g, sel)
-
-
 def _components(n_nodes, u, v):
     """Labels of the connected components of the graph (u, v edges): each component's minimum node."""
     from scipy.sparse import coo_matrix
@@ -348,15 +320,11 @@ def triangulate_tracks_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, 
     row_points3d / row_lines3d, edges_k (per match row), label_k (each row's component: its minimum row), and per track
     the winner (anchor_k / partner_k observation index, winner_k its coordinates, support_k its supporter mask, bit o =
     observation o) and refit_k (the refit was kept); F [P, 3, 3] and offsets_p / offsets_l [n + 1]."""
-    S = _check(keypoints, klines, pairs, res, K, R, t, who=_WHO)
+    S = check_set(keypoints, klines, pairs, res, K, R, t, _WHO)
     _check_params(thresh, min_angle, min_views, epi_thresh, min_overlap)
     n, P = len(keypoints), len(S.pairs)
-    kp_off = np.concatenate([[0], np.cumsum(S.n_kp)]).astype(np.int64)
-    kl_off = np.concatenate([[0], np.cumsum(S.n_kl)]).astype(np.int64)
-    kp = [_host(k, np.float32).reshape(-1, 2) for k in keypoints]
-    kl = [_host(k, np.float32).reshape(-1, 4) for k in klines]
-    kp_pool = (np.concatenate(kp) if n else np.zeros((0, 2), np.float32)).astype(np.float64)
-    kl_pool = (np.concatenate(kl) if n else np.zeros((0, 4), np.float32)).astype(np.float64)
+    kp_off, kl_off = offsets(S.n_kp).astype(np.int64), offsets(S.n_kl).astype(np.int64)
+    kp_pool, kl_pool = pool64(keypoints, 2), pool64(klines, 4)
     F = pair_fundamentals(S) if P else np.zeros((0, 3, 3))
     t2, epi2 = float(thresh) * float(thresh), float(epi_thresh) * float(epi_thresh)
     rad = float(min_angle) * (math.pi / 180.0)
@@ -366,7 +334,7 @@ def triangulate_tracks_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, 
     for kind, off, pool, mt, cu, width in (
             ("p", kp_off, kp_pool, res.matches_p, res.offsets_p, 2), ("l", kl_off, kl_pool, res.matches_l, res.offsets_l, 4)):
         lines = kind == "l"
-        m = _host(mt, np.int64).reshape(-1)
+        m = host(mt, np.int64).reshape(-1)
         cu = np.asarray(cu, dtype=np.int64)
         Nn = int(off[-1])
         edges = np.zeros(len(m), bool)
@@ -438,11 +406,8 @@ def triangulate_tracks_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, 
                     d = [Xb[k] - Xa[k] for k in range(3)]
                     Cq = [c[vq, q] for c in o.C]
                     w = [Xa[k] - Cq[k] for k in range(3)]
-                    for e, ray in enumerate((o.r0, o.r1)):
-                        rr = [x[vq, q] for x in ray]
-                        aa, bb, cc, dd, ee = _dot(d, d), _dot(d, rr), _dot(rr, rr), _dot(d, w), _dot(rr, w)
-                        uu = (bb * ee - cc * dd) / (aa * cc - bb * bb)
-                        row_X[rows, 3 * e:3 * e + 3] = np.stack([Xa[k] + uu * d[k] for k in range(3)], 1)
+                    for e, r_e in enumerate((o.r0, o.r1)):
+                        row_X[rows, 3 * e:3 * e + 3] = np.stack(closest_on_line(Xa, d, w, [x[vq, q] for x in r_e]), 1)
         out.update({f"track_{kind}": track.astype(np.int32), f"n_tracks_{kind}": T,
                     f"track_off_{kind}": track_off.astype(np.int32), f"obs_{kind}": obs.astype(np.int32),
                     f"n_obs_{kind}": n_obs.astype(np.int32), f"n_inliers_{kind}": n_inl,
@@ -518,11 +483,11 @@ def triangulate_tracks(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_a
     call (six kernel launches, no synchronisation).  Arguments as `triangulation.triangulate`; epi_thresh (pixels) and
     min_overlap decide which matches agree with the poses.  Raises LtrError before any device work on the arguments
     `triangulate` refuses, except that an image may take part in any number of pairs."""
-    S = _check(keypoints, klines, pairs, res, K, R, t, who=_WHO)
+    S = check_set(keypoints, klines, pairs, res, K, R, t, _WHO)
     _check_params(thresh, min_angle, min_views, epi_thresh, min_overlap)
     n, P = len(keypoints), len(S.pairs)
     dev = res.matches_p.device
-    op, ol = _offsets(S.n_kp), _offsets(S.n_kl)
+    op, ol = offsets(S.n_kp), offsets(S.n_kl)
     Np, Nl = int(op[-1]), int(ol[-1])
     Tp, Tl = max(Np // 2, 1), max(Nl // 2, 1)
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
@@ -542,18 +507,11 @@ def triangulate_tracks(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_a
         o["track_p"].fill_(-1)
         o["track_l"].fill_(-1)
     else:
-        kpts, segs = _pool_rows(keypoints, 2, dev), _pool_rows(klines, 4, dev)
         arrays = {"K": S.K, "R": S.R, "t": S.t, "F": pair_fundamentals(S).reshape(-1, 9) if P else np.zeros((1, 9)),
                   "pairs": S.pairs.reshape(-1, 2) if P else np.zeros((1, 2), np.int32),
                   "cu_p": np.asarray(res.offsets_p, dtype=np.int32), "cu_l": np.asarray(res.offsets_l, dtype=np.int32),
                   "kp_off": op, "seg_off": ol}
-        for nm, a in (("kpts", kpts), ("segs", segs)):
-            if isinstance(a, np.ndarray):
-                arrays[nm] = a if len(a) else np.zeros((1, a.shape[1]), np.float32)
-        dv = _ops.stage(arrays, dev)
-        for nm, a in (("kpts", kpts), ("segs", segs)):
-            if isinstance(a, torch.Tensor):
-                dv[nm] = a
+        dv = stage_with_pools(arrays, keypoints, klines, dev)
         _ops.tracks(kpts=dv["kpts"], kp_off=dv["kp_off"], segs=dv["segs"], seg_off=dv["seg_off"], K=dv["K"],
                     R=dv["R"], t=dv["t"], F=dv["F"], pairs=dv["pairs"], matches_p=res.matches_p.contiguous(),
                     cu_p=dv["cu_p"], matches_l=res.matches_l.contiguous(), cu_l=dv["cu_l"], n_images=n, n_pairs=P,

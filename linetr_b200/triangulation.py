@@ -30,7 +30,8 @@ import torch
 
 from . import _native as N
 from . import _ops
-from .geometry import _intrinsics
+from ._posed import (PosedSet, centre, check_set, dot3, host, line_normal, mv3, offsets, pool64, ray,
+                     stage_with_pools)
 
 TRI_THREADS = 128          # rows per block of the triangulation kernel
 TRI_GN_ITERS = 5           # Gauss-Newton steps of the refit (fixed budget)
@@ -38,81 +39,12 @@ TRI_MAX_VIEWS = N.TRI_MAX_VIEWS
 
 
 # ------------------------------------------------------------------ arguments
-def _host(a, dtype):
-    return np.asarray(a.cpu() if isinstance(a, torch.Tensor) else a, dtype=dtype)
+def _check(keypoints, klines, pairs, res, K, R, t, who="triangulate") -> PosedSet:
+    """The posed-set checks (`_posed.check_set`) with `triangulate`'s messages unless `who` is given."""
+    return check_set(keypoints, klines, pairs, res, K, R, t, who)
 
 
-@dataclass
-class _Set:
-    pairs: np.ndarray        # int32 [P, 2]
-    K: np.ndarray            # [n, 3, 3]
-    R: np.ndarray            # [n, 3, 3]
-    t: np.ndarray            # [n, 3]
-    n_kp: np.ndarray         # int64 [n]
-    n_kl: np.ndarray         # int64 [n]
-    views: np.ndarray        # int32: image i's observations [view_off[i], view_off[i + 1]), pair << 1 | side
-    view_off: np.ndarray     # int32 [n + 1]
-
-
-def _rows(items, width, what, who="triangulate"):
-    n = []
-    for i, k in enumerate(items):
-        shape = tuple(k.shape) if hasattr(k, "shape") else np.shape(k)
-        m = shape[0] if len(shape) else 0
-        if int(np.prod(shape)) != m * width:
-            raise N.LtrError(f"{who}: {what}[{i}] must hold {width} coordinates per row, got shape {list(shape)}")
-        n.append(m)
-    return np.array(n, dtype=np.int64)
-
-
-def _check(keypoints, klines, pairs, res, K, R, t, who="triangulate") -> _Set:
-    """The argument checks shared by `triangulate` and `tracks.triangulate_tracks` (all on the host, before any device
-    work; messages start with `who`) -> the set's host tables."""
-    n = len(keypoints)
-    if len(klines) != n:
-        raise N.LtrError(f"{who}: {n} keypoint arrays but {len(klines)} key-line arrays")
-    n_kp, n_kl = _rows(keypoints, 2, "keypoints", who), _rows(klines, 4, "klines", who)
-    pr = _host(pairs, np.int64)
-    if pr.size == 0:
-        pr = pr.reshape(0, 2)
-    if pr.ndim != 2 or pr.shape[1] != 2:
-        raise N.LtrError(f"{who}: pairs must be [P, 2], got {list(pr.shape)}")
-    P = len(pr)
-    if P != res.n_pairs:
-        raise N.LtrError(f"{who}: {P} pairs but the matches hold {res.n_pairs}")
-    if P and (pr.min() < 0 or pr.max() >= n):
-        raise N.LtrError(f"{who}: pair indices must lie in [0, {n})")
-    if (pr[:, 0] == pr[:, 1]).any():
-        raise N.LtrError(f"{who}: pair {int(np.flatnonzero(pr[:, 0] == pr[:, 1])[0])} is a self pair")
-    key = np.sort(pr, 1)
-    if len(np.unique(key[:, 0] * max(n, 1) + key[:, 1])) != P:
-        raise N.LtrError(f"{who}: an unordered pair is listed twice")
-    op, ol = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
-    for nm, off, cnt0, side1, cnt1 in (("keypoint", op, n_kp, res.keypoints1, n_kp), ("key-line", ol, n_kl, res.klines1, n_kl)):
-        bad = np.flatnonzero(np.diff(off) != cnt0[pr[:, 0]])
-        if len(bad):
-            raise N.LtrError(f"{who}: pair {int(bad[0])} has {int(np.diff(off)[bad[0]])} {nm} match rows for "
-                             f"{int(cnt0[pr[bad[0], 0]])} {nm}s of image {int(pr[bad[0], 0])}")
-        for p in range(P):
-            if len(side1[p]) != cnt1[pr[p, 1]]:
-                raise N.LtrError(f"{who}: side 1 of pair {p} has {len(side1[p])} {nm}s, image {int(pr[p, 1])} "
-                                 f"{int(cnt1[pr[p, 1]])}")
-    Kn = _intrinsics(K, n, "K")
-    Rn, tn = _host(R, np.float64), _host(t, np.float64)
-    if Rn.shape != (n, 3, 3) or tn.shape != (n, 3):
-        raise N.LtrError(f"{who}: R must be [{n}, 3, 3] and t [{n}, 3], got {list(Rn.shape)} and {list(tn.shape)}")
-    if not (np.isfinite(Rn).all() and np.isfinite(tn).all()):
-        raise N.LtrError(f"{who}: R and t must be finite")
-    img = np.concatenate([pr[:, 0], pr[:, 1]])
-    code = np.concatenate([2 * np.arange(P), 2 * np.arange(P) + 1])
-    order = np.lexsort((code, img))
-    cnt = np.bincount(img, minlength=n)
-    view_off = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int32)
-    return _Set(pr.astype(np.int32), Kn, np.ascontiguousarray(Rn), np.ascontiguousarray(tn), n_kp, n_kl,
-                code[order].astype(np.int32), view_off)
-
-
-def _check_views(S: _Set):
+def _check_views(S: PosedSet):
     """`triangulate`'s capacity: at most LTR_TRI_MAX_VIEWS pairs per image (tracks have no such limit)."""
     cnt = np.diff(S.view_off)
     if len(cnt) and cnt.max(initial=0) > TRI_MAX_VIEWS:
@@ -122,37 +54,20 @@ def _check_views(S: _Set):
 
 
 # ------------------------------------------------------------------ the model in numpy
-def _dot(a, b):
-    return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]
-
-
-def _mv(M, v):
-    return [(M[i, 0] * v[0] + M[i, 1] * v[1]) + M[i, 2] * v[2] for i in range(3)]
-
-
-def _centre(R, t):
-    return [-((R[0, j] * t[0] + R[1, j] * t[1]) + R[2, j] * t[2]) for j in range(3)]
-
-
-def _ray(R, K, x, y):
-    nx, ny = (x - K[0, 2]) / K[0, 0], (y - K[1, 2]) / K[1, 1]
-    return [(R[0, k] * nx + R[1, k] * ny) + R[2, k] for k in range(3)]
-
-
-def _cameras(S: _Set, a):
+def _cameras(S: PosedSet, a):
     """The anchor a's centre and, per observation, (fx, fy, cx, cy, R_v, A = R_v C_a + t_v, pair, side, partner)."""
-    C = _centre(S.R[a], S.t[a])
+    C = centre(S.R[a].reshape(9), S.t[a])
     out = []
     for code in S.views[S.view_off[a]:S.view_off[a + 1]]:
         p, side = int(code) >> 1, int(code) & 1
         v = int(S.pairs[p, 1 - side])
-        Rv = S.R[v]
-        A = [x + S.t[v, i] for i, x in enumerate(_mv(Rv, C))]
+        Rv = S.R[v].reshape(9)
+        A = [x + S.t[v, i] for i, x in enumerate(mv3(Rv, C))]
         out.append((S.K[v, 0, 0], S.K[v, 1, 1], S.K[v, 0, 2], S.K[v, 1, 2], Rv, A, p, side, v))
     return C, out
 
 
-def _partner_rows(S: _Set, matches, cu, counts, a, cams):
+def _partner_rows(S: PosedSet, matches, cu, counts, a, cams):
     """Per observation of anchor a: its partner row for each of a's rows, or -1."""
     na = int(counts[a])
     out = []
@@ -178,7 +93,7 @@ def _gather(pool, off, v, j, width):
 
 def _point_terms(cam, r, px):
     fx, fy, cx, cy, Rv, A = cam[:6]
-    B = _mv(Rv, r)
+    B = mv3(Rv, r)
     dx, dy = px[:, 0] - cx, px[:, 1] - cy
     return dict(ax=fx * A[0] - dx * A[2], bx=fx * B[0] - dx * B[2], ay=fy * A[1] - dy * A[2], by=fy * B[1] - dy * B[2],
                 g=A[2], d=B[2], B=B, A=A)
@@ -190,18 +105,9 @@ def _point_support(o, s, t2):
     return (pz > 0) & ((ex * ex + ey * ey) <= t2 * (pz * pz))
 
 
-def _line_normal(cam, seg):
-    fx, fy, cx, cy = cam[:4]
-    x0, y0, x1, y1 = seg[:, 0], seg[:, 1], seg[:, 2], seg[:, 3]
-    a, b, c = y0 - y1, x1 - x0, x0 * y1 - x1 * y0
-    rn = 1.0 / np.sqrt(a * a + b * b)
-    la, lb, lc = a * rn, b * rn, c * rn
-    return [la * fx, lb * fy, (la * cx + lb * cy) + lc]
-
-
 def _end_terms(cam, n, r):
-    B = _mv(cam[4], r)
-    return dict(alpha=_dot(n, cam[5]), beta=_dot(n, B), g=cam[5][2], d=B[2], BB=_dot(B, B))
+    B = mv3(cam[4], r)
+    return dict(alpha=dot3(n, cam[5]), beta=dot3(n, B), g=cam[5][2], d=B[2], BB=dot3(B, B))
 
 
 def _end_support(e, s, t2):
@@ -262,13 +168,9 @@ def triangulate_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_ang
     if not (float(thresh) > 0 and math.isfinite(float(thresh))) or not (0 <= float(min_angle) < 90) or int(min_views) < 1:
         raise N.LtrError("triangulate: thresh must be finite and > 0, min_angle in [0, 90) and min_views >= 1")
     n = len(keypoints)
-    kp = [_host(k, np.float32).reshape(-1, 2).astype(np.float64) for k in keypoints]
-    kl = [_host(k, np.float32).reshape(-1, 4).astype(np.float64) for k in klines]
-    kp_off = np.concatenate([[0], np.cumsum(S.n_kp)]).astype(np.int64)
-    kl_off = np.concatenate([[0], np.cumsum(S.n_kl)]).astype(np.int64)
-    kp_pool = np.concatenate(kp) if n else np.zeros((0, 2))
-    kl_pool = np.concatenate(kl) if n else np.zeros((0, 4))
-    mp, ml = _host(res.matches_p, np.int64).reshape(-1), _host(res.matches_l, np.int64).reshape(-1)
+    kp_off, kl_off = offsets(S.n_kp).astype(np.int64), offsets(S.n_kl).astype(np.int64)
+    kp_pool, kl_pool = pool64(keypoints, 2), pool64(klines, 4)
+    mp, ml = host(res.matches_p, np.int64).reshape(-1), host(res.matches_l, np.int64).reshape(-1)
     cu_p, cu_l = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
     t2 = float(thresh) * float(thresh)
     rad = float(min_angle) * (math.pi / 180.0)
@@ -287,7 +189,9 @@ def triangulate_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_ang
             # points
             rows = int(S.n_kp[a])
             if rows:
-                r = _ray(S.R[a], S.K[a], kp[a][:, 0], kp[a][:, 1])
+                Ra, fx, fy, cx, cy = S.R[a].reshape(9), S.K[a, 0, 0], S.K[a, 1, 1], S.K[a, 0, 2], S.K[a, 1, 2]
+                kp = kp_pool[kp_off[a]:kp_off[a + 1]]
+                r = ray(Ra, fx, fy, cx, cy, kp[:, 0], kp[:, 1])
                 js = _partner_rows(S, mp, cu_p, S.n_kp, a, cams)
                 T = [_point_terms(c, r, _gather(kp_pool, kp_off, c[8], j, 2)) for c, j in zip(cams, js)]
 
@@ -295,7 +199,7 @@ def triangulate_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_ang
                     o_ = T[o]
                     s = -((o_["ax"] * o_["bx"] + o_["ay"] * o_["by"]) / (o_["bx"] * o_["bx"] + o_["by"] * o_["by"]))
                     P = [A + s * B for A, B in zip(o_["A"], o_["B"])]
-                    ang = _dot(o_["B"], P) <= cmin * np.sqrt(_dot(o_["B"], o_["B"]) * _dot(P, P))
+                    ang = dot3(o_["B"], P) <= cmin * np.sqrt(dot3(o_["B"], o_["B"]) * dot3(P, P))
                     return (s > 0) & ang, [s]
 
                 best, win, mask = _select(cand, lambda s: [_point_support(o_, s[0], t2) for o_ in T], V, rows)
@@ -319,13 +223,15 @@ def triangulate_host(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_ang
             # key lines
             rows = int(S.n_kl[a])
             if rows:
-                r0 = _ray(S.R[a], S.K[a], kl[a][:, 0], kl[a][:, 1])
-                r1 = _ray(S.R[a], S.K[a], kl[a][:, 2], kl[a][:, 3])
+                Ra, fx, fy, cx, cy = S.R[a].reshape(9), S.K[a, 0, 0], S.K[a, 1, 1], S.K[a, 0, 2], S.K[a, 1, 2]
+                kl = kl_pool[kl_off[a]:kl_off[a + 1]]
+                r0 = ray(Ra, fx, fy, cx, cy, kl[:, 0], kl[:, 1])
+                r1 = ray(Ra, fx, fy, cx, cy, kl[:, 2], kl[:, 3])
                 js = _partner_rows(S, ml, cu_l, S.n_kl, a, cams)
                 T = []
                 for c, j in zip(cams, js):
-                    nrm = _line_normal(c, _gather(kl_pool, kl_off, c[8], j, 4))
-                    T.append((_end_terms(c, nrm, r0), _end_terms(c, nrm, r1), _dot(nrm, nrm)))
+                    nrm = line_normal(*c[:4], _gather(kl_pool, kl_off, c[8], j, 4))
+                    T.append((_end_terms(c, nrm, r0), _end_terms(c, nrm, r1), dot3(nrm, nrm)))
 
                 def cand(o):
                     e0, e1, nn = T[o]
@@ -381,19 +287,6 @@ class TriangulationResult:
         return ([P[op[i]:op[i + 1]] for i in range(len(op) - 1)], [L[ol[i]:ol[i + 1]] for i in range(len(ol) - 1)])
 
 
-def _pool_rows(items, width, dev):
-    """The images' rows back to back as float32 [*, width]: one device concatenation when every item is a CUDA
-    tensor, else a host array for the staging copy."""
-    if items and all(isinstance(k, torch.Tensor) and k.is_cuda for k in items):
-        return torch.cat([k.to(device=dev, dtype=torch.float32).reshape(-1, width) for k in items]).contiguous()
-    parts = [_host(k, np.float32).reshape(-1, width) for k in items]
-    return np.concatenate(parts) if parts else np.zeros((0, width), np.float32)
-
-
-def _offsets(counts):
-    return np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
-
-
 def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.5, min_views=2) -> TriangulationResult:
     """World points of every keypoint and world end points of every key line of n posed images, from the matches `res`
     (an `ImagePairMatches`, as `match_set(images, pairs)` returns) of the host pair list pairs [P, 2], in one
@@ -407,7 +300,7 @@ def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.
     _check_views(S)
     n, P = len(keypoints), len(S.pairs)
     dev = res.matches_p.device
-    op, ol = _offsets(S.n_kp), _offsets(S.n_kl)
+    op, ol = offsets(S.n_kp), offsets(S.n_kl)
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
     out = TriangulationResult(torch.empty((int(op[-1]), 3), **f64), torch.empty((int(ol[-1]), 2, 3), **f64),
                               torch.empty(int(op[-1]), **i32), torch.empty(int(ol[-1]), **i32),
@@ -415,21 +308,14 @@ def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.
     if n == 0:
         return out
     blocks = np.concatenate([(S.n_kp + TRI_THREADS - 1) // TRI_THREADS, (S.n_kl + TRI_THREADS - 1) // TRI_THREADS])
-    block_off = _offsets(blocks)
-    inv_off_p = _offsets(S.n_kp[S.pairs[:, 1]] if P else [])
-    inv_off_l = _offsets(S.n_kl[S.pairs[:, 1]] if P else [])
-    kpts, segs = _pool_rows(keypoints, 2, dev), _pool_rows(klines, 4, dev)
+    block_off = offsets(blocks)
+    inv_off_p = offsets(S.n_kp[S.pairs[:, 1]] if P else [])
+    inv_off_l = offsets(S.n_kl[S.pairs[:, 1]] if P else [])
     arrays = {"K": S.K, "R": S.R, "t": S.t, "pairs": S.pairs.reshape(-1, 2),
               "cu_p": np.asarray(res.offsets_p, dtype=np.int32), "cu_l": np.asarray(res.offsets_l, dtype=np.int32),
               "views": S.views, "view_off": S.view_off, "block_off": block_off, "inv_off_p": inv_off_p,
               "inv_off_l": inv_off_l, "kp_off": op, "seg_off": ol}
-    for nm, a in (("kpts", kpts), ("segs", segs)):
-        if isinstance(a, np.ndarray):
-            arrays[nm] = a
-    dv = _ops.stage(arrays, dev)
-    for nm, a in (("kpts", kpts), ("segs", segs)):
-        if isinstance(a, torch.Tensor):
-            dv[nm] = a
+    dv = stage_with_pools(arrays, keypoints, klines, dev)
     inv_p = torch.empty(max(int(inv_off_p[-1]), 1), **i32)
     inv_l = torch.empty(max(int(inv_off_l[-1]), 1), **i32)
     _ops.triangulate(kpts=dv["kpts"], kp_off=dv["kp_off"], segs=dv["segs"], seg_off=dv["seg_off"], K=dv["K"],
