@@ -982,6 +982,80 @@ typedef struct {
  * them; each returns at once after the stop) and one for the outputs. */
 int ltr_bundle_adjust(const LtrBundleInput* in, const LtrBundleOutput* out, int32_t device, void* stream);
 
+/* Global poses of an unposed image set from the relative poses of its pairs (rotation averaging, then BATA camera
+ * positions); DESIGN.md "Global poses" states the model:
+ *   - view graph: pair p is usable iff valid[p] and n_cheirality[p] >= min_inliers; the component of usable pairs with
+ *     the most images (ties: the one holding the lowest image) is registered and anchor < 0 picks its lowest image;
+ *     an anchor >= 0 registers its own component instead (the largest one when the caller checked it);
+ *   - loop support of a usable pair (i, j): the third images k whose triangle |cayinv(R_ij^T R_kj R_ik)| <= rot_tan
+ *     through usable pairs (cayinv(Q) = vee(Q - Q^T) / (1 + tr Q), |cayinv| = tan(theta / 2));
+ *   - rotations: Prim's maximum spanning tree from the anchor on (support, n_cheirality, -p), chained, then IRLS on
+ *     cayinv(R_j^T R_p R_i) with R_k <- R_k cay(w_k): LTR_GP_L1_ITERS L1 iterations, then Geman-McClure ones (scale
+ *     LTR_GP_SIGMA_ROT) while the cost falls, up to rot_iters; a pair is a rotation outlier iff |cayinv| > rot_tan;
+ *   - rigidity: images with fewer than two rotation-inlier pairs to kept images, or whose directions are all within
+ *     LTR_GP_MIN_ANGLE of parallel, are dropped until none is (not the anchor, not below three images); the images
+ *     still connected to the anchor are registered;
+ *   - positions (BATA): C_anchor = 0, sum_p <dC_p, v_p> = E (v_p = -R_j^T t_p, E the pairs used), alternating C, the
+ *     scales and Geman-McClure weights (scale LTR_GP_SIGMA_POS) up to pos_iters; a pair is a direction outlier iff not
+ *     <dC_p, v_p> > dir_cos |dC_p|; t_k = -R_k C_k.
+ * Both stages stop after an accepted step whose relative cost decrease is <= ftol.  Every operation is explicitly
+ * rounded fp64 in a fixed order, so two calls give the same bits. */
+#define LTR_GP_MAX_IMAGES 128
+#define LTR_GP_MAX_ITERS 100000
+#define LTR_GP_L1_ITERS 5
+#define LTR_GP_L1_EPS 1e-9
+#define LTR_GP_SIGMA_ROT 0.04366094290851206   /* tan(2.5 deg) */
+#define LTR_GP_SIGMA_POS 0.1
+#define LTR_GP_MIN_ANGLE 2                      /* degrees; the kernels compare against sin(2 deg) */
+#define LTR_GP_EDGE_UNUSED 0                    /* not usable */
+#define LTR_GP_EDGE_OUTSIDE 1                   /* usable, but an image is not registered */
+#define LTR_GP_EDGE_ROT_OUTLIER 2
+#define LTR_GP_EDGE_DIR_OUTLIER 3
+#define LTR_GP_EDGE_INLIER 4
+#define LTR_GP_STATS 7
+typedef struct {
+  const int32_t* pairs;           /* device [n_pairs, 2]: image i side 0, image j side 1; no self or repeated pair */
+  const double* R;                /* device [n_pairs, 3, 3]: X_j = R_p X_i + t_p (ltr_essential) */
+  const double* t;                /* device [n_pairs, 3] unit */
+  const uint8_t* valid;           /* device [n_pairs] */
+  const int32_t* n_cheirality;    /* device [n_pairs] */
+  int32_t n_images;               /* in [1, LTR_GP_MAX_IMAGES] */
+  int32_t n_pairs;                /* >= 0 */
+  int32_t min_inliers;            /* (20) */
+  int32_t anchor;                 /* < 0: the largest component's lowest image; else its own component is registered */
+  int32_t rot_iters;              /* in [0, LTR_GP_MAX_ITERS] (100) */
+  int32_t pos_iters;              /* in [0, LTR_GP_MAX_ITERS] (500) */
+  double rot_tan;                 /* tan(rot_thresh / 2), finite > 0 */
+  double dir_cos;                 /* cos(dir_thresh), finite */
+  double ftol;                    /* finite, >= 0 (1e-12) */
+} LtrGlobalPoseInput;
+
+/* Outputs (device, caller-owned).  R [n_images, 3, 3] and t [n_images, 3] world -> camera, NaN for an image not
+ * registered, exactly I and 0 for the anchor; registered uint8 [n_images]; per pair: edge_status int32 (LTR_GP_EDGE_*),
+ * support int32 (-1 for a pair not usable), rot_residual fp64 (the final |cayinv(R_j^T R_p R_i)| of the registered
+ * component's pairs, NaN elsewhere), dir_cos fp64 (<dC_p, v_p> / |dC_p| of the pairs of the position solve, NaN
+ * elsewhere); stats fp64 [LTR_GP_STATS]: rotation iterations and final cost, position iterations and final cost,
+ * images registered, inlier pairs, anchor.  workspace: LTR_GP_WORKSPACE_BYTES(n_images, n_pairs) bytes, 8-byte
+ * aligned. */
+#define LTR_GP_WORKSPACE_BYTES(n, n_pairs) \
+  (8 * (16 * (int64_t)(n_pairs) + 24 * (int64_t)(n)) + 4 * (2 * (int64_t)(n) * (n) + 8 * (int64_t)(n) + 16))
+typedef struct {
+  double* R;
+  double* t;
+  uint8_t* registered;
+  int32_t* edge_status;
+  int32_t* support;
+  double* rot_residual;
+  double* dir_cos;
+  double* stats;
+  void* workspace;
+} LtrGlobalPoseOutput;
+
+/* Asynchronous on `stream`; never synchronises.  Errors come before any launch: LTR_E_INVALID for bad arguments,
+ * LTR_E_UNSUPPORTED for more than LTR_GP_MAX_IMAGES images.  Three launches: the view graph (one CTA), the loop support
+ * (one CTA per pair) and one persistent CTA for the tree, both iterative stages and the outputs. */
+int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* out, int32_t device, void* stream);
+
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where
  * the warped colour image is 0 in every channel, eroded with a 5 x 5 kernel of ones.

@@ -80,6 +80,9 @@ _LAZY = {
     "TrackResult": ("tracks", "TrackResult"),
     "bundle_adjust": ("bundle", "bundle_adjust"),
     "BundleResult": ("bundle", "BundleResult"),
+    "global_poses": ("global_poses", "global_poses"),
+    "GlobalPoseResult": ("global_poses", "GlobalPoseResult"),
+    "registered_set": ("global_poses", "registered_set"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

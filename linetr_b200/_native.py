@@ -31,12 +31,21 @@ BA_MAX_ITERS = 1000          # LTR_BA_MAX_ITERS
 BA_IN, BA_NOT_VALID, BA_SAME_IMAGE, BA_DEGENERATE = 0, 1, 2, 3     # LTR_BA_IN .. LTR_BA_DEGENERATE
 BA_STOP_ITERS, BA_STOP_FTOL, BA_STOP_LAMBDA = 0, 1, 2              # LTR_BA_STOP_ITERS .. LTR_BA_STOP_LAMBDA
 BA_STATS = 8                 # LTR_BA_STATS
+GP_MAX_IMAGES = 128          # LTR_GP_MAX_IMAGES
+GP_EDGE_UNUSED, GP_EDGE_OUTSIDE, GP_EDGE_ROT_OUTLIER, GP_EDGE_DIR_OUTLIER, GP_EDGE_INLIER = 0, 1, 2, 3, 4   # LTR_GP_EDGE_*
+GP_STATS = 7                 # LTR_GP_STATS
 
 
 def ba_workspace_bytes(n_images, n_kp, n_kl, t_p, t_l) -> int:
     """LTR_BA_WORKSPACE_BYTES(n_images, n_kp, n_kl, t_p, t_l)."""
     n, rows, trk = int(n_images), int(n_kp) + int(n_kl), int(t_p) + int(t_l)
     return 8 * (64 * rows + 40 * trk + 36 * n * n + 60 * n + 16) + 4 * (2 * rows + 4 * trk + 7 * n + 24) + n
+
+
+def gp_workspace_bytes(n_images, n_pairs) -> int:
+    """LTR_GP_WORKSPACE_BYTES(n_images, n_pairs)."""
+    n, P = int(n_images), int(n_pairs)
+    return 8 * (16 * P + 24 * n) + 4 * (2 * n * n + 8 * n + 16)
 
 
 def photometric_workspace_bytes(n, h, w) -> int:
@@ -243,6 +252,17 @@ class LtrBundleOutput(C.Structure):
         "row_lines3d", "n_views_p", "n_views_l", "stats", "workspace")]
 
 
+class LtrGlobalPoseInput(C.Structure):
+    _fields_ = [(nm, C.c_void_p) for nm in ("pairs", "R", "t", "valid", "n_cheirality")] + [
+        (nm, C.c_int32) for nm in ("n_images", "n_pairs", "min_inliers", "anchor", "rot_iters", "pos_iters")] + [
+        (nm, C.c_double) for nm in ("rot_tan", "dir_cos", "ftol")]
+
+
+class LtrGlobalPoseOutput(C.Structure):
+    _fields_ = [(nm, C.c_void_p) for nm in (
+        "R", "t", "registered", "edge_status", "support", "rot_residual", "dir_cos", "stats", "workspace")]
+
+
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
 # {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
 # of them, and each entry against its C prototype)
@@ -273,6 +293,7 @@ PROTOTYPES = {
     "ltr_triangulate": (C.c_int, [_ptr(LtrTriangulateInput), _ptr(LtrTriangulateOutput), _I32, _P]),
     "ltr_tracks": (C.c_int, [_ptr(LtrTracksInput), _ptr(LtrTracksOutput), _I32, _P]),
     "ltr_bundle_adjust": (C.c_int, [_ptr(LtrBundleInput), _ptr(LtrBundleOutput), _I32, _P]),
+    "ltr_global_poses": (C.c_int, [_ptr(LtrGlobalPoseInput), _ptr(LtrGlobalPoseOutput), _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),

@@ -69,12 +69,12 @@ def _check_tensors(who: str, dev, specs):
 
 _staging = []   # (pinned host buffer, event behind its copy) until the copy has finished
 _TORCH_DTYPE = {np.dtype(np.float64): torch.float64, np.dtype(np.float32): torch.float32,
-                np.dtype(np.int32): torch.int32}
+                np.dtype(np.int32): torch.int32, np.dtype(np.uint8): torch.uint8}
 
 
 def stage(arrays: dict, device) -> dict:
     """One pinned staging buffer, one non-blocking H2D copy on the current stream of `device`: -> device views of the
-    host arrays (float64, float32 or int32).  The buffer is held (with an event behind the copy) until the copy has
+    host arrays (float64, float32, int32 or uint8).  The buffer is held (with an event behind the copy) until the copy has
     finished, so it is never reused early."""
     global _staging
     _staging = [(b, e) for b, e in _staging if not e.query()]
@@ -639,6 +639,30 @@ def bundle_adjust(*, inputs: dict, outputs: dict, n_images, n_fixed, n_kp, n_kl,
                   max_iters=int(max_iters), ftol=float(ftol))
     out = _struct(N.LtrBundleOutput, **{nm: outputs[nm] for nm, _ in _BUNDLE_OUTPUTS})
     _call("ltr_bundle_adjust", dev, C.byref(inp), C.byref(out))
+
+
+_GP_INPUTS = (("pairs", torch.int32), ("R", torch.float64), ("t", torch.float64), ("valid", torch.uint8),
+              ("n_cheirality", torch.int32))
+_GP_OUTPUTS = (("R", torch.float64), ("t", torch.float64), ("registered", torch.bool), ("edge_status", torch.int32),
+               ("support", torch.int32), ("rot_residual", torch.float64), ("dir_cos", torch.float64),
+               ("stats", torch.float64), ("workspace", torch.float64))
+
+
+def global_poses(*, inputs: dict, outputs: dict, n_images, n_pairs, min_inliers, anchor, rot_iters, pos_iters, rot_tan,
+                 dir_cos, ftol):
+    """ltr_global_poses into caller-allocated outputs: inputs {name: tensor} holds every LtrGlobalPoseInput pointer
+    field, outputs every LtrGlobalPoseOutput field (an fp64 workspace of at least LTR_GP_WORKSPACE_BYTES)."""
+    dev = outputs["workspace"].device
+    _req_cuda(outputs["workspace"], "workspace")
+    _check_tensors("global_poses", dev, tuple((nm, inputs[nm], dt) for nm, dt in _GP_INPUTS)
+                   + tuple((nm, outputs[nm], dt) for nm, dt in _GP_OUTPUTS))
+    if outputs["workspace"].numel() * 8 < N.gp_workspace_bytes(n_images, n_pairs):
+        raise N.LtrError("global_poses: the workspace is smaller than LTR_GP_WORKSPACE_BYTES")
+    inp = _struct(N.LtrGlobalPoseInput, **{nm: inputs[nm] for nm, _ in _GP_INPUTS}, n_images=int(n_images),
+                  n_pairs=int(n_pairs), min_inliers=int(min_inliers), anchor=int(anchor), rot_iters=int(rot_iters),
+                  pos_iters=int(pos_iters), rot_tan=float(rot_tan), dir_cos=float(dir_cos), ftol=float(ftol))
+    out = _struct(N.LtrGlobalPoseOutput, **{nm: outputs[nm] for nm, _ in _GP_OUTPUTS})
+    _call("ltr_global_poses", dev, C.byref(inp), C.byref(out))
 
 
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):

@@ -92,6 +92,29 @@ def block_sum(terms, nt):
     return out
 
 
+def cholesky_solve(A, x) -> bool:
+    """The dense solver of rn_fp64.cuh rc_cholesky_solve: a right-looking Cholesky of the m x m matrix A (its lower
+    triangle read, L written over it), then the forward and back substitutions of the right-hand sides x [m] or
+    [m, k], in place.  -> False (x untouched) at the first pivot that is not > 0."""
+    m = len(A)
+    if m == 0:
+        return True
+    for c in range(m):
+        if not A[c, c] > 0:
+            return False
+        A[c, c] = np.sqrt(A[c, c])
+        A[c + 1:, c] = A[c + 1:, c] / A[c, c]
+        A[c + 1:, c + 1:] = A[c + 1:, c + 1:] - np.outer(A[c + 1:, c], A[c + 1:, c])
+    xs = x.reshape(m, -1)
+    for c in range(m):
+        xs[c] = xs[c] / A[c, c]
+        xs[c + 1:] = xs[c + 1:] - A[c + 1:, c, None] * xs[c]
+    for c in range(m - 1, -1, -1):
+        xs[c] = xs[c] / A[c, c]
+        xs[:c] = xs[:c] - A[c, :c, None] * xs[c]
+    return True
+
+
 # ------------------------------------------------------------------ arguments
 def host(a, dtype):
     return np.asarray(a.cpu() if isinstance(a, torch.Tensor) else a, dtype=dtype)

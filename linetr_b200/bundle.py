@@ -30,8 +30,8 @@ import torch
 
 from . import _native as N
 from . import _ops
-from ._posed import (block_sum, cayley, centre, check_poses, closest_on_line, cross3, dot3, line_normal, offsets,
-                     pool64, ray, row_counts, stage_with_pools)
+from ._posed import (block_sum, cayley, centre, check_poses, cholesky_solve, closest_on_line, cross3, dot3,
+                     line_normal, offsets, pool64, ray, row_counts, stage_with_pools)
 from .triangulation import TriangulationResult
 
 BA_MAX_IMAGES, BA_MAX_ITERS = N.BA_MAX_IMAGES, N.BA_MAX_ITERS
@@ -419,24 +419,12 @@ def bundle_adjust_host(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters
                 for a in range(6):
                     if col[i, a] >= 0:
                         rhs[col[i, a]] = -gs[i, a]
-            # dense right-looking Cholesky and the two triangular solves (skipped, with a zero camera step, once a
-            # landmark factorization has failed: the step is rejected either way)
-            for c in (range(m) if ok else ()):
-                if not A[c, c] > 0:
-                    ok = False
-                    break
-                A[c, c] = np.sqrt(A[c, c])
-                A[c + 1:, c] = A[c + 1:, c] / A[c, c]
-                A[c + 1:, c + 1:] = A[c + 1:, c + 1:] - np.outer(A[c + 1:, c], A[c + 1:, c])
-            x = np.zeros(m)
-            if ok:
-                x = rhs.copy()
-                for c in range(m):
-                    x[c] = x[c] / A[c, c]
-                    x[c + 1:] = x[c + 1:] - A[c + 1:, c] * x[c]
-                for c in range(m - 1, -1, -1):
-                    x[c] = x[c] / A[c, c]
-                    x[:c] = x[:c] - A[c, :c] * x[c]
+            # the dense solver (skipped, with a zero camera step, once a landmark factorization has failed: the step is
+            # rejected either way)
+            x = rhs.copy()
+            ok = ok and cholesky_solve(A, x)
+            if not ok:
+                x = np.zeros(m)
             dcam = np.zeros((n, 6))
             for i in range(n):
                 for a in range(6):

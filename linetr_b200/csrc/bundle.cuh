@@ -492,56 +492,13 @@ __global__ void __launch_bounds__(BA_CTA_THREADS) ba_solve_kernel(const BaArgs a
   pdl_launch_dependents();
   pdl_wait();
   if (ba_stopped(a)) return;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, m = a.si[BA_I_M], ld = 6 * a.n_images;
-  double* A = a.A;
+  const int tid = threadIdx.x, m = a.si[BA_I_M];
   double* x = a.rhs;
   // a failed landmark factorization already rejects the step: the camera step is then zero, as on the host
   if (tid == 0) s_fail = a.si[BA_I_FAIL] != 0;
   __syncthreads();
-  // right-looking Cholesky: column c, then every later lower element once, in column order
-  for (int c = 0; c < m && !s_fail; ++c) {
-    const double piv = A[(size_t)ld * c + c];
-    if (!(piv > 0.0)) {
-      __syncthreads();
-      if (tid == 0) s_fail = 1;
-      break;
-    }
-    const double l = __dsqrt_rn(piv);
-    if (tid == 0) A[(size_t)ld * c + c] = l;
-    for (int i = c + 1 + tid; i < m; i += BA_CTA_THREADS) {
-      const double v = RC_D(A[(size_t)ld * i + c], l);
-      A[(size_t)ld * i + c] = v;
-      s_col[i] = v;
-    }
-    __syncthreads();
-    // one warp per row of the trailing block, lanes over its columns c < j <= i
-    for (int i = c + 1 + wid; i < m; i += BA_CTA_THREADS / 32) {
-      const double li = s_col[i];
-      double* Ai = A + (size_t)ld * i;
-      for (int j = c + 1 + lane; j <= i; j += 32) Ai[j] = RC_S(Ai[j], RC_M(li, s_col[j]));
-    }
-    __syncthreads();
-  }
-  __syncthreads();
-  const bool fail = s_fail != 0;
-  if (!fail) {
-    for (int c = 0; c < m; ++c) {
-      if (tid == 0) x[c] = RC_D(x[c], A[(size_t)ld * c + c]);
-      __syncthreads();
-      const double xc = x[c];
-      for (int i = c + 1 + tid; i < m; i += BA_CTA_THREADS) x[i] = RC_S(x[i], RC_M(A[(size_t)ld * i + c], xc));
-      __syncthreads();
-    }
-    for (int c = m - 1; c >= 0; --c) {
-      if (tid == 0) x[c] = RC_D(x[c], A[(size_t)ld * c + c]);
-      __syncthreads();
-      const double xc = x[c];
-      for (int i = tid; i < c; i += BA_CTA_THREADS) x[i] = RC_S(x[i], RC_M(A[(size_t)ld * c + i], xc));
-      __syncthreads();
-    }
-  } else if (tid == 0) {
-    atomicExch(a.si + BA_I_FAIL, 1);
-  }
+  const bool fail = rc_cholesky_solve<BA_CTA_THREADS>(a.A, 6 * a.n_images, m, x, 1, s_col, &s_fail);
+  if (fail && tid == 0) atomicExch(a.si + BA_I_FAIL, 1);
   // candidate cameras
   if (tid < a.n_images) {
     double* cm = a.cam + (size_t)BA_CAM * tid;

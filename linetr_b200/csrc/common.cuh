@@ -50,6 +50,7 @@ enum KernelClass : int {
   KC_TRIANGULATE,
   KC_TRACKS,
   KC_BUNDLE,
+  KC_GLOBAL_POSES,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

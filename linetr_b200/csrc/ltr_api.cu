@@ -28,6 +28,7 @@
 #include "triangulation.cuh"
 #include "tracks.cuh"
 #include "bundle.cuh"
+#include "global_poses.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -49,7 +50,7 @@ const char* kernel_class_name(int kc) {
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
                                          "fundamental", "absolute_pose", "triangulate", "tracks",
-                                         "bundle"};
+                                         "bundle", "global_poses"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1576,6 +1577,58 @@ int ltr_bundle_adjust(const LtrBundleInput* in, const LtrBundleOutput* out, int3
   }
   const dim3 fg(std::max(1, std::min(cdiv(std::max(rows, trk), BA_THREADS), 4 * sms)));
   LTR_CUDA_TRY(launch_pdl(ba_finish_kernel, fg, tb, 0, s, a));
+  return LTR_OK;
+}
+
+int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_global_poses: null argument");
+  if (in->n_images < 1 || in->n_pairs < 0)
+    return set_error(LTR_E_INVALID, "ltr_global_poses: n_images must be >= 1 and n_pairs >= 0");
+  if (in->n_images > LTR_GP_MAX_IMAGES)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_global_poses: more than LTR_GP_MAX_IMAGES images");
+  if ((long long)in->n_pairs > (long long)in->n_images * (in->n_images - 1) / 2)
+    return set_error(LTR_E_INVALID, "ltr_global_poses: more pairs than distinct image pairs");
+  if (in->anchor >= in->n_images)
+    return set_error(LTR_E_INVALID, "ltr_global_poses: anchor out of range");
+  if (in->rot_iters < 0 || in->rot_iters > LTR_GP_MAX_ITERS || in->pos_iters < 0 || in->pos_iters > LTR_GP_MAX_ITERS)
+    return set_error(LTR_E_INVALID, "ltr_global_poses: iteration counts must lie in [0, LTR_GP_MAX_ITERS]");
+  if (!std::isfinite(in->rot_tan) || !(in->rot_tan > 0.0) || !std::isfinite(in->dir_cos) || !std::isfinite(in->ftol) ||
+      !(in->ftol >= 0.0))
+    return set_error(LTR_E_INVALID, "ltr_global_poses: rot_tan must be finite > 0, dir_cos finite, ftol finite >= 0");
+  if (in->n_pairs && (!in->pairs || !in->R || !in->t || !in->valid || !in->n_cheirality))
+    return set_error(LTR_E_INVALID, "ltr_global_poses: null input");
+  if (!out->R || !out->t || !out->registered || !out->edge_status || !out->support || !out->rot_residual ||
+      !out->dir_cos || !out->stats || !out->workspace)
+    return set_error(LTR_E_INVALID, "ltr_global_poses: null output or workspace");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  const int n = in->n_images, P = in->n_pairs;
+  char* w = static_cast<char*>(out->workspace);
+  auto take = [&](size_t bytes) {
+    char* p = w;
+    w += bytes;
+    return p;
+  };
+  GpArgs a{};
+  a.pairs = in->pairs; a.Rp = in->R; a.tp = in->t; a.valid = in->valid; a.ncheir = in->n_cheirality;
+  a.n = n; a.P = P; a.min_inliers = in->min_inliers; a.anchor_in = in->anchor < 0 ? -1 : in->anchor;
+  a.rot_iters = in->rot_iters; a.pos_iters = in->pos_iters; a.rot_tan = in->rot_tan; a.dir_cos = in->dir_cos;
+  a.ftol = in->ftol;
+  a.R = out->R; a.t = out->t; a.registered = out->registered; a.status = out->edge_status; a.support = out->support;
+  a.rot_res = out->rot_residual; a.dcos = out->dir_cos; a.stats = out->stats;
+  a.edge = reinterpret_cast<double*>(take(8ull * GP_EDGE * P));
+  a.cam = reinterpret_cast<double*>(take(8ull * GP_CAM * n));
+  a.table = reinterpret_cast<int*>(take(4ull * n * n));
+  a.inc = reinterpret_cast<int*>(take(4ull * n * std::max(n - 1, 1)));
+  a.deg = reinterpret_cast<int*>(take(4ull * n));
+  a.comp = reinterpret_cast<int*>(take(4ull * n));
+  a.si = reinterpret_cast<int*>(take(4ull * 16));
+  const size_t smem = gp_smem_bytes(n);
+  LTR_CUDA_TRY(ensure_dynamic_smem(gp_solve_kernel, (int)gp_smem_bytes(GP_MAX_IMAGES)));
+  LaunchScope ls(KC_GLOBAL_POSES, s);
+  LTR_CUDA_TRY(launch_pdl(gp_graph_kernel, dim3(1), dim3(GP_THREADS), 0, s, a));
+  if (P) LTR_CUDA_TRY(launch_pdl(gp_support_kernel, dim3(P), dim3(GP_MAX_IMAGES), 0, s, a));
+  LTR_CUDA_TRY(launch_pdl(gp_solve_kernel, dim3(1), dim3(GP_THREADS), smem, s, a));
   return LTR_OK;
 }
 

@@ -82,4 +82,60 @@ __device__ __forceinline__ void rc_cayley(const double* w, double* Q) {
       Q[3 * i + k] = RC_D(RC_A(RC_A(i == k ? s : 0.0, RC_M(2.0, RC_M(w[i], w[k]))), RC_M(2.0, wx[3 * i + k])), den);
 }
 
+// The dense SPD solver of one CTA of NT threads (_posed.cholesky_solve): a right-looking Cholesky of the m x m matrix
+// A (leading dimension ld; the lower triangle is read and L written over it), then the forward and back substitutions
+// of the k right-hand sides x [m, k] in place.  A and x may be global or shared.  s_col holds m doubles of shared
+// memory; *s_fail (shared) enters as 1 to skip the call, and leaves as 1 iff a pivot was not > 0, with x untouched.
+template <int NT>
+__device__ __forceinline__ bool rc_cholesky_solve(double* A, int ld, int m, double* x, int k, double* s_col,
+                                                  int* s_fail) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  // column c, then every later lower element once, in column order
+  for (int c = 0; c < m && !*s_fail; ++c) {
+    const double piv = A[(size_t)ld * c + c];
+    if (!(piv > 0.0)) {
+      __syncthreads();
+      if (tid == 0) *s_fail = 1;
+      break;
+    }
+    const double l = __dsqrt_rn(piv);
+    if (tid == 0) A[(size_t)ld * c + c] = l;
+    for (int i = c + 1 + tid; i < m; i += NT) {
+      const double v = RC_D(A[(size_t)ld * i + c], l);
+      A[(size_t)ld * i + c] = v;
+      s_col[i] = v;
+    }
+    __syncthreads();
+    // one warp per row of the trailing block, lanes over its columns c < j <= i
+    for (int i = c + 1 + wid; i < m; i += NT / 32) {
+      const double li = s_col[i];
+      double* Ai = A + (size_t)ld * i;
+      for (int j = c + 1 + lane; j <= i; j += 32) Ai[j] = RC_S(Ai[j], RC_M(li, s_col[j]));
+    }
+    __syncthreads();
+  }
+  __syncthreads();
+  const bool fail = *s_fail != 0;
+  if (fail) return true;
+  for (int c = 0; c < m; ++c) {
+    if (tid < k) x[(size_t)k * c + tid] = RC_D(x[(size_t)k * c + tid], A[(size_t)ld * c + c]);
+    __syncthreads();
+    for (int e = c * k + k + tid; e < m * k; e += NT) {
+      const int i = e / k;
+      x[e] = RC_S(x[e], RC_M(A[(size_t)ld * i + c], x[(size_t)k * c + e % k]));
+    }
+    __syncthreads();
+  }
+  for (int c = m - 1; c >= 0; --c) {
+    if (tid < k) x[(size_t)k * c + tid] = RC_D(x[(size_t)k * c + tid], A[(size_t)ld * c + c]);
+    __syncthreads();
+    for (int e = tid; e < c * k; e += NT) {
+      const int i = e / k;
+      x[e] = RC_S(x[e], RC_M(A[(size_t)ld * c + i], x[(size_t)k * c + e % k]));
+    }
+    __syncthreads();
+  }
+  return false;
+}
+
 }  // namespace ltr

@@ -726,3 +726,36 @@ def make_line_map_set(seed: int, n_views: int, n_points: int, n_lines: int, K=DE
     return {"keypoints": kps, "klines": kls, "K": K, "R": Rs, "t": ts, "points3d": X, "segments3d": S,
             "lines3d": np.stack(L3) if n_views else np.zeros((0, len(S), 2, 3)), "outlier_p": out_p,
             "outlier_l": out_l}
+
+
+def _axis_angle(ax, a):
+    S = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
+    return np.eye(3) + np.sin(a) * S + (1 - np.cos(a)) * S @ S
+
+
+def make_relative_poses(R, t, pairs, noise_deg: float = 0.0, outlier_frac: float = 0.0, seed: int = 0,
+                        n_cheirality: int = 100) -> dict:
+    """The relative poses of `pairs` (int [P, 2], image i side 0, image j side 1) of the world -> camera poses R [n, 3,
+    3], t [n, 3], shaped as an `estimate_poses` PoseResult on the host: R [P, 3, 3] and unit t [P, 3] with X_j = R_p
+    X_i + t_p, valid (all True) and n_cheirality (all n_cheirality).  Each clean pose is turned by N(0, noise_deg) about
+    a random axis and its direction by N(0, noise_deg) about another; a random outlier_frac of the pairs (exactly
+    round(outlier_frac P)) get a random rotation of 30 to 180 degrees and a random direction.  Also returns outlier
+    bool [P]."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    R, t = np.asarray(R, np.float64), np.asarray(t, np.float64)
+    pr = np.asarray(pairs, np.int64).reshape(-1, 2)
+    P = len(pr)
+    C = -np.einsum("nji,nj->ni", R, t)
+    out = np.zeros(P, bool)
+    out[rng.permutation(P)[:int(round(outlier_frac * P))]] = True
+    Rp, tp = np.zeros((P, 3, 3)), np.zeros((P, 3))
+    for p, (i, j) in enumerate(pr):
+        if out[p]:
+            Rp[p] = _axis_angle(_unit(rng.normal(size=3)), np.deg2rad(rng.uniform(30.0, 180.0)))
+            tp[p] = _unit(rng.normal(size=3))
+            continue
+        Rr = R[j] @ R[i].T
+        d = _unit(R[j] @ (C[i] - C[j]))
+        Rp[p] = _axis_angle(_unit(rng.normal(size=3)), np.deg2rad(noise_deg * rng.normal())) @ Rr
+        tp[p] = _axis_angle(_unit(rng.normal(size=3)), np.deg2rad(noise_deg * rng.normal())) @ d
+    return dict(R=Rp, t=tp, valid=np.ones(P, bool), n_cheirality=np.full(P, n_cheirality, np.int32), outlier=out)
