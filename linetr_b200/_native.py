@@ -57,8 +57,28 @@ class LtrError(RuntimeError):
     pass
 
 
+class _Tag:
+    """A `[const] T*` field of a struct mirror: ctypes passes it as C.c_void_p, `_typed` records T."""
+
+    def __init__(self, pointee):
+        self.pointee = pointee
+
+
+F32P, F64P, I32P, U8P, U64P = (_Tag(t) for t in (C.c_float, C.c_double, C.c_int32, C.c_uint8, C.c_uint64))
+
+
+def _typed(fields):
+    """(_fields_, _pointees_) of a struct mirror from its fields with tagged pointers: every field the header declares
+    `[const] T*` (T float, double, int32_t, uint8_t or uint64_t) is a tag, and goes into _fields_ as C.c_void_p, so
+    it takes an address as an int or None; _pointees_ {field: ctypes T} is what tests/test_abi.py holds to the header
+    and _ops.call_struct holds a tensor's dtype to."""
+    return ([(nm, C.c_void_p if isinstance(t, _Tag) else t) for nm, t in fields],
+            {nm: t.pointee for nm, t in fields if isinstance(t, _Tag)})
+
+
 class LtrTensor(C.Structure):
-    _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("numel", C.c_int64)]
+    _fields_, _pointees_ = _typed([
+        ("name", C.c_char_p), ("data", F32P), ("numel", C.c_int64)])
 
 
 class LtrConfig(C.Structure):
@@ -67,33 +87,34 @@ class LtrConfig(C.Structure):
 
 
 class LtrEncodeInput(C.Structure):
-    _fields_ = [("sublines", C.c_void_p), ("resp", C.c_void_p), ("angle", C.c_void_p),
-                ("pnt", C.c_void_p), ("desc", C.c_void_p), ("score", C.c_void_p),
-                ("cu_lines_host", C.c_void_p), ("cu_lines_dev", C.c_void_p),
-                ("n_images", C.c_int32), ("n_lines", C.c_int32), ("n_tokens", C.c_int32),
-                ("lines_per_image", C.c_int32), ("image_width", C.c_float), ("image_height", C.c_float)]
+    _fields_, _pointees_ = _typed([
+        ("sublines", F32P), ("resp", F32P), ("angle", F32P), ("pnt", F32P), ("desc", F32P), ("score", F32P),
+        ("cu_lines_host", I32P), ("cu_lines_dev", I32P), ("n_images", C.c_int32), ("n_lines", C.c_int32),
+        ("n_tokens", C.c_int32), ("lines_per_image", C.c_int32), ("image_width", C.c_float),
+        ("image_height", C.c_float)])
 
 
 class LtrEncodeOutput(C.Structure):
-    _fields_ = [("desc_cf", C.c_void_p), ("desc_rows", C.c_void_p), ("desc_tiles", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("desc_cf", F32P), ("desc_rows", F32P), ("desc_tiles", C.c_void_p)])
 
 
 class LtrMatchInput(C.Structure):
-    _fields_ = [("desc0", C.c_void_p), ("desc1", C.c_void_p), ("layout", C.c_int32), ("d", C.c_int32),
-                ("n_pairs", C.c_int32), ("n0", C.c_int32), ("n1", C.c_int32),
-                ("cu0", C.c_void_p), ("cu1", C.c_void_p), ("sub_off0", C.c_void_p), ("sub_off1", C.c_void_p),
-                ("cuk0", C.c_void_p), ("cuk1", C.c_void_p),
-                ("max_n0", C.c_int32), ("max_n1", C.c_int32), ("max_k0", C.c_int32), ("max_k1", C.c_int32),
-                ("dist_pair_stride", C.c_int64), ("nn_thresh", C.c_float), ("mutual", C.c_int32),
-                ("total_n0", C.c_int32), ("total_n1", C.c_int32), ("dist_mode", C.c_int32),
-                ("tiles0", C.c_void_p), ("tiles1", C.c_void_p), ("tiles_lines0", C.c_int32), ("tiles_lines1", C.c_int32),
-                ("tiles_row0_0", C.c_int32), ("tiles_row0_1", C.c_int32)]
+    _fields_, _pointees_ = _typed([
+        ("desc0", F32P), ("desc1", F32P), ("layout", C.c_int32), ("d", C.c_int32), ("n_pairs", C.c_int32),
+        ("n0", C.c_int32), ("n1", C.c_int32), ("cu0", I32P), ("cu1", I32P), ("sub_off0", I32P), ("sub_off1", I32P),
+        ("cuk0", I32P), ("cuk1", I32P), ("max_n0", C.c_int32), ("max_n1", C.c_int32), ("max_k0", C.c_int32),
+        ("max_k1", C.c_int32), ("dist_pair_stride", C.c_int64), ("nn_thresh", C.c_float), ("mutual", C.c_int32),
+        ("total_n0", C.c_int32), ("total_n1", C.c_int32), ("dist_mode", C.c_int32), ("tiles0", C.c_void_p),
+        ("tiles1", C.c_void_p), ("tiles_lines0", C.c_int32), ("tiles_lines1", C.c_int32), ("tiles_row0_0", C.c_int32),
+        ("tiles_row0_1", C.c_int32)])
 
 
 class LtrPairIndex(C.Structure):
-    _fields_ = [("img0", C.c_void_p), ("img1", C.c_void_p), ("tiles0", C.c_void_p), ("tiles1", C.c_void_p),
-                ("tile_off0", C.c_void_p), ("tile_off1", C.c_void_p), ("n_tiles0", C.c_int32), ("n_tiles1", C.c_int32),
-                ("out_off0", C.c_void_p), ("out_off1", C.c_void_p), ("total_out0", C.c_int32), ("total_out1", C.c_int32)]
+    _fields_, _pointees_ = _typed([
+        ("img0", I32P), ("img1", I32P), ("tiles0", C.c_void_p), ("tiles1", C.c_void_p), ("tile_off0", I32P),
+        ("tile_off1", I32P), ("n_tiles0", C.c_int32), ("n_tiles1", C.c_int32), ("out_off0", I32P), ("out_off1", I32P),
+        ("total_out0", C.c_int32), ("total_out1", C.c_int32)])
 
 
 GATHER_SLOTS = 8
@@ -105,162 +126,175 @@ class LtrPeerGather(C.Structure):
 
 
 class LtrMatchOutput(C.Structure):
-    _fields_ = [("matches0", C.c_void_p), ("scores0", C.c_void_p), ("nn1", C.c_void_p),
-                ("counts", C.c_void_p), ("dist_key", C.c_void_p), ("dist_sub", C.c_void_p),
-                ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64), ("gather", C.POINTER(LtrPeerGather))]
+    _fields_, _pointees_ = _typed([
+        ("matches0", I32P), ("scores0", F32P), ("nn1", I32P), ("counts", I32P), ("dist_key", F32P), ("dist_sub", F32P),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64), ("gather", C.POINTER(LtrPeerGather))])
 
 
 class LtrTokenizeImage(C.Structure):
-    _fields_ = [("dense_desc", C.c_void_p), ("dense_score", C.c_void_p), ("token_distance", C.c_double),
-                ("desc_h", C.c_int32), ("desc_w", C.c_int32), ("score_h", C.c_int32), ("score_w", C.c_int32)]
+    _fields_, _pointees_ = _typed([
+        ("dense_desc", F32P), ("dense_score", F32P), ("token_distance", C.c_double), ("desc_h", C.c_int32),
+        ("desc_w", C.c_int32), ("score_h", C.c_int32), ("score_w", C.c_int32)])
 
 
 class LtrTokenizeBatchInput(C.Structure):
-    _fields_ = [("sp", C.c_void_p), ("ep", C.c_void_p), ("ep_clipped", C.c_void_p), ("length", C.c_void_p),
-                ("angle", C.c_void_p), ("n_tok", C.c_void_p), ("sub0", C.c_void_p), ("sub2line", C.c_void_p),
-                ("line_image", C.c_void_p), ("n_images", C.c_int32), ("n_keylines", C.c_int32),
-                ("n_sublines", C.c_int32), ("n_tokens", C.c_int32), ("desc_channels", C.c_int32),
-                ("align_corners", C.c_int32), ("images", C.POINTER(LtrTokenizeImage)), ("cu_sublines", c_int32_p)]
+    _fields_, _pointees_ = _typed([
+        ("sp", F64P), ("ep", F64P), ("ep_clipped", F64P), ("length", F64P), ("angle", F32P), ("n_tok", I32P),
+        ("sub0", I32P), ("sub2line", I32P), ("line_image", I32P), ("n_images", C.c_int32), ("n_keylines", C.c_int32),
+        ("n_sublines", C.c_int32), ("n_tokens", C.c_int32), ("desc_channels", C.c_int32), ("align_corners", C.c_int32),
+        ("images", C.POINTER(LtrTokenizeImage)), ("cu_sublines", c_int32_p)])
 
 
 class LtrLineGtInput(C.Structure):
-    _fields_ = [("segs0", C.c_void_p), ("segs1", C.c_void_p), ("cu0", C.c_void_p), ("cu1", C.c_void_p),
-                ("homography", C.c_void_p), ("homography_inv", C.c_void_p), ("proj0", C.c_void_p), ("proj1", C.c_void_p),
-                ("pred0", C.c_void_p), ("n_pairs", C.c_int32), ("max_n0", C.c_int32), ("max_n1", C.c_int32),
-                ("thres_reprojected", C.c_float), ("thres_angdiff", C.c_double), ("min_overlap_ratio", C.c_double)]
+    _fields_, _pointees_ = _typed([
+        ("segs0", F32P), ("segs1", F32P), ("cu0", I32P), ("cu1", I32P), ("homography", F64P), ("homography_inv", F64P),
+        ("proj0", F32P), ("proj1", F32P), ("pred0", I32P), ("n_pairs", C.c_int32), ("max_n0", C.c_int32),
+        ("max_n1", C.c_int32), ("thres_reprojected", C.c_float), ("thres_angdiff", C.c_double),
+        ("min_overlap_ratio", C.c_double)])
 
 
 class LtrLineGtOutput(C.Structure):
-    _fields_ = [("assign", C.c_void_p), ("assign_stride", C.c_int64), ("n_gt", C.c_void_p), ("tfpn", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("assign", F32P), ("assign_stride", C.c_int64), ("n_gt", I32P), ("tfpn", I32P)])
 
 
 class LtrTripletInput(C.Structure):
-    _fields_ = [("desc0", C.c_void_p), ("desc1", C.c_void_p), ("layout", C.c_int32), ("d", C.c_int32),
-                ("n_pairs", C.c_int32), ("n0", C.c_int32), ("n1", C.c_int32), ("cu0", C.c_void_p), ("cu1", C.c_void_p),
-                ("max_n0", C.c_int32), ("max_n1", C.c_int32), ("assign", C.c_void_p), ("assign_stride", C.c_int64),
-                ("assign_ld", C.c_int32), ("match_thr", C.c_double), ("unmatch_thr", C.c_double), ("pred0", C.c_void_p),
-                ("n_groups", C.c_int32), ("group_off", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("desc0", F32P), ("desc1", F32P), ("layout", C.c_int32), ("d", C.c_int32), ("n_pairs", C.c_int32),
+        ("n0", C.c_int32), ("n1", C.c_int32), ("cu0", I32P), ("cu1", I32P), ("max_n0", C.c_int32),
+        ("max_n1", C.c_int32), ("assign", F32P), ("assign_stride", C.c_int64), ("assign_ld", C.c_int32),
+        ("match_thr", C.c_double), ("unmatch_thr", C.c_double), ("pred0", I32P), ("n_groups", C.c_int32),
+        ("group_off", I32P)])
 
 
 class LtrTripletOutput(C.Structure):
-    _fields_ = [("pos", C.c_void_p), ("neg", C.c_void_p), ("state", C.c_void_p), ("loss", C.c_void_p),
-                ("hardest_pos", C.c_void_p), ("hardest_neg", C.c_void_p), ("n_valid", C.c_void_p), ("tfpn", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("pos", F32P), ("neg", F32P), ("state", I32P), ("loss", F32P), ("hardest_pos", F32P), ("hardest_neg", F32P),
+        ("n_valid", I32P), ("tfpn", I32P)])
 
 
 class LtrHomographyInput(C.Structure):
-    _fields_ = [("pts0", C.c_void_p), ("pts1", C.c_void_p), ("pts_off0", C.c_void_p), ("pts_off1", C.c_void_p),
-                ("n_pts1", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("segs0", C.c_void_p),
-                ("segs1", C.c_void_p), ("seg_off0", C.c_void_p), ("seg_off1", C.c_void_p), ("n_segs1", C.c_void_p),
-                ("matches_l", C.c_void_p), ("cu_l", C.c_void_p), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32),
-                ("max_rows_l", C.c_int32), ("thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64),
-                ("use_points", C.c_int32), ("use_lines", C.c_int32)]
+    _fields_, _pointees_ = _typed([
+        ("pts0", F32P), ("pts1", F32P), ("pts_off0", I32P), ("pts_off1", I32P), ("n_pts1", I32P), ("matches_p", I32P),
+        ("cu_p", I32P), ("segs0", F32P), ("segs1", F32P), ("seg_off0", I32P), ("seg_off1", I32P), ("n_segs1", I32P),
+        ("matches_l", I32P), ("cu_l", I32P), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32),
+        ("max_rows_l", C.c_int32), ("thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64),
+        ("use_points", C.c_int32), ("use_lines", C.c_int32)])
 
 
 class LtrHomographyOutput(C.Structure):
-    _fields_ = [("H", C.c_void_p), ("valid", C.c_void_p), ("inliers_p", C.c_void_p), ("inliers_l", C.c_void_p),
-                ("n_inliers_p", C.c_void_p), ("n_inliers_l", C.c_void_p), ("hypothesis", C.c_void_p),
-                ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("H", F64P), ("valid", U8P), ("inliers_p", U8P), ("inliers_l", U8P), ("n_inliers_p", I32P),
+        ("n_inliers_l", I32P), ("hypothesis", I32P), ("hypothesis_inliers", I32P), ("key", U64P)])
 
 
 class LtrEssentialInput(C.Structure):
-    _fields_ = [("pts0", C.c_void_p), ("pts1", C.c_void_p), ("pts_off0", C.c_void_p), ("pts_off1", C.c_void_p),
-                ("n_pts1", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("K0", C.c_void_p),
-                ("K1", C.c_void_p), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32), ("thresh", C.c_double),
-                ("dist_thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64)]
+    _fields_, _pointees_ = _typed([
+        ("pts0", F32P), ("pts1", F32P), ("pts_off0", I32P), ("pts_off1", I32P), ("n_pts1", I32P), ("matches_p", I32P),
+        ("cu_p", I32P), ("K0", F64P), ("K1", F64P), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32),
+        ("thresh", C.c_double), ("dist_thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64)])
 
 
 class LtrEssentialOutput(C.Structure):
-    _fields_ = [("E", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("valid", C.c_void_p),
-                ("inliers_p", C.c_void_p), ("n_inliers", C.c_void_p), ("n_cheirality", C.c_void_p),
-                ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("E", F64P), ("R", F64P), ("t", F64P), ("valid", U8P), ("inliers_p", U8P), ("n_inliers", I32P),
+        ("n_cheirality", I32P), ("hypothesis", I32P), ("hypothesis_inliers", I32P), ("key", U64P)])
 
 
 class LtrFundamentalInput(C.Structure):
-    _fields_ = [("pts0", C.c_void_p), ("pts1", C.c_void_p), ("pts_off0", C.c_void_p), ("pts_off1", C.c_void_p),
-                ("n_pts1", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("segs0", C.c_void_p),
-                ("segs1", C.c_void_p), ("seg_off0", C.c_void_p), ("seg_off1", C.c_void_p), ("n_segs1", C.c_void_p),
-                ("matches_l", C.c_void_p), ("cu_l", C.c_void_p), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32),
-                ("max_rows_l", C.c_int32), ("thresh", C.c_double), ("min_overlap", C.c_double),
-                ("n_hypotheses", C.c_int32), ("seed", C.c_uint64)]
+    _fields_, _pointees_ = _typed([
+        ("pts0", F32P), ("pts1", F32P), ("pts_off0", I32P), ("pts_off1", I32P), ("n_pts1", I32P), ("matches_p", I32P),
+        ("cu_p", I32P), ("segs0", F32P), ("segs1", F32P), ("seg_off0", I32P), ("seg_off1", I32P), ("n_segs1", I32P),
+        ("matches_l", I32P), ("cu_l", I32P), ("n_pairs", C.c_int32), ("max_rows_p", C.c_int32),
+        ("max_rows_l", C.c_int32), ("thresh", C.c_double), ("min_overlap", C.c_double), ("n_hypotheses", C.c_int32),
+        ("seed", C.c_uint64)])
 
 
 class LtrFundamentalOutput(C.Structure):
-    _fields_ = [("F", C.c_void_p), ("valid", C.c_void_p), ("refit", C.c_void_p), ("inliers_p", C.c_void_p),
-                ("lines_consistent", C.c_void_p), ("n_inliers", C.c_void_p), ("n_lines_consistent", C.c_void_p),
-                ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p), ("key", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("F", F64P), ("valid", U8P), ("refit", U8P), ("inliers_p", U8P), ("lines_consistent", U8P), ("n_inliers", I32P),
+        ("n_lines_consistent", I32P), ("hypothesis", I32P), ("hypothesis_inliers", I32P), ("key", U64P)])
 
 
 class LtrAbsPoseInput(C.Structure):
-    _fields_ = [("pts0", C.c_void_p), ("pts_off0", C.c_void_p), ("matches_p", C.c_void_p), ("cu_p", C.c_void_p),
-                ("X1", C.c_void_p), ("x_off1", C.c_void_p), ("n_x1", C.c_void_p), ("segs0", C.c_void_p),
-                ("seg_off0", C.c_void_p), ("matches_l", C.c_void_p), ("cu_l", C.c_void_p), ("L1", C.c_void_p),
-                ("l_off1", C.c_void_p), ("n_l1", C.c_void_p), ("groups", C.c_void_p), ("K0", C.c_void_p),
-                ("n_pairs", C.c_int32), ("n_groups", C.c_int32), ("max_rows_p", C.c_int32), ("max_rows_l", C.c_int32),
-                ("thresh", C.c_double), ("n_hypotheses", C.c_int32), ("seed", C.c_uint64), ("use_lines", C.c_int32)]
+    _fields_, _pointees_ = _typed([
+        ("pts0", F32P), ("pts_off0", I32P), ("matches_p", I32P), ("cu_p", I32P), ("X1", F64P), ("x_off1", I32P),
+        ("n_x1", I32P), ("segs0", F32P), ("seg_off0", I32P), ("matches_l", I32P), ("cu_l", I32P), ("L1", F64P),
+        ("l_off1", I32P), ("n_l1", I32P), ("groups", I32P), ("K0", F64P), ("n_pairs", C.c_int32),
+        ("n_groups", C.c_int32), ("max_rows_p", C.c_int32), ("max_rows_l", C.c_int32), ("thresh", C.c_double),
+        ("n_hypotheses", C.c_int32), ("seed", C.c_uint64), ("use_lines", C.c_int32)])
 
 
 class LtrAbsPoseOutput(C.Structure):
-    _fields_ = [("R", C.c_void_p), ("t", C.c_void_p), ("valid", C.c_void_p), ("refit", C.c_void_p),
-                ("inliers_p", C.c_void_p), ("inliers_l", C.c_void_p), ("n_inliers_p", C.c_void_p),
-                ("n_inliers_l", C.c_void_p), ("hypothesis", C.c_void_p), ("hypothesis_inliers", C.c_void_p),
-                ("key", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("R", F64P), ("t", F64P), ("valid", U8P), ("refit", U8P), ("inliers_p", U8P), ("inliers_l", U8P),
+        ("n_inliers_p", I32P), ("n_inliers_l", I32P), ("hypothesis", I32P), ("hypothesis_inliers", I32P),
+        ("key", U64P)])
 
 
 class LtrTriangulateInput(C.Structure):
-    _fields_ = [("kpts", C.c_void_p), ("kp_off", C.c_void_p), ("segs", C.c_void_p), ("seg_off", C.c_void_p),
-                ("K", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("pairs", C.c_void_p),
-                ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("matches_l", C.c_void_p), ("cu_l", C.c_void_p),
-                ("views", C.c_void_p), ("view_off", C.c_void_p), ("block_off", C.c_void_p), ("inv_off_p", C.c_void_p),
-                ("inv_off_l", C.c_void_p), ("n_images", C.c_int32), ("n_pairs", C.c_int32), ("total_p", C.c_int32),
-                ("total_l", C.c_int32), ("n_inv_p", C.c_int32), ("n_inv_l", C.c_int32), ("n_blocks", C.c_int32),
-                ("max_views", C.c_int32), ("thresh", C.c_double), ("min_angle", C.c_double), ("min_views", C.c_int32)]
+    _fields_, _pointees_ = _typed([
+        ("kpts", F32P), ("kp_off", I32P), ("segs", F32P), ("seg_off", I32P), ("K", F64P), ("R", F64P), ("t", F64P),
+        ("pairs", I32P), ("matches_p", I32P), ("cu_p", I32P), ("matches_l", I32P), ("cu_l", I32P), ("views", I32P),
+        ("view_off", I32P), ("block_off", I32P), ("inv_off_p", I32P), ("inv_off_l", I32P), ("n_images", C.c_int32),
+        ("n_pairs", C.c_int32), ("total_p", C.c_int32), ("total_l", C.c_int32), ("n_inv_p", C.c_int32),
+        ("n_inv_l", C.c_int32), ("n_blocks", C.c_int32), ("max_views", C.c_int32), ("thresh", C.c_double),
+        ("min_angle", C.c_double), ("min_views", C.c_int32)])
 
 
 class LtrTriangulateOutput(C.Structure):
-    _fields_ = [("points3d", C.c_void_p), ("lines3d", C.c_void_p), ("n_views_p", C.c_void_p), ("n_views_l", C.c_void_p),
-                ("inv_p", C.c_void_p), ("inv_l", C.c_void_p)]
+    _fields_, _pointees_ = _typed([
+        ("points3d", F64P), ("lines3d", F64P), ("n_views_p", I32P), ("n_views_l", I32P), ("inv_p", I32P),
+        ("inv_l", I32P)])
 
 
 class LtrTracksInput(C.Structure):
-    _fields_ = [("kpts", C.c_void_p), ("kp_off", C.c_void_p), ("segs", C.c_void_p), ("seg_off", C.c_void_p),
-                ("K", C.c_void_p), ("R", C.c_void_p), ("t", C.c_void_p), ("F", C.c_void_p), ("pairs", C.c_void_p),
-                ("matches_p", C.c_void_p), ("cu_p", C.c_void_p), ("matches_l", C.c_void_p), ("cu_l", C.c_void_p),
-                ("n_images", C.c_int32), ("n_pairs", C.c_int32), ("total_p", C.c_int32), ("total_l", C.c_int32),
-                ("n_kp", C.c_int32), ("n_kl", C.c_int32), ("thresh", C.c_double), ("min_angle", C.c_double),
-                ("min_views", C.c_int32), ("epi_thresh", C.c_double), ("min_overlap", C.c_double)]
+    _fields_, _pointees_ = _typed([
+        ("kpts", F32P), ("kp_off", I32P), ("segs", F32P), ("seg_off", I32P), ("K", F64P), ("R", F64P), ("t", F64P),
+        ("F", F64P), ("pairs", I32P), ("matches_p", I32P), ("cu_p", I32P), ("matches_l", I32P), ("cu_l", I32P),
+        ("n_images", C.c_int32), ("n_pairs", C.c_int32), ("total_p", C.c_int32), ("total_l", C.c_int32),
+        ("n_kp", C.c_int32), ("n_kl", C.c_int32), ("thresh", C.c_double), ("min_angle", C.c_double),
+        ("min_views", C.c_int32), ("epi_thresh", C.c_double), ("min_overlap", C.c_double)])
 
 
 class LtrTracksOutput(C.Structure):
-    _fields_ = [(nm, C.c_void_p) for nm in (
-        "track_p", "track_l", "n_tracks_p", "n_tracks_l", "track_off_p", "track_off_l", "obs_p", "obs_l", "points3d",
-        "lines3d", "n_obs_p", "n_obs_l", "n_inliers_p", "n_inliers_l", "n_images_p", "n_images_l", "status_p",
-        "status_l", "inlier_p", "inlier_l", "row_points3d", "row_lines3d", "n_views_p", "n_views_l", "workspace")]
+    _fields_, _pointees_ = _typed([
+        ("track_p", I32P), ("track_l", I32P), ("n_tracks_p", I32P), ("n_tracks_l", I32P), ("track_off_p", I32P),
+        ("track_off_l", I32P), ("obs_p", I32P), ("obs_l", I32P), ("points3d", F64P), ("lines3d", F64P),
+        ("n_obs_p", I32P), ("n_obs_l", I32P), ("n_inliers_p", I32P), ("n_inliers_l", I32P), ("n_images_p", I32P),
+        ("n_images_l", I32P), ("status_p", I32P), ("status_l", I32P), ("inlier_p", U8P), ("inlier_l", U8P),
+        ("row_points3d", F64P), ("row_lines3d", F64P), ("n_views_p", I32P), ("n_views_l", I32P), ("workspace", I32P)])
 
 
 class LtrBundleInput(C.Structure):
-    _fields_ = [(nm, C.c_void_p) for nm in (
-        "kpts", "kp_off", "segs", "seg_off", "K", "R", "t", "hold", "fixed", "n_tracks_p", "n_tracks_l", "track_off_p",
-        "track_off_l", "obs_p", "obs_l", "status_p", "status_l", "inlier_p", "inlier_l", "track_p", "track_l",
-        "n_views_p", "n_views_l", "points3d", "lines3d")] + [
-        (nm, C.c_int32) for nm in ("n_images", "n_fixed", "n_kp", "n_kl", "t_p", "t_l", "max_iters")] + [
-        ("ftol", C.c_double)]
+    _fields_, _pointees_ = _typed([
+        ("kpts", F32P), ("kp_off", I32P), ("segs", F32P), ("seg_off", I32P), ("K", F64P), ("R", F64P), ("t", F64P),
+        ("hold", I32P), ("fixed", I32P), ("n_tracks_p", I32P), ("n_tracks_l", I32P), ("track_off_p", I32P),
+        ("track_off_l", I32P), ("obs_p", I32P), ("obs_l", I32P), ("status_p", I32P), ("status_l", I32P),
+        ("inlier_p", U8P), ("inlier_l", U8P), ("track_p", I32P), ("track_l", I32P), ("n_views_p", I32P),
+        ("n_views_l", I32P), ("points3d", F64P), ("lines3d", F64P), ("n_images", C.c_int32), ("n_fixed", C.c_int32),
+        ("n_kp", C.c_int32), ("n_kl", C.c_int32), ("t_p", C.c_int32), ("t_l", C.c_int32), ("max_iters", C.c_int32),
+        ("ftol", C.c_double)])
 
 
 class LtrBundleOutput(C.Structure):
-    _fields_ = [(nm, C.c_void_p) for nm in (
-        "R", "t", "points3d", "lines3d", "status_p", "status_l", "residual_p", "residual_l", "row_points3d",
-        "row_lines3d", "n_views_p", "n_views_l", "stats", "workspace")]
+    _fields_, _pointees_ = _typed([
+        ("R", F64P), ("t", F64P), ("points3d", F64P), ("lines3d", F64P), ("status_p", I32P), ("status_l", I32P),
+        ("residual_p", F64P), ("residual_l", F64P), ("row_points3d", F64P), ("row_lines3d", F64P), ("n_views_p", I32P),
+        ("n_views_l", I32P), ("stats", F64P), ("workspace", C.c_void_p)])
 
 
 class LtrGlobalPoseInput(C.Structure):
-    _fields_ = [(nm, C.c_void_p) for nm in ("pairs", "R", "t", "valid", "n_cheirality")] + [
-        (nm, C.c_int32) for nm in ("n_images", "n_pairs", "min_inliers", "anchor", "rot_iters", "pos_iters")] + [
-        (nm, C.c_double) for nm in ("rot_tan", "dir_cos", "ftol")]
+    _fields_, _pointees_ = _typed([
+        ("pairs", I32P), ("R", F64P), ("t", F64P), ("valid", U8P), ("n_cheirality", I32P), ("n_images", C.c_int32),
+        ("n_pairs", C.c_int32), ("min_inliers", C.c_int32), ("anchor", C.c_int32), ("rot_iters", C.c_int32),
+        ("pos_iters", C.c_int32), ("rot_tan", C.c_double), ("dir_cos", C.c_double), ("ftol", C.c_double)])
 
 
 class LtrGlobalPoseOutput(C.Structure):
-    _fields_ = [(nm, C.c_void_p) for nm in (
-        "R", "t", "registered", "edge_status", "support", "rot_residual", "dir_cos", "stats", "workspace")]
+    _fields_, _pointees_ = _typed([
+        ("R", F64P), ("t", F64P), ("registered", U8P), ("edge_status", I32P), ("support", I32P), ("rot_residual", F64P),
+        ("dir_cos", F64P), ("stats", F64P), ("workspace", C.c_void_p)])
 
 
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER

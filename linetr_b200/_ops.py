@@ -7,6 +7,7 @@ device (no CPU fallback).
 from __future__ import annotations
 
 import ctypes as C
+import functools
 
 import numpy as np
 import torch
@@ -370,299 +371,57 @@ def tokenize(dv: dict, maps, cu_lines: np.ndarray, max_tokens: int, dev) -> list
     return out
 
 
-def line_gt(segs0, segs1, n_pairs, *, cu0, cu1, max_n0, max_n1, homography, homography_inv, n_gt, assign=None,
-            assign_stride=0, pred0=None, tfpn=None, proj0=None, proj1=None, thres_reprojected=3.0, thres_angdiff=2.0,
-            min_overlap_ratio=0.3):
-    """ltr_line_gt into caller-allocated outputs: homography ground truth of P line-segment pairs (segs [S,2,2] fp32,
-    side s of pair p = [cu_s[p], cu_s[p+1]), homography [P,3,3] fp64 image 0 -> 1 and its inverse), n_gt [P] int32,
-    optionally the dense assignment (pair p at p * assign_stride, row-major [n0_p, n1_p]) and, with pred0 (int32 [S0]
-    local side-1 index or -1), tfpn [P,4] int32 (TP, FP, FN, TN)."""
-    _req_cuda(segs0, "segs0")
-    _req_cuda(segs1, "segs1")
-    dev = segs0.device
-    specs = (("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32), ("cu0", cu0, torch.int32),
-             ("cu1", cu1, torch.int32), ("homography", homography, torch.float64),
-             ("homography_inv", homography_inv, torch.float64), ("n_gt", n_gt, torch.int32),
-             ("assign", assign, torch.float32), ("pred0", pred0, torch.int32), ("tfpn", tfpn, torch.int32),
-             ("proj0", proj0, torch.float32), ("proj1", proj1, torch.float32))
-    for nm, t, _ in specs:
-        if t is not None:
+# the tensor dtypes a pointer field takes by its pointee (_native._pointees_; a void* field takes any) and the
+# conversion of each scalar field type
+_POINTEE_DTYPES = {C.c_float: (torch.float32,), C.c_double: (torch.float64,), C.c_int32: (torch.int32,),
+                   C.c_uint64: (torch.int64,), C.c_uint8: (torch.uint8, torch.bool)}
+_SCALAR = {C.c_int32: int, C.c_int64: int, C.c_float: float, C.c_double: float,
+           C.c_uint64: lambda v: int(v) & 0xFFFFFFFFFFFFFFFF}
+
+
+@functools.cache
+def _layout(cls):
+    """(field names, pointer fields as (name, dtypes or None for void*), scalar fields as (name, conversion)) of a
+    struct mirror."""
+    ptrs = tuple((nm, _POINTEE_DTYPES[cls._pointees_[nm]] if nm in cls._pointees_ else None)
+                 for nm, t in cls._fields_ if t is C.c_void_p)
+    scalars = tuple((nm, _SCALAR[t]) for nm, t in cls._fields_ if t is not C.c_void_p)
+    return frozenset(nm for nm, _ in cls._fields_), ptrs, scalars
+
+
+def call_struct(entry: str, inputs: dict, outputs: dict, workspace_bytes=None):
+    """`entry`(const In*, const Out*, device, stream) with the fields of its In and Out structs by name: every scalar
+    field is required; a pointer field takes None (NULL) or a contiguous CUDA tensor of the dtype its mirror names (any
+    dtype for void*), on the device of the outputs.  Runs on that device's current stream.  workspace_bytes, when given,
+    is the least size of the `workspace` output.  The caller keeps the tensors alive until the call."""
+    who = entry[4:]
+    _, (p_in, p_out, *_) = N.PROTOTYPES[entry]
+    dev, structs = None, {}
+    for cls, given in ((p_out._type_, outputs), (p_in._type_, inputs)):
+        names, ptrs, scalars = _layout(cls)
+        if not given.keys() <= names:
+            raise N.LtrError(f"{who}: {cls.__name__} has no field {sorted(given.keys() - names)}")
+        fields = {}
+        for nm, dts in ptrs:
+            t = given.get(nm)
+            if t is None:
+                continue
             _req_cuda(t, nm)
-    _check_tensors("line_gt", dev, specs)
-    inp = _struct(N.LtrLineGtInput, segs0=segs0, segs1=segs1, cu0=cu0, cu1=cu1, homography=homography,
-                  homography_inv=homography_inv, proj0=proj0, proj1=proj1, pred0=pred0, n_pairs=int(n_pairs),
-                  max_n0=int(max_n0), max_n1=int(max_n1), thres_reprojected=float(thres_reprojected),
-                  thres_angdiff=float(thres_angdiff), min_overlap_ratio=float(min_overlap_ratio))
-    out = _struct(N.LtrLineGtOutput, assign=assign, assign_stride=int(assign_stride), n_gt=n_gt, tfpn=tfpn)
-    _call("ltr_line_gt", dev, C.byref(inp), C.byref(out))
-
-
-def triplet_loss(desc0, desc1, layout, n_pairs, *, assign, assign_stride, pos, neg, state, loss, hardest_pos,
-                 hardest_neg, n_valid, n0=0, n1=0, cu0=None, cu1=None, max_n0=0, max_n1=0, assign_ld=0, match_thr=0.3,
-                 unmatch_thr=0.0, pred0=None, tfpn=None, n_groups=1, group_off=None):
-    """ltr_triplet_loss into caller-allocated outputs: per anchor pos / neg (fp32) and state (int32) [S0 + S1], per
-    group loss / hardest_pos / hardest_neg (fp32) and n_valid (int32), tfpn [P, 4] int32 with pred0."""
-    _req_cuda(desc0, "desc0")
-    _req_cuda(desc1, "desc1")
-    dev = desc0.device
-    _check_tensors("triplet_loss", dev, (
-        ("desc0", desc0, torch.float32), ("desc1", desc1, torch.float32), ("assign", assign, torch.float32),
-        ("cu0", cu0, torch.int32), ("cu1", cu1, torch.int32), ("pred0", pred0, torch.int32),
-        ("group_off", group_off, torch.int32), ("pos", pos, torch.float32), ("neg", neg, torch.float32),
-        ("state", state, torch.int32), ("loss", loss, torch.float32), ("hardest_pos", hardest_pos, torch.float32),
-        ("hardest_neg", hardest_neg, torch.float32), ("n_valid", n_valid, torch.int32), ("tfpn", tfpn, torch.int32)))
-    inp = _struct(N.LtrTripletInput, desc0=desc0, desc1=desc1, layout=int(layout), d=256, n_pairs=int(n_pairs), n0=int(n0),
-                  n1=int(n1), cu0=cu0, cu1=cu1, max_n0=int(max_n0), max_n1=int(max_n1), assign=assign,
-                  assign_stride=int(assign_stride), assign_ld=int(assign_ld), match_thr=float(match_thr),
-                  unmatch_thr=float(unmatch_thr), pred0=pred0, n_groups=int(n_groups), group_off=group_off)
-    out = _struct(N.LtrTripletOutput, pos=pos, neg=neg, state=state, loss=loss, hardest_pos=hardest_pos,
-                  hardest_neg=hardest_neg, n_valid=n_valid, tfpn=tfpn)
-    _call("ltr_triplet_loss", dev, C.byref(inp), C.byref(out))
-
-
-def homography(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, segs0, segs1, seg_off0,
-               seg_off1, n_segs1, matches_l, cu_l, max_rows_l, H, valid, inliers_p, inliers_l, n_inliers_p, n_inliers_l,
-               hypothesis, hypothesis_inliers, key, thresh=3.0, n_hypotheses=2048, seed=0, use_points=True,
-               use_lines=True):
-    """ltr_homography into caller-allocated outputs: keypoint pools [*,2] / segment pools [*,2,2] fp32, per-pair pool
-    offsets and side-1 counts int32 [P], match rows int32 with offsets cu_p / cu_l [P+1]; H [P,3,3] fp64, valid [P]
-    uint8, inliers_p / inliers_l uint8 aligned with the match rows, counts / hypothesis int32 [P], key [P] int64
-    workspace."""
-    _req_cuda(H, "H")
-    dev = H.device
-    _check_tensors("homography", dev, (
-        ("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
-        ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32), ("matches_p", matches_p, torch.int32),
-        ("cu_p", cu_p, torch.int32), ("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32),
-        ("seg_off0", seg_off0, torch.int32), ("seg_off1", seg_off1, torch.int32), ("n_segs1", n_segs1, torch.int32),
-        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("H", H, torch.float64),
-        ("valid", valid, torch.uint8), ("inliers_p", inliers_p, torch.uint8), ("inliers_l", inliers_l, torch.uint8),
-        ("n_inliers_p", n_inliers_p, torch.int32), ("n_inliers_l", n_inliers_l, torch.int32),
-        ("hypothesis", hypothesis, torch.int32), ("hypothesis_inliers", hypothesis_inliers, torch.int32),
-        ("key", key, torch.int64)))
-    inp = _struct(N.LtrHomographyInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
-                  matches_p=matches_p, cu_p=cu_p, segs0=segs0, segs1=segs1, seg_off0=seg_off0, seg_off1=seg_off1,
-                  n_segs1=n_segs1, matches_l=matches_l, cu_l=cu_l, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
-                  max_rows_l=int(max_rows_l), thresh=float(thresh), n_hypotheses=int(n_hypotheses),
-                  seed=int(seed) & 0xFFFFFFFFFFFFFFFF, use_points=int(bool(use_points)), use_lines=int(bool(use_lines)))
-    out = _struct(N.LtrHomographyOutput, H=H, valid=valid, inliers_p=inliers_p, inliers_l=inliers_l,
-                  n_inliers_p=n_inliers_p, n_inliers_l=n_inliers_l, hypothesis=hypothesis,
-                  hypothesis_inliers=hypothesis_inliers, key=key)
-    _call("ltr_homography", dev, C.byref(inp), C.byref(out))
-
-
-def essential(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, K0, K1, E, R, t, valid,
-              inliers_p, n_inliers, n_cheirality, hypothesis, hypothesis_inliers, key, thresh=1.0, dist_thresh=1e9,
-              n_hypotheses=1024, seed=0):
-    """ltr_essential into caller-allocated outputs: keypoint pools [*,2] fp32, per-pair pool offsets and side-1 counts
-    int32 [P], match rows int32 with offsets cu_p [P+1], intrinsics K0 / K1 fp64 [P,3,3]; E / R [P,3,3] and t [P,3]
-    fp64, valid [P] uint8, inliers_p uint8 aligned with the match rows, counts / hypothesis int32 [P], key [P] int64
-    workspace."""
-    _req_cuda(E, "E")
-    dev = E.device
-    _check_tensors("essential", dev, (
-        ("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
-        ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32), ("matches_p", matches_p, torch.int32),
-        ("cu_p", cu_p, torch.int32), ("K0", K0, torch.float64), ("K1", K1, torch.float64), ("E", E, torch.float64),
-        ("R", R, torch.float64), ("t", t, torch.float64), ("valid", valid, torch.uint8),
-        ("inliers_p", inliers_p, torch.uint8), ("n_inliers", n_inliers, torch.int32),
-        ("n_cheirality", n_cheirality, torch.int32), ("hypothesis", hypothesis, torch.int32),
-        ("hypothesis_inliers", hypothesis_inliers, torch.int32), ("key", key, torch.int64)))
-    inp = _struct(N.LtrEssentialInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
-                  matches_p=matches_p, cu_p=cu_p, K0=K0, K1=K1, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
-                  thresh=float(thresh), dist_thresh=float(dist_thresh), n_hypotheses=int(n_hypotheses),
-                  seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
-    out = _struct(N.LtrEssentialOutput, E=E, R=R, t=t, valid=valid, inliers_p=inliers_p, n_inliers=n_inliers,
-                  n_cheirality=n_cheirality, hypothesis=hypothesis, hypothesis_inliers=hypothesis_inliers, key=key)
-    _call("ltr_essential", dev, C.byref(inp), C.byref(out))
-
-
-def fundamental(n_pairs, *, pts0, pts1, pts_off0, pts_off1, n_pts1, matches_p, cu_p, max_rows_p, segs0, segs1,
-                seg_off0, seg_off1, n_segs1, matches_l, cu_l, max_rows_l, F, valid, refit, inliers_p, lines_consistent,
-                n_inliers, n_lines_consistent, hypothesis, hypothesis_inliers, key, thresh=3.0, min_overlap=0.5,
-                n_hypotheses=2048, seed=0):
-    """ltr_fundamental into caller-allocated outputs: keypoint pools [*,2] / segment pools [*,2,2] fp32, per-pair pool
-    offsets and side-1 counts int32 [P], match rows int32 with offsets cu_p / cu_l [P+1]; F [P,3,3] fp64, valid / refit
-    [P] uint8, inliers_p / lines_consistent uint8 aligned with the match rows, counts / hypothesis int32 [P], key [P]
-    int64 workspace."""
-    _req_cuda(F, "F")
-    dev = F.device
-    _check_tensors("fundamental", dev, (
-        ("pts0", pts0, torch.float32), ("pts1", pts1, torch.float32), ("pts_off0", pts_off0, torch.int32),
-        ("pts_off1", pts_off1, torch.int32), ("n_pts1", n_pts1, torch.int32), ("matches_p", matches_p, torch.int32),
-        ("cu_p", cu_p, torch.int32), ("segs0", segs0, torch.float32), ("segs1", segs1, torch.float32),
-        ("seg_off0", seg_off0, torch.int32), ("seg_off1", seg_off1, torch.int32), ("n_segs1", n_segs1, torch.int32),
-        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("F", F, torch.float64),
-        ("valid", valid, torch.uint8), ("refit", refit, torch.uint8), ("inliers_p", inliers_p, torch.uint8),
-        ("lines_consistent", lines_consistent, torch.uint8), ("n_inliers", n_inliers, torch.int32),
-        ("n_lines_consistent", n_lines_consistent, torch.int32), ("hypothesis", hypothesis, torch.int32),
-        ("hypothesis_inliers", hypothesis_inliers, torch.int32), ("key", key, torch.int64)))
-    inp = _struct(N.LtrFundamentalInput, pts0=pts0, pts1=pts1, pts_off0=pts_off0, pts_off1=pts_off1, n_pts1=n_pts1,
-                  matches_p=matches_p, cu_p=cu_p, segs0=segs0, segs1=segs1, seg_off0=seg_off0, seg_off1=seg_off1,
-                  n_segs1=n_segs1, matches_l=matches_l, cu_l=cu_l, n_pairs=int(n_pairs), max_rows_p=int(max_rows_p),
-                  max_rows_l=int(max_rows_l), thresh=float(thresh), min_overlap=float(min_overlap),
-                  n_hypotheses=int(n_hypotheses), seed=int(seed) & 0xFFFFFFFFFFFFFFFF)
-    out = _struct(N.LtrFundamentalOutput, F=F, valid=valid, refit=refit, inliers_p=inliers_p,
-                  lines_consistent=lines_consistent, n_inliers=n_inliers, n_lines_consistent=n_lines_consistent,
-                  hypothesis=hypothesis, hypothesis_inliers=hypothesis_inliers, key=key)
-    _call("ltr_fundamental", dev, C.byref(inp), C.byref(out))
-
-
-def absolute_pose(n_pairs, n_groups, *, pts0, pts_off0, matches_p, cu_p, X1, x_off1, n_x1, segs0, seg_off0, matches_l,
-                  cu_l, L1, l_off1, n_l1, groups, K0, max_rows_p, max_rows_l, R, t, valid, refit, inliers_p, inliers_l,
-                  n_inliers_p, n_inliers_l, hypothesis, hypothesis_inliers, key, thresh=8.0, n_hypotheses=1024, seed=0,
-                  use_lines=True):
-    """ltr_absolute_pose into caller-allocated outputs: query keypoint pool [*,2] / segment pool [*,2,2] fp32 with
-    per-pair first rows, world points X1 [*,3] / end points L1 [*,2,3] fp64 with per-pair first rows and counts int32
-    [P], match rows int32 with offsets cu_p / cu_l [P+1], group offsets int32 [G+1], K0 fp64 [G,3,3]; R [G,3,3] / t
-    [G,3] fp64, valid / refit [G] uint8, inliers_p / inliers_l uint8 aligned with the match rows, counts / hypothesis
-    int32 [G], key [G] int64 workspace."""
-    _req_cuda(R, "R")
-    dev = R.device
-    _check_tensors("absolute_pose", dev, (
-        ("pts0", pts0, torch.float32), ("pts_off0", pts_off0, torch.int32), ("matches_p", matches_p, torch.int32),
-        ("cu_p", cu_p, torch.int32), ("X1", X1, torch.float64), ("x_off1", x_off1, torch.int32),
-        ("n_x1", n_x1, torch.int32), ("segs0", segs0, torch.float32), ("seg_off0", seg_off0, torch.int32),
-        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("L1", L1, torch.float64),
-        ("l_off1", l_off1, torch.int32), ("n_l1", n_l1, torch.int32), ("groups", groups, torch.int32),
-        ("K0", K0, torch.float64), ("R", R, torch.float64), ("t", t, torch.float64), ("valid", valid, torch.uint8),
-        ("refit", refit, torch.uint8), ("inliers_p", inliers_p, torch.uint8), ("inliers_l", inliers_l, torch.uint8),
-        ("n_inliers_p", n_inliers_p, torch.int32), ("n_inliers_l", n_inliers_l, torch.int32),
-        ("hypothesis", hypothesis, torch.int32), ("hypothesis_inliers", hypothesis_inliers, torch.int32),
-        ("key", key, torch.int64)))
-    inp = _struct(N.LtrAbsPoseInput, pts0=pts0, pts_off0=pts_off0, matches_p=matches_p, cu_p=cu_p, X1=X1,
-                  x_off1=x_off1, n_x1=n_x1, segs0=segs0, seg_off0=seg_off0, matches_l=matches_l, cu_l=cu_l, L1=L1,
-                  l_off1=l_off1, n_l1=n_l1, groups=groups, K0=K0, n_pairs=int(n_pairs), n_groups=int(n_groups),
-                  max_rows_p=int(max_rows_p), max_rows_l=int(max_rows_l), thresh=float(thresh),
-                  n_hypotheses=int(n_hypotheses), seed=int(seed) & 0xFFFFFFFFFFFFFFFF, use_lines=int(bool(use_lines)))
-    out = _struct(N.LtrAbsPoseOutput, R=R, t=t, valid=valid, refit=refit, inliers_p=inliers_p, inliers_l=inliers_l,
-                  n_inliers_p=n_inliers_p, n_inliers_l=n_inliers_l, hypothesis=hypothesis,
-                  hypothesis_inliers=hypothesis_inliers, key=key)
-    _call("ltr_absolute_pose", dev, C.byref(inp), C.byref(out))
-
-
-def triangulate(*, kpts, kp_off, segs, seg_off, K, R, t, pairs, matches_p, cu_p, matches_l, cu_l, views, view_off,
-                block_off, inv_off_p, inv_off_l, n_images, n_pairs, total_p, total_l, n_inv_p, n_inv_l, n_blocks,
-                max_views, points3d, lines3d, n_views_p, n_views_l, inv_p, inv_l, thresh=4.0, min_angle=1.5,
-                min_views=2):
-    """ltr_triangulate into caller-allocated outputs: keypoint pool [*,2] / key-line pool [*,2,2] fp32 with image
-    offsets [n+1], K / R [n,3,3] and t [n,3] fp64, pairs [P,2] and match rows int32 with offsets cu_p / cu_l [P+1],
-    the observation lists (views, view_off), the block table block_off [2n+1] and the side-1 index offsets inv_off_*
-    [P+1] int32; points3d [*,3] / lines3d [*,2,3] fp64, n_views_p / n_views_l int32, inv_p / inv_l int32 workspace."""
-    _req_cuda(points3d, "points3d")
-    dev = points3d.device
-    _check_tensors("triangulate", dev, (
-        ("kpts", kpts, torch.float32), ("kp_off", kp_off, torch.int32), ("segs", segs, torch.float32),
-        ("seg_off", seg_off, torch.int32), ("K", K, torch.float64), ("R", R, torch.float64), ("t", t, torch.float64),
-        ("pairs", pairs, torch.int32), ("matches_p", matches_p, torch.int32), ("cu_p", cu_p, torch.int32),
-        ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32), ("views", views, torch.int32),
-        ("view_off", view_off, torch.int32), ("block_off", block_off, torch.int32),
-        ("inv_off_p", inv_off_p, torch.int32), ("inv_off_l", inv_off_l, torch.int32),
-        ("points3d", points3d, torch.float64), ("lines3d", lines3d, torch.float64),
-        ("n_views_p", n_views_p, torch.int32), ("n_views_l", n_views_l, torch.int32), ("inv_p", inv_p, torch.int32),
-        ("inv_l", inv_l, torch.int32)))
-    inp = _struct(N.LtrTriangulateInput, kpts=kpts, kp_off=kp_off, segs=segs, seg_off=seg_off, K=K, R=R, t=t,
-                  pairs=pairs, matches_p=matches_p, cu_p=cu_p, matches_l=matches_l, cu_l=cu_l, views=views,
-                  view_off=view_off, block_off=block_off, inv_off_p=inv_off_p, inv_off_l=inv_off_l,
-                  n_images=int(n_images), n_pairs=int(n_pairs), total_p=int(total_p), total_l=int(total_l),
-                  n_inv_p=int(n_inv_p), n_inv_l=int(n_inv_l), n_blocks=int(n_blocks), max_views=int(max_views),
-                  thresh=float(thresh), min_angle=float(min_angle), min_views=int(min_views))
-    out = _struct(N.LtrTriangulateOutput, points3d=points3d, lines3d=lines3d, n_views_p=n_views_p, n_views_l=n_views_l,
-                  inv_p=inv_p, inv_l=inv_l)
-    _call("ltr_triangulate", dev, C.byref(inp), C.byref(out))
-
-
-_TRACK_OUTPUTS = (("track_p", torch.int32), ("track_l", torch.int32), ("n_tracks_p", torch.int32),
-                  ("n_tracks_l", torch.int32), ("track_off_p", torch.int32), ("track_off_l", torch.int32),
-                  ("obs_p", torch.int32), ("obs_l", torch.int32), ("points3d", torch.float64),
-                  ("lines3d", torch.float64), ("n_obs_p", torch.int32), ("n_obs_l", torch.int32),
-                  ("n_inliers_p", torch.int32), ("n_inliers_l", torch.int32), ("n_images_p", torch.int32),
-                  ("n_images_l", torch.int32), ("status_p", torch.int32), ("status_l", torch.int32),
-                  ("inlier_p", torch.uint8), ("inlier_l", torch.uint8), ("row_points3d", torch.float64),
-                  ("row_lines3d", torch.float64), ("n_views_p", torch.int32), ("n_views_l", torch.int32),
-                  ("workspace", torch.int32))
-
-
-def tracks(*, kpts, kp_off, segs, seg_off, K, R, t, F, pairs, matches_p, cu_p, matches_l, cu_l, n_images, n_pairs,
-           total_p, total_l, n_kp, n_kl, outputs: dict, thresh=4.0, min_angle=1.5, min_views=2, epi_thresh=4.0,
-           min_overlap=0.5):
-    """ltr_tracks into caller-allocated outputs: keypoint pool [*,2] / key-line pool [*,2,2] fp32 with image offsets
-    [n+1], K / R [n,3,3], t [n,3] and the pairs' pixel fundamental matrices F [P,3,3] fp64, pairs [P,2] and match rows
-    int32 with offsets cu_p / cu_l [P+1]; outputs {name: tensor} holds every LtrTracksOutput field (int32 workspace of
-    5 (n_kp + n_kl))."""
-    dev = outputs["workspace"].device
-    _req_cuda(outputs["workspace"], "workspace")
-    _check_tensors("tracks", dev, (
-        ("kpts", kpts, torch.float32), ("kp_off", kp_off, torch.int32), ("segs", segs, torch.float32),
-        ("seg_off", seg_off, torch.int32), ("K", K, torch.float64), ("R", R, torch.float64), ("t", t, torch.float64),
-        ("F", F, torch.float64), ("pairs", pairs, torch.int32), ("matches_p", matches_p, torch.int32),
-        ("cu_p", cu_p, torch.int32), ("matches_l", matches_l, torch.int32), ("cu_l", cu_l, torch.int32))
-        + tuple((nm, outputs[nm], dt) for nm, dt in _TRACK_OUTPUTS))
-    if outputs["workspace"].numel() < 5 * (int(n_kp) + int(n_kl)):
-        raise N.LtrError("tracks: the workspace must hold 5 (n_kp + n_kl) int32")
-    inp = _struct(N.LtrTracksInput, kpts=kpts, kp_off=kp_off, segs=segs, seg_off=seg_off, K=K, R=R, t=t, F=F,
-                  pairs=pairs, matches_p=matches_p, cu_p=cu_p, matches_l=matches_l, cu_l=cu_l, n_images=int(n_images),
-                  n_pairs=int(n_pairs), total_p=int(total_p), total_l=int(total_l), n_kp=int(n_kp), n_kl=int(n_kl),
-                  thresh=float(thresh), min_angle=float(min_angle), min_views=int(min_views),
-                  epi_thresh=float(epi_thresh), min_overlap=float(min_overlap))
-    out = _struct(N.LtrTracksOutput, **{nm: outputs[nm] for nm, _ in _TRACK_OUTPUTS})
-    _call("ltr_tracks", dev, C.byref(inp), C.byref(out))
-
-
-_BUNDLE_INPUTS = (("kpts", torch.float32), ("kp_off", torch.int32), ("segs", torch.float32), ("seg_off", torch.int32),
-                  ("K", torch.float64), ("R", torch.float64), ("t", torch.float64), ("hold", torch.int32),
-                  ("fixed", torch.int32), ("n_tracks_p", torch.int32), ("n_tracks_l", torch.int32),
-                  ("track_off_p", torch.int32), ("track_off_l", torch.int32), ("obs_p", torch.int32),
-                  ("obs_l", torch.int32), ("status_p", torch.int32), ("status_l", torch.int32),
-                  ("inlier_p", torch.uint8), ("inlier_l", torch.uint8), ("track_p", torch.int32),
-                  ("track_l", torch.int32), ("n_views_p", torch.int32), ("n_views_l", torch.int32),
-                  ("points3d", torch.float64), ("lines3d", torch.float64))
-_BUNDLE_OUTPUTS = (("R", torch.float64), ("t", torch.float64), ("points3d", torch.float64), ("lines3d", torch.float64),
-                   ("status_p", torch.int32), ("status_l", torch.int32), ("residual_p", torch.float64),
-                   ("residual_l", torch.float64), ("row_points3d", torch.float64), ("row_lines3d", torch.float64),
-                   ("n_views_p", torch.int32), ("n_views_l", torch.int32), ("stats", torch.float64),
-                   ("workspace", torch.float64))
-
-
-def bundle_adjust(*, inputs: dict, outputs: dict, n_images, n_fixed, n_kp, n_kl, t_p, t_l, max_iters=50, ftol=1e-10):
-    """ltr_bundle_adjust into caller-allocated outputs: inputs {name: tensor} holds every LtrBundleInput pointer field
-    (the set's rows and cameras, the held coordinates and fixed flags, and the ltr_tracks outputs), outputs every
-    LtrBundleOutput field (an fp64 workspace of at least LTR_BA_WORKSPACE_BYTES)."""
-    dev = outputs["workspace"].device
-    _req_cuda(outputs["workspace"], "workspace")
-    _check_tensors("bundle_adjust", dev, tuple((nm, inputs[nm], dt) for nm, dt in _BUNDLE_INPUTS)
-                   + tuple((nm, outputs[nm], dt) for nm, dt in _BUNDLE_OUTPUTS))
-    if outputs["workspace"].numel() * 8 < N.ba_workspace_bytes(n_images, n_kp, n_kl, t_p, t_l):
-        raise N.LtrError("bundle_adjust: the workspace is smaller than LTR_BA_WORKSPACE_BYTES")
-    inp = _struct(N.LtrBundleInput, **{nm: inputs[nm] for nm, _ in _BUNDLE_INPUTS}, n_images=int(n_images),
-                  n_fixed=int(n_fixed), n_kp=int(n_kp), n_kl=int(n_kl), t_p=int(t_p), t_l=int(t_l),
-                  max_iters=int(max_iters), ftol=float(ftol))
-    out = _struct(N.LtrBundleOutput, **{nm: outputs[nm] for nm, _ in _BUNDLE_OUTPUTS})
-    _call("ltr_bundle_adjust", dev, C.byref(inp), C.byref(out))
-
-
-_GP_INPUTS = (("pairs", torch.int32), ("R", torch.float64), ("t", torch.float64), ("valid", torch.uint8),
-              ("n_cheirality", torch.int32))
-_GP_OUTPUTS = (("R", torch.float64), ("t", torch.float64), ("registered", torch.bool), ("edge_status", torch.int32),
-               ("support", torch.int32), ("rot_residual", torch.float64), ("dir_cos", torch.float64),
-               ("stats", torch.float64), ("workspace", torch.float64))
-
-
-def global_poses(*, inputs: dict, outputs: dict, n_images, n_pairs, min_inliers, anchor, rot_iters, pos_iters, rot_tan,
-                 dir_cos, ftol):
-    """ltr_global_poses into caller-allocated outputs: inputs {name: tensor} holds every LtrGlobalPoseInput pointer
-    field, outputs every LtrGlobalPoseOutput field (an fp64 workspace of at least LTR_GP_WORKSPACE_BYTES)."""
-    dev = outputs["workspace"].device
-    _req_cuda(outputs["workspace"], "workspace")
-    _check_tensors("global_poses", dev, tuple((nm, inputs[nm], dt) for nm, dt in _GP_INPUTS)
-                   + tuple((nm, outputs[nm], dt) for nm, dt in _GP_OUTPUTS))
-    if outputs["workspace"].numel() * 8 < N.gp_workspace_bytes(n_images, n_pairs):
-        raise N.LtrError("global_poses: the workspace is smaller than LTR_GP_WORKSPACE_BYTES")
-    inp = _struct(N.LtrGlobalPoseInput, **{nm: inputs[nm] for nm, _ in _GP_INPUTS}, n_images=int(n_images),
-                  n_pairs=int(n_pairs), min_inliers=int(min_inliers), anchor=int(anchor), rot_iters=int(rot_iters),
-                  pos_iters=int(pos_iters), rot_tan=float(rot_tan), dir_cos=float(dir_cos), ftol=float(ftol))
-    out = _struct(N.LtrGlobalPoseOutput, **{nm: outputs[nm] for nm, _ in _GP_OUTPUTS})
-    _call("ltr_global_poses", dev, C.byref(inp), C.byref(out))
+            dev = t.device if dev is None else dev
+            if (dts is not None and t.dtype not in dts) or not t.is_contiguous() or t.device != dev:
+                raise N.LtrError(f"{who}: '{nm}' must be a contiguous {f'{dts[0]} ' if dts else ''}tensor on {dev}")
+            fields[nm] = t.data_ptr()
+        for nm, conv in scalars:
+            if nm not in given:
+                raise N.LtrError(f"{who}: {cls.__name__}.{nm} is not given")
+            fields[nm] = conv(given[nm])
+        structs[cls] = cls(**fields)
+    if workspace_bytes is not None:
+        ws = outputs["workspace"]
+        if ws.numel() * ws.element_size() < workspace_bytes:
+            raise N.LtrError(f"{who}: the workspace holds {ws.numel() * ws.element_size()} bytes, {workspace_bytes} "
+                             "needed")
+    _call(entry, dev, C.byref(structs[p_in._type_]), C.byref(structs[p_out._type_]))
 
 
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):

@@ -579,12 +579,13 @@ def bundle_adjust(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters=50, 
     fx[fixed] = 1
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
     rp, rl = max(Np, 1), max(Nl, 1)
+    ws = N.ba_workspace_bytes(n, Np, Nl, Tp, Tl)
     o = dict(R=torch.empty((n, 3, 3), **f64), t=torch.empty((n, 3), **f64), points3d=torch.empty((Tp, 3), **f64),
              lines3d=torch.empty((Tl, 2, 3), **f64), status_p=torch.empty(Tp, **i32), status_l=torch.empty(Tl, **i32),
              residual_p=torch.empty(rp, **f64), residual_l=torch.empty(rl, **f64),
              row_points3d=torch.empty((rp, 3), **f64), row_lines3d=torch.empty((rl, 2, 3), **f64),
              n_views_p=torch.empty(rp, **i32), n_views_l=torch.empty(rl, **i32), stats=torch.empty(8, **f64),
-             workspace=torch.empty(-(-N.ba_workspace_bytes(n, Np, Nl, Tp, Tl) // 8), **f64))
+             workspace=torch.empty(-(-ws // 8), **f64))
     arrays = {"K": Kn, "R": Rn, "t": tn, "kp_off": offsets(np.diff(op)), "seg_off": offsets(np.diff(ol)),
               "hold": np.maximum(_hold(Rn, tn, fixed), 0).astype(np.int32), "fixed": fx}
     dv = stage_with_pools(arrays, keypoints, klines, dev)
@@ -592,7 +593,8 @@ def bundle_adjust(keypoints, klines, K, R, t, tracks, fixed=(0,), max_iters=50, 
                "inlier_p", "inlier_l", "track_p", "track_l", "n_views_p", "n_views_l", "points3d", "lines3d"):
         dv[nm] = getattr(tracks, nm).contiguous()
     dv["segs"] = dv["segs"].reshape(-1, 4)
-    _ops.bundle_adjust(inputs=dv, outputs=o, n_images=n, n_fixed=len(fixed), n_kp=Np, n_kl=Nl, t_p=Tp, t_l=Tl,
-                       max_iters=max_iters, ftol=ftol)
+    _ops.call_struct("ltr_bundle_adjust", {**dv, "n_images": n, "n_fixed": len(fixed), "n_kp": Np, "n_kl": Nl,
+                                           "t_p": Tp, "t_l": Tl, "max_iters": max_iters, "ftol": ftol},
+                     o, workspace_bytes=ws)
     del o["workspace"]     # the caching allocator reuses it only behind this stream's kernels
     return BundleResult(**o, offsets_p=op, offsets_l=ol)

@@ -213,10 +213,12 @@ def _run(b, layout, match_thr, unmatch_thr, pred0) -> TripletLoss:
             raise N.LtrError(f"triplet_loss: pred0 must be a CUDA tensor [{int(b['n0'].sum())}]")
         pred0 = pred0.to(device=dev, dtype=torch.int32).contiguous()
         tfpn = torch.zeros((b["P"], 4), **i32)
-    _ops.triplet_loss(b["d0"], b["d1"], layout, b["P"], assign=b["assign"], assign_stride=b["stride"],
-                      n0=b["u0"] or 0, n1=b["u1"] or 0, cu0=b["cu0"], cu1=b["cu1"], max_n0=b["mx0"], max_n1=b["mx1"],
-                      assign_ld=b["ld"], match_thr=match_thr, unmatch_thr=unmatch_thr, pred0=pred0, tfpn=tfpn,
-                      n_groups=G, group_off=b["group_off"], **out)
+    _ops.call_struct("ltr_triplet_loss",
+                     dict(desc0=b["d0"], desc1=b["d1"], layout=layout, d=256, n_pairs=b["P"], n0=b["u0"] or 0,
+                          n1=b["u1"] or 0, cu0=b["cu0"], cu1=b["cu1"], max_n0=b["mx0"], max_n1=b["mx1"],
+                          assign=b["assign"], assign_stride=b["stride"], assign_ld=b["ld"], match_thr=match_thr,
+                          unmatch_thr=unmatch_thr, pred0=pred0, n_groups=G, group_off=b["group_off"]),
+                     dict(out, tfpn=tfpn))
     return TripletLoss(tfpn=tfpn, n0=b["n0"], n1=b["n1"], groups=b["groups"], **out)
 
 

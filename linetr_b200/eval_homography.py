@@ -239,7 +239,8 @@ def homography_ground_truth(segs0, segs1, cu0, cu1, homographies, pred0=None, wa
     if device is None:
         device = next((t.device for t in devs.values()), None) or _ops.current_cuda_device()
     device = torch.device(device)
-    dv = _ops.stage({**host, "cu0": c0, "cu1": c1, "H": hs, "Hinv": np.ascontiguousarray(hinv)}, device)
+    dv = _ops.stage({**host, "cu0": c0, "cu1": c1, "homography": hs, "homography_inv": np.ascontiguousarray(hinv)},
+                    device)
     dv.update(devs)
     n0, n1 = np.diff(c0), np.diff(c1)
     mx0, mx1 = int(n0.max(initial=0)), int(n1.max(initial=0))
@@ -254,10 +255,10 @@ def homography_ground_truth(segs0, segs1, cu0, cu1, homographies, pred0=None, wa
         proj0 = proj0.float().contiguous()
     if proj1 is not None:
         proj1 = proj1.float().contiguous()
-    _ops.line_gt(dv["segs0"], dv["segs1"], P, cu0=dv["cu0"], cu1=dv["cu1"], max_n0=mx0, max_n1=mx1, homography=dv["H"],
-                 homography_inv=dv["Hinv"], n_gt=counts, assign=assign, assign_stride=stride, pred0=pred0, tfpn=tfpn,
-                 proj0=proj0, proj1=proj1, thres_reprojected=thres_reprojected, thres_angdiff=thres_angdiff,
-                 min_overlap_ratio=min_overlap_ratio)
+    _ops.call_struct("ltr_line_gt", {**dv, "proj0": proj0, "proj1": proj1, "pred0": pred0, "n_pairs": P,
+                                     "max_n0": mx0, "max_n1": mx1, "thres_reprojected": thres_reprojected,
+                                     "thres_angdiff": thres_angdiff, "min_overlap_ratio": min_overlap_ratio},
+                     dict(assign=assign, assign_stride=stride, n_gt=counts, tfpn=tfpn))
     return LineGroundTruth(counts, tfpn, assign, stride, n0, n1, float(min_overlap_ratio))
 
 

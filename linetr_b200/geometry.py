@@ -344,6 +344,39 @@ def _pool(items, P, to_rows):
     return parts, off, cnt
 
 
+def _stage_pairs(res, dev, who, lines, extra=None) -> dict:
+    """The pair estimators' inputs of `res`: its side-0 / side-1 keypoints and, with `lines`, key lines (float32
+    segments) pooled by `_pool`, their pool offsets and side-1 counts, the match offsets and the `extra` host arrays in
+    one pinned copy.  -> device tensors and row bounds by input-struct field name (pts0 / pts1, pts_off0 / pts_off1,
+    n_pts1, matches_p, cu_p, max_rows_p, with lines the same for segs, and the `extra` names)."""
+    P = res.n_pairs
+    op = np.asarray(res.offsets_p, dtype=np.int64)
+    pt_rows = lambda k: torch.as_tensor(k).to(device=dev, dtype=torch.float32).reshape(-1, 2)
+    p0, poff0, pn0 = _pool(res.keypoints0, P, pt_rows)
+    p1, poff1, pn1 = _pool(res.keypoints1, P, pt_rows)
+    arrays = {**(extra or {}), "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1,
+              "cu_p": np.ascontiguousarray(op, dtype=np.int32)}
+    agree = np.array_equal(pn0, np.diff(op))
+    if lines:
+        ol = np.asarray(res.offsets_l, dtype=np.int64)
+        seg_rows = lambda k: np.asarray(k, dtype=np.float32).reshape(-1, 4)
+        s0, soff0, sn0 = _pool(res.klines0, P, seg_rows)
+        s1, soff1, sn1 = _pool(res.klines1, P, seg_rows)
+        agree &= np.array_equal(sn0, np.diff(ol))
+        cat_np = lambda parts: np.concatenate(parts) if parts else np.zeros((0, 4), dtype=np.float32)
+        arrays.update(segs0=cat_np(s0), segs1=cat_np(s1), seg_off0=soff0, seg_off1=soff1, n_segs1=sn1,
+                      cu_l=np.ascontiguousarray(ol, dtype=np.int32))
+    if not agree:
+        raise N.LtrError(f"{who}: side-0 {'key lines / ' if lines else ''}keypoints and the match offsets disagree")
+    dv = _ops.stage(arrays, dev)
+    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
+    dv.update(pts0=cat_t(p0).contiguous(), pts1=cat_t(p1).contiguous(), matches_p=res.matches_p.contiguous(),
+              max_rows_p=int(np.diff(op).max(initial=0)))
+    if lines:
+        dv.update(matches_l=res.matches_l.contiguous(), max_rows_l=int(np.diff(ol).max(initial=0)))
+    return dv
+
+
 def estimate_homographies(res, thresh=3.0, n_hypotheses=2048, seed=0, use_lines=True, use_points=True) -> HomographyResult:
     """RANSAC homographies (image 0 -> image 1) of every pair of an `ImagePairMatches` (`match_images`, `match_sets`)
     from its line matches (res.klines0 / klines1 as float32 segments) and point matches (res.keypoints0 / keypoints1),
@@ -352,37 +385,17 @@ def estimate_homographies(res, thresh=3.0, n_hypotheses=2048, seed=0, use_lines=
     rows than one CTA can stage (SMEM_PER_POINT / SMEM_PER_LINE bytes per row, SMEM_MAX in all)."""
     P = res.n_pairs
     dev = res.matches_l.device
-    op, ol = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
     if int(n_hypotheses) < 1:
         raise N.LtrError("estimate_homographies: n_hypotheses must be >= 1")
-    seg_rows = lambda k: np.asarray(k, dtype=np.float32).reshape(-1, 4)
-    pt_rows = lambda k: torch.as_tensor(k).to(device=dev, dtype=torch.float32).reshape(-1, 2)
-    s0, soff0, sn0 = _pool(res.klines0, P, seg_rows)
-    s1, soff1, sn1 = _pool(res.klines1, P, seg_rows)
-    p0, poff0, pn0 = _pool(res.keypoints0, P, pt_rows)
-    p1, poff1, pn1 = _pool(res.keypoints1, P, pt_rows)
-    if not (np.array_equal(sn0, np.diff(ol)) and np.array_equal(pn0, np.diff(op))):
-        raise N.LtrError("estimate_homographies: side-0 key lines / keypoints and the match offsets disagree")
-    cat_np = lambda parts: np.concatenate(parts) if parts else np.zeros((0, 4), dtype=np.float32)
-    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
-    i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
-    dv = _ops.stage({"segs0": cat_np(s0), "segs1": cat_np(s1), "seg_off0": soff0, "seg_off1": soff1, "n_segs1": sn1,
-                      "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1, "cu_p": i32(op), "cu_l": i32(ol)}, dev)
+    dv = _stage_pairs(res, dev, "estimate_homographies", lines=True)
     u8, i32d = dict(dtype=torch.uint8, device=dev), dict(dtype=torch.int32, device=dev)
     out = HomographyResult(torch.empty((P, 3, 3), dtype=torch.float64, device=dev), torch.empty(P, **u8),
                            torch.empty(res.matches_l.shape[0], **u8), torch.empty(res.matches_p.shape[0], **u8),
                            torch.empty(P, **i32d), torch.empty(P, **i32d), torch.empty(P, **i32d),
                            torch.empty(P, **i32d))
-    key = torch.empty(P, dtype=torch.int64, device=dev)
-    mx = lambda a: int(np.diff(a).max(initial=0))
-    _ops.homography(P, pts0=cat_t(p0).contiguous(), pts1=cat_t(p1).contiguous(), pts_off0=dv["pts_off0"],
-                    pts_off1=dv["pts_off1"], n_pts1=dv["n_pts1"], matches_p=res.matches_p.contiguous(), cu_p=dv["cu_p"],
-                    max_rows_p=mx(op), segs0=dv["segs0"], segs1=dv["segs1"], seg_off0=dv["seg_off0"],
-                    seg_off1=dv["seg_off1"], n_segs1=dv["n_segs1"], matches_l=res.matches_l.contiguous(),
-                    cu_l=dv["cu_l"], max_rows_l=mx(ol), H=out.H, valid=out.valid, inliers_p=out.inliers_p,
-                    inliers_l=out.inliers_l, n_inliers_p=out.n_inliers_p, n_inliers_l=out.n_inliers_l,
-                    hypothesis=out.hypothesis, hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh,
-                    n_hypotheses=n_hypotheses, seed=seed, use_points=use_points, use_lines=use_lines)
+    _ops.call_struct("ltr_homography", {**dv, "n_pairs": P, "thresh": thresh, "n_hypotheses": n_hypotheses,
+                                        "seed": seed, "use_points": use_points, "use_lines": use_lines},
+                     {**vars(out), "key": torch.empty(P, dtype=torch.int64, device=dev)})
     out.valid = out.valid.view(torch.bool)
     return out
 
@@ -877,30 +890,19 @@ def estimate_poses(res, K0, K1, thresh=1.0, n_hypotheses=1024, seed=0, dist_thre
     per row, SMEM_MAX in all)."""
     P = res.n_pairs
     dev = res.matches_p.device
-    op = np.asarray(res.offsets_p, dtype=np.int64)
     if int(n_hypotheses) < 1:
         raise N.LtrError("estimate_poses: n_hypotheses must be >= 1")
     k0, k1 = _intrinsics(K0, P, "K0"), _intrinsics(K1, P, "K1")
-    pt_rows = lambda k: torch.as_tensor(k).to(device=dev, dtype=torch.float32).reshape(-1, 2)
-    p0, poff0, pn0 = _pool(res.keypoints0, P, pt_rows)
-    p1, poff1, pn1 = _pool(res.keypoints1, P, pt_rows)
-    if not np.array_equal(pn0, np.diff(op)):
-        raise N.LtrError("estimate_poses: side-0 keypoints and the match offsets disagree")
-    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
-    dv = _ops.stage({"K0": k0, "K1": k1, "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1,
-                      "cu_p": np.ascontiguousarray(op, dtype=np.int32)}, dev)
+    dv = _stage_pairs(res, dev, "estimate_poses", lines=False, extra={"K0": k0, "K1": k1})
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
     out = PoseResult(torch.empty((P, 3, 3), **f64), torch.empty((P, 3, 3), **f64), torch.empty((P, 3), **f64),
                      torch.empty(P, dtype=torch.uint8, device=dev),
                      torch.empty(res.matches_p.shape[0], dtype=torch.uint8, device=dev),
                      torch.empty(P, **i32), torch.empty(P, **i32), torch.empty(P, **i32), torch.empty(P, **i32))
-    key = torch.empty(P, dtype=torch.int64, device=dev)
-    _ops.essential(P, pts0=cat_t(p0).contiguous(), pts1=cat_t(p1).contiguous(), pts_off0=dv["pts_off0"],
-                   pts_off1=dv["pts_off1"], n_pts1=dv["n_pts1"], matches_p=res.matches_p.contiguous(), cu_p=dv["cu_p"],
-                   max_rows_p=int(np.diff(op).max(initial=0)), K0=dv["K0"], K1=dv["K1"], E=out.E, R=out.R, t=out.t,
-                   valid=out.valid, inliers_p=out.inliers, n_inliers=out.n_inliers, n_cheirality=out.n_cheirality,
-                   hypothesis=out.hypothesis, hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh,
-                   dist_thresh=dist_thresh, n_hypotheses=n_hypotheses, seed=seed)
+    outputs = {**vars(out), "inliers_p": out.inliers, "key": torch.empty(P, dtype=torch.int64, device=dev)}
+    del outputs["inliers"]
+    _ops.call_struct("ltr_essential", {**dv, "n_pairs": P, "thresh": thresh, "dist_thresh": dist_thresh,
+                                       "n_hypotheses": n_hypotheses, "seed": seed}, outputs)
     out.valid = out.valid.view(torch.bool)
     return out
 
@@ -1150,38 +1152,17 @@ def estimate_fundamentals(res, thresh=3.0, n_hypotheses=2048, seed=0, min_overla
     (SMEM_PER_ROW_F bytes per row, SMEM_MAX in all)."""
     P = res.n_pairs
     dev = res.matches_p.device
-    op, ol = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
     if int(n_hypotheses) < 1:
         raise N.LtrError("estimate_fundamentals: n_hypotheses must be >= 1")
-    seg_rows = lambda k: np.asarray(k, dtype=np.float32).reshape(-1, 4)
-    pt_rows = lambda k: torch.as_tensor(k).to(device=dev, dtype=torch.float32).reshape(-1, 2)
-    s0, soff0, sn0 = _pool(res.klines0, P, seg_rows)
-    s1, soff1, sn1 = _pool(res.klines1, P, seg_rows)
-    p0, poff0, pn0 = _pool(res.keypoints0, P, pt_rows)
-    p1, poff1, pn1 = _pool(res.keypoints1, P, pt_rows)
-    if not (np.array_equal(sn0, np.diff(ol)) and np.array_equal(pn0, np.diff(op))):
-        raise N.LtrError("estimate_fundamentals: side-0 key lines / keypoints and the match offsets disagree")
-    cat_np = lambda parts: np.concatenate(parts) if parts else np.zeros((0, 4), dtype=np.float32)
-    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
-    i32 = lambda a: np.ascontiguousarray(a, dtype=np.int32)
-    dv = _ops.stage({"segs0": cat_np(s0), "segs1": cat_np(s1), "seg_off0": soff0, "seg_off1": soff1, "n_segs1": sn1,
-                      "pts_off0": poff0, "pts_off1": poff1, "n_pts1": pn1, "cu_p": i32(op), "cu_l": i32(ol)}, dev)
+    dv = _stage_pairs(res, dev, "estimate_fundamentals", lines=True)
     u8, i32d = dict(dtype=torch.uint8, device=dev), dict(dtype=torch.int32, device=dev)
     out = FundamentalResult(torch.empty((P, 3, 3), dtype=torch.float64, device=dev), torch.empty(P, **u8),
                             torch.empty(res.matches_p.shape[0], **u8), torch.empty(P, **i32d), torch.empty(P, **i32d),
                             torch.empty(P, **i32d), torch.empty(P, **u8), torch.empty(res.matches_l.shape[0], **u8),
                             torch.empty(P, **i32d))
-    key = torch.empty(P, dtype=torch.int64, device=dev)
-    mx = lambda a: int(np.diff(a).max(initial=0))
-    _ops.fundamental(P, pts0=cat_t(p0).contiguous(), pts1=cat_t(p1).contiguous(), pts_off0=dv["pts_off0"],
-                     pts_off1=dv["pts_off1"], n_pts1=dv["n_pts1"], matches_p=res.matches_p.contiguous(),
-                     cu_p=dv["cu_p"], max_rows_p=mx(op), segs0=dv["segs0"], segs1=dv["segs1"], seg_off0=dv["seg_off0"],
-                     seg_off1=dv["seg_off1"], n_segs1=dv["n_segs1"], matches_l=res.matches_l.contiguous(),
-                     cu_l=dv["cu_l"], max_rows_l=mx(ol), F=out.F, valid=out.valid, refit=out.refit,
-                     inliers_p=out.inliers_p, lines_consistent=out.lines_consistent, n_inliers=out.n_inliers,
-                     n_lines_consistent=out.n_lines_consistent, hypothesis=out.hypothesis,
-                     hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh, min_overlap=min_overlap,
-                     n_hypotheses=n_hypotheses, seed=seed)
+    _ops.call_struct("ltr_fundamental", {**dv, "n_pairs": P, "thresh": thresh, "min_overlap": min_overlap,
+                                         "n_hypotheses": n_hypotheses, "seed": seed},
+                     {**vars(out), "key": torch.empty(P, dtype=torch.int64, device=dev)})
     out.valid = out.valid.view(torch.bool)
     out.refit = out.refit.view(torch.bool)
     return out

@@ -450,14 +450,16 @@ def global_poses(pairs, poses, n_images, min_inliers=20, rot_thresh=5.0, dir_thr
     dv.update(_ops.stage(arrays, dev))
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
     pb = max(P, 1)
+    ws = N.gp_workspace_bytes(n, P)
     o = dict(R=torch.empty((n, 3, 3), **f64), t=torch.empty((n, 3), **f64),
              registered=torch.empty(n, dtype=torch.bool, device=dev), edge_status=torch.empty(pb, **i32),
              support=torch.empty(pb, **i32), rot_residual=torch.empty(pb, **f64), dir_cos=torch.empty(pb, **f64),
              stats=torch.empty(N.GP_STATS, **f64),
-             workspace=torch.empty(-(-N.gp_workspace_bytes(n, P) // 8), **f64))
-    _ops.global_poses(inputs=dv, outputs=o, n_images=n, n_pairs=P, min_inliers=int(min_inliers),
-                      anchor=-1 if anchor is None else anchor, rot_iters=int(rot_iters), pos_iters=int(pos_iters),
-                      rot_tan=tan_rot, dir_cos=cos_dir, ftol=float(ftol))
+             workspace=torch.empty(-(-ws // 8), **f64))
+    _ops.call_struct("ltr_global_poses", {**dv, "n_images": n, "n_pairs": P, "min_inliers": min_inliers,
+                                          "anchor": -1 if anchor is None else anchor, "rot_iters": rot_iters,
+                                          "pos_iters": pos_iters, "rot_tan": tan_rot, "dir_cos": cos_dir, "ftol": ftol},
+                     o, workspace_bytes=ws)
     del o["workspace"]     # the caching allocator reuses it only behind this stream's kernels
     for k in ("edge_status", "support", "rot_residual", "dir_cos"):
         o[k] = o[k][:P]

@@ -494,18 +494,13 @@ def estimate_absolute_poses(res, K0, points3d1, lines3d1=None, groups=None, thre
                              torch.empty(G_, **u8), torch.empty(res.matches_p.shape[0], **u8),
                              torch.empty(res.matches_l.shape[0], **u8), torch.empty(G_, **i32), torch.empty(G_, **i32),
                              torch.empty(G_, **i32), torch.empty(G_, **i32))
-    key = torch.empty(G_, dtype=torch.int64, device=dev)
-    cat_t = lambda parts: torch.cat(parts) if parts else torch.zeros((0, 2), dtype=torch.float32, device=dev)
-    _ops.absolute_pose(P, G_, pts0=cat_t(p0).contiguous(), pts_off0=dv["pts_off0"], matches_p=res.matches_p.contiguous(),
-                       cu_p=dv["cu_p"], X1=dv["X1"], x_off1=dv["x_off1"], n_x1=dv["n_x1"], segs0=dv.get("segs0"),
-                       seg_off0=dv.get("seg_off0"), matches_l=res.matches_l.contiguous(),
-                       cu_l=dv["cu_l"], L1=dv.get("L1"), l_off1=dv.get("l_off1"), n_l1=dv.get("n_l1"),
-                       groups=dv["groups"], K0=dv["K0"], max_rows_p=int((op[gr[1:]] - op[gr[:-1]]).max(initial=0)),
-                       max_rows_l=rows_l, R=out.R, t=out.t, valid=out.valid, refit=out.refit,
-                       inliers_p=out.inliers_p, inliers_l=out.inliers_l,
-                       n_inliers_p=out.n_inliers_p, n_inliers_l=out.n_inliers_l, hypothesis=out.hypothesis,
-                       hypothesis_inliers=out.hypothesis_inliers, key=key, thresh=thresh, n_hypotheses=n_hypotheses,
-                       seed=seed, use_lines=lines)
+    pts0 = torch.cat(p0) if p0 else torch.zeros((0, 2), dtype=torch.float32, device=dev)
+    _ops.call_struct("ltr_absolute_pose",
+                     {**dv, "pts0": pts0.contiguous(), "matches_p": res.matches_p.contiguous(),
+                      "matches_l": res.matches_l.contiguous(), "n_pairs": P, "n_groups": G_,
+                      "max_rows_p": int((op[gr[1:]] - op[gr[:-1]]).max(initial=0)), "max_rows_l": rows_l,
+                      "thresh": thresh, "n_hypotheses": n_hypotheses, "seed": seed, "use_lines": lines},
+                     {**vars(out), "key": torch.empty(G_, dtype=torch.int64, device=dev)})
     out.valid = out.valid.view(torch.bool)
     out.refit = out.refit.view(torch.bool)
     return out

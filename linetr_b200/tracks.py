@@ -512,11 +512,12 @@ def triangulate_tracks(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_a
                   "cu_p": np.asarray(res.offsets_p, dtype=np.int32), "cu_l": np.asarray(res.offsets_l, dtype=np.int32),
                   "kp_off": op, "seg_off": ol}
         dv = stage_with_pools(arrays, keypoints, klines, dev)
-        _ops.tracks(kpts=dv["kpts"], kp_off=dv["kp_off"], segs=dv["segs"], seg_off=dv["seg_off"], K=dv["K"],
-                    R=dv["R"], t=dv["t"], F=dv["F"], pairs=dv["pairs"], matches_p=res.matches_p.contiguous(),
-                    cu_p=dv["cu_p"], matches_l=res.matches_l.contiguous(), cu_l=dv["cu_l"], n_images=n, n_pairs=P,
-                    total_p=int(res.offsets_p[-1]), total_l=int(res.offsets_l[-1]), n_kp=Np, n_kl=Nl, outputs=o,
-                    thresh=thresh, min_angle=min_angle, min_views=min_views, epi_thresh=epi_thresh,
-                    min_overlap=min_overlap)
+        _ops.call_struct("ltr_tracks",
+                         {**dv, "matches_p": res.matches_p.contiguous(), "matches_l": res.matches_l.contiguous(),
+                          "n_images": n, "n_pairs": P, "total_p": int(res.offsets_p[-1]),
+                          "total_l": int(res.offsets_l[-1]), "n_kp": Np, "n_kl": Nl, "thresh": thresh,
+                          "min_angle": min_angle, "min_views": min_views, "epi_thresh": epi_thresh,
+                          "min_overlap": min_overlap},
+                         o, workspace_bytes=4 * 5 * (Np + Nl))
     del o["workspace"]     # the caching allocator reuses it only behind this stream's kernels
     return TrackResult(**o, offsets_p=op.astype(np.int64), offsets_l=ol.astype(np.int64))

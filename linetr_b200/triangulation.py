@@ -318,13 +318,12 @@ def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.
     dv = stage_with_pools(arrays, keypoints, klines, dev)
     inv_p = torch.empty(max(int(inv_off_p[-1]), 1), **i32)
     inv_l = torch.empty(max(int(inv_off_l[-1]), 1), **i32)
-    _ops.triangulate(kpts=dv["kpts"], kp_off=dv["kp_off"], segs=dv["segs"], seg_off=dv["seg_off"], K=dv["K"],
-                     R=dv["R"], t=dv["t"], pairs=dv["pairs"], matches_p=res.matches_p.contiguous(), cu_p=dv["cu_p"],
-                     matches_l=res.matches_l.contiguous(), cu_l=dv["cu_l"], views=dv["views"],
-                     view_off=dv["view_off"], block_off=dv["block_off"], inv_off_p=dv["inv_off_p"],
-                     inv_off_l=dv["inv_off_l"], n_images=n, n_pairs=P, total_p=int(res.offsets_p[-1]),
-                     total_l=int(res.offsets_l[-1]), n_inv_p=int(inv_off_p[-1]), n_inv_l=int(inv_off_l[-1]),
-                     n_blocks=int(block_off[-1]), max_views=int(np.diff(S.view_off).max(initial=0)),
-                     points3d=out.points3d, lines3d=out.lines3d, n_views_p=out.n_views_p, n_views_l=out.n_views_l,
-                     inv_p=inv_p, inv_l=inv_l, thresh=thresh, min_angle=min_angle, min_views=min_views)
+    _ops.call_struct("ltr_triangulate",
+                     {**dv, "matches_p": res.matches_p.contiguous(), "matches_l": res.matches_l.contiguous(),
+                      "n_images": n, "n_pairs": P, "total_p": int(res.offsets_p[-1]), "total_l": int(res.offsets_l[-1]),
+                      "n_inv_p": int(inv_off_p[-1]), "n_inv_l": int(inv_off_l[-1]), "n_blocks": int(block_off[-1]),
+                      "max_views": int(np.diff(S.view_off).max(initial=0)), "thresh": thresh,
+                      "min_angle": min_angle, "min_views": min_views},
+                     dict(points3d=out.points3d, lines3d=out.lines3d, n_views_p=out.n_views_p,
+                          n_views_l=out.n_views_l, inv_p=inv_p, inv_l=inv_l))
     return out

@@ -1,7 +1,7 @@
 """The ctypes mirror of the C ABI (linetr_b200/_native.py) against include/linetr_b200.h and
-include/linetr_b200_debug.h: every struct's fields, widths, offsets and size, every ltr_* prototype's argument and
-return types, and every constant the binding repeats.  A mismatch would otherwise only show as garbage read on the
-GPU.  CPU only; offsets, sizes and macro values come from the host C compiler and are skipped without one."""
+include/linetr_b200_debug.h: every struct's fields, widths, pointee types, offsets and size, every ltr_* prototype's
+argument and return types, and every constant the binding repeats.  A mismatch would otherwise only show as garbage
+read on the GPU.  CPU only; offsets, sizes and macro values come from the host C compiler and are skipped without one."""
 import ctypes as C
 import os
 import re
@@ -16,8 +16,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 INCLUDE = os.path.join(ROOT, "include")
 HEADERS = ("linetr_b200.h", "linetr_b200_debug.h")
 # what the ABI fixes of a C scalar type: integer or floating point, and its width
-SCALARS = {"int": "int32", "int32_t": "int32", "int64_t": "int64", "uint64_t": "int64", "float": "float32",
-           "double": "float64"}
+SCALARS = {"int": "int32", "int32_t": "int32", "int64_t": "int64", "uint64_t": "int64", "uint8_t": "int8",
+           "float": "float32", "double": "float64"}
 WORKSPACE_SIZES = ((0, 0, 0), (1, 480, 640), (256, 480, 640), (3, 7, 5), (1000, 1200, 1600))   # the last > 2^31
 
 
@@ -39,6 +39,13 @@ def _kind(c_type, declarator=""):
     return None if t == "void" else SCALARS[t]
 
 
+def _pointee(c_type, declarator):
+    """SCALARS[T] of a `[const] T*` declaration with a scalar T, else None (void*, char*, struct pointers, pointers to
+    pointers and arrays)."""
+    t = " ".join(w for w in c_type.split() if w not in ("const", "struct"))
+    return SCALARS.get(t) if declarator.count("*") == 1 and "[" not in declarator else None
+
+
 def _ctype_kind(t):
     if t is None:
         return None
@@ -47,18 +54,29 @@ def _ctype_kind(t):
     return ("float" if t._type_ in "fdg" else "int") + str(8 * C.sizeof(t))
 
 
+def _ctype_pointee(st, f, t):
+    """The kind of what field f of mirror st (type t) points to: its tag in st._pointees_ (_native.F32P ...) or c_T of
+    POINTER(c_T), else None."""
+    if f in getattr(st, "_pointees_", {}):
+        return _ctype_kind(st._pointees_[f])
+    if issubclass(t, C._Pointer) and issubclass(t._type_, C._SimpleCData):
+        return _ctype_kind(t._type_)
+    return None
+
+
 def _declarators(decl):
-    """'const int32_t* a, b[4]' -> [('a', kind), ('b', kind)]."""
+    """'const int32_t* a, b[4]' -> [('a', kind, pointee), ('b', kind, pointee)]."""
     m = re.fullmatch(r"\s*((?:const\s+|struct\s+|unsigned\s+|long\s+)*\w+)(.*?)\s*", decl, re.S)
     out = []
     for d in m.group(2).split(","):
         p = re.fullmatch(r"([\s*]*(?:const\s*\*?\s*)*)(\w+)\s*(\[\w*\])?\s*", d)
-        out.append((p.group(2), _kind(m.group(1), p.group(1) + (p.group(3) or ""))))
+        declarator = p.group(1) + (p.group(3) or "")
+        out.append((p.group(2), _kind(m.group(1), declarator), _pointee(m.group(1), declarator)))
     return out
 
 
 def _structs():
-    """{name: [(field, kind)]} of every `typedef struct {...} Name;` of the headers, fields in order."""
+    """{name: [(field, kind, pointee)]} of every `typedef struct {...} Name;` of the headers, fields in order."""
     out = {}
     for h in HEADERS:
         for body, name in re.findall(r"typedef\s+struct\s*\{([^{}]*)\}\s*(\w+)\s*;", _text(h)):
@@ -74,7 +92,7 @@ def _prototypes():
             m = re.fullmatch(r"\s*(.*?)\b(ltr_\w+)\s*\((.*)\)\s*", decl, re.S)
             if m:
                 args = [] if m.group(3).strip() == "void" else m.group(3).split(",")
-                out[m.group(2)] = (_kind(m.group(1)), [k for a in args for _, k in _declarators(a)])
+                out[m.group(2)] = (_kind(m.group(1)), [k for a in args for _, k, _ in _declarators(a)])
     return out
 
 
@@ -91,7 +109,7 @@ def compiled(tmp_path_factory):
         return None
     lines = []
     for name, fields in STRUCTS.items():
-        lines += [f'  printf("{name}.{f} %zu\\n", offsetof({name}, {f}));' for f, _ in fields]
+        lines += [f'  printf("{name}.{f} %zu\\n", offsetof({name}, {f}));' for f, _, _ in fields]
         lines.append(f'  printf("{name} %zu\\n", sizeof({name}));')
     for n, h, w in WORKSPACE_SIZES:
         lines.append(f'  printf("ws {n} {h} {w} %lld\\n", (long long)LTR_PHOTOMETRIC_WORKSPACE_BYTES({n}, {h}, {w}));')
@@ -116,13 +134,14 @@ def test_every_struct_and_prototype_is_mirrored():
 def test_struct_layout_matches_header(name, compiled):
     st = getattr(N, name)
     want = STRUCTS[name]
-    got = [(f, _ctype_kind(t)) for f, t in st._fields_]
-    assert [f for f, _ in got] == [f for f, _ in want], f"{name}: fields differ from the header"
-    for (f, k), (_, g) in zip(want, got):
+    got = [(f, _ctype_kind(t), _ctype_pointee(st, f, t)) for f, t in st._fields_]
+    assert [f for f, _, _ in got] == [f for f, _, _ in want], f"{name}: fields differ from the header"
+    for (f, k, e), (_, g, ge) in zip(want, got):
         assert g == k, f"{name}.{f}: {g} in the binding, {k} in the header"
+        assert ge == e, f"{name}.{f}: points to {ge} in the binding, {e} in the header"
     if compiled is None:
         pytest.skip("no host C compiler for the offsetof check")
-    for f, _ in want:
+    for f, _, _ in want:
         assert getattr(st, f).offset == compiled[f"{name}.{f}"], f"{name}.{f}: offset differs from the header"
     assert C.sizeof(st) == compiled[name], f"{name}: size differs from the header"
 
@@ -142,7 +161,7 @@ def test_routed_entries_take_device_and_stream():
     every entry routed through it must end its prototype with them."""
     pkg = os.path.join(ROOT, "linetr_b200")
     src = "".join(open(os.path.join(pkg, f)).read() for f in sorted(os.listdir(pkg)) if f.endswith(".py"))
-    routed = set(re.findall(r"\b_(?:call|match)\(\s*\"(ltr_\w+)\"", src))
+    routed = set(re.findall(r"\b(?:_call|_match|call_struct)\(\s*\"(ltr_\w+)\"", src))
     assert {"ltr_match", "ltr_tokenize_batch", "ltr_gather_wait"} <= routed
     decls = "".join(_declarations("linetr_b200.h"))
     for name in routed:

@@ -963,7 +963,7 @@ def test_fundamental_staging_filled_exactly():
 
 
 @pytest.mark.gpu
-def test_absolute_pose_staging_filled_exactly_and_caller_bounds(monkeypatch):
+def test_absolute_pose_staging_filled_exactly_and_struct_row_bounds(monkeypatch):
     """A group of 4 pairs with 1000 point and 300 line rows each stages exactly SMEM_MAX bytes: accepted and compared;
     one more point row is refused (code -4) before any launch.  A caller's max_rows_p / max_rows_l below a multi-pair
     group's rows leaves that group invalid and the others as they were."""
@@ -985,9 +985,10 @@ def test_absolute_pose_staging_filled_exactly_and_caller_bounds(monkeypatch):
     two = [syn.make_localization_correspondences(96 + i, 60, 15, noise_px=0.3, outlier_frac=0.3) for i in range(2)]
     res, X1, L1, groups, Ks = _ap_matches([small, two, small], shuffle_rows=False)
     ref = _ap_run(res, Ks, X1, L1, groups, n_hypotheses=64, seed=6)
-    call = L._ops.absolute_pose
+    call = L._ops.call_struct
     for bound in ({"max_rows_p": 100}, {"max_rows_l": 20}):
-        monkeypatch.setattr(L._ops, "absolute_pose", lambda *a, **kw: call(*a, **{**kw, **bound}))
+        monkeypatch.setattr(L._ops, "call_struct",
+                            lambda entry, inputs, *a, **kw: call(entry, {**inputs, **bound}, *a, **kw))
         got = _ap_run(res, Ks, X1, L1, groups, n_hypotheses=64, seed=6)
         monkeypatch.undo()
         assert got["valid"].tolist() == [True, False, True], bound

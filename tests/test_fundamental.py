@@ -416,7 +416,7 @@ def test_end_to_end_match_images_and_match_sets():
 
 
 @pytest.mark.gpu
-def test_capacity_bounds_and_empty_batches(monkeypatch):
+def test_capacity_and_struct_row_bounds_and_empty_batches(monkeypatch):
     big = syn.make_fundamental_correspondences(1, G.SMEM_MAX // G.SMEM_PER_ROW_F + 1, 0)
     N.reset_launch_count()
     with pytest.raises(N.LtrError, match=r"code -4"):
@@ -425,8 +425,9 @@ def test_capacity_bounds_and_empty_batches(monkeypatch):
     # a C-ABI caller's max_rows_p sizes the staging; a pair with more rows is invalid, not staged
     res = _matches([syn.make_fundamental_correspondences(2, n, 10, outlier_frac=0.3) for n in (300, 100)],
                    shuffle_rows=False)
-    call = G._ops.fundamental
-    monkeypatch.setattr(G._ops, "fundamental", lambda *a, **kw: call(*a, **{**kw, "max_rows_p": 200}))
+    call = G._ops.call_struct
+    monkeypatch.setattr(G._ops, "call_struct",
+                        lambda entry, inputs, *a, **kw: call(entry, {**inputs, "max_rows_p": 200}, *a, **kw))
     out = G.estimate_fundamentals(res, n_hypotheses=256)
     assert out.valid.tolist() == [False, True]
     assert not out.inliers_p[:300].any() and not out.lines_consistent[:10].any() and int(out.hypothesis[0]) == -1

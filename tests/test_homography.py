@@ -311,13 +311,14 @@ def test_over_capacity_is_unsupported_before_any_launch():
 
 
 @pytest.mark.gpu
-def test_pair_over_the_callers_row_bound_is_invalid(monkeypatch):
+def test_pair_over_the_struct_row_bound_is_invalid(monkeypatch):
     """A C-ABI caller's max_rows_p sizes the shared-memory staging; a pair with more rows is invalid, not staged."""
     Ht = syn.random_homography(np.random.default_rng(0))
     res = _matches([syn.make_homography_correspondences(2, n, 20, Ht, outlier_frac=0.3) for n in (300, 100)],
                    shuffle_rows=False)
-    call = G._ops.homography
-    monkeypatch.setattr(G._ops, "homography", lambda *a, **kw: call(*a, **{**kw, "max_rows_p": 200}))
+    call = G._ops.call_struct
+    monkeypatch.setattr(G._ops, "call_struct",
+                        lambda entry, inputs, *a, **kw: call(entry, {**inputs, "max_rows_p": 200}, *a, **kw))
     out = G.estimate_homographies(res, n_hypotheses=256)
     assert out.valid.tolist() == [False, True]
     assert not out.inliers_p[:300].any() and not out.inliers_l[:20].any() and int(out.hypothesis[0]) == -1

@@ -350,7 +350,7 @@ def test_end_to_end_match_images_and_match_sets():
 
 
 @pytest.mark.gpu
-def test_capacity_bounds_and_empty_batches(monkeypatch):
+def test_capacity_and_struct_row_bounds_and_empty_batches(monkeypatch):
     R, t = syn.random_pose(np.random.default_rng(0))
     big = syn.make_pose_correspondences(1, G.SMEM_MAX // G.SMEM_PER_ROW_E + 1, R, t)
     N.reset_launch_count()
@@ -359,8 +359,9 @@ def test_capacity_bounds_and_empty_batches(monkeypatch):
     assert N.launch_count() == 0
     # a C-ABI caller's max_rows_p sizes the staging; a pair with more rows is invalid, not staged
     res = _matches([syn.make_pose_correspondences(2, n, R, t, outlier_frac=0.3) for n in (300, 100)], shuffle_rows=False)
-    call = G._ops.essential
-    monkeypatch.setattr(G._ops, "essential", lambda *a, **kw: call(*a, **{**kw, "max_rows_p": 200}))
+    call = G._ops.call_struct
+    monkeypatch.setattr(G._ops, "call_struct",
+                        lambda entry, inputs, *a, **kw: call(entry, {**inputs, "max_rows_p": 200}, *a, **kw))
     out = G.estimate_poses(res, K, K, n_hypotheses=256)
     assert out.valid.tolist() == [False, True]
     assert not out.inliers[:300].any() and int(out.hypothesis[0]) == -1 and np.isnan(out.E[0].cpu().numpy()).all()

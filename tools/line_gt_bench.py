@@ -4,7 +4,7 @@
 
 1000 pairs of 250 x 250 segments (synthetic lines mapped by a homography plus noise, so there are many true
 matches, plus distractors) with predictions.  Device times are CUDA-event medians over --reps launches after a
-warm-up: the kernel alone (`_ops.line_gt` on staged inputs) and the whole `homography_ground_truth` call (host
+warm-up: the kernel alone (`ltr_line_gt` on staged inputs) and the whole `homography_ground_truth` call (host
 checks, np.linalg.inv, one pinned copy).  The host number is `line_assignment` + `calc_tfpn` per pair, timed on
 --host-pairs pairs.  Prints the GPU model and power limit with the numbers, then one JSON line.
 """
@@ -89,8 +89,11 @@ def main():
     assign = torch.zeros(P * n * n, dtype=torch.float32, device=dev)
 
     def kernel(dense):
-        _ops.line_gt(s0, s1, P, cu0=cu_d, cu1=cu_d, max_n0=n, max_n1=n, homography=h_d, homography_inv=hi_d, n_gt=counts,
-                     assign=assign if dense else None, assign_stride=n * n, pred0=pred, tfpn=tfpn)
+        _ops.call_struct("ltr_line_gt",
+                         dict(segs0=s0, segs1=s1, cu0=cu_d, cu1=cu_d, homography=h_d, homography_inv=hi_d, pred0=pred,
+                              n_pairs=P, max_n0=n, max_n1=n, thres_reprojected=3.0, thres_angdiff=2.0,
+                              min_overlap_ratio=0.3),
+                         dict(assign=assign if dense else None, assign_stride=n * n, n_gt=counts, tfpn=tfpn))
 
     res = {}
     res["kernel_dense_ms"] = time_cuda(lambda: kernel(True), args.reps)
