@@ -1056,6 +1056,128 @@ typedef struct {
  * (one CTA per pair) and one persistent CTA for the tree, both iterative stages and the outputs. */
 int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* out, int32_t device, void* stream);
 
+/* Image retrieval (DESIGN.md "Image retrieval"; linetr_b200/retrieval.py is the numpy model of every output bit).
+ * Local descriptors are 256-dim fp32 rows of a part (points or lines): layout LTR_LAYOUT_ROWS [n_rows, 256], or
+ * LTR_LAYOUT_CHANNEL_FIRST [256, n_i] blocks back to back (image i at 256 * cu[i]); cu [n_images + 1] row offsets.
+ * A vocabulary part holds K <= LTR_RT_MAX_CLUSTERS unit fp32 centroids [K, 256]; a global descriptor has
+ * D = 256 (K_p + K_l) components.  fp64 is explicitly rounded throughout; two calls give the same bits. */
+#define LTR_RT_MAX_CLUSTERS 256
+#define LTR_RT_MAX_K 64
+/* bound on |screened - exact| score of descriptors of norm <= 1 at dimension D (DESIGN.md "Image retrieval") */
+#define LTR_RT_EPS(D) (1e-4 + 3e-8 * (double)(D))
+
+/* One step of spherical k-means over all rows of a part.  With init_rows (device [K]): centroid c = row init_rows[c].
+ * Otherwise assign (device [n_rows], each in [0, K), the matcher's nearest centroid) groups the rows, and centroid c
+ * becomes fl32(s / sqrt(|s|^2)) for s the fp64 sum of its rows in ascending row order; a cluster without rows (or
+ * with |s| = 0) keeps centroids_in[c].  scores (device [n_rows], optional): the matcher's distances, summed into
+ * out.cost. */
+#define LTR_RT_KMEANS_WORKSPACE_BYTES(n_rows, K) (4 * ((int64_t)(n_rows) + (K) + 1))
+typedef struct {
+  const float* desc;
+  const int32_t* cu;              /* device [n_images + 1] */
+  int32_t layout;
+  int32_t n_images;
+  int32_t n_rows;                 /* = cu[n_images] */
+  int32_t K;                      /* in [1, LTR_RT_MAX_CLUSTERS] */
+  const float* centroids_in;      /* device [K, 256] */
+  const int32_t* assign;
+  const float* scores;
+  const int32_t* init_rows;
+} LtrKmeansInput;
+
+/* centroids [K, 256] (may be centroids_in), centroids_cf [256, K], tiles: the centroids' descriptor tile image
+ * (kblocks 4, ceil(K / 128) tiles of 2 x 16 KB; rows past K are not written), counts [K] rows per cluster (0 with
+ * init_rows), cost fp64 [1] (written when scores is given), workspace LTR_RT_KMEANS_WORKSPACE_BYTES. */
+typedef struct {
+  float* centroids;
+  float* centroids_cf;
+  void* tiles;
+  int32_t* counts;
+  double* cost;
+  void* workspace;
+  int64_t workspace_bytes;
+} LtrKmeansOutput;
+
+/* Errors before any launch: LTR_E_INVALID for a null pointer, a bad layout or count, n_rows < K with init_rows;
+ * LTR_E_UNSUPPORTED for K outside [1, LTR_RT_MAX_CLUSTERS]; LTR_E_WORKSPACE for a short workspace.  Two launches
+ * (bucketing, centroids) or one with init_rows; asynchronous on `stream`, never synchronises. */
+int ltr_kmeans_update(const LtrKmeansInput* in, const LtrKmeansOutput* out, int32_t device, void* stream);
+
+/* Intra-normalised VLAD of n_images images: per part with K clusters, v_c = sum (x - c) over the image's rows
+ * assigned to c (ascending row order, fp64); each v_c of norm > 0 divided by its norm (others 0); the part divided by
+ * its norm (when > 0) and multiplied by sqrt(w).  The descriptor is [points part, lines part]. */
+#define LTR_RT_VLAD_WORKSPACE_BYTES(n_images, rows_p, rows_l, k_p, k_l) \
+  (4 * ((int64_t)(rows_p) + (rows_l) + (int64_t)(n_images) * ((k_p) + (k_l)) + 2))
+typedef struct {
+  const float* desc_p;
+  const int32_t* cu_p;
+  int32_t layout_p;
+  int32_t rows_p;
+  const int32_t* assign_p;        /* device [rows_p] in [0, k_p) */
+  const float* centroids_p;       /* device [k_p, 256] */
+  int32_t k_p;
+  double w_p;                     /* finite, >= 0 */
+  const float* desc_l;
+  const int32_t* cu_l;
+  int32_t layout_l;
+  int32_t rows_l;
+  const int32_t* assign_l;
+  const float* centroids_l;
+  int32_t k_l;
+  double w_l;
+  int32_t n_images;               /* >= 1 */
+} LtrVladInput;
+
+/* desc [n_images, D] fp32; tiles: its tile image (kblocks D / 64, ceil(n_images / 128) row tiles, padding rows 0). */
+typedef struct {
+  float* desc;
+  void* tiles;
+  void* workspace;
+  int64_t workspace_bytes;
+} LtrVladOutput;
+
+/* Errors before any launch: LTR_E_INVALID for a null pointer, a bad layout, count or weight; LTR_E_UNSUPPORTED for
+ * k_p or k_l outside [1, LTR_RT_MAX_CLUSTERS]; LTR_E_WORKSPACE for a short workspace.  Three launches. */
+int ltr_vlad(const LtrVladInput* in, const LtrVladOutput* out, int32_t device, void* stream);
+
+/* Top-k database images of every query by the exact score: the fp64 sum of the products of the fp32 components,
+ * lane l of a warp summing components l, l + 32, ... in ascending order, then the xor butterfly 16, 8, 4, 2, 1.
+ * Sorted by score descending, ties to the lower index; exclude_self skips database index q for query q.  The GPU
+ * screens with a split-bf16 tensor-core product and rescores exactly every candidate within 2 LTR_RT_EPS(D) of the k-th
+ * screened score; a query whose tiles may have dropped a candidate there takes an exact pass over all N. */
+#define LTR_RT_WORKSPACE_BYTES(Q, N, k) ((int64_t)(Q) * (((int64_t)(N) + 127) / 128) * (8 * (int64_t)(k) + 4))
+typedef struct {
+  const float* q;                 /* device [Q, D] */
+  const void* q_tiles;            /* their tile image (kblocks D / 64) */
+  const float* db;                /* device [N, D] */
+  const void* db_tiles;
+  int32_t Q;                      /* >= 1 */
+  int32_t N;                      /* >= 1 */
+  int32_t D;                      /* a positive multiple of 64, <= 2 * 256 * LTR_RT_MAX_CLUSTERS */
+  int32_t k;                      /* in [1, LTR_RT_MAX_K] */
+  int32_t exclude_self;
+} LtrRetrieveInput;
+
+/* idx [Q, k] int32 (-1 past the candidates), score [Q, k] fp64 (NaN there), n_full [1] int32: queries that took the
+ * full exact pass; workspace LTR_RT_WORKSPACE_BYTES(Q, N, k) bytes. */
+typedef struct {
+  int32_t* idx;
+  double* score;
+  int32_t* n_full;
+  void* workspace;
+  int64_t workspace_bytes;
+} LtrRetrieveOutput;
+
+/* Errors before any launch: LTR_E_INVALID for a null pointer or a bad count; LTR_E_UNSUPPORTED for k or D out of range,
+ * more than 65535 query tiles; LTR_E_WORKSPACE for a short workspace.  Two launches (screening, merge). */
+int ltr_retrieve(const LtrRetrieveInput* in, const LtrRetrieveOutput* out, int32_t device, void* stream);
+
+/* The descriptor tile image of fp32 rows x [n, D] (device; D a positive multiple of 64): kblocks D / 64,
+ * ceil(n / 128) row tiles, padding rows 0; LTR_RT_TILES_BYTES(n, D) bytes.  What ltr_retrieve takes for descriptors
+ * that do not come from ltr_vlad.  Errors before any launch: LTR_E_INVALID for n < 1, a bad D or a null pointer. */
+#define LTR_RT_TILES_BYTES(n, D) (4 * (((int64_t)(n) + 127) / 128) * 128 * (int64_t)(D))
+int ltr_rt_tiles(const float* x, int32_t n, int32_t D, void* tiles, int32_t device, void* stream);
+
 /* Homography image pairs <- the warp and valid mask of the homography dataset builder
  * (dataloaders/build_homography_dataset.py:164-184): cv2.warpPerspective of the grey image, and the mask that is 0 where
  * the warped colour image is 0 in every channel, eroded with a 5 x 5 kernel of ones.

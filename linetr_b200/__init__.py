@@ -29,6 +29,9 @@ set, and one robust multi-view world point or world line per track, batched on t
 Bundle adjustment (bundle): the poses of a posed image set and the world points and lines of its tracks refined
 together (Levenberg-Marquardt with a Schur complement onto the cameras), on the GPU:
     bundle_adjust, BundleResult
+Image retrieval (retrieval): a spherical k-means vocabulary over an image set's point and line descriptors, VLAD
+global descriptors and the exact top-k database images of every query, as pair lists, on the GPU:
+    Vocabulary, train_vocabulary, global_descriptors, retrieve, retrieval_pairs
 Homography image pairs (homography_pairs): sampled homographies, warped images and valid masks, batched on the GPU:
     sample_homographies, warp_pairs, homography_pairs, apply_valid_masks
 Photometric augmentation (photometric): the homography builder's brightness, contrast, noise, motion blur and shade,
@@ -83,6 +86,13 @@ _LAZY = {
     "global_poses": ("global_poses", "global_poses"),
     "GlobalPoseResult": ("global_poses", "GlobalPoseResult"),
     "registered_set": ("global_poses", "registered_set"),
+    "Vocabulary": ("retrieval", "Vocabulary"),
+    "train_vocabulary": ("retrieval", "train_vocabulary"),
+    "global_descriptors": ("retrieval", "global_descriptors"),
+    "GlobalDescriptors": ("retrieval", "GlobalDescriptors"),
+    "retrieve": ("retrieval", "retrieve"),
+    "Retrieval": ("retrieval", "Retrieval"),
+    "retrieval_pairs": ("retrieval", "retrieval_pairs"),
     "sample_homographies": ("homography_pairs", "sample_homographies"),
     "warp_pairs": ("homography_pairs", "warp_pairs"),
     "homography_pairs": ("homography_pairs", "homography_pairs"),

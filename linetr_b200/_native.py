@@ -34,6 +34,8 @@ BA_STATS = 8                 # LTR_BA_STATS
 GP_MAX_IMAGES = 128          # LTR_GP_MAX_IMAGES
 GP_EDGE_UNUSED, GP_EDGE_OUTSIDE, GP_EDGE_ROT_OUTLIER, GP_EDGE_DIR_OUTLIER, GP_EDGE_INLIER = 0, 1, 2, 3, 4   # LTR_GP_EDGE_*
 GP_STATS = 7                 # LTR_GP_STATS
+RT_MAX_CLUSTERS = 256        # LTR_RT_MAX_CLUSTERS
+RT_MAX_K = 64                # LTR_RT_MAX_K
 
 
 def ba_workspace_bytes(n_images, n_kp, n_kl, t_p, t_l) -> int:
@@ -46,6 +48,26 @@ def gp_workspace_bytes(n_images, n_pairs) -> int:
     """LTR_GP_WORKSPACE_BYTES(n_images, n_pairs)."""
     n, P = int(n_images), int(n_pairs)
     return 8 * (16 * P + 24 * n) + 4 * (2 * n * n + 8 * n + 16)
+
+
+def rt_kmeans_workspace_bytes(n_rows, K) -> int:
+    """LTR_RT_KMEANS_WORKSPACE_BYTES(n_rows, K)."""
+    return 4 * (int(n_rows) + int(K) + 1)
+
+
+def rt_vlad_workspace_bytes(n_images, rows_p, rows_l, k_p, k_l) -> int:
+    """LTR_RT_VLAD_WORKSPACE_BYTES(n_images, rows_p, rows_l, k_p, k_l)."""
+    return 4 * (int(rows_p) + int(rows_l) + int(n_images) * (int(k_p) + int(k_l)) + 2)
+
+
+def rt_eps(D) -> float:
+    """LTR_RT_EPS(D)."""
+    return 1e-4 + 3e-8 * float(D)
+
+
+def rt_workspace_bytes(Q, N, k) -> int:
+    """LTR_RT_WORKSPACE_BYTES(Q, N, k)."""
+    return int(Q) * ((int(N) + 127) // 128) * (8 * int(k) + 4)
 
 
 def photometric_workspace_bytes(n, h, w) -> int:
@@ -297,6 +319,42 @@ class LtrGlobalPoseOutput(C.Structure):
         ("dir_cos", F64P), ("stats", F64P), ("workspace", C.c_void_p)])
 
 
+class LtrKmeansInput(C.Structure):
+    _fields_, _pointees_ = _typed([
+        ("desc", F32P), ("cu", I32P), ("layout", C.c_int32), ("n_images", C.c_int32), ("n_rows", C.c_int32),
+        ("K", C.c_int32), ("centroids_in", F32P), ("assign", I32P), ("scores", F32P), ("init_rows", I32P)])
+
+
+class LtrKmeansOutput(C.Structure):
+    _fields_, _pointees_ = _typed([
+        ("centroids", F32P), ("centroids_cf", F32P), ("tiles", C.c_void_p), ("counts", I32P), ("cost", F64P),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64)])
+
+
+class LtrVladInput(C.Structure):
+    _fields_, _pointees_ = _typed([
+        ("desc_p", F32P), ("cu_p", I32P), ("layout_p", C.c_int32), ("rows_p", C.c_int32), ("assign_p", I32P),
+        ("centroids_p", F32P), ("k_p", C.c_int32), ("w_p", C.c_double), ("desc_l", F32P), ("cu_l", I32P),
+        ("layout_l", C.c_int32), ("rows_l", C.c_int32), ("assign_l", I32P), ("centroids_l", F32P), ("k_l", C.c_int32),
+        ("w_l", C.c_double), ("n_images", C.c_int32)])
+
+
+class LtrVladOutput(C.Structure):
+    _fields_, _pointees_ = _typed([
+        ("desc", F32P), ("tiles", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64)])
+
+
+class LtrRetrieveInput(C.Structure):
+    _fields_, _pointees_ = _typed([
+        ("q", F32P), ("q_tiles", C.c_void_p), ("db", F32P), ("db_tiles", C.c_void_p), ("Q", C.c_int32),
+        ("N", C.c_int32), ("D", C.c_int32), ("k", C.c_int32), ("exclude_self", C.c_int32)])
+
+
+class LtrRetrieveOutput(C.Structure):
+    _fields_, _pointees_ = _typed([
+        ("idx", I32P), ("score", F64P), ("n_full", I32P), ("workspace", C.c_void_p), ("workspace_bytes", C.c_int64)])
+
+
 _P, _I32, _I64, _F32, _ptr = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.POINTER
 # {name: (restype, argtypes)} of every function include/linetr_b200.h declares (tests check the library exports all
 # of them, and each entry against its C prototype)
@@ -328,6 +386,10 @@ PROTOTYPES = {
     "ltr_tracks": (C.c_int, [_ptr(LtrTracksInput), _ptr(LtrTracksOutput), _I32, _P]),
     "ltr_bundle_adjust": (C.c_int, [_ptr(LtrBundleInput), _ptr(LtrBundleOutput), _I32, _P]),
     "ltr_global_poses": (C.c_int, [_ptr(LtrGlobalPoseInput), _ptr(LtrGlobalPoseOutput), _I32, _P]),
+    "ltr_kmeans_update": (C.c_int, [_ptr(LtrKmeansInput), _ptr(LtrKmeansOutput), _I32, _P]),
+    "ltr_vlad": (C.c_int, [_ptr(LtrVladInput), _ptr(LtrVladOutput), _I32, _P]),
+    "ltr_retrieve": (C.c_int, [_ptr(LtrRetrieveInput), _ptr(LtrRetrieveOutput), _I32, _P]),
+    "ltr_rt_tiles": (C.c_int, [_P, _I32, _I32, _P, _I32, _P]),
     "ltr_warp_pairs": (C.c_int, [_P, _P] + [_I32] * 4 + [c_int32_p, _P, _P, _I32, _P, _P, _I32, _P]),
     "ltr_photometric": (C.c_int, [_P, _P] + [_I32] * 3 + [_P, _P, _I32, _P, _I32, _P, _P, _I64, _I32, _P]),
     "ltr_linear_img": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P, _I32, _P] + [_I32] * 6 + [_P]),

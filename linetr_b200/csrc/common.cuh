@@ -51,6 +51,7 @@ enum KernelClass : int {
   KC_TRACKS,
   KC_BUNDLE,
   KC_GLOBAL_POSES,
+  KC_RETRIEVAL,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);

@@ -29,6 +29,7 @@
 #include "tracks.cuh"
 #include "bundle.cuh"
 #include "global_poses.cuh"
+#include "retrieval.cuh"
 #include "photometric.cuh"
 
 namespace ltr {
@@ -50,7 +51,7 @@ const char* kernel_class_name(int kc) {
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
                                          "fundamental", "absolute_pose", "triangulate", "tracks",
-                                         "bundle", "global_poses"};
+                                         "bundle", "global_poses", "retrieval"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -1629,6 +1630,147 @@ int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* ou
   LTR_CUDA_TRY(launch_pdl(gp_graph_kernel, dim3(1), dim3(GP_THREADS), 0, s, a));
   if (P) LTR_CUDA_TRY(launch_pdl(gp_support_kernel, dim3(P), dim3(GP_MAX_IMAGES), 0, s, a));
   LTR_CUDA_TRY(launch_pdl(gp_solve_kernel, dim3(1), dim3(GP_THREADS), smem, s, a));
+  return LTR_OK;
+}
+
+static int rt_check_rows(const char* who, const float* desc, const int32_t* cu, int32_t layout, int32_t rows) {
+  if (layout != LTR_LAYOUT_ROWS && layout != LTR_LAYOUT_CHANNEL_FIRST)
+    return set_error(LTR_E_INVALID, std::string(who) + ": layout must be LTR_LAYOUT_ROWS or LTR_LAYOUT_CHANNEL_FIRST");
+  if (rows < 0) return set_error(LTR_E_INVALID, std::string(who) + ": negative row count");
+  if (!cu || (rows > 0 && !desc)) return set_error(LTR_E_INVALID, std::string(who) + ": null descriptors or offsets");
+  return LTR_OK;
+}
+
+int ltr_kmeans_update(const LtrKmeansInput* in, const LtrKmeansOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_kmeans_update: null argument");
+  if (in->K < 1 || in->K > LTR_RT_MAX_CLUSTERS)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_kmeans_update: K must lie in [1, LTR_RT_MAX_CLUSTERS]");
+  if (in->n_images < 1) return set_error(LTR_E_INVALID, "ltr_kmeans_update: n_images must be >= 1");
+  if (int rc = rt_check_rows("ltr_kmeans_update", in->desc, in->cu, in->layout, in->n_rows)) return rc;
+  if (in->init_rows ? in->n_rows < in->K : (!in->centroids_in || (in->n_rows > 0 && !in->assign)))
+    return set_error(LTR_E_INVALID, "ltr_kmeans_update: fewer rows than clusters, or null centroids or assignments");
+  if (!out->centroids || !out->centroids_cf || !out->tiles || !out->counts || (in->scores && !out->cost) || !out->workspace)
+    return set_error(LTR_E_INVALID, "ltr_kmeans_update: null output or workspace");
+  if (out->workspace_bytes < LTR_RT_KMEANS_WORKSPACE_BYTES(in->n_rows, in->K))
+    return set_error(LTR_E_WORKSPACE, "ltr_kmeans_update: workspace too small");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  int* cstart = static_cast<int*>(out->workspace);
+  int* perm = cstart + in->K + 1;
+  const int K = in->K;
+  RtKmeansArgs a{};
+  a.rows = RtRows{in->desc, in->cu, in->layout, in->n_images};
+  a.K = K; a.cstart = cstart; a.perm = perm; a.init_rows = in->init_rows; a.cent_in = in->centroids_in;
+  a.cent = out->centroids; a.cent_cf = out->centroids_cf; a.counts = out->counts;
+  a.img.hi = static_cast<__nv_bfloat16*>(out->tiles);
+  a.img.lo = a.img.hi + (size_t)cdiv(K, 128) * 4 * IMG_TILE_ELEMS;
+  a.img.kblocks = 4;
+  LaunchScope ls(KC_RETRIEVAL, s);
+  if (!in->init_rows) {
+    RtBucketArgs b{in->assign, nullptr, 1, in->n_rows, K, cstart, perm, in->scores, in->scores ? out->cost : nullptr};
+    LTR_CUDA_TRY(launch_pdl(rt_bucket_kernel, dim3(1), dim3(RT_BUCKET_THREADS), 0, s, b));
+  }
+  LTR_CUDA_TRY(launch_pdl(rt_kmeans_kernel, dim3(K), dim3(256), 0, s, a));
+  return LTR_OK;
+}
+
+int ltr_vlad(const LtrVladInput* in, const LtrVladOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_vlad: null argument");
+  if (in->k_p < 1 || in->k_p > LTR_RT_MAX_CLUSTERS || in->k_l < 1 || in->k_l > LTR_RT_MAX_CLUSTERS)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_vlad: k_p and k_l must lie in [1, LTR_RT_MAX_CLUSTERS]");
+  if (in->n_images < 1) return set_error(LTR_E_INVALID, "ltr_vlad: n_images must be >= 1");
+  if (int rc = rt_check_rows("ltr_vlad", in->desc_p, in->cu_p, in->layout_p, in->rows_p)) return rc;
+  if (int rc = rt_check_rows("ltr_vlad", in->desc_l, in->cu_l, in->layout_l, in->rows_l)) return rc;
+  if (!(std::isfinite(in->w_p) && in->w_p >= 0.0 && std::isfinite(in->w_l) && in->w_l >= 0.0))
+    return set_error(LTR_E_INVALID, "ltr_vlad: the part weights must be finite and >= 0");
+  if (!in->centroids_p || !in->centroids_l || (in->rows_p && !in->assign_p) || (in->rows_l && !in->assign_l))
+    return set_error(LTR_E_INVALID, "ltr_vlad: null centroids or assignments");
+  if (!out->desc || !out->tiles || !out->workspace) return set_error(LTR_E_INVALID, "ltr_vlad: null output or workspace");
+  if (out->workspace_bytes < LTR_RT_VLAD_WORKSPACE_BYTES(in->n_images, in->rows_p, in->rows_l, in->k_p, in->k_l))
+    return set_error(LTR_E_WORKSPACE, "ltr_vlad: workspace too small");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  const int n = in->n_images, D = RT_DL * (in->k_p + in->k_l);
+  int* w = static_cast<int*>(out->workspace);
+  RtVladArgs a{};
+  const float* desc[2] = {in->desc_p, in->desc_l};
+  const int32_t* cu[2] = {in->cu_p, in->cu_l};
+  const int32_t layout[2] = {in->layout_p, in->layout_l}, rows[2] = {in->rows_p, in->rows_l}, K[2] = {in->k_p, in->k_l};
+  const int32_t* assign[2] = {in->assign_p, in->assign_l};
+  const float* cent[2] = {in->centroids_p, in->centroids_l};
+  const double wt[2] = {in->w_p, in->w_l};
+  RtBucketArgs b[2];
+  for (int pi = 0; pi < 2; ++pi) {
+    RtPart& p = a.part[pi];
+    p.rows = RtRows{desc[pi], cu[pi], layout[pi], n};
+    p.K = K[pi]; p.cent = cent[pi]; p.sw = std::sqrt(wt[pi]); p.col0 = pi ? RT_DL * in->k_p : 0;
+    int* cstart = w;
+    w += (size_t)n * K[pi] + 1;
+    int* perm = w;
+    w += rows[pi];
+    p.cstart = cstart; p.perm = perm;
+    b[pi] = RtBucketArgs{assign[pi], cu[pi], n, rows[pi], K[pi], cstart, perm, nullptr, nullptr};
+  }
+  a.n_images = n; a.D = D; a.desc = out->desc;
+  a.img.hi = static_cast<__nv_bfloat16*>(out->tiles);
+  a.img.lo = a.img.hi + (size_t)cdiv(n, 128) * (D / 64) * IMG_TILE_ELEMS;
+  a.img.kblocks = D / 64;
+  LaunchScope ls(KC_RETRIEVAL, s);
+  for (int pi = 0; pi < 2; ++pi) LTR_CUDA_TRY(launch_pdl(rt_bucket_kernel, dim3(n), dim3(RT_BUCKET_THREADS), 0, s, b[pi]));
+  LTR_CUDA_TRY(launch_pdl(rt_vlad_kernel, dim3(cdiv(n, 128) * 128), dim3(256), 0, s, a));
+  return LTR_OK;
+}
+
+int ltr_retrieve(const LtrRetrieveInput* in, const LtrRetrieveOutput* out, int32_t device, void* stream) {
+  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_retrieve: null argument");
+  if (in->Q < 1 || in->N < 1) return set_error(LTR_E_INVALID, "ltr_retrieve: Q and N must be >= 1");
+  if (in->k < 1 || in->k > LTR_RT_MAX_K) return set_error(LTR_E_UNSUPPORTED, "ltr_retrieve: k must lie in [1, LTR_RT_MAX_K]");
+  if (in->D < 64 || in->D % 64 || in->D > 2 * RT_DL * LTR_RT_MAX_CLUSTERS)
+    return set_error(LTR_E_UNSUPPORTED, "ltr_retrieve: D must be a positive multiple of 64, at most 2 * 256 * LTR_RT_MAX_CLUSTERS");
+  if (cdiv(in->Q, 128) > 65535) return set_error(LTR_E_UNSUPPORTED, "ltr_retrieve: more than 65535 query tiles");
+  if (!in->q || !in->q_tiles || !in->db || !in->db_tiles) return set_error(LTR_E_INVALID, "ltr_retrieve: null input");
+  if (!out->idx || !out->score || !out->n_full || !out->workspace)
+    return set_error(LTR_E_INVALID, "ltr_retrieve: null output or workspace");
+  if (out->workspace_bytes < LTR_RT_WORKSPACE_BYTES(in->Q, in->N, in->k))
+    return set_error(LTR_E_WORKSPACE, "ltr_retrieve: workspace too small");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  const int nt = cdiv(in->N, 128), kbs = in->D / 64;
+  const size_t nc = (size_t)in->Q * nt * in->k;
+  RtScreenArgs a{};
+  auto img = [&](const void* t, int rows) {
+    ActImg m;
+    m.hi = static_cast<__nv_bfloat16*>(const_cast<void*>(t));
+    m.lo = m.hi + (size_t)cdiv(rows, 128) * kbs * IMG_TILE_ELEMS;
+    m.kblocks = kbs;
+    return m;
+  };
+  a.q = img(in->q_tiles, in->Q); a.db = img(in->db_tiles, in->N);
+  a.Q = in->Q; a.N = in->N; a.kb = kbs; a.k = in->k; a.exclude_self = in->exclude_self != 0; a.n_tiles = nt;
+  a.cand_score = static_cast<float*>(out->workspace);
+  a.cand_idx = reinterpret_cast<int*>(a.cand_score + nc);
+  a.drop = reinterpret_cast<float*>(a.cand_idx + nc);
+  a.n_full = out->n_full;
+  RtMergeArgs m{in->q, in->db, in->Q, in->N, in->D, in->k, a.exclude_self, nt, a.cand_score, a.cand_idx, a.drop,
+                out->idx, out->score, out->n_full};
+  LTR_CUDA_TRY(ensure_dynamic_smem(rt_screen_kernel, RT_SMEM));
+  LaunchScope ls(KC_RETRIEVAL, s);
+  LTR_CUDA_TRY(launch_pdl(rt_screen_kernel, dim3(nt, cdiv(in->Q, 128)), dim3(RT_THREADS), (size_t)RT_SMEM, s, a));
+  LTR_CUDA_TRY(launch_pdl(rt_merge_kernel, dim3(in->Q), dim3(RT_MERGE_THREADS), 0, s, m));
+  return LTR_OK;
+}
+
+int ltr_rt_tiles(const float* x, int32_t n, int32_t D, void* tiles, int32_t device, void* stream) {
+  if (n < 1 || D < 64 || D % 64 || !x || !tiles)
+    return set_error(LTR_E_INVALID, "ltr_rt_tiles: n must be >= 1, D a positive multiple of 64, pointers not null");
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  cudaStream_t s = as_stream(stream);
+  ActImg img;
+  img.hi = static_cast<__nv_bfloat16*>(tiles);
+  img.lo = img.hi + (size_t)cdiv(n, 128) * (D / 64) * IMG_TILE_ELEMS;
+  img.kblocks = D / 64;
+  LaunchScope ls(KC_RETRIEVAL, s);
+  LTR_CUDA_TRY(launch_pdl(rt_tiles_kernel, dim3(cdiv(n, 128) * 128), dim3(256), 0, s, x, n, D, img));
   return LTR_OK;
 }
 

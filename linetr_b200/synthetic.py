@@ -759,3 +759,35 @@ def make_relative_poses(R, t, pairs, noise_deg: float = 0.0, outlier_frac: float
         Rp[p] = _axis_angle(_unit(rng.normal(size=3)), np.deg2rad(noise_deg * rng.normal())) @ Rr
         tp[p] = _axis_angle(_unit(rng.normal(size=3)), np.deg2rad(noise_deg * rng.normal())) @ d
     return dict(R=Rp, t=tp, valid=np.ones(P, bool), n_cheirality=np.full(P, n_cheirality, np.int32), outlier=out)
+
+
+def make_covisibility_set(seed: int, n_views: int = 24, window: int = 8, step: int = 2, n_distractors: int = 6,
+                          per_landmark: int = 3, noise: float = 0.25, d: int = D_MODEL):
+    """Views moving along a corridor of landmarks, each seeing `window` consecutive landmarks (view v from landmark
+    v * step), plus distractor views of unrelated scenes.  Every landmark has a point and a key-line descriptor, and a
+    view holds `per_landmark` observations of each (unit fp32 rows, noise of norm about `noise`), so both parts carry the overlap.  -> dict
+    points / lines: per view [m, d] rows; overlap bool [n, n]: views sharing a landmark (distractors share none, the
+    diagonal is False); distractor bool [n]."""
+    rng = np.random.default_rng(seed)
+    n_lm = (n_views - 1) * step + window
+    lm_p, lm_l = _unit(rng.standard_normal((n_lm, d))), _unit(rng.standard_normal((n_lm, d)))
+    points, lines, seen = [], [], []
+
+    def observe(lp, ll):
+        rep = lambda x: _unit(np.repeat(x, per_landmark, 0) + noise / np.sqrt(d) * rng.standard_normal((len(x) * per_landmark, d)))  # noqa: E731
+        return rep(lp).astype(np.float32), rep(ll).astype(np.float32)
+
+    for v in range(n_views):
+        ids = np.arange(v * step, v * step + window)
+        p, l = observe(lm_p[ids], lm_l[ids])
+        points.append(p)
+        lines.append(l)
+        seen.append(set(ids.tolist()))
+    for _ in range(n_distractors):
+        p, l = observe(_unit(rng.standard_normal((window, d))), _unit(rng.standard_normal((window, d))))
+        points.append(p)
+        lines.append(l)
+        seen.append(set())
+    n = n_views + n_distractors
+    overlap = np.array([[i != j and bool(seen[i] & seen[j]) for j in range(n)] for i in range(n)])
+    return dict(points=points, lines=lines, overlap=overlap, distractor=np.arange(n) >= n_views)
