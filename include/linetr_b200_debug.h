@@ -84,6 +84,16 @@ int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double
 int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s1, int32_t n, double min_overlap,
                                 double* r1, double* r0, uint8_t* ok, int32_t device, void* stream);
 
+/* The pose stages' dense SPD solver (rc_cholesky_solve) on its own, one 1024-thread CTA per system, the instantiation
+ * ba_solve_kernel and gp_solve_kernel run: A [n, m, ld] (its lower triangle read, L written over it) and the
+ * right-hand sides x [n, m, k] (device), solved in place; ok [n] (device) is 1, or 0 at the first pivot that is not
+ * > 0, with x untouched.  shared = 1 copies A (m <= 127) and x into dynamic shared memory first, as gp_solve_kernel
+ * keeps them; shared = 0 works in place in global memory with leading dimension ld, as ba_solve_kernel does.  Returns
+ * 0, or LTR_E_INVALID before any launch unless 0 <= m <= 1024 (<= 127 when shared), 1 <= k <= 6, ld >= m, shared
+ * is 0 or 1, and (n > 0) ok and (m > 0) A and x are given. */
+int ltr_debug_cholesky_solve(double* A, int32_t n, int32_t m, int32_t ld, double* x, int32_t k, int32_t shared,
+                             uint8_t* ok, int32_t device, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -414,6 +414,7 @@ DEBUG_PROTOTYPES = {
     "ltr_debug_fundamental_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),
     "ltr_debug_p3p": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _I32, _P]),
     "ltr_debug_fundamental_lines": (C.c_int, [_P, _P, _P, _I32, C.c_double, _P, _P, _P, _I32, _P]),
+    "ltr_debug_cholesky_solve": (C.c_int, [_P, _I32, _I32, _I32, _P, _I32, _I32, _P, _I32, _P]),
 }
 EXPORTED_SYMBOLS = tuple(PROTOTYPES)
 DEBUG_SYMBOLS = tuple(DEBUG_PROTOTYPES)

@@ -2073,6 +2073,38 @@ static __global__ void debug_fundamental_lines_kernel(const double* F, const flo
   ok[i] = fm_ratios_consistent(a, b, min_overlap);
 }
 
+// One CTA of 1024 threads per system, the rc_cholesky_solve<1024> instantiation of ba_solve_kernel and gp_solve_kernel.
+// shared: A (square, ld m) and x are copied into dynamic shared memory first, as gp_solve_kernel keeps them, and copied
+// back after; else the solve works in place on the caller's A (leading dimension ld) and x, as ba_solve_kernel does.
+constexpr int DEBUG_CHOL_THREADS = 1024;
+static __global__ void __launch_bounds__(DEBUG_CHOL_THREADS) debug_cholesky_kernel(double* A, int m, int ld, double* x,
+                                                                                   int k, int shared, uint8_t* ok) {
+  extern __shared__ double s_dyn[];
+  __shared__ int s_fail;
+  const int tid = threadIdx.x;
+  double* Ag = A + (size_t)blockIdx.x * m * ld;
+  double* xg = x + (size_t)blockIdx.x * m * k;
+  double* As = Ag;
+  double* xs = xg;
+  int lds = ld;
+  if (shared) {
+    As = s_dyn;
+    xs = As + (size_t)m * m;
+    lds = m;
+    for (int e = tid; e < m * m; e += DEBUG_CHOL_THREADS) As[e] = Ag[(size_t)ld * (e / m) + e % m];
+    for (int e = tid; e < m * k; e += DEBUG_CHOL_THREADS) xs[e] = xg[e];
+  }
+  double* scol = shared ? xs + (size_t)m * k : s_dyn;
+  if (tid == 0) s_fail = 0;
+  __syncthreads();
+  const bool fail = rc_cholesky_solve<DEBUG_CHOL_THREADS>(As, lds, m, xs, k, scol, &s_fail);
+  if (shared) {
+    for (int e = tid; e < m * m; e += DEBUG_CHOL_THREADS) Ag[(size_t)ld * (e / m) + e % m] = As[e];
+    for (int e = tid; e < m * k; e += DEBUG_CHOL_THREADS) xg[e] = xs[e];
+  }
+  if (tid == 0) ok[blockIdx.x] = !fail;
+}
+
 int ltr_debug_sturm_roots(const double* poly, int32_t n, double* roots, int32_t* count, int32_t device, void* stream) {
   if (n < 0 || (n > 0 && (!poly || !roots || !count))) return set_error(LTR_E_INVALID, "ltr_debug_sturm_roots: bad argument");
   if (n == 0) return LTR_OK;
@@ -2122,6 +2154,21 @@ int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
   debug_fundamental_lines_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(F, s0, s1, n, min_overlap, r1, r0, ok);
+  LTR_CUDA_TRY(cudaGetLastError());
+  return LTR_OK;
+}
+
+int ltr_debug_cholesky_solve(double* A, int32_t n, int32_t m, int32_t ld, double* x, int32_t k, int32_t shared,
+                             uint8_t* ok, int32_t device, void* stream) {
+  if (n < 0 || m < 0 || m > DEBUG_CHOL_THREADS || k < 1 || k > 6 || ld < m || (shared != 0 && shared != 1) ||
+      (shared && m > GP_MAX_IMAGES - 1) || (n > 0 && (!ok || (m > 0 && (!A || !x)))))
+    return set_error(LTR_E_INVALID, "ltr_debug_cholesky_solve: bad argument");
+  if (n == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  const size_t smem = 8 * (shared ? (size_t)m * m + (size_t)m * k + m : (size_t)(m > 0 ? m : 1));
+  // the largest shared case (m = 127, k = 6: gp_smem_bytes(128)) once, so the attribute holds for every later call
+  LTR_CUDA_TRY(ensure_dynamic_smem(debug_cholesky_kernel, (int)gp_smem_bytes(GP_MAX_IMAGES)));
+  debug_cholesky_kernel<<<n, DEBUG_CHOL_THREADS, smem, as_stream(stream)>>>(A, m, ld, x, k, shared, ok);
   LTR_CUDA_TRY(cudaGetLastError());
   return LTR_OK;
 }

@@ -86,6 +86,10 @@ __device__ __forceinline__ void rc_cayley(const double* w, double* Q) {
 // A (leading dimension ld; the lower triangle is read and L written over it), then the forward and back substitutions
 // of the k right-hand sides x [m, k] in place.  A and x may be global or shared.  s_col holds m doubles of shared
 // memory; *s_fail (shared) enters as 1 to skip the call, and leaves as 1 iff a pivot was not > 0, with x untouched.
+// Barriers: every thread reads the pivot A[c][c], so thread 0 writes its root l there only after the barrier that
+// follows the column's scaling; the trailing update reads columns > c, and the next column's pivot read and the solves
+// come after a later barrier.  On a failed pivot A keeps the columns before it as L, the pivot and the trailing lower
+// triangle as its Schur complement; the upper triangle is never touched.
 template <int NT>
 __device__ __forceinline__ bool rc_cholesky_solve(double* A, int ld, int m, double* x, int k, double* s_col,
                                                   int* s_fail) {
@@ -99,13 +103,13 @@ __device__ __forceinline__ bool rc_cholesky_solve(double* A, int ld, int m, doub
       break;
     }
     const double l = __dsqrt_rn(piv);
-    if (tid == 0) A[(size_t)ld * c + c] = l;
     for (int i = c + 1 + tid; i < m; i += NT) {
       const double v = RC_D(A[(size_t)ld * i + c], l);
       A[(size_t)ld * i + c] = v;
       s_col[i] = v;
     }
     __syncthreads();
+    if (tid == 0) A[(size_t)ld * c + c] = l;
     // one warp per row of the trailing block, lanes over its columns c < j <= i
     for (int i = c + 1 + wid; i < m; i += NT / 32) {
       const double li = s_col[i];

@@ -302,8 +302,12 @@ def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.
     dev = res.matches_p.device
     op, ol = offsets(S.n_kp), offsets(S.n_kl)
     f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
-    out = TriangulationResult(torch.empty((int(op[-1]), 3), **f64), torch.empty((int(ol[-1]), 2, 3), **f64),
-                              torch.empty(int(op[-1]), **i32), torch.empty(int(ol[-1]), **i32),
+    # at least one row each, so a set without keypoints or without key lines hands ltr_triangulate no null output
+    Np, Nl = int(op[-1]), int(ol[-1])
+    rp, rl = max(Np, 1), max(Nl, 1)
+    buf = dict(points3d=torch.empty((rp, 3), **f64), lines3d=torch.empty((rl, 2, 3), **f64),
+               n_views_p=torch.empty(rp, **i32), n_views_l=torch.empty(rl, **i32))
+    out = TriangulationResult(buf["points3d"][:Np], buf["lines3d"][:Nl], buf["n_views_p"][:Np], buf["n_views_l"][:Nl],
                               op.astype(np.int64), ol.astype(np.int64))
     if n == 0:
         return out
@@ -324,6 +328,5 @@ def triangulate(keypoints, klines, pairs, res, K, R, t, thresh=4.0, min_angle=1.
                       "n_inv_p": int(inv_off_p[-1]), "n_inv_l": int(inv_off_l[-1]), "n_blocks": int(block_off[-1]),
                       "max_views": int(np.diff(S.view_off).max(initial=0)), "thresh": thresh,
                       "min_angle": min_angle, "min_views": min_views},
-                     dict(points3d=out.points3d, lines3d=out.lines3d, n_views_p=out.n_views_p,
-                          n_views_l=out.n_views_l, inv_p=inv_p, inv_l=inv_l))
+                     dict(**buf, inv_p=inv_p, inv_l=inv_l))
     return out
