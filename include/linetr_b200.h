@@ -1053,7 +1053,8 @@ typedef struct {
 
 /* Asynchronous on `stream`; never synchronises.  Errors come before any launch: LTR_E_INVALID for bad arguments,
  * LTR_E_UNSUPPORTED for more than LTR_GP_MAX_IMAGES images.  Three launches: the view graph (one CTA), the loop support
- * (one CTA per pair) and one persistent CTA for the tree, both iterative stages and the outputs. */
+ * (one CTA per pair; not launched without pairs) and one persistent CTA for the tree, both iterative stages and the
+ * outputs. */
 int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* out, int32_t device, void* stream);
 
 /* Image retrieval (DESIGN.md "Image retrieval"; linetr_b200/retrieval.py is the numpy model of every output bit).
@@ -1264,12 +1265,16 @@ int ltr_linear_img_norm(const float* x, int32_t ldx, const float* w_host, const 
                         const float* beta, const float* add, int32_t ldadd, float* y, int32_t ldy,
                         float* y_from_image, int32_t m, int32_t k, int32_t device, void* stream);
 
-/* Instrumentation.  Kernel launches issued by this library since the last reset. */
+/* Instrumentation.  Kernel launches issued by this library since the last reset: one count per kernel
+ * launch, those of the debug hooks (include/linetr_b200_debug.h) included.  A launch that fails is not
+ * counted. */
 int64_t ltr_launch_count(void);
 void ltr_reset_launch_count(void);
-/* Per-kernel-class device timing with CUDA events on the launching stream.
- * ltr_profile_begin() arms it; ltr_profile_end() synchronises, fills `names` (pointers to
- * static strings), `ms` (summed elapsed per class) and `launches`, returns the class count. */
+/* Per-kernel-class device timing with CUDA events on the launching stream, one event pair around each
+ * kernel launch.  ltr_profile_begin() arms it; ltr_profile_end() synchronises, fills `names` (pointers to
+ * static strings), `ms` (summed elapsed per class) and `launches` (one per kernel launch issued, debug
+ * hooks included, in class "debug" unless they run a production kernel; failed launches are not counted),
+ * returns the class count. */
 void ltr_profile_begin(void);
 int ltr_profile_end(const char** names, float* ms, int32_t* launches, int32_t max_classes);
 

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <algorithm>
 #include <atomic>
+#include <map>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -19,6 +20,12 @@ int set_error(int code, const std::string& msg);
     cudaError_t _e = (expr);                                                            \
     if (_e != cudaSuccess)                                                              \
       return ::ltr::set_error(-2, std::string(#expr) + ": " + cudaGetErrorString(_e));  \
+  } while (0)
+
+#define LTR_TRY(expr)        \
+  do {                       \
+    int _rc = (expr);        \
+    if (_rc != 0) return _rc; \
   } while (0)
 
 // ---------------------------------------------------------------- instrumentation
@@ -52,6 +59,7 @@ enum KernelClass : int {
   KC_BUNDLE,
   KC_GLOBAL_POSES,
   KC_RETRIEVAL,
+  KC_DEBUG,
   KC_COUNT
 };
 const char* kernel_class_name(int kc);
@@ -72,38 +80,53 @@ struct Profiler {
 };
 extern Profiler g_prof;
 
-// RAII bracket around one kernel launch: counts it, and when profiling is armed records
-// CUDA events on the launching stream (so the measurement sees exactly that kernel).
-struct LaunchScope {
-  cudaStream_t s;
-  cudaEvent_t end = nullptr;
-  LaunchScope(int kc, cudaStream_t stream) : s(stream) {
-    g_launches.fetch_add(1, std::memory_order_relaxed);
-    if (g_prof.on.load(std::memory_order_relaxed)) {
-      std::lock_guard<std::mutex> lk(g_state_mutex);
-      Profiler::Rec r{kc, g_prof.get(), g_prof.get()};
-      cudaEventRecord(r.a, s);
-      g_prof.recs.push_back(r);
-      end = r.b;
-    }
-  }
-  ~LaunchScope() {
-    if (end) cudaEventRecord(end, s);
-  }
-};
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per device AND per kernel: the value set for each
+// (kernel address, device) pair.  Guarded by g_state_mutex.
+inline std::map<std::pair<const void*, int>, size_t>& smem_set() {
+  static std::map<std::pair<const void*, int>, size_t> set;
+  return set;
+}
 
 // ---------------------------------------------------------------- programmatic dependent launch (PDL)
-// Every kernel of the path is launched with programmaticStreamSerialization: its CTAs may become
-// resident as soon as SMs free up at the tail of the previous kernel and run their prologue
-// (barrier init, constant staging) there; pdl_wait() then blocks until the
+// A kernel launched with pdl (programmaticStreamSerialization) may have its CTAs become resident as
+// soon as SMs free up at the tail of the previous kernel and run their prologue (barrier init,
+// constant staging) there; pdl_wait() then blocks until the
 // previous grid has completed and flushed, BEFORE anything it produced is read or anything it
 // still reads is overwritten.  pdl_launch_dependents() at kernel entry lets the next kernel do
 // the same behind this one.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ---------------------------------------------------------------- kernel launch
+// Every kernel the library launches goes through this call, one call per launch, in kernel class kc:
+//  - smem > 0: first raises the kernel's MaxDynamicSharedMemorySize on the current device to smem, unless smem_set()
+//    already holds at least that.  Without it a kernel gets 48 KB of static and dynamic shared memory together, so a
+//    kernel with static shared memory can need it below 48 KB of dynamic.  The encoder's sizes are constant, so no
+//    attribute call happens after its first encode, graph captures included;
+//  - pdl: launched with programmatic stream serialization (the kernel must call pdl_wait(), above);
+//  - profiling armed (ltr_profile_begin): an event pair on s brackets exactly this launch;
+//  - a successful launch is counted (ltr_launch_count).  A failed one is neither counted nor profiled, and returns
+//    LTR_E_CUDA (-2) with "<class> launch: <CUDA error>"; the error is taken off the runtime's last-error state, so the
+//    caller's next CUDA error check does not see it again.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
+inline int launch(int kc, bool pdl, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
+                  Args&&... args) {
+  auto fail = [kc](cudaError_t e) {
+    cudaGetLastError();
+    return set_error(-2, std::string(kernel_class_name(kc)) + " launch: " + cudaGetErrorString(e));
+  };
+  if (smem > 0) {
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return fail(e);
+    std::lock_guard<std::mutex> lk(g_state_mutex);
+    size_t& set = smem_set()[{reinterpret_cast<const void*>(kernel), dev}];
+    if (set < smem) {
+      e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return fail(e);
+      set = smem;
+    }
+  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -113,8 +136,28 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  cfg.numAttrs = pdl ? 1 : 0;
+  Profiler::Rec r{kc, nullptr, nullptr};
+  if (g_prof.on.load(std::memory_order_relaxed)) {
+    std::lock_guard<std::mutex> lk(g_state_mutex);
+    r.a = g_prof.get();
+    r.b = g_prof.get();
+  }
+  if (r.a) cudaEventRecord(r.a, s);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+  if (r.a) {
+    if (e == cudaSuccess) cudaEventRecord(r.b, s);
+    std::lock_guard<std::mutex> lk(g_state_mutex);
+    if (e == cudaSuccess) {
+      g_prof.recs.push_back(r);
+    } else {
+      g_prof.pool.push_back(r.a);
+      g_prof.pool.push_back(r.b);
+    }
+  }
+  if (e != cudaSuccess) return fail(e);
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+  return 0;
 }
 
 // ---------------------------------------------------------------- debug tracing (clock64 stamps of CTA 0)
@@ -139,25 +182,6 @@ __device__ __forceinline__ float warp_max(float v) {
 // Lines of image i: [begin, end).  cu == nullptr means a uniform batch of lpi lines/image.
 __device__ __forceinline__ void image_range(const int* __restrict__ cu, int lpi, int i, int& b, int& e) {
   if (cu) { b = cu[i]; e = cu[i + 1]; } else { b = i * lpi; e = b + lpi; }
-}
-
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per device AND per kernel: remember the
-// (kernel address, device) pairs already configured.  (Kernels sharing a signature share the
-// template instantiation below, so the cache must be keyed by the function pointer.)
-extern std::vector<std::pair<const void*, int>> g_smem_configured;   // guarded by g_state_mutex
-template <typename K>
-inline cudaError_t ensure_dynamic_smem(K kernel, int bytes) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  const void* key = reinterpret_cast<const void*>(kernel);
-  std::lock_guard<std::mutex> lk(g_state_mutex);
-  auto& done = g_smem_configured;
-  for (auto& d : done)
-    if (d.first == key && d.second == dev) return cudaSuccess;
-  e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e == cudaSuccess) done.emplace_back(key, dev);
-  return e;
 }
 
 // SMs of the current device (persistent grids size themselves by it)

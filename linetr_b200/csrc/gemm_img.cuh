@@ -678,14 +678,11 @@ __global__ void __launch_bounds__(384, 1) gemm_img_kernel(GemmImgArgs p) {
 template <int BN, bool FRAG>
 static int launch_gemm_img_bn(GemmImgArgs a, cudaStream_t s) {
   using Cfg = GemmImgCfg<BN>;
-  LTR_CUDA_TRY(ensure_dynamic_smem(gemm_img_kernel<BN, FRAG>, Cfg::SMEM));
   a.m_tiles = cdiv(a.M, 128);
   a.n_blks = a.W.N / BN;
   const int tiles = a.m_tiles * a.n_blks;
   const int grid = tiles < device_sm_count() ? tiles : device_sm_count();
-  LaunchScope ls(KC_LINEAR, s);
-  LTR_CUDA_TRY(launch_pdl(gemm_img_kernel<BN, FRAG>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, a));
-  return 0;
+  return launch(KC_LINEAR, true, gemm_img_kernel<BN, FRAG>, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, a);
 }
 
 // bn_hint: 0 = choose (256 when N % 256 == 0 and that still gives >= 1 tile per SM, else 128)
@@ -923,11 +920,8 @@ inline int launch_gemm_chain(const GemmImgArgs* ops, int n_ops, cudaStream_t s) 
     c.op[i].n_blks = ops[i].W.N / 256;
   }
   using Cfg = GemmImgCfg<256>;
-  LTR_CUDA_TRY(ensure_dynamic_smem(gemm_chain_kernel, Cfg::SMEM));
   const int grid = c.m_tiles < device_sm_count() ? c.m_tiles : device_sm_count();
-  LaunchScope ls(KC_LINEAR, s);
-  LTR_CUDA_TRY(launch_pdl(gemm_chain_kernel, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, c));
-  return 0;
+  return launch(KC_LINEAR, true, gemm_chain_kernel, dim3(grid), dim3(Cfg::THREADS), Cfg::SMEM, s, c);
 }
 
 // ---------------------------------------------------------------- image <-> fp32 helpers

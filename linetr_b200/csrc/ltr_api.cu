@@ -38,7 +38,6 @@ thread_local std::string g_last_error;
 std::atomic<int64_t> g_launches{0};
 Profiler g_prof;
 std::mutex g_state_mutex;
-std::vector<std::pair<const void*, int>> g_smem_configured;
 
 int set_error(int code, const std::string& msg) {
   g_last_error = msg;
@@ -51,7 +50,7 @@ const char* kernel_class_name(int kc) {
                                          "tokenize", "desc_tiles", "match_tc", "match_exact", "match_tail", "line_gt",
                                          "triplet", "homography", "warp", "essential", "photometric",
                                          "fundamental", "absolute_pose", "triangulate", "tracks",
-                                         "bundle", "global_poses", "retrieval"};
+                                         "bundle", "global_poses", "retrieval", "debug"};
   return (kc >= 0 && kc < KC_COUNT) ? names[kc] : "?";
 }
 
@@ -287,23 +286,13 @@ static int gemm(const Lin& L, const ActImg& A, int a_kb0, int M, int act, cudaSt
 static int launch_small_mlp(const SmallMlpWeights& w, const float* in0, const float* in1, const float* in2, ActImg out,
                             int rows, float width, float height, cudaStream_t s) {
   if (rows <= 0) return 0;
-  const int smem = (int)sizeof(SmallMlpSmem);
-  LTR_CUDA_TRY(ensure_dynamic_smem(small_mlp_kernel, smem));
   const int groups = cdiv(rows, SM_ROWS);
   int grid = cdiv(groups, SM_WARPS);
   if (grid > 132 * 3) grid = 132 * 3;
   const float scale = fmaxf(width, height) * 0.7f;
-  LaunchScope ls(KC_SMALL_MLP, s);
-  LTR_CUDA_TRY(launch_pdl(small_mlp_kernel, dim3(grid), dim3(SM_WARPS * 32), (size_t)smem, s, w, in0, in1, in2, out, rows,
-                          width / 2.f, height / 2.f, scale));
-  return 0;
+  return launch(KC_SMALL_MLP, true, small_mlp_kernel, dim3(grid), dim3(SM_WARPS * 32), sizeof(SmallMlpSmem), s, w, in0, in1,
+                in2, out, rows, width / 2.f, height / 2.f, scale);
 }
-
-#define LTR_TRY(expr)        \
-  do {                       \
-    int _rc = (expr);        \
-    if (_rc != 0) return _rc; \
-  } while (0)
 
 static ActImg tiles_image(void* tiles, int64_t n_lines) {
   ActImg a;
@@ -414,11 +403,9 @@ static int encode_impl(LtrModel* m, const LtrEncodeInput& in, float* out_cf, flo
     return flush();
   }
   LTR_TRY(gemm(m->wf, w.xm, 0, R, ACT_NONE, s, w.yf, 256));
-  if (max_l > 0) {
-    LaunchScope ls(KC_FINAL_NORM, s);
-    dim3 grid(cdiv(max_l, 32), in.n_images);
-    LTR_CUDA_TRY(launch_pdl(final_norm_kernel, grid, dim3(256), 0, s, (const float*)w.yf, out_rows, out_cf, cu, in.lines_per_image));
-  }
+  if (max_l > 0)
+    LTR_TRY(launch(KC_FINAL_NORM, true, final_norm_kernel, dim3(cdiv(max_l, 32), in.n_images), dim3(256), 0, s,
+                   (const float*)w.yf, out_rows, out_cf, cu, in.lines_per_image));
   return 0;
 }
 
@@ -427,19 +414,11 @@ static int run_nn(const NNArgs& a, int n_pairs, int max_k0, int max_k1, cudaStre
     LTR_CUDA_TRY(cudaMemsetAsync(a.counts, 0, sizeof(int) * n_pairs, s));
     return 0;
   }
-  {
-    LaunchScope ls(KC_ARGMIN, s);   // also zeroes counts[pair]
-    LTR_CUDA_TRY(launch_pdl(row_argmin_kernel, dim3(cdiv(max_k0, 8), n_pairs), dim3(256), 0, s, a));
-  }
-  if (a.mutual && max_k1 > 0) {
-    LaunchScope ls(KC_ARGMIN, s);
-    LTR_CUDA_TRY(launch_pdl(col_argmin_kernel, dim3(cdiv(max_k1, 32), n_pairs), dim3(256), 0, s, a));
-  }
-  {
-    LaunchScope ls(KC_MUTUAL, s);
-    LTR_CUDA_TRY(launch_pdl(mutual_kernel, dim3(cdiv(max_k0, 256), n_pairs), dim3(256), 0, s, a));
-  }
-  return 0;
+  // row_argmin_kernel also zeroes counts[pair]
+  LTR_TRY(launch(KC_ARGMIN, true, row_argmin_kernel, dim3(cdiv(max_k0, 8), n_pairs), dim3(256), 0, s, a));
+  if (a.mutual && max_k1 > 0)
+    LTR_TRY(launch(KC_ARGMIN, true, col_argmin_kernel, dim3(cdiv(max_k1, 32), n_pairs), dim3(256), 0, s, a));
+  return launch(KC_MUTUAL, true, mutual_kernel, dim3(cdiv(max_k0, 256), n_pairs), dim3(256), 0, s, a);
 }
 
 // Images per launch of the tokenizer kernels: their table travels as a kernel parameter (40 bytes each, 5 KB in
@@ -453,17 +432,10 @@ static int launch_tokenize(const TokLines& L, const TokImages<NI>& I, int s_begi
                            cudaStream_t s) {
   const long long n_tok = (long long)(s_end - s_begin) * L.T;
   if (n_tok <= 0) return LTR_OK;
-  {
-    LaunchScope ls(KC_TOKENIZE, s);
-    tok_points_kernel<NI><<<cdiv(n_tok, 256), 256, 0, s>>>(L, I, s_begin, s_end, pnt, mask, sublines, resp, angle);
-    LTR_CUDA_TRY(cudaGetLastError());
-  }
-  {
-    LaunchScope ls(KC_TOKENIZE, s);
-    tok_sample_kernel<NI><<<cdiv(n_tok, 8), 256, 0, s>>>(L, I, s_begin, s_end, align_corners, pnt, desc, score);
-    LTR_CUDA_TRY(cudaGetLastError());
-  }
-  return LTR_OK;
+  LTR_TRY(launch(KC_TOKENIZE, false, tok_points_kernel<NI>, dim3(cdiv(n_tok, 256)), dim3(256), 0, s, L, I, s_begin, s_end, pnt,
+                 mask, sublines, resp, angle));
+  return launch(KC_TOKENIZE, false, tok_sample_kernel<NI>, dim3(cdiv(n_tok, 8)), dim3(256), 0, s, L, I, s_begin, s_end,
+                align_corners, pnt, desc, score);
 }
 
 }  // namespace ltr
@@ -478,6 +450,7 @@ int64_t ltr_launch_count(void) { return g_launches.load(); }
 void ltr_reset_launch_count(void) { g_launches.store(0); }
 
 void ltr_profile_begin(void) {
+  std::lock_guard<std::mutex> lk(g_state_mutex);
   for (auto& r : g_prof.recs) { g_prof.pool.push_back(r.a); g_prof.pool.push_back(r.b); }
   g_prof.recs.clear();
   g_prof.on = true;
@@ -488,6 +461,7 @@ int ltr_profile_end(const char** names, float* ms, int32_t* launches, int32_t ma
   cudaDeviceSynchronize();
   float tot[KC_COUNT] = {0};
   int cnt[KC_COUNT] = {0};
+  std::lock_guard<std::mutex> lk(g_state_mutex);
   for (auto& r : g_prof.recs) {
     float t = 0.f;
     if (cudaEventElapsedTime(&t, r.a, r.b) == cudaSuccess) { tot[r.kc] += t; cnt[r.kc]++; }
@@ -811,8 +785,7 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
         da.sq[sd] = pl.sq[sd];
         tm = std::max(tm, da.tmax[sd]);
       }
-      LaunchScope ls(KC_DESC_TILES, s);
-      LTR_CUDA_TRY(launch_pdl(desc_tiles_kernel, dim3(tm * 4, P, 2), dim3(256), 0, s, da));
+      LTR_TRY(launch(KC_DESC_TILES, true, desc_tiles_kernel, dim3(tm * 4, P, 2), dim3(256), 0, s, da));
     }
     MatchTcArgs ma{};
     const int* cu[2] = {in.cu0, in.cu1};
@@ -836,9 +809,8 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
     ma.counts = want_nn ? out.counts : nullptr;
     ma.done = want_nn ? pl.done : nullptr;
     ma.n_pairs = P;
-    LTR_CUDA_TRY(ensure_dynamic_smem(match_tc_kernel, MT_SMEM));
-    LaunchScope ls(KC_MATCH_TC, s);
-    LTR_CUDA_TRY(launch_pdl(match_tc_kernel, dim3(pl.tmax[0] + (both ? pl.tmax[1] : 0), P), dim3(MT_THREADS), (size_t)MT_SMEM, s, ma));
+    LTR_TRY(launch(KC_MATCH_TC, true, match_tc_kernel, dim3(pl.tmax[0] + (both ? pl.tmax[1] : 0), P), dim3(MT_THREADS),
+                   (size_t)MT_SMEM, s, ma));
   } else if (want_nn) {
     LTR_CUDA_TRY(cudaMemsetAsync(out.counts, 0, sizeof(int) * P, s));
     LTR_CUDA_TRY(cudaMemsetAsync(pl.done, 0, sizeof(int), s));
@@ -856,9 +828,7 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
       xa.out_off[0] = ix->out_off0; xa.out_off[1] = ix->out_off1;
     }
     const int windows = std::min(cdiv(std::max(pl.mx[0], in.mutual ? pl.mx[1] : 0), MX_WIN), 65535);
-    LTR_CUDA_TRY(ensure_dynamic_smem(match_exact_kernel, MX_SMEM));
-    LaunchScope ls(KC_MATCH_EXACT, s);
-    LTR_CUDA_TRY(launch_pdl(match_exact_kernel, dim3(P, 2, windows), dim3(256), (size_t)MX_SMEM, s, xa));
+    LTR_TRY(launch(KC_MATCH_EXACT, true, match_exact_kernel, dim3(P, 2, windows), dim3(256), (size_t)MX_SMEM, s, xa));
   }
   if (want_nn && pl.mx[0] > 0) {
     MatchTailArgs ta{};
@@ -878,17 +848,14 @@ static int run_match_tc(const LtrMatchInput& in, const LtrMatchOutput& out, cons
       ta.peer_bases = reinterpret_cast<int* const*>(g.peer_bases);
       ta.rank = g.rank; ta.world = g.world; ta.gslot = g.slot; ta.epoch = g.epoch;
     }
-    LaunchScope ls(KC_MATCH_TAIL, s);
-    LTR_CUDA_TRY(launch_pdl(match_tail_kernel, dim3(cdiv(pl.mx[0] + (in.mutual ? pl.mx[1] : 0), 256), P), dim3(256), 0, s, ta));
+    LTR_TRY(launch(KC_MATCH_TAIL, true, match_tail_kernel, dim3(cdiv(pl.mx[0] + (in.mutual ? pl.mx[1] : 0), 256), P),
+                   dim3(256), 0, s, ta));
   }
   return 0;
 }
 
 static int launch_segmean(const SegMeanArgs& a, int max_k0, int max_k1, int n_pairs, cudaStream_t s) {
-  LaunchScope ls(KC_SEGMEAN, s);
-  segmean_kernel<<<dim3(cdiv(max_k1, 32), cdiv(max_k0, 8), n_pairs), 256, 0, s>>>(a);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_SEGMEAN, false, segmean_kernel, dim3(cdiv(max_k1, 32), cdiv(max_k0, 8), n_pairs), dim3(256), 0, s, a);
 }
 
 // the output checks both matcher entries share; `who` (the entry's name) prefixes the message
@@ -934,9 +901,8 @@ static int run_match(const char* who, const LtrMatchInput& in, const LtrPairInde
     da.out = seg ? out.dist_sub : out.dist_key;
     da.stride = seg ? (long long)mx0 * mx1 : stride_key;
     dim3 grid(cdiv(mx0, DK_BM), cdiv(mx1, DK_BN), in.n_pairs);
-    LaunchScope ls(KC_DIST, s);
-    if (in.layout == LTR_LAYOUT_CHANNEL_FIRST) LTR_CUDA_TRY(launch_pdl(dist_kernel<true>, grid, dim3(DK_THREADS), 0, s, da));
-    else LTR_CUDA_TRY(launch_pdl(dist_kernel<false>, grid, dim3(DK_THREADS), 0, s, da));
+    LTR_TRY(launch(KC_DIST, true, in.layout == LTR_LAYOUT_CHANNEL_FIRST ? dist_kernel<true> : dist_kernel<false>, grid,
+                   dim3(DK_THREADS), 0, s, da));
   }
   if (seg && mx0 > 0 && mx1 > 0 && mk0 > 0 && mk1 > 0)
     LTR_TRY(launch_segmean({out.dist_sub, (long long)mx0 * mx1, out.dist_key, stride_key, in.cuk0, in.cuk1, in.sub_off0,
@@ -1007,9 +973,7 @@ int ltr_image_tiles(const float* desc, int32_t layout, const int32_t* cu_dev, co
   da.d[0] = desc; da.cu[0] = cu_dev; da.tile_off[0] = tile_off_dev;
   da.img[0] = tiles_image(out, (int64_t)n_tiles * 128);
   da.tmax[0] = cdiv(max_n, 128);
-  LaunchScope ls(KC_DESC_TILES, s);
-  LTR_CUDA_TRY(launch_pdl(desc_tiles_kernel, dim3(da.tmax[0] * 4, n_images, 1), dim3(256), 0, s, da));
-  return LTR_OK;
+  return launch(KC_DESC_TILES, true, desc_tiles_kernel, dim3(da.tmax[0] * 4, n_images, 1), dim3(256), 0, s, da);
 }
 
 static const char* check_match_indexed(const LtrMatchInput* in, const LtrPairIndex* ix) {
@@ -1050,11 +1014,8 @@ int ltr_gather_wait(const void* local_base, int32_t world, int32_t n_pairs, int3
   if (!local_base || !out || world < 1 || world > 256 || n_pairs < 1 || slot < 0 || slot >= LTR_GATHER_SLOTS)
     return set_error(LTR_E_INVALID, "ltr_gather_wait: bad argument");
   LTR_CUDA_TRY(cudaSetDevice(device));
-  cudaStream_t s = as_stream(stream);
-  LaunchScope ls(KC_MUTUAL, s);
-  LTR_CUDA_TRY(launch_pdl(gather_wait_kernel, dim3(1), dim3(256), 0, s, reinterpret_cast<const int*>(local_base), world, n_pairs, slot,
-                          epoch, out));
-  return LTR_OK;
+  return launch(KC_MUTUAL, true, gather_wait_kernel, dim3(1), dim3(256), 0, as_stream(stream),
+                reinterpret_cast<const int*>(local_base), world, n_pairs, slot, epoch, out);
 }
 
 int ltr_match_distmat(const float* dist, int32_t n_pairs, int32_t n0, int32_t n1, int64_t dist_pair_stride, float nn_thresh,
@@ -1151,10 +1112,7 @@ int ltr_line_gt(const LtrLineGtInput* in, const LtrLineGtOutput* out, int32_t de
                in->thres_reprojected, in->thres_angdiff, in->min_overlap_ratio, out->assign, (long long)out->assign_stride,
                out->n_gt, out->tfpn};
   const dim3 grid(in->n_pairs, cdiv(in->max_n0, LG_ROWS));
-  LaunchScope ls(KC_LINE_GT, s);
-  if (out->assign) LTR_CUDA_TRY(launch_pdl(line_gt_kernel<true>, grid, dim3(LG_ROWS), 0, s, a));
-  else LTR_CUDA_TRY(launch_pdl(line_gt_kernel<false>, grid, dim3(LG_ROWS), 0, s, a));
-  return LTR_OK;
+  return launch(KC_LINE_GT, true, out->assign ? line_gt_kernel<true> : line_gt_kernel<false>, grid, dim3(LG_ROWS), 0, s, a);
 }
 
 int ltr_triplet_loss(const LtrTripletInput* in, const LtrTripletOutput* out, int32_t device, void* stream) {
@@ -1191,18 +1149,14 @@ int ltr_triplet_loss(const LtrTripletInput* in, const LtrTripletOutput* out, int
     a.pred0 = in->pred0;
     a.pos = out->pos; a.neg = out->neg; a.state = out->state; a.tfpn = out->tfpn;
     const int windows = std::min(cdiv(std::max(mx0, mx1), MX_R), 65535);
-    LTR_CUDA_TRY(ensure_dynamic_smem(triplet_mine_kernel, MX_SMEM));
-    LaunchScope ls(KC_TRIPLET, s);
-    LTR_CUDA_TRY(launch_pdl(triplet_mine_kernel, dim3(in->n_pairs, 2, windows), dim3(256), (size_t)MX_SMEM, s, a));
+    LTR_TRY(launch(KC_TRIPLET, true, triplet_mine_kernel, dim3(in->n_pairs, 2, windows), dim3(256), (size_t)MX_SMEM, s, a));
   }
   TripletReduceArgs r{};
   r.cu[0] = in->cu0; r.cu[1] = in->cu1; r.n[0] = in->n0; r.n[1] = in->n1;
   r.group_off = in->group_off; r.n_pairs = in->n_pairs;
   r.pos = out->pos; r.neg = out->neg; r.state = out->state;
   r.loss = out->loss; r.hardest_pos = out->hardest_pos; r.hardest_neg = out->hardest_neg; r.n_valid = out->n_valid;
-  LaunchScope ls(KC_TRIPLET, s);
-  LTR_CUDA_TRY(launch_pdl(triplet_reduce_kernel, dim3(in->n_groups), dim3(256), 0, s, r));
-  return LTR_OK;
+  return launch(KC_TRIPLET, true, triplet_reduce_kernel, dim3(in->n_groups), dim3(256), 0, s, r);
 }
 
 int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out, int32_t device, void* stream) {
@@ -1237,16 +1191,9 @@ int ltr_homography(const LtrHomographyInput* in, const LtrHomographyOutput* out,
                    reinterpret_cast<unsigned long long*>(out->key), out->H, out->valid, out->inliers_p, out->inliers_l,
                    out->n_inliers_p, out->n_inliers_l, out->hypothesis, out->hypothesis_inliers};
   LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_pairs, s));
-  LTR_CUDA_TRY(ensure_dynamic_smem(homography_hyp_kernel, HG_SMEM_MAX));
-  LTR_CUDA_TRY(ensure_dynamic_smem(homography_refit_kernel, HG_SMEM_MAX));
-  {
-    LaunchScope ls(KC_HOMOGRAPHY, s);
-    LTR_CUDA_TRY(launch_pdl(homography_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, HG_THREADS)), dim3(HG_THREADS),
-                            (size_t)hg_smem_bytes(rows_p, rows_l, false), s, a));
-  }
-  LaunchScope ls(KC_HOMOGRAPHY, s);
-  LTR_CUDA_TRY(launch_pdl(homography_refit_kernel, dim3(in->n_pairs), dim3(HG_REFIT_THREADS), (size_t)smem, s, a));
-  return LTR_OK;
+  LTR_TRY(launch(KC_HOMOGRAPHY, true, homography_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, HG_THREADS)),
+                 dim3(HG_THREADS), (size_t)hg_smem_bytes(rows_p, rows_l, false), s, a));
+  return launch(KC_HOMOGRAPHY, true, homography_refit_kernel, dim3(in->n_pairs), dim3(HG_REFIT_THREADS), (size_t)smem, s, a);
 }
 
 int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, int32_t device, void* stream) {
@@ -1276,16 +1223,9 @@ int ltr_essential(const LtrEssentialInput* in, const LtrEssentialOutput* out, in
                   reinterpret_cast<unsigned long long*>(out->key), out->E, out->R, out->t, out->valid, out->inliers_p,
                   out->n_inliers, out->n_cheirality, out->hypothesis, out->hypothesis_inliers};
   LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_pairs, s));
-  LTR_CUDA_TRY(ensure_dynamic_smem(essential_hyp_kernel, ESS_SMEM_MAX));
-  LTR_CUDA_TRY(ensure_dynamic_smem(essential_pose_kernel, ESS_SMEM_MAX));
-  {
-    LaunchScope ls(KC_ESSENTIAL, s);
-    LTR_CUDA_TRY(launch_pdl(essential_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, ESS_THREADS)),
-                            dim3(ESS_THREADS), (size_t)ess_smem_bytes(in->max_rows_p, false), s, a));
-  }
-  LaunchScope ls(KC_ESSENTIAL, s);
-  LTR_CUDA_TRY(launch_pdl(essential_pose_kernel, dim3(in->n_pairs), dim3(ESS_POSE_THREADS), (size_t)smem, s, a));
-  return LTR_OK;
+  LTR_TRY(launch(KC_ESSENTIAL, true, essential_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, ESS_THREADS)),
+                 dim3(ESS_THREADS), (size_t)ess_smem_bytes(in->max_rows_p, false), s, a));
+  return launch(KC_ESSENTIAL, true, essential_pose_kernel, dim3(in->n_pairs), dim3(ESS_POSE_THREADS), (size_t)smem, s, a);
 }
 
 int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* out, int32_t device, void* stream) {
@@ -1321,16 +1261,9 @@ int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* o
                     out->inliers_p, out->lines_consistent, out->refit, out->n_inliers, out->n_lines_consistent,
                     out->hypothesis, out->hypothesis_inliers};
   LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_pairs, s));
-  LTR_CUDA_TRY(ensure_dynamic_smem(fundamental_hyp_kernel, FM_SMEM_MAX));
-  LTR_CUDA_TRY(ensure_dynamic_smem(fundamental_fit_kernel, FM_SMEM_MAX));
-  {
-    LaunchScope ls(KC_FUNDAMENTAL, s);
-    LTR_CUDA_TRY(launch_pdl(fundamental_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, FM_THREADS)),
-                            dim3(FM_THREADS), (size_t)fm_smem_bytes(in->max_rows_p, false), s, a));
-  }
-  LaunchScope ls(KC_FUNDAMENTAL, s);
-  LTR_CUDA_TRY(launch_pdl(fundamental_fit_kernel, dim3(in->n_pairs), dim3(FM_FIT_THREADS), (size_t)smem, s, a));
-  return LTR_OK;
+  LTR_TRY(launch(KC_FUNDAMENTAL, true, fundamental_hyp_kernel, dim3(in->n_pairs, cdiv(in->n_hypotheses, FM_THREADS)),
+                 dim3(FM_THREADS), (size_t)fm_smem_bytes(in->max_rows_p, false), s, a));
+  return launch(KC_FUNDAMENTAL, true, fundamental_fit_kernel, dim3(in->n_pairs), dim3(FM_FIT_THREADS), (size_t)smem, s, a);
 }
 
 int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream) {
@@ -1366,16 +1299,9 @@ int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, in
                 out->valid, out->refit, out->inliers_p, out->inliers_l, out->n_inliers_p, out->n_inliers_l,
                 out->hypothesis, out->hypothesis_inliers};
   LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_groups, s));
-  LTR_CUDA_TRY(ensure_dynamic_smem(abspose_hyp_kernel, AP_SMEM_MAX));
-  LTR_CUDA_TRY(ensure_dynamic_smem(abspose_fit_kernel, AP_SMEM_MAX));
-  {
-    LaunchScope ls(KC_ABSOLUTE_POSE, s);
-    LTR_CUDA_TRY(launch_pdl(abspose_hyp_kernel, dim3(in->n_groups, cdiv(in->n_hypotheses, AP_THREADS)),
-                            dim3(AP_THREADS), (size_t)smem, s, a));
-  }
-  LaunchScope ls(KC_ABSOLUTE_POSE, s);
-  LTR_CUDA_TRY(launch_pdl(abspose_fit_kernel, dim3(in->n_groups), dim3(AP_FIT_THREADS), (size_t)smem, s, a));
-  return LTR_OK;
+  LTR_TRY(launch(KC_ABSOLUTE_POSE, true, abspose_hyp_kernel, dim3(in->n_groups, cdiv(in->n_hypotheses, AP_THREADS)),
+                 dim3(AP_THREADS), (size_t)smem, s, a));
+  return launch(KC_ABSOLUTE_POSE, true, abspose_fit_kernel, dim3(in->n_groups), dim3(AP_FIT_THREADS), (size_t)smem, s, a);
 }
 
 static_assert(LTR_TRI_MAX_VIEWS == ltr::TRI_MAX_VIEWS, "LTR_TRI_MAX_VIEWS and the kernels' bound differ");
@@ -1414,16 +1340,11 @@ int ltr_triangulate(const LtrTriangulateInput* in, const LtrTriangulateOutput* o
   if (in->n_inv_p > 0) LTR_CUDA_TRY(cudaMemsetAsync(out->inv_p, 0x7f, sizeof(int32_t) * in->n_inv_p, s));
   if (in->n_inv_l > 0) LTR_CUDA_TRY(cudaMemsetAsync(out->inv_l, 0x7f, sizeof(int32_t) * in->n_inv_l, s));
   const long long rows = (long long)in->total_p + in->total_l;
-  if (rows > 0) {
-    LaunchScope ls(KC_TRIANGULATE, s);
-    LTR_CUDA_TRY(launch_pdl(tri_scatter_kernel, dim3(cdiv(rows, TRI_SCATTER_THREADS)), dim3(TRI_SCATTER_THREADS), 0,
-                            s, a));
-  }
+  if (rows > 0)
+    LTR_TRY(launch(KC_TRIANGULATE, true, tri_scatter_kernel, dim3(cdiv(rows, TRI_SCATTER_THREADS)), dim3(TRI_SCATTER_THREADS),
+                   0, s, a));
   const int smem = (in->max_views > 0 ? in->max_views : 1) * TRI_THREADS * (int)sizeof(float4);
-  LTR_CUDA_TRY(ensure_dynamic_smem(tri_kernel, TRI_MAX_VIEWS * TRI_THREADS * (int)sizeof(float4)));
-  LaunchScope ls(KC_TRIANGULATE, s);
-  LTR_CUDA_TRY(launch_pdl(tri_kernel, dim3(in->n_blocks), dim3(TRI_THREADS), (size_t)smem, s, a));
-  return LTR_OK;
+  return launch(KC_TRIANGULATE, true, tri_kernel, dim3(in->n_blocks), dim3(TRI_THREADS), (size_t)smem, s, a);
 }
 
 static_assert(LTR_TRK_MAX_OBS == ltr::TRK_MAX_OBS && LTR_TRK_OK == ltr::TRK_OK && LTR_TRK_TOO_LONG == ltr::TRK_TOO_LONG &&
@@ -1469,33 +1390,16 @@ int ltr_tracks(const LtrTracksInput* in, const LtrTracksOutput* out, int32_t dev
             {out->n_images_p, out->n_images_l}, {out->status_p, out->status_l}, out->points3d, out->lines3d,
             out->row_points3d, out->row_lines3d, {out->inlier_p, out->inlier_l}, {out->n_views_p, out->n_views_l}};
   const dim3 node_grid(cdiv(nodes, TRK_ROW_THREADS)), rows(TRK_ROW_THREADS);
-  {
-    LaunchScope ls(KC_TRACKS, s);
-    LTR_CUDA_TRY(launch_pdl(trk_init_kernel, node_grid, rows, 0, s, a));
-  }
+  LTR_TRY(launch(KC_TRACKS, true, trk_init_kernel, node_grid, rows, 0, s, a));
   const long long edges = (long long)in->total_p + in->total_l;
-  if (edges > 0) {
-    LaunchScope ls(KC_TRACKS, s);
-    LTR_CUDA_TRY(launch_pdl(trk_edge_kernel, dim3(cdiv(edges, TRK_ROW_THREADS)), rows, 0, s, a));
-  }
-  {
-    LaunchScope ls(KC_TRACKS, s);
-    LTR_CUDA_TRY(launch_pdl(trk_root_kernel, node_grid, rows, 0, s, a));
-  }
-  {
-    LaunchScope ls(KC_TRACKS, s);
-    LTR_CUDA_TRY(launch_pdl(trk_scan_kernel, dim3(2), dim3(TRK_SCAN_THREADS), 0, s, a));
-  }
-  {
-    LaunchScope ls(KC_TRACKS, s);
-    LTR_CUDA_TRY(launch_pdl(trk_assign_kernel, node_grid, rows, 0, s, a));
-  }
+  if (edges > 0) LTR_TRY(launch(KC_TRACKS, true, trk_edge_kernel, dim3(cdiv(edges, TRK_ROW_THREADS)), rows, 0, s, a));
+  LTR_TRY(launch(KC_TRACKS, true, trk_root_kernel, node_grid, rows, 0, s, a));
+  LTR_TRY(launch(KC_TRACKS, true, trk_scan_kernel, dim3(2), dim3(TRK_SCAN_THREADS), 0, s, a));
+  LTR_TRY(launch(KC_TRACKS, true, trk_assign_kernel, node_grid, rows, 0, s, a));
   // persistent: enough CTAs for the larger bound, at most 8 per SM
   const int bound = std::max(in->n_kp / 2, in->n_kl / 2);
   const int ctas = std::max(1, std::min(bound, 8 * device_sm_count()));
-  LaunchScope ls(KC_TRACKS, s);
-  LTR_CUDA_TRY(launch_pdl(trk_kernel, dim3(ctas, 2), dim3(TRK_THREADS), 0, s, a));
-  return LTR_OK;
+  return launch(KC_TRACKS, true, trk_kernel, dim3(ctas, 2), dim3(TRK_THREADS), 0, s, a);
 }
 
 static_assert(LTR_BA_MAX_IMAGES == ltr::BA_MAX_IMAGES && LTR_BA_IN == ltr::BA_IN &&
@@ -1565,20 +1469,18 @@ int ltr_bundle_adjust(const LtrBundleInput* in, const LtrBundleOutput* out, int3
   a.part = reinterpret_cast<uint8_t*>(take(n));
   const int sms = device_sm_count();
   const dim3 tg(std::max(1, std::min(cdiv(trk, BA_THREADS), 4 * sms))), tb(BA_THREADS);
-  LaunchScope ls(KC_BUNDLE, s);
-  LTR_CUDA_TRY(launch_pdl(ba_start_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
-  LTR_CUDA_TRY(launch_pdl(ba_init_kernel, tg, tb, 0, s, a));
-  LTR_CUDA_TRY(launch_pdl(ba_setup_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
+  LTR_TRY(launch(KC_BUNDLE, true, ba_start_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
+  LTR_TRY(launch(KC_BUNDLE, true, ba_init_kernel, tg, tb, 0, s, a));
+  LTR_TRY(launch(KC_BUNDLE, true, ba_setup_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
   for (int it = 0; it < in->max_iters; ++it) {
-    LTR_CUDA_TRY(launch_pdl(ba_track_kernel, tg, tb, 0, s, a));
-    LTR_CUDA_TRY(launch_pdl(ba_reduce_kernel, dim3(n, n), dim3(64), 0, s, a));
-    LTR_CUDA_TRY(launch_pdl(ba_solve_kernel, dim3(1), dim3(BA_CTA_THREADS), 0, s, a));
-    LTR_CUDA_TRY(launch_pdl(ba_update_kernel, tg, tb, 0, s, a));
-    LTR_CUDA_TRY(launch_pdl(ba_accept_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
+    LTR_TRY(launch(KC_BUNDLE, true, ba_track_kernel, tg, tb, 0, s, a));
+    LTR_TRY(launch(KC_BUNDLE, true, ba_reduce_kernel, dim3(n, n), dim3(64), 0, s, a));
+    LTR_TRY(launch(KC_BUNDLE, true, ba_solve_kernel, dim3(1), dim3(BA_CTA_THREADS), 0, s, a));
+    LTR_TRY(launch(KC_BUNDLE, true, ba_update_kernel, tg, tb, 0, s, a));
+    LTR_TRY(launch(KC_BUNDLE, true, ba_accept_kernel, dim3(1), dim3(BA_COST_THREADS), 0, s, a));
   }
   const dim3 fg(std::max(1, std::min(cdiv(std::max(rows, trk), BA_THREADS), 4 * sms)));
-  LTR_CUDA_TRY(launch_pdl(ba_finish_kernel, fg, tb, 0, s, a));
-  return LTR_OK;
+  return launch(KC_BUNDLE, true, ba_finish_kernel, fg, tb, 0, s, a);
 }
 
 int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* out, int32_t device, void* stream) {
@@ -1624,13 +1526,9 @@ int ltr_global_poses(const LtrGlobalPoseInput* in, const LtrGlobalPoseOutput* ou
   a.deg = reinterpret_cast<int*>(take(4ull * n));
   a.comp = reinterpret_cast<int*>(take(4ull * n));
   a.si = reinterpret_cast<int*>(take(4ull * 16));
-  const size_t smem = gp_smem_bytes(n);
-  LTR_CUDA_TRY(ensure_dynamic_smem(gp_solve_kernel, (int)gp_smem_bytes(GP_MAX_IMAGES)));
-  LaunchScope ls(KC_GLOBAL_POSES, s);
-  LTR_CUDA_TRY(launch_pdl(gp_graph_kernel, dim3(1), dim3(GP_THREADS), 0, s, a));
-  if (P) LTR_CUDA_TRY(launch_pdl(gp_support_kernel, dim3(P), dim3(GP_MAX_IMAGES), 0, s, a));
-  LTR_CUDA_TRY(launch_pdl(gp_solve_kernel, dim3(1), dim3(GP_THREADS), smem, s, a));
-  return LTR_OK;
+  LTR_TRY(launch(KC_GLOBAL_POSES, true, gp_graph_kernel, dim3(1), dim3(GP_THREADS), 0, s, a));
+  if (P) LTR_TRY(launch(KC_GLOBAL_POSES, true, gp_support_kernel, dim3(P), dim3(GP_MAX_IMAGES), 0, s, a));
+  return launch(KC_GLOBAL_POSES, true, gp_solve_kernel, dim3(1), dim3(GP_THREADS), gp_smem_bytes(n), s, a);
 }
 
 static int rt_check_rows(const char* who, const float* desc, const int32_t* cu, int32_t layout, int32_t rows) {
@@ -1665,13 +1563,11 @@ int ltr_kmeans_update(const LtrKmeansInput* in, const LtrKmeansOutput* out, int3
   a.img.hi = static_cast<__nv_bfloat16*>(out->tiles);
   a.img.lo = a.img.hi + (size_t)cdiv(K, 128) * 4 * IMG_TILE_ELEMS;
   a.img.kblocks = 4;
-  LaunchScope ls(KC_RETRIEVAL, s);
   if (!in->init_rows) {
     RtBucketArgs b{in->assign, nullptr, 1, in->n_rows, K, cstart, perm, in->scores, in->scores ? out->cost : nullptr};
-    LTR_CUDA_TRY(launch_pdl(rt_bucket_kernel, dim3(1), dim3(RT_BUCKET_THREADS), 0, s, b));
+    LTR_TRY(launch(KC_RETRIEVAL, true, rt_bucket_kernel, dim3(1), dim3(RT_BUCKET_THREADS), 0, s, b));
   }
-  LTR_CUDA_TRY(launch_pdl(rt_kmeans_kernel, dim3(K), dim3(256), 0, s, a));
-  return LTR_OK;
+  return launch(KC_RETRIEVAL, true, rt_kmeans_kernel, dim3(K), dim3(256), 0, s, a);
 }
 
 int ltr_vlad(const LtrVladInput* in, const LtrVladOutput* out, int32_t device, void* stream) {
@@ -1715,10 +1611,9 @@ int ltr_vlad(const LtrVladInput* in, const LtrVladOutput* out, int32_t device, v
   a.img.hi = static_cast<__nv_bfloat16*>(out->tiles);
   a.img.lo = a.img.hi + (size_t)cdiv(n, 128) * (D / 64) * IMG_TILE_ELEMS;
   a.img.kblocks = D / 64;
-  LaunchScope ls(KC_RETRIEVAL, s);
-  for (int pi = 0; pi < 2; ++pi) LTR_CUDA_TRY(launch_pdl(rt_bucket_kernel, dim3(n), dim3(RT_BUCKET_THREADS), 0, s, b[pi]));
-  LTR_CUDA_TRY(launch_pdl(rt_vlad_kernel, dim3(cdiv(n, 128) * 128), dim3(256), 0, s, a));
-  return LTR_OK;
+  for (int pi = 0; pi < 2; ++pi)
+    LTR_TRY(launch(KC_RETRIEVAL, true, rt_bucket_kernel, dim3(n), dim3(RT_BUCKET_THREADS), 0, s, b[pi]));
+  return launch(KC_RETRIEVAL, true, rt_vlad_kernel, dim3(cdiv(n, 128) * 128), dim3(256), 0, s, a);
 }
 
 int ltr_retrieve(const LtrRetrieveInput* in, const LtrRetrieveOutput* out, int32_t device, void* stream) {
@@ -1753,11 +1648,8 @@ int ltr_retrieve(const LtrRetrieveInput* in, const LtrRetrieveOutput* out, int32
   a.n_full = out->n_full;
   RtMergeArgs m{in->q, in->db, in->Q, in->N, in->D, in->k, a.exclude_self, nt, a.cand_score, a.cand_idx, a.drop,
                 out->idx, out->score, out->n_full};
-  LTR_CUDA_TRY(ensure_dynamic_smem(rt_screen_kernel, RT_SMEM));
-  LaunchScope ls(KC_RETRIEVAL, s);
-  LTR_CUDA_TRY(launch_pdl(rt_screen_kernel, dim3(nt, cdiv(in->Q, 128)), dim3(RT_THREADS), (size_t)RT_SMEM, s, a));
-  LTR_CUDA_TRY(launch_pdl(rt_merge_kernel, dim3(in->Q), dim3(RT_MERGE_THREADS), 0, s, m));
-  return LTR_OK;
+  LTR_TRY(launch(KC_RETRIEVAL, true, rt_screen_kernel, dim3(nt, cdiv(in->Q, 128)), dim3(RT_THREADS), (size_t)RT_SMEM, s, a));
+  return launch(KC_RETRIEVAL, true, rt_merge_kernel, dim3(in->Q), dim3(RT_MERGE_THREADS), 0, s, m);
 }
 
 int ltr_rt_tiles(const float* x, int32_t n, int32_t D, void* tiles, int32_t device, void* stream) {
@@ -1769,9 +1661,7 @@ int ltr_rt_tiles(const float* x, int32_t n, int32_t D, void* tiles, int32_t devi
   img.hi = static_cast<__nv_bfloat16*>(tiles);
   img.lo = img.hi + (size_t)cdiv(n, 128) * (D / 64) * IMG_TILE_ELEMS;
   img.kblocks = D / 64;
-  LaunchScope ls(KC_RETRIEVAL, s);
-  LTR_CUDA_TRY(launch_pdl(rt_tiles_kernel, dim3(cdiv(n, 128) * 128), dim3(256), 0, s, x, n, D, img));
-  return LTR_OK;
+  return launch(KC_RETRIEVAL, true, rt_tiles_kernel, dim3(cdiv(n, 128) * 128), dim3(256), 0, s, x, n, D, img);
 }
 
 int ltr_warp_pairs(const uint8_t* gray, const uint8_t* colour, int32_t n_images, int32_t height, int32_t width,
@@ -1794,9 +1684,7 @@ int ltr_warp_pairs(const uint8_t* gray, const uint8_t* colour, int32_t n_images,
   cudaStream_t s = as_stream(stream);
   WarpArgs a{gray, colour, src_index, inv_maps, warped, mask, n_images, height, width, channels,
              std::min(1024 / std::min(16, (int)height), (int)width), tiles_x, tiles};
-  LaunchScope ls(KC_WARP, s);
-  LTR_CUDA_TRY(launch_pdl(warp_pairs_kernel, dim3(tiles * n_pairs), dim3(WP_THREADS), 0, s, a));
-  return LTR_OK;
+  return launch(KC_WARP, true, warp_pairs_kernel, dim3(tiles * n_pairs), dim3(WP_THREADS), 0, s, a);
 }
 
 static bool ph_is_int(double v, double lo, double hi) { return std::isfinite(v) && v == std::floor(v) && v >= lo && v <= hi; }
@@ -1853,24 +1741,14 @@ int ltr_photometric(const uint8_t* in, uint8_t* out, int32_t n_images, int32_t h
   PhotoArgs a{in, out, params, ellipses, taps, ws, ws + a1, reinterpret_cast<float*>(ws + 2 * a1),
               height, width, max_ellipses};
   LTR_CUDA_TRY(cudaMemsetAsync(a.mask, 0, (size_t)plane, s));
-  {
-    LaunchScope ls(KC_PHOTOMETRIC, s);
-    LTR_CUDA_TRY(launch_pdl(photo_stage1_kernel, dim3(cdiv(width, PS_TW), cdiv(height, PS_TH), n_images),
-                            dim3(PS_THREADS), 0, s, a));
-  }
-  if (max_ellipses > 0) {
-    LaunchScope ls(KC_PHOTOMETRIC, s);
-    LTR_CUDA_TRY(launch_pdl(photo_ellipse_kernel, dim3(max_ellipses, n_images), dim3(PE_THREADS), 0, s, a));
-  }
-  {
-    LaunchScope ls(KC_PHOTOMETRIC, s);
-    LTR_CUDA_TRY(launch_pdl(photo_blur_row_kernel, dim3(cdiv(width, PR_W), cdiv(height, PR_ROWS), n_images),
-                            dim3(PR_ROWS * 32), 0, s, a));
-  }
-  LaunchScope ls(KC_PHOTOMETRIC, s);
-  LTR_CUDA_TRY(launch_pdl(photo_blur_col_kernel, dim3(cdiv(width, PC_W), cdiv(height, PC_H), n_images),
-                          dim3(PC_W * (PC_H / PC_Q)), 0, s, a));
-  return LTR_OK;
+  LTR_TRY(launch(KC_PHOTOMETRIC, true, photo_stage1_kernel, dim3(cdiv(width, PS_TW), cdiv(height, PS_TH), n_images),
+                 dim3(PS_THREADS), 0, s, a));
+  if (max_ellipses > 0)
+    LTR_TRY(launch(KC_PHOTOMETRIC, true, photo_ellipse_kernel, dim3(max_ellipses, n_images), dim3(PE_THREADS), 0, s, a));
+  LTR_TRY(launch(KC_PHOTOMETRIC, true, photo_blur_row_kernel, dim3(cdiv(width, PR_W), cdiv(height, PR_ROWS), n_images),
+                 dim3(PR_ROWS * 32), 0, s, a));
+  return launch(KC_PHOTOMETRIC, true, photo_blur_col_kernel, dim3(cdiv(width, PC_W), cdiv(height, PC_H), n_images),
+                dim3(PC_W * (PC_H / PC_Q)), 0, s, a);
 }
 
 struct NormSpec { int norm; float eps; const float* g; const float* beta; const float* add; int ldadd; };
@@ -1899,14 +1777,11 @@ static int linear_img_impl(const float* x, int32_t ldx, const float* w_host, con
   if (ce == cudaSuccess) {
     ActImg A{reinterpret_cast<__nv_bfloat16*>(da), reinterpret_cast<__nv_bfloat16*>(da + mpad * k), k / 64};
     ActImg O{reinterpret_cast<__nv_bfloat16*>(dout), reinterpret_cast<__nv_bfloat16*>(dout + mpad * n), n / 64};
-    {
-      LaunchScope ls(KC_IMG_CONVERT, s);
-      to_image_kernel<<<cdiv((long long)m * (k / 8), 256), 256, 0, s>>>(x, ldx, m, k, A, 0);
-    }
-    if (res_image) {
-      LaunchScope ls(KC_IMG_CONVERT, s);
-      to_image_kernel<<<cdiv((long long)m * (n / 8), 256), 256, 0, s>>>(res, ldr, m, n, O, 0);
-    }
+    rc = launch(KC_IMG_CONVERT, false, to_image_kernel, dim3(cdiv((long long)m * (k / 8), 256)), dim3(256), 0, s, x, ldx, m, k,
+                A, 0);
+    if (rc == 0 && res_image)
+      rc = launch(KC_IMG_CONVERT, false, to_image_kernel, dim3(cdiv((long long)m * (n / 8), 256)), dim3(256), 0, s, res, ldr, m,
+                  n, O, 0);
     GemmImgArgs a{};
     a.A = A; a.a_kb0 = 0; a.bias = bias; a.C = y; a.ldc = ldy; a.M = m; a.act = act;
     if (res_image) { a.Rimg = O; a.r_kb0 = 0; } else { a.R = res; a.ldr = ldr; }
@@ -1915,11 +1790,10 @@ static int linear_img_impl(const float* x, int32_t ldx, const float* w_host, con
     a.W.N = n; a.W.K = k;
     if (y_from_image) { a.O = O; a.o_kb0 = 0; }
     a.norm = ns.norm; a.eps = ns.eps; a.ng = ns.g; a.nbeta = ns.beta; a.nadd = ns.add; a.ldadd = ns.ldadd;
-    rc = launch_gemm_img(a, s, bn_hint);
-    if (rc == 0 && y_from_image) {
-      LaunchScope ls(KC_IMG_CONVERT, s);
-      from_image_kernel<<<cdiv((long long)m * n, 256), 256, 0, s>>>(O, 0, y_from_image, n, m, n);
-    }
+    if (rc == 0) rc = launch_gemm_img(a, s, bn_hint);
+    if (rc == 0 && y_from_image)
+      rc = launch(KC_IMG_CONVERT, false, from_image_kernel, dim3(cdiv((long long)m * n, 256)), dim3(256), 0, s, O, 0,
+                  y_from_image, n, m, n);
     ce = cudaStreamSynchronize(s);
   }
   cudaFree(dw); cudaFree(da); cudaFree(dout);
@@ -2109,9 +1983,8 @@ int ltr_debug_sturm_roots(const double* poly, int32_t n, double* roots, int32_t*
   if (n < 0 || (n > 0 && (!poly || !roots || !count))) return set_error(LTR_E_INVALID, "ltr_debug_sturm_roots: bad argument");
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
-  debug_sturm_roots_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(poly, n, roots, count);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_DEBUG, false, debug_sturm_roots_kernel, dim3(cdiv(n, 128)), dim3(128), 0, as_stream(stream), poly, n,
+                roots, count);
 }
 
 int ltr_debug_essential_solve(const double* q, int32_t n, double* E, int32_t* root_index, int32_t* n_solutions,
@@ -2120,9 +1993,8 @@ int ltr_debug_essential_solve(const double* q, int32_t n, double* E, int32_t* ro
     return set_error(LTR_E_INVALID, "ltr_debug_essential_solve: bad argument");
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
-  debug_essential_solve_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(q, n, E, root_index, n_solutions);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_DEBUG, false, debug_essential_solve_kernel, dim3(cdiv(n, 128)), dim3(128), 0, as_stream(stream), q, n, E,
+                root_index, n_solutions);
 }
 
 int ltr_debug_fundamental_solve(const double* q, int32_t n, double* F, int32_t* root_index, int32_t* n_solutions,
@@ -2131,9 +2003,8 @@ int ltr_debug_fundamental_solve(const double* q, int32_t n, double* F, int32_t* 
     return set_error(LTR_E_INVALID, "ltr_debug_fundamental_solve: bad argument");
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
-  debug_fundamental_solve_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(q, n, F, root_index, n_solutions);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_DEBUG, false, debug_fundamental_solve_kernel, dim3(cdiv(n, 128)), dim3(128), 0, as_stream(stream), q, n, F,
+                root_index, n_solutions);
 }
 
 int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double* t, int32_t* root_index,
@@ -2142,9 +2013,8 @@ int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double
     return set_error(LTR_E_INVALID, "ltr_debug_p3p: bad argument");
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
-  debug_p3p_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(j, X, n, R, t, root_index, n_solutions);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_DEBUG, false, debug_p3p_kernel, dim3(cdiv(n, 128)), dim3(128), 0, as_stream(stream), j, X, n, R, t,
+                root_index, n_solutions);
 }
 
 int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s1, int32_t n, double min_overlap,
@@ -2153,9 +2023,8 @@ int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s
     return set_error(LTR_E_INVALID, "ltr_debug_fundamental_lines: bad argument");
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
-  debug_fundamental_lines_kernel<<<cdiv(n, 128), 128, 0, as_stream(stream)>>>(F, s0, s1, n, min_overlap, r1, r0, ok);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_DEBUG, false, debug_fundamental_lines_kernel, dim3(cdiv(n, 128)), dim3(128), 0, as_stream(stream), F, s0,
+                s1, n, min_overlap, r1, r0, ok);
 }
 
 int ltr_debug_cholesky_solve(double* A, int32_t n, int32_t m, int32_t ld, double* x, int32_t k, int32_t shared,
@@ -2166,11 +2035,8 @@ int ltr_debug_cholesky_solve(double* A, int32_t n, int32_t m, int32_t ld, double
   if (n == 0) return LTR_OK;
   LTR_CUDA_TRY(cudaSetDevice(device));
   const size_t smem = 8 * (shared ? (size_t)m * m + (size_t)m * k + m : (size_t)(m > 0 ? m : 1));
-  // the largest shared case (m = 127, k = 6: gp_smem_bytes(128)) once, so the attribute holds for every later call
-  LTR_CUDA_TRY(ensure_dynamic_smem(debug_cholesky_kernel, (int)gp_smem_bytes(GP_MAX_IMAGES)));
-  debug_cholesky_kernel<<<n, DEBUG_CHOL_THREADS, smem, as_stream(stream)>>>(A, m, ld, x, k, shared, ok);
-  LTR_CUDA_TRY(cudaGetLastError());
-  return LTR_OK;
+  return launch(KC_DEBUG, false, debug_cholesky_kernel, dim3(n), dim3(DEBUG_CHOL_THREADS), smem, as_stream(stream), A, m, ld, x,
+                k, shared, ok);
 }
 
 float ltr_gemm_bench(int32_t m, int32_t n, int32_t k, int32_t bn_hint, int32_t out_mode, int32_t iters, int32_t device) {

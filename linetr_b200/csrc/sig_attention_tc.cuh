@@ -469,18 +469,12 @@ inline int launch_sig_attention_tc(ActImg qkv, ActImg out, int out_k0, const int
                                    int n_images, cudaStream_t s) {
   if (max_l <= 0 || n_images <= 0) return 0;
   if (!cu && lpi == 128 && attn_pipe_enabled()) {
-    LTR_CUDA_TRY(ensure_dynamic_smem(sig_attention_pipe_kernel, SigAttnPipeSmem::TOTAL));
     const int grid = std::min(n_images, device_sm_count());
-    LaunchScope ls(KC_SIG_ATTN, s);
-    LTR_CUDA_TRY(launch_pdl(sig_attention_pipe_kernel, dim3(grid), dim3(384), SigAttnPipeSmem::TOTAL, s, qkv, out, out_k0,
-                            n_images));
-    return 0;
+    return launch(KC_SIG_ATTN, true, sig_attention_pipe_kernel, dim3(grid), dim3(384), SigAttnPipeSmem::TOTAL, s, qkv, out,
+                  out_k0, n_images);
   }
-  LTR_CUDA_TRY(ensure_dynamic_smem(sig_attention_tc_kernel, SigAttnSmem::TOTAL));
   dim3 grid(cdiv(max_l, 128), 4, n_images);
-  LaunchScope ls(KC_SIG_ATTN, s);
-  LTR_CUDA_TRY(launch_pdl(sig_attention_tc_kernel, grid, dim3(256), SigAttnSmem::TOTAL, s, qkv, out, out_k0, cu, lpi));
-  return 0;
+  return launch(KC_SIG_ATTN, true, sig_attention_tc_kernel, grid, dim3(256), SigAttnSmem::TOTAL, s, qkv, out, out_k0, cu, lpi);
 }
 
 }  // namespace ltr

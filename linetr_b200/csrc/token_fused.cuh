@@ -455,7 +455,6 @@ inline int launch_token_fused(TokenFusedArgs a, cudaStream_t s) {
   if (a.T < 1 || a.T > 128) return set_error(-1, "token_fused: T must be in 1..128");
   if ((long long)a.R * a.T >= (1ll << 31)) return set_error(-1, "token_fused: more than 2^31 tokens in one call");
   if (reinterpret_cast<uintptr_t>(a.desc) % 16) return set_error(-1, "token_fused: desc_sublines must be 16-byte aligned");
-  LTR_CUDA_TRY(ensure_dynamic_smem(token_fused_kernel, TokenFusedSmem::TOTAL));
   a.lpt = 128 / a.T;
   a.n_tiles = cdiv(a.R, a.lpt);
   // tensor map of the sampled descriptors viewed as [R*T rows, 256] fp32; box = 32 columns (128 B) x 128 rows
@@ -475,9 +474,7 @@ inline int launch_token_fused(TokenFusedArgs a, cudaStream_t s) {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if (sms <= 0) sms = 132;
   const int grid = a.n_tiles < sms ? a.n_tiles : sms;
-  LaunchScope ls(KC_TOKEN_FUSED, s);
-  LTR_CUDA_TRY(launch_pdl(token_fused_kernel, dim3(grid), dim3(384), TokenFusedSmem::TOTAL, s, a, map));
-  return 0;
+  return launch(KC_TOKEN_FUSED, true, token_fused_kernel, dim3(grid), dim3(384), TokenFusedSmem::TOTAL, s, a, map);
 }
 
 }  // namespace ltr

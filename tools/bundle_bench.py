@@ -213,7 +213,8 @@ def main():
     keys = ("rot_deg", "centre", "point", "line")
     print(f"{gpu}: {V} posed images, {len(pairs)} pairs, {args.points} keypoints and {args.lines} key lines per image, "
           f"{args.outliers:.0%} moved, poses perturbed {args.deg} deg / {args.shift}")
-    print(f"  bundle_adjust call median {med:8.3f} ms (min {lo:.3f}, max {hi:.3f}); kernels {kern[0]:.3f} ms; "
+    print(f"  bundle_adjust call median {med:8.3f} ms (min {lo:.3f}, max {hi:.3f}); kernels {kern[0]:.3f} ms in "
+          f"{kern[1]} launches; "
           f"{st['iterations']} iterations, {st['accepted']} accepted, stop {st['stop_reason']}; cost "
           f"{st['initial_cost']:.1f} -> {st['final_cost']:.1f} over {st['n_obs']} rows of {st['n_tracks']} tracks")
     print("  kernels (ms, launches): " + ", ".join(f"{k} {v[0]:.3f} ({v[1]})" for k, v in per_kernel.items()))
