@@ -728,6 +728,24 @@ typedef struct {
  * [groups[0], groups[n_groups]). */
 int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream);
 
+/* ltr_absolute_pose with line hypotheses too: n_line_hypotheses (0 to 2^21) hypotheses for each of three minimal
+ * solvers that use line matches, next to the n_hypotheses P3P ones and competing for the same winner (DESIGN.md
+ * "Absolute pose"):
+ *   - solver s = 0 P2P1L (2 point rows, 1 line row), 1 P1P2L (1 point, 2 lines), 2 P3L (3 lines); it draws its point
+ *     rows with seed + 2 s + 1 and its line rows with seed + 2 s + 2, and runs only in groups with that many rows;
+ *   - a line row constrains the pose by both world end points lying on the plane through the camera centre and the
+ *     query segment; each solver reduces its six constraints to two equations in the two angles of R' = Rz(a) Rx(b)
+ *     between a world and a camera triad, and up to 8 solutions j (real root j of a degree-8 polynomial in tan(b / 2),
+ *     ascending; b = pi is not found);
+ *   - hypothesis k of solver s has index 4 n_hypotheses + 8 (s n_line_hypotheses + k) + j; ties still go to the
+ *     lowest index, so P3P wins equal counts.  A group without point rows can be valid.
+ * Samples degenerate for their solver have no solution: |j1 x j2| <= 1e-10 for P2P1L's two unit bearings, |n1 . j1|
+ * <= 1e-10 |n1| for P1P2L (the point on line 1), |n1 . (n2 x n3)| <= 1e-10 |n1| |n2| |n3| for P3L (concurrent query
+ * lines).  With n_line_hypotheses > 0, n_hypotheses may be 0 and use_lines is required (LTR_E_INVALID otherwise);
+ * with 0 this is ltr_absolute_pose, the same bits. */
+int ltr_absolute_pose_lines(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t n_line_hypotheses,
+                            int32_t device, void* stream);
+
 /* Triangulation of posed images: a world point for every keypoint and two world end points for every key line of every
  * image, from the pair matches of the set (ltr_match_indexed / match_set); DESIGN.md "Triangulation" states the model:
  *   - image i has intrinsics K[i] (zero skew: fx, fy, cx, cy are read) and the world -> camera pose X_cam = R[i] X +

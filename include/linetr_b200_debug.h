@@ -77,6 +77,15 @@ int ltr_debug_fundamental_solve(const double* q, int32_t n, double* F, int32_t* 
 int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double* t, int32_t* root_index,
                   int32_t* n_solutions, int32_t device, void* stream);
 
+/* The absolute-pose estimator's line solvers on their own, one thread per sample of solver 0 (P2P1L), 1 (P1P2L) or 2
+ * (P3L): j and X [count, 2 - solver, 3] unit bearings and world points of the sample's points (NULL for P3L), n
+ * [count, solver + 1, 3] camera-ray normals of its query lines and E [count, solver + 1, 2, 3] the world end points
+ * of its lines (device) -> R [count, 8, 9] row-major, t [count, 8, 3] (X_cam = R X + t), root_index [count, 8] (the
+ * real root of the degree-8 polynomial each pose came from) and n_solutions [count] (device); entries past
+ * n_solutions are NaN / -1.  The same compiled function the estimator runs. */
+int ltr_debug_line_pose(int32_t solver, const double* j, const double* X, const double* n, const double* E, int32_t count,
+                        double* R, double* t, int32_t* root_index, int32_t* n_solutions, int32_t device, void* stream);
+
 /* The fundamental-matrix estimator's line check on its own, one thread per key-line pair: F [n, 9] pixel F (row-major,
  * fp64), s0 / s1 [n, 4] the matched segments (a, b; fp32) -> r1 [n] (the overlap ratio in image 1), r0 [n] (in
  * image 0; NaN where the side cannot reject) and ok [n] (1 iff consistent at min_overlap in [0, 1]; device).  The same

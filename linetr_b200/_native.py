@@ -382,6 +382,7 @@ PROTOTYPES = {
     "ltr_essential": (C.c_int, [_ptr(LtrEssentialInput), _ptr(LtrEssentialOutput), _I32, _P]),
     "ltr_fundamental": (C.c_int, [_ptr(LtrFundamentalInput), _ptr(LtrFundamentalOutput), _I32, _P]),
     "ltr_absolute_pose": (C.c_int, [_ptr(LtrAbsPoseInput), _ptr(LtrAbsPoseOutput), _I32, _P]),
+    "ltr_absolute_pose_lines": (C.c_int, [_ptr(LtrAbsPoseInput), _ptr(LtrAbsPoseOutput), _I32, _I32, _P]),
     "ltr_triangulate": (C.c_int, [_ptr(LtrTriangulateInput), _ptr(LtrTriangulateOutput), _I32, _P]),
     "ltr_tracks": (C.c_int, [_ptr(LtrTracksInput), _ptr(LtrTracksOutput), _I32, _P]),
     "ltr_bundle_adjust": (C.c_int, [_ptr(LtrBundleInput), _ptr(LtrBundleOutput), _I32, _P]),
@@ -413,6 +414,7 @@ DEBUG_PROTOTYPES = {
     "ltr_debug_essential_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),
     "ltr_debug_fundamental_solve": (C.c_int, [_P, _I32, _P, _P, _P, _I32, _P]),
     "ltr_debug_p3p": (C.c_int, [_P, _P, _I32, _P, _P, _P, _P, _I32, _P]),
+    "ltr_debug_line_pose": (C.c_int, [_I32, _P, _P, _P, _P, _I32, _P, _P, _P, _P, _I32, _P]),
     "ltr_debug_fundamental_lines": (C.c_int, [_P, _P, _P, _I32, C.c_double, _P, _P, _P, _I32, _P]),
     "ltr_debug_cholesky_solve": (C.c_int, [_P, _I32, _I32, _I32, _P, _I32, _I32, _P, _I32, _P]),
 }

@@ -389,16 +389,17 @@ def _layout(cls):
     return frozenset(nm for nm, _ in cls._fields_), ptrs, scalars
 
 
-def call_struct(entry: str, inputs: dict, outputs: dict, workspace_bytes=None):
-    """`entry`(const In*, const Out*, device, stream) with the fields of its In and Out structs by name: every scalar
-    field is required; a pointer field takes None (NULL) or a contiguous CUDA tensor of the dtype its mirror names (any
-    dtype for void*), on the device of the outputs.  Runs on that device's current stream.  workspace_bytes, when given,
-    is the least size of the `workspace` output.  The caller keeps the tensors alive until the call."""
+def call_struct(entry: str, inputs: dict, outputs: dict, workspace_bytes=None, scalars=()):
+    """`entry`(const In*, const Out*, *scalars, device, stream) with the fields of its In and Out structs by name (and
+    the entry's own scalar arguments after the structs, in order): every scalar field is required; a pointer field
+    takes None (NULL) or a contiguous CUDA tensor of the dtype its mirror names (any dtype for void*), on the device of
+    the outputs.  Runs on that device's current stream.  workspace_bytes, when given, is the least size of the
+    `workspace` output.  The caller keeps the tensors alive until the call."""
     who = entry[4:]
     _, (p_in, p_out, *_) = N.PROTOTYPES[entry]
     dev, structs = None, {}
     for cls, given in ((p_out._type_, outputs), (p_in._type_, inputs)):
-        names, ptrs, scalars = _layout(cls)
+        names, ptrs, fixed = _layout(cls)
         if not given.keys() <= names:
             raise N.LtrError(f"{who}: {cls.__name__} has no field {sorted(given.keys() - names)}")
         fields = {}
@@ -411,7 +412,7 @@ def call_struct(entry: str, inputs: dict, outputs: dict, workspace_bytes=None):
             if (dts is not None and t.dtype not in dts) or not t.is_contiguous() or t.device != dev:
                 raise N.LtrError(f"{who}: '{nm}' must be a contiguous {f'{dts[0]} ' if dts else ''}tensor on {dev}")
             fields[nm] = t.data_ptr()
-        for nm, conv in scalars:
+        for nm, conv in fixed:
             if nm not in given:
                 raise N.LtrError(f"{who}: {cls.__name__}.{nm} is not given")
             fields[nm] = conv(given[nm])
@@ -421,7 +422,7 @@ def call_struct(entry: str, inputs: dict, outputs: dict, workspace_bytes=None):
         if ws.numel() * ws.element_size() < workspace_bytes:
             raise N.LtrError(f"{who}: the workspace holds {ws.numel() * ws.element_size()} bytes, {workspace_bytes} "
                              "needed")
-    _call(entry, dev, C.byref(structs[p_in._type_]), C.byref(structs[p_out._type_]))
+    _call(entry, dev, C.byref(structs[p_in._type_]), C.byref(structs[p_out._type_]), *scalars)
 
 
 def warp_pairs(gray, colour, src_index_host: np.ndarray, src_index, inv_maps, warped, mask):

@@ -16,7 +16,10 @@
 //   inlier (pixels through K0): a point iff depth > 0 and |fx Px - (kx - cx) Pz|^2 + |fy Py - (ky - cy) Pz|^2 <
 //   thresh^2 Pz^2 (the squared reprojection error below thresh^2 without the division); a line iff both end points
 //   have depth > 0 and (n . P)^2 < thresh^2 Pz^2 for each, n the query line through s0 in camera-ray form.
-//   winner: most inliers (points and lines), then lowest k, then lowest j (atomicMax of (count << 32) | ~(4 k + j)).
+//   line hypotheses (ltr_absolute_pose_lines): hypothesis k of line solver s (0 P2P1L, 1 P1P2L, 2 P3L) draws 2 - s
+//   point rows and s + 1 line rows and solves them through two bilinear trigonometric equations (ap_line_pose), up to
+//   8 solutions; its index is 4 n_hyp + 8 (s n_line_hyp + k) + j.
+//   winner: most inliers (points and lines), then lowest index (atomicMax of (count << 32) | ~index, 4 k + j for P3P).
 //   refit (at least AP_MIN_REFIT winner inliers): Levenberg-Marquardt over the winner's inliers, R <- cay(w) R,
 //   t <- t + dt, J^T J and J^T r summed in a fixed order, the damped 6 x 6 system by Gaussian elimination with partial
 //   pivoting, a fixed budget and damping schedule; kept iff its inlier count >= the hypothesis'.
@@ -24,6 +27,8 @@
 // Kernels:
 //   abspose_hyp_kernel  grid (group, chunk of AP_THREADS hypotheses): stage the group's rows, one hypothesis per
 //                       thread (P3P + up to 4 solutions scored against every staged row), one atomicMax per CTA.
+//   abspose_line_hyp_kernel  grid (group, chunk of AP_THREADS over 3 n_line_hyp): the same for the line hypotheses
+//                       (up to 8 solutions each), into the same key; launched only with n_line_hyp > 0.
 //   abspose_fit_kernel  grid (group): the winner again, the block-parallel refit, the masks, counts and pose.
 #pragma once
 #include "common.cuh"
@@ -42,6 +47,14 @@ constexpr double AP_LM_LAMBDA0 = 1e-3;     // initial damping (A_ii + lambda A_i
 constexpr double AP_LM_ACCEPT = 0.1;       // damping factor after a step that lowers the cost
 constexpr double AP_LM_REJECT = 10.0;      // damping factor after one that does not
 constexpr double AP_COLLINEAR_EPS = 1e-10;
+// Line hypotheses (ap_line_pose): solver s = 0 P2P1L, 1 P1P2L, 2 P3L samples 2 - s point and s + 1 line rows and
+// gives up to AP_LINE_MAX_SOLUTIONS poses (the real roots of a degree-8 polynomial).
+constexpr int AP_LINE_SOLVERS = 3;
+constexpr int AP_LINE_MAX_SOLUTIONS = 8;
+constexpr int AP_LINE_MAX_HYP = 1 << 21;   // n_line_hypotheses bound: the index space fits int32, the grid y 65535
+constexpr double AP_BEARING_EPS = 1e-10;    // P2P1L: |j1 x j2| of the unit bearings at most this rejects the sample
+constexpr double AP_POINT_LINE_EPS = 1e-10; // P1P2L: |n1 . j1| / |n1| at most this (the point on line 1) rejects it
+constexpr double AP_CONCURRENT_EPS = 1e-10; // P3L: |n1 . (n2 x n3)| at most this times |n1| |n2| |n3| rejects it
 constexpr int AP_PT_BYTES = 32;            // shared bytes per point row: query pixel fp32, world point fp64
 constexpr int AP_LN_BYTES = 64;            // per line row: query segment fp32, two world end points fp64
 constexpr int AP_SMEM_MAX = 200 * 1024;
@@ -58,6 +71,7 @@ struct AbsPoseArgs {
   int rows_p, rows_l;                        // staging rows per group (rows_l 0: lines unused)
   double thresh2;
   int n_hyp;
+  int n_line_hyp;                            // hypotheses per line solver
   unsigned long long seed;
   unsigned long long* key;
   double* R; double* t; uint8_t* valid; uint8_t* refit; uint8_t* inl_p; uint8_t* inl_l;
@@ -292,6 +306,309 @@ __device__ __forceinline__ int ap_hypothesis(const ApStage& st, const ApGroup& s
   return ap_p3p(j, X, Rs, ts, jr);
 }
 
+// ---- line hypotheses: P2P1L, P1P2L and P3L through one pair of bilinear trigonometric equations
+// The rotation between a world triad H and a camera triad G (rows) is R' = Rz(a) Rx(b), R = G^T R' H.  Each solver
+// gives two equations [cos a, sin a, 1] M_i [cos b, sin b, 1]^T = 0; tau = tan(b / 2) makes row r of M_i the
+// quadratic q_ir = M_i[r][0] (1 - tau^2) + 2 M_i[r][1] tau + M_i[r][2] (1 + tau^2), A_i, B_i, C_i = rows 0, 1, 2, and
+// with D = A1 B2 - A2 B1, X = B1 C2 - B2 C1, Y = A2 C1 - A1 C2 (cos a, sin a) = (X, Y) / D on X^2 + Y^2 - D^2 = 0.
+// b = pi (tau = inf) is not found.
+
+// Point and line rows of a sample of solver s.
+__host__ __device__ constexpr int ap_line_np(int s) { return 2 - s; }
+__host__ __device__ constexpr int ap_line_nl(int s) { return s + 1; }
+
+// The coefficients of n' . Rz(a) Rx(b) E' in M (row-major; rows cos a, sin a, 1; columns cos b, sin b, 1).
+__device__ __forceinline__ void ap_trig_terms(const double* n, const double* E, double* M) {
+  M[0] = RC_M(n[1], E[1]);
+  M[1] = -RC_M(n[1], E[2]);
+  M[2] = RC_M(n[0], E[0]);
+  M[3] = -RC_M(n[0], E[1]);
+  M[4] = RC_M(n[0], E[2]);
+  M[5] = RC_M(n[1], E[0]);
+  M[6] = RC_M(n[2], E[2]);
+  M[7] = RC_M(n[2], E[1]);
+  M[8] = 0.0;
+}
+
+// c = a b (ascending coefficients; a has na, b nb), each c[k] summed over a's index ascending from 0.
+__device__ __forceinline__ void ap_pmul(const double* a, int na, const double* b, int nb, double* c) {
+  for (int k = 0; k < na + nb - 1; ++k) {
+    double acc = 0.0;
+    for (int i = 0; i < na; ++i)
+      if (k - i >= 0 && k - i < nb) acc = RC_A(acc, RC_M(a[i], b[k - i]));
+    c[k] = acc;
+  }
+}
+
+// The quartics D, X, Y [5] and p = (X^2 + Y^2) - D^2 [11] (degree 8, zero-padded) of M1, M2 [9].
+__device__ __noinline__ void ap_trig_poly(const double* M1, const double* M2, double* D, double* X, double* Y,
+                                          double* p) {
+  double q[2][3][3];   // q[i][r]: row r of M_i as a quadratic in tau
+  for (int i = 0; i < 2; ++i) {
+    const double* M = i ? M2 : M1;
+    for (int r = 0; r < 3; ++r) {
+      q[i][r][0] = RC_A(M[3 * r], M[3 * r + 2]);
+      q[i][r][1] = RC_M(2.0, M[3 * r + 1]);
+      q[i][r][2] = RC_S(M[3 * r + 2], M[3 * r]);
+    }
+  }
+  double u[5], v[5];
+  ap_pmul(q[0][0], 3, q[1][1], 3, u);
+  ap_pmul(q[1][0], 3, q[0][1], 3, v);
+  for (int k = 0; k < 5; ++k) D[k] = RC_S(u[k], v[k]);
+  ap_pmul(q[0][1], 3, q[1][2], 3, u);
+  ap_pmul(q[1][1], 3, q[0][2], 3, v);
+  for (int k = 0; k < 5; ++k) X[k] = RC_S(u[k], v[k]);
+  ap_pmul(q[1][0], 3, q[0][2], 3, u);
+  ap_pmul(q[0][0], 3, q[1][2], 3, v);
+  for (int k = 0; k < 5; ++k) Y[k] = RC_S(u[k], v[k]);
+  double xx[9], yy[9], dd[9];
+  ap_pmul(X, 5, X, 5, xx);
+  ap_pmul(Y, 5, Y, 5, yy);
+  ap_pmul(D, 5, D, 5, dd);
+  for (int k = 0; k < 9; ++k) p[k] = RC_S(RC_A(xx[k], yy[k]), dd[k]);
+  p[9] = p[10] = 0.0;
+}
+
+__device__ __forceinline__ double ap_horner4(const double* c, double x) {
+  double v = c[4];
+  for (int k = 3; k >= 0; --k) v = RC_A(RC_M(v, x), c[k]);
+  return v;
+}
+
+// (cos a, sin a, cos b, sin b) at the root tau of p.  -> false where D(tau) == 0.
+__device__ __forceinline__ bool ap_trig_angles(const double* D, const double* X, const double* Y, double tau,
+                                               double* cs) {
+  const double d = ap_horner4(D, tau);
+  if (d == 0.0) return false;
+  const double c = RC_D(ap_horner4(X, tau), d), s = RC_D(ap_horner4(Y, tau), d);
+  const double nr = __dsqrt_rn(RC_A(RC_M(c, c), RC_M(s, s)));
+  const double t2 = RC_M(tau, tau), den = RC_A(1.0, t2);
+  cs[0] = RC_D(c, nr);
+  cs[1] = RC_D(s, nr);
+  cs[2] = RC_D(RC_S(1.0, t2), den);
+  cs[3] = RC_D(RC_M(2.0, tau), den);
+  return true;
+}
+
+// T rows (f, u, v): the unit f, then u = f x e / |f x e| for the coordinate axis e least aligned with f (the first of
+// the smallest |f_k|), v = f x u; a right-handed orthonormal frame.
+__device__ __forceinline__ void ap_triad(const double* f, double* T) {
+  int k = 0;
+  if (fabs(f[1]) < fabs(f[k])) k = 1;
+  if (fabs(f[2]) < fabs(f[k])) k = 2;
+  double e[3] = {0.0, 0.0, 0.0}, c[3];
+  e[k] = 1.0;
+  rc_cross3(f, e, c);
+  const double nc = __dsqrt_rn(rc_dot3(c, c));
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    T[i] = f[i];
+    T[3 + i] = RC_D(c[i], nc);
+  }
+  rc_cross3(T, T + 3, T + 6);
+}
+
+// The unit vector of v.  -> |v|.
+__device__ __forceinline__ double ap_unit(const double* v, double* u) {
+  const double n = __dsqrt_rn(rc_dot3(v, v));
+#pragma unroll
+  for (int i = 0; i < 3; ++i) u[i] = RC_D(v[i], n);
+  return n;
+}
+
+__device__ __forceinline__ void ap_sub3(const double* a, const double* b, double* c) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i) c[i] = RC_S(a[i], b[i]);
+}
+
+// Line solver s on unit bearings j [ap_line_np(s)][3] and world points X (same shape) of the sample's points, camera-
+// ray line normals n [ap_line_nl(s)][3] and world end points E [ap_line_nl(s)][2][3] of its lines (DESIGN.md
+// "Absolute pose"): up to 8 poses (Rs[9 i] row-major, ts[3 i]) with their root indices jr[i].  -> solution count.
+__device__ __noinline__ int ap_line_pose(int s, const double* j, const double* X, const double* n, const double* E,
+                                         double* Rs, double* ts, int* jr) {
+  double G[9], H[9], M[18], w[3], c[3], aux[3];
+  if (s == 0) {   // P2P1L: h1 along X2 - X1; g1 = j1, g3 = j1 x j2 / |j1 x j2|
+    ap_sub3(X + 3, X, w);
+    ap_unit(w, c);
+    const double L = __dsqrt_rn(rc_dot3(w, w));
+    ap_triad(c, H);
+    rc_cross3(j, j + 3, c);
+    const double sg = __dsqrt_rn(rc_dot3(c, c));
+    if (!(sg > AP_BEARING_EPS)) return 0;
+    const double gs = RC_D(rc_dot3(j, j + 3), sg);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      G[i] = j[i];
+      G[6 + i] = RC_D(c[i], sg);
+    }
+    rc_cross3(G + 6, G, G + 3);
+    double np_[3], Ep[3];
+    rc_mv3(G, n, np_);
+    const double Ln = RC_M(L, np_[0]);
+    for (int e = 0; e < 2; ++e) {
+      ap_sub3(E + 3 * e, X, w);
+      rc_mv3(H, w, Ep);
+      double* Me = M + 9 * e;
+      ap_trig_terms(np_, Ep, Me);
+      Me[2] = RC_S(Me[2], Ln);
+      Me[5] = RC_A(Me[5], RC_M(Ln, gs));
+    }
+    aux[0] = L;
+    aux[1] = gs;
+    aux[2] = sg;
+  } else {        // P1P2L, P3L: g3 along n1, h1 along line 1's direction
+    ap_unit(n, c);
+    double T[9];   // (g3, g1, g2)
+    ap_triad(c, T);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      G[i] = T[3 + i];
+      G[3 + i] = T[6 + i];
+      G[6 + i] = T[i];
+    }
+    ap_sub3(E + 3, E, w);
+    ap_unit(w, c);
+    ap_triad(c, H);
+    double np_[3], Ep[3];
+    if (s == 1) {   // P1P2L: line 2's direction; line 2's end point a with s1 from line 1's end point a
+      const double m1 = rc_dot3(G + 6, j), m2 = rc_dot3(n + 3, j);
+      if (!(fabs(m1) > AP_POINT_LINE_EPS)) return 0;
+      rc_mv3(G, n + 3, np_);
+      ap_sub3(E + 9, E + 6, w);
+      rc_mv3(H, w, Ep);
+      ap_trig_terms(np_, Ep, M);
+#pragma unroll
+      for (int i = 0; i < 3; ++i) np_[i] = RC_M(m1, np_[i]);
+      ap_sub3(E + 6, X, w);
+      rc_mv3(H, w, Ep);
+      ap_trig_terms(np_, Ep, M + 9);
+      ap_sub3(E, X, w);
+      rc_mv3(H, w, Ep);
+      M[15] = RC_S(M[15], RC_M(m2, Ep[2]));
+      M[16] = RC_S(M[16], RC_M(m2, Ep[1]));
+      aux[0] = m1;
+      aux[1] = Ep[1];
+      aux[2] = Ep[2];
+    } else {        // P3L: the directions of lines 2 and 3
+      double cr[3];
+      rc_cross3(n + 3, n + 6, cr);
+      const double det = rc_dot3(n, cr);
+      const double n1 = __dsqrt_rn(rc_dot3(n, n)), n2 = __dsqrt_rn(rc_dot3(n + 3, n + 3)),
+                   n3 = __dsqrt_rn(rc_dot3(n + 6, n + 6));
+      if (!(fabs(det) > RC_M(RC_M(RC_M(AP_CONCURRENT_EPS, n1), n2), n3))) return 0;
+      for (int e = 0; e < 2; ++e) {
+        rc_mv3(G, n + 3 * (e + 1), np_);
+        ap_sub3(E + 6 * (e + 1) + 3, E + 6 * (e + 1), w);
+        rc_mv3(H, w, Ep);
+        ap_trig_terms(np_, Ep, M + 9 * e);
+      }
+    }
+  }
+  double D[5], Xq[5], Yq[5], p[11], roots[10];
+  ap_trig_poly(M, M + 9, D, Xq, Yq, p);
+  const int nr = ess_roots(p, roots);
+  int ns = 0;
+  for (int r = 0; r < nr && r < AP_LINE_MAX_SOLUTIONS; ++r) {
+    double cs[4];
+    if (!ap_trig_angles(D, Xq, Yq, roots[r], cs)) continue;
+    const double ca = cs[0], sa = cs[1], cb = cs[2], sb = cs[3];
+    double s1 = 0.0;
+    if (s == 0) {
+      const double s2 = RC_D(RC_M(aux[0], sa), aux[2]);
+      s1 = RC_M(aux[0], RC_S(RC_M(aux[1], sa), ca));
+      if (!(s1 > 0.0) || !(s2 > 0.0)) continue;
+    } else if (s == 1) {
+      s1 = RC_D(-RC_A(RC_M(sb, aux[1]), RC_M(cb, aux[2])), aux[0]);
+      if (!(s1 > 0.0)) continue;
+    }
+    const double Rp[9] = {ca, -RC_M(sa, cb), RC_M(sa, sb), sa, RC_M(ca, cb), -RC_M(ca, sb), 0.0, sb, cb};
+    double W[9];
+    double* R = Rs + 9 * ns;
+    double* t = ts + 3 * ns;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        W[3 * i + k] = RC_A(RC_A(RC_M(Rp[3 * i], H[k]), RC_M(Rp[3 * i + 1], H[3 + k])), RC_M(Rp[3 * i + 2], H[6 + k]));
+    bool fin = true;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        R[3 * i + k] = RC_A(RC_A(RC_M(G[i], W[k]), RC_M(G[3 + i], W[3 + k])), RC_M(G[6 + i], W[6 + k]));
+        fin &= isfinite(R[3 * i + k]);
+      }
+    if (s < 2) {   // t = s1 j1 - R X1
+#pragma unroll
+      for (int i = 0; i < 3; ++i) t[i] = RC_S(RC_M(s1, j[i]), rc_dot3(R + 3 * i, X));
+    } else {       // n_i . t = -n_i . R A_i by Gaussian elimination with partial pivoting (first largest |pivot|)
+      double A[3][4];
+      for (int i = 0; i < 3; ++i) {
+        double RA[3];
+        rc_mv3(R, E + 6 * i, RA);
+        for (int k = 0; k < 3; ++k) A[i][k] = n[3 * i + k];
+        A[i][3] = -rc_dot3(n + 3 * i, RA);
+      }
+      for (int cc = 0; cc < 3; ++cc) {
+        int piv = cc;
+        double best = fabs(A[cc][cc]);
+        for (int q = cc + 1; q < 3; ++q)
+          if (fabs(A[q][cc]) > best) { best = fabs(A[q][cc]); piv = q; }
+        if (piv != cc)
+          for (int k = cc; k < 4; ++k) { const double tmp = A[cc][k]; A[cc][k] = A[piv][k]; A[piv][k] = tmp; }
+        for (int q = cc + 1; q < 3; ++q) {
+          const double f = RC_D(A[q][cc], A[cc][cc]);
+          for (int k = cc + 1; k < 4; ++k) A[q][k] = RC_S(A[q][k], RC_M(f, A[cc][k]));
+        }
+      }
+      for (int i = 2; i >= 0; --i) {
+        double acc = A[i][3];
+        for (int k = i + 1; k < 3; ++k) acc = RC_S(acc, RC_M(A[i][k], t[k]));
+        t[i] = RC_D(acc, A[i][i]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) fin &= isfinite(t[i]);
+    if (fin) jr[ns++] = r;
+  }
+  return ns;
+}
+
+__device__ __forceinline__ bool ap_line_rows_ok(int s, int np, int nl) {
+  return np >= ap_line_np(s) && nl >= ap_line_nl(s);
+}
+
+// Line hypothesis k of solver s of group g: its poses (shifted frame) with root indices.  -> solution count.  The
+// point rows are drawn with seed + 2 s + 1, the line rows with seed + 2 s + 2.
+__device__ __forceinline__ int ap_line_hypothesis(const ApStage& st, const ApGroup& sg, unsigned long long seed, int g,
+                                                  int s, int k, double* Rs, double* ts, int* jr) {
+  if (!ap_line_rows_ok(s, sg.np, sg.nl)) return 0;
+  int ip[2], il[3];
+  bool ok = true;
+  if (s == 0) ok = hg_draw<2>(seed + 1, g, k, sg.np, ip) && hg_draw<1>(seed + 2, g, k, sg.nl, il);
+  else if (s == 1) ok = hg_draw<1>(seed + 3, g, k, sg.np, ip) && hg_draw<2>(seed + 4, g, k, sg.nl, il);
+  else ok = hg_draw<3>(seed + 6, g, k, sg.nl, il);
+  if (!ok) return 0;
+  double j[6], X[6], n[9], E[18];
+  const int np = ap_line_np(s), nl = ap_line_nl(s);
+  for (int q = 0; q < np; ++q) {
+    const float2 kk = st.k[ip[q]];
+    const double qx = RC_D(RC_S(kk.x, sg.cx), sg.fx), qy = RC_D(RC_S(kk.y, sg.cy), sg.fy);
+    const double nb = __dsqrt_rn(RC_A(RC_A(RC_M(qx, qx), RC_M(qy, qy)), 1.0));
+    j[3 * q] = RC_D(qx, nb);
+    j[3 * q + 1] = RC_D(qy, nb);
+    j[3 * q + 2] = RC_D(1.0, nb);
+    for (int e = 0; e < 3; ++e) X[3 * q + e] = st.X[3 * ip[q] + e];
+  }
+  const double cam[4] = {sg.fx, sg.fy, sg.cx, sg.cy};
+  for (int q = 0; q < nl; ++q) {
+    rc_line_normal(cam, st.s0[il[q]], n + 3 * q);
+    for (int e = 0; e < 6; ++e) E[6 * q + e] = st.E[6 * il[q] + e];
+  }
+  return ap_line_pose(s, j, X, n, E, Rs, ts, jr);
+}
+
 // Camera coordinates of world point X under pose C (R row-major, then t): Y = R X, P = Y + t.
 __device__ __forceinline__ void ap_cam(const double* C, const double* X, double* Y, double* P) {
 #pragma unroll
@@ -368,6 +685,77 @@ __global__ void __launch_bounds__(AP_THREADS) abspose_hyp_kernel(AbsPoseArgs a) 
     for (int i = 1; i < AP_THREADS / 32; ++i) key = wbest[i] > key ? wbest[i] : key;
     if (key) atomicMax(a.key + g, key);
   }
+}
+
+// Thread h = s n_line_hyp + k runs hypothesis k of line solver s, index 4 n_hyp + 8 h + j.
+__global__ void __launch_bounds__(AP_THREADS) abspose_line_hyp_kernel(AbsPoseArgs a) {
+  extern __shared__ __align__(16) unsigned char ap_smem[];
+  __shared__ ApGroup sg;
+  __shared__ int warp_cnt[AP_THREADS / 32];
+  __shared__ double red[AP_THREADS / 32 * 6];
+  __shared__ unsigned long long wbest[AP_THREADS / 32];
+  pdl_launch_dependents();
+  pdl_wait();
+  const int g = blockIdx.x;
+  const ApStage st = ap_stage_ptrs(ap_smem, a.rows_p, a.rows_l);
+  ap_stage_group<AP_THREADS>(a, g, st, sg, warp_cnt, red);
+  if (sg.nl < 1) return;
+  const int n = sg.np + sg.nl;
+  const int h = blockIdx.y * AP_THREADS + threadIdx.x;
+  unsigned long long key = 0;
+  if (h < AP_LINE_SOLVERS * a.n_line_hyp) {
+    double Rs[9 * AP_LINE_MAX_SOLUTIONS], ts[3 * AP_LINE_MAX_SOLUTIONS];
+    int jr[AP_LINE_MAX_SOLUTIONS];
+    const int ns = ap_line_hypothesis(st, sg, a.seed, g, h / a.n_line_hyp, h % a.n_line_hyp, Rs, ts, jr);
+    const unsigned base = AP_MAX_SOLUTIONS * (unsigned)a.n_hyp + AP_LINE_MAX_SOLUTIONS * (unsigned)h;
+    for (int s = 0; s < ns; ++s) {
+      double C[12];
+#pragma unroll
+      for (int i = 0; i < 9; ++i) C[i] = Rs[9 * s + i];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) C[9 + i] = ts[3 * s + i];
+      unsigned cnt = 0;
+      for (int d = 0; d < n; ++d) cnt += ap_inlier(st, sg, C, a.thresh2, d);
+      const unsigned long long kk = ((unsigned long long)cnt << 32) | (unsigned long long)(~(base + jr[s]));
+      key = kk > key ? kk : key;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long t = __shfl_xor_sync(0xffffffffu, key, o);
+    key = t > key ? t : key;
+  }
+  if ((threadIdx.x & 31) == 0) wbest[threadIdx.x >> 5] = key;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < AP_THREADS / 32; ++i) key = wbest[i] > key ? wbest[i] : key;
+    if (key) atomicMax(a.key + g, key);
+  }
+}
+
+// The winner's pose C (shifted frame) from its index kj: hypothesis kj / 4, root kj % 4 of P3P below 4 n_hyp, else
+// line hypothesis (kj - 4 n_hyp) / 8, root (kj - 4 n_hyp) % 8.  -> false when that solution does not exist.
+__device__ __noinline__ bool ap_winner_pose(const AbsPoseArgs& a, const ApStage& st, const ApGroup& sg, int g,
+                                            unsigned kj, double* C) {
+  double Rs[9 * AP_LINE_MAX_SOLUTIONS], ts[3 * AP_LINE_MAX_SOLUTIONS];
+  int jr[AP_LINE_MAX_SOLUTIONS], ns = 0, j;
+  const unsigned p3p = AP_MAX_SOLUTIONS * (unsigned)a.n_hyp;
+  if (kj < p3p) {
+    j = (int)(kj % AP_MAX_SOLUTIONS);
+    if (sg.np >= AP_SAMPLE) ns = ap_hypothesis(st, sg, a.seed, g, (int)(kj / AP_MAX_SOLUTIONS), Rs, ts, jr);
+  } else {
+    const int h = (int)((kj - p3p) / AP_LINE_MAX_SOLUTIONS);
+    j = (int)((kj - p3p) % AP_LINE_MAX_SOLUTIONS);
+    if (h < AP_LINE_SOLVERS * a.n_line_hyp)
+      ns = ap_line_hypothesis(st, sg, a.seed, g, h / a.n_line_hyp, h % a.n_line_hyp, Rs, ts, jr);
+  }
+  for (int s = 0; s < ns; ++s)
+    if (jr[s] == j) {
+      for (int i = 0; i < 9; ++i) C[i] = Rs[9 * s + i];
+      for (int i = 0; i < 3; ++i) C[9 + i] = ts[3 * s + i];
+      return true;
+    }
+  return false;
 }
 
 // Block-wide inlier counts (points, lines) of pose C (shared), returned to every thread.
@@ -552,20 +940,10 @@ __global__ void __launch_bounds__(AP_FIT_THREADS) abspose_fit_kernel(AbsPoseArgs
   ap_stage_group<NT>(a, g, st, sg, warp_cnt, red);
   const unsigned long long key = a.key[g];
   const unsigned kj = ~(unsigned)(key & 0xffffffffull);
-  const int k = (int)(kj / AP_MAX_SOLUTIONS), j = (int)(kj % AP_MAX_SOLUTIONS);
   if (threadIdx.x == 0) {
-    s_ok[0] = 0;
-    if (sg.np >= AP_SAMPLE && key != 0) {
-      double Rs[9 * AP_MAX_SOLUTIONS], ts[3 * AP_MAX_SOLUTIONS];
-      int jr[AP_MAX_SOLUTIONS];
-      const int ns = ap_hypothesis(st, sg, a.seed, g, k, Rs, ts, jr);
-      for (int s = 0; s < ns; ++s)
-        if (jr[s] == j) {
-          for (int i = 0; i < 9; ++i) sC[0][i] = sC[1][i] = Rs[9 * s + i];
-          for (int i = 0; i < 3; ++i) sC[0][9 + i] = sC[1][9 + i] = ts[3 * s + i];
-          s_ok[0] = 1;
-        }
-    }
+    s_ok[0] = key != 0 && ap_winner_pose(a, st, sg, g, kj, sC[0]);
+    if (s_ok[0])
+      for (int i = 0; i < 12; ++i) sC[1][i] = sC[0][i];
   }
   __syncthreads();
   const bool valid = s_ok[0];

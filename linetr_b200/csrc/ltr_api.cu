@@ -1266,42 +1266,64 @@ int ltr_fundamental(const LtrFundamentalInput* in, const LtrFundamentalOutput* o
   return launch(KC_FUNDAMENTAL, true, fundamental_fit_kernel, dim3(in->n_pairs), dim3(FM_FIT_THREADS), (size_t)smem, s, a);
 }
 
-int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream) {
-  if (!in || !out) return set_error(LTR_E_INVALID, "ltr_absolute_pose: null argument");
+// ltr_absolute_pose is this body with no line hypotheses; `who` names the entry in its errors.
+static int absolute_pose(const char* who, const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int n_line_hyp,
+                         int32_t device, void* stream) {
+  const std::string w = who;
+  if (!in || !out) return set_error(LTR_E_INVALID, w + ": null argument");
   if (in->n_pairs < 0 || in->n_groups < 0 || in->max_rows_p < 0 || in->max_rows_l < 0)
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: negative count");
-  if (in->n_hypotheses < 1 || cdiv(in->n_hypotheses, AP_THREADS) > 65535)
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: n_hypotheses must be in [1, 65535 * 128]");
+    return set_error(LTR_E_INVALID, w + ": negative count");
+  if (n_line_hyp < 0 || n_line_hyp > AP_LINE_MAX_HYP)
+    return set_error(LTR_E_INVALID, w + ": n_line_hypotheses must be in [0, 2^21]");
+  if (in->n_hypotheses < (n_line_hyp ? 0 : 1) || cdiv(in->n_hypotheses, AP_THREADS) > 65535)
+    return set_error(LTR_E_INVALID, w + (n_line_hyp ? ": n_hypotheses must be in [0, 65535 * 128]"
+                                                    : ": n_hypotheses must be in [1, 65535 * 128]"));
+  if (n_line_hyp && !in->use_lines)
+    return set_error(LTR_E_INVALID, w + ": line hypotheses need use_lines");
   if (!(in->thresh > 0.0) || !std::isfinite(in->thresh))
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: thresh must be finite and > 0");
+    return set_error(LTR_E_INVALID, w + ": thresh must be finite and > 0");
   const int rows_l = in->use_lines ? in->max_rows_l : 0;
   const long long smem = ap_smem_bytes(in->max_rows_p, rows_l);
   if (smem > AP_SMEM_MAX)
-    return set_error(LTR_E_UNSUPPORTED, "ltr_absolute_pose: a group's correspondences need " + std::to_string(smem) +
+    return set_error(LTR_E_UNSUPPORTED, w + ": a group's correspondences need " + std::to_string(smem) +
                                             " bytes of shared memory (32 per keypoint row, 64 per segment row), over " +
                                             std::to_string(AP_SMEM_MAX));
   if (in->n_groups == 0) return LTR_OK;
   if (!out->R || !out->t || !out->valid || !out->refit || !out->n_inliers_p || !out->n_inliers_l || !out->hypothesis ||
       !out->hypothesis_inliers || !out->key)
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null output");
+    return set_error(LTR_E_INVALID, w + ": null output");
   if (!in->groups || !in->K0 || !in->cu_p || !in->cu_l || !out->inliers_p || !out->inliers_l)
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null groups, intrinsics, offsets or masks");
+    return set_error(LTR_E_INVALID, w + ": null groups, intrinsics, offsets or masks");
   if (in->max_rows_p > 0 && (!in->pts0 || !in->pts_off0 || !in->matches_p || !in->X1 || !in->x_off1 || !in->n_x1))
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null keypoint pools, 3D points or matches");
+    return set_error(LTR_E_INVALID, w + ": null keypoint pools, 3D points or matches");
   if (rows_l > 0 && (!in->segs0 || !in->seg_off0 || !in->matches_l || !in->L1 || !in->l_off1 || !in->n_l1))
-    return set_error(LTR_E_INVALID, "ltr_absolute_pose: null segment pools, 3D segments or line matches");
+    return set_error(LTR_E_INVALID, w + ": null segment pools, 3D segments or line matches");
   LTR_CUDA_TRY(cudaSetDevice(device));
   cudaStream_t s = as_stream(stream);
   AbsPoseArgs a{in->pts0, in->pts_off0, in->matches_p, in->cu_p, in->X1, in->x_off1, in->n_x1,
                 in->segs0, in->seg_off0, in->matches_l, in->cu_l, in->L1, in->l_off1, in->n_l1,
-                in->groups, in->K0, in->max_rows_p, rows_l, in->thresh * in->thresh, in->n_hypotheses,
+                in->groups, in->K0, in->max_rows_p, rows_l, in->thresh * in->thresh, in->n_hypotheses, n_line_hyp,
                 (unsigned long long)in->seed, reinterpret_cast<unsigned long long*>(out->key), out->R, out->t,
                 out->valid, out->refit, out->inliers_p, out->inliers_l, out->n_inliers_p, out->n_inliers_l,
                 out->hypothesis, out->hypothesis_inliers};
   LTR_CUDA_TRY(cudaMemsetAsync(out->key, 0, sizeof(uint64_t) * in->n_groups, s));
-  LTR_TRY(launch(KC_ABSOLUTE_POSE, true, abspose_hyp_kernel, dim3(in->n_groups, cdiv(in->n_hypotheses, AP_THREADS)),
-                 dim3(AP_THREADS), (size_t)smem, s, a));
+  if (in->n_hypotheses)
+    LTR_TRY(launch(KC_ABSOLUTE_POSE, true, abspose_hyp_kernel, dim3(in->n_groups, cdiv(in->n_hypotheses, AP_THREADS)),
+                   dim3(AP_THREADS), (size_t)smem, s, a));
+  if (n_line_hyp)
+    LTR_TRY(launch(KC_ABSOLUTE_POSE, true, abspose_line_hyp_kernel,
+                   dim3(in->n_groups, cdiv(AP_LINE_SOLVERS * n_line_hyp, AP_THREADS)), dim3(AP_THREADS), (size_t)smem,
+                   s, a));
   return launch(KC_ABSOLUTE_POSE, true, abspose_fit_kernel, dim3(in->n_groups), dim3(AP_FIT_THREADS), (size_t)smem, s, a);
+}
+
+int ltr_absolute_pose(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t device, void* stream) {
+  return absolute_pose("ltr_absolute_pose", in, out, 0, device, stream);
+}
+
+int ltr_absolute_pose_lines(const LtrAbsPoseInput* in, const LtrAbsPoseOutput* out, int32_t n_line_hypotheses,
+                            int32_t device, void* stream) {
+  return absolute_pose("ltr_absolute_pose_lines", in, out, n_line_hypotheses, device, stream);
 }
 
 static_assert(LTR_TRI_MAX_VIEWS == ltr::TRI_MAX_VIEWS, "LTR_TRI_MAX_VIEWS and the kernels' bound differ");
@@ -1934,6 +1956,30 @@ static __global__ void debug_p3p_kernel(const double* jb, const double* X, int n
   n_sol[i] = ns;
 }
 
+// One thread per sample of line solver s: j, X [n, 2 - s, 3], normals [n, s + 1, 3], end points [n, s + 1, 2, 3].
+static __global__ void debug_line_pose_kernel(int s, const double* jb, const double* Xb, const double* nb,
+                                              const double* Eb, int n, double* R, double* t, int* root_index,
+                                              int* n_sol) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int np = ap_line_np(s), nl = ap_line_nl(s);
+  double j[6], X[6], nn[9], E[18];
+  for (int e = 0; e < 3 * np; ++e) {
+    j[e] = jb[3ll * np * i + e];
+    X[e] = Xb[3ll * np * i + e];
+  }
+  for (int e = 0; e < 3 * nl; ++e) nn[e] = nb[3ll * nl * i + e];
+  for (int e = 0; e < 6 * nl; ++e) E[e] = Eb[6ll * nl * i + e];
+  double Rs[9 * AP_LINE_MAX_SOLUTIONS], ts[3 * AP_LINE_MAX_SOLUTIONS];
+  int jr[AP_LINE_MAX_SOLUTIONS];
+  const int ns = ap_line_pose(s, j, X, nn, E, Rs, ts, jr);
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  for (int e = 0; e < 9 * AP_LINE_MAX_SOLUTIONS; ++e) R[72ll * i + e] = e < 9 * ns ? Rs[e] : nan;
+  for (int e = 0; e < 3 * AP_LINE_MAX_SOLUTIONS; ++e) t[24ll * i + e] = e < 3 * ns ? ts[e] : nan;
+  for (int e = 0; e < AP_LINE_MAX_SOLUTIONS; ++e) root_index[8ll * i + e] = e < ns ? jr[e] : -1;
+  n_sol[i] = ns;
+}
+
 static __global__ void debug_fundamental_lines_kernel(const double* F, const float* s0, const float* s1, int n,
                                                       double min_overlap, double* r1, double* r0, uint8_t* ok) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2015,6 +2061,17 @@ int ltr_debug_p3p(const double* j, const double* X, int32_t n, double* R, double
   LTR_CUDA_TRY(cudaSetDevice(device));
   return launch(KC_DEBUG, false, debug_p3p_kernel, dim3(cdiv(n, 128)), dim3(128), 0, as_stream(stream), j, X, n, R, t,
                 root_index, n_solutions);
+}
+
+int ltr_debug_line_pose(int32_t solver, const double* j, const double* X, const double* n, const double* E, int32_t count,
+                        double* R, double* t, int32_t* root_index, int32_t* n_solutions, int32_t device, void* stream) {
+  if (solver < 0 || solver >= AP_LINE_SOLVERS || count < 0 ||
+      (count > 0 && ((solver < 2 && (!j || !X)) || !n || !E || !R || !t || !root_index || !n_solutions)))
+    return set_error(LTR_E_INVALID, "ltr_debug_line_pose: bad argument");
+  if (count == 0) return LTR_OK;
+  LTR_CUDA_TRY(cudaSetDevice(device));
+  return launch(KC_DEBUG, false, debug_line_pose_kernel, dim3(cdiv(count, 128)), dim3(128), 0, as_stream(stream),
+                (int)solver, j, X, n, E, (int)count, R, t, root_index, n_solutions);
 }
 
 int ltr_debug_fundamental_lines(const double* F, const float* s0, const float* s1, int32_t n, double min_overlap,

@@ -2,13 +2,14 @@
 3D coordinates (PL-Loc's last step), batched on the GPU, and the localization metrics.
 
     estimate_absolute_poses(res, K0, points3d1, lines3d1=None, groups=None, thresh=8.0, n_hypotheses=1024, seed=0,
-                            use_lines=True) -> AbsolutePoseResult
-        one `ltr_absolute_pose` call for every query (group of pairs) of a `match_images` / `match_sets` result;
+                            use_lines=True, n_line_hypotheses=0) -> AbsolutePoseResult
+        one `ltr_absolute_pose_lines` call for every query (group of pairs) of a `match_images` / `match_sets` result;
         device outputs, no synchronisation
     ransac_absolute_pose_host(kpts0, matches_p, points3d1, K0, klines0=None, matches_l=None, lines3d1=None, ...)
         the same model for one group in numpy: every operation is the kernels' operation in the kernels' order, the
         refit included, so the winner, its inlier count and the refitted pose are the same bits
-    p3p_solutions(bearings, X): the minimal solver; refine_pose_host: the refit
+    p3p_solutions(bearings, X): the point solver; p2p1l_solutions, p1p2l_solutions, p3l_solutions: the line solvers
+        (line_pose_solutions), all three through trig_pair_roots; refine_pose_host: the refit
     absolute_pose_errors, localization_recall: rotation / camera-centre errors and the InLoc recall bins
     lift_to_3d: 3D coordinates of database keypoints / segment end points from a depth map
 
@@ -24,6 +25,8 @@ real root j.  Every operation is one explicitly rounded fp64 operation.  A point
 its reprojection error in pixels is below thresh; a line iff both end points have depth > 0 and lie within thresh of
 the line through its query segment.  The winner has the most inliers (points and lines), then the lowest k, then the
 lowest j, and is refined by Levenberg-Marquardt over its inliers, kept iff the refit has at least as many inliers.
+With n_line_hypotheses, three line solvers (P2P1L: 2 points and 1 line; P1P2L: 1 point and 2 lines; P3L: 3 lines)
+add hypotheses that compete for the same winner at indices after the P3P ones.
 """
 from __future__ import annotations
 
@@ -42,6 +45,11 @@ AP_SAMPLE = 3
 AP_MAX_SOLUTIONS = 4
 AP_COLLINEAR_EPS = 1e-10   # a sample whose world cross-product norm is at most this times the edge lengths is rejected
 AP_MIN_REFIT = 3           # winner inliers needed for the refit
+AP_LINE_MAX_SOLUTIONS = 8  # line solvers: solutions per sample (the real roots of a degree-8 polynomial)
+AP_LINE_NP, AP_LINE_NL = (2, 1, 0), (1, 2, 3)   # point and line rows of a sample of P2P1L, P1P2L, P3L
+AP_BEARING_EPS = 1e-10     # P2P1L: |j1 x j2| of the unit bearings at most this rejects the sample
+AP_POINT_LINE_EPS = 1e-10  # P1P2L: |n1 . j1| / |n1| at most this (the query point on query line 1) rejects it
+AP_CONCURRENT_EPS = 1e-10  # P3L: |n1 . (n2 x n3)| at most this times |n1| |n2| |n3| (concurrent query lines) rejects it
 AP_LM_ITERS = 20           # Levenberg-Marquardt iterations (fixed budget)
 AP_LM_LAMBDA0 = 1e-3       # initial damping (Marquardt: A_ii + lambda A_ii)
 AP_LM_ACCEPT = 0.1         # damping factor after a step that lowers the cost
@@ -136,6 +144,225 @@ def p3p_solutions(j, X):
         t = P1 - ((R[..., 0] * X1[..., 0:1] + R[..., 1] * X1[..., 1:2]) + R[..., 2] * X1[..., 2:3])
         live &= np.isfinite(R).all((-1, -2)) & np.isfinite(t).all(-1)
     return R, t, live
+
+
+# ------------------------------------------------------------------ line solvers (P2P1L, P1P2L, P3L)
+def _unit(v):
+    """(v / |v|, |v|) of vectors v [..., 3]."""
+    n = np.sqrt(_dot(v, v))
+    return v / n[..., None], n
+
+
+def _mv(M, v):
+    """M v for row-major M [..., 9] (or [..., 3, 3]) and v [..., 3]."""
+    M = M.reshape(M.shape[:-2] + (9,)) if M.shape[-2:] == (3, 3) else M
+    return np.stack([_dot(M[..., 3 * i:3 * i + 3], v) for i in range(3)], -1)
+
+
+def trig_terms(n, E):
+    """The coefficients [..., 9] of n' . Rz(a) Rx(b) E' (row-major; rows cos a, sin a, 1; columns cos b, sin b, 1)."""
+    z = np.zeros(np.broadcast_shapes(n.shape, E.shape)[:-1])
+    return np.stack([n[..., 1] * E[..., 1], -(n[..., 1] * E[..., 2]), n[..., 0] * E[..., 0],
+                     -(n[..., 0] * E[..., 1]), n[..., 0] * E[..., 2], n[..., 1] * E[..., 0],
+                     n[..., 2] * E[..., 2], n[..., 2] * E[..., 1], z], -1)
+
+
+def _pmul(a, b):
+    """a b over the last axis (ascending coefficients), each coefficient summed over a's index ascending from 0."""
+    na, nb = a.shape[-1], b.shape[-1]
+    out = []
+    for k in range(na + nb - 1):
+        acc = np.zeros(a.shape[:-1])
+        for i in range(na):
+            if 0 <= k - i < nb:
+                acc = acc + a[..., i] * b[..., k - i]
+        out.append(acc)
+    return np.stack(out, -1)
+
+
+def trig_pair_poly(M1, M2):
+    """The core's polynomials of the equations [cos a, sin a, 1] M_i [cos b, sin b, 1]^T = 0, M1, M2 [K, 9] (row-major
+    3 x 3): with tau = tan(b / 2), row r of M_i is the quadratic M_i[r,0] (1 - tau^2) + 2 M_i[r,1] tau + M_i[r,2]
+    (1 + tau^2); A_i, B_i, C_i its rows 0, 1, 2.  -> (D = A1 B2 - A2 B1, X = B1 C2 - B2 C1, Y = A2 C1 - A1 C2 [K, 5],
+    p = (X^2 + Y^2) - D^2 [K, 9]), ascending coefficients."""
+    M1, M2 = np.asarray(M1, dtype=np.float64), np.asarray(M2, dtype=np.float64)
+    q = [[np.stack([M[..., 3 * r] + M[..., 3 * r + 2], 2.0 * M[..., 3 * r + 1], M[..., 3 * r + 2] - M[..., 3 * r]], -1)
+          for r in range(3)] for M in (M1, M2)]
+    (A1, B1, C1), (A2, B2, C2) = q
+    D = _pmul(A1, B2) - _pmul(A2, B1)
+    X = _pmul(B1, C2) - _pmul(B2, C1)
+    Y = _pmul(A2, C1) - _pmul(A1, C2)
+    return D, X, Y, (_pmul(X, X) + _pmul(Y, Y)) - _pmul(D, D)
+
+
+def _horner4(c, x):
+    v = c[..., 4]
+    for k in range(3, -1, -1):
+        v = v * x + c[..., k]
+    return v
+
+
+def trig_pair_roots(M1, M2):
+    """The two bilinear trigonometric equations' solutions (DESIGN.md "Absolute pose"): the real roots tau of p by
+    `sturm_roots`, then at each (cos a, sin a) = (X, Y) / D normalised by their norm and (cos b, sin b) = (1 - tau^2,
+    2 tau) / (1 + tau^2); a root with D == 0 is dropped.  Solution j is real root j (ascending).  -> (cs [K, 8, 4] of
+    (cos a, sin a, cos b, sin b), ok [K, 8], p [K, 9])."""
+    D, X, Y, p = trig_pair_poly(M1, M2)
+    K = len(p)
+    poly = np.zeros((K, 11))
+    poly[:, :9] = p
+    with np.errstate(all="ignore"):
+        roots, _ = sturm_roots(poly)
+        tau = roots[:, :AP_LINE_MAX_SOLUTIONS]
+        ok = ~np.isnan(tau)
+        tau = np.where(ok, tau, 0.0)
+        c = lambda a: a[:, None, :]
+        d = _horner4(c(D), tau)
+        ok &= d != 0
+        ca, sa = _horner4(c(X), tau) / d, _horner4(c(Y), tau) / d
+        nr = np.sqrt(ca * ca + sa * sa)
+        t2 = tau * tau
+        den = 1.0 + t2
+        cs = np.stack([ca / nr, sa / nr, (1.0 - t2) / den, (2.0 * tau) / den], -1)
+    return cs, ok, p
+
+
+def _triad(f):
+    """Rows (f, u, v) [K, 3, 3] of unit f [K, 3]: u = f x e / |f x e| for the coordinate axis e least aligned with f
+    (the first of the smallest |f_k|), v = f x u."""
+    a = np.abs(f)
+    k = np.where(a[:, 1] < a[:, 0], 1, 0)
+    k = np.where(a[:, 2] < a[np.arange(len(f)), k], 2, k)
+    e = np.zeros_like(f)
+    e[np.arange(len(f)), k] = 1.0
+    u, _ = _unit(_cross(f, e))
+    return np.stack([f, u, _cross(f, u)], 1)
+
+
+def line_pose_solutions(solver, j, X, n, E):
+    """Line solver `solver` (0 P2P1L, 1 P1P2L, 2 P3L; DESIGN.md "Absolute pose") on K samples: unit bearings j and
+    world points X [K, 2 - solver, 3] of the sample's points, camera-ray normals n [K, solver + 1, 3] of its query
+    lines and world end points E [K, solver + 1, 2, 3] of its lines.  -> (R [K, 8, 3, 3], t [K, 8, 3], ok [K, 8]) with
+    X_cam = R X + t; solution j is real root j of the degree-8 polynomial."""
+    j, X = np.asarray(j, dtype=np.float64), np.asarray(X, dtype=np.float64)
+    n, E = np.asarray(n, dtype=np.float64), np.asarray(E, dtype=np.float64)
+    K = len(n)
+    with np.errstate(all="ignore"):
+        if solver == 0:
+            w = X[:, 1] - X[:, 0]
+            h1, _ = _unit(w)
+            L = np.sqrt(_dot(w, w))
+            H = _triad(h1)
+            c = _cross(j[:, 0], j[:, 1])
+            sg = np.sqrt(_dot(c, c))
+            ok_s = sg > AP_BEARING_EPS
+            gs = _dot(j[:, 0], j[:, 1]) / sg
+            g3 = c / sg[:, None]
+            G = np.stack([j[:, 0], _cross(g3, j[:, 0]), g3], 1)
+            npr = _mv(G, n[:, 0])
+            Ln = L * npr[:, 0]
+            Ms = []
+            for e in range(2):
+                M = trig_terms(npr, _mv(H, E[:, 0, e] - X[:, 0]))
+                M[:, 2] = M[:, 2] - Ln
+                M[:, 5] = M[:, 5] + Ln * gs
+                Ms.append(M)
+        else:
+            T = _triad(_unit(n[:, 0])[0])
+            G = np.stack([T[:, 1], T[:, 2], T[:, 0]], 1)
+            H = _triad(_unit(E[:, 0, 1] - E[:, 0, 0])[0])
+            if solver == 1:
+                m1, m2 = _dot(G[:, 2], j[:, 0]), _dot(n[:, 1], j[:, 0])
+                ok_s = np.abs(m1) > AP_POINT_LINE_EPS
+                npr = _mv(G, n[:, 1])
+                M1 = trig_terms(npr, _mv(H, E[:, 1, 1] - E[:, 1, 0]))
+                M2 = trig_terms(m1[:, None] * npr, _mv(H, E[:, 1, 0] - X[:, 0]))
+                E1 = _mv(H, E[:, 0, 0] - X[:, 0])
+                M2[:, 6] = M2[:, 6] - m2 * E1[:, 2]
+                M2[:, 7] = M2[:, 7] - m2 * E1[:, 1]
+                Ms = [M1, M2]
+            else:
+                det = _dot(n[:, 0], _cross(n[:, 1], n[:, 2]))
+                nn = [np.sqrt(_dot(n[:, i], n[:, i])) for i in range(3)]
+                ok_s = np.abs(det) > ((AP_CONCURRENT_EPS * nn[0]) * nn[1]) * nn[2]
+                Ms = [trig_terms(_mv(G, n[:, e]), _mv(H, E[:, e, 1] - E[:, e, 0])) for e in (1, 2)]
+        cs, ok, _ = trig_pair_roots(Ms[0], Ms[1])
+        ok &= ok_s[:, None]
+        ca, sa, cb, sb = (cs[..., i] for i in range(4))
+        c = lambda a: a[:, None]
+        if solver == 0:
+            s2 = (c(L) * sa) / c(sg)
+            s1 = c(L) * (c(gs) * sa - ca)
+            ok &= (s1 > 0) & (s2 > 0)
+        elif solver == 1:
+            s1 = -(sb * c(E1[:, 1]) + cb * c(E1[:, 2])) / c(m1)
+            ok &= s1 > 0
+        z = np.zeros_like(ca)
+        Rp = np.stack([ca, -(sa * cb), sa * sb, sa, ca * cb, -(ca * sb), z, sb, cb], -1).reshape(K, -1, 3, 3)
+        Hb, Gb = H[:, None], G[:, None]
+        W = np.empty_like(Rp)
+        R = np.empty_like(Rp)
+        for i in range(3):
+            for k in range(3):
+                W[..., i, k] = (Rp[..., i, 0] * Hb[..., 0, k] + Rp[..., i, 1] * Hb[..., 1, k]) + Rp[..., i, 2] * Hb[..., 2, k]
+        for i in range(3):
+            for k in range(3):
+                R[..., i, k] = (Gb[..., 0, i] * W[..., 0, k] + Gb[..., 1, i] * W[..., 1, k]) + Gb[..., 2, i] * W[..., 2, k]
+        if solver < 2:
+            X1 = X[:, None, 0]
+            t = np.stack([s1 * c(j[:, 0, i]) - _dot(R[..., i, :], X1) for i in range(3)], -1)
+        else:
+            t = _solve3(R, n, E)
+        ok &= np.isfinite(R).all((-1, -2)) & np.isfinite(t).all(-1)
+    return R, t, ok
+
+
+def _solve3(R, n, E):
+    """P3L's translations [K, S, 3]: n_i . t = -n_i . R A_i (A_i line i's first end point) by Gaussian elimination with
+    partial pivoting (first largest |pivot|) and back substitution, as the kernels do."""
+    K, S = R.shape[:2]
+    A = np.empty((K, S, 3, 4))
+    for i in range(3):
+        RA = np.stack([_dot(R[..., r, :], E[:, None, i, 0]) for r in range(3)], -1)
+        A[..., i, :3] = n[:, None, i]
+        A[..., i, 3] = -_dot(n[:, None, i], RA)
+    A = A.reshape(K * S, 3, 4)
+    rows = np.arange(K * S)
+    for cc in range(3):
+        piv, best = np.full(K * S, cc), np.abs(A[:, cc, cc])
+        for q in range(cc + 1, 3):
+            m = np.abs(A[:, q, cc]) > best
+            best, piv = np.where(m, np.abs(A[:, q, cc]), best), np.where(m, q, piv)
+        top, pr = A[rows, cc].copy(), A[rows, piv].copy()
+        A[rows, cc], A[rows, piv] = pr, top
+        for q in range(cc + 1, 3):
+            f = A[:, q, cc] / A[:, cc, cc]
+            for k in range(cc + 1, 4):
+                A[:, q, k] = A[:, q, k] - f * A[:, cc, k]
+    t = np.zeros((K * S, 3))
+    for i in range(2, -1, -1):
+        acc = A[:, i, 3]
+        for k in range(i + 1, 3):
+            acc = acc - A[:, i, k] * t[:, k]
+        t[:, i] = acc / A[:, i, i]
+    return t.reshape(K, S, 3)
+
+
+def p2p1l_solutions(j, X, n, E):
+    """P2P1L: two points (unit bearings j [K, 2, 3], world points X [K, 2, 3]) and one line (normal n [K, 3], world
+    end points E [K, 2, 3]).  -> `line_pose_solutions`' (R, t, ok)."""
+    return line_pose_solutions(0, j, X, np.asarray(n)[:, None], np.asarray(E)[:, None])
+
+
+def p1p2l_solutions(j, X, n, E):
+    """P1P2L: one point (j [K, 3], X [K, 3]) and two lines (n [K, 2, 3], E [K, 2, 2, 3])."""
+    return line_pose_solutions(1, np.asarray(j)[:, None], np.asarray(X)[:, None], n, E)
+
+
+def p3l_solutions(n, E):
+    """P3L: three lines (n [K, 3, 3], E [K, 3, 2, 3])."""
+    K = len(n)
+    return line_pose_solutions(2, np.zeros((K, 0, 3)), np.zeros((K, 0, 3)), n, E)
 
 
 def _cam(R, t, X):
@@ -346,15 +573,18 @@ def stage_group(kpts0, matches_p, points3d1, K0, klines0=None, matches_l=None, l
 
 
 def ransac_absolute_pose_host(kpts0, matches_p, points3d1, K0, klines0=None, matches_l=None, lines3d1=None, group=0,
-                              thresh=8.0, n_hypotheses=1024, seed=0, use_lines=True) -> dict:
+                              thresh=8.0, n_hypotheses=1024, seed=0, use_lines=True, n_line_hypotheses=0) -> dict:
     """The absolute-pose estimator's model for one group in numpy (DESIGN.md "Absolute pose").  kpts0 [N0, 2] /
     klines0 [K0, 2, 2] are the query's (used as float32); matches_p / points3d1 (and matches_l / lines3d1) are one
     array per pair of the group in a list (or one array for a single pair): matches_p [N0] the local side-1 index or -1
     per query keypoint, points3d1 [n1, 3] fp64 (NaN rows: no 3D), lines3d1 [m1, 2, 3].  `group` seeds the samples.
     Returns R [3, 3], t [3] (X_cam = R X + t; NaN when invalid), valid, refit, inliers_p / inliers_l uint8 (the pairs'
-    match rows concatenated), n_inliers_p, n_inliers_l, hypothesis (4 k + j of the winning sample k and root j, or
-    -1), hypothesis_inliers, R_hypothesis / t_hypothesis (the winner before the refit) and cost (the refit's final sum
-    of squared residuals, NaN without a refit)."""
+    match rows concatenated), n_inliers_p, n_inliers_l, hypothesis (the winner's index: 4 k + j of P3P sample k and root
+    j, 4 n_hypotheses + 8 (s n_line_hypotheses + k) + j of line solver s's sample k, or -1), hypothesis_inliers,
+    R_hypothesis / t_hypothesis (the winner before the refit) and cost (the refit's final sum of squared residuals, NaN
+    without a refit).  n_line_hypotheses samples of each line solver s (`line_pose_solutions`) join the P3P ones: the
+    point rows drawn with seed + 2 s + 1, the line rows with seed + 2 s + 2, in groups with the rows the solver
+    needs."""
     single = not isinstance(matches_p, (list, tuple))
     mps = [matches_p] if single else list(matches_p)
     mls = ([matches_l] if single else list(matches_l)) if matches_l is not None else [np.zeros(0)] * len(mps)
@@ -365,19 +595,37 @@ def ransac_absolute_pose_host(kpts0, matches_p, points3d1, K0, klines0=None, mat
                inliers_p=np.zeros(sum(n_rows_p), np.uint8), inliers_l=np.zeros(sum(n_rows_l), np.uint8),
                n_inliers_p=0, n_inliers_l=0, hypothesis=-1, hypothesis_inliers=0, R_hypothesis=np.full((3, 3), np.nan),
                t_hypothesis=np.full(3, np.nan), cost=np.nan)
-    n = len(g.X)
-    if n < AP_SAMPLE:
-        return out
     t2 = float(thresh) * float(thresh)
-    idx, ok = draw_samples(seed, group, n_hypotheses, n, AP_SAMPLE)
-    idx = np.maximum(idx, 0)
     fx, fy = g.K[0, 0], g.K[1, 1]
     q = np.stack([g.d[:, 0] / fx, g.d[:, 1] / fy], 1)
-    R, t, oks = p3p_solutions(bearings(q[idx]), g.X[idx])
-    flat = np.flatnonzero((oks & ok[:, None]).reshape(-1))
+    cands = []   # (winner index, R, t, ok) per hypothesis kind
+    if len(g.X) >= AP_SAMPLE and n_hypotheses > 0:
+        idx, ok = draw_samples(seed, group, n_hypotheses, len(g.X), AP_SAMPLE)
+        idx = np.maximum(idx, 0)
+        R, t, oks = p3p_solutions(bearings(q[idx]), g.X[idx])
+        cands.append((np.arange(AP_MAX_SOLUTIONS * n_hypotheses), R, t, oks & ok[:, None]))
+    for s in range(3) if n_line_hypotheses > 0 else ():
+        mp, ml = AP_LINE_NP[s], AP_LINE_NL[s]
+        if len(g.X) < mp or len(g.E) < ml:
+            continue
+        il, ok = draw_samples(seed + 2 * s + 2, group, n_line_hypotheses, len(g.E), ml)
+        ip = np.zeros((n_line_hypotheses, 0), np.int64)
+        if mp:
+            ip, okp = draw_samples(seed + 2 * s + 1, group, n_line_hypotheses, len(g.X), mp)
+            ok &= okp
+        ip, il = np.maximum(ip, 0), np.maximum(il, 0)
+        R, t, oks = line_pose_solutions(s, bearings(q[ip]), g.X[ip], g.n[il], g.E[il])
+        base = AP_MAX_SOLUTIONS * n_hypotheses + AP_LINE_MAX_SOLUTIONS * s * n_line_hypotheses
+        cands.append((base + np.arange(AP_LINE_MAX_SOLUTIONS * n_line_hypotheses), R, t, oks & ok[:, None]))
+    if not cands:
+        return out
+    okf = np.concatenate([c[3].reshape(-1) for c in cands])
+    flat = np.concatenate([c[0] for c in cands])[okf]
+    R = np.concatenate([c[1].reshape(-1, 3, 3) for c in cands])[okf]
+    t = np.concatenate([c[2].reshape(-1, 3) for c in cands])[okf]
     if not len(flat):
         return out
-    Rf, tf = R.reshape(-1, 3, 3)[flat], t.reshape(-1, 3)[flat]
+    Rf, tf = R, t
     cnt = np.concatenate([_inliers(g, Rf[s:s + 256], tf[s:s + 256], t2).sum(1) for s in range(0, len(flat), 256)])
     order = np.lexsort((flat, -cnt))[0]
     w = int(flat[order])
@@ -413,8 +661,9 @@ class AbsolutePoseResult:
     R float64 [G, 3, 3] and t float64 [G, 3] with X_cam = R X_world + t (NaN where not valid), valid bool [G], refit
     bool [G] (the pose is the Levenberg-Marquardt refit), inliers_p / inliers_l uint8 aligned with the result's
     matches_p / matches_l (0 for unmatched rows, rows without 3D and invalid groups), n_inliers_p / n_inliers_l int32
-    [G], hypothesis int32 [G] (4 k + j of the winning sample k and root j, -1 when not valid) and hypothesis_inliers
-    int32 [G] (its inlier count, points and lines)."""
+    [G], hypothesis int32 [G] (the winner's index, -1 when not valid: 4 k + j of P3P sample k and root j, or
+    4 n_hypotheses + 8 (s n_line_hypotheses + k) + j of sample k of line solver s = 0 P2P1L, 1 P1P2L, 2 P3L) and
+    hypothesis_inliers int32 [G] (its inlier count, points and lines)."""
     R: torch.Tensor
     t: torch.Tensor
     valid: torch.Tensor
@@ -433,22 +682,30 @@ def _f64_rows(a, width):
 
 
 def estimate_absolute_poses(res, K0, points3d1, lines3d1=None, groups=None, thresh=8.0, n_hypotheses=1024, seed=0,
-                            use_lines=True) -> AbsolutePoseResult:
+                            use_lines=True, n_line_hypotheses=0) -> AbsolutePoseResult:
     """Absolute pose of every query of an `ImagePairMatches` (`match_images`, `match_sets`) whose side 1 are database
     images with 3D: P3P RANSAC over the point matches, scored and refined with the line matches too, in one
-    `ltr_absolute_pose` call (two kernel launches).  points3d1[p] fp64 [n1, 3] is aligned with res.keypoints1[p] and
+    `ltr_absolute_pose_lines` call (two kernel launches, three with line hypotheses).  points3d1[p] fp64 [n1, 3] is aligned with res.keypoints1[p] and
     lines3d1[p] fp64 [m1, 2, 3] with res.klines1[p] (NaN rows: no 3D); both are pooled by identity, so a database
     image repeated by `match_sets` goes up once.  groups int [G + 1]: offsets over the pairs, group g is the query of
     pairs [groups[g], groups[g + 1]), which must share one side-0 image (None: one group per pair).  K0: the query
     intrinsics, [3, 3] or [G, 3, 3] (zero skew).  thresh in pixels (cv2.solvePnPRansac's default 8); use_lines=False
-    scores points only.  Host arrays go up in one pinned copy; the call never waits for the device.  Raises LtrError
+    scores points only.  n_line_hypotheses > 0 adds that many hypotheses of each line solver (P2P1L, P1P2L, P3L;
+    DESIGN.md "Absolute pose") next to the n_hypotheses P3P ones, which may then be 0: queries with fewer than 3
+    point matches, or few point inliers, are localized from their line matches too (one more kernel launch); it needs
+    lines3d1 and use_lines.  Host arrays go up in one pinned copy; the call never waits for the device.  Raises LtrError
     for bad K0, misaligned 3D arrays, bad groups or groups that mix query images, and (LTR_E_UNSUPPORTED) when a group
     has more match rows than one CTA can stage (SMEM_PER_POINT_A / SMEM_PER_LINE_A bytes per row, SMEM_MAX in all)."""
     P = res.n_pairs
     dev = res.matches_p.device
     op, ol = np.asarray(res.offsets_p, dtype=np.int64), np.asarray(res.offsets_l, dtype=np.int64)
-    if int(n_hypotheses) < 1:
-        raise N.LtrError("estimate_absolute_poses: n_hypotheses must be >= 1")
+    n_line_hypotheses = int(n_line_hypotheses)
+    if n_line_hypotheses < 0:
+        raise N.LtrError("estimate_absolute_poses: n_line_hypotheses must be >= 0")
+    if int(n_hypotheses) < (0 if n_line_hypotheses else 1):
+        raise N.LtrError("estimate_absolute_poses: n_hypotheses must be >= 1 (>= 0 with line hypotheses)")
+    if n_line_hypotheses and not (use_lines and lines3d1 is not None):
+        raise N.LtrError("estimate_absolute_poses: line hypotheses need lines3d1 and use_lines")
     gr = np.arange(P + 1, dtype=np.int64) if groups is None else np.asarray(groups, dtype=np.int64).reshape(-1)
     if len(gr) < 1 or gr[0] != 0 or gr[-1] != P or (np.diff(gr) < 0).any():
         raise N.LtrError(f"estimate_absolute_poses: groups must be non-decreasing offsets from 0 to {P}")
@@ -489,18 +746,22 @@ def estimate_absolute_poses(res, K0, points3d1, lines3d1=None, groups=None, thre
         rows_l = int((ol[gr[1:]] - ol[gr[:-1]]).max(initial=0))
     dv = _ops.stage(arrays, dev)
     u8, i32 = dict(dtype=torch.uint8, device=dev), dict(dtype=torch.int32, device=dev)
+    # the entry takes a mask buffer even for a batch without point (or line) match rows, as line-only queries give
+    n_mp, n_ml = res.matches_p.shape[0], res.matches_l.shape[0]
+    masks = {"inliers_p": torch.empty(max(n_mp, 1), **u8), "inliers_l": torch.empty(max(n_ml, 1), **u8)}
     out = AbsolutePoseResult(torch.empty((G_, 3, 3), dtype=torch.float64, device=dev),
                              torch.empty((G_, 3), dtype=torch.float64, device=dev), torch.empty(G_, **u8),
-                             torch.empty(G_, **u8), torch.empty(res.matches_p.shape[0], **u8),
-                             torch.empty(res.matches_l.shape[0], **u8), torch.empty(G_, **i32), torch.empty(G_, **i32),
-                             torch.empty(G_, **i32), torch.empty(G_, **i32))
+                             torch.empty(G_, **u8), masks["inliers_p"][:n_mp], masks["inliers_l"][:n_ml],
+                             torch.empty(G_, **i32), torch.empty(G_, **i32), torch.empty(G_, **i32),
+                             torch.empty(G_, **i32))
     pts0 = torch.cat(p0) if p0 else torch.zeros((0, 2), dtype=torch.float32, device=dev)
-    _ops.call_struct("ltr_absolute_pose",
+    _ops.call_struct("ltr_absolute_pose_lines",
                      {**dv, "pts0": pts0.contiguous(), "matches_p": res.matches_p.contiguous(),
                       "matches_l": res.matches_l.contiguous(), "n_pairs": P, "n_groups": G_,
                       "max_rows_p": int((op[gr[1:]] - op[gr[:-1]]).max(initial=0)), "max_rows_l": rows_l,
                       "thresh": thresh, "n_hypotheses": n_hypotheses, "seed": seed, "use_lines": lines},
-                     {**vars(out), "key": torch.empty(G_, dtype=torch.int64, device=dev)})
+                     {**vars(out), **masks, "key": torch.empty(G_, dtype=torch.int64, device=dev)},
+                     scalars=(n_line_hypotheses,))
     out.valid = out.valid.view(torch.bool)
     out.refit = out.refit.view(torch.bool)
     return out
